@@ -112,6 +112,34 @@ int b200sv_heston_mc_chain_batch(const b200sv_heston_params* params, int B, int 
                                  long long nb_path, int nb_steps_per_year, uint64_t seed, int flags, int scheme, double* prices_out,
                                  double* stderr_out, double* ivols_out);
 
+/* Pathwise (forward-mode) Monte Carlo sensitivities of the chain pricers, in one pass (DESIGN.md §3.9).  Same arguments as
+ * b200sv_logsv_mc_chain / b200sv_heston_mc_chain, same prices and std errors; in addition greeks_out and greeks_se_out, each
+ * [1 + P][J] in chain order (J = offsets[M]-offsets[0]): row 0 = the forward delta d price / d forwards[m] of every strike of maturity m,
+ * then one row per model parameter in struct field order --
+ *   LogSV  (P = 6): sigma0, theta, kappa1, kappa2, beta, volvol   (kappa2 is held fixed when kappa1 or theta moves)
+ *   Heston (P = 5): v0, theta, kappa, rho, volvol
+ * greeks_se_out = discfactor * std(pathwise derivative) / sqrt(nb_path), the price's convention.  etas and discount factors are inputs,
+ * not differentiated.  Unbiased for the discretised scheme.  flags: fp64 state with B200SV_GAUSS_F32 or B200SV_GAUSS_F64; Heston takes
+ * scheme = B200SV_HESTON_EULER_FLOOR only.  Anything else returns an error.  Single GPU, synchronous. */
+int b200sv_logsv_mc_chain_greeks(const b200sv_logsv_params* params, int M, const double* ttms, const double* forwards,
+                                 const double* discfactors, const double* etas, const int* offsets, const double* strikes,
+                                 const int8_t* types, long long nb_path, int nb_steps_per_year, int is_spot_measure, int variable_type,
+                                 uint64_t seed, int flags, double* prices_out, double* stderr_out, double* greeks_out, double* greeks_se_out);
+int b200sv_heston_mc_chain_greeks(const b200sv_heston_params* params, int M, const double* ttms, const double* forwards,
+                                  const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
+                                  long long nb_path, int nb_steps_per_year, int variable_type, uint64_t seed, int flags, int scheme,
+                                  double* prices_out, double* stderr_out, double* greeks_out, double* greeks_se_out);
+
+/* test entry points of the tangent stepper: one slice of ttm from (0, sigma0 | v0, 0) for the global paths [path_offset, path_offset + nb_path)
+ * of Philox slice `slice_index`.  x, sigma | var, qvar: nb_path doubles; dx, dsigma | dvar, dqvar: [P][nb_path] tangents in the parameter
+ * order above (host, out).  The state is the one b200sv_logsv_terminal / b200sv_heston_terminal compute. */
+int b200sv_logsv_tangent_terminal(const b200sv_logsv_params* params, double ttm, long long nb_path, int nb_steps_per_year, int is_spot_measure,
+                                  double eta, uint64_t seed, int flags, int slice_index, long long path_offset, double* x, double* sigma,
+                                  double* qvar, double* dx, double* dsigma, double* dqvar);
+int b200sv_heston_tangent_terminal(const b200sv_heston_params* params, double ttm, long long nb_path, int nb_steps_per_year, uint64_t seed,
+                                   int flags, int slice_index, long long path_offset, double* x, double* var, double* qvar, double* dx,
+                                   double* dvar, double* dqvar);
+
 /* replaces LogSVPricer.simulate_terminal_values (pricers/logsv_pricer.py:590-611) -> simulate_logsv_x_vol_terminal.
  * x, sigma, qvar: nb_path doubles each (host, out). */
 int b200sv_logsv_terminal(const b200sv_logsv_params* params, double ttm, long long nb_path, int nb_steps_per_year,

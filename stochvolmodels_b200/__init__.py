@@ -9,6 +9,7 @@ from .pricers.heston_pricer import BTC_HESTON_PARAMS, HestonParams, HestonPricer
 from .pricers.logsv.affine_expansion import ExpansionOrder
 from .pricers.logsv.vol_moments import compute_analytic_qvar
 from .pricers.logsv_pricer import LOGSV_BTC_PARAMS, LogSvParams, LogSVPricer
+from .pricers.mc_greeks import McChainGreeks
 from .pricers.model_pricer import ModelParams, ModelPricer
 from .utils.config import OptionType, VariableType
 from .utils.funcs import set_seed, set_time_grid
@@ -18,4 +19,4 @@ __version__ = "0.1.0"
 __all__ = ["HawkesJDParams", "HawkesJDPricer", "OptionChain", "get_btc_test_chain_data", "HestonParams", "HestonPricer", "BTC_HESTON_PARAMS", "ExpansionOrder",
            "LogSvParams", "LogSVPricer", "CalibrationEngine", "CalibrationError", "ConstraintsType", "LogsvModelCalibrationType", "LOGSV_BTC_PARAMS", "ModelParams", "ModelPricer", "OptionType", "VariableType", "set_seed", "set_time_grid",
            "compute_integration_weights", "OptionSlice", "compute_analytic_qvar", "infer_bsm_ivols_from_slice_prices",
-           "infer_bsm_ivols_from_model_chain_prices"]
+           "infer_bsm_ivols_from_model_chain_prices", "McChainGreeks"]

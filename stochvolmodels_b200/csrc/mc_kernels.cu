@@ -314,10 +314,11 @@ struct SliceArgs {
 // advance one path through the slice, drawing its normals in the order philox.cuh defines.  SAFE = clamp the log-vol every step (re-run
 // of a path whose fast pass left the representable range); !SAFE = the production loop with the generator software-pipelined one call
 // ahead of the fp64 recursion (the integer / SFU stream of call c+1 overlaps the fp64 stream of call c inside a warp).
-template <bool SAFE, typename Path, typename Real, int GAUSS>
+// PREFETCH = false: no software pipelining (register-bound callers).
+template <bool SAFE, bool PREFETCH = (B200SV_SLICE_PREFETCH != 0), typename Path, typename Real, int GAUSS>
 __device__ __forceinline__ void run_slice_steps(Path& p, StepNormals<Real, GAUSS>& rng, int nsteps) {
   if constexpr (GAUSS == kGaussF64) {
-    if constexpr (SAFE || !B200SV_SLICE_PREFETCH) {
+    if constexpr (SAFE || !PREFETCH) {
       for (int s = 0; s < nsteps; ++s) {
         Real z0, z1;
         rng.get((uint32_t)s, z0, z1);
@@ -338,7 +339,7 @@ __device__ __forceinline__ void run_slice_steps(Path& p, StepNormals<Real, GAUSS
   } else {
     // one Philox call feeds two steps
     const int ncalls = nsteps >> 1;
-    if constexpr (SAFE || !B200SV_SLICE_PREFETCH) {
+    if constexpr (SAFE || !PREFETCH) {
       for (int c = 0; c < ncalls; ++c) {
         Real n0, n1, n2, n3;
         rng.get2((uint32_t)c, n0, n1, n2, n3);
@@ -898,6 +899,332 @@ __global__ void __launch_bounds__(kSliceThreads, B200SV_SLICE_MINBLOCKS) mc_chai
 }
 
 // --------------------------------------------------------------------------------------------------------------------
+// pathwise (forward-mode) sensitivities of the chain pricer, DESIGN.md §3.9
+// --------------------------------------------------------------------------------------------------------------------
+// A tangent path wraps the production path object and calls its step() unchanged, so the base recursion -- and the prices -- are the
+// same code as mc_slice_kernel's.  Per model parameter p it carries, in registers, the tangent of the vol state (dL = d log sigma for
+// LogSV, dv for Heston) and two running sums from which the tangents of x and q follow.  Parameter order = the dataclass field order.
+constexpr int kLogsvParams = 6;    // sigma0, theta, kappa1, kappa2, beta, volvol
+constexpr int kHestonParams = 5;   // v0, theta, kappa, rho, volvol
+
+struct TangentState {    // SoA [P][n] fp64, persisted across maturities like x, v, q
+  double* dx;
+  double* dv;            // d log sigma (LogSV) or d variance (Heston)
+  double* dq;
+};
+
+struct LogsvTangentConsts {
+  LogsvConsts c;
+  double a1, a2;                     // natural-unit a1, a2 of LogsvConsts (the recursion's Jacobian 1 - a1/sigma + a2*sigma)
+  double cx2, cq4;                   // 2 cx, 4 cq
+  double dt, sdt, k1dt, k2dt, thdt, bdt, vvdt, etadt;   // parameter derivatives of a0..b1 (etadt = eta*dt under the inverse measure, else 0)
+};
+
+struct HestonTangentConsts {
+  HestonConsts c;
+  double drc0, drc1, dvc0, dvc1;     // d(c0, c1)/d rho, d(c0, c1)/d volvol
+};
+
+static LogsvTangentConsts make_logsv_tangent_consts(const b200sv_logsv_params& p, double eta, bool spot, double dt) {
+  LogsvTangentConsts k;
+  k.c = make_logsv_consts(p, eta, spot, dt);
+  k.a1 = k.c.a1;
+  k.a2 = k.c.a2;
+  k.cx2 = 2.0 * k.c.cx;
+  k.cq4 = 4.0 * k.c.cq;
+  k.dt = dt;
+  k.sdt = std::sqrt(dt);
+  k.k1dt = p.kappa1 * dt;
+  k.k2dt = p.kappa2 * dt;
+  k.thdt = p.theta * dt;
+  k.bdt = p.beta * dt;
+  k.vvdt = p.volvol * dt;
+  k.etadt = spot ? 0.0 : eta * dt;
+  return k;
+}
+
+static HestonTangentConsts make_heston_tangent_consts(const b200sv_heston_params& p, double dt) {
+  HestonTangentConsts k;
+  k.c = make_heston_consts(p, dt, B200SV_HESTON_EULER_FLOOR);
+  const double sdt = std::sqrt(dt), r1 = std::sqrt(1.0 - p.rho * p.rho);
+  k.drc0 = p.volvol * sdt;
+  k.drc1 = -p.volvol * p.rho / r1 * sdt;
+  k.dvc0 = p.rho * sdt;
+  k.dvc1 = r1 * sdt;
+  return k;
+}
+
+// LogSV: dL' = dL (1 - a1/sigma + a2 sigma) + da0 + da1/sigma + da2 sigma + db0 z0 + db1 z1 on the OLD sigma;
+// dx += (2 cx sigma^2 + ce sigma z0) dL on the old sigma; dq is kept as dq0 + 2 cq sigma_0^2 dL_0 + sum_k 4 cq sigma_k^2 dL_k (new sigma
+// of every step) and corrected by -2 cq sigma_S^2 dL_S when read, the same telescoping as LogsvPath's q.
+struct LogsvTangentPath {
+  static constexpr int NP = kLogsvParams;
+  static constexpr bool kPrefetch = false;   // 18 tangent registers leave no room for a second set of normals in flight
+  using Consts = LogsvTangentConsts;
+  LogsvPath<double> b;
+  double dx[NP], dL[NP], dq[NP];
+  double s_first;      // sigma at load
+  const Consts& k;     // the kernel's __grid_constant__ parameter: read as constant-bank operands, not held in registers
+  __device__ __forceinline__ LogsvTangentPath(const Consts& k_) : b(k_.c), k(k_) {}
+  __device__ __forceinline__ void load(double x, double v, double q, const TangentState& t, long long i, long long n, bool init) {
+    b.load(x, v, q);
+    s_first = v;
+#pragma unroll
+    for (int p = 0; p < NP; ++p) {
+      double tx = 0.0, tl = (p == 0) ? 1.0 / v : 0.0, tq = 0.0;    // dL_0 = 1/sigma0 for sigma0
+      if (!init) {
+        tx = t.dx[p * n + i];
+        tl = t.dv[p * n + i];
+        tq = t.dq[p * n + i];
+      }
+      dx[p] = tx;
+      dL[p] = tl;
+      dq[p] = fma(2.0 * k.c.cq * b.s2_first, tl, tq);
+    }
+  }
+  template <bool SAFE>
+  __device__ __forceinline__ void step(double z0, double z1) {
+    const double so = b.s, io = b.inv;
+    b.template step<SAFE>(z0, z1);
+    const double sn = b.s;
+    const double jac = fma(k.a2, so, fma(-k.a1, io, 1.0));
+    const double fx = so * fma(k.cx2, so, k.c.ce * z0);
+    const double fq = k.cq4 * sn * sn;
+    double drive[NP];
+    drive[0] = 0.0;
+    drive[1] = fma(k.k1dt, io, k.k2dt);                      // theta:  kappa2 dt + kappa1 dt / sigma
+    drive[2] = fma(k.thdt, io, -k.dt);                       // kappa1: -dt + theta dt / sigma
+    drive[3] = fma(-k.dt, so, k.thdt);                       // kappa2: theta dt - dt sigma
+    drive[4] = fma(k.sdt, z0, fma(k.etadt, so, -k.bdt));     // beta:   -beta dt + eta dt sigma (inverse measure) + sqrt(dt) z0
+    drive[5] = fma(k.sdt, z1, -k.vvdt);                      // volvol: -volvol dt + sqrt(dt) z1
+    // a clamped step (SAFE re-run of a path that left the representable range) has a zero tangent through the clamp
+    const bool clamped = SAFE && fabs(b.Ls) == kLogScaledMax;
+#pragma unroll
+    for (int p = 0; p < NP; ++p) {
+      dx[p] = fma(fx, dL[p], dx[p]);
+      dL[p] = clamped ? 0.0 : fma(jac, dL[p], drive[p]);
+      dq[p] = fma(fq, dL[p], dq[p]);
+    }
+  }
+  __device__ __forceinline__ bool overflowed() const { return b.overflowed(); }
+  __device__ __forceinline__ double sigma() const { return b.sigma(); }
+  // LogsvPath::x() / q() with the contraction nvcc applies to them in every production kernel spelled out -- s2_first - s*s is
+  // fma(sigma_0, sigma_0, -rn(s*s)) there -- so that the state stays bit-identical to mc_slice_kernel's in this different context
+  __device__ __forceinline__ double s2_diff() const { return fma(s_first, s_first, -__dmul_rn(b.s, b.s)); }
+  __device__ __forceinline__ double x() const { return fma(b.ce, b.XM, fma(b.cx, s2_diff() + b.A, b.x0)); }
+  __device__ __forceinline__ double q() const { return fma(b.cq, s2_diff() + 2.0 * b.A, b.q0); }
+  __device__ __forceinline__ double tx(int p) const { return dx[p]; }
+  __device__ __forceinline__ double tq(int p) const { return fma(-2.0 * k.c.cq * b.s * b.s, dL[p], dq[p]); }
+  __device__ __forceinline__ double tv(int p) const { return dL[p]; }
+};
+
+// Heston floor-Euler: dv' = 0 where the floor binds, else dv (1 - kappa dt) + dv (c0 z0 + c1 z1)/(2 sqrt v) + d(kappa dt) (theta - v)
+// + kappa dt d(theta) + sqrt(v) (dc0 z0 + dc1 z1); dx += (-dt/2 + sqrt(dt) z0 / (2 sqrt v)) dv, dq += dt dv, all on the old v.
+struct HestonTangentPath {
+  static constexpr int NP = kHestonParams;
+  static constexpr bool kPrefetch = B200SV_SLICE_PREFETCH != 0;
+  using Consts = HestonTangentConsts;
+  HestonPath<double, false> b;
+  double dx[NP], dv[NP], dq[NP];
+  const Consts& k;     // the kernel's __grid_constant__ parameter
+  __device__ __forceinline__ HestonTangentPath(const Consts& k_) : b(k_.c), k(k_) {}
+  __device__ __forceinline__ void load(double x, double v, double q, const TangentState& t, long long i, long long n, bool init) {
+    b.load(x, v, q);
+#pragma unroll
+    for (int p = 0; p < NP; ++p) {
+      if (init) {
+        dx[p] = 0.0;
+        dv[p] = (p == 0) ? 1.0 : 0.0;                    // dv_0 = 1 for v0
+        dq[p] = 0.0;
+      } else {
+        dx[p] = t.dx[p * n + i];
+        dv[p] = t.dv[p * n + i];
+        dq[p] = t.dq[p * n + i];
+      }
+    }
+  }
+  template <bool SAFE>
+  __device__ __forceinline__ void step(double z0, double z1) {
+    const double v = b.v, sig = sqrt(v), hs = 0.5 / sig;
+    b.template step<SAFE>(z0, z1);
+    const bool live = b.v > 1e-4;                        // np.maximum(v, 1e-4) did not bind
+    const double fx = fma(b.sdt * z0, hs, b.hx);
+    const double jac = fma(fma(b.c0, z0, b.c1 * z1), hs, 1.0 - b.kdt);
+    double drive[NP];
+    drive[0] = 0.0;
+    drive[1] = b.kdt;                                    // theta
+    drive[2] = b.dt * (b.theta - v);                     // kappa
+    drive[3] = sig * fma(k.drc0, z0, k.drc1 * z1);       // rho
+    drive[4] = sig * fma(k.dvc0, z0, k.dvc1 * z1);       // volvol
+#pragma unroll
+    for (int p = 0; p < NP; ++p) {
+      dx[p] = fma(fx, dv[p], dx[p]);
+      dq[p] = fma(b.dt, dv[p], dq[p]);
+      dv[p] = live ? fma(jac, dv[p], drive[p]) : 0.0;
+    }
+  }
+  __device__ __forceinline__ bool overflowed() const { return false; }
+  __device__ __forceinline__ double sigma() const { return b.sigma(); }
+  __device__ __forceinline__ double x() const { return b.x(); }
+  __device__ __forceinline__ double q() const { return b.q(); }
+  __device__ __forceinline__ double tx(int p) const { return dx[p]; }
+  __device__ __forceinline__ double tq(int p) const { return dq[p]; }
+  __device__ __forceinline__ double tv(int p) const { return dv[p]; }
+};
+
+// mc_slice_kernel with tangents: same persistent grid-stride loop, same Philox stream (counter = global path id, slice), same
+// overflow re-run.  Per-CTA partials [gridDim.x][2 + P]: sum F e^x, count, sum F e^x dx_p over the non-NaN spots.
+template <typename TPath, int GAUSS>
+__global__ void __launch_bounds__(kSliceThreads, B200SV_SLICE_MINBLOCKS) mc_tangent_slice_kernel(SliceArgs<double> a, TangentState t,
+                                                                                                 const __grid_constant__ typename TPath::Consts consts) {
+  constexpr int NP = TPath::NP, K = 2 + NP;
+  __shared__ double red[K * kSliceThreads / 32];
+  exp_table_init();
+  if constexpr (GAUSS != kGaussF32) gauss64_table_init();
+  double acc[K];
+#pragma unroll
+  for (int k = 0; k < K; ++k) acc[k] = 0.0;
+  TPath p(consts);
+  const long long stride = (long long)gridDim.x * kSliceThreads;
+  for (long long i = (long long)blockIdx.x * kSliceThreads + threadIdx.x; i < a.n; i += stride) {
+    double xi = 0.0, vi = a.v_init, qi = 0.0;
+    if (!a.init) {
+      xi = a.x[i];
+      vi = a.v[i];
+      qi = a.q[i];
+    }
+    p.load(xi, vi, qi, t, i, a.n, a.init != 0);
+    StepNormals<double, GAUSS> rng(a.seed, a.path_offset + (unsigned long long)i, a.slice);
+    run_slice_steps<false, TPath::kPrefetch>(p, rng, a.nsteps);
+    if (p.overflowed()) {
+      p.load(xi, vi, qi, t, i, a.n, a.init != 0);
+      run_slice_steps<true>(p, rng, a.nsteps);
+    }
+    const double xT = p.x();
+    a.x[i] = xT;
+    a.v[i] = p.sigma();
+    a.q[i] = p.q();
+    const double spot = a.forward * exp(xT);
+#pragma unroll
+    for (int k = 0; k < NP; ++k) {
+      const double d = p.tx(k);
+      t.dx[k * a.n + i] = d;
+      t.dv[k * a.n + i] = p.tv(k);
+      t.dq[k * a.n + i] = p.tq(k);
+      if (spot == spot) acc[2 + k] = fma(spot, d, acc[2 + k]);
+    }
+    if (spot == spot) {
+      acc[0] += spot;
+      acc[1] += 1.0;
+    }
+  }
+  block_sum<K, kSliceThreads>(acc, red);
+  if (threadIdx.x == 0) {
+#pragma unroll
+    for (int k = 0; k < K; ++k) a.partials[K * blockIdx.x + k] = acc[k];
+  }
+}
+
+// Per-strike sums of the payoff and of its pathwise derivatives.  U = re-centred spot S (LOG_RETURN) or q/ttm (Q_VAR);
+// dS_p = F e^x dx_p - mean(F e^x dx_p) over the nanmean's set, dS/dF = S/F; dU_p = dq_p/ttm, dU/dF = 0 under Q_VAR.
+// pay = h(U) (C/P) or h(U)/S (IC/IP) with h = (U-K)^+ or (K-U)^+; g = h'(U) dU or (h'(U) dU - pay dS)/S.  A path whose payoff is NaN
+// is skipped for every sum.  Row layout per strike: (sum pay, sum pay^2, count, then (sum g, sum g^2) for delta and every parameter).
+constexpr int kGreeksStrikeChunk = 2;
+template <int NP>
+__global__ void __launch_bounds__(kThreads) payoff_greeks_kernel(const double* __restrict__ x, const double* __restrict__ q,
+                                                                const double* __restrict__ dx, const double* __restrict__ dq, long long n,
+                                                                double ttm, double forward, const double* __restrict__ strikes,
+                                                                const int8_t* __restrict__ types, int J, int variable_type,
+                                                                const double* __restrict__ moments, double* __restrict__ partials, int Kpad) {
+  constexpr int KV = 3 + 2 * (1 + NP), KC = KV * kGreeksStrikeChunk;
+  __shared__ double red[KC * kThreads / 32];
+  __shared__ double sh_mom[2 + NP];
+  if (threadIdx.x < 2 + NP) sh_mom[threadIdx.x] = moments[threadIdx.x];
+  __syncthreads();
+  const double corr = sh_mom[0] / sh_mom[1] - forward;
+  double mean_d[NP];
+#pragma unroll
+  for (int k = 0; k < NP; ++k) mean_d[k] = sh_mom[2 + k] / sh_mom[1];
+  const int j0 = blockIdx.y * kGreeksStrikeChunk;
+  double kk[kGreeksStrikeChunk];
+  int ty[kGreeksStrikeChunk];
+#pragma unroll
+  for (int c = 0; c < kGreeksStrikeChunk; ++c) {
+    kk[c] = j0 + c < J ? strikes[j0 + c] : 0.0;
+    ty[c] = j0 + c < J ? (int)types[j0 + c] : -1;
+  }
+  const bool is_qvar = variable_type == B200SV_Q_VAR;
+  const double inv_f = 1.0 / forward, inv_ttm = 1.0 / ttm;
+  double acc[KC];
+#pragma unroll
+  for (int c = 0; c < KC; ++c) acc[c] = 0.0;
+  const long long stride = (long long)gridDim.x * kThreads;
+  for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < n; i += stride) {
+    const double fe = forward * exp(x[i]);
+    const double spot = fe - corr;
+    double dS[1 + NP], dU[1 + NP];
+    dS[0] = spot * inv_f;
+    dU[0] = is_qvar ? 0.0 : dS[0];
+#pragma unroll
+    for (int k = 0; k < NP; ++k) {
+      dS[1 + k] = fma(fe, dx[k * n + i], -mean_d[k]);
+      dU[1 + k] = is_qvar ? dq[k * n + i] * inv_ttm : dS[1 + k];
+    }
+    const double under = is_qvar ? q[i] * inv_ttm : spot;
+#pragma unroll
+    for (int c = 0; c < kGreeksStrikeChunk; ++c) {
+      if (ty[c] < 0) continue;
+      const bool is_put = ty[c] & 1, inverse = ty[c] >= 2;
+      const bool itm = is_put ? under < kk[c] : under > kk[c];
+      const double h = itm ? (is_put ? kk[c] - under : under - kk[c]) : 0.0;
+      const double hp = itm ? (is_put ? -1.0 : 1.0) : 0.0;
+      const double pay = inverse ? h / spot : h;
+      if (pay != pay) continue;
+      double* a = acc + KV * c;
+      a[0] += pay;
+      a[1] += pay * pay;
+      a[2] += 1.0;
+#pragma unroll
+      for (int k = 0; k < 1 + NP; ++k) {
+        double g = itm ? hp * dU[k] : 0.0;
+        if (inverse) g = (g - pay * dS[k]) / spot;
+        a[3 + 2 * k] += g;
+        a[4 + 2 * k] = fma(g, g, a[4 + 2 * k]);
+      }
+    }
+  }
+  block_sum<KC, kThreads>(acc, red);
+  if (threadIdx.x == 0) {
+#pragma unroll
+    for (int c = 0; c < KC; ++c) partials[(size_t)blockIdx.x * Kpad + KV * j0 + c] = acc[c];
+  }
+}
+
+// prices / std errors exactly as payoff_finalize_kernel, plus greeks_out[k][Jtot] = df * mean(g_k), greeks_se = df * std(g_k) / sqrt(N)
+__global__ void greeks_finalize_kernel(const double* __restrict__ sums, int KV, int J, int Jtot, double discfactor, double total_paths,
+                                       double* __restrict__ prices, double* __restrict__ stderrs, double* __restrict__ greeks,
+                                       double* __restrict__ greeks_se) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= J) return;
+  const double* s = sums + (size_t)KV * j;
+  const double cnt = s[2];
+  for (int k = -1; k < (KV - 3) / 2; ++k) {
+    const double s1 = k < 0 ? s[0] : s[3 + 2 * k], s2 = k < 0 ? s[1] : s[4 + 2 * k];
+    const double mean = s1 / cnt;
+    double var = s2 / cnt - mean * mean;
+    var = var > 0.0 ? var : 0.0;
+    const double m = discfactor * mean, e = discfactor * sqrt(var) / sqrt(total_paths);
+    if (k < 0) {
+      prices[j] = m;
+      stderrs[j] = e;
+    } else {
+      greeks[(size_t)k * Jtot + j] = m;
+      greeks_se[(size_t)k * Jtot + j] = e;
+    }
+  }
+}
+
+// --------------------------------------------------------------------------------------------------------------------
 // debug / parity export of the normals the fused kernel draws
 // --------------------------------------------------------------------------------------------------------------------
 template <int GAUSS>
@@ -1419,6 +1746,193 @@ static int terminal_host(const b200sv_logsv_params* lp, const b200sv_heston_para
   return rc;
 }
 
+// ---- pathwise sensitivities: host side --------------------------------------------------------------------------------
+// fp64 state, Gaussian mode fp32 or fp64 (the two production streams); anything else is an error, not a fallback
+static int greeks_gauss(int flags) {
+  if (flags & B200SV_STATE_F32) return fail(-1, "invalid argument: pathwise sensitivities need fp64 state (B200SV_STATE_F64)");
+  const int g = gauss_mode(flags);
+  if (g != kGaussF32 && g != kGaussF64) return fail(-1, "invalid argument: pathwise sensitivities support B200SV_GAUSS_F32 and B200SV_GAUSS_F64");
+  return g;
+}
+
+// one maturity slice with tangents; moments_out[2 + P] = (sum F e^x, count, sum F e^x dx_p)
+template <int MODEL, int GAUSS>
+static int launch_tangent_slice_g(double* x, double* v, double* q, const TangentState& t, long long n, long long path_offset, int init,
+                                  double v_init, int nsteps, int slice_index, double forward, uint64_t seed, const LogsvTangentConsts* lc,
+                                  const HestonTangentConsts* hc, double* moments_out, cudaStream_t st) {
+  using TPath = typename std::conditional<MODEL == 0, LogsvTangentPath, HestonTangentPath>::type;
+  constexpr int K = 2 + TPath::NP;
+  SliceArgs<double> a;
+  a.x = x;
+  a.v = v;
+  a.q = q;
+  a.n = n;
+  a.path_offset = (unsigned long long)path_offset;
+  a.init = init;
+  a.v_init = v_init;
+  a.nsteps = nsteps;
+  a.slice = (unsigned int)slice_index;
+  a.seed = seed;
+  a.forward = forward;
+  const Grid g = persistent_grid(mc_tangent_slice_kernel<TPath, GAUSS>, kSliceThreads, n);
+  double* partials = nullptr;
+  B200SV_CUDA(cudaMallocAsync(&partials, sizeof(double) * K * g.blocks, st));
+  a.partials = partials;
+  if constexpr (MODEL == 0)
+    mc_tangent_slice_kernel<TPath, GAUSS><<<g.blocks, g.threads, 0, st>>>(a, t, *lc);
+  else
+    mc_tangent_slice_kernel<TPath, GAUSS><<<g.blocks, g.threads, 0, st>>>(a, t, *hc);
+  if (int rc = check_launch("mc_tangent_slice_kernel")) return rc;
+  reduce_partials_kernel<<<1, 64, 0, st>>>(partials, g.blocks, K, K, moments_out, P2pPublish{});
+  if (int rc = check_launch("reduce_partials_kernel")) return rc;
+  B200SV_CUDA(cudaFreeAsync(partials, st));
+  return 0;
+}
+
+template <int MODEL>
+static int launch_tangent_slice(int gauss, double* x, double* v, double* q, const TangentState& t, long long n, long long path_offset, int init,
+                                double v_init, int nsteps, int slice_index, double forward, uint64_t seed, const LogsvTangentConsts* lc,
+                                const HestonTangentConsts* hc, double* moments_out, cudaStream_t st) {
+  if (gauss == kGaussF64)
+    return launch_tangent_slice_g<MODEL, kGaussF64>(x, v, q, t, n, path_offset, init, v_init, nsteps, slice_index, forward, seed, lc, hc, moments_out, st);
+  return launch_tangent_slice_g<MODEL, kGaussF32>(x, v, q, t, n, path_offset, init, v_init, nsteps, slice_index, forward, seed, lc, hc, moments_out, st);
+}
+
+// chain driver: per maturity tangent slice -> moments -> per-strike payoff / sensitivity sums -> finalize (stand-alone launches, fixed-order
+// reductions).  greeks_out / greeks_se_out: [1 + P][Jtot], row 0 = forward delta.
+template <int MODEL>
+static int mc_chain_greeks_host(const b200sv_logsv_params* lp, const b200sv_heston_params* hp, int M, const double* ttms, const double* forwards,
+                                const double* discfactors, const double* etas, const int* offsets, const double* strikes, const int8_t* types,
+                                long long nb_path, int nb_steps_per_year, int is_spot, int variable_type, uint64_t seed, int flags,
+                                double* prices_out, double* stderr_out, double* greeks_out, double* greeks_se_out) {
+  constexpr int NP = MODEL == 0 ? kLogsvParams : kHestonParams, KV = 3 + 2 * (1 + NP);
+  B200SV_REQUIRE(nb_path >= 1, "nb_path must be >= 1");
+  B200SV_REQUIRE(nb_steps_per_year >= 1, "nb_steps_per_year must be >= 1");
+  if (int rc = validate_chain(M, ttms, offsets, types, variable_type)) return rc;
+  const int gauss = greeks_gauss(flags);
+  if (gauss < 0) return gauss;
+  const int Jtot = offsets[M] - offsets[0], Jalloc = std::max(Jtot, 1);
+  cudaStream_t st = current_stream();
+  ensure_pool_threshold();
+  const size_t n = (size_t)nb_path;
+  const size_t state_doubles = 3 * n + 3 * (size_t)NP * n;
+  const size_t out_doubles = 2 * (size_t)Jalloc * (2 + NP);        // prices, std errors, greeks [1+P][J], greeks_se [1+P][J]
+  double *d_state = nullptr, *d_strikes = nullptr, *d_out = nullptr, *d_mom = nullptr, *d_sums = nullptr;
+  int8_t* d_types = nullptr;
+  B200SV_CUDA(cudaMallocAsync(&d_state, sizeof(double) * state_doubles, st));
+  B200SV_CUDA(cudaMallocAsync(&d_strikes, sizeof(double) * Jalloc, st));
+  B200SV_CUDA(cudaMallocAsync(&d_types, Jalloc, st));
+  B200SV_CUDA(cudaMallocAsync(&d_out, sizeof(double) * out_doubles, st));
+  B200SV_CUDA(cudaMallocAsync(&d_mom, sizeof(double) * (2 + NP), st));
+  B200SV_CUDA(cudaMallocAsync(&d_sums, sizeof(double) * KV * Jalloc, st));
+  if (Jtot > 0) {
+    B200SV_CUDA(cudaMemcpyAsync(d_strikes, strikes + offsets[0], sizeof(double) * Jtot, cudaMemcpyHostToDevice, st));
+    B200SV_CUDA(cudaMemcpyAsync(d_types, types + offsets[0], Jtot, cudaMemcpyHostToDevice, st));
+  }
+  double *x = d_state, *v = x + n, *q = v + n;
+  const TangentState t{q + n, q + n + NP * n, q + n + 2 * NP * n};
+  double *o_price = d_out, *o_se = o_price + Jalloc, *o_g = o_se + Jalloc, *o_gse = o_g + (size_t)(1 + NP) * Jalloc;
+  int rc = 0;
+  double t0 = 0.0;
+  for (int m = 0; m < M && rc == 0; ++m) {
+    int S;
+    double dt;
+    time_grid(ttms[m] - t0, nb_steps_per_year, &S, &dt);
+    t0 = ttms[m];
+    if constexpr (MODEL == 0) {
+      const LogsvTangentConsts c = make_logsv_tangent_consts(*lp, etas ? etas[m] : 1.0, is_spot != 0, dt);
+      rc = launch_tangent_slice<0>(gauss, x, v, q, t, nb_path, 0, m == 0, lp->sigma0, S, m, forwards[m], seed, &c, nullptr, d_mom, st);
+    } else {
+      const HestonTangentConsts c = make_heston_tangent_consts(*hp, dt);
+      rc = launch_tangent_slice<1>(gauss, x, v, q, t, nb_path, 0, m == 0, hp->v0, S, m, forwards[m], seed, nullptr, &c, d_mom, st);
+    }
+    if (rc) break;
+    const int J = offsets[m + 1] - offsets[m], jo = offsets[m] - offsets[0];
+    if (J == 0) continue;
+    const int chunks = (J + kGreeksStrikeChunk - 1) / kGreeksStrikeChunk;
+    const int Kpad = KV * kGreeksStrikeChunk * chunks;
+    Grid g = persistent_grid(payoff_greeks_kernel<NP>, kThreads, nb_path);
+    g.blocks = std::max(1, g.blocks / chunks);
+    double* partials = nullptr;
+    B200SV_CUDA(cudaMallocAsync(&partials, sizeof(double) * (size_t)Kpad * g.blocks, st));
+    payoff_greeks_kernel<NP><<<dim3(g.blocks, chunks), g.threads, 0, st>>>(x, q, t.dx, t.dq, nb_path, ttms[m], forwards[m], d_strikes + jo,
+                                                                           d_types + jo, J, variable_type, d_mom, partials, Kpad);
+    if ((rc = check_launch("payoff_greeks_kernel"))) break;
+    reduce_partials_kernel<<<1, 256, 0, st>>>(partials, g.blocks, Kpad, KV * J, d_sums, P2pPublish{});
+    if ((rc = check_launch("reduce_partials_kernel"))) break;
+    B200SV_CUDA(cudaFreeAsync(partials, st));
+    greeks_finalize_kernel<<<(J + 127) / 128, 128, 0, st>>>(d_sums, KV, J, Jalloc, discfactors[m], (double)nb_path, o_price + jo, o_se + jo,
+                                                            o_g + jo, o_gse + jo);
+    rc = check_launch("greeks_finalize_kernel");
+  }
+  if (rc == 0 && Jtot > 0) {
+    cudaError_t e = cudaMemcpyAsync(prices_out, o_price, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(stderr_out, o_se, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st);
+    for (int k = 0; k < 1 + NP && e == cudaSuccess; ++k) {
+      e = cudaMemcpyAsync(greeks_out + (size_t)k * Jtot, o_g + (size_t)k * Jalloc, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st);
+      if (e == cudaSuccess)
+        e = cudaMemcpyAsync(greeks_se_out + (size_t)k * Jtot, o_gse + (size_t)k * Jalloc, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st);
+    }
+    if (e != cudaSuccess) rc = fail(-2, std::string("D2H: ") + cudaGetErrorString(e));
+  }
+  cudaFreeAsync(d_state, st);
+  cudaFreeAsync(d_strikes, st);
+  cudaFreeAsync(d_types, st);
+  cudaFreeAsync(d_out, st);
+  cudaFreeAsync(d_mom, st);
+  cudaFreeAsync(d_sums, st);
+  cudaError_t e = cudaStreamSynchronize(st);
+  if (rc == 0 && e != cudaSuccess) rc = fail(-2, std::string("sync: ") + cudaGetErrorString(e));
+  return rc;
+}
+
+// one slice from the initial state (0, v_init, 0) with initial tangents, for paths [path_offset, path_offset + n) of Philox slice
+// `slice_index`; returns the terminal state and tangents [P][n] (LogSV: dv = d sigma = sigma * d log sigma)
+template <int MODEL>
+static int tangent_terminal_host(const b200sv_logsv_params* lp, const b200sv_heston_params* hp, double ttm, long long nb_path, int nb_steps_per_year,
+                                 int is_spot, double eta, uint64_t seed, int flags, int slice_index, long long path_offset, double* x, double* v,
+                                 double* q, double* dx, double* dv, double* dq) {
+  constexpr int NP = MODEL == 0 ? kLogsvParams : kHestonParams;
+  B200SV_REQUIRE(nb_path >= 1 && ttm > 0.0 && nb_steps_per_year >= 1, "nb_path, ttm, nb_steps_per_year must be positive");
+  B200SV_REQUIRE(slice_index >= 0 && path_offset >= 0, "slice_index and path_offset must be >= 0");
+  const int gauss = greeks_gauss(flags);
+  if (gauss < 0) return gauss;
+  cudaStream_t st = current_stream();
+  ensure_pool_threshold();
+  const size_t n = (size_t)nb_path, total = 3 * n + 3 * (size_t)NP * n;
+  double *d = nullptr, *d_mom = nullptr;
+  B200SV_CUDA(cudaMallocAsync(&d, sizeof(double) * total, st));
+  B200SV_CUDA(cudaMallocAsync(&d_mom, sizeof(double) * (2 + NP), st));
+  const TangentState t{d + 3 * n, d + 3 * n + NP * n, d + 3 * n + 2 * NP * n};
+  int S;
+  double dt;
+  time_grid(ttm, nb_steps_per_year, &S, &dt);
+  int rc;
+  if constexpr (MODEL == 0) {
+    const LogsvTangentConsts c = make_logsv_tangent_consts(*lp, eta, is_spot != 0, dt);
+    rc = launch_tangent_slice<0>(gauss, d, d + n, d + 2 * n, t, nb_path, path_offset, 1, lp->sigma0, S, slice_index, 1.0, seed, &c, nullptr, d_mom, st);
+  } else {
+    const HestonTangentConsts c = make_heston_tangent_consts(*hp, dt);
+    rc = launch_tangent_slice<1>(gauss, d, d + n, d + 2 * n, t, nb_path, path_offset, 1, hp->v0, S, slice_index, 1.0, seed, nullptr, &c, d_mom, st);
+  }
+  if (rc == 0) {
+    double* dst[6] = {x, v, q, dx, dv, dq};
+    const size_t cnt[6] = {n, n, n, NP * n, NP * n, NP * n};
+    const double* src[6] = {d, d + n, d + 2 * n, t.dx, t.dv, t.dq};
+    cudaError_t e = cudaSuccess;
+    for (int k = 0; k < 6 && e == cudaSuccess; ++k) e = cudaMemcpyAsync(dst[k], src[k], sizeof(double) * cnt[k], cudaMemcpyDeviceToHost, st);
+    if (e != cudaSuccess) rc = fail(-2, std::string("D2H: ") + cudaGetErrorString(e));
+  }
+  cudaFreeAsync(d, st);
+  cudaFreeAsync(d_mom, st);
+  cudaError_t e = cudaStreamSynchronize(st);
+  if (rc == 0 && e != cudaSuccess) rc = fail(-2, std::string("sync: ") + cudaGetErrorString(e));
+  if (rc == 0 && MODEL == 0)
+    for (size_t p = 0; p < (size_t)NP; ++p)
+      for (size_t i = 0; i < n; ++i) dv[p * n + i] *= v[i];
+  return rc;
+}
+
 }  // namespace b200sv
 
 #include "rough_kernels.cuh"
@@ -1478,6 +1992,41 @@ int b200sv_heston_mc_chain_batch(const b200sv_heston_params* params, int B, int 
   B200SV_REQUIRE(scheme == B200SV_HESTON_EULER_FLOOR || scheme == B200SV_HESTON_QE, "unknown Heston scheme");
   return mc_chain_host<1>(nullptr, params, M, ttms, forwards, discfactors, nullptr, offsets, strikes, types, nb_path, nb_steps_per_year, 1,
                           B200SV_LOG_RETURN, seed, flags, prices_out, stderr_out, scheme, B, ivols_out);
+}
+
+int b200sv_logsv_mc_chain_greeks(const b200sv_logsv_params* params, int M, const double* ttms, const double* forwards,
+                                 const double* discfactors, const double* etas, const int* offsets, const double* strikes,
+                                 const int8_t* types, long long nb_path, int nb_steps_per_year, int is_spot_measure, int variable_type,
+                                 uint64_t seed, int flags, double* prices_out, double* stderr_out, double* greeks_out, double* greeks_se_out) {
+  B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && stderr_out && greeks_out && greeks_se_out, "null pointer");
+  return mc_chain_greeks_host<0>(params, nullptr, M, ttms, forwards, discfactors, etas, offsets, strikes, types, nb_path, nb_steps_per_year,
+                                 is_spot_measure, variable_type, seed, flags, prices_out, stderr_out, greeks_out, greeks_se_out);
+}
+
+int b200sv_heston_mc_chain_greeks(const b200sv_heston_params* params, int M, const double* ttms, const double* forwards,
+                                  const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
+                                  long long nb_path, int nb_steps_per_year, int variable_type, uint64_t seed, int flags, int scheme,
+                                  double* prices_out, double* stderr_out, double* greeks_out, double* greeks_se_out) {
+  B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && stderr_out && greeks_out && greeks_se_out, "null pointer");
+  B200SV_REQUIRE(scheme == B200SV_HESTON_EULER_FLOOR, "pathwise sensitivities need scheme = B200SV_HESTON_EULER_FLOOR");
+  return mc_chain_greeks_host<1>(nullptr, params, M, ttms, forwards, discfactors, nullptr, offsets, strikes, types, nb_path, nb_steps_per_year, 1,
+                                 variable_type, seed, flags, prices_out, stderr_out, greeks_out, greeks_se_out);
+}
+
+int b200sv_logsv_tangent_terminal(const b200sv_logsv_params* params, double ttm, long long nb_path, int nb_steps_per_year, int is_spot_measure,
+                                  double eta, uint64_t seed, int flags, int slice_index, long long path_offset, double* x, double* sigma,
+                                  double* qvar, double* dx, double* dsigma, double* dqvar) {
+  B200SV_REQUIRE(params && x && sigma && qvar && dx && dsigma && dqvar, "null pointer");
+  return tangent_terminal_host<0>(params, nullptr, ttm, nb_path, nb_steps_per_year, is_spot_measure, eta, seed, flags, slice_index, path_offset,
+                                  x, sigma, qvar, dx, dsigma, dqvar);
+}
+
+int b200sv_heston_tangent_terminal(const b200sv_heston_params* params, double ttm, long long nb_path, int nb_steps_per_year, uint64_t seed,
+                                   int flags, int slice_index, long long path_offset, double* x, double* var, double* qvar, double* dx,
+                                   double* dvar, double* dqvar) {
+  B200SV_REQUIRE(params && x && var && qvar && dx && dvar && dqvar, "null pointer");
+  return tangent_terminal_host<1>(nullptr, params, ttm, nb_path, nb_steps_per_year, 1, 1.0, seed, flags, slice_index, path_offset, x, var, qvar,
+                                  dx, dvar, dqvar);
 }
 
 int b200sv_logsv_terminal(const b200sv_logsv_params* params, double ttm, long long nb_path, int nb_steps_per_year,

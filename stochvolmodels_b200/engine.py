@@ -94,6 +94,68 @@ def heston_mc_chain(params: C.HestonParamsC, ttms, forwards, discfactors, strike
     return C.split_chain(prices, offsets), C.split_chain(stds, offsets)
 
 
+LOGSV_GREEK_PARAMS = ("sigma0", "theta", "kappa1", "kappa2", "beta", "volvol")
+HESTON_GREEK_PARAMS = ("v0", "theta", "kappa", "rho", "volvol")
+
+
+def _greeks_result(prices, stds, greeks, greeks_se, offsets):
+    """flat library outputs -> (prices, std errors, greeks [1+P, J], greeks_se [1+P, J], offsets)"""
+    return C.split_chain(prices, offsets), C.split_chain(stds, offsets), greeks, greeks_se, offsets
+
+
+def logsv_mc_chain_greeks(params: C.LogsvParamsC, ttms, forwards, discfactors, etas, strikes_ttms, optiontypes_ttms, nb_path: int,
+                          nb_steps_per_year: int, is_spot_measure: bool, variable_type, seed: int, flags: int):
+    """prices, std errors and pathwise sensitivities of the chain in one pass (b200sv_logsv_mc_chain_greeks).  Returns (prices, std errors,
+    greeks [1+6, J], greeks_se [1+6, J], offsets): row 0 the forward delta, then LOGSV_GREEK_PARAMS; J runs over the flattened chain."""
+    vt = variable_code(variable_type)
+    M, ttms, forwards, discfactors, offsets, strikes, types = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
+    etas = C.f64(np.ones(M) if etas is None else etas)
+    J = strikes.shape[0]
+    prices, stds = np.empty(J), np.empty(J)
+    greeks, greeks_se = np.empty((1 + len(LOGSV_GREEK_PARAMS), J)), np.empty((1 + len(LOGSV_GREEK_PARAMS), J))
+    C.call("b200sv_logsv_mc_chain_greeks", byref(params), M, C.dptr(ttms), C.dptr(forwards), C.dptr(discfactors), C.dptr(etas),
+           C.iptr(offsets), C.dptr(strikes), C.i8ptr(types), int(nb_path), int(nb_steps_per_year), int(bool(is_spot_measure)), vt,
+           int(seed) & 0xFFFFFFFFFFFFFFFF, int(flags), C.dptr(prices), C.dptr(stds), C.dptr(greeks), C.dptr(greeks_se))
+    return _greeks_result(prices, stds, greeks, greeks_se, offsets)
+
+
+def heston_mc_chain_greeks(params: C.HestonParamsC, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, nb_path: int,
+                           nb_steps_per_year: int, variable_type, seed: int, flags: int, scheme: int = C.HESTON_EULER_FLOOR):
+    """Heston twin of logsv_mc_chain_greeks (b200sv_heston_mc_chain_greeks): greeks rows = forward delta, then HESTON_GREEK_PARAMS."""
+    vt = variable_code(variable_type)
+    M, ttms, forwards, discfactors, offsets, strikes, types = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
+    J = strikes.shape[0]
+    prices, stds = np.empty(J), np.empty(J)
+    greeks, greeks_se = np.empty((1 + len(HESTON_GREEK_PARAMS), J)), np.empty((1 + len(HESTON_GREEK_PARAMS), J))
+    C.call("b200sv_heston_mc_chain_greeks", byref(params), M, C.dptr(ttms), C.dptr(forwards), C.dptr(discfactors), C.iptr(offsets),
+           C.dptr(strikes), C.i8ptr(types), int(nb_path), int(nb_steps_per_year), vt, int(seed) & 0xFFFFFFFFFFFFFFFF, int(flags),
+           int(scheme), C.dptr(prices), C.dptr(stds), C.dptr(greeks), C.dptr(greeks_se))
+    return _greeks_result(prices, stds, greeks, greeks_se, offsets)
+
+
+def logsv_tangent_terminal(params: C.LogsvParamsC, ttm: float, nb_path: int, nb_steps_per_year: int, is_spot_measure: bool, eta: float,
+                           seed: int, flags: int, slice_index: int = 0, path_offset: int = 0):
+    """one slice of the tangent stepper from (0, sigma0, 0): (x, sigma, qvar, dx [6, n], dsigma [6, n], dqvar [6, n])"""
+    P = len(LOGSV_GREEK_PARAMS)
+    x, s, q = np.empty(nb_path), np.empty(nb_path), np.empty(nb_path)
+    dx, ds, dq = np.empty((P, nb_path)), np.empty((P, nb_path)), np.empty((P, nb_path))
+    C.call("b200sv_logsv_tangent_terminal", byref(params), float(ttm), int(nb_path), int(nb_steps_per_year), int(bool(is_spot_measure)),
+           float(eta), int(seed) & 0xFFFFFFFFFFFFFFFF, int(flags), int(slice_index), int(path_offset), C.dptr(x), C.dptr(s), C.dptr(q),
+           C.dptr(dx), C.dptr(ds), C.dptr(dq))
+    return x, s, q, dx, ds, dq
+
+
+def heston_tangent_terminal(params: C.HestonParamsC, ttm: float, nb_path: int, nb_steps_per_year: int, seed: int, flags: int,
+                            slice_index: int = 0, path_offset: int = 0):
+    """one slice of the Heston tangent stepper from (0, v0, 0): (x, var, qvar, dx [5, n], dvar [5, n], dqvar [5, n])"""
+    P = len(HESTON_GREEK_PARAMS)
+    x, v, q = np.empty(nb_path), np.empty(nb_path), np.empty(nb_path)
+    dx, dv, dq = np.empty((P, nb_path)), np.empty((P, nb_path)), np.empty((P, nb_path))
+    C.call("b200sv_heston_tangent_terminal", byref(params), float(ttm), int(nb_path), int(nb_steps_per_year), int(seed) & 0xFFFFFFFFFFFFFFFF,
+           int(flags), int(slice_index), int(path_offset), C.dptr(x), C.dptr(v), C.dptr(q), C.dptr(dx), C.dptr(dv), C.dptr(dq))
+    return x, v, q, dx, dv, dq
+
+
 def logsv_mc_chain_batch(params_list: Sequence[C.LogsvParamsC], ttms, forwards, discfactors, etas, strikes_ttms, optiontypes_ttms,
                          nb_path: int, nb_steps_per_year: int, is_spot_measure: bool, seed: int, flags: int, with_ivols: bool = True):
     """B parameter sets through the fused chain MC on the SAME seed in one call -> (prices, std errors, ivols | None), each [B, J]."""

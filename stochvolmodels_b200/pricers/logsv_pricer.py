@@ -269,6 +269,25 @@ class LogSVPricer(ModelPricer):
                                      exchange=kwargs.get("exchange"))
 
     @timer
+    def model_mc_chain_greeks(self, option_chain: OptionChain, params: LogSvParams, is_spot_measure: bool = True,
+                              variable_type: VariableType = VariableType.LOG_RETURN, nb_path: int = 100000,
+                              nb_steps: Optional[int] = None, **kwargs):
+        """MC prices and standard errors as ``model_mc_price_chain`` (same defaults, ``seed`` / ``gauss`` kwargs, same numbers on the same
+        seed) plus pathwise sensitivities in the same pass: the forward delta and d price / d (sigma0, theta, kappa1, kappa2, beta, volvol),
+        each with its standard error -> ``McChainGreeks``.  ``kappa2`` is the value after ``__post_init__`` and is held fixed when kappa1 or
+        theta moves; the vol backbone and discount factors are not differentiated.  fp64 state only; no rough-vol route, no ``exchange``.
+        Under torch.distributed every rank prices all paths (replicated, bit-identical results)."""
+        from .mc_greeks import check_greeks_kwargs, to_mc_chain_greeks
+        check_greeks_kwargs(kwargs)
+        vt = engine.variable_code(variable_type)
+        flags = engine.mc_flags("fp64", kwargs.get("gauss", "fp32"))
+        res = engine.logsv_mc_chain_greeks(_params_c(params), option_chain.ttms, option_chain.forwards, option_chain.discfactors,
+                                           params.get_vol_backbone_etas(ttms=option_chain.ttms), option_chain.strikes_ttms,
+                                           option_chain.optiontypes_ttms, nb_path, nb_steps or int(360 * np.max(option_chain.ttms)) + 1,
+                                           is_spot_measure, vt, _shared_seed(kwargs.get("seed")), flags)
+        return to_mc_chain_greeks(res, engine.LOGSV_GREEK_PARAMS)
+
+    @timer
     def simulate_vol_paths(self, params: LogSvParams, brownians: np.ndarray = None, ttm: float = 1.0, nb_path: int = 100000,
                            is_spot_measure: bool = True, nb_steps: int = None, year_days: int = 360, **kwargs) -> Tuple[np.ndarray, np.ndarray]:
         """volatility paths on the time grid, ``(sigma_t [nb_steps+1, nb_path], grid_t)`` (reference :561-587): note the reference
