@@ -318,6 +318,14 @@ int b200sv_dev_rough_logsv_slice(double* log_spot, double* vol_factors, double* 
 int b200sv_debug_exp_pair(const double* L, long long n, double* out);
 /* same for the variant the stepper runs on its table-unit state: out[2i] = exp(Ls[i] ln2/256), out[2i+1] = exp(-Ls[i] ln2/256) */
 int b200sv_debug_exp_pair_scaled(const double* Ls, long long n, double* out);
+/* test hook: the Box-Muller device functions on caller-chosen Philox output words (words [n][4] = r0..r3, host; z_out [n][4] host doubles).
+ * flags B200SV_GAUSS_F64: box_muller_f64_fast(r0..r3) -> (z0, z1, NaN, NaN); B200SV_GAUSS_F64_PAIRED: box_muller_f64_u32 on (r0, r1) and on
+ * (r2, r3); otherwise the default float draw box_muller_f32 on the same two pairs.  The shared tables are initialised as in the kernels. */
+int b200sv_debug_box_muller(const uint32_t* words, long long n, int flags, double* z_out);
+/* test hook: out[i] = op(a[i], b[i]) through the fp64 device helpers (host arrays; b is read by B200SV_DEBUG_FAST_DIV only, else may be NULL):
+ * fast_div(a, b), fast_sqrt(a), fast_sqrt_pos(a), neg2_log(a) = -2 ln(a), exp_table(a) */
+enum { B200SV_DEBUG_FAST_DIV = 0, B200SV_DEBUG_FAST_SQRT = 1, B200SV_DEBUG_FAST_SQRT_POS = 2, B200SV_DEBUG_NEG2_LOG = 3, B200SV_DEBUG_EXP_TABLE = 4 };
+int b200sv_debug_fastmath(int op, const double* a, const double* b, long long n, double* out);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Fourier / MGF, host-level

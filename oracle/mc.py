@@ -28,10 +28,22 @@ def set_time_grid(ttm: float, nb_steps_per_year: int = 360):
 # --------------------------------------------------------------------------------------------
 # steppers with caller-supplied unit normals Z0, Z1 of shape (S, N)
 # --------------------------------------------------------------------------------------------
-def logsv_step_fixed(x, sigma, qvar, Z0, Z1, dt, theta, kappa1, kappa2, beta, volvol, eta=1.0, is_spot_measure=True):
+# the fp64 kernels' log-vol guard (fastmath64.cuh, state in table units Ls = L 256/ln2): a value trips it when the high word of |Ls| exceeds
+# that of 258530, i.e. |Ls| >= 258530.125, and is then set to +-258530 (699.997 in log units)
+LOG_VOL_CLAMP = 258530.0 * np.log(2.0) / 256.0
+LOG_VOL_TRIP = 258530.125 * np.log(2.0) / 256.0
+
+
+def _clamp_log_vol(L):
+    return np.where(np.abs(L) < LOG_VOL_TRIP, L, np.copysign(LOG_VOL_CLAMP, L))
+
+
+def logsv_step_fixed(x, sigma, qvar, Z0, Z1, dt, theta, kappa1, kappa2, beta, volvol, eta=1.0, is_spot_measure=True, clamp=False):
     """``simulate_logsv_x_vol_terminal`` with W0/W1/dt supplied (pricers/logsv_pricer.py:1027-1047).
 
-    Evaluation order follows the reference expression by expression (it is ``fastmath=False``)."""
+    Evaluation order follows the reference expression by expression (it is ``fastmath=False``).
+    clamp=True restates the fp64 kernels' guarded re-run of a path whose log-vol leaves the representable range: the initial and
+    every updated log-vol that trips the guard are set to +-LOG_VOL_CLAMP.  The reference has no clamp; the default keeps its recursion."""
     x = np.array(x, dtype=np.float64, copy=True)
     sigma = np.array(sigma, dtype=np.float64, copy=True)
     qvar = np.array(qvar, dtype=np.float64, copy=True)
@@ -43,12 +55,16 @@ def logsv_step_fixed(x, sigma, qvar, Z0, Z1, dt, theta, kappa1, kappa2, beta, vo
     vartheta2 = beta * beta + volvol * volvol
     eta2 = eta * eta
     L = np.log(sigma)
+    if clamp:
+        L = _clamp_log_vol(L)
     for z0, z1 in zip(Z0, Z1):
         w0 = sdt * z0
         w1 = sdt * z1
         s2dt = eta2 * sigma * sigma * dt
         x = x + alpha * 0.5 * s2dt + eta * sigma * w0
         L = L + ((kappa1 * theta / sigma - kappa1) + kappa2 * (theta - sigma) + adj * sigma - 0.5 * vartheta2) * dt + beta * w0 + volvol * w1
+        if clamp:
+            L = _clamp_log_vol(L)
         sigma = np.exp(L)
         qvar = qvar + 0.5 * (s2dt + eta2 * sigma * sigma * dt)
     return x, sigma, qvar

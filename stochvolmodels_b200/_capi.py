@@ -21,6 +21,7 @@ LOG_RETURN, Q_VAR, SIGMA = 1, 2, 3
 ORDER_FIRST, ORDER_SECOND = 1, 2
 STATE_F64, STATE_F32, GAUSS_F32, GAUSS_F64, GAUSS_F64_PAIRED = 0, 1, 0, 2, 4
 HESTON_EULER_FLOOR, HESTON_QE = 0, 1
+DEBUG_FAST_DIV, DEBUG_FAST_SQRT, DEBUG_FAST_SQRT_POS, DEBUG_NEG2_LOG, DEBUG_EXP_TABLE = 0, 1, 2, 3, 4
 TYPE_CODES = {"C": CALL, "P": PUT, "IC": INV_CALL, "IP": INV_PUT}
 
 
@@ -110,6 +111,8 @@ SIGNATURES = {
                                      c_uint64, c_int, c_void_p, c_void_p, c_void_p],
     "b200sv_debug_exp_pair": [_dp, c_longlong, _dp],
     "b200sv_debug_exp_pair_scaled": [_dp, c_longlong, _dp],
+    "b200sv_debug_box_muller": [POINTER(ctypes.c_uint32), c_longlong, c_int, _dp],
+    "b200sv_debug_fastmath": [c_int, _dp, _dp, c_longlong, _dp],
     "b200sv_logsv_price_chain": [_lp, c_int, _dp, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_int, c_int, c_double, c_int, _dp, _dp, _dp],
     "b200sv_heston_price_chain": [_hp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_double, c_int, _dp, _dp],
     "b200sv_logsv_price_chain_batch": [_lp, c_int, c_int, _dp, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_int, c_double, c_int, _dp, _dp],

@@ -12,8 +12,9 @@
 //   sin/cos(2 pi u2): j = 8 leading bits of u2 (table of sin/cos at the interval centres), f = u2 - centre, |2 pi f| <= 0.0123:
 //                     sin to f^5, cos to f^6 (next terms 8e-18, 1e-20), angle addition.                               12 fp64
 //   z0 = R cos, z1 = R sin                                                                                             2 fp64
-// => 27 fp64-pipe instructions per pair instead of ~80.  Max observed error against numpy: 4e-16 absolute on the normals
-// (tests/test_gpu_mc.py::test_device_normals_match_oracle).  Tables: 2 KB + 4 KB of shared memory per CTA (gauss64_table_init()).
+// => 27 fp64-pipe instructions per pair instead of ~80.  Max error against 40-digit references on every table seam and at u1 = 2^-52
+// (R = 8.49) and 1 - 2^-52: 1.89 x 2^-52 max(1, R) on the normals, an absolute error that grows with R (one ulp of R = 8.49 is 1.8e-15)
+// (tests/test_gpu_mc_edges.py, H100).  Tables: 2 KB + 4 KB of shared memory per CTA (gauss64_table_init()).
 #pragma once
 #include <cstdint>
 

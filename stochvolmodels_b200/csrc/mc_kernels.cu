@@ -1277,6 +1277,52 @@ __global__ void exp_pair_scaled_kernel(const double* __restrict__ Ls, long long 
   out[2 * i + 1] = b;
 }
 
+// Box-Muller self-test kernel (tests): the draw functions of philox.cuh / gauss64.cuh on caller-chosen Philox output words, tables
+// initialised as the production kernels do.  out[4i..4i+3]: fp64 mode (z0, z1, NaN, NaN); the two-pair modes (z0, z1) of (r0, r1), then of (r2, r3)
+template <int GAUSS>
+__global__ void box_muller_words_kernel(const uint4* __restrict__ words, long long n, double* __restrict__ out) {
+  if constexpr (GAUSS != kGaussF32) gauss64_table_init();
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint4 r = words[i];
+  double z[4];
+  if constexpr (GAUSS == kGaussF64) {
+    box_muller_f64_fast(r, z[0], z[1]);
+    z[2] = z[3] = __longlong_as_double(0x7ff8000000000000ll);
+  } else if constexpr (GAUSS == kGaussF64Paired) {
+    box_muller_f64_u32(r.x, r.y, z[0], z[1]);
+    box_muller_f64_u32(r.z, r.w, z[2], z[3]);
+  } else {
+    float a, b, c, d;
+    box_muller_f32(r.x, r.y, a, b);
+    box_muller_f32(r.z, r.w, c, d);
+    z[0] = a;
+    z[1] = b;
+    z[2] = c;
+    z[3] = d;
+  }
+#pragma unroll
+  for (int k = 0; k < 4; ++k) out[4 * i + k] = z[k];
+}
+
+// fp64 helper self-test kernel (tests): out[i] = op(a[i], b[i]) for the B200SV_DEBUG_* codes of b200sv.h
+__global__ void fastmath_kernel(int op, const double* __restrict__ a, const double* __restrict__ b, long long n, double* __restrict__ out) {
+  exp_table_init();
+  gauss64_table_init();
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const double x = a[i];
+  double y;
+  switch (op) {
+    case B200SV_DEBUG_FAST_DIV: y = fast_div(x, b[i]); break;
+    case B200SV_DEBUG_FAST_SQRT: y = fast_sqrt(x); break;
+    case B200SV_DEBUG_FAST_SQRT_POS: y = fast_sqrt_pos(x); break;
+    case B200SV_DEBUG_NEG2_LOG: y = neg2_log((uint32_t)__double2hiint(x), (uint32_t)__double2loint(x)); break;
+    default: y = exp_table(x); break;
+  }
+  out[i] = y;
+}
+
 // --------------------------------------------------------------------------------------------------------------------
 // host side
 // --------------------------------------------------------------------------------------------------------------------
@@ -2316,6 +2362,54 @@ int b200sv_debug_exp_pair_scaled(const double* Ls, long long n, double* out /* 2
   int rc = check_launch("exp_pair_scaled_kernel");
   if (rc == 0) B200SV_CUDA(cudaMemcpyAsync(out, dout, sizeof(double) * 2 * n, cudaMemcpyDeviceToHost, st));
   cudaFreeAsync(dl, st);
+  cudaFreeAsync(dout, st);
+  B200SV_CUDA(cudaStreamSynchronize(st));
+  return rc;
+}
+
+int b200sv_debug_box_muller(const uint32_t* words, long long n, int flags, double* z_out) {
+  B200SV_REQUIRE(words && z_out && n >= 1, "null pointer / n");
+  const int g = gauss_mode(flags);
+  B200SV_REQUIRE(g >= 0, "B200SV_GAUSS_F64 and B200SV_GAUSS_F64_PAIRED are mutually exclusive");
+  cudaStream_t st = current_stream();
+  uint4* dw = nullptr;
+  double* dout = nullptr;
+  B200SV_CUDA(cudaMallocAsync(&dw, sizeof(uint4) * n, st));
+  B200SV_CUDA(cudaMallocAsync(&dout, sizeof(double) * 4 * n, st));
+  B200SV_CUDA(cudaMemcpyAsync(dw, words, sizeof(uint4) * n, cudaMemcpyHostToDevice, st));
+  const int blocks = (int)((n + 127) / 128);
+  if (g == kGaussF64)
+    box_muller_words_kernel<kGaussF64><<<blocks, 128, 0, st>>>(dw, n, dout);
+  else if (g == kGaussF64Paired)
+    box_muller_words_kernel<kGaussF64Paired><<<blocks, 128, 0, st>>>(dw, n, dout);
+  else
+    box_muller_words_kernel<kGaussF32><<<blocks, 128, 0, st>>>(dw, n, dout);
+  int rc = check_launch("box_muller_words_kernel");
+  if (rc == 0) B200SV_CUDA(cudaMemcpyAsync(z_out, dout, sizeof(double) * 4 * n, cudaMemcpyDeviceToHost, st));
+  cudaFreeAsync(dw, st);
+  cudaFreeAsync(dout, st);
+  B200SV_CUDA(cudaStreamSynchronize(st));
+  return rc;
+}
+
+int b200sv_debug_fastmath(int op, const double* a, const double* b, long long n, double* out) {
+  B200SV_REQUIRE(a && out && n >= 1, "null pointer / n");
+  B200SV_REQUIRE(op >= B200SV_DEBUG_FAST_DIV && op <= B200SV_DEBUG_EXP_TABLE, "unknown B200SV_DEBUG_* operation");
+  B200SV_REQUIRE(op != B200SV_DEBUG_FAST_DIV || b, "fast_div needs the divisors b");
+  cudaStream_t st = current_stream();
+  double *da = nullptr, *db = nullptr, *dout = nullptr;
+  B200SV_CUDA(cudaMallocAsync(&da, sizeof(double) * n, st));
+  B200SV_CUDA(cudaMallocAsync(&dout, sizeof(double) * n, st));
+  B200SV_CUDA(cudaMemcpyAsync(da, a, sizeof(double) * n, cudaMemcpyHostToDevice, st));
+  if (op == B200SV_DEBUG_FAST_DIV) {
+    B200SV_CUDA(cudaMallocAsync(&db, sizeof(double) * n, st));
+    B200SV_CUDA(cudaMemcpyAsync(db, b, sizeof(double) * n, cudaMemcpyHostToDevice, st));
+  }
+  fastmath_kernel<<<(int)((n + 127) / 128), 128, 0, st>>>(op, da, db, n, dout);
+  int rc = check_launch("fastmath_kernel");
+  if (rc == 0) B200SV_CUDA(cudaMemcpyAsync(out, dout, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
+  cudaFreeAsync(da, st);
+  if (db) cudaFreeAsync(db, st);
   cudaFreeAsync(dout, st);
   B200SV_CUDA(cudaStreamSynchronize(st));
   return rc;

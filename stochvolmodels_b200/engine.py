@@ -5,6 +5,7 @@ the CUDA library.  No function in this module computes a price on the CPU.
 """
 from __future__ import annotations
 
+import ctypes
 import os
 from ctypes import byref
 from typing import List, Optional, Sequence, Tuple
@@ -374,6 +375,23 @@ def debug_exp_pair_scaled(Ls):
     out = np.empty(2 * Ls.shape[0])
     C.call("b200sv_debug_exp_pair_scaled", C.dptr(Ls), Ls.shape[0], C.dptr(out))
     return out[0::2].copy(), out[1::2].copy()
+
+
+def debug_box_muller(words, flags: int):
+    """the device Box-Muller on Philox output words [n, 4] (uint32) -> [n, 4] float64 normals (b200sv_debug_box_muller)."""
+    w = np.ascontiguousarray(np.asarray(words, dtype=np.uint32).reshape(-1, 4))
+    out = np.empty((w.shape[0], 4))
+    C.call("b200sv_debug_box_muller", w.ctypes.data_as(ctypes.POINTER(ctypes.c_uint32)), w.shape[0], int(flags), C.dptr(out))
+    return out
+
+
+def debug_fastmath(op: int, a, b=None):
+    """op(a, b) through one of the fp64 device helpers, op = C.DEBUG_* (b200sv_debug_fastmath)."""
+    a = C.f64(np.atleast_1d(a))
+    b = None if b is None else C.f64(np.broadcast_to(b, a.shape))
+    out = np.empty_like(a)
+    C.call("b200sv_debug_fastmath", int(op), C.dptr(a), C.dptr(b), a.shape[0], C.dptr(out))
+    return out
 
 
 # ---- Fourier / MGF --------------------------------------------------------------------------------------------------------

@@ -194,6 +194,50 @@ def test_large_n_fp64_chain_vs_c_port(cuda_lib):
         np.testing.assert_allclose(eg[m], ec[m], rtol=1e-8)
 
 
+@pytest.mark.parametrize("model,N", [("logsv", 4_000_003), ("heston", 500_001)])
+def test_large_n_fp64_chain_vs_c_port_multi_launch_driver(cuda_lib, model, N):
+    """BTC chain, as test_large_n_fp64_chain_vs_c_port, at path counts just above the cooperative driver's limits (4e6 LogSV, 5e5 Heston):
+    the multi-launch driver (slice kernel, stand-alone payoff kernels, reductions) against the C port on the same Philox stream.  The LogSV
+    case gives slice 2 mixed C / P / IC / IP codes, so the general payoff kernel runs next to the vanilla one."""
+    from stochvolmodels_b200 import engine, get_btc_test_chain_data
+    chain = get_btc_test_chain_data()
+    seed, flags = 31337, engine.mc_flags("fp64", "fp64")
+    types = list(chain.optiontypes_ttms)
+    if model == "logsv":
+        types[2] = np.array(["C", "P", "IC", "IP"] * 4)[:len(chain.strikes_ttms[2])]
+        params, npy = (0.8376, 1.0413, 3.1844, 3.058, 0.1514, 1.8458), 252
+        pc, ec = cport.mc_chain("logsv", params, chain.ttms, chain.forwards, chain.discfactors, None, chain.strikes_ttms, types, N, npy, True, 1,
+                                seed, "f64")
+        pg, eg = engine.logsv_mc_chain(engine.logsv_params_c(*params), chain.ttms, chain.forwards, chain.discfactors, None, chain.strikes_ttms,
+                                       types, N, npy, True, 1, seed, flags)
+    else:
+        params, npy = (0.04, 0.04, 4.0, -0.5, 0.4), 360
+        pc, ec = cport.mc_chain("heston", params, chain.ttms, chain.forwards, chain.discfactors, None, chain.strikes_ttms, types, N, npy, True, 1,
+                                seed, "f64")
+        pg, eg = engine.heston_mc_chain(engine.heston_params_c(*params), chain.ttms, chain.forwards, chain.discfactors, chain.strikes_ttms, types,
+                                        N, npy, 1, seed, flags)
+    for m in range(4):
+        np.testing.assert_allclose(pg[m], pc[m], rtol=1e-9)
+        np.testing.assert_allclose(eg[m], ec[m], rtol=1e-8)
+
+
+def test_small_n_same_normals_tests_on_the_multi_launch_driver(cuda_lib):
+    """The same-normals chain tests run at path counts the cooperative driver serves.  Re-run them in a process that forces the
+    multi-launch driver (B200SV_CHAIN_COOP=0; the choice is cached per process): at 1 to 20000 paths most of its CTAs are empty, which
+    is where the vanilla payoff kernel's per-CTA path count and the grid / strike-chunk split matter."""
+    import os
+    import subprocess
+    import sys
+    from conftest import ROOT
+    tests = ["fused_logsv_kernel_vs_oracle_same_normals", "fused_heston_kernel_vs_oracle_same_normals",
+             "edge_cases_ragged_chain_many_strikes_single_step_tiny_path_counts", "qvar_payoffs_in_fused_chain"]
+    env = dict(os.environ, B200SV_CHAIN_COOP="0")
+    r = subprocess.run([sys.executable, "-m", "pytest", "-q", "-m", "gpu", "-p", "no:cacheprovider", os.path.join("tests", "test_gpu_mc.py"),
+                        "-k", " or ".join(tests)], cwd=ROOT, env=env, capture_output=True, text=True, timeout=900)
+    assert r.returncode == 0, r.stdout[-4000:] + r.stderr[-2000:]
+    assert "8 passed" in r.stdout, r.stdout[-2000:]
+
+
 def _assert_within_3se(p_gpu, se_gpu, p_ref, se_ref, what):
     """MC-vs-MC gate.  z uses the combined standard error of the two independent samples.  Every strike must be within 4 SE
     (the reference's own bar: tests/test_logsv_characterization.py:407, test_heston_characterization.py:292) and at least 90% of
