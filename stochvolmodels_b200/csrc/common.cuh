@@ -23,6 +23,8 @@ inline int fail(int code, const std::string& msg) {
 // mc_kernels.cu; the other translation units reach it through these accessors (one shared library, one thread-local).
 cudaStream_t& current_stream_ref();
 inline cudaStream_t current_stream() { return current_stream_ref(); }
+// Kernel launches of the calling thread since b200sv_reset_launch_count (b200sv_launch_count); defined once in mc_kernels.cu like the stream.
+long long& launch_count_ref();
 
 #define B200SV_CUDA(call)                                                                           \
   do {                                                                                              \
@@ -35,6 +37,52 @@ inline cudaStream_t current_stream() { return current_stream_ref(); }
   do {                                                                                              \
     if (!(cond)) return ::b200sv::fail(-1, std::string("invalid argument: ") + (msg));              \
   } while (0)
+
+// after every kernel launch: a launch error is reported under `what`, a successful launch is counted.  Launch APIs that return their
+// error (cudaLaunchCooperativeKernel) pass it as `e`.
+inline int check_launch(const char* what, cudaError_t e = cudaGetLastError()) {
+  if (e != cudaSuccess) return fail(-2, std::string(what) + ": " + cudaGetErrorString(e));
+  ++launch_count_ref();
+  return 0;
+}
+
+struct DevBuf {   // RAII for stream-ordered temporaries
+  void* p = nullptr;
+  cudaStream_t st;
+  explicit DevBuf(cudaStream_t s) : st(s) {}
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  cudaError_t alloc(size_t n) { return cudaMallocAsync(&p, n ? n : 1, st); }
+  ~DevBuf() {
+    if (p) cudaFreeAsync(p, st);
+  }
+  template <typename T>
+  T* as() const {
+    return (T*)p;
+  }
+};
+
+// Every host-level call declares one before its first stream operation and ends with `return sync.done();`, which waits for the
+// stream and reports a failed wait (a kernel fault surfaces here).  An early error return waits in the destructor instead, so no
+// copy or kernel the call queued still reads or writes the caller's host buffers after it returns.
+class StreamSync {
+ public:
+  explicit StreamSync(cudaStream_t s) : st_(s) {}
+  StreamSync(const StreamSync&) = delete;
+  StreamSync& operator=(const StreamSync&) = delete;
+  ~StreamSync() {
+    if (!waited_) cudaStreamSynchronize(st_);
+  }
+  int done() {
+    waited_ = true;
+    B200SV_CUDA(cudaStreamSynchronize(st_));
+    return 0;
+  }
+
+ private:
+  cudaStream_t st_;
+  bool waited_ = false;
+};
 
 inline int device_sm_count() {
   int dev = 0, sms = 132;

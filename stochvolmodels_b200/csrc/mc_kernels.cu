@@ -34,10 +34,13 @@
 
 namespace b200sv {
 
-static thread_local long long g_launches = 0;
 cudaStream_t& current_stream_ref() {
   static thread_local cudaStream_t st = nullptr;
   return st;
+}
+long long& launch_count_ref() {
+  static thread_local long long n = 0;
+  return n;
 }
 constexpr int kThreads = 256;
 #ifndef B200SV_SLICE_PREFETCH
@@ -1369,70 +1372,10 @@ static P2pGather make_gather(P2pCtx* c) {
   return g;
 }
 
-static int check_launch(const char* what) {
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(-2, std::string(what) + ": " + cudaGetErrorString(e));
-  ++g_launches;
-  return 0;
-}
-
 // int(ttm * n) + 1 and dt = linspace(0, ttm, S+1)[1] - [0] (utils/funcs.py:44-47; numpy linspace: step = ttm / S, y[1] = 1*step)
 static void time_grid(double ttm, int n_per_year, int* S, double* dt) {
   *S = (int)(ttm * (double)n_per_year) + 1;
   *dt = (*S == 1) ? ttm : ttm / (double)(*S);   // linspace sets the LAST point to `stop` exactly; with S == 1 y[1] is that point
-}
-
-template <int MODEL, typename Real, int G64>
-static int launch_slice_t(void* x, void* v, void* q, long long n, long long path_offset, int init, double v_init, int nsteps,
-                          int slice_index, double forward, uint64_t seed, const LogsvConsts* lc, const HestonConsts* hc,
-                          double* moments_out, cudaStream_t st, P2pCtx* p2p = nullptr) {
-  SliceArgs<Real> a;
-  a.x = (Real*)x;
-  a.v = (Real*)v;
-  a.q = (Real*)q;
-  a.n = n;
-  a.path_offset = (unsigned long long)path_offset;
-  a.init = init;
-  a.v_init = v_init;
-  a.nsteps = nsteps;
-  a.slice = (unsigned int)slice_index;
-  a.seed = seed;
-  a.forward = forward;
-  const bool qe = MODEL == 1 && hc->qe;
-  Grid g;
-  if constexpr (MODEL == 0)
-    g = persistent_grid(mc_slice_kernel<LogsvPath<Real>, LogsvConsts, Real, G64>, kSliceThreads, n);
-  else if (qe)
-    g = persistent_grid(mc_slice_kernel<HestonPath<Real, true>, HestonConsts, Real, G64>, kSliceThreads, n);
-  else
-    g = persistent_grid(mc_slice_kernel<HestonPath<Real, false>, HestonConsts, Real, G64>, kSliceThreads, n);
-  size_t dyn_smem = 0;
-#ifdef B200SV_TUNING   // occupancy sweep for profiles/: cap resident CTAs per SM with dynamic shared memory (tuning builds only)
-  if (const char* e = getenv("B200SV_DEBUG_BLOCKS_PER_SM")) {
-    const int bps = atoi(e);
-    if (bps > 0) {
-      dyn_smem = (size_t)(200 * 1024) / bps;
-      if constexpr (MODEL == 0)
-        cudaFuncSetAttribute(mc_slice_kernel<LogsvPath<Real>, LogsvConsts, Real, G64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn_smem);
-      g.blocks = (int)std::min<long long>((long long)device_sm_count() * bps, (n + kSliceThreads - 1) / kSliceThreads);
-    }
-  }
-#endif
-  double* partials = nullptr;
-  ensure_pool_threshold();      // device-level callers too: a pool that trims at every synchronisation stalls the whole node (DESIGN.md 5)
-  B200SV_CUDA(cudaMallocAsync(&partials, sizeof(double) * 2 * g.blocks, st));
-  a.partials = partials;
-  if constexpr (MODEL == 0)
-    mc_slice_kernel<LogsvPath<Real>, LogsvConsts, Real, G64><<<g.blocks, g.threads, dyn_smem, st>>>(a, *lc);
-  else if (qe)
-    mc_slice_kernel<HestonPath<Real, true>, HestonConsts, Real, G64><<<g.blocks, g.threads, dyn_smem, st>>>(a, *hc);
-  else
-    mc_slice_kernel<HestonPath<Real, false>, HestonConsts, Real, G64><<<g.blocks, g.threads, dyn_smem, st>>>(a, *hc);
-  if (int rc = check_launch("mc_slice_kernel")) return rc;
-  reduce_partials_kernel<<<1, 64, 0, st>>>(partials, g.blocks, 2, 2, moments_out, make_publish(p2p, st));   // exchange #1 (producer)
-  if (int rc = check_launch("reduce_partials_kernel")) return rc;
-  B200SV_CUDA(cudaFreeAsync(partials, st));
-  return 0;
 }
 
 // B200SV_GAUSS_* bits -> GaussMode (philox.cuh); -1 = contradictory
@@ -1442,22 +1385,90 @@ static int gauss_mode(int flags) {
   return paired ? kGaussF64Paired : (g64 ? kGaussF64 : kGaussF32);
 }
 
-template <int MODEL>
-static int launch_slice(void* x, void* v, void* q, long long n, long long path_offset, int init, double v_init, int nsteps,
-                        int slice_index, double forward, uint64_t seed, int flags, const LogsvConsts* lc, const HestonConsts* hc,
-                        double* moments_out, cudaStream_t st, P2pCtx* p2p = nullptr) {
-  const bool f32 = flags & B200SV_STATE_F32;
+// ---- model dispatch ------------------------------------------------------------------------------------------------------
+// The parameter type picks the model and its consts; the consts type picks the kernel instantiation (HestonConsts::qe the scheme).
+static LogsvConsts slice_consts(const b200sv_logsv_params& p, double eta, bool spot, double dt, int) { return make_logsv_consts(p, eta, spot, dt); }
+static HestonConsts slice_consts(const b200sv_heston_params& p, double, bool, double dt, int scheme) { return make_heston_consts(p, dt, scheme); }
+static LogsvTangentConsts tangent_consts(const b200sv_logsv_params& p, double eta, bool spot, double dt) {
+  return make_logsv_tangent_consts(p, eta, spot, dt);
+}
+static HestonTangentConsts tangent_consts(const b200sv_heston_params& p, double, bool, double dt) { return make_heston_tangent_consts(p, dt); }
+static double v_init(const b200sv_logsv_params& p) { return p.sigma0; }
+static double v_init(const b200sv_heston_params& p) { return p.v0; }
+template <typename TConsts>
+using TangentPathOf = std::conditional_t<std::is_same<TConsts, LogsvTangentConsts>::value, LogsvTangentPath, HestonTangentPath>;
+
+// (model, Heston scheme, state precision Real, Gaussian mode g) -> mc_slice_kernel; nullptr: the paired check mode on fp32 state
+template <typename Real, typename Consts>
+using SliceKernel = void (*)(SliceArgs<Real>, Consts);
+template <typename Real, typename Path, typename Consts>
+static SliceKernel<Real, Consts> slice_kernel_g(int g) {
+  if (g == kGaussF32) return mc_slice_kernel<Path, Consts, Real, kGaussF32>;
+  if (g == kGaussF64) return mc_slice_kernel<Path, Consts, Real, kGaussF64>;
+  if constexpr (std::is_same<Real, double>::value) return mc_slice_kernel<Path, Consts, Real, kGaussF64Paired>;
+  return nullptr;
+}
+template <typename Real>
+static SliceKernel<Real, LogsvConsts> slice_kernel(const LogsvConsts&, int g) { return slice_kernel_g<Real, LogsvPath<Real>, LogsvConsts>(g); }
+template <typename Real>
+static SliceKernel<Real, HestonConsts> slice_kernel(const HestonConsts& c, int g) {
+  return c.qe ? slice_kernel_g<Real, HestonPath<Real, true>, HestonConsts>(g) : slice_kernel_g<Real, HestonPath<Real, false>, HestonConsts>(g);
+}
+
+// (model, Heston scheme, Gaussian mode fp32 | fp64) -> mc_chain_coop_kernel (fp64 state)
+template <typename Consts>
+using CoopKernel = void (*)(CoopArgs, const CoopSliceSpec<Consts>*);
+template <typename Path, typename Consts>
+static CoopKernel<Consts> coop_kernel_g(int g) {
+  return g == kGaussF64 ? mc_chain_coop_kernel<Path, Consts, kGaussF64> : mc_chain_coop_kernel<Path, Consts, kGaussF32>;
+}
+static CoopKernel<LogsvConsts> coop_kernel(const LogsvConsts&, int g) { return coop_kernel_g<LogsvPath<double>, LogsvConsts>(g); }
+static CoopKernel<HestonConsts> coop_kernel(const HestonConsts& c, int g) {
+  return c.qe ? coop_kernel_g<HestonPath<double, true>, HestonConsts>(g) : coop_kernel_g<HestonPath<double, false>, HestonConsts>(g);
+}
+
+// ---- launchers ---------------------------------------------------------------------------------------------------------
+// one maturity slice on paths [path_offset, path_offset + n), then their re-centring moments (sum F e^x, count) into moments_out
+template <typename Real, typename Consts>
+static int launch_slice_k(SliceKernel<Real, Consts> kernel, void* x, void* v, void* q, long long n, long long path_offset, int init,
+                          double v_init, int nsteps, int slice_index, double forward, uint64_t seed, const Consts& c, double* moments_out,
+                          cudaStream_t st, P2pCtx* p2p) {
+  Grid g = persistent_grid(kernel, kSliceThreads, n);
+  size_t dyn_smem = 0;
+#ifdef B200SV_TUNING   // occupancy sweep for profiles/: cap resident CTAs per SM with dynamic shared memory (tuning builds only)
+  if (const char* e = getenv("B200SV_DEBUG_BLOCKS_PER_SM")) {
+    const int bps = atoi(e);
+    if (bps > 0) {
+      dyn_smem = (size_t)(200 * 1024) / bps;
+      if constexpr (std::is_same<Consts, LogsvConsts>::value)
+        cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn_smem);
+      g.blocks = (int)std::min<long long>((long long)device_sm_count() * bps, (n + kSliceThreads - 1) / kSliceThreads);
+    }
+  }
+#endif
+  ensure_pool_threshold();      // device-level callers too: a pool that trims at every synchronisation stalls the whole node (DESIGN.md 5)
+  DevBuf partials(st);
+  B200SV_CUDA(partials.alloc(sizeof(double) * 2 * g.blocks));
+  const SliceArgs<Real> a{(Real*)x, (Real*)v, (Real*)q, n, (unsigned long long)path_offset, init, v_init, nsteps, (unsigned int)slice_index,
+                          seed, forward, partials.as<double>()};
+  kernel<<<g.blocks, g.threads, dyn_smem, st>>>(a, c);
+  if (int rc = check_launch("mc_slice_kernel")) return rc;
+  reduce_partials_kernel<<<1, 64, 0, st>>>(a.partials, g.blocks, 2, 2, moments_out, make_publish(p2p, st));   // exchange #1 (producer)
+  return check_launch("reduce_partials_kernel");
+}
+
+template <typename Consts>
+static int launch_slice(void* x, void* v, void* q, long long n, long long path_offset, int init, double v_init, int nsteps, int slice_index,
+                        double forward, uint64_t seed, int flags, const Consts& c, double* moments_out, cudaStream_t st, P2pCtx* p2p = nullptr) {
   const int g = gauss_mode(flags);
   if (g < 0) return fail(-1, "invalid argument: B200SV_GAUSS_F64 and B200SV_GAUSS_F64_PAIRED are mutually exclusive");
-#define B200SV_SLICE_CASE(REAL, G) \
-  return launch_slice_t<MODEL, REAL, G>(x, v, q, n, path_offset, init, v_init, nsteps, slice_index, forward, seed, lc, hc, moments_out, st, p2p)
-  if (!f32 && g == kGaussF32) B200SV_SLICE_CASE(double, kGaussF32);
-  if (!f32 && g == kGaussF64) B200SV_SLICE_CASE(double, kGaussF64);
-  if (!f32 && g == kGaussF64Paired) B200SV_SLICE_CASE(double, kGaussF64Paired);
-  if (f32 && g == kGaussF32) B200SV_SLICE_CASE(float, kGaussF32);
-  if (f32 && g == kGaussF64) B200SV_SLICE_CASE(float, kGaussF64);
+  if (flags & B200SV_STATE_F32) {
+    if (const auto k = slice_kernel<float>(c, g))
+      return launch_slice_k(k, x, v, q, n, path_offset, init, v_init, nsteps, slice_index, forward, seed, c, moments_out, st, p2p);
+  } else if (const auto k = slice_kernel<double>(c, g)) {
+    return launch_slice_k(k, x, v, q, n, path_offset, init, v_init, nsteps, slice_index, forward, seed, c, moments_out, st, p2p);
+  }
   return fail(-1, "invalid argument: the paired Gaussian check mode needs fp64 state");
-#undef B200SV_SLICE_CASE
 }
 
 // kinds: bit 0 = some 'C'/'P', bit 1 = some 'IC'/'IP' in this slice; 0 = unknown (device-level callers) -> general kernel
@@ -1472,20 +1483,29 @@ static int launch_payoff_t(const void* x, const void* q, long long n, double ttm
   const bool vanilla = kinds == 1;
   Grid g = vanilla ? persistent_grid(payoff_vanilla_kernel<Real>, kThreads, n, kPayoffUnroll) : persistent_grid(payoff_kernel<Real>, kThreads, n);
   g.blocks = std::max(1, g.blocks / chunks);
-  double* partials = nullptr;
   ensure_pool_threshold();
-  B200SV_CUDA(cudaMallocAsync(&partials, sizeof(double) * (size_t)Kpad * g.blocks, st));
+  DevBuf partials(st);
+  B200SV_CUDA(partials.alloc(sizeof(double) * (size_t)Kpad * g.blocks));
   if (vanilla)
     payoff_vanilla_kernel<Real><<<dim3(g.blocks, chunks), g.threads, 0, st>>>((const Real*)x, (const Real*)q, n, ttm, forward, strikes,
-                                                                                types, J, variable_type, moments, partials, Kpad, gat);
+                                                                                types, J, variable_type, moments, partials.as<double>(), Kpad, gat);
   else
     payoff_kernel<Real><<<dim3(g.blocks, chunks), g.threads, 0, st>>>((const Real*)x, (const Real*)q, n, ttm, forward, strikes,
-                                                                        types, J, variable_type, moments, partials, Kpad, gat);
+                                                                        types, J, variable_type, moments, partials.as<double>(), Kpad, gat);
   if (int rc = check_launch("payoff_kernel")) return rc;
-  reduce_partials_kernel<<<1, 256, 0, st>>>(partials, g.blocks, Kpad, 3 * J, sums_out, make_publish(p2p, st));   // exchange #2 (producer)
-  if (int rc = check_launch("reduce_partials_kernel")) return rc;
-  B200SV_CUDA(cudaFreeAsync(partials, st));
-  return 0;
+  reduce_partials_kernel<<<1, 256, 0, st>>>(partials.as<double>(), g.blocks, Kpad, 3 * J, sums_out, make_publish(p2p, st));   // exchange #2 (producer)
+  return check_launch("reduce_partials_kernel");
+}
+
+static int spot_moments_impl(const double* x, long long n, double forward, double* moments_out, cudaStream_t st, P2pCtx* p2p) {
+  Grid g = persistent_grid(spot_moments_kernel, kThreads, n);
+  ensure_pool_threshold();
+  DevBuf partials(st);
+  B200SV_CUDA(partials.alloc(sizeof(double) * 2 * g.blocks));
+  spot_moments_kernel<<<g.blocks, g.threads, 0, st>>>(x, n, forward, partials.as<double>());
+  if (int rc = check_launch("spot_moments_kernel")) return rc;
+  reduce_partials_kernel<<<1, 64, 0, st>>>(partials.as<double>(), g.blocks, 2, 2, moments_out, make_publish(p2p, st));
+  return check_launch("reduce_partials_kernel");
 }
 
 static int payoff_kinds(const int8_t* types, int J) {
@@ -1509,45 +1529,100 @@ static int validate_chain(int M, const double* ttms, const int* offsets, const i
   return 0;
 }
 
-// one cooperative launch for the whole chain of one parameter set (fp64 state); buffers come from the caller
-template <int MODEL, int GAUSS>
-static int launch_chain_coop_g(const CoopArgs& args, const void* d_specs, int grid_blocks, cudaStream_t st) {
-  CoopArgs a = args;
-  const void* sp = d_specs;
-  void* kargs[] = {(void*)&a, (void*)&sp};
-  cudaError_t e;
-  if constexpr (MODEL == 0)
-    e = cudaLaunchCooperativeKernel((void*)mc_chain_coop_kernel<LogsvPath<double>, LogsvConsts, GAUSS>, dim3(grid_blocks), dim3(kSliceThreads), kargs, 0, st);
-  else if constexpr (MODEL == 1)
-    e = cudaLaunchCooperativeKernel((void*)mc_chain_coop_kernel<HestonPath<double, false>, HestonConsts, GAUSS>, dim3(grid_blocks), dim3(kSliceThreads), kargs, 0, st);
-  else
-    e = cudaLaunchCooperativeKernel((void*)mc_chain_coop_kernel<HestonPath<double, true>, HestonConsts, GAUSS>, dim3(grid_blocks), dim3(kSliceThreads), kargs, 0, st);
-  if (e != cudaSuccess) return fail(-2, std::string("mc_chain_coop_kernel: ") + cudaGetErrorString(e));
-  ++g_launches;
+// ---- host-level I/O ------------------------------------------------------------------------------------------------------
+// Copies a chain driver's [B][prices | stderrs | ivols][Jalloc] result block into the caller's [B][Jtot] outputs: one device-to-host
+// copy, the synchronisation that ends the call, then the scatter on the host (ivols only when ivols_out is given).
+static int copy_chain_results(StreamSync& sync, const double* d_out, int B, int Jtot, double* prices_out, double* stderr_out,
+                              double* ivols_out, cudaStream_t st) {
+  const int Jalloc = std::max(Jtot, 1);
+  std::vector<double> h((size_t)3 * Jalloc * B);
+  if (Jtot > 0) B200SV_CUDA(cudaMemcpyAsync(h.data(), d_out, sizeof(double) * h.size(), cudaMemcpyDeviceToHost, st));
+  if (int rc = sync.done()) return rc;
+  for (int b = 0; b < B && Jtot > 0; ++b) {
+    const double* o = h.data() + (size_t)3 * Jalloc * b;
+    memcpy(prices_out + (size_t)b * Jtot, o, sizeof(double) * Jtot);
+    memcpy(stderr_out + (size_t)b * Jtot, o + Jalloc, sizeof(double) * Jtot);
+    if (ivols_out) memcpy(ivols_out + (size_t)b * Jtot, o + 2 * Jalloc, sizeof(double) * Jtot);
+  }
   return 0;
 }
 
-template <int MODEL>
-static int coop_grid_blocks(int gauss, long long n) {
-  Grid g;
-  if (gauss == kGaussF64) {
-    if constexpr (MODEL == 0) g = persistent_grid(mc_chain_coop_kernel<LogsvPath<double>, LogsvConsts, kGaussF64>, kSliceThreads, n);
-    else if constexpr (MODEL == 1) g = persistent_grid(mc_chain_coop_kernel<HestonPath<double, false>, HestonConsts, kGaussF64>, kSliceThreads, n);
-    else g = persistent_grid(mc_chain_coop_kernel<HestonPath<double, true>, HestonConsts, kGaussF64>, kSliceThreads, n);
-  } else {
-    if constexpr (MODEL == 0) g = persistent_grid(mc_chain_coop_kernel<LogsvPath<double>, LogsvConsts, kGaussF32>, kSliceThreads, n);
-    else if constexpr (MODEL == 1) g = persistent_grid(mc_chain_coop_kernel<HestonPath<double, false>, HestonConsts, kGaussF32>, kSliceThreads, n);
-    else g = persistent_grid(mc_chain_coop_kernel<HestonPath<double, true>, HestonConsts, kGaussF32>, kSliceThreads, n);
+// The chain of a multi-launch chain driver on the device: its strikes and types, the current maturity's re-centring moments and payoff
+// sums, and the result block of copy_chain_results for B parameter sets.
+struct ChainIO {
+  int M, B, Jtot, Jalloc, variable_type;
+  const double *ttms, *forwards, *discfactors;
+  const int* offsets;
+  const int8_t* types;
+  cudaStream_t st;
+  DevBuf d_strikes, d_types, d_out, d_mom, d_sums;
+
+  ChainIO(int B_, int M_, const double* ttms_, const double* forwards_, const double* discfactors_, const int* offsets_, const int8_t* types_,
+          int variable_type_, cudaStream_t s)
+      : M(M_), B(B_), Jtot(offsets_[M_] - offsets_[0]), Jalloc(std::max(Jtot, 1)), variable_type(variable_type_), ttms(ttms_),
+        forwards(forwards_), discfactors(discfactors_), offsets(offsets_), types(types_), st(s), d_strikes(s), d_types(s), d_out(s), d_mom(s),
+        d_sums(s) {}
+
+  int upload(const double* strikes) {
+    B200SV_CUDA(d_strikes.alloc(sizeof(double) * Jalloc));
+    B200SV_CUDA(d_types.alloc(Jalloc));
+    B200SV_CUDA(d_out.alloc(sizeof(double) * 3 * Jalloc * B));
+    B200SV_CUDA(d_mom.alloc(sizeof(double) * 2));
+    B200SV_CUDA(d_sums.alloc(sizeof(double) * 3 * Jalloc));
+    if (Jtot > 0) {
+      B200SV_CUDA(cudaMemcpyAsync(d_strikes.p, strikes + offsets[0], sizeof(double) * Jtot, cudaMemcpyHostToDevice, st));
+      B200SV_CUDA(cudaMemcpyAsync(d_types.p, types + offsets[0], Jtot, cudaMemcpyHostToDevice, st));
+    }
+    return 0;
   }
-  return g.blocks;
-}
+  double* moments() const { return d_mom.as<double>(); }
 
-template <int MODEL>
-static int launch_chain_coop(int gauss, const CoopArgs& args, const void* d_specs, int grid_blocks, cudaStream_t st) {
-  if (gauss == kGaussF64) return launch_chain_coop_g<MODEL, kGaussF64>(args, d_specs, grid_blocks, st);
-  return launch_chain_coop_g<MODEL, kGaussF32>(args, d_specs, grid_blocks, st);
-}
+  // maturity m of parameter set b: payoff sums over the state (x, q) -> prices, std errors (/ sqrt(total_paths)) and, with_ivols, implied
+  // vols into the result block.  moments_from_x: the re-centring moments are taken from x here, not left by the slice launch.
+  int payoff(int b, int m, const void* x, const void* q, bool f32, long long n, double total_paths, bool with_ivols, bool moments_from_x = false) {
+    const int J = offsets[m + 1] - offsets[m], jo = offsets[m] - offsets[0];
+    if (J == 0) return 0;
+    if (moments_from_x)
+      if (int rc = spot_moments_impl((const double*)x, n, forwards[m], moments(), st, nullptr)) return rc;
+    const double* ks = d_strikes.as<double>() + jo;
+    const int8_t* ts = d_types.as<int8_t>() + jo;
+    const int kinds = payoff_kinds(types + offsets[m], J);
+    if (int rc = f32 ? launch_payoff_t<float>(x, q, n, ttms[m], forwards[m], ks, ts, J, variable_type, kinds, moments(), d_sums.as<double>(), st)
+                     : launch_payoff_t<double>(x, q, n, ttms[m], forwards[m], ks, ts, J, variable_type, kinds, moments(), d_sums.as<double>(), st))
+      return rc;
+    double* o = d_out.as<double>() + (size_t)3 * Jalloc * b + jo;
+    const IvolSpec iv{ks, ts, forwards[m], ttms[m], with_ivols ? o + 2 * Jalloc : nullptr};
+    payoff_finalize_kernel<<<(J + 127) / 128, 128, 0, st>>>(d_sums.as<double>(), J, discfactors[m], total_paths, o, o + Jalloc, P2pGather{}, iv);
+    return check_launch("payoff_finalize_kernel");
+  }
 
+  int copy_back(StreamSync& sync, double* prices_out, double* stderr_out, double* ivols_out) const {
+    return copy_chain_results(sync, d_out.as<double>(), B, Jtot, prices_out, stderr_out, ivols_out, st);
+  }
+};
+
+// The [3][n] fp64 path state (x, vol, qvar) of a host-level call on the device, and the caller's three arrays it is uploaded from
+// (alloc(true)) and copied back to (download).
+struct HostState {
+  double* h[3];
+  size_t n;
+  cudaStream_t st;
+  DevBuf d;
+
+  HostState(double* x, double* v, double* q, long long n_, cudaStream_t s) : h{x, v, q}, n((size_t)n_), st(s), d(s) {}
+  double* dev(int k) const { return d.as<double>() + k * n; }
+  int alloc(bool upload) {
+    B200SV_CUDA(d.alloc(sizeof(double) * 3 * n));
+    for (int k = 0; k < 3 && upload; ++k) B200SV_CUDA(cudaMemcpyAsync(dev(k), h[k], sizeof(double) * n, cudaMemcpyHostToDevice, st));
+    return 0;
+  }
+  int download() const {
+    for (int k = 0; k < 3; ++k) B200SV_CUDA(cudaMemcpyAsync(h[k], dev(k), sizeof(double) * n, cudaMemcpyDeviceToHost, st));
+    return 0;
+  }
+};
+
+// ---- host-level chain drivers ----------------------------------------------------------------------------------------------
 // Which chain driver?  The cooperative single-launch kernel wins where launch and host overhead matter (small path counts) and loses at
 // large ones, where its 128-register budget (slice + payoff phases in one kernel) costs more than 20 launches: it serves
 // nb_path <= kCoopMaxPaths.
@@ -1571,16 +1646,14 @@ static bool use_coop_chain(int flags, long long nb_path, bool heston = false) {
 
 // Small-chain fast path: ONE stream-ordered allocation, ONE host-to-device copy (strikes, types and the per-maturity specs of all B sets in
 // one blob), ONE cooperative launch per parameter set, ONE device-to-host copy.
-template <int MODEL>
-static int mc_chain_host_coop(const b200sv_logsv_params* lp, const b200sv_heston_params* hp, int M, const double* ttms, const double* forwards,
-                              const double* discfactors, const double* etas, const int* offsets, const double* strikes, const int8_t* types,
-                              long long nb_path, int nb_steps_per_year, int is_spot, int variable_type, uint64_t seed, int flags,
-                              double* prices_out, double* stderr_out, int scheme, int B, double* ivols_out) {
-  using Spec = CoopSliceSpec<typename std::conditional<MODEL == 0, LogsvConsts, HestonConsts>::type>;
+template <typename Params>
+static int mc_chain_host_coop(const Params* params, int M, const double* ttms, const double* forwards, const double* discfactors,
+                              const double* etas, const int* offsets, const double* strikes, const int8_t* types, long long nb_path,
+                              int nb_steps_per_year, int is_spot, int variable_type, uint64_t seed, int flags, double* prices_out,
+                              double* stderr_out, int scheme, int B, double* ivols_out) {
+  using Consts = decltype(slice_consts(*params, 1.0, false, 1.0, scheme));
+  using Spec = CoopSliceSpec<Consts>;
   const int Jtot = offsets[M] - offsets[0], Jalloc = std::max(Jtot, 1);
-  const int gauss = gauss_mode(flags);
-  const bool qe = MODEL == 1 && scheme == B200SV_HESTON_QE;
-  const int blocks = MODEL == 0 ? coop_grid_blocks<0>(gauss, nb_path) : (qe ? coop_grid_blocks<2>(gauss, nb_path) : coop_grid_blocks<1>(gauss, nb_path));
   int Jmax = 1;
   for (int m = 0; m < M; ++m) Jmax = std::max(Jmax, offsets[m + 1] - offsets[m]);
   const int Kpad_max = 3 * kStrikeChunk * ((Jmax + kStrikeChunk - 1) / kStrikeChunk);
@@ -1588,7 +1661,6 @@ static int mc_chain_host_coop(const b200sv_logsv_params* lp, const b200sv_heston
   const size_t spec_bytes = sizeof(Spec) * (size_t)M * B;
   const size_t in_bytes = sizeof(double) * Jalloc + spec_bytes + (((size_t)Jalloc + 7) & ~(size_t)7);
   const size_t out_doubles = (size_t)3 * Jalloc * B;
-  const size_t total = in_bytes + sizeof(double) * (3 * (size_t)nb_path + out_doubles + 2 * (size_t)blocks + (size_t)Kpad_max * blocks);
   std::vector<char> h_in(in_bytes, 0);
   if (Jtot > 0) {
     memcpy(h_in.data(), strikes + offsets[0], sizeof(double) * Jtot);
@@ -1604,10 +1676,7 @@ static int mc_chain_host_coop(const b200sv_logsv_params* lp, const b200sv_heston
       t0 = ttms[m];
       const int J = offsets[m + 1] - offsets[m];
       Spec& sp = h_specs[(size_t)b * M + m];
-      if constexpr (MODEL == 0)
-        sp.c = make_logsv_consts(lp[b], etas ? etas[(size_t)b * M + m] : 1.0, is_spot != 0, dt);
-      else
-        sp.c = make_heston_consts(hp[b], dt, scheme);
+      sp.c = slice_consts(params[b], etas ? etas[(size_t)b * M + m] : 1.0, is_spot != 0, dt, scheme);
       sp.nsteps = S;
       sp.jo = offsets[m] - offsets[0];
       sp.J = J;
@@ -1617,179 +1686,108 @@ static int mc_chain_host_coop(const b200sv_logsv_params* lp, const b200sv_heston
       sp.discfactor = discfactors[m];
     }
   }
+  const CoopKernel<Consts> kernel = coop_kernel(h_specs[0].c, gauss_mode(flags));
+  const int blocks = persistent_grid(kernel, kSliceThreads, nb_path).blocks;
+  const size_t total = in_bytes + sizeof(double) * (3 * (size_t)nb_path + out_doubles + 2 * (size_t)blocks + (size_t)Kpad_max * blocks);
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
-  char* arena = nullptr;
-  B200SV_CUDA(cudaMallocAsync(&arena, total, st));
-  B200SV_CUDA(cudaMemcpyAsync(arena, h_in.data(), in_bytes, cudaMemcpyHostToDevice, st));      // pageable source: staged before the call returns
-  double* d_strikes = (double*)arena;
-  const Spec* d_specs = (const Spec*)(arena + sizeof(double) * Jalloc);
-  const int8_t* d_types = (const int8_t*)(arena + sizeof(double) * Jalloc + spec_bytes);
-  double* d_state = (double*)(arena + in_bytes);
+  StreamSync sync(st);
+  DevBuf arena(st);
+  B200SV_CUDA(arena.alloc(total));
+  B200SV_CUDA(cudaMemcpyAsync(arena.p, h_in.data(), in_bytes, cudaMemcpyHostToDevice, st));      // pageable source: staged before the call returns
+  char* base = arena.as<char>();
+  const Spec* d_specs = (const Spec*)(base + sizeof(double) * Jalloc);
+  double* d_state = (double*)(base + in_bytes);
   double* d_out = d_state + 3 * (size_t)nb_path;
   double* d_pm = d_out + out_doubles;
-  double* d_pp = d_pm + 2 * (size_t)blocks;
-  int rc = 0;
-  for (int b = 0; b < B && rc == 0; ++b) {
+  for (int b = 0; b < B; ++b) {
     double* out_b = d_out + (size_t)3 * Jalloc * b;
     CoopArgs a{};
     a.x = d_state;
     a.v = d_state + nb_path;
     a.q = d_state + 2 * nb_path;
     a.n = nb_path;
-    a.v_init = MODEL == 0 ? lp[b].sigma0 : hp[b].v0;
+    a.v_init = v_init(params[b]);
     a.seed = seed;
     a.M = M;
     a.variable_type = variable_type;
-    a.strikes = d_strikes;
-    a.types = d_types;
+    a.strikes = (const double*)base;
+    a.types = (const int8_t*)(base + sizeof(double) * Jalloc + spec_bytes);
     a.part_mom = d_pm;
-    a.part_pay = d_pp;
+    a.part_pay = d_pm + 2 * (size_t)blocks;
     a.Kpad_max = Kpad_max;
     a.total_paths = (double)nb_path;
     a.prices = out_b;
     a.stderrs = out_b + Jalloc;
     a.ivols = ivols_out ? out_b + 2 * Jalloc : nullptr;
-    const void* sp = d_specs + (size_t)b * M;
-    if (MODEL == 0)
-      rc = launch_chain_coop<0>(gauss, a, sp, blocks, st);
-    else if (qe)
-      rc = launch_chain_coop<2>(gauss, a, sp, blocks, st);
-    else
-      rc = launch_chain_coop<1>(gauss, a, sp, blocks, st);
+    const Spec* sp = d_specs + (size_t)b * M;
+    void* kargs[] = {(void*)&a, (void*)&sp};
+    if (int rc = check_launch("mc_chain_coop_kernel",
+                              cudaLaunchCooperativeKernel((void*)kernel, dim3(blocks), dim3(kSliceThreads), kargs, 0, st)))
+      return rc;
   }
-  std::vector<double> h_out(out_doubles);
-  if (rc == 0 && Jtot > 0) {
-    cudaError_t e = cudaMemcpyAsync(h_out.data(), d_out, sizeof(double) * out_doubles, cudaMemcpyDeviceToHost, st);
-    if (e != cudaSuccess) rc = fail(-2, std::string("D2H: ") + cudaGetErrorString(e));
-  }
-  cudaFreeAsync(arena, st);
-  cudaError_t e = cudaStreamSynchronize(st);
-  if (rc == 0 && e != cudaSuccess) rc = fail(-2, std::string("sync: ") + cudaGetErrorString(e));
-  for (int b = 0; b < B && rc == 0 && Jtot > 0; ++b) {
-    const double* o = h_out.data() + (size_t)3 * Jalloc * b;
-    memcpy(prices_out + (size_t)b * Jtot, o, sizeof(double) * Jtot);
-    memcpy(stderr_out + (size_t)b * Jtot, o + Jalloc, sizeof(double) * Jtot);
-    if (ivols_out) memcpy(ivols_out + (size_t)b * Jtot, o + 2 * Jalloc, sizeof(double) * Jtot);
-  }
-  return rc;
+  return copy_chain_results(sync, d_out, B, Jtot, prices_out, stderr_out, ivols_out, st);
 }
 
 // shared host-level chain driver
-template <int MODEL>
-static int mc_chain_host(const b200sv_logsv_params* lp, const b200sv_heston_params* hp, int M, const double* ttms,
-                         const double* forwards, const double* discfactors, const double* etas, const int* offsets,
-                         const double* strikes, const int8_t* types, long long nb_path, int nb_steps_per_year, int is_spot,
+template <typename Params>
+static int mc_chain_host(const Params* params, int M, const double* ttms, const double* forwards, const double* discfactors, const double* etas,
+                         const int* offsets, const double* strikes, const int8_t* types, long long nb_path, int nb_steps_per_year, int is_spot,
                          int variable_type, uint64_t seed, int flags, double* prices_out, double* stderr_out, int scheme = 0, int B = 1,
                          double* ivols_out = nullptr) {
-  // B > 1: lp / hp point to B parameter sets, etas to [B][M], outputs to [B][Jtot]; the sets run back to back on one stream with the SAME
+  // B > 1: params points to B parameter sets, etas to [B][M], outputs to [B][Jtot]; the sets run back to back on one stream with the SAME
   // seed (common random numbers => a smooth objective in the parameters), no host synchronisation until the single copy back
   B200SV_REQUIRE(B >= 1, "B must be >= 1");
   B200SV_REQUIRE(nb_path >= 1, "nb_path must be >= 1");
   B200SV_REQUIRE(nb_steps_per_year >= 1, "nb_steps_per_year must be >= 1");
   if (int rc = validate_chain(M, ttms, offsets, types, variable_type)) return rc;
-  if (use_coop_chain(flags, nb_path, MODEL == 1))
-    return mc_chain_host_coop<MODEL>(lp, hp, M, ttms, forwards, discfactors, etas, offsets, strikes, types, nb_path, nb_steps_per_year, is_spot,
-                                     variable_type, seed, flags, prices_out, stderr_out, scheme, B, ivols_out);
-  const int Jtot = offsets[M] - offsets[0];
-  const size_t esz = (flags & B200SV_STATE_F32) ? 4 : 8;
+  if (use_coop_chain(flags, nb_path, std::is_same<Params, b200sv_heston_params>::value))
+    return mc_chain_host_coop(params, M, ttms, forwards, discfactors, etas, offsets, strikes, types, nb_path, nb_steps_per_year, is_spot,
+                              variable_type, seed, flags, prices_out, stderr_out, scheme, B, ivols_out);
+  const bool f32 = flags & B200SV_STATE_F32;
+  const size_t esz = f32 ? 4 : 8;
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
-  char *x = nullptr;
-  double *d_strikes = nullptr, *d_out = nullptr, *d_mom = nullptr, *d_sums = nullptr;
-  int8_t* d_types = nullptr;
-  B200SV_CUDA(cudaMallocAsync(&x, 3 * esz * (size_t)nb_path, st));
-  char *v = x + esz * (size_t)nb_path, *q = x + 2 * esz * (size_t)nb_path;
-  const int Jalloc = std::max(Jtot, 1);
-  B200SV_CUDA(cudaMallocAsync(&d_strikes, sizeof(double) * Jalloc, st));
-  B200SV_CUDA(cudaMallocAsync(&d_types, Jalloc, st));
-  const size_t out_stride = (size_t)3 * Jalloc;                 // per set: prices, std errors, implied vols
-  B200SV_CUDA(cudaMallocAsync(&d_out, sizeof(double) * out_stride * B, st));
-  B200SV_CUDA(cudaMallocAsync(&d_mom, sizeof(double) * 2, st));
-  B200SV_CUDA(cudaMallocAsync(&d_sums, sizeof(double) * 3 * Jalloc, st));
-  if (Jtot > 0) {
-    B200SV_CUDA(cudaMemcpyAsync(d_strikes, strikes + offsets[0], sizeof(double) * Jtot, cudaMemcpyHostToDevice, st));
-    B200SV_CUDA(cudaMemcpyAsync(d_types, types + offsets[0], Jtot, cudaMemcpyHostToDevice, st));
-  }
-  int rc = 0;
-  for (int b = 0; b < B && rc == 0; ++b) {
-    double* out_b = d_out + out_stride * b;
+  StreamSync sync(st);
+  DevBuf state(st);
+  ChainIO io(B, M, ttms, forwards, discfactors, offsets, types, variable_type, st);
+  B200SV_CUDA(state.alloc(3 * esz * (size_t)nb_path));
+  if (int rc = io.upload(strikes)) return rc;
+  char *x = state.as<char>(), *v = x + esz * (size_t)nb_path, *q = x + 2 * esz * (size_t)nb_path;
+  for (int b = 0; b < B; ++b) {
     double t0 = 0.0;
-    for (int m = 0; m < M && rc == 0; ++m) {
+    for (int m = 0; m < M; ++m) {
       int S;
       double dt;
       time_grid(ttms[m] - t0, nb_steps_per_year, &S, &dt);
       t0 = ttms[m];
-      if (MODEL == 0) {
-        const LogsvConsts c = make_logsv_consts(lp[b], etas ? etas[(size_t)b * M + m] : 1.0, is_spot != 0, dt);
-        rc = launch_slice<0>(x, v, q, nb_path, 0, m == 0, lp[b].sigma0, S, m, forwards[m], seed, flags, &c, nullptr, d_mom, st);
-      } else {
-        const HestonConsts c = make_heston_consts(hp[b], dt, scheme);
-        rc = launch_slice<1>(x, v, q, nb_path, 0, m == 0, hp[b].v0, S, m, forwards[m], seed, flags, nullptr, &c, d_mom, st);
-      }
-      if (rc) break;
-      const int J = offsets[m + 1] - offsets[m], jo = offsets[m] - offsets[0];
-      if (J == 0) continue;
-      if (flags & B200SV_STATE_F32)
-        rc = launch_payoff_t<float>(x, q, nb_path, ttms[m], forwards[m], d_strikes + jo, d_types + jo, J, variable_type, payoff_kinds(types + offsets[m], J), d_mom, d_sums, st);
-      else
-        rc = launch_payoff_t<double>(x, q, nb_path, ttms[m], forwards[m], d_strikes + jo, d_types + jo, J, variable_type, payoff_kinds(types + offsets[m], J), d_mom, d_sums, st);
-      if (rc) break;
-      const IvolSpec iv{d_strikes + jo, d_types + jo, forwards[m], ttms[m], ivols_out ? out_b + 2 * Jalloc + jo : nullptr};
-      payoff_finalize_kernel<<<(J + 127) / 128, 128, 0, st>>>(d_sums, J, discfactors[m], (double)nb_path, out_b + jo, out_b + Jalloc + jo, P2pGather{}, iv);
-      rc = check_launch("payoff_finalize_kernel");
+      const auto c = slice_consts(params[b], etas ? etas[(size_t)b * M + m] : 1.0, is_spot != 0, dt, scheme);
+      if (int rc = launch_slice(x, v, q, nb_path, 0, m == 0, v_init(params[b]), S, m, forwards[m], seed, flags, c, io.moments(), st)) return rc;
+      if (int rc = io.payoff(b, m, x, q, f32, nb_path, (double)nb_path, ivols_out != nullptr)) return rc;
     }
   }
-  for (int b = 0; b < B && rc == 0 && Jtot > 0; ++b) {
-    const double* out_b = d_out + out_stride * b;
-    cudaError_t e = cudaMemcpyAsync(prices_out + (size_t)b * Jtot, out_b, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(stderr_out + (size_t)b * Jtot, out_b + Jalloc, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess && ivols_out) e = cudaMemcpyAsync(ivols_out + (size_t)b * Jtot, out_b + 2 * Jalloc, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st);
-    if (e != cudaSuccess) rc = fail(-2, std::string("D2H: ") + cudaGetErrorString(e));
-  }
-  cudaFreeAsync(x, st);
-  cudaFreeAsync(d_strikes, st);
-  cudaFreeAsync(d_types, st);
-  cudaFreeAsync(d_out, st);
-  cudaFreeAsync(d_mom, st);
-  cudaFreeAsync(d_sums, st);
-  cudaError_t e = cudaStreamSynchronize(st);
-  if (rc == 0 && e != cudaSuccess) rc = fail(-2, std::string("sync: ") + cudaGetErrorString(e));
-  return rc;
+  return io.copy_back(sync, prices_out, stderr_out, ivols_out);
 }
 
-template <int MODEL>
-static int terminal_host(const b200sv_logsv_params* lp, const b200sv_heston_params* hp, double ttm, long long nb_path,
-                         int nb_steps_per_year, int is_spot, double eta, uint64_t seed, int flags, double* x, double* v, double* q, int scheme = 0) {
+template <typename Params>
+static int terminal_host(const Params& p, double ttm, long long nb_path, int nb_steps_per_year, int is_spot, double eta, uint64_t seed, int flags,
+                         double* x, double* v, double* q, int scheme = 0) {
   B200SV_REQUIRE(nb_path >= 1 && ttm > 0.0 && nb_steps_per_year >= 1, "nb_path, ttm, nb_steps_per_year must be positive");
   B200SV_REQUIRE(!(flags & B200SV_STATE_F32), "terminal values are returned as float64: use B200SV_STATE_F64");
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
-  double *d = nullptr, *d_mom = nullptr;
-  B200SV_CUDA(cudaMallocAsync(&d, sizeof(double) * 3 * (size_t)nb_path, st));
-  B200SV_CUDA(cudaMallocAsync(&d_mom, sizeof(double) * 2, st));
+  StreamSync sync(st);
+  HostState s(x, v, q, nb_path, st);
+  DevBuf d_mom(st);
+  if (int rc = s.alloc(false)) return rc;
+  B200SV_CUDA(d_mom.alloc(sizeof(double) * 2));
   int S;
   double dt;
   time_grid(ttm, nb_steps_per_year, &S, &dt);
-  int rc;
-  if (MODEL == 0) {
-    const LogsvConsts c = make_logsv_consts(*lp, eta, is_spot != 0, dt);
-    rc = launch_slice<0>(d, d + nb_path, d + 2 * nb_path, nb_path, 0, 1, lp->sigma0, S, 0, 1.0, seed, flags, &c, nullptr, d_mom, st);
-  } else {
-    const HestonConsts c = make_heston_consts(*hp, dt, scheme);
-    rc = launch_slice<1>(d, d + nb_path, d + 2 * nb_path, nb_path, 0, 1, hp->v0, S, 0, 1.0, seed, flags, nullptr, &c, d_mom, st);
-  }
-  if (rc == 0) {
-    cudaError_t e = cudaMemcpyAsync(x, d, sizeof(double) * nb_path, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(v, d + nb_path, sizeof(double) * nb_path, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(q, d + 2 * nb_path, sizeof(double) * nb_path, cudaMemcpyDeviceToHost, st);
-    if (e != cudaSuccess) rc = fail(-2, std::string("D2H: ") + cudaGetErrorString(e));
-  }
-  cudaFreeAsync(d, st);
-  cudaFreeAsync(d_mom, st);
-  cudaError_t e = cudaStreamSynchronize(st);
-  if (rc == 0 && e != cudaSuccess) rc = fail(-2, std::string("sync: ") + cudaGetErrorString(e));
-  return rc;
+  const auto c = slice_consts(p, eta, is_spot != 0, dt, scheme);
+  if (int rc = launch_slice(s.dev(0), s.dev(1), s.dev(2), nb_path, 0, 1, v_init(p), S, 0, 1.0, seed, flags, c, d_mom.as<double>(), st)) return rc;
+  if (int rc = s.download()) return rc;
+  return sync.done();
 }
 
 // ---- pathwise sensitivities: host side --------------------------------------------------------------------------------
@@ -1802,56 +1800,33 @@ static int greeks_gauss(int flags) {
 }
 
 // one maturity slice with tangents; moments_out[2 + P] = (sum F e^x, count, sum F e^x dx_p)
-template <int MODEL, int GAUSS>
-static int launch_tangent_slice_g(double* x, double* v, double* q, const TangentState& t, long long n, long long path_offset, int init,
-                                  double v_init, int nsteps, int slice_index, double forward, uint64_t seed, const LogsvTangentConsts* lc,
-                                  const HestonTangentConsts* hc, double* moments_out, cudaStream_t st) {
-  using TPath = typename std::conditional<MODEL == 0, LogsvTangentPath, HestonTangentPath>::type;
-  constexpr int K = 2 + TPath::NP;
-  SliceArgs<double> a;
-  a.x = x;
-  a.v = v;
-  a.q = q;
-  a.n = n;
-  a.path_offset = (unsigned long long)path_offset;
-  a.init = init;
-  a.v_init = v_init;
-  a.nsteps = nsteps;
-  a.slice = (unsigned int)slice_index;
-  a.seed = seed;
-  a.forward = forward;
-  const Grid g = persistent_grid(mc_tangent_slice_kernel<TPath, GAUSS>, kSliceThreads, n);
-  double* partials = nullptr;
-  B200SV_CUDA(cudaMallocAsync(&partials, sizeof(double) * K * g.blocks, st));
-  a.partials = partials;
-  if constexpr (MODEL == 0)
-    mc_tangent_slice_kernel<TPath, GAUSS><<<g.blocks, g.threads, 0, st>>>(a, t, *lc);
-  else
-    mc_tangent_slice_kernel<TPath, GAUSS><<<g.blocks, g.threads, 0, st>>>(a, t, *hc);
-  if (int rc = check_launch("mc_tangent_slice_kernel")) return rc;
-  reduce_partials_kernel<<<1, 64, 0, st>>>(partials, g.blocks, K, K, moments_out, P2pPublish{});
-  if (int rc = check_launch("reduce_partials_kernel")) return rc;
-  B200SV_CUDA(cudaFreeAsync(partials, st));
-  return 0;
-}
-
-template <int MODEL>
+template <typename TConsts>
 static int launch_tangent_slice(int gauss, double* x, double* v, double* q, const TangentState& t, long long n, long long path_offset, int init,
-                                double v_init, int nsteps, int slice_index, double forward, uint64_t seed, const LogsvTangentConsts* lc,
-                                const HestonTangentConsts* hc, double* moments_out, cudaStream_t st) {
-  if (gauss == kGaussF64)
-    return launch_tangent_slice_g<MODEL, kGaussF64>(x, v, q, t, n, path_offset, init, v_init, nsteps, slice_index, forward, seed, lc, hc, moments_out, st);
-  return launch_tangent_slice_g<MODEL, kGaussF32>(x, v, q, t, n, path_offset, init, v_init, nsteps, slice_index, forward, seed, lc, hc, moments_out, st);
+                                double v_init, int nsteps, int slice_index, double forward, uint64_t seed, const TConsts& c, double* moments_out,
+                                cudaStream_t st) {
+  using TPath = TangentPathOf<TConsts>;
+  constexpr int K = 2 + TPath::NP;
+  const auto kernel = gauss == kGaussF64 ? mc_tangent_slice_kernel<TPath, kGaussF64> : mc_tangent_slice_kernel<TPath, kGaussF32>;
+  const Grid g = persistent_grid(kernel, kSliceThreads, n);
+  DevBuf partials(st);
+  B200SV_CUDA(partials.alloc(sizeof(double) * K * g.blocks));
+  const SliceArgs<double> a{x, v, q, n, (unsigned long long)path_offset, init, v_init, nsteps, (unsigned int)slice_index, seed, forward,
+                            partials.as<double>()};
+  kernel<<<g.blocks, g.threads, 0, st>>>(a, t, c);
+  if (int rc = check_launch("mc_tangent_slice_kernel")) return rc;
+  reduce_partials_kernel<<<1, 64, 0, st>>>(a.partials, g.blocks, K, K, moments_out, P2pPublish{});
+  return check_launch("reduce_partials_kernel");
 }
 
 // chain driver: per maturity tangent slice -> moments -> per-strike payoff / sensitivity sums -> finalize (stand-alone launches, fixed-order
 // reductions).  greeks_out / greeks_se_out: [1 + P][Jtot], row 0 = forward delta.
-template <int MODEL>
-static int mc_chain_greeks_host(const b200sv_logsv_params* lp, const b200sv_heston_params* hp, int M, const double* ttms, const double* forwards,
-                                const double* discfactors, const double* etas, const int* offsets, const double* strikes, const int8_t* types,
-                                long long nb_path, int nb_steps_per_year, int is_spot, int variable_type, uint64_t seed, int flags,
-                                double* prices_out, double* stderr_out, double* greeks_out, double* greeks_se_out) {
-  constexpr int NP = MODEL == 0 ? kLogsvParams : kHestonParams, KV = 3 + 2 * (1 + NP);
+template <typename Params>
+static int mc_chain_greeks_host(const Params& p, int M, const double* ttms, const double* forwards, const double* discfactors, const double* etas,
+                                const int* offsets, const double* strikes, const int8_t* types, long long nb_path, int nb_steps_per_year,
+                                int is_spot, int variable_type, uint64_t seed, int flags, double* prices_out, double* stderr_out,
+                                double* greeks_out, double* greeks_se_out) {
+  using TConsts = decltype(tangent_consts(p, 1.0, false, 1.0));
+  constexpr int NP = TangentPathOf<TConsts>::NP, KV = 3 + 2 * (1 + NP);
   B200SV_REQUIRE(nb_path >= 1, "nb_path must be >= 1");
   B200SV_REQUIRE(nb_steps_per_year >= 1, "nb_steps_per_year must be >= 1");
   if (int rc = validate_chain(M, ttms, offsets, types, variable_type)) return rc;
@@ -1860,123 +1835,121 @@ static int mc_chain_greeks_host(const b200sv_logsv_params* lp, const b200sv_hest
   const int Jtot = offsets[M] - offsets[0], Jalloc = std::max(Jtot, 1);
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
+  StreamSync sync(st);
   const size_t n = (size_t)nb_path;
   const size_t state_doubles = 3 * n + 3 * (size_t)NP * n;
   const size_t out_doubles = 2 * (size_t)Jalloc * (2 + NP);        // prices, std errors, greeks [1+P][J], greeks_se [1+P][J]
-  double *d_state = nullptr, *d_strikes = nullptr, *d_out = nullptr, *d_mom = nullptr, *d_sums = nullptr;
-  int8_t* d_types = nullptr;
-  B200SV_CUDA(cudaMallocAsync(&d_state, sizeof(double) * state_doubles, st));
-  B200SV_CUDA(cudaMallocAsync(&d_strikes, sizeof(double) * Jalloc, st));
-  B200SV_CUDA(cudaMallocAsync(&d_types, Jalloc, st));
-  B200SV_CUDA(cudaMallocAsync(&d_out, sizeof(double) * out_doubles, st));
-  B200SV_CUDA(cudaMallocAsync(&d_mom, sizeof(double) * (2 + NP), st));
-  B200SV_CUDA(cudaMallocAsync(&d_sums, sizeof(double) * KV * Jalloc, st));
+  DevBuf d_state(st), d_strikes(st), d_types(st), d_out(st), d_mom(st), d_sums(st);
+  B200SV_CUDA(d_state.alloc(sizeof(double) * state_doubles));
+  B200SV_CUDA(d_strikes.alloc(sizeof(double) * Jalloc));
+  B200SV_CUDA(d_types.alloc(Jalloc));
+  B200SV_CUDA(d_out.alloc(sizeof(double) * out_doubles));
+  B200SV_CUDA(d_mom.alloc(sizeof(double) * (2 + NP)));
+  B200SV_CUDA(d_sums.alloc(sizeof(double) * KV * Jalloc));
   if (Jtot > 0) {
-    B200SV_CUDA(cudaMemcpyAsync(d_strikes, strikes + offsets[0], sizeof(double) * Jtot, cudaMemcpyHostToDevice, st));
-    B200SV_CUDA(cudaMemcpyAsync(d_types, types + offsets[0], Jtot, cudaMemcpyHostToDevice, st));
+    B200SV_CUDA(cudaMemcpyAsync(d_strikes.p, strikes + offsets[0], sizeof(double) * Jtot, cudaMemcpyHostToDevice, st));
+    B200SV_CUDA(cudaMemcpyAsync(d_types.p, types + offsets[0], Jtot, cudaMemcpyHostToDevice, st));
   }
-  double *x = d_state, *v = x + n, *q = v + n;
+  double *x = d_state.as<double>(), *v = x + n, *q = v + n;
   const TangentState t{q + n, q + n + NP * n, q + n + 2 * NP * n};
-  double *o_price = d_out, *o_se = o_price + Jalloc, *o_g = o_se + Jalloc, *o_gse = o_g + (size_t)(1 + NP) * Jalloc;
-  int rc = 0;
+  double *o_price = d_out.as<double>(), *o_se = o_price + Jalloc, *o_g = o_se + Jalloc, *o_gse = o_g + (size_t)(1 + NP) * Jalloc;
   double t0 = 0.0;
-  for (int m = 0; m < M && rc == 0; ++m) {
+  for (int m = 0; m < M; ++m) {
     int S;
     double dt;
     time_grid(ttms[m] - t0, nb_steps_per_year, &S, &dt);
     t0 = ttms[m];
-    if constexpr (MODEL == 0) {
-      const LogsvTangentConsts c = make_logsv_tangent_consts(*lp, etas ? etas[m] : 1.0, is_spot != 0, dt);
-      rc = launch_tangent_slice<0>(gauss, x, v, q, t, nb_path, 0, m == 0, lp->sigma0, S, m, forwards[m], seed, &c, nullptr, d_mom, st);
-    } else {
-      const HestonTangentConsts c = make_heston_tangent_consts(*hp, dt);
-      rc = launch_tangent_slice<1>(gauss, x, v, q, t, nb_path, 0, m == 0, hp->v0, S, m, forwards[m], seed, nullptr, &c, d_mom, st);
-    }
-    if (rc) break;
+    const TConsts c = tangent_consts(p, etas ? etas[m] : 1.0, is_spot != 0, dt);
+    if (int rc = launch_tangent_slice(gauss, x, v, q, t, nb_path, 0, m == 0, v_init(p), S, m, forwards[m], seed, c, d_mom.as<double>(), st)) return rc;
     const int J = offsets[m + 1] - offsets[m], jo = offsets[m] - offsets[0];
     if (J == 0) continue;
     const int chunks = (J + kGreeksStrikeChunk - 1) / kGreeksStrikeChunk;
     const int Kpad = KV * kGreeksStrikeChunk * chunks;
     Grid g = persistent_grid(payoff_greeks_kernel<NP>, kThreads, nb_path);
     g.blocks = std::max(1, g.blocks / chunks);
-    double* partials = nullptr;
-    B200SV_CUDA(cudaMallocAsync(&partials, sizeof(double) * (size_t)Kpad * g.blocks, st));
-    payoff_greeks_kernel<NP><<<dim3(g.blocks, chunks), g.threads, 0, st>>>(x, q, t.dx, t.dq, nb_path, ttms[m], forwards[m], d_strikes + jo,
-                                                                           d_types + jo, J, variable_type, d_mom, partials, Kpad);
-    if ((rc = check_launch("payoff_greeks_kernel"))) break;
-    reduce_partials_kernel<<<1, 256, 0, st>>>(partials, g.blocks, Kpad, KV * J, d_sums, P2pPublish{});
-    if ((rc = check_launch("reduce_partials_kernel"))) break;
-    B200SV_CUDA(cudaFreeAsync(partials, st));
-    greeks_finalize_kernel<<<(J + 127) / 128, 128, 0, st>>>(d_sums, KV, J, Jalloc, discfactors[m], (double)nb_path, o_price + jo, o_se + jo,
-                                                            o_g + jo, o_gse + jo);
-    rc = check_launch("greeks_finalize_kernel");
+    DevBuf partials(st);
+    B200SV_CUDA(partials.alloc(sizeof(double) * (size_t)Kpad * g.blocks));
+    payoff_greeks_kernel<NP><<<dim3(g.blocks, chunks), g.threads, 0, st>>>(x, q, t.dx, t.dq, nb_path, ttms[m], forwards[m], d_strikes.as<double>() + jo,
+                                                                           d_types.as<int8_t>() + jo, J, variable_type, d_mom.as<double>(),
+                                                                           partials.as<double>(), Kpad);
+    if (int rc = check_launch("payoff_greeks_kernel")) return rc;
+    reduce_partials_kernel<<<1, 256, 0, st>>>(partials.as<double>(), g.blocks, Kpad, KV * J, d_sums.as<double>(), P2pPublish{});
+    if (int rc = check_launch("reduce_partials_kernel")) return rc;
+    greeks_finalize_kernel<<<(J + 127) / 128, 128, 0, st>>>(d_sums.as<double>(), KV, J, Jalloc, discfactors[m], (double)nb_path, o_price + jo,
+                                                            o_se + jo, o_g + jo, o_gse + jo);
+    if (int rc = check_launch("greeks_finalize_kernel")) return rc;
   }
-  if (rc == 0 && Jtot > 0) {
-    cudaError_t e = cudaMemcpyAsync(prices_out, o_price, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(stderr_out, o_se, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st);
-    for (int k = 0; k < 1 + NP && e == cudaSuccess; ++k) {
-      e = cudaMemcpyAsync(greeks_out + (size_t)k * Jtot, o_g + (size_t)k * Jalloc, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st);
-      if (e == cudaSuccess)
-        e = cudaMemcpyAsync(greeks_se_out + (size_t)k * Jtot, o_gse + (size_t)k * Jalloc, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st);
+  if (Jtot > 0) {
+    B200SV_CUDA(cudaMemcpyAsync(prices_out, o_price, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st));
+    B200SV_CUDA(cudaMemcpyAsync(stderr_out, o_se, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st));
+    for (int k = 0; k < 1 + NP; ++k) {
+      B200SV_CUDA(cudaMemcpyAsync(greeks_out + (size_t)k * Jtot, o_g + (size_t)k * Jalloc, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st));
+      B200SV_CUDA(cudaMemcpyAsync(greeks_se_out + (size_t)k * Jtot, o_gse + (size_t)k * Jalloc, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st));
     }
-    if (e != cudaSuccess) rc = fail(-2, std::string("D2H: ") + cudaGetErrorString(e));
   }
-  cudaFreeAsync(d_state, st);
-  cudaFreeAsync(d_strikes, st);
-  cudaFreeAsync(d_types, st);
-  cudaFreeAsync(d_out, st);
-  cudaFreeAsync(d_mom, st);
-  cudaFreeAsync(d_sums, st);
-  cudaError_t e = cudaStreamSynchronize(st);
-  if (rc == 0 && e != cudaSuccess) rc = fail(-2, std::string("sync: ") + cudaGetErrorString(e));
-  return rc;
+  return sync.done();
 }
 
 // one slice from the initial state (0, v_init, 0) with initial tangents, for paths [path_offset, path_offset + n) of Philox slice
 // `slice_index`; returns the terminal state and tangents [P][n] (LogSV: dv = d sigma = sigma * d log sigma)
-template <int MODEL>
-static int tangent_terminal_host(const b200sv_logsv_params* lp, const b200sv_heston_params* hp, double ttm, long long nb_path, int nb_steps_per_year,
-                                 int is_spot, double eta, uint64_t seed, int flags, int slice_index, long long path_offset, double* x, double* v,
-                                 double* q, double* dx, double* dv, double* dq) {
-  constexpr int NP = MODEL == 0 ? kLogsvParams : kHestonParams;
+template <typename Params>
+static int tangent_terminal_host(const Params& p, double ttm, long long nb_path, int nb_steps_per_year, int is_spot, double eta, uint64_t seed,
+                                 int flags, int slice_index, long long path_offset, double* x, double* v, double* q, double* dx, double* dv,
+                                 double* dq) {
+  using TConsts = decltype(tangent_consts(p, 1.0, false, 1.0));
+  constexpr int NP = TangentPathOf<TConsts>::NP;
   B200SV_REQUIRE(nb_path >= 1 && ttm > 0.0 && nb_steps_per_year >= 1, "nb_path, ttm, nb_steps_per_year must be positive");
   B200SV_REQUIRE(slice_index >= 0 && path_offset >= 0, "slice_index and path_offset must be >= 0");
   const int gauss = greeks_gauss(flags);
   if (gauss < 0) return gauss;
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
-  const size_t n = (size_t)nb_path, total = 3 * n + 3 * (size_t)NP * n;
-  double *d = nullptr, *d_mom = nullptr;
-  B200SV_CUDA(cudaMallocAsync(&d, sizeof(double) * total, st));
-  B200SV_CUDA(cudaMallocAsync(&d_mom, sizeof(double) * (2 + NP), st));
-  const TangentState t{d + 3 * n, d + 3 * n + NP * n, d + 3 * n + 2 * NP * n};
+  StreamSync sync(st);
+  const size_t n = (size_t)nb_path;
+  HostState s(x, v, q, nb_path, st);
+  DevBuf d_tan(st), d_mom(st);
+  if (int rc = s.alloc(false)) return rc;
+  B200SV_CUDA(d_tan.alloc(sizeof(double) * 3 * (size_t)NP * n));
+  B200SV_CUDA(d_mom.alloc(sizeof(double) * (2 + NP)));
+  const TangentState t{d_tan.as<double>(), d_tan.as<double>() + NP * n, d_tan.as<double>() + 2 * NP * n};
   int S;
   double dt;
   time_grid(ttm, nb_steps_per_year, &S, &dt);
-  int rc;
-  if constexpr (MODEL == 0) {
-    const LogsvTangentConsts c = make_logsv_tangent_consts(*lp, eta, is_spot != 0, dt);
-    rc = launch_tangent_slice<0>(gauss, d, d + n, d + 2 * n, t, nb_path, path_offset, 1, lp->sigma0, S, slice_index, 1.0, seed, &c, nullptr, d_mom, st);
-  } else {
-    const HestonTangentConsts c = make_heston_tangent_consts(*hp, dt);
-    rc = launch_tangent_slice<1>(gauss, d, d + n, d + 2 * n, t, nb_path, path_offset, 1, hp->v0, S, slice_index, 1.0, seed, nullptr, &c, d_mom, st);
+  const TConsts c = tangent_consts(p, eta, is_spot != 0, dt);
+  if (int rc = launch_tangent_slice(gauss, s.dev(0), s.dev(1), s.dev(2), t, nb_path, path_offset, 1, v_init(p), S, slice_index, 1.0, seed, c,
+                                    d_mom.as<double>(), st))
+    return rc;
+  if (int rc = s.download()) return rc;
+  double* dst[3] = {dx, dv, dq};
+  const double* src[3] = {t.dx, t.dv, t.dq};
+  for (int k = 0; k < 3; ++k) B200SV_CUDA(cudaMemcpyAsync(dst[k], src[k], sizeof(double) * NP * n, cudaMemcpyDeviceToHost, st));
+  if (int rc = sync.done()) return rc;
+  if (std::is_same<Params, b200sv_logsv_params>::value)
+    for (size_t k = 0; k < (size_t)NP; ++k)
+      for (size_t i = 0; i < n; ++i) dv[k * n + i] *= v[i];
+  return 0;
+}
+
+// host-level fixed-random steppers: the state and the normals W0, W1 [S][N] are uploaded, `step` (a device-level stepper) advances the
+// state on the device, and the state is copied back in place
+template <typename Step>
+static int step_fixed_host(double* x, double* v, double* q, const double* W0, const double* W1, int S, long long N, double dt, Step step) {
+  B200SV_REQUIRE(x && v && q && (S == 0 || (W0 && W1)), "null pointer");
+  B200SV_REQUIRE(S >= 0 && N >= 1 && dt > 0.0, "S, N, dt");
+  cudaStream_t st = current_stream();
+  StreamSync sync(st);
+  HostState s(x, v, q, N, st);
+  DevBuf w(st);
+  const size_t wb = sizeof(double) * (size_t)N * (size_t)std::max(S, 1);
+  if (int rc = s.alloc(true)) return rc;
+  B200SV_CUDA(w.alloc(2 * wb));
+  if (S > 0) {
+    B200SV_CUDA(cudaMemcpyAsync(w.p, W0, wb, cudaMemcpyHostToDevice, st));
+    B200SV_CUDA(cudaMemcpyAsync(w.as<double>() + (size_t)N * S, W1, wb, cudaMemcpyHostToDevice, st));
   }
-  if (rc == 0) {
-    double* dst[6] = {x, v, q, dx, dv, dq};
-    const size_t cnt[6] = {n, n, n, NP * n, NP * n, NP * n};
-    const double* src[6] = {d, d + n, d + 2 * n, t.dx, t.dv, t.dq};
-    cudaError_t e = cudaSuccess;
-    for (int k = 0; k < 6 && e == cudaSuccess; ++k) e = cudaMemcpyAsync(dst[k], src[k], sizeof(double) * cnt[k], cudaMemcpyDeviceToHost, st);
-    if (e != cudaSuccess) rc = fail(-2, std::string("D2H: ") + cudaGetErrorString(e));
-  }
-  cudaFreeAsync(d, st);
-  cudaFreeAsync(d_mom, st);
-  cudaError_t e = cudaStreamSynchronize(st);
-  if (rc == 0 && e != cudaSuccess) rc = fail(-2, std::string("sync: ") + cudaGetErrorString(e));
-  if (rc == 0 && MODEL == 0)
-    for (size_t p = 0; p < (size_t)NP; ++p)
-      for (size_t i = 0; i < n; ++i) dv[p * n + i] *= v[i];
-  return rc;
+  if (int rc = step(s.dev(0), s.dev(1), s.dev(2), w.as<double>(), w.as<double>() + (size_t)N * S, st)) return rc;
+  if (int rc = s.download()) return rc;
+  return sync.done();
 }
 
 }  // namespace b200sv
@@ -1996,19 +1969,16 @@ int b200sv_set_stream(void* stream) {
   return 0;
 }
 void* b200sv_get_stream(void) { return (void*)current_stream(); }
-long long b200sv_launch_count(void) { return g_launches; }
-void b200sv_reset_launch_count(void) { g_launches = 0; }
-
-// internal hook for the MGF translation unit
-void b200sv_internal_count_launch(void) { ++g_launches; }
+long long b200sv_launch_count(void) { return launch_count_ref(); }
+void b200sv_reset_launch_count(void) { launch_count_ref() = 0; }
 
 int b200sv_logsv_mc_chain(const b200sv_logsv_params* params, int M, const double* ttms, const double* forwards,
                           const double* discfactors, const double* etas, const int* offsets, const double* strikes,
                           const int8_t* types, long long nb_path, int nb_steps_per_year, int is_spot_measure, int variable_type,
                           uint64_t seed, int flags, double* prices_out, double* stderr_out) {
   B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && stderr_out, "null pointer");
-  return mc_chain_host<0>(params, nullptr, M, ttms, forwards, discfactors, etas, offsets, strikes, types, nb_path,
-                          nb_steps_per_year, is_spot_measure, variable_type, seed, flags, prices_out, stderr_out);
+  return mc_chain_host(params, M, ttms, forwards, discfactors, etas, offsets, strikes, types, nb_path, nb_steps_per_year, is_spot_measure,
+                       variable_type, seed, flags, prices_out, stderr_out);
 }
 
 int b200sv_heston_mc_chain(const b200sv_heston_params* params, int M, const double* ttms, const double* forwards,
@@ -2017,8 +1987,8 @@ int b200sv_heston_mc_chain(const b200sv_heston_params* params, int M, const doub
                            double* prices_out, double* stderr_out) {
   B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && stderr_out, "null pointer");
   B200SV_REQUIRE(scheme == B200SV_HESTON_EULER_FLOOR || scheme == B200SV_HESTON_QE, "unknown Heston scheme");
-  return mc_chain_host<1>(nullptr, params, M, ttms, forwards, discfactors, nullptr, offsets, strikes, types, nb_path,
-                          nb_steps_per_year, 1, variable_type, seed, flags, prices_out, stderr_out, scheme);
+  return mc_chain_host(params, M, ttms, forwards, discfactors, nullptr, offsets, strikes, types, nb_path, nb_steps_per_year, 1, variable_type,
+                       seed, flags, prices_out, stderr_out, scheme);
 }
 
 int b200sv_logsv_mc_chain_batch(const b200sv_logsv_params* params, int B, int M, const double* ttms, const double* forwards,
@@ -2026,8 +1996,8 @@ int b200sv_logsv_mc_chain_batch(const b200sv_logsv_params* params, int B, int M,
                                 const int8_t* types, long long nb_path, int nb_steps_per_year, int is_spot_measure, uint64_t seed,
                                 int flags, double* prices_out, double* stderr_out, double* ivols_out) {
   B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && stderr_out, "null pointer");
-  return mc_chain_host<0>(params, nullptr, M, ttms, forwards, discfactors, etas, offsets, strikes, types, nb_path, nb_steps_per_year,
-                          is_spot_measure, B200SV_LOG_RETURN, seed, flags, prices_out, stderr_out, 0, B, ivols_out);
+  return mc_chain_host(params, M, ttms, forwards, discfactors, etas, offsets, strikes, types, nb_path, nb_steps_per_year, is_spot_measure,
+                       B200SV_LOG_RETURN, seed, flags, prices_out, stderr_out, 0, B, ivols_out);
 }
 
 int b200sv_heston_mc_chain_batch(const b200sv_heston_params* params, int B, int M, const double* ttms, const double* forwards,
@@ -2036,8 +2006,8 @@ int b200sv_heston_mc_chain_batch(const b200sv_heston_params* params, int B, int 
                                  double* stderr_out, double* ivols_out) {
   B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && stderr_out, "null pointer");
   B200SV_REQUIRE(scheme == B200SV_HESTON_EULER_FLOOR || scheme == B200SV_HESTON_QE, "unknown Heston scheme");
-  return mc_chain_host<1>(nullptr, params, M, ttms, forwards, discfactors, nullptr, offsets, strikes, types, nb_path, nb_steps_per_year, 1,
-                          B200SV_LOG_RETURN, seed, flags, prices_out, stderr_out, scheme, B, ivols_out);
+  return mc_chain_host(params, M, ttms, forwards, discfactors, nullptr, offsets, strikes, types, nb_path, nb_steps_per_year, 1, B200SV_LOG_RETURN,
+                       seed, flags, prices_out, stderr_out, scheme, B, ivols_out);
 }
 
 int b200sv_logsv_mc_chain_greeks(const b200sv_logsv_params* params, int M, const double* ttms, const double* forwards,
@@ -2045,8 +2015,8 @@ int b200sv_logsv_mc_chain_greeks(const b200sv_logsv_params* params, int M, const
                                  const int8_t* types, long long nb_path, int nb_steps_per_year, int is_spot_measure, int variable_type,
                                  uint64_t seed, int flags, double* prices_out, double* stderr_out, double* greeks_out, double* greeks_se_out) {
   B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && stderr_out && greeks_out && greeks_se_out, "null pointer");
-  return mc_chain_greeks_host<0>(params, nullptr, M, ttms, forwards, discfactors, etas, offsets, strikes, types, nb_path, nb_steps_per_year,
-                                 is_spot_measure, variable_type, seed, flags, prices_out, stderr_out, greeks_out, greeks_se_out);
+  return mc_chain_greeks_host(*params, M, ttms, forwards, discfactors, etas, offsets, strikes, types, nb_path, nb_steps_per_year, is_spot_measure,
+                              variable_type, seed, flags, prices_out, stderr_out, greeks_out, greeks_se_out);
 }
 
 int b200sv_heston_mc_chain_greeks(const b200sv_heston_params* params, int M, const double* ttms, const double* forwards,
@@ -2055,30 +2025,30 @@ int b200sv_heston_mc_chain_greeks(const b200sv_heston_params* params, int M, con
                                   double* prices_out, double* stderr_out, double* greeks_out, double* greeks_se_out) {
   B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && stderr_out && greeks_out && greeks_se_out, "null pointer");
   B200SV_REQUIRE(scheme == B200SV_HESTON_EULER_FLOOR, "pathwise sensitivities need scheme = B200SV_HESTON_EULER_FLOOR");
-  return mc_chain_greeks_host<1>(nullptr, params, M, ttms, forwards, discfactors, nullptr, offsets, strikes, types, nb_path, nb_steps_per_year, 1,
-                                 variable_type, seed, flags, prices_out, stderr_out, greeks_out, greeks_se_out);
+  return mc_chain_greeks_host(*params, M, ttms, forwards, discfactors, nullptr, offsets, strikes, types, nb_path, nb_steps_per_year, 1,
+                              variable_type, seed, flags, prices_out, stderr_out, greeks_out, greeks_se_out);
 }
 
 int b200sv_logsv_tangent_terminal(const b200sv_logsv_params* params, double ttm, long long nb_path, int nb_steps_per_year, int is_spot_measure,
                                   double eta, uint64_t seed, int flags, int slice_index, long long path_offset, double* x, double* sigma,
                                   double* qvar, double* dx, double* dsigma, double* dqvar) {
   B200SV_REQUIRE(params && x && sigma && qvar && dx && dsigma && dqvar, "null pointer");
-  return tangent_terminal_host<0>(params, nullptr, ttm, nb_path, nb_steps_per_year, is_spot_measure, eta, seed, flags, slice_index, path_offset,
-                                  x, sigma, qvar, dx, dsigma, dqvar);
+  return tangent_terminal_host(*params, ttm, nb_path, nb_steps_per_year, is_spot_measure, eta, seed, flags, slice_index, path_offset, x, sigma,
+                               qvar, dx, dsigma, dqvar);
 }
 
 int b200sv_heston_tangent_terminal(const b200sv_heston_params* params, double ttm, long long nb_path, int nb_steps_per_year, uint64_t seed,
                                    int flags, int slice_index, long long path_offset, double* x, double* var, double* qvar, double* dx,
                                    double* dvar, double* dqvar) {
   B200SV_REQUIRE(params && x && var && qvar && dx && dvar && dqvar, "null pointer");
-  return tangent_terminal_host<1>(nullptr, params, ttm, nb_path, nb_steps_per_year, 1, 1.0, seed, flags, slice_index, path_offset, x, var, qvar,
-                                  dx, dvar, dqvar);
+  return tangent_terminal_host(*params, ttm, nb_path, nb_steps_per_year, 1, 1.0, seed, flags, slice_index, path_offset, x, var, qvar, dx, dvar,
+                               dqvar);
 }
 
 int b200sv_logsv_terminal(const b200sv_logsv_params* params, double ttm, long long nb_path, int nb_steps_per_year,
                           int is_spot_measure, double eta, uint64_t seed, int flags, double* x, double* sigma, double* qvar) {
   B200SV_REQUIRE(params && x && sigma && qvar, "null pointer");
-  return terminal_host<0>(params, nullptr, ttm, nb_path, nb_steps_per_year, is_spot_measure, eta, seed, flags, x, sigma, qvar);
+  return terminal_host(*params, ttm, nb_path, nb_steps_per_year, is_spot_measure, eta, seed, flags, x, sigma, qvar);
 }
 
 // simulate_logsv_x_vol_terminal with PER-PATH initial arrays and in-kernel draws (pricers/logsv_pricer.py:1007-1020 accepts length-N x0 / sigma0 /
@@ -2092,36 +2062,26 @@ int b200sv_logsv_terminal_from_state(const b200sv_logsv_params* params, double t
   B200SV_REQUIRE(!(flags & B200SV_STATE_F32), "terminal values are returned as float64: use B200SV_STATE_F64");
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
-  double *d = nullptr, *d_mom = nullptr;
-  const size_t nb = sizeof(double) * (size_t)nb_path;
-  B200SV_CUDA(cudaMallocAsync(&d, 3 * nb, st));
-  B200SV_CUDA(cudaMallocAsync(&d_mom, sizeof(double) * 2, st));
-  B200SV_CUDA(cudaMemcpyAsync(d, x_inout, nb, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d + nb_path, sigma_inout, nb, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d + 2 * nb_path, qvar_inout, nb, cudaMemcpyHostToDevice, st));
+  StreamSync sync(st);
+  HostState s(x_inout, sigma_inout, qvar_inout, nb_path, st);
+  DevBuf d_mom(st);
+  if (int rc = s.alloc(true)) return rc;
+  B200SV_CUDA(d_mom.alloc(sizeof(double) * 2));
   int S;
   double dt;
   time_grid(ttm, nb_steps_per_year, &S, &dt);
   const LogsvConsts c = make_logsv_consts(*params, eta, is_spot_measure != 0, dt);
-  int rc = launch_slice<0>(d, d + nb_path, d + 2 * nb_path, nb_path, 0, 0, params->sigma0, S, slice_index, 1.0, seed, flags, &c, nullptr, d_mom, st);
-  if (rc == 0) {
-    cudaError_t e = cudaMemcpyAsync(x_inout, d, nb, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(sigma_inout, d + nb_path, nb, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(qvar_inout, d + 2 * nb_path, nb, cudaMemcpyDeviceToHost, st);
-    if (e != cudaSuccess) rc = fail(-2, std::string("D2H: ") + cudaGetErrorString(e));
-  }
-  cudaFreeAsync(d, st);
-  cudaFreeAsync(d_mom, st);
-  cudaError_t e = cudaStreamSynchronize(st);
-  if (rc == 0 && e != cudaSuccess) rc = fail(-2, std::string("sync: ") + cudaGetErrorString(e));
-  return rc;
+  if (int rc = launch_slice(s.dev(0), s.dev(1), s.dev(2), nb_path, 0, 0, params->sigma0, S, slice_index, 1.0, seed, flags, c, d_mom.as<double>(), st))
+    return rc;
+  if (int rc = s.download()) return rc;
+  return sync.done();
 }
 
 int b200sv_heston_terminal(const b200sv_heston_params* params, double ttm, long long nb_path, int nb_steps_per_year,
                            uint64_t seed, int flags, int scheme, double* x, double* var, double* qvar) {
   B200SV_REQUIRE(params && x && var && qvar, "null pointer");
   B200SV_REQUIRE(scheme == B200SV_HESTON_EULER_FLOOR || scheme == B200SV_HESTON_QE, "unknown Heston scheme");
-  return terminal_host<1>(nullptr, params, ttm, nb_path, nb_steps_per_year, 1, 1.0, seed, flags, x, var, qvar, scheme);
+  return terminal_host(*params, ttm, nb_path, nb_steps_per_year, 1, 1.0, seed, flags, x, var, qvar, scheme);
 }
 
 // ---- device-level ---------------------------------------------------------------------------------------------------
@@ -2131,8 +2091,8 @@ int b200sv_dev_logsv_slice(void* x, void* sigma, void* qvar, long long n_local, 
   B200SV_REQUIRE(x && sigma && qvar && params && moments_out, "null pointer");
   B200SV_REQUIRE(n_local >= 1 && nsteps >= 1 && dt > 0.0, "n_local, nsteps, dt must be positive");
   const LogsvConsts c = make_logsv_consts(*params, eta, is_spot_measure != 0, dt);
-  return launch_slice<0>(x, sigma, qvar, n_local, path_offset, init, params->sigma0, nsteps, slice_index, forward, seed, flags,
-                         &c, nullptr, moments_out, (cudaStream_t)stream, (P2pCtx*)p2p);
+  return launch_slice(x, sigma, qvar, n_local, path_offset, init, params->sigma0, nsteps, slice_index, forward, seed, flags, c, moments_out,
+                      (cudaStream_t)stream, (P2pCtx*)p2p);
 }
 
 int b200sv_dev_heston_slice(void* x, void* var, void* qvar, long long n_local, long long path_offset, int init,
@@ -2142,8 +2102,8 @@ int b200sv_dev_heston_slice(void* x, void* var, void* qvar, long long n_local, l
   B200SV_REQUIRE(n_local >= 1 && nsteps >= 1 && dt > 0.0, "n_local, nsteps, dt must be positive");
   B200SV_REQUIRE(scheme == B200SV_HESTON_EULER_FLOOR || scheme == B200SV_HESTON_QE, "unknown Heston scheme");
   const HestonConsts c = make_heston_consts(*params, dt, scheme);
-  return launch_slice<1>(x, var, qvar, n_local, path_offset, init, params->v0, nsteps, slice_index, forward, seed, flags, nullptr,
-                         &c, moments_out, (cudaStream_t)stream, (P2pCtx*)p2p);
+  return launch_slice(x, var, qvar, n_local, path_offset, init, params->v0, nsteps, slice_index, forward, seed, flags, c, moments_out,
+                      (cudaStream_t)stream, (P2pCtx*)p2p);
 }
 
 int b200sv_dev_payoff_sums(const void* x, const void* qvar, long long n_local, int flags, double ttm, double forward,
@@ -2193,19 +2153,6 @@ int b200sv_dev_heston_step_fixed(double* x, double* var, double* qvar, const dou
   return check_launch("heston_step_fixed_kernel");
 }
 
-static int spot_moments_impl(const double* x, long long n, double forward, double* moments_out, cudaStream_t st, P2pCtx* p2p) {
-  Grid g = persistent_grid(spot_moments_kernel, kThreads, n);
-  double* partials = nullptr;
-  ensure_pool_threshold();
-  B200SV_CUDA(cudaMallocAsync(&partials, sizeof(double) * 2 * g.blocks, st));
-  spot_moments_kernel<<<g.blocks, g.threads, 0, st>>>(x, n, forward, partials);
-  if (int rc = check_launch("spot_moments_kernel")) return rc;
-  reduce_partials_kernel<<<1, 64, 0, st>>>(partials, g.blocks, 2, 2, moments_out, make_publish(p2p, st));
-  if (int rc = check_launch("reduce_partials_kernel")) return rc;
-  B200SV_CUDA(cudaFreeAsync(partials, st));
-  return 0;
-}
-
 int b200sv_dev_spot_moments(const double* x, long long n, double forward, double* moments_out, void* stream) {
   B200SV_REQUIRE(x && moments_out && n >= 1, "null pointer / n");
   return spot_moments_impl(x, n, forward, moments_out, (cudaStream_t)stream, nullptr);
@@ -2240,47 +2187,20 @@ int b200sv_dev_rough_logsv_slice(double* log_spot, double* vol_factors, double* 
 }
 
 // ---- host-level fixed-random steppers and payoffs ------------------------------------------------------------------------
-static int step_fixed_host(int model, double* x, double* v, double* q, const double* W0, const double* W1, int S, long long N,
-                           double dt, const b200sv_logsv_params* lp, double eta, int is_spot, const b200sv_heston_params* hp) {
-  B200SV_REQUIRE(x && v && q && (S == 0 || (W0 && W1)), "null pointer");
-  B200SV_REQUIRE(S >= 0 && N >= 1 && dt > 0.0, "S, N, dt");
-  cudaStream_t st = current_stream();
-  double *d = nullptr, *w = nullptr;
-  const size_t nb = sizeof(double) * (size_t)N, wb = sizeof(double) * (size_t)N * (size_t)std::max(S, 1);
-  B200SV_CUDA(cudaMallocAsync(&d, 3 * nb, st));
-  B200SV_CUDA(cudaMallocAsync(&w, 2 * wb, st));
-  B200SV_CUDA(cudaMemcpyAsync(d, x, nb, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d + N, v, nb, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d + 2 * N, q, nb, cudaMemcpyHostToDevice, st));
-  if (S > 0) {
-    B200SV_CUDA(cudaMemcpyAsync(w, W0, wb, cudaMemcpyHostToDevice, st));
-    B200SV_CUDA(cudaMemcpyAsync(w + (size_t)N * S, W1, wb, cudaMemcpyHostToDevice, st));
-  }
-  int rc = model == 0 ? b200sv_dev_logsv_step_fixed(d, d + N, d + 2 * N, w, w + (size_t)N * S, S, N, dt, lp, eta, is_spot, 0, st)
-                      : b200sv_dev_heston_step_fixed(d, d + N, d + 2 * N, w, w + (size_t)N * S, S, N, dt, hp, st);
-  if (rc == 0) {
-    cudaError_t e = cudaMemcpyAsync(x, d, nb, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(v, d + N, nb, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(q, d + 2 * N, nb, cudaMemcpyDeviceToHost, st);
-    if (e != cudaSuccess) rc = fail(-2, std::string("D2H: ") + cudaGetErrorString(e));
-  }
-  cudaFreeAsync(d, st);
-  cudaFreeAsync(w, st);
-  cudaError_t e = cudaStreamSynchronize(st);
-  if (rc == 0 && e != cudaSuccess) rc = fail(-2, std::string("sync: ") + cudaGetErrorString(e));
-  return rc;
-}
-
 int b200sv_logsv_step_fixed(double* x, double* sigma, double* qvar, const double* W0, const double* W1, int S, long long N,
                             double dt, const b200sv_logsv_params* params, double eta, int is_spot_measure) {
   B200SV_REQUIRE(params, "null pointer");
-  return step_fixed_host(0, x, sigma, qvar, W0, W1, S, N, dt, params, eta, is_spot_measure, nullptr);
+  return step_fixed_host(x, sigma, qvar, W0, W1, S, N, dt, [&](double* dx, double* dv, double* dq, const double* w0, const double* w1, cudaStream_t st) {
+    return b200sv_dev_logsv_step_fixed(dx, dv, dq, w0, w1, S, N, dt, params, eta, is_spot_measure, 0, st);
+  });
 }
 
 int b200sv_heston_step_fixed(double* x, double* var, double* qvar, const double* W0, const double* W1, int S, long long N,
                              double dt, const b200sv_heston_params* params) {
   B200SV_REQUIRE(params, "null pointer");
-  return step_fixed_host(1, x, var, qvar, W0, W1, S, N, dt, nullptr, 1.0, 1, params);
+  return step_fixed_host(x, var, qvar, W0, W1, S, N, dt, [&](double* dx, double* dv, double* dq, const double* w0, const double* w1, cudaStream_t st) {
+    return b200sv_dev_heston_step_fixed(dx, dv, dq, w0, w1, S, N, dt, params, st);
+  });
 }
 
 int b200sv_mc_payoffs(const double* x, const double* qvar, long long N, double ttm, double forward, const double* strikes,
@@ -2292,79 +2212,65 @@ int b200sv_mc_payoffs(const double* x, const double* qvar, long long N, double t
   if (variable_type != B200SV_LOG_RETURN && variable_type != B200SV_Q_VAR) return fail(-4, "variable_type not implemented");
   B200SV_REQUIRE(variable_type == B200SV_LOG_RETURN || qvar, "qvar required for Q_VAR");
   cudaStream_t st = current_stream();
-  double *d = nullptr, *dk = nullptr, *d_mom = nullptr, *d_sums = nullptr, *d_out = nullptr;
-  int8_t* dt_ = nullptr;
+  StreamSync sync(st);
+  DevBuf d(st), dk(st), dt_(st), d_mom(st), d_sums(st), d_out(st);
   const size_t nb = sizeof(double) * (size_t)N;
-  B200SV_CUDA(cudaMallocAsync(&d, 2 * nb, st));
-  B200SV_CUDA(cudaMallocAsync(&dk, sizeof(double) * J, st));
-  B200SV_CUDA(cudaMallocAsync(&dt_, J, st));
-  B200SV_CUDA(cudaMallocAsync(&d_mom, sizeof(double) * 2, st));
-  B200SV_CUDA(cudaMallocAsync(&d_sums, sizeof(double) * 3 * J, st));
-  B200SV_CUDA(cudaMallocAsync(&d_out, sizeof(double) * 2 * J, st));
-  B200SV_CUDA(cudaMemcpyAsync(d, x, nb, cudaMemcpyHostToDevice, st));
-  if (qvar) B200SV_CUDA(cudaMemcpyAsync(d + N, qvar, nb, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(dk, strikes, sizeof(double) * J, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(dt_, types, J, cudaMemcpyHostToDevice, st));
-  int rc = b200sv_dev_spot_moments(d, N, forward, d_mom, st);
-  if (rc == 0) rc = launch_payoff_t<double>(d, d + N, N, ttm, forward, dk, dt_, J, variable_type, payoff_kinds(types, J), d_mom, d_sums, st);
-  if (rc == 0) rc = b200sv_dev_payoff_finalize(d_sums, J, discfactor, N, d_out, d_out + J, nullptr, st);
-  if (rc == 0) {
-    cudaError_t e = cudaMemcpyAsync(prices_out, d_out, sizeof(double) * J, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(stderr_out, d_out + J, sizeof(double) * J, cudaMemcpyDeviceToHost, st);
-    if (e != cudaSuccess) rc = fail(-2, std::string("D2H: ") + cudaGetErrorString(e));
-  }
-  cudaFreeAsync(d, st);
-  cudaFreeAsync(dk, st);
-  cudaFreeAsync(dt_, st);
-  cudaFreeAsync(d_mom, st);
-  cudaFreeAsync(d_sums, st);
-  cudaFreeAsync(d_out, st);
-  cudaError_t e = cudaStreamSynchronize(st);
-  if (rc == 0 && e != cudaSuccess) rc = fail(-2, std::string("sync: ") + cudaGetErrorString(e));
-  return rc;
+  B200SV_CUDA(d.alloc(2 * nb));
+  B200SV_CUDA(dk.alloc(sizeof(double) * J));
+  B200SV_CUDA(dt_.alloc(J));
+  B200SV_CUDA(d_mom.alloc(sizeof(double) * 2));
+  B200SV_CUDA(d_sums.alloc(sizeof(double) * 3 * J));
+  B200SV_CUDA(d_out.alloc(sizeof(double) * 2 * J));
+  B200SV_CUDA(cudaMemcpyAsync(d.p, x, nb, cudaMemcpyHostToDevice, st));
+  if (qvar) B200SV_CUDA(cudaMemcpyAsync(d.as<double>() + N, qvar, nb, cudaMemcpyHostToDevice, st));
+  B200SV_CUDA(cudaMemcpyAsync(dk.p, strikes, sizeof(double) * J, cudaMemcpyHostToDevice, st));
+  B200SV_CUDA(cudaMemcpyAsync(dt_.p, types, J, cudaMemcpyHostToDevice, st));
+  const double* dx = d.as<double>();
+  if (int rc = b200sv_dev_spot_moments(dx, N, forward, d_mom.as<double>(), st)) return rc;
+  if (int rc = launch_payoff_t<double>(dx, dx + N, N, ttm, forward, dk.as<double>(), dt_.as<int8_t>(), J, variable_type, payoff_kinds(types, J),
+                                       d_mom.as<double>(), d_sums.as<double>(), st))
+    return rc;
+  if (int rc = b200sv_dev_payoff_finalize(d_sums.as<double>(), J, discfactor, N, d_out.as<double>(), d_out.as<double>() + J, nullptr, st)) return rc;
+  B200SV_CUDA(cudaMemcpyAsync(prices_out, d_out.p, sizeof(double) * J, cudaMemcpyDeviceToHost, st));
+  B200SV_CUDA(cudaMemcpyAsync(stderr_out, d_out.as<double>() + J, sizeof(double) * J, cudaMemcpyDeviceToHost, st));
+  return sync.done();
 }
 
 int b200sv_device_normals(uint64_t seed, long long path0, long long n, int slice, int nsteps, int flags, double* z0, double* z1) {
   B200SV_REQUIRE(z0 && z1 && n >= 1 && nsteps >= 1, "null pointer / sizes");
-  cudaStream_t st = current_stream();
-  double* d = nullptr;
-  const size_t nb = sizeof(double) * (size_t)n * nsteps;
-  B200SV_CUDA(cudaMallocAsync(&d, 2 * nb, st));
-  const int blocks = (int)((n + 127) / 128);
   const int g = gauss_mode(flags);
   B200SV_REQUIRE(g >= 0, "B200SV_GAUSS_F64 and B200SV_GAUSS_F64_PAIRED are mutually exclusive");
+  cudaStream_t st = current_stream();
+  StreamSync sync(st);
+  DevBuf d(st);
+  const size_t nb = sizeof(double) * (size_t)n * nsteps;
+  B200SV_CUDA(d.alloc(2 * nb));
+  double *d0 = d.as<double>(), *d1 = d0 + (size_t)n * nsteps;
+  const int blocks = (int)((n + 127) / 128);
   if (g == kGaussF64)
-    device_normals_kernel<kGaussF64><<<blocks, 128, 0, st>>>(seed, (unsigned long long)path0, n, (unsigned)slice, nsteps, d, d + (size_t)n * nsteps);
+    device_normals_kernel<kGaussF64><<<blocks, 128, 0, st>>>(seed, (unsigned long long)path0, n, (unsigned)slice, nsteps, d0, d1);
   else if (g == kGaussF64Paired)
-    device_normals_kernel<kGaussF64Paired><<<blocks, 128, 0, st>>>(seed, (unsigned long long)path0, n, (unsigned)slice, nsteps, d, d + (size_t)n * nsteps);
+    device_normals_kernel<kGaussF64Paired><<<blocks, 128, 0, st>>>(seed, (unsigned long long)path0, n, (unsigned)slice, nsteps, d0, d1);
   else
-    device_normals_kernel<kGaussF32><<<blocks, 128, 0, st>>>(seed, (unsigned long long)path0, n, (unsigned)slice, nsteps, d, d + (size_t)n * nsteps);
-  int rc = check_launch("device_normals_kernel");
-  if (rc == 0) {
-    cudaError_t e = cudaMemcpyAsync(z0, d, nb, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(z1, d + (size_t)n * nsteps, nb, cudaMemcpyDeviceToHost, st);
-    if (e != cudaSuccess) rc = fail(-2, std::string("D2H: ") + cudaGetErrorString(e));
-  }
-  cudaFreeAsync(d, st);
-  cudaError_t e = cudaStreamSynchronize(st);
-  if (rc == 0 && e != cudaSuccess) rc = fail(-2, std::string("sync: ") + cudaGetErrorString(e));
-  return rc;
+    device_normals_kernel<kGaussF32><<<blocks, 128, 0, st>>>(seed, (unsigned long long)path0, n, (unsigned)slice, nsteps, d0, d1);
+  if (int rc = check_launch("device_normals_kernel")) return rc;
+  B200SV_CUDA(cudaMemcpyAsync(z0, d0, nb, cudaMemcpyDeviceToHost, st));
+  B200SV_CUDA(cudaMemcpyAsync(z1, d1, nb, cudaMemcpyDeviceToHost, st));
+  return sync.done();
 }
 
 int b200sv_debug_exp_pair_scaled(const double* Ls, long long n, double* out /* 2n */) {
   B200SV_REQUIRE(Ls && out && n >= 1, "null pointer / n");
   cudaStream_t st = current_stream();
-  double *dl = nullptr, *dout = nullptr;
-  B200SV_CUDA(cudaMallocAsync(&dl, sizeof(double) * n, st));
-  B200SV_CUDA(cudaMallocAsync(&dout, sizeof(double) * 2 * n, st));
-  B200SV_CUDA(cudaMemcpyAsync(dl, Ls, sizeof(double) * n, cudaMemcpyHostToDevice, st));
-  exp_pair_scaled_kernel<<<(int)((n + 127) / 128), 128, 0, st>>>(dl, n, dout);
-  int rc = check_launch("exp_pair_scaled_kernel");
-  if (rc == 0) B200SV_CUDA(cudaMemcpyAsync(out, dout, sizeof(double) * 2 * n, cudaMemcpyDeviceToHost, st));
-  cudaFreeAsync(dl, st);
-  cudaFreeAsync(dout, st);
-  B200SV_CUDA(cudaStreamSynchronize(st));
-  return rc;
+  StreamSync sync(st);
+  DevBuf dl(st), dout(st);
+  B200SV_CUDA(dl.alloc(sizeof(double) * n));
+  B200SV_CUDA(dout.alloc(sizeof(double) * 2 * n));
+  B200SV_CUDA(cudaMemcpyAsync(dl.p, Ls, sizeof(double) * n, cudaMemcpyHostToDevice, st));
+  exp_pair_scaled_kernel<<<(int)((n + 127) / 128), 128, 0, st>>>(dl.as<double>(), n, dout.as<double>());
+  if (int rc = check_launch("exp_pair_scaled_kernel")) return rc;
+  B200SV_CUDA(cudaMemcpyAsync(out, dout.p, sizeof(double) * 2 * n, cudaMemcpyDeviceToHost, st));
+  return sync.done();
 }
 
 int b200sv_debug_box_muller(const uint32_t* words, long long n, int flags, double* z_out) {
@@ -2372,24 +2278,21 @@ int b200sv_debug_box_muller(const uint32_t* words, long long n, int flags, doubl
   const int g = gauss_mode(flags);
   B200SV_REQUIRE(g >= 0, "B200SV_GAUSS_F64 and B200SV_GAUSS_F64_PAIRED are mutually exclusive");
   cudaStream_t st = current_stream();
-  uint4* dw = nullptr;
-  double* dout = nullptr;
-  B200SV_CUDA(cudaMallocAsync(&dw, sizeof(uint4) * n, st));
-  B200SV_CUDA(cudaMallocAsync(&dout, sizeof(double) * 4 * n, st));
-  B200SV_CUDA(cudaMemcpyAsync(dw, words, sizeof(uint4) * n, cudaMemcpyHostToDevice, st));
+  StreamSync sync(st);
+  DevBuf dw(st), dout(st);
+  B200SV_CUDA(dw.alloc(sizeof(uint4) * n));
+  B200SV_CUDA(dout.alloc(sizeof(double) * 4 * n));
+  B200SV_CUDA(cudaMemcpyAsync(dw.p, words, sizeof(uint4) * n, cudaMemcpyHostToDevice, st));
   const int blocks = (int)((n + 127) / 128);
   if (g == kGaussF64)
-    box_muller_words_kernel<kGaussF64><<<blocks, 128, 0, st>>>(dw, n, dout);
+    box_muller_words_kernel<kGaussF64><<<blocks, 128, 0, st>>>(dw.as<uint4>(), n, dout.as<double>());
   else if (g == kGaussF64Paired)
-    box_muller_words_kernel<kGaussF64Paired><<<blocks, 128, 0, st>>>(dw, n, dout);
+    box_muller_words_kernel<kGaussF64Paired><<<blocks, 128, 0, st>>>(dw.as<uint4>(), n, dout.as<double>());
   else
-    box_muller_words_kernel<kGaussF32><<<blocks, 128, 0, st>>>(dw, n, dout);
-  int rc = check_launch("box_muller_words_kernel");
-  if (rc == 0) B200SV_CUDA(cudaMemcpyAsync(z_out, dout, sizeof(double) * 4 * n, cudaMemcpyDeviceToHost, st));
-  cudaFreeAsync(dw, st);
-  cudaFreeAsync(dout, st);
-  B200SV_CUDA(cudaStreamSynchronize(st));
-  return rc;
+    box_muller_words_kernel<kGaussF32><<<blocks, 128, 0, st>>>(dw.as<uint4>(), n, dout.as<double>());
+  if (int rc = check_launch("box_muller_words_kernel")) return rc;
+  B200SV_CUDA(cudaMemcpyAsync(z_out, dout.p, sizeof(double) * 4 * n, cudaMemcpyDeviceToHost, st));
+  return sync.done();
 }
 
 int b200sv_debug_fastmath(int op, const double* a, const double* b, long long n, double* out) {
@@ -2397,38 +2300,33 @@ int b200sv_debug_fastmath(int op, const double* a, const double* b, long long n,
   B200SV_REQUIRE(op >= B200SV_DEBUG_FAST_DIV && op <= B200SV_DEBUG_EXP_TABLE, "unknown B200SV_DEBUG_* operation");
   B200SV_REQUIRE(op != B200SV_DEBUG_FAST_DIV || b, "fast_div needs the divisors b");
   cudaStream_t st = current_stream();
-  double *da = nullptr, *db = nullptr, *dout = nullptr;
-  B200SV_CUDA(cudaMallocAsync(&da, sizeof(double) * n, st));
-  B200SV_CUDA(cudaMallocAsync(&dout, sizeof(double) * n, st));
-  B200SV_CUDA(cudaMemcpyAsync(da, a, sizeof(double) * n, cudaMemcpyHostToDevice, st));
+  StreamSync sync(st);
+  DevBuf da(st), db(st), dout(st);
+  B200SV_CUDA(da.alloc(sizeof(double) * n));
+  B200SV_CUDA(dout.alloc(sizeof(double) * n));
+  B200SV_CUDA(cudaMemcpyAsync(da.p, a, sizeof(double) * n, cudaMemcpyHostToDevice, st));
   if (op == B200SV_DEBUG_FAST_DIV) {
-    B200SV_CUDA(cudaMallocAsync(&db, sizeof(double) * n, st));
-    B200SV_CUDA(cudaMemcpyAsync(db, b, sizeof(double) * n, cudaMemcpyHostToDevice, st));
+    B200SV_CUDA(db.alloc(sizeof(double) * n));
+    B200SV_CUDA(cudaMemcpyAsync(db.p, b, sizeof(double) * n, cudaMemcpyHostToDevice, st));
   }
-  fastmath_kernel<<<(int)((n + 127) / 128), 128, 0, st>>>(op, da, db, n, dout);
-  int rc = check_launch("fastmath_kernel");
-  if (rc == 0) B200SV_CUDA(cudaMemcpyAsync(out, dout, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
-  cudaFreeAsync(da, st);
-  if (db) cudaFreeAsync(db, st);
-  cudaFreeAsync(dout, st);
-  B200SV_CUDA(cudaStreamSynchronize(st));
-  return rc;
+  fastmath_kernel<<<(int)((n + 127) / 128), 128, 0, st>>>(op, da.as<double>(), db.as<double>(), n, dout.as<double>());
+  if (int rc = check_launch("fastmath_kernel")) return rc;
+  B200SV_CUDA(cudaMemcpyAsync(out, dout.p, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
+  return sync.done();
 }
 
 int b200sv_debug_exp_pair(const double* L, long long n, double* out /* 2n */) {
   B200SV_REQUIRE(L && out && n >= 1, "null pointer / n");
   cudaStream_t st = current_stream();
-  double *dl = nullptr, *dout = nullptr;
-  B200SV_CUDA(cudaMallocAsync(&dl, sizeof(double) * n, st));
-  B200SV_CUDA(cudaMallocAsync(&dout, sizeof(double) * 2 * n, st));
-  B200SV_CUDA(cudaMemcpyAsync(dl, L, sizeof(double) * n, cudaMemcpyHostToDevice, st));
-  exp_pair_kernel<<<(int)((n + 127) / 128), 128, 0, st>>>(dl, n, dout);
-  int rc = check_launch("exp_pair_kernel");
-  if (rc == 0) B200SV_CUDA(cudaMemcpyAsync(out, dout, sizeof(double) * 2 * n, cudaMemcpyDeviceToHost, st));
-  cudaFreeAsync(dl, st);
-  cudaFreeAsync(dout, st);
-  B200SV_CUDA(cudaStreamSynchronize(st));
-  return rc;
+  StreamSync sync(st);
+  DevBuf dl(st), dout(st);
+  B200SV_CUDA(dl.alloc(sizeof(double) * n));
+  B200SV_CUDA(dout.alloc(sizeof(double) * 2 * n));
+  B200SV_CUDA(cudaMemcpyAsync(dl.p, L, sizeof(double) * n, cudaMemcpyHostToDevice, st));
+  exp_pair_kernel<<<(int)((n + 127) / 128), 128, 0, st>>>(dl.as<double>(), n, dout.as<double>());
+  if (int rc = check_launch("exp_pair_kernel")) return rc;
+  B200SV_CUDA(cudaMemcpyAsync(out, dout.p, sizeof(double) * 2 * n, cudaMemcpyDeviceToHost, st));
+  return sync.done();
 }
 
 int b200sv_logsv_vol_paths(const b200sv_logsv_params* params, double ttm, long long nb_path, int nb_steps_per_year, int is_spot_measure,
@@ -2443,25 +2341,19 @@ int b200sv_logsv_vol_paths(const b200sv_logsv_params* params, double ttm, long l
              is_spot_measure ? 0.0 : params->beta, dt};
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
-  double *d_out = nullptr, *d_w = nullptr;
+  StreamSync sync(st);
+  DevBuf d_out(st), d_w(st);
   const size_t ob = sizeof(double) * (size_t)(S + 1) * (size_t)nb_path, wb = sizeof(double) * (size_t)S * (size_t)nb_path;
-  B200SV_CUDA(cudaMallocAsync(&d_out, ob, st));
+  B200SV_CUDA(d_out.alloc(ob));
   if (brownians) {
-    B200SV_CUDA(cudaMallocAsync(&d_w, wb, st));
-    B200SV_CUDA(cudaMemcpyAsync(d_w, brownians, wb, cudaMemcpyHostToDevice, st));
+    B200SV_CUDA(d_w.alloc(wb));
+    B200SV_CUDA(cudaMemcpyAsync(d_w.p, brownians, wb, cudaMemcpyHostToDevice, st));
   }
   Grid g = persistent_grid(logsv_vol_paths_kernel, kThreads, nb_path);
-  logsv_vol_paths_kernel<<<g.blocks, g.threads, 0, st>>>(d_out, d_w, S, nb_path, r, params->sigma0, seed, 0ull);
-  int rc = check_launch("logsv_vol_paths_kernel");
-  if (rc == 0) {
-    cudaError_t e = cudaMemcpyAsync(sigma_t_out, d_out, ob, cudaMemcpyDeviceToHost, st);
-    if (e != cudaSuccess) rc = fail(-2, std::string("D2H: ") + cudaGetErrorString(e));
-  }
-  cudaFreeAsync(d_out, st);
-  if (d_w) cudaFreeAsync(d_w, st);
-  cudaError_t e = cudaStreamSynchronize(st);
-  if (rc == 0 && e != cudaSuccess) rc = fail(-2, std::string("sync: ") + cudaGetErrorString(e));
-  return rc;
+  logsv_vol_paths_kernel<<<g.blocks, g.threads, 0, st>>>(d_out.as<double>(), d_w.as<double>(), S, nb_path, r, params->sigma0, seed, 0ull);
+  if (int rc = check_launch("logsv_vol_paths_kernel")) return rc;
+  B200SV_CUDA(cudaMemcpyAsync(sigma_t_out, d_out.p, ob, cudaMemcpyDeviceToHost, st));
+  return sync.done();
 }
 
 // ---- rough-LogSV multi-factor MC (rough_kernels.cuh) ------------------------------------------------------------------------
@@ -2481,7 +2373,7 @@ int b200sv_hawkesjd_mc_chain(const b200sv_hawkes_params* params, int M, const do
                              int flags, double* prices_out, double* stderr_out) {
   B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && stderr_out, "null pointer");
   return hawkes_chain_host(params, M, ttms, forwards, discfactors, offsets, strikes, types, nb_path, variable_type, seed, flags, prices_out,
-                           stderr_out, nullptr);
+                           stderr_out);
 }
 
 int b200sv_hawkesjd_terminal(const b200sv_hawkes_params* params, double ttm, long long nb_path, uint64_t seed, int flags, int slice_index,
@@ -2490,31 +2382,19 @@ int b200sv_hawkesjd_terminal(const b200sv_hawkes_params* params, double ttm, lon
   B200SV_REQUIRE(nb_path >= 1 && ttm > 0.0 && slice_index >= 0, "nb_path, ttm must be positive");
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
-  double *d = nullptr, *d_mom = nullptr;
-  const size_t nb = sizeof(double) * (size_t)nb_path;
-  B200SV_CUDA(cudaMallocAsync(&d, 3 * nb, st));
-  B200SV_CUDA(cudaMallocAsync(&d_mom, sizeof(double) * 2, st));
-  if (use_initial_arrays) {
-    B200SV_CUDA(cudaMemcpyAsync(d, x_inout, nb, cudaMemcpyHostToDevice, st));
-    B200SV_CUDA(cudaMemcpyAsync(d + nb_path, lambda_p_inout, nb, cudaMemcpyHostToDevice, st));
-    B200SV_CUDA(cudaMemcpyAsync(d + 2 * nb_path, lambda_m_inout, nb, cudaMemcpyHostToDevice, st));
-  }
+  StreamSync sync(st);
+  HostState s(x_inout, lambda_p_inout, lambda_m_inout, nb_path, st);
+  DevBuf d_mom(st);
+  if (int rc = s.alloc(use_initial_arrays != 0)) return rc;
+  B200SV_CUDA(d_mom.alloc(sizeof(double) * 2));
   int S;
   double dt;
   time_grid(ttm, kHawkesStepsPerYear, &S, &dt);
-  int rc = launch_hawkes_slice(d, d + nb_path, d + 2 * nb_path, nb_path, 0, use_initial_arrays ? 0 : 1, *params, S, dt, slice_index, 1.0, seed, flags,
-                               d_mom, st);
-  if (rc == 0) {
-    cudaError_t e = cudaMemcpyAsync(x_inout, d, nb, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(lambda_p_inout, d + nb_path, nb, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(lambda_m_inout, d + 2 * nb_path, nb, cudaMemcpyDeviceToHost, st);
-    if (e != cudaSuccess) rc = fail(-2, std::string("D2H: ") + cudaGetErrorString(e));
-  }
-  cudaFreeAsync(d, st);
-  cudaFreeAsync(d_mom, st);
-  cudaError_t e = cudaStreamSynchronize(st);
-  if (rc == 0 && e != cudaSuccess) rc = fail(-2, std::string("sync: ") + cudaGetErrorString(e));
-  return rc;
+  if (int rc = launch_hawkes_slice(s.dev(0), s.dev(1), s.dev(2), nb_path, 0, use_initial_arrays ? 0 : 1, *params, S, dt, slice_index, 1.0, seed,
+                                   flags, d_mom.as<double>(), st))
+    return rc;
+  if (int rc = s.download()) return rc;
+  return sync.done();
 }
 
 int b200sv_hawkesjd_step_fixed(double* x, double* lambda_p, double* lambda_m, const double* W0, const double* U_P, const double* U_M,
@@ -2523,31 +2403,22 @@ int b200sv_hawkesjd_step_fixed(double* x, double* lambda_p, double* lambda_m, co
   B200SV_REQUIRE(S >= 0 && N >= 1 && dt > 0.0, "S, N, dt");
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
-  double *d = nullptr, *w = nullptr;
-  const size_t nb = sizeof(double) * (size_t)N, wb = sizeof(double) * (size_t)N * (size_t)std::max(S, 1), wn = (size_t)N * (size_t)std::max(S, 1);
-  B200SV_CUDA(cudaMallocAsync(&d, 3 * nb, st));
-  B200SV_CUDA(cudaMallocAsync(&w, 5 * wb, st));
-  B200SV_CUDA(cudaMemcpyAsync(d, x, nb, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d + N, lambda_p, nb, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d + 2 * N, lambda_m, nb, cudaMemcpyHostToDevice, st));
+  StreamSync sync(st);
+  HostState s(x, lambda_p, lambda_m, N, st);
+  DevBuf w(st);
+  const size_t wb = sizeof(double) * (size_t)N * (size_t)std::max(S, 1), wn = (size_t)N * (size_t)std::max(S, 1);
+  if (int rc = s.alloc(true)) return rc;
+  B200SV_CUDA(w.alloc(5 * wb));
+  double* wd = w.as<double>();
   const double* src[5] = {W0, U_P, U_M, J_P, J_M};
   if (S > 0)
-    for (int k = 0; k < 5; ++k) B200SV_CUDA(cudaMemcpyAsync(w + k * wn, src[k], wb, cudaMemcpyHostToDevice, st));
+    for (int k = 0; k < 5; ++k) B200SV_CUDA(cudaMemcpyAsync(wd + k * wn, src[k], wb, cudaMemcpyHostToDevice, st));
   Grid g = persistent_grid(hawkes_step_fixed_kernel, kThreads, N);
-  hawkes_step_fixed_kernel<<<g.blocks, g.threads, 0, st>>>(d, d + N, d + 2 * N, w, w + wn, w + 2 * wn, w + 3 * wn, w + 4 * wn, S, N,
+  hawkes_step_fixed_kernel<<<g.blocks, g.threads, 0, st>>>(s.dev(0), s.dev(1), s.dev(2), wd, wd + wn, wd + 2 * wn, wd + 3 * wn, wd + 4 * wn, S, N,
                                                             make_hawkes_consts(*params, dt));
-  int rc = check_launch("hawkes_step_fixed_kernel");
-  if (rc == 0) {
-    cudaError_t e = cudaMemcpyAsync(x, d, nb, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(lambda_p, d + N, nb, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(lambda_m, d + 2 * N, nb, cudaMemcpyDeviceToHost, st);
-    if (e != cudaSuccess) rc = fail(-2, std::string("D2H: ") + cudaGetErrorString(e));
-  }
-  cudaFreeAsync(d, st);
-  cudaFreeAsync(w, st);
-  cudaError_t e = cudaStreamSynchronize(st);
-  if (rc == 0 && e != cudaSuccess) rc = fail(-2, std::string("sync: ") + cudaGetErrorString(e));
-  return rc;
+  if (int rc = check_launch("hawkes_step_fixed_kernel")) return rc;
+  if (int rc = s.download()) return rc;
+  return sync.done();
 }
 
 int b200sv_hawkesjd_device_draws(uint64_t seed, long long path0, long long n, int slice, int S, double dt, const b200sv_hawkes_params* params,
@@ -2557,25 +2428,21 @@ int b200sv_hawkesjd_device_draws(uint64_t seed, long long path0, long long n, in
   B200SV_REQUIRE(g == kGaussF32 || g == kGaussF64, "gauss flags");
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
-  double* d = nullptr;
+  StreamSync sync(st);
+  DevBuf d(st);
   const size_t wn = (size_t)n * S;
-  B200SV_CUDA(cudaMallocAsync(&d, sizeof(double) * 5 * wn, st));
+  B200SV_CUDA(d.alloc(sizeof(double) * 5 * wn));
+  double* w = d.as<double>();
   const HawkesConsts c = make_hawkes_consts(*params, dt);
   const int blocks = (int)((n + 127) / 128);
   if (g == kGaussF64)
-    hawkes_device_draws_kernel<kGaussF64><<<blocks, 128, 0, st>>>(seed, (unsigned long long)path0, n, (unsigned)slice, S, c, d, d + wn, d + 2 * wn, d + 3 * wn, d + 4 * wn);
+    hawkes_device_draws_kernel<kGaussF64><<<blocks, 128, 0, st>>>(seed, (unsigned long long)path0, n, (unsigned)slice, S, c, w, w + wn, w + 2 * wn, w + 3 * wn, w + 4 * wn);
   else
-    hawkes_device_draws_kernel<kGaussF32><<<blocks, 128, 0, st>>>(seed, (unsigned long long)path0, n, (unsigned)slice, S, c, d, d + wn, d + 2 * wn, d + 3 * wn, d + 4 * wn);
-  int rc = check_launch("hawkes_device_draws_kernel");
+    hawkes_device_draws_kernel<kGaussF32><<<blocks, 128, 0, st>>>(seed, (unsigned long long)path0, n, (unsigned)slice, S, c, w, w + wn, w + 2 * wn, w + 3 * wn, w + 4 * wn);
+  if (int rc = check_launch("hawkes_device_draws_kernel")) return rc;
   double* dst[5] = {W0, U_P, U_M, J_P, J_M};
-  for (int k = 0; k < 5 && rc == 0; ++k) {
-    cudaError_t e = cudaMemcpyAsync(dst[k], d + k * wn, sizeof(double) * wn, cudaMemcpyDeviceToHost, st);
-    if (e != cudaSuccess) rc = fail(-2, std::string("D2H: ") + cudaGetErrorString(e));
-  }
-  cudaFreeAsync(d, st);
-  cudaError_t e = cudaStreamSynchronize(st);
-  if (rc == 0 && e != cudaSuccess) rc = fail(-2, std::string("sync: ") + cudaGetErrorString(e));
-  return rc;
+  for (int k = 0; k < 5; ++k) B200SV_CUDA(cudaMemcpyAsync(dst[k], w + k * wn, sizeof(double) * wn, cudaMemcpyDeviceToHost, st));
+  return sync.done();
 }
 
 // ---- P2P mailbox (p2p.cuh) -----------------------------------------------------------------------------------------------

@@ -25,8 +25,6 @@
 #include "black.cuh"
 #include "fastmath64.cuh"
 
-extern "C" void b200sv_internal_count_launch(void);
-
 namespace b200sv {
 
 struct cd {
@@ -870,13 +868,6 @@ __global__ void __launch_bounds__(kFourierThreads) fourier_gamma_kernel(const cd
 // --------------------------------------------------------------------------------------------------------------------
 // host side
 // --------------------------------------------------------------------------------------------------------------------
-static int launched(const char* what) {
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(-2, std::string(what) + ": " + cudaGetErrorString(e));
-  b200sv_internal_count_launch();
-  return 0;
-}
-
 // Latency regime (few grid points in total): lane-parallel kernel; throughput regime (batches, the 40000-point psi grid): one thread per
 // point.  B200SV_MGF_LANES=0/1 overrides the choice (A/B timing in tools/bench_mgf.py).
 static bool use_lane_kernel(long long points) {
@@ -1481,20 +1472,6 @@ static bool all_half_re(const double* phi, int P) {
   return true;
 }
 
-struct DevBuf {   // RAII for stream-ordered temporaries
-  void* p = nullptr;
-  cudaStream_t st;
-  explicit DevBuf(cudaStream_t s) : st(s) {}
-  cudaError_t alloc(size_t n) { return cudaMallocAsync(&p, n ? n : 1, st); }
-  ~DevBuf() {
-    if (p) cudaFreeAsync(p, st);
-  }
-  template <typename T>
-  T* as() {
-    return (T*)p;
-  }
-};
-
 }  // namespace b200sv
 
 using namespace b200sv;
@@ -1549,6 +1526,7 @@ int b200sv_logsv_price_chain(const b200sv_logsv_params* params, int M, const dou
     }
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
+  StreamSync sync(st);
   DevBuf d_phi(st), d_psi(st), d_spec(st), d_a(st), d_lm(st), d_ss(st), d_pr(st), d_stat(st);
   B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
   B200SV_CUDA(d_psi.alloc(sizeof(cd) * P));
@@ -1572,19 +1550,18 @@ int b200sv_logsv_price_chain(const b200sv_logsv_params* params, int M, const dou
     launch_logsv_mgf<5>(tpb, nb, st, d_phi.as<cd>(), dpsi, P, M, d_spec.as<ChainSpec>(), nullptr, d_a.as<cd>(), d_lm.as<cd>(), y, d_stat.as<int>());
   else
     launch_logsv_mgf<3>(tpb, nb, st, d_phi.as<cd>(), dpsi, P, M, d_spec.as<ChainSpec>(), nullptr, d_a.as<cd>(), d_lm.as<cd>(), y, d_stat.as<int>());
-  if (int rc = launched("logsv_mgf_kernel")) return rc;
+  if (int rc = check_launch("logsv_mgf_kernel")) return rc;
   if (Jtot > 0) {
     if (qvar)
       fourier_sum_kernel<<<Jtot, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_psi.as<cd>(), P, d_ss.as<SumSpec>(), kModeQvar, 0, d_pr.as<double>());
     else
       fourier_vanilla_kernel<<<Jtot, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_phi.as<cd>(), P, d_ss.as<StrikeSpec>(), spot ? 1 : 0, 1, d_pr.as<double>());
-    if (int rc = launched("fourier_vanilla_kernel")) return rc;
+    if (int rc = check_launch("fourier_vanilla_kernel")) return rc;
     B200SV_CUDA(cudaMemcpyAsync(prices_out, d_pr.p, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st));
   }
   if (a_out) B200SV_CUDA(cudaMemcpyAsync(a_out, d_a.p, sizeof(cd) * (size_t)M * P * N, cudaMemcpyDeviceToHost, st));
   if (log_mgf_out) B200SV_CUDA(cudaMemcpyAsync(log_mgf_out, d_lm.p, sizeof(cd) * (size_t)M * P, cudaMemcpyDeviceToHost, st));
-  B200SV_CUDA(cudaStreamSynchronize(st));
-  return 0;
+  return sync.done();
 }
 
 int b200sv_heston_price_chain(const b200sv_heston_params* params, int M, const double* ttms, const double* forwards,
@@ -1622,6 +1599,7 @@ int b200sv_heston_price_chain(const b200sv_heston_params* params, int M, const d
     }
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
+  StreamSync sync(st);
   DevBuf d_phi(st), d_psi(st), d_dt(st), d_lm(st), d_ss(st), d_pr(st);
   B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
   B200SV_CUDA(d_psi.alloc(sizeof(cd) * P));
@@ -1639,18 +1617,17 @@ int b200sv_heston_price_chain(const b200sv_heston_params* params, int M, const d
   const int tpb = mgf_block_threads(P), nb = (P + tpb - 1) / tpb;
   heston_mgf_kernel<<<nb, tpb, 0, st>>>(d_phi.as<cd>(), qvar ? d_psi.as<cd>() : nullptr, P, M, d_dt.as<double>(), *params, nullptr, nullptr,
                                         nullptr, nullptr, d_lm.as<cd>());
-  if (int rc = launched("heston_mgf_kernel")) return rc;
+  if (int rc = check_launch("heston_mgf_kernel")) return rc;
   if (Jtot > 0) {
     if (qvar)
       fourier_sum_kernel<<<Jtot, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_psi.as<cd>(), P, d_ss.as<SumSpec>(), kModeQvar, 0, d_pr.as<double>());
     else
       fourier_vanilla_kernel<<<Jtot, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_phi.as<cd>(), P, d_ss.as<StrikeSpec>(), 1, 1, d_pr.as<double>());
-    if (int rc = launched("fourier_vanilla_kernel")) return rc;
+    if (int rc = check_launch("fourier_vanilla_kernel")) return rc;
     B200SV_CUDA(cudaMemcpyAsync(prices_out, d_pr.p, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st));
   }
   if (log_mgf_out) B200SV_CUDA(cudaMemcpyAsync(log_mgf_out, d_lm.p, sizeof(cd) * (size_t)M * P, cudaMemcpyDeviceToHost, st));
-  B200SV_CUDA(cudaStreamSynchronize(st));
-  return 0;
+  return sync.done();
 }
 
 /* ---- batched chain pricers: B parameter sets on one chain in one pass (calibration objective + its finite-difference gradient) ---- */
@@ -1706,6 +1683,7 @@ int b200sv_logsv_price_chain_batch(const b200sv_logsv_params* params, int B, int
   }
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
+  StreamSync sync(st);
   DevBuf d_phi(st), d_spec(st), d_y(st), d_a(st), d_lm(st), d_ss(st), d_pr(st), d_iv(st);
   const size_t nq = (size_t)B * Jtot;
   B200SV_CUDA(d_phi.alloc(sizeof(cd) * (size_t)G * P));
@@ -1728,14 +1706,13 @@ int b200sv_logsv_price_chain_batch(const b200sv_logsv_params* params, int B, int
   else
     launch_logsv_mgf<3>(tpb, nb, st, d_phi.as<cd>(), nullptr, P, M, d_spec.as<ChainSpec>(), nullptr, d_a.as<cd>(), d_lm.as<cd>(), 0.0, nullptr, B,
                         d_y.as<double>(), per_set_grid ? P : 0);
-  if (int rc = launched("logsv_mgf_kernel")) return rc;
+  if (int rc = check_launch("logsv_mgf_kernel")) return rc;
   fourier_vanilla_kernel<<<(unsigned)nq, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_phi.as<cd>(), P, d_ss.as<StrikeSpec>(), spot ? 1 : 0, 1,
                                                                     d_pr.as<double>(), ivols_out ? d_iv.as<double>() : nullptr);
-  if (int rc = launched("fourier_vanilla_kernel")) return rc;
+  if (int rc = check_launch("fourier_vanilla_kernel")) return rc;
   B200SV_CUDA(cudaMemcpyAsync(prices_out, d_pr.p, sizeof(double) * nq, cudaMemcpyDeviceToHost, st));
   if (ivols_out) B200SV_CUDA(cudaMemcpyAsync(ivols_out, d_iv.p, sizeof(double) * nq, cudaMemcpyDeviceToHost, st));
-  B200SV_CUDA(cudaStreamSynchronize(st));
-  return 0;
+  return sync.done();
 }
 
 int b200sv_heston_price_chain_batch(const b200sv_heston_params* params, int B, int M, const double* ttms, const double* forwards,
@@ -1756,6 +1733,7 @@ int b200sv_heston_price_chain_batch(const b200sv_heston_params* params, int B, i
   }
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
+  StreamSync sync(st);
   DevBuf d_phi(st), d_hp(st), d_dt(st), d_lm(st), d_ss(st), d_pr(st), d_iv(st);
   const size_t nq = (size_t)B * Jtot;
   B200SV_CUDA(d_phi.alloc(sizeof(cd) * (size_t)G * P));
@@ -1772,14 +1750,13 @@ int b200sv_heston_price_chain_batch(const b200sv_heston_params* params, int B, i
   const int tpb = 64, nb = (P + tpb - 1) / tpb;
   heston_mgf_kernel<<<dim3(nb, B), tpb, 0, st>>>(d_phi.as<cd>(), nullptr, P, M, d_dt.as<double>(), params[0], nullptr, nullptr, nullptr, nullptr,
                                                  d_lm.as<cd>(), d_hp.as<b200sv_heston_params>(), per_set_grid ? P : 0);
-  if (int rc = launched("heston_mgf_kernel")) return rc;
+  if (int rc = check_launch("heston_mgf_kernel")) return rc;
   fourier_vanilla_kernel<<<(unsigned)nq, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_phi.as<cd>(), P, d_ss.as<StrikeSpec>(), 1, 1, d_pr.as<double>(),
                                                                     ivols_out ? d_iv.as<double>() : nullptr);
-  if (int rc = launched("fourier_vanilla_kernel")) return rc;
+  if (int rc = check_launch("fourier_vanilla_kernel")) return rc;
   B200SV_CUDA(cudaMemcpyAsync(prices_out, d_pr.p, sizeof(double) * nq, cudaMemcpyDeviceToHost, st));
   if (ivols_out) B200SV_CUDA(cudaMemcpyAsync(ivols_out, d_iv.p, sizeof(double) * nq, cudaMemcpyDeviceToHost, st));
-  B200SV_CUDA(cudaStreamSynchronize(st));
-  return 0;
+  return sync.done();
 }
 
 /* Hawkes jump-diffusion Fourier chain (hawkesjd_chain_pricer / hawkesjd_chain_pricer_with_risk_premia, hawkes_jd_pricer.py:365-515).
@@ -1819,6 +1796,7 @@ int b200sv_hawkesjd_price_chain(const b200sv_hawkes_params* params, int M, const
   const HawkesMgfConsts c = make_hawkes_mgf_consts(*params);
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
+  StreamSync sync(st);
   DevBuf d_phi(st), d_dt(st), d_a(st), d_lm(st), d_ss(st), d_pr(st), d_g(st);
   B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
   B200SV_CUDA(d_dt.alloc(sizeof(double) * 2 * M));
@@ -1834,7 +1812,7 @@ int b200sv_hawkesjd_price_chain(const b200sv_hawkes_params* params, int M, const
     B200SV_CUDA(d_g.alloc(sizeof(cd) * (2 + 2 * (size_t)M)));
     B200SV_CUDA(cudaMemcpyAsync(d_g.p, two, sizeof(two), cudaMemcpyHostToDevice, st));
     hawkes_mgf_kernel<4><<<1, 4, 0, st>>>(d_g.as<cd>(), nullptr, 2, M, d_dt.as<double>() + M, c, nullptr, nullptr, d_g.as<cd>() + 2, 1, nullptr);
-    if (int rc = launched("hawkes_mgf_kernel")) return rc;
+    if (int rc = check_launch("hawkes_mgf_kernel")) return rc;
     std::vector<double> lm2(4 * (size_t)M);
     B200SV_CUDA(cudaMemcpyAsync(lm2.data(), d_g.as<cd>() + 2, sizeof(cd) * 2 * M, cudaMemcpyDeviceToHost, st));
     B200SV_CUDA(cudaStreamSynchronize(st));
@@ -1861,18 +1839,18 @@ int b200sv_hawkesjd_price_chain(const b200sv_hawkes_params* params, int M, const
     case 32: hawkes_mgf_kernel<32><<<nb, 32, 0, st>>>(d_phi.as<cd>(), nullptr, P, M, d_dt.as<double>(), c, nullptr, d_a.as<cd>(), d_lm.as<cd>(), 0, nullptr); break;
     default: hawkes_mgf_kernel<64><<<nb, 64, 0, st>>>(d_phi.as<cd>(), nullptr, P, M, d_dt.as<double>(), c, nullptr, d_a.as<cd>(), d_lm.as<cd>(), 0, nullptr); break;
   }
-  if (int rc = launched("hawkes_mgf_kernel")) return rc;
+  if (int rc = check_launch("hawkes_mgf_kernel")) return rc;
   if (Jtot > 0) {
     if (with_gamma)
       fourier_gamma_kernel<<<Jtot, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_phi.as<cd>(), P, d_ss.as<StrikeSpec>(), risk_premia_gamma, d_pr.as<double>());
     else
       fourier_vanilla_kernel<<<Jtot, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_phi.as<cd>(), P, d_ss.as<StrikeSpec>(), spot ? 1 : 0, 1, d_pr.as<double>());
-    if (int rc = launched("fourier kernel")) return rc;
+    if (int rc = check_launch("fourier kernel")) return rc;
     B200SV_CUDA(cudaMemcpyAsync(prices_out, d_pr.p, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st));
   }
   if (a_out) B200SV_CUDA(cudaMemcpyAsync(a_out, d_a.p, sizeof(cd) * (size_t)M * P * 3, cudaMemcpyDeviceToHost, st));
   if (log_mgf_out) B200SV_CUDA(cudaMemcpyAsync(log_mgf_out, d_lm.p, sizeof(cd) * (size_t)M * P, cudaMemcpyDeviceToHost, st));
-  B200SV_CUDA(cudaStreamSynchronize(st));
+  if (int rc = sync.done()) return rc;
   if (normalizers_out) std::copy(normalizers.begin(), normalizers.end(), normalizers_out);
   if (gamma_forwards_out) std::copy(gamma_forwards.begin(), gamma_forwards.end(), gamma_forwards_out);
   return 0;
@@ -1886,6 +1864,7 @@ int b200sv_hawkesjd_mgf_grid(const double* phi, const double* psi, int P, double
   const HawkesMgfConsts c = make_hawkes_mgf_consts(*params);
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
+  StreamSync sync(st);
   DevBuf d_phi(st), d_psi(st), d_dt(st), d_a0(st), d_a1(st), d_lm(st);
   B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
   B200SV_CUDA(d_psi.alloc(sizeof(cd) * P));
@@ -1906,11 +1885,10 @@ int b200sv_hawkesjd_mgf_grid(const double* phi, const double* psi, int P, double
     case 32: hawkes_mgf_kernel<32><<<nb, 32, 0, st>>>(d_phi.as<cd>(), dpsi, P, 1, d_dt.as<double>(), c, d_a0.as<cd>(), d_a1.as<cd>(), d_lm.as<cd>(), 0, nullptr); break;
     default: hawkes_mgf_kernel<64><<<nb, 64, 0, st>>>(d_phi.as<cd>(), dpsi, P, 1, d_dt.as<double>(), c, d_a0.as<cd>(), d_a1.as<cd>(), d_lm.as<cd>(), 0, nullptr); break;
   }
-  if (int rc = launched("hawkes_mgf_kernel")) return rc;
+  if (int rc = check_launch("hawkes_mgf_kernel")) return rc;
   B200SV_CUDA(cudaMemcpyAsync(a_inout, d_a1.p, sizeof(cd) * (size_t)P * 3, cudaMemcpyDeviceToHost, st));
   B200SV_CUDA(cudaMemcpyAsync(log_mgf_out, d_lm.p, sizeof(cd) * P, cudaMemcpyDeviceToHost, st));
-  B200SV_CUDA(cudaStreamSynchronize(st));
-  return 0;
+  return sync.done();
 }
 
 int b200sv_logsv_mgf_grid(const double* phi, const double* psi, int P, double dtau, double* a_inout,
@@ -1924,6 +1902,7 @@ int b200sv_logsv_mgf_grid(const double* phi, const double* psi, int P, double dt
   ChainSpec spec{dtau, make_model(*params, eta, is_spot_measure != 0)};
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
+  StreamSync sync(st);
   DevBuf d_phi(st), d_psi(st), d_spec(st), d_a0(st), d_a1(st), d_lm(st);
   B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
   B200SV_CUDA(d_psi.alloc(sizeof(cd) * P));
@@ -1942,11 +1921,10 @@ int b200sv_logsv_mgf_grid(const double* phi, const double* psi, int P, double dt
     launch_logsv_mgf<5>(tpb, nb, st, d_phi.as<cd>(), dpsi, P, 1, d_spec.as<ChainSpec>(), d_a0.as<cd>(), d_a1.as<cd>(), d_lm.as<cd>(), y, nullptr);
   else
     launch_logsv_mgf<3>(tpb, nb, st, d_phi.as<cd>(), dpsi, P, 1, d_spec.as<ChainSpec>(), d_a0.as<cd>(), d_a1.as<cd>(), d_lm.as<cd>(), y, nullptr);
-  if (int rc = launched("logsv_mgf_kernel")) return rc;
+  if (int rc = check_launch("logsv_mgf_kernel")) return rc;
   B200SV_CUDA(cudaMemcpyAsync(a_inout, d_a1.p, sizeof(cd) * (size_t)P * N, cudaMemcpyDeviceToHost, st));
   B200SV_CUDA(cudaMemcpyAsync(log_mgf_out, d_lm.p, sizeof(cd) * P, cudaMemcpyDeviceToHost, st));
-  B200SV_CUDA(cudaStreamSynchronize(st));
-  return 0;
+  return sync.done();
 }
 
 // func_a_ode_quadratic_terms (pricers/logsv/affine_expansion.py:67-184) for a grid of transform points: the dense tensors the reference
@@ -1962,6 +1940,7 @@ int b200sv_logsv_ode_terms(const double* phi, const double* psi, int P, const b2
   const LogsvModel model = make_model(*params, eta, is_spot_measure != 0);
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
+  StreamSync sync(st);
   DevBuf d_phi(st), d_psi(st), d_M(st), d_L(st), d_H(st);
   const size_t nM = (size_t)P * N * N * N, nL = (size_t)P * N * N, nH = (size_t)P * N;
   B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
@@ -1976,12 +1955,11 @@ int b200sv_logsv_ode_terms(const double* phi, const double* psi, int P, const b2
     logsv_ode_terms_kernel<5><<<(P + 63) / 64, 64, 0, st>>>(d_phi.as<cd>(), dpsi, P, model, d_M.as<cd>(), d_L.as<cd>(), d_H.as<cd>());
   else
     logsv_ode_terms_kernel<3><<<(P + 63) / 64, 64, 0, st>>>(d_phi.as<cd>(), dpsi, P, model, d_M.as<cd>(), d_L.as<cd>(), d_H.as<cd>());
-  if (int rc = launched("logsv_ode_terms_kernel")) return rc;
+  if (int rc = check_launch("logsv_ode_terms_kernel")) return rc;
   B200SV_CUDA(cudaMemcpyAsync(M_out, d_M.p, sizeof(cd) * nM, cudaMemcpyDeviceToHost, st));
   B200SV_CUDA(cudaMemcpyAsync(L_out, d_L.p, sizeof(cd) * nL, cudaMemcpyDeviceToHost, st));
   B200SV_CUDA(cudaMemcpyAsync(H_out, d_H.p, sizeof(cd) * nH, cudaMemcpyDeviceToHost, st));
-  B200SV_CUDA(cudaStreamSynchronize(st));
-  return 0;
+  return sync.done();
 }
 
 int b200sv_logsv_ode_rhs(const double* phi, const double* psi, int P, const double* A, const b200sv_logsv_params* params, double eta,
@@ -1993,6 +1971,7 @@ int b200sv_logsv_ode_rhs(const double* phi, const double* psi, int P, const doub
   const LogsvModel model = make_model(*params, eta, is_spot_measure != 0);
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
+  StreamSync sync(st);
   DevBuf d_phi(st), d_psi(st), d_A(st), d_R(st);
   B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
   B200SV_CUDA(d_psi.alloc(sizeof(cd) * P));
@@ -2006,10 +1985,9 @@ int b200sv_logsv_ode_rhs(const double* phi, const double* psi, int P, const doub
     logsv_ode_rhs_kernel<5><<<(P + 63) / 64, 64, 0, st>>>(d_phi.as<cd>(), dpsi, P, model, d_A.as<cd>(), d_R.as<cd>());
   else
     logsv_ode_rhs_kernel<3><<<(P + 63) / 64, 64, 0, st>>>(d_phi.as<cd>(), dpsi, P, model, d_A.as<cd>(), d_R.as<cd>());
-  if (int rc = launched("logsv_ode_rhs_kernel")) return rc;
+  if (int rc = check_launch("logsv_ode_rhs_kernel")) return rc;
   B200SV_CUDA(cudaMemcpyAsync(rhs_out, d_R.p, sizeof(cd) * (size_t)P * N, cudaMemcpyDeviceToHost, st));
-  B200SV_CUDA(cudaStreamSynchronize(st));
-  return 0;
+  return sync.done();
 }
 
 int b200sv_ode_rhs_dense(const double* A, int P, int n, const double* M, const double* L, const double* H, double* rhs_out) {
@@ -2017,6 +1995,7 @@ int b200sv_ode_rhs_dense(const double* A, int P, int n, const double* M, const d
   B200SV_REQUIRE(P >= 1 && n >= 1 && n <= 16, "P >= 1, 1 <= n <= 16");
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
+  StreamSync sync(st);
   DevBuf d_A(st), d_M(st), d_L(st), d_H(st), d_R(st);
   B200SV_CUDA(d_A.alloc(sizeof(cd) * (size_t)P * n));
   B200SV_CUDA(d_M.alloc(sizeof(cd) * (size_t)n * n * n));
@@ -2028,10 +2007,9 @@ int b200sv_ode_rhs_dense(const double* A, int P, int n, const double* M, const d
   B200SV_CUDA(cudaMemcpyAsync(d_L.p, L, sizeof(cd) * (size_t)n * n, cudaMemcpyHostToDevice, st));
   B200SV_CUDA(cudaMemcpyAsync(d_H.p, H, sizeof(cd) * n, cudaMemcpyHostToDevice, st));
   ode_rhs_dense_kernel<<<(P * n + 127) / 128, 128, 0, st>>>(d_A.as<cd>(), P, n, d_M.as<cd>(), d_L.as<cd>(), d_H.as<cd>(), d_R.as<cd>());
-  if (int rc = launched("ode_rhs_dense_kernel")) return rc;
+  if (int rc = check_launch("ode_rhs_dense_kernel")) return rc;
   B200SV_CUDA(cudaMemcpyAsync(rhs_out, d_R.p, sizeof(cd) * (size_t)P * n, cudaMemcpyDeviceToHost, st));
-  B200SV_CUDA(cudaStreamSynchronize(st));
-  return 0;
+  return sync.done();
 }
 
 // compute_logsv_a_mgf_grid(is_analytic=True): the semi-analytic branch over a transform grid (affine_expansion.py:388-470 -> :306-384)
@@ -2044,6 +2022,7 @@ int b200sv_logsv_mgf_grid_analytic(const double* phi, const double* psi, int P, 
   const LogsvModel model = make_model(*params, 1.0, is_spot_measure != 0);      // eta is ignored on this branch (reference :340-348)
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
+  StreamSync sync(st);
   DevBuf d_phi(st), d_psi(st), d_a0(st), d_a1(st), d_lm(st);
   B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
   B200SV_CUDA(d_psi.alloc(sizeof(cd) * P));
@@ -2059,11 +2038,10 @@ int b200sv_logsv_mgf_grid_analytic(const double* phi, const double* psi, int P, 
     logsv_mgf_analytic_kernel<5><<<(P + 63) / 64, 64, 0, st>>>(d_phi.as<cd>(), dpsi, P, model, dtau, year_days, d_a0.as<cd>(), d_a1.as<cd>(), d_lm.as<cd>(), y);
   else
     logsv_mgf_analytic_kernel<3><<<(P + 63) / 64, 64, 0, st>>>(d_phi.as<cd>(), dpsi, P, model, dtau, year_days, d_a0.as<cd>(), d_a1.as<cd>(), d_lm.as<cd>(), y);
-  if (int rc = launched("logsv_mgf_analytic_kernel")) return rc;
+  if (int rc = check_launch("logsv_mgf_analytic_kernel")) return rc;
   B200SV_CUDA(cudaMemcpyAsync(a_inout, d_a1.p, sizeof(cd) * (size_t)P * N, cudaMemcpyDeviceToHost, st));
   B200SV_CUDA(cudaMemcpyAsync(log_mgf_out, d_lm.p, sizeof(cd) * P, cudaMemcpyDeviceToHost, st));
-  B200SV_CUDA(cudaStreamSynchronize(st));
-  return 0;
+  return sync.done();
 }
 
 // compute_logsv_a_mgf_grid(is_stiff_solver=True): SciPy's BDF control law per grid point (affine_expansion.py:229-303)
@@ -2076,6 +2054,7 @@ int b200sv_logsv_mgf_grid_bdf(const double* phi, const double* psi, int P, doubl
   const LogsvModel model = make_model(*params, eta, is_spot_measure != 0);
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
+  StreamSync sync(st);
   DevBuf d_phi(st), d_psi(st), d_a0(st), d_a1(st), d_lm(st);
   B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
   B200SV_CUDA(d_psi.alloc(sizeof(cd) * P));
@@ -2091,11 +2070,10 @@ int b200sv_logsv_mgf_grid_bdf(const double* phi, const double* psi, int P, doubl
     logsv_mgf_bdf_kernel<5><<<(P + 63) / 64, 64, 0, st>>>(d_phi.as<cd>(), dpsi, P, model, dtau, d_a0.as<cd>(), d_a1.as<cd>(), d_lm.as<cd>(), y, nullptr);
   else
     logsv_mgf_bdf_kernel<3><<<(P + 63) / 64, 64, 0, st>>>(d_phi.as<cd>(), dpsi, P, model, dtau, d_a0.as<cd>(), d_a1.as<cd>(), d_lm.as<cd>(), y, nullptr);
-  if (int rc = launched("logsv_mgf_bdf_kernel")) return rc;
+  if (int rc = check_launch("logsv_mgf_bdf_kernel")) return rc;
   B200SV_CUDA(cudaMemcpyAsync(a_inout, d_a1.p, sizeof(cd) * (size_t)P * N, cudaMemcpyDeviceToHost, st));
   B200SV_CUDA(cudaMemcpyAsync(log_mgf_out, d_lm.p, sizeof(cd) * P, cudaMemcpyDeviceToHost, st));
-  B200SV_CUDA(cudaStreamSynchronize(st));
-  return 0;
+  return sync.done();
 }
 
 int b200sv_heston_mgf_grid(const double* phi, const double* psi, int P, double dtau, double* a_inout, double* b_inout,
@@ -2104,6 +2082,7 @@ int b200sv_heston_mgf_grid(const double* phi, const double* psi, int P, double d
   B200SV_REQUIRE(P >= 1 && dtau > 0.0, "P >= 1, dtau > 0");
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
+  StreamSync sync(st);
   DevBuf d_phi(st), d_psi(st), d_dt(st), d_a(st), d_b(st), d_a1(st), d_b1(st), d_lm(st);
   B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
   B200SV_CUDA(d_psi.alloc(sizeof(cd) * P));
@@ -2121,12 +2100,11 @@ int b200sv_heston_mgf_grid(const double* phi, const double* psi, int P, double d
   const int tpb = mgf_block_threads(P), nb = (P + tpb - 1) / tpb;
   heston_mgf_kernel<<<nb, tpb, 0, st>>>(d_phi.as<cd>(), psi ? d_psi.as<cd>() : nullptr, P, 1, d_dt.as<double>(), *params,
                                         d_a.as<cd>(), d_b.as<cd>(), d_a1.as<cd>(), d_b1.as<cd>(), d_lm.as<cd>());
-  if (int rc = launched("heston_mgf_kernel")) return rc;
+  if (int rc = check_launch("heston_mgf_kernel")) return rc;
   B200SV_CUDA(cudaMemcpyAsync(a_inout, d_a1.p, sizeof(cd) * P, cudaMemcpyDeviceToHost, st));
   B200SV_CUDA(cudaMemcpyAsync(b_inout, d_b1.p, sizeof(cd) * P, cudaMemcpyDeviceToHost, st));
   B200SV_CUDA(cudaMemcpyAsync(log_mgf_out, d_lm.p, sizeof(cd) * P, cudaMemcpyDeviceToHost, st));
-  B200SV_CUDA(cudaStreamSynchronize(st));
-  return 0;
+  return sync.done();
 }
 
 int b200sv_fourier_vanilla(const double* log_mgf, const double* phi, int P, double forward, const double* strikes,
@@ -2139,6 +2117,7 @@ int b200sv_fourier_vanilla(const double* log_mgf, const double* phi, int P, doub
   for (int j = 0; j < J; ++j) ss[j] = StrikeSpec{strikes[j], forward, discfactor, (int)types[j], 0, 1.0, 0};
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
+  StreamSync sync(st);
   DevBuf d_phi(st), d_lm(st), d_ss(st), d_pr(st);
   B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
   B200SV_CUDA(d_lm.alloc(sizeof(cd) * P));
@@ -2149,10 +2128,9 @@ int b200sv_fourier_vanilla(const double* log_mgf, const double* phi, int P, doub
   B200SV_CUDA(cudaMemcpyAsync(d_ss.p, ss.data(), sizeof(StrikeSpec) * J, cudaMemcpyHostToDevice, st));
   fourier_vanilla_kernel<<<J, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_phi.as<cd>(), P, d_ss.as<StrikeSpec>(), spot ? 1 : 0,
                                                         all_half_re(phi, P) ? 1 : 0, d_pr.as<double>());
-  if (int rc = launched("fourier_vanilla_kernel")) return rc;
+  if (int rc = check_launch("fourier_vanilla_kernel")) return rc;
   B200SV_CUDA(cudaMemcpyAsync(prices_out, d_pr.p, sizeof(double) * J, cudaMemcpyDeviceToHost, st));
-  B200SV_CUDA(cudaStreamSynchronize(st));
-  return 0;
+  return sync.done();
 }
 
 /* slice_pricer_with_mgf_grid_with_gamma (utils/mgf_pricer.py:273-320) on caller-supplied log-MGF / transform grids: 'C' / 'P' under the spot
@@ -2169,6 +2147,7 @@ int b200sv_fourier_gamma(const double* log_mgf, const double* phi, int P, double
   }
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
+  StreamSync sync(st);
   DevBuf d_phi(st), d_lm(st), d_ss(st), d_pr(st);
   B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
   B200SV_CUDA(d_lm.alloc(sizeof(cd) * P));
@@ -2178,10 +2157,9 @@ int b200sv_fourier_gamma(const double* log_mgf, const double* phi, int P, double
   B200SV_CUDA(cudaMemcpyAsync(d_lm.p, log_mgf, sizeof(cd) * P, cudaMemcpyHostToDevice, st));
   B200SV_CUDA(cudaMemcpyAsync(d_ss.p, ss.data(), sizeof(StrikeSpec) * J, cudaMemcpyHostToDevice, st));
   fourier_gamma_kernel<<<J, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_phi.as<cd>(), P, d_ss.as<StrikeSpec>(), risk_premia_gamma, d_pr.as<double>());
-  if (int rc = launched("fourier_gamma_kernel")) return rc;
+  if (int rc = check_launch("fourier_gamma_kernel")) return rc;
   B200SV_CUDA(cudaMemcpyAsync(prices_out, d_pr.p, sizeof(double) * J, cudaMemcpyDeviceToHost, st));
-  B200SV_CUDA(cudaStreamSynchronize(st));
-  return 0;
+  return sync.done();
 }
 
 // shared driver of the generic sums
@@ -2190,6 +2168,7 @@ static int fourier_sum_host(const double* log_mgf, const double* grid, int P, co
   const int J = (int)specs.size();
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
+  StreamSync sync(st);
   DevBuf d_g(st), d_lm(st), d_ss(st), d_pr(st);
   B200SV_CUDA(d_g.alloc(sizeof(cd) * P));
   B200SV_CUDA(d_lm.alloc(sizeof(cd) * P));
@@ -2199,10 +2178,9 @@ static int fourier_sum_host(const double* log_mgf, const double* grid, int P, co
   B200SV_CUDA(cudaMemcpyAsync(d_lm.p, log_mgf, sizeof(cd) * P, cudaMemcpyHostToDevice, st));
   B200SV_CUDA(cudaMemcpyAsync(d_ss.p, specs.data(), sizeof(SumSpec) * J, cudaMemcpyHostToDevice, st));
   fourier_sum_kernel<<<J, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_g.as<cd>(), P, d_ss.as<SumSpec>(), mode, all_calls, d_pr.as<double>());
-  if (int rc = launched("fourier_sum_kernel")) return rc;
+  if (int rc = check_launch("fourier_sum_kernel")) return rc;
   B200SV_CUDA(cudaMemcpyAsync(out, d_pr.p, sizeof(double) * J, cudaMemcpyDeviceToHost, st));
-  B200SV_CUDA(cudaStreamSynchronize(st));
-  return 0;
+  return sync.done();
 }
 
 int b200sv_fourier_qvar(const double* log_mgf, const double* psi, int P, double ttm, const double* strikes, const int8_t* types, int J,
