@@ -350,6 +350,21 @@ int b200sv_heston_price_chain(const b200sv_heston_params* params, int M, const d
                               const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
                               int variable_type, double vol_scaler, int P, double* prices_out, double* log_mgf_out);
 
+/* prices and forward-mode sensitivities of the two Fourier chain pricers above (DESIGN.md §4.2), LOG_RETURN only (else -4).  Arguments as
+ * in b200sv_*_price_chain; prices_out is bit-identical to it.  greeks_out [2 + n][J], J = offsets[M]-offsets[0]: d price / d forwards[m],
+ * d^2 price / d forwards[m]^2, then d price / d parameter in struct field order (n = 6 LogSV, 5 Heston; vol_scaler, etas and discount
+ * factors held fixed).  Optional outputs (may be NULL): dlog_mgf_out [n][M][P] complex128 interleaved, the parameter derivatives of the
+ * log-MGF grid; nfev_out [P], right-hand-side evaluations per grid point over the chain (the mesh the tangents were stepped on). */
+int b200sv_logsv_price_chain_greeks(const b200sv_logsv_params* params, int M, const double* ttms, const double* forwards,
+                                    const double* discfactors, const double* etas, const int* offsets, const double* strikes,
+                                    const int8_t* types, int is_spot_measure, int variable_type, int expansion_order,
+                                    double vol_scaler, int P, double* prices_out, double* greeks_out, double* dlog_mgf_out,
+                                    int* nfev_out);
+int b200sv_heston_price_chain_greeks(const b200sv_heston_params* params, int M, const double* ttms, const double* forwards,
+                                     const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
+                                     int variable_type, double vol_scaler, int P, double* prices_out, double* greeks_out,
+                                     double* dlog_mgf_out);
+
 /* B parameter sets on ONE chain in one pass -- the objective of the calibration drivers and its finite-difference gradient:
  * _LogSvCalibrationObjective.__call__ (pricers/logsv_pricer.py:234-294: compute_model_ivols_for_chain = logsv_chain_pricer +
  * option_chain.compute_model_ivols_from_chain_data), which scipy SLSQP evaluates n+1 times per iteration, one parameter set at a time.

@@ -18,6 +18,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/b200sv.h"
@@ -214,11 +215,17 @@ struct StageStore {
   __device__ __forceinline__ cd& at(int stage, int k) { return base[(stage * N + k) * TPB]; }
 };
 
+// No tangent: the default of rk45_generic, every hook call compiles away.
+struct NoTangent {};
+
 // returns 0 ok, 1 step size underflow (SciPy: TOO_SMALL_STEP -> solver fails, reference keeps the last accepted state)
 // Rhs: functor ``void operator()(const cd (&A)[N], cd (&out)[N]) const`` -- the LogSV coefficient ODEs (LogsvRhsFn) or the Hawkes Riccati
 // system (HawkesRhsFn); the control law does not depend on it.
-template <int N, int TPB, typename Rhs>
-__device__ int rk45_generic(cd (&y)[N], double T, const Rhs& rhs_fn, StageStore<N, TPB> K, int* nfev_out) {
+// Tan (optional, LogsvTangentHook): a forward-mode derivative stepped on the SAME attempts -- it sees every stage input, the step size
+// and the acceptance, and never feeds back into the error norm, so the mesh is the primal's.
+template <int N, int TPB, typename Rhs, typename Tan = NoTangent>
+__device__ int rk45_generic(cd (&y)[N], double T, const Rhs& rhs_fn, StageStore<N, TPB> K, int* nfev_out, Tan* tan = nullptr) {
+  constexpr bool kTan = !std::is_same<Tan, NoTangent>::value;
   // stage coefficients: c_A in constant memory (indexed by the non-unrolled stage loop)
   constexpr double B[6] = {35.0 / 384, 0, 500.0 / 1113, 125.0 / 192, -2187.0 / 6784, 11.0 / 84};
   constexpr double E[7] = {-71.0 / 57600, 0, 71.0 / 16695, -71.0 / 1920, 17253.0 / 339200, -22.0 / 525, 1.0 / 40};
@@ -250,6 +257,7 @@ __device__ int rk45_generic(cd (&y)[N], double T, const Rhs& rhs_fn, StageStore<
   int status = 0;
 #pragma unroll
   for (int k = 0; k < N; ++k) K.at(0, k) = f[k];
+  if constexpr (kTan) tan->start(y);
   // ONE loop over step ATTEMPTS (SciPy nests "while not accepted" inside the step loop): a lane that rejects an attempt simply goes round
   // again with the lanes that accepted theirs, so a warp runs max-over-lanes of the TOTAL attempts instead of the sum over steps of
   // the per-step maximum.  Same arithmetic per point.
@@ -280,6 +288,7 @@ __device__ int rk45_generic(cd (&y)[N], double T, const Rhs& rhs_fn, StageStore<
           for (int jj = 1; jj < 5; ++jj) acc = acc + K.at(jj, k) * c_A[s][jj];
           yt[k] = y[k] + acc * h;
         }
+        if constexpr (kTan) tan->stage(s, yt, h);
         rhs_fn(yt, kn);
 #pragma unroll
         for (int k = 0; k < N; ++k) K.at(s, k) = kn[k];
@@ -293,6 +302,7 @@ __device__ int rk45_generic(cd (&y)[N], double T, const Rhs& rhs_fn, StageStore<
         yn[k] = y[k] + h * acc;
       }
       rhs_fn(yn, kn);                                                   // K[6] = f(t + h, y_new)
+      if constexpr (kTan) tan->last(yn, h);
       nfev += 6;
       cd err[N];
 #pragma unroll
@@ -316,6 +326,7 @@ __device__ int rk45_generic(cd (&y)[N], double T, const Rhs& rhs_fn, StageStore<
           y[k] = yn[k];
           K.at(0, k) = kn[k];     // FSAL: K[6] of this step is K[0] of the next
         }
+        if constexpr (kTan) tan->accept();
       }
       rejected = !accepted;
     }
@@ -862,6 +873,343 @@ __global__ void __launch_bounds__(kFourierThreads) fourier_gamma_kernel(const cd
   if (threadIdx.x == 0) {
     const double gk = pow(sp.strike, 1.0 + gamma);
     prices[blockIdx.x] = (sp.type == B200SV_CALL ? sp.ttm : sp.strike) - sp.discfactor * gk * acc[0];
+  }
+}
+
+// --------------------------------------------------------------------------------------------------------------------
+// Forward-mode sensitivities of the Fourier chain pricers (DESIGN.md §4.2)
+// --------------------------------------------------------------------------------------------------------------------
+// d(LogsvModel field) / d(one parameter), built on the host (make_model_tangents); eta2 does not depend on the parameters.
+struct LogsvModelTangent {
+  double theta, th2, v2, qv, qv2, lam, k2p, kp, beta_eta;
+};
+constexpr int kLogsvOdeDirs = 5;     // theta, kappa1, kappa2, beta, volvol (sigma0 enters only through y = sigma0 - theta)
+constexpr int kHestonOdeDirs = 4;    // theta, kappa, rho, volvol (v0 enters only through log_mgf = a + b v0)
+
+// make_model differentiated field by field; kappa2 is held fixed when kappa1 or theta moves
+static void make_model_tangents(const b200sv_logsv_params& p, double eta, bool spot, LogsvModelTangent (&d)[kLogsvOdeDirs]) {
+  for (auto& t : d) t = LogsvModelTangent{0, 0, 0, 0, 0, 0, 0, 0, 0};
+  const double v2 = p.beta * p.beta + p.volvol * p.volvol, th2 = p.theta * p.theta;
+  LogsvModelTangent& th = d[0];      // theta
+  th.theta = 1.0;
+  th.th2 = 2.0 * p.theta;
+  th.qv = v2;
+  th.qv2 = 2.0 * p.theta * v2;
+  th.lam = spot ? 0.0 : 2.0 * p.beta * p.theta * eta;
+  th.kp = spot ? p.kappa2 : p.kappa2 - 2.0 * p.beta * eta;
+  d[1].kp = 1.0;                     // kappa1
+  d[2].k2p = 1.0;                    // kappa2
+  d[2].kp = p.theta;
+  LogsvModelTangent& be = d[3];      // beta
+  be.v2 = 2.0 * p.beta;
+  be.qv = 2.0 * p.beta * p.theta;
+  be.qv2 = 2.0 * p.beta * th2;
+  be.lam = spot ? 0.0 : th2 * eta;
+  be.k2p = spot ? 0.0 : -eta;
+  be.kp = spot ? 0.0 : -2.0 * p.theta * eta;
+  be.beta_eta = eta;
+  LogsvModelTangent& vv = d[4];      // volvol
+  vv.v2 = 2.0 * p.volvol;
+  vv.qv = 2.0 * p.volvol * p.theta;
+  vv.qv2 = 2.0 * p.volvol * th2;
+}
+
+// make_coef differentiated: linear in the model fields except the products th2 * beta_eta, theta * beta_eta (in b) and th2 * eta2,
+// theta * eta2 (in h0, h1), which take the product rule
+__device__ __forceinline__ Coef make_dcoef(const LogsvModel& m, const LogsvModelTangent& d, cd phi, cd psi) {
+  Coef c;
+  const cd b = m.beta_eta * phi, db = d.beta_eta * phi;
+  const cd dtb = d.th2 * b + m.th2 * db;          // d(th2 b)
+  const cd d1b = d.theta * b + m.theta * db;      // d(theta b)
+  c.l01 = mk(d.lam) - dtb;
+  c.l11 = mk(-d.kp) - 2.0 * d1b;
+  c.l12 = 2.0 * (mk(d.lam + d.qv) - dtb);
+  c.l21 = mk(-d.k2p) - db;
+  c.l22 = mk(d.v2 - 2.0 * d.kp) - 4.0 * d1b;
+  c.l23 = 3.0 * (mk(2.0 * d.qv) - dtb);
+  c.l32 = -2.0 * (mk(d.k2p) + db);
+  c.l33 = 3.0 * (mk(d.v2 - d.kp) - 2.0 * d1b);
+  c.l34 = 4.0 * (mk(3.0 * d.qv) - dtb);
+  c.l43 = -3.0 * (mk(d.k2p) + db);
+  c.l44 = 2.0 * (mk(d.v2 - 2.0 * d.kp) - 4.0 * d1b);
+  const cd r = m.spot ? phi * (phi + mk(1.0)) - 2.0 * psi : phi * (phi - mk(1.0)) - 2.0 * psi;
+  c.h0 = (0.5 * d.th2 * m.eta2) * r;
+  c.h1 = (d.theta * m.eta2) * r;
+  c.h2 = mk(0.0);
+  return c;
+}
+
+// The rows of rhs<>() with the products A_i A_j given as q = {11, 12, 22, 13, 14, 23, 24, 33} and the linear inputs as u, H added if
+// WithH.  The right-hand side is linear in q, in u and in (v2, qv, qv2, Coef) separately, so both halves of its tangent are this function.
+template <int N, int TPB, bool WithH>
+__device__ __forceinline__ void rhs_rows(const cd (&q)[8], const cd (&u)[N], double v2, double qv, double qv2, const CoefView<TPB>& cv,
+                                         cd (&out)[N]) {
+  const cd h0 = WithH ? cv.at(11) : mk(0.0), h1 = WithH ? cv.at(12) : mk(0.0), h2 = WithH ? cv.at(13) : mk(0.0);
+  out[0] = (0.5 * qv2) * q[0] + cv.at(0) * u[1] + qv2 * u[2] + h0;
+  if constexpr (N == 5) {
+    out[1] = qv * q[0] + (2.0 * qv2) * q[1] + cv.at(1) * u[1] + cv.at(2) * u[2] + (3.0 * qv2) * u[3] + h1;
+    out[2] = (0.5 * v2) * q[0] + (2.0 * qv2) * q[2] + (4.0 * qv) * q[1] + (3.0 * qv2) * q[3] + cv.at(3) * u[1] + cv.at(4) * u[2] +
+             cv.at(5) * u[3] + (6.0 * qv2) * u[4] + h2;
+    out[3] = (4.0 * qv) * q[2] + (2.0 * v2) * q[1] + (6.0 * qv) * q[3] + (4.0 * qv2) * q[4] + (6.0 * qv2) * q[5] + cv.at(6) * u[2] +
+             cv.at(7) * u[3] + cv.at(8) * u[4];
+    out[4] = (2.0 * v2) * q[2] + (4.5 * qv2) * q[7] + (3.0 * v2) * q[3] + (8.0 * qv) * q[4] + (12.0 * qv) * q[5] + (8.0 * qv2) * q[6] +
+             cv.at(9) * u[3] + cv.at(10) * u[4];
+  } else {
+    out[1] = qv * q[0] + (2.0 * qv2) * q[1] + cv.at(1) * u[1] + cv.at(2) * u[2] + h1;
+    out[2] = (0.5 * v2) * q[0] + (2.0 * qv2) * q[2] + (4.0 * qv) * q[1] + cv.at(3) * u[1] + cv.at(4) * u[2] + h2;
+  }
+}
+
+// d f(A) = J(A) dA + d_p f(A):  J(A) dA = rows(products A_i dA_j + dA_i A_j, dA; model, Coef without H) and d_p f(A) = rows(A_i A_j, A;
+// d model, d Coef with d H).
+template <int N, int TPB>
+__device__ __forceinline__ void rhs_tangent(const cd (&A)[N], const cd (&dA)[N], const LogsvModel& m, const CoefView<TPB>& c,
+                                            const LogsvModelTangent& dm, const CoefView<TPB>& dc, cd (&out)[N]) {
+  const cd z = mk(0.0);
+  cd q[8] = {A[1] * A[1], A[1] * A[2], A[2] * A[2], z, z, z, z, z};
+  cd dq[8] = {2.0 * (A[1] * dA[1]), A[1] * dA[2] + dA[1] * A[2], 2.0 * (A[2] * dA[2]), z, z, z, z, z};
+  if constexpr (N == 5) {
+    q[3] = A[1] * A[3]; q[4] = A[1] * A[4]; q[5] = A[2] * A[3]; q[6] = A[2] * A[4]; q[7] = A[3] * A[3];
+    dq[3] = A[1] * dA[3] + dA[1] * A[3];
+    dq[4] = A[1] * dA[4] + dA[1] * A[4];
+    dq[5] = A[2] * dA[3] + dA[2] * A[3];
+    dq[6] = A[2] * dA[4] + dA[2] * A[4];
+    dq[7] = 2.0 * (A[3] * dA[3]);
+  }
+  cd jv[N], pv[N];
+  rhs_rows<N, TPB, false>(dq, dA, m.v2, m.qv, m.qv2, c, jv);
+  rhs_rows<N, TPB, true>(q, A, dm.v2, dm.qv, dm.qv2, dc, pv);
+#pragma unroll
+  for (int k = 0; k < N; ++k) out[k] = jv[k] + pv[k];
+}
+
+// The tangent of one parameter direction stepped on rk45_generic's attempts: dY_s = dy + h sum_j a_sj dK_j, dK_s = d f(Y_s), accepted
+// steps commit dy <- dy + h sum_j b_j dK_j and dK_0 <- dK_6 (FSAL).  dK: 8 "stages" in shared memory, 0..6 the stage tangents, 7 the
+// candidate dy of the current attempt.  dy stays in registers and carries over maturities like A.
+template <int N, int TPB>
+struct LogsvTangentHook {
+  const LogsvModel* m;
+  const CoefView<TPB>* c;
+  LogsvModelTangent dm;
+  CoefView<TPB> dc;
+  StageStore<N, TPB> dK;        // StageStore indexes (stage * N + k) * TPB: 8 stages fit in 8 * N * TPB entries
+  cd dy[N];
+
+  __device__ __forceinline__ void eval(int s, const cd (&Y)[N], const cd (&dY)[N]) {
+    cd o[N];
+    rhs_tangent<N, TPB>(Y, dY, *m, *c, dm, dc, o);
+#pragma unroll
+    for (int k = 0; k < N; ++k) dK.at(s, k) = o[k];
+  }
+  __device__ __forceinline__ void start(const cd (&y)[N]) { eval(0, y, dy); }
+  __device__ __forceinline__ void stage(int s, const cd (&yt)[N], double h) {
+    cd dyt[N];
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+      cd acc = dK.at(0, k) * c_A[s][0];
+#pragma unroll
+      for (int jj = 1; jj < 5; ++jj) acc = acc + dK.at(jj, k) * c_A[s][jj];
+      dyt[k] = dy[k] + acc * h;
+    }
+    eval(s, yt, dyt);
+  }
+  __device__ __forceinline__ void last(const cd (&yn)[N], double h) {
+    constexpr double B[6] = {35.0 / 384, 0, 500.0 / 1113, 125.0 / 192, -2187.0 / 6784, 11.0 / 84};
+    cd dyn[N];
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+      cd acc = dK.at(0, k) * B[0];
+#pragma unroll
+      for (int jj = 2; jj < 6; ++jj) acc = acc + dK.at(jj, k) * B[jj];
+      dyn[k] = dy[k] + h * acc;
+      dK.at(7, k) = dyn[k];
+    }
+    eval(6, yn, dyn);
+  }
+  __device__ __forceinline__ void accept() {
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+      dy[k] = dK.at(7, k);
+      dK.at(0, k) = dK.at(6, k);
+    }
+  }
+};
+
+constexpr int kTangentTPB = 16;      // shared memory per thread: 6N primal stages + 8N tangent stages + 2 x 14 coefficients
+
+// One thread = one (grid point, parameter direction): the primal integration of logsv_mgf_kernel (same rk45_generic, same mesh) plus one
+// tangent.  The D = 5 directions of a point are neighbouring threads, so a warp runs few meshes.  dspec [M][5]: d(model)/d(direction).
+// Outputs: dlog_mgf [6][M][P] (row 0 sigma0, rows 1.. the directions, LOGSV_GREEK_PARAMS order), log_mgf [M][P], status [P], nfev [P].
+template <int N>
+__global__ void __launch_bounds__(kTangentTPB) logsv_mgf_tangent_kernel(const cd* __restrict__ phi, int P, int M, const ChainSpec* __restrict__ spec,
+                                                                         const LogsvModelTangent* __restrict__ dspec, double y,
+                                                                         cd* __restrict__ dlog_mgf, cd* __restrict__ log_mgf,
+                                                                         int* __restrict__ status, int* __restrict__ nfev) {
+  constexpr int TPB = kTangentTPB, D = kLogsvOdeDirs;
+  __shared__ cd stage_smem[6 * N * TPB];
+  __shared__ cd tan_smem[8 * N * TPB];
+  __shared__ cd coef_smem[14 * TPB];
+  __shared__ cd dcoef_smem[14 * TPB];
+  const int t = blockIdx.x * TPB + threadIdx.x;
+  if (t >= P * D) return;
+  const int p = t / D, dir = t % D;
+#pragma unroll
+  for (int i = 0; i < 6 * N; ++i) stage_smem[threadIdx.x + i * TPB] = mk(0.0);
+#pragma unroll
+  for (int i = 0; i < 8 * N; ++i) tan_smem[threadIdx.x + i * TPB] = mk(0.0);
+  StageStore<N, TPB> K{stage_smem + threadIdx.x};
+  const CoefView<TPB> c{coef_smem + threadIdx.x};
+  LogsvTangentHook<N, TPB> tan;
+  tan.c = &c;
+  tan.dc = CoefView<TPB>{dcoef_smem + threadIdx.x};
+  tan.dK = StageStore<N, TPB>{tan_smem + threadIdx.x};
+  cd A[N];
+#pragma unroll
+  for (int k = 0; k < N; ++k) {
+    A[k] = mk(0.0);
+    tan.dy[k] = mk(0.0);
+  }
+  const cd ph = phi[p], ps = mk(0.0);
+  const double y2 = y * y;
+  const double ys[5] = {1.0, y, y2, y2 * y, y2 * y2};
+  const double dys[5] = {0.0, 1.0, 2.0 * y, 3.0 * y2, 4.0 * (y2 * y)};      // d ys / d y; dy/dsigma0 = 1, dy/dtheta = -1
+  const double dy_dp = dir == 0 ? -1.0 : 0.0;
+  int st = 0, nf = 0;
+  for (int mm = 0; mm < M; ++mm) {
+    const LogsvModel model = spec[mm].model;
+    store_coef<TPB>(coef_smem + threadIdx.x, make_coef(model, ph, ps));
+    tan.m = &model;
+    tan.dm = dspec[mm * D + dir];
+    store_coef<TPB>(dcoef_smem + threadIdx.x, make_dcoef(model, tan.dm, ph, ps));
+    int nfe = 0;
+    st |= rk45_generic<N, TPB>(A, spec[mm].dtau, LogsvRhsFn<N, TPB>{model, c}, K, &nfe, &tan);
+    nf += nfe;
+    cd lm = mk(0.0), dlm = mk(0.0), dls = mk(0.0);
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+      lm = lm + A[k] * ys[k];
+      dlm = dlm + (tan.dy[k] * ys[k] + A[k] * (dys[k] * dy_dp));
+      dls = dls + A[k] * dys[k];
+    }
+    dlog_mgf[((size_t)(1 + dir) * M + mm) * P + p] = dlm;
+    if (dir == 0) {
+      dlog_mgf[(size_t)mm * P + p] = dls;
+      log_mgf[(size_t)mm * P + p] = lm;
+    }
+  }
+  if (dir == 0) {
+    if (status) status[p] = st;
+    if (nfev) nfev[p] = nf;
+  }
+}
+
+// dual complex numbers (value, derivative in one direction) for the Heston closed form
+struct dcd {
+  cd v, d;
+};
+__device__ __forceinline__ dcd dmk(cd v, cd d = mk(0.0)) { return dcd{v, d}; }
+__device__ __forceinline__ dcd operator+(dcd a, dcd b) { return dcd{a.v + b.v, a.d + b.d}; }
+__device__ __forceinline__ dcd operator-(dcd a, dcd b) { return dcd{a.v - b.v, a.d - b.d}; }
+__device__ __forceinline__ dcd operator-(dcd a) { return dcd{-a.v, -a.d}; }
+__device__ __forceinline__ dcd operator*(dcd a, dcd b) { return dcd{a.v * b.v, a.d * b.v + a.v * b.d}; }
+__device__ __forceinline__ dcd operator*(double s, dcd a) { return dcd{s * a.v, s * a.d}; }
+__device__ __forceinline__ dcd operator/(dcd a, dcd b) {
+  const cd q = a.v / b.v;
+  return dcd{q, (a.d - q * b.d) / b.v};
+}
+__device__ __forceinline__ dcd dsqrt(dcd z) {
+  const cd s = csqrt_(z.v);
+  return dcd{s, z.d / (2.0 * s)};
+}
+__device__ __forceinline__ dcd dexp(dcd z) {
+  const cd e = cexp_(z.v);
+  return dcd{e, e * z.d};
+}
+__device__ __forceinline__ dcd dlog(dcd z) { return dcd{clog_(z.v), z.d / z.v}; }
+
+// heston_mgf_kernel in forward mode: one thread = one (grid point, direction theta | kappa | rho | volvol), (a, b) and their tangents
+// carried over the maturities.  dlog_mgf [5][M][P]: row 0 d/dv0 = b, rows 1.. the directions (HESTON_GREEK_PARAMS order).
+__global__ void heston_mgf_tangent_kernel(const cd* __restrict__ phi, int P, int M, const double* __restrict__ dtaus, b200sv_heston_params hp,
+                                          cd* __restrict__ dlog_mgf) {
+  constexpr int D = kHestonOdeDirs;
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= P * D) return;
+  const int p = t / D, dir = t % D;
+  const dcd th = dmk(mk(hp.theta), mk(dir == 0 ? 1.0 : 0.0)), ka = dmk(mk(hp.kappa), mk(dir == 1 ? 1.0 : 0.0));
+  const dcd rho = dmk(mk(hp.rho), mk(dir == 2 ? 1.0 : 0.0)), vv = dmk(mk(hp.volvol), mk(dir == 3 ? 1.0 : 0.0));
+  const dcd ph = dmk(phi[p]);
+  const dcd vv2 = vv * vv;
+  const dcd b1 = ka + (rho * vv) * ph;
+  const dcd b0 = dmk((0.5 * ph.v) * (ph.v + mk(1.0)));
+  const dcd zeta = dsqrt(b1 * b1 - (2.0 * b0) * vv2);
+  const dcd psi_p = zeta - b1, psi_m = b1 + zeta;
+  const dcd two_zeta = 2.0 * zeta;
+  dcd a = dmk(mk(0.0)), b = dmk(mk(0.0));
+  for (int mm = 0; mm < M; ++mm) {
+    const double tau = dtaus[mm];
+    const dcd ez = dexp(-(tau * zeta));
+    const dcd c_p = (psi_p + vv2 * b) / two_zeta, c_m = (psi_m - vv2 * b) / two_zeta;
+    const dcd den = c_p * ez + c_m;
+    const dcd b_new = -((-(psi_m * c_p)) * ez + psi_p * c_m) / (vv2 * den);
+    const dcd a_new = (-((th * ka) / vv2)) * (tau * psi_p + 2.0 * dlog(den)) + a;
+    a = a_new;
+    b = b_new;
+    dlog_mgf[((size_t)(1 + dir) * M + mm) * P + p] = a.d + b.d * hp.v0;
+    if (dir == 0) dlog_mgf[(size_t)mm * P + p] = b.v;
+  }
+}
+
+// Fourier sums of fourier_vanilla_kernel (|Re phi| = 1/2 branch, real weights w) and their derivatives, one CTA per strike, fixed-order
+// block_sum:  S = sum w Re e^z,  S_x = sum w Re(-phi e^z),  S_xx = sum w Re(phi^2 e^z),  S_p = sum w Re(e^z dlm_p),  z = lm - x phi,
+// x = ln(F/K); a grid point whose price term is NaN is skipped in every sum.  greeks [2 + NP][J]: delta, gamma, d price / d parameter.
+template <int NP>
+__global__ void __launch_bounds__(kFourierThreads) fourier_vanilla_greeks_kernel(const cd* __restrict__ log_mgf, const cd* __restrict__ dlog_mgf,
+                                                                                const cd* __restrict__ phi, int P, int M,
+                                                                                const StrikeSpec* __restrict__ specs, int is_spot,
+                                                                                double* __restrict__ greeks) {
+  constexpr int NV = 3 + NP;
+  __shared__ double red[NV * (kFourierThreads / 32)];
+  const StrikeSpec sp = specs[blockIdx.x];
+  const cd* lm = log_mgf + (size_t)sp.slice * P;
+  const double x = log(sp.forward / sp.strike);
+  const double h3 = (phi[1].im - phi[0].im) / 3.0;
+  double acc[NV];
+#pragma unroll
+  for (int i = 0; i < NV; ++i) acc[i] = 0.0;
+  for (int j = threadIdx.x; j < P; j += kFourierThreads) {
+    const double wq = (j & 1) ? 4.0 : ((j == 0 || j == P - 1) ? 1.0 : 2.0);
+    const double dp = h3 * wq;
+    const cd ph = phi[j];
+    const double w = (dp / M_PI) / (ph.im * ph.im + 0.25);
+    const cd e = cexp_(lm[j] - x * ph);
+    const cd term = mk(w) * e;
+    if (term.re == term.re) {
+      acc[0] += term.re;
+      acc[1] += w * (-(ph * e)).re;
+      acc[2] += w * ((ph * ph) * e).re;
+#pragma unroll
+      for (int k = 0; k < NP; ++k) acc[3 + k] += w * (e * dlog_mgf[((size_t)k * M + sp.slice) * P + j]).re;
+    }
+  }
+  block_sum<NV, kFourierThreads>(acc, red);
+  if (threadIdx.x == 0) {
+    const double S = acc[0], Sx = acc[1], Sxx = acc[2], F = sp.forward, K = sp.strike, df = sp.discfactor;
+    const int J = gridDim.x;
+    const bool call = sp.type == B200SV_CALL || sp.type == B200SV_INV_CALL;
+    double delta, gamma, scale;
+    if (is_spot) {             // C = df (F - K S), P = df (K - K S)
+      delta = call ? df * (1.0 - K * Sx / F) : -df * K * Sx / F;
+      gamma = -df * K * (Sxx - Sx) / (F * F);
+      scale = -df * K;
+    } else {                   // C = F df (1 - S), P = df (K - F S)
+      delta = call ? df * (1.0 - S - Sx) : -df * (S + Sx);
+      gamma = -df * (Sx + Sxx) / F;
+      scale = -F * df;
+    }
+    greeks[blockIdx.x] = delta;
+    greeks[J + blockIdx.x] = gamma;
+#pragma unroll
+    for (int k = 0; k < NP; ++k) greeks[(size_t)(2 + k) * J + blockIdx.x] = scale * acc[3 + k];
   }
 }
 
@@ -1627,6 +1975,131 @@ int b200sv_heston_price_chain(const b200sv_heston_params* params, int M, const d
     B200SV_CUDA(cudaMemcpyAsync(prices_out, d_pr.p, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st));
   }
   if (log_mgf_out) B200SV_CUDA(cudaMemcpyAsync(log_mgf_out, d_lm.p, sizeof(cd) * (size_t)M * P, cudaMemcpyDeviceToHost, st));
+  return sync.done();
+}
+
+/* ---- forward-mode sensitivities of the two Fourier chain pricers (DESIGN.md §4.2) ----
+ * The prices come from b200sv_*_price_chain itself (same launches, bit-identical); the tangent kernel then re-runs the primal next to
+ * one tangent per thread and fourier_vanilla_greeks_kernel assembles delta, gamma and the parameter rows. */
+static int greeks_strike_specs(int M, const double* ttms, const double* forwards, const double* discfactors, const int* offsets,
+                               const double* strikes, std::vector<StrikeSpec>& ss, std::vector<double>& dtaus) {
+  const int Jtot = offsets[M] - offsets[0];
+  ss.resize(std::max(Jtot, 1));
+  dtaus.resize(M);
+  double t0 = 0.0;
+  for (int m = 0; m < M; ++m) {
+    dtaus[m] = ttms[m] - t0;
+    t0 = ttms[m];
+    for (int j = offsets[m]; j < offsets[m + 1]; ++j) ss[j - offsets[0]] = StrikeSpec{strikes[j], forwards[m], discfactors[m], 0, m, ttms[m], 0};
+  }
+  return Jtot;
+}
+
+int b200sv_logsv_price_chain_greeks(const b200sv_logsv_params* params, int M, const double* ttms, const double* forwards,
+                                    const double* discfactors, const double* etas, const int* offsets, const double* strikes,
+                                    const int8_t* types, int is_spot_measure, int variable_type, int expansion_order,
+                                    double vol_scaler, int P, double* prices_out, double* greeks_out, double* dlog_mgf_out,
+                                    int* nfev_out) {
+  B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && greeks_out, "null pointer");
+  if (variable_type != B200SV_LOG_RETURN) return fail(-4, "variable_type not implemented: sensitivities cover LOG_RETURN only");
+  if (int rc = b200sv_logsv_price_chain(params, M, ttms, forwards, discfactors, etas, offsets, strikes, types, is_spot_measure, variable_type,
+                                        expansion_order, vol_scaler, P, prices_out, nullptr, nullptr))
+    return rc;                                                             // validates every argument the two routes share
+  if (P <= 0) P = 1000;
+  const bool spot = is_spot_measure != 0;
+  const int N = expansion_order == B200SV_ORDER_FIRST ? 3 : 5, NP = 1 + kLogsvOdeDirs;
+  if (!(vol_scaler > 0.0)) vol_scaler = params->sigma0 * std::sqrt(std::min(*std::min_element(ttms, ttms + M), 0.5 / 12.0));
+  std::vector<double> phi, dtaus;
+  build_phi(vol_scaler, spot, P, phi);
+  std::vector<StrikeSpec> ss;
+  const int Jtot = greeks_strike_specs(M, ttms, forwards, discfactors, offsets, strikes, ss, dtaus);
+  for (int j = 0; j < Jtot; ++j) ss[j].type = types[offsets[0] + j];
+  std::vector<ChainSpec> spec(M);
+  std::vector<LogsvModelTangent> dspec((size_t)M * kLogsvOdeDirs);
+  for (int m = 0; m < M; ++m) {
+    const double eta = etas ? etas[m] : 1.0;
+    spec[m] = ChainSpec{dtaus[m], make_model(*params, eta, spot)};
+    LogsvModelTangent d[kLogsvOdeDirs];
+    make_model_tangents(*params, eta, spot, d);
+    std::copy(d, d + kLogsvOdeDirs, dspec.begin() + (size_t)m * kLogsvOdeDirs);
+  }
+  cudaStream_t st = current_stream();
+  StreamSync sync(st);
+  DevBuf d_phi(st), d_spec(st), d_dspec(st), d_dlm(st), d_lm(st), d_nfev(st), d_ss(st), d_g(st);
+  B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
+  B200SV_CUDA(d_spec.alloc(sizeof(ChainSpec) * M));
+  B200SV_CUDA(d_dspec.alloc(sizeof(LogsvModelTangent) * dspec.size()));
+  B200SV_CUDA(d_dlm.alloc(sizeof(cd) * (size_t)NP * M * P));
+  B200SV_CUDA(d_lm.alloc(sizeof(cd) * (size_t)M * P));
+  B200SV_CUDA(d_nfev.alloc(sizeof(int) * P));
+  B200SV_CUDA(d_ss.alloc(sizeof(StrikeSpec) * ss.size()));
+  B200SV_CUDA(d_g.alloc(sizeof(double) * (size_t)(2 + NP) * ss.size()));
+  B200SV_CUDA(cudaMemcpyAsync(d_phi.p, phi.data(), sizeof(cd) * P, cudaMemcpyHostToDevice, st));
+  B200SV_CUDA(cudaMemcpyAsync(d_spec.p, spec.data(), sizeof(ChainSpec) * M, cudaMemcpyHostToDevice, st));
+  B200SV_CUDA(cudaMemcpyAsync(d_dspec.p, dspec.data(), sizeof(LogsvModelTangent) * dspec.size(), cudaMemcpyHostToDevice, st));
+  B200SV_CUDA(cudaMemcpyAsync(d_ss.p, ss.data(), sizeof(StrikeSpec) * ss.size(), cudaMemcpyHostToDevice, st));
+  const int nb = (P * kLogsvOdeDirs + kTangentTPB - 1) / kTangentTPB;
+  const double y = params->sigma0 - params->theta;
+  if (N == 5)
+    logsv_mgf_tangent_kernel<5><<<nb, kTangentTPB, 0, st>>>(d_phi.as<cd>(), P, M, d_spec.as<ChainSpec>(), d_dspec.as<LogsvModelTangent>(), y,
+                                                            d_dlm.as<cd>(), d_lm.as<cd>(), nullptr, d_nfev.as<int>());
+  else
+    logsv_mgf_tangent_kernel<3><<<nb, kTangentTPB, 0, st>>>(d_phi.as<cd>(), P, M, d_spec.as<ChainSpec>(), d_dspec.as<LogsvModelTangent>(), y,
+                                                            d_dlm.as<cd>(), d_lm.as<cd>(), nullptr, d_nfev.as<int>());
+  if (int rc = check_launch("logsv_mgf_tangent_kernel")) return rc;
+  if (Jtot > 0) {
+    fourier_vanilla_greeks_kernel<1 + kLogsvOdeDirs><<<Jtot, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_dlm.as<cd>(), d_phi.as<cd>(), P, M,
+                                                                                       d_ss.as<StrikeSpec>(), spot ? 1 : 0, d_g.as<double>());
+    if (int rc = check_launch("fourier_vanilla_greeks_kernel")) return rc;
+    B200SV_CUDA(cudaMemcpyAsync(greeks_out, d_g.p, sizeof(double) * (size_t)(2 + NP) * Jtot, cudaMemcpyDeviceToHost, st));
+  }
+  if (dlog_mgf_out) B200SV_CUDA(cudaMemcpyAsync(dlog_mgf_out, d_dlm.p, sizeof(cd) * (size_t)NP * M * P, cudaMemcpyDeviceToHost, st));
+  if (nfev_out) B200SV_CUDA(cudaMemcpyAsync(nfev_out, d_nfev.p, sizeof(int) * P, cudaMemcpyDeviceToHost, st));
+  return sync.done();
+}
+
+int b200sv_heston_price_chain_greeks(const b200sv_heston_params* params, int M, const double* ttms, const double* forwards,
+                                     const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
+                                     int variable_type, double vol_scaler, int P, double* prices_out, double* greeks_out,
+                                     double* dlog_mgf_out) {
+  B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && greeks_out, "null pointer");
+  if (variable_type != B200SV_LOG_RETURN) return fail(-4, "variable_type not implemented: sensitivities cover LOG_RETURN only");
+  if (int rc = b200sv_heston_price_chain(params, M, ttms, forwards, discfactors, offsets, strikes, types, variable_type, vol_scaler, P,
+                                         prices_out, nullptr))
+    return rc;
+  if (P <= 0) P = 1000;
+  const int NP = 1 + kHestonOdeDirs;
+  if (!(vol_scaler > 0.0)) vol_scaler = std::min(0.3, std::sqrt(params->v0 * ttms[0]));
+  std::vector<double> phi, dtaus;
+  build_phi(vol_scaler, true, P, phi);
+  std::vector<StrikeSpec> ss;
+  const int Jtot = greeks_strike_specs(M, ttms, forwards, discfactors, offsets, strikes, ss, dtaus);
+  for (int j = 0; j < Jtot; ++j) ss[j].type = types[offsets[0] + j];
+  cudaStream_t st = current_stream();
+  StreamSync sync(st);
+  DevBuf d_phi(st), d_dt(st), d_dlm(st), d_lm(st), d_ss(st), d_g(st);
+  B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
+  B200SV_CUDA(d_dt.alloc(sizeof(double) * M));
+  B200SV_CUDA(d_dlm.alloc(sizeof(cd) * (size_t)NP * M * P));
+  B200SV_CUDA(d_lm.alloc(sizeof(cd) * (size_t)M * P));
+  B200SV_CUDA(d_ss.alloc(sizeof(StrikeSpec) * ss.size()));
+  B200SV_CUDA(d_g.alloc(sizeof(double) * (size_t)(2 + NP) * ss.size()));
+  B200SV_CUDA(cudaMemcpyAsync(d_phi.p, phi.data(), sizeof(cd) * P, cudaMemcpyHostToDevice, st));
+  B200SV_CUDA(cudaMemcpyAsync(d_dt.p, dtaus.data(), sizeof(double) * M, cudaMemcpyHostToDevice, st));
+  B200SV_CUDA(cudaMemcpyAsync(d_ss.p, ss.data(), sizeof(StrikeSpec) * ss.size(), cudaMemcpyHostToDevice, st));
+  const int tpb = 64;
+  heston_mgf_kernel<<<(P + tpb - 1) / tpb, tpb, 0, st>>>(d_phi.as<cd>(), nullptr, P, M, d_dt.as<double>(), *params, nullptr, nullptr, nullptr,
+                                                        nullptr, d_lm.as<cd>());
+  if (int rc = check_launch("heston_mgf_kernel")) return rc;
+  heston_mgf_tangent_kernel<<<(P * kHestonOdeDirs + tpb - 1) / tpb, tpb, 0, st>>>(d_phi.as<cd>(), P, M, d_dt.as<double>(), *params, d_dlm.as<cd>());
+  if (int rc = check_launch("heston_mgf_tangent_kernel")) return rc;
+  if (Jtot > 0) {
+    fourier_vanilla_greeks_kernel<1 + kHestonOdeDirs><<<Jtot, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_dlm.as<cd>(), d_phi.as<cd>(), P, M,
+                                                                                        d_ss.as<StrikeSpec>(), 1, d_g.as<double>());
+    if (int rc = check_launch("fourier_vanilla_greeks_kernel")) return rc;
+    B200SV_CUDA(cudaMemcpyAsync(greeks_out, d_g.p, sizeof(double) * (size_t)(2 + NP) * Jtot, cudaMemcpyDeviceToHost, st));
+  }
+  if (dlog_mgf_out) B200SV_CUDA(cudaMemcpyAsync(dlog_mgf_out, d_dlm.p, sizeof(cd) * (size_t)NP * M * P, cudaMemcpyDeviceToHost, st));
   return sync.done();
 }
 

@@ -450,6 +450,45 @@ def heston_price_chain(params: C.HestonParamsC, ttms, forwards, discfactors, str
     return (out, lm_out) if return_grids else out
 
 
+def logsv_price_chain_greeks(params: C.LogsvParamsC, ttms, forwards, discfactors, etas, strikes_ttms, optiontypes_ttms,
+                             is_spot_measure: bool = True, expansion_order: int = C.ORDER_SECOND, vol_scaler: Optional[float] = None,
+                             max_phi: Optional[int] = None, return_grids: bool = False):
+    """Fourier prices and forward-mode sensitivities of the chain (b200sv_logsv_price_chain_greeks).  Returns (prices per maturity,
+    greeks [2 + 6, J], offsets) -- greeks rows: delta, gamma, then LOGSV_GREEK_PARAMS -- and with ``return_grids`` also
+    (dlog_mgf [6, M, P], nfev [P])."""
+    _check_fourier_types(optiontypes_ttms, is_spot_measure)
+    max_phi = int(max_phi) if max_phi else 1000
+    M, ttms, forwards, discfactors, offsets, strikes, types = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
+    etas = C.f64(np.ones(M) if etas is None else etas)
+    n = len(LOGSV_GREEK_PARAMS)
+    prices, greeks = np.empty(strikes.shape[0]), np.empty((2 + n, strikes.shape[0]))
+    dlm = np.empty((n, M, max_phi), dtype=np.complex128) if return_grids else None
+    nfev = np.empty(max_phi, dtype=np.int32) if return_grids else None
+    C.call("b200sv_logsv_price_chain_greeks", byref(params), M, C.dptr(ttms), C.dptr(forwards), C.dptr(discfactors), C.dptr(etas),
+           C.iptr(offsets), C.dptr(strikes), C.i8ptr(types), int(bool(is_spot_measure)), C.LOG_RETURN, int(expansion_order),
+           float(vol_scaler) if vol_scaler is not None else -1.0, max_phi, C.dptr(prices), C.dptr(greeks),
+           dlm.ctypes.data_as(C._dp) if return_grids else None, C.iptr(nfev) if return_grids else None)
+    out = (C.split_chain(prices, offsets), greeks, offsets)
+    return out + (dlm, nfev) if return_grids else out
+
+
+def heston_price_chain_greeks(params: C.HestonParamsC, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms,
+                              vol_scaler: Optional[float] = None, max_phi: Optional[int] = None, return_grids: bool = False):
+    """Heston twin of logsv_price_chain_greeks (b200sv_heston_price_chain_greeks): greeks rows = delta, gamma, then HESTON_GREEK_PARAMS;
+    ``return_grids`` adds dlog_mgf [5, M, P]."""
+    _check_fourier_types(optiontypes_ttms, True)
+    max_phi = int(max_phi) if max_phi else 1000
+    M, ttms, forwards, discfactors, offsets, strikes, types = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
+    n = len(HESTON_GREEK_PARAMS)
+    prices, greeks = np.empty(strikes.shape[0]), np.empty((2 + n, strikes.shape[0]))
+    dlm = np.empty((n, M, max_phi), dtype=np.complex128) if return_grids else None
+    C.call("b200sv_heston_price_chain_greeks", byref(params), M, C.dptr(ttms), C.dptr(forwards), C.dptr(discfactors), C.iptr(offsets),
+           C.dptr(strikes), C.i8ptr(types), C.LOG_RETURN, float(vol_scaler) if vol_scaler is not None else -1.0, max_phi, C.dptr(prices),
+           C.dptr(greeks), dlm.ctypes.data_as(C._dp) if return_grids else None)
+    out = (C.split_chain(prices, offsets), greeks, offsets)
+    return out + (dlm,) if return_grids else out
+
+
 def logsv_price_chain_batch(params_list: Sequence[C.LogsvParamsC], ttms, forwards, discfactors, etas, strikes_ttms, optiontypes_ttms,
                             is_spot_measure: bool = True, expansion_order: int = C.ORDER_SECOND, vol_scaler: Optional[float] = None,
                             max_phi: int = 1000, with_ivols: bool = True):

@@ -57,6 +57,17 @@ class HestonPricer(ModelPricer):
                                    strikes_ttms=option_chain.strikes_ttms, optiontypes_ttms=option_chain.optiontypes_ttms,
                                    vol_scaler=kwargs.get("vol_scaler"))
 
+    def price_chain_greeks(self, option_chain: OptionChain, params: HestonParams, **kwargs):
+        """Fourier prices (bit-identical to ``price_chain`` with the same ``vol_scaler``) plus forward-mode sensitivities in one call ->
+        ``FourierChainGreeks``: delta and gamma in the slice forward and d price / d (v0, theta, kappa, rho, volvol), exact derivatives of
+        the closed form on a fixed transform grid.  Q_VAR raises NotImplementedError."""
+        from .fourier_greeks import check_fourier_greeks_kwargs, to_fourier_chain_greeks
+        check_fourier_greeks_kwargs(kwargs)
+        prices, greeks, offsets = engine.heston_price_chain_greeks(
+            _params_c(params.v0, params.theta, params.kappa, params.rho, params.volvol), option_chain.ttms, option_chain.forwards,
+            option_chain.discfactors, option_chain.strikes_ttms, option_chain.optiontypes_ttms, vol_scaler=kwargs.get("vol_scaler"))
+        return to_fourier_chain_greeks(prices, greeks, offsets, engine.HESTON_GREEK_PARAMS)
+
     @timer
     def calibrate_model_params_to_chain(self, option_chain: OptionChain, params0: HestonParams = None, is_vega_weighted: bool = True,
                                         is_unit_ttm_vega: bool = False, **kwargs) -> HestonParams:

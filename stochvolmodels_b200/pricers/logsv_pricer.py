@@ -210,6 +210,21 @@ class LogSVPricer(ModelPricer):
                                   discfactors=option_chain.discfactors, strikes_ttms=option_chain.strikes_ttms,
                                   optiontypes_ttms=option_chain.optiontypes_ttms, is_spot_measure=is_spot_measure, **kwargs)
 
+    def price_chain_greeks(self, option_chain: OptionChain, params: LogSvParams, is_spot_measure: bool = True, **kwargs):
+        """Fourier prices (bit-identical to ``price_chain`` with the same arguments) plus forward-mode sensitivities in one call ->
+        ``FourierChainGreeks``: delta and gamma in the slice forward and d price / d (sigma0, theta, kappa1, kappa2, beta, volvol).  Takes
+        ``expansion_order``, ``vol_scaler`` and ``max_phi`` like ``price_chain``; ``kappa2`` is the value after ``__post_init__`` and is held
+        fixed when kappa1 or theta moves; the vol backbone, the discount factors and the transform grid are not differentiated.  The
+        semi-analytic and BDF branches, Q_VAR and the rough-vol route raise NotImplementedError."""
+        from .fourier_greeks import check_fourier_greeks_kwargs, to_fourier_chain_greeks
+        check_fourier_greeks_kwargs(kwargs)
+        prices, greeks, offsets = engine.logsv_price_chain_greeks(
+            _params_c(params), option_chain.ttms, option_chain.forwards, option_chain.discfactors,
+            params.get_vol_backbone_etas(ttms=option_chain.ttms), option_chain.strikes_ttms, option_chain.optiontypes_ttms,
+            is_spot_measure=is_spot_measure, expansion_order=_order_code(kwargs.get("expansion_order", ExpansionOrder.SECOND)),
+            vol_scaler=kwargs.get("vol_scaler"), max_phi=kwargs.get("max_phi"))
+        return to_fourier_chain_greeks(prices, greeks, offsets, engine.LOGSV_GREEK_PARAMS)
+
     def set_vol_scaler(self, option_chain: OptionChain) -> float:
         """transform-grid scaler from the first slice's ATM vol (reference :436-439)."""
         return set_vol_scaler(sigma0=option_chain.get_chain_atm_vols()[0], ttm=option_chain.ttms[0])
