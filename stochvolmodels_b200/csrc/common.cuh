@@ -53,6 +53,17 @@ struct DevBuf {   // RAII for stream-ordered temporaries
   DevBuf(const DevBuf&) = delete;
   DevBuf& operator=(const DevBuf&) = delete;
   cudaError_t alloc(size_t n) { return cudaMallocAsync(&p, n ? n : 1, st); }
+  // allocate n elements of T and queue the copy of host[0, n) into them
+  template <typename T>
+  cudaError_t upload(const T* host, size_t n) {
+    const cudaError_t e = alloc(sizeof(T) * n);
+    return e != cudaSuccess ? e : cudaMemcpyAsync(p, host, sizeof(T) * n, cudaMemcpyHostToDevice, st);
+  }
+  // queue the copy of the first n elements of T back into host; nothing to do for an optional output left null
+  template <typename T>
+  cudaError_t download(T* host, size_t n) const {
+    return host ? cudaMemcpyAsync(host, p, sizeof(T) * n, cudaMemcpyDeviceToHost, st) : cudaSuccess;
+  }
   ~DevBuf() {
     if (p) cudaFreeAsync(p, st);
   }

@@ -1227,32 +1227,6 @@ static bool use_lane_kernel(long long points) {
   return points <= 8192;
 }
 
-template <int N>
-static void launch_logsv_mgf(int tpb, int nb, cudaStream_t st, const cd* phi, const cd* psi, int P, int M, const ChainSpec* spec,
-                             const cd* a_in, cd* a_out, cd* lm, double y, int* status, int B = 1, const double* yb = nullptr,
-                             int phi_stride = 0) {
-  if (use_lane_kernel((long long)P * B)) {
-    constexpr int PPW = 32 / (N == 5 ? 8 : 4);
-    const int per_block = PPW * kLaneWarpsPerBlock;
-    logsv_mgf_lanes_kernel<N><<<dim3((P + per_block - 1) / per_block, B), 32 * kLaneWarpsPerBlock, 0, st>>>(phi, psi, P, M, spec, a_in, a_out, lm, y,
-                                                                                                      status, yb, phi_stride);
-    return;
-  }
-  static const bool set_major = [] {
-    const char* e = getenv("B200SV_MGF_SET_MAJOR");      // A/B timing switch (tools/bench_calibration.py); default on
-    return !e || atoi(e) != 0;
-  }();
-  const int smB = (B > 1 && set_major) ? B : 0;
-  const dim3 grid = smB ? dim3((unsigned)(((long long)B * P + tpb - 1) / tpb), 1) : dim3(nb, B);
-  switch (tpb) {
-    case 4: logsv_mgf_kernel<N, 4><<<grid, 4, 0, st>>>(phi, psi, P, M, spec, a_in, a_out, lm, y, status, nullptr, yb, phi_stride, smB); break;
-    case 8: logsv_mgf_kernel<N, 8><<<grid, 8, 0, st>>>(phi, psi, P, M, spec, a_in, a_out, lm, y, status, nullptr, yb, phi_stride, smB); break;
-    case 16: logsv_mgf_kernel<N, 16><<<grid, 16, 0, st>>>(phi, psi, P, M, spec, a_in, a_out, lm, y, status, nullptr, yb, phi_stride, smB); break;
-    case 32: logsv_mgf_kernel<N, 32><<<grid, 32, 0, st>>>(phi, psi, P, M, spec, a_in, a_out, lm, y, status, nullptr, yb, phi_stride, smB); break;
-    default: logsv_mgf_kernel<N, 64><<<grid, 64, 0, st>>>(phi, psi, P, M, spec, a_in, a_out, lm, y, status, nullptr, yb, phi_stride, smB); break;
-  }
-}
-
 // dense M / L / H of affine_expansion.py:139-184 from the row tables (parity entry b200sv_logsv_ode_terms)
 template <int N>
 __global__ void logsv_ode_terms_kernel(const cd* __restrict__ phi, const cd* __restrict__ psi, int P, LogsvModel m, cd* __restrict__ M_out,
@@ -1814,10 +1788,308 @@ static int check_fourier_types(const int8_t* types, int n, bool spot) {
   return 0;
 }
 
+// the gamma slice pricer prices 'C' / 'P' under the spot measure only (utils/mgf_pricer.py:310-318)
+static int check_gamma_types(const int8_t* types, int n, bool spot) {
+  if (!spot) return fail(-5, "not implemented");
+  for (int j = 0; j < n; ++j)
+    if (types[j] != B200SV_CALL && types[j] != B200SV_PUT) return fail(-5, "not implemented");
+  return 0;
+}
+
 static bool all_half_re(const double* phi, int P) {
   for (int i = 0; i < P; ++i)
     if (std::fabs(phi[2 * i]) != 0.5) return false;
   return true;
+}
+
+// caller arrays of complex numbers are interleaved doubles
+static const cd* cplx(const double* p) { return reinterpret_cast<const cd*>(p); }
+static cd* cplx(double* p) { return reinterpret_cast<cd*>(p); }
+
+// ---- kernel maps: one instantiation per expansion order N (3 or 5) and block size (mgf_block_threads: 4 .. 64) ----
+using LogsvMgfKernel = decltype(&logsv_mgf_kernel<5, 64>);
+static LogsvMgfKernel logsv_mgf_kernel_for(int N, int tpb) {
+  switch (tpb) {
+    case 4: return N == 5 ? logsv_mgf_kernel<5, 4> : logsv_mgf_kernel<3, 4>;
+    case 8: return N == 5 ? logsv_mgf_kernel<5, 8> : logsv_mgf_kernel<3, 8>;
+    case 16: return N == 5 ? logsv_mgf_kernel<5, 16> : logsv_mgf_kernel<3, 16>;
+    case 32: return N == 5 ? logsv_mgf_kernel<5, 32> : logsv_mgf_kernel<3, 32>;
+    default: return N == 5 ? logsv_mgf_kernel<5, 64> : logsv_mgf_kernel<3, 64>;
+  }
+}
+
+using HawkesMgfKernel = decltype(&hawkes_mgf_kernel<64>);
+static HawkesMgfKernel hawkes_mgf_kernel_for(int tpb) {
+  switch (tpb) {
+    case 4: return hawkes_mgf_kernel<4>;
+    case 8: return hawkes_mgf_kernel<8>;
+    case 16: return hawkes_mgf_kernel<16>;
+    case 32: return hawkes_mgf_kernel<32>;
+    default: return hawkes_mgf_kernel<64>;
+  }
+}
+
+// logsv_mgf_kernel (or its lane-parallel form) over B parameter sets; block size from the B * P points in flight
+static void launch_logsv_mgf(int N, cudaStream_t st, const cd* phi, const cd* psi, int P, int M, const ChainSpec* spec, const cd* a_in,
+                             cd* a_out, cd* lm, double y, int B = 1, const double* yb = nullptr, int phi_stride = 0) {
+  if (use_lane_kernel((long long)P * B)) {
+    const int per_block = 32 / (N == 5 ? 8 : 4) * kLaneWarpsPerBlock;      // grid points per warp x warps
+    const auto lanes = N == 5 ? logsv_mgf_lanes_kernel<5> : logsv_mgf_lanes_kernel<3>;
+    lanes<<<dim3((P + per_block - 1) / per_block, B), 32 * kLaneWarpsPerBlock, 0, st>>>(phi, psi, P, M, spec, a_in, a_out, lm, y, nullptr, yb,
+                                                                                        phi_stride);
+    return;
+  }
+  static const bool set_major = [] {
+    const char* e = getenv("B200SV_MGF_SET_MAJOR");      // A/B timing switch (tools/bench_calibration.py); default on
+    return !e || atoi(e) != 0;
+  }();
+  const int tpb = mgf_block_threads((int)std::min<long long>((long long)B * P, 1 << 30));
+  const int smB = (B > 1 && set_major) ? B : 0;
+  const dim3 grid = smB ? dim3((unsigned)(((long long)B * P + tpb - 1) / tpb), 1) : dim3((P + tpb - 1) / tpb, B);
+  const LogsvMgfKernel k = logsv_mgf_kernel_for(N, tpb);
+  k<<<grid, tpb, 0, st>>>(phi, psi, P, M, spec, a_in, a_out, lm, y, nullptr, nullptr, yb, phi_stride, smB);
+}
+
+static void launch_hawkes_mgf(cudaStream_t st, const cd* phi, const cd* psi, int P, int M, const double* dtaus, const HawkesMgfConsts& c,
+                              const cd* a_in, cd* a_out, cd* lm, int restart) {
+  const int tpb = mgf_block_threads(P);
+  const HawkesMgfKernel k = hawkes_mgf_kernel_for(tpb);
+  k<<<(P + tpb - 1) / tpb, tpb, 0, st>>>(phi, psi, P, M, dtaus, c, a_in, a_out, lm, restart, nullptr);
+}
+
+// ---- chain preparation ----
+// Default transform-grid scale when the caller passes vol_scaler <= 0; t0 is the first (shortest) maturity.
+static double default_vol_scaler(const b200sv_logsv_params& p, double t0) {      // logsv_pricer.py:664-666
+  return p.sigma0 * std::sqrt(std::min(t0, 0.5 / 12.0));
+}
+static double default_vol_scaler(const b200sv_heston_params& p, double t0) {     // heston_pricer.py:234-235
+  return std::min(0.3, std::sqrt(p.v0 * t0));
+}
+static double default_vol_scaler(const b200sv_hawkes_params& p, double t0) {     // hawkes_jd_pricer.py:360-362
+  return std::min(std::max(p.sigma, 0.2), 0.5) * std::sqrt(std::min(t0, 1.0 / 12.0));
+}
+
+enum class ChainTypes { kFourier, kQvar, kGamma };   // which payoffs the route prices: check_fourier_types / _qvar_ / _gamma_
+
+// One option chain of a Fourier chain pricer, validated once, with everything its launches read: the maturity increments, the transform
+// grid(s) and one strike row per (parameter set, strike).  init() checks the sizes; build() the option types, maturities and strikes.
+struct FourierChain {
+  bool batch = false, spot = true, qvar = false, per_set_grid = false;
+  int B = 1, M = 0, P = 0, Jtot = 0;
+  std::vector<double> dtaus, phi, psi;    // phi [G][P] complex (G = B with a per-set grid, else 1); psi [P] under Q_VAR only
+  std::vector<StrikeSpec> ss;             // [B][Jtot]: slice b * M + m, grid b (per-set grid) or 0
+  std::vector<SumSpec> qs;                // [Jtot], Q_VAR only
+
+  // batch: the B sets of b200sv_*_price_chain_batch, which also need at least one strike
+  int init(bool is_batch, int nsets, int nmat, int npoints, const int* offsets) {
+    batch = is_batch;
+    B = nsets;
+    M = nmat;
+    P = npoints;
+    if (batch)
+      B200SV_REQUIRE(B >= 1 && B <= 65535 && M >= 1 && P >= 3, "1 <= B <= 65535, M >= 1, P >= 3");
+    else
+      B200SV_REQUIRE(M >= 1 && P >= 3, "M >= 1, P >= 3");
+    Jtot = offsets[M] - offsets[0];
+    if (batch) B200SV_REQUIRE(Jtot >= 1, "the chain has no strikes");
+    return 0;
+  }
+
+  template <class Params>
+  int build(const Params* params, const double* ttms, const double* forwards, const double* discfactors, const int* offsets,
+            const double* strikes, const int8_t* types, bool is_spot, ChainTypes payoffs, double vol_scaler) {
+    spot = is_spot;
+    qvar = payoffs == ChainTypes::kQvar;
+    B200SV_REQUIRE(Jtot == 0 || types, "null pointer");
+    const int8_t* t = types + offsets[0];
+    if (int rc = qvar ? check_qvar_types(t, Jtot)
+                      : payoffs == ChainTypes::kGamma ? check_gamma_types(t, Jtot, spot) : check_fourier_types(t, Jtot, spot))
+      return rc;
+    dtaus.resize(M);
+    double t0 = 0.0;
+    for (int m = 0; m < M; ++m) {
+      B200SV_REQUIRE(ttms[m] > t0, "ttms must be positive and strictly increasing");
+      dtaus[m] = ttms[m] - t0;
+      t0 = ttms[m];
+    }
+    B200SV_REQUIRE(Jtot == 0 || strikes, "null pointer");
+    per_set_grid = !(vol_scaler > 0.0);
+    ss.resize(std::max((size_t)B * Jtot, (size_t)1));
+    if (qvar) qs.resize(std::max(Jtot, 1));
+    for (int b = 0; b < B; ++b)
+      for (int m = 0; m < M; ++m)
+        for (int j = offsets[m]; j < offsets[m + 1]; ++j) {
+          B200SV_REQUIRE(strikes[j] > 0.0, "strikes must be positive");
+          ss[(size_t)b * Jtot + (j - offsets[0])] = StrikeSpec{strikes[j], forwards[m], discfactors[m], (int)types[j], b * M + m, ttms[m],
+                                                               per_set_grid ? b : 0};
+          if (qvar) qs[j - offsets[0]] = SumSpec{strikes[j] * ttms[m], discfactors[m], ttms[m], (int)types[j], m};
+        }
+    if (qvar) {                                     // utils/mgf_pricer.py:79-85: psi grid, phi = 0 (MMA) | 1 (inverse)
+      build_grid(-0.5, 4000.0, P, psi);
+      phi.assign(2 * (size_t)P, 0.0);
+      if (!spot)
+        for (int i = 0; i < P; ++i) phi[2 * i] = 1.0;
+      return 0;
+    }
+    std::vector<double> one;
+    for (int g = 0; g < (per_set_grid ? B : 1); ++g) {
+      build_phi(per_set_grid ? default_vol_scaler(params[g], ttms[0]) : vol_scaler, spot, P, one);
+      phi.insert(phi.end(), one.begin(), one.end());
+    }
+    return 0;
+  }
+};
+
+// The stream, memory-pool setting and closing synchronisation of one host-level call: `return call.sync.done();`.
+struct HostCall {
+  cudaStream_t st = current_stream();
+  StreamSync sync{st};
+  HostCall() { ensure_pool_threshold(); }
+};
+
+// A prepared chain on the device: upload() queues the grid(s), psi and strike rows; the model routes add their per-maturity inputs
+// (spec or dt), write the [B][M][P] log-MGF into lm (and A into a), and sums() prices every strike and copies the prices back.
+struct ChainDev : HostCall {
+  DevBuf phi{st}, psi{st}, rows{st}, spec{st}, dt{st}, a{st}, lm{st}, pr{st}, iv{st};
+
+  int upload(const FourierChain& c) {
+    B200SV_CUDA(phi.upload(c.phi.data(), c.phi.size()));
+    if (c.qvar) {
+      B200SV_CUDA(psi.upload(c.psi.data(), c.psi.size()));
+      B200SV_CUDA(rows.upload(c.qs.data(), c.qs.size()));
+    } else {
+      B200SV_CUDA(rows.upload(c.ss.data(), c.ss.size()));
+    }
+    B200SV_CUDA(lm.alloc(sizeof(cd) * (size_t)c.B * c.M * c.P));
+    B200SV_CUDA(pr.alloc(sizeof(double) * c.ss.size()));
+    return 0;
+  }
+
+  // vanilla (or Q_VAR, or with a risk-premia gamma the gamma) Fourier sum, one CTA per strike; no launch on an empty chain
+  int sums(const FourierChain& c, double* prices_out, double* ivols_out, double gamma = NAN) {
+    if (c.Jtot == 0) return 0;
+    const size_t nq = (size_t)c.B * c.Jtot;
+    if (ivols_out) B200SV_CUDA(iv.alloc(sizeof(double) * nq));
+    if (c.qvar)
+      fourier_sum_kernel<<<(unsigned)nq, kFourierThreads, 0, st>>>(lm.as<cd>(), psi.as<cd>(), c.P, rows.as<SumSpec>(), kModeQvar, 0,
+                                                                    pr.as<double>());
+    else if (gamma == gamma)
+      fourier_gamma_kernel<<<(unsigned)nq, kFourierThreads, 0, st>>>(lm.as<cd>(), phi.as<cd>(), c.P, rows.as<StrikeSpec>(), gamma,
+                                                                      pr.as<double>());
+    else
+      fourier_vanilla_kernel<<<(unsigned)nq, kFourierThreads, 0, st>>>(lm.as<cd>(), phi.as<cd>(), c.P, rows.as<StrikeSpec>(), c.spot ? 1 : 0,
+                                                                        1, pr.as<double>(), iv.as<double>());
+    if (int rc = check_launch("fourier sum kernel")) return rc;
+    B200SV_CUDA(pr.download(prices_out, nq));
+    B200SV_CUDA(iv.download(ivols_out, nq));
+    return 0;
+  }
+};
+
+// Validation of b200sv_logsv_price_chain and its greeks, in this order: variable type, sizes, expansion order, the chain.
+static int prepare_logsv_chain(FourierChain& c, const b200sv_logsv_params* params, int M, const double* ttms, const double* forwards,
+                               const double* discfactors, const int* offsets, const double* strikes, const int8_t* types, int is_spot_measure,
+                               int variable_type, int expansion_order, double vol_scaler, int P) {
+  if (variable_type != B200SV_LOG_RETURN && variable_type != B200SV_Q_VAR) return fail(-4, "variable_type not implemented");   // logsv_pricer.py:733-734
+  const bool qvar = variable_type == B200SV_Q_VAR;
+  if (int rc = c.init(false, 1, M, P > 0 ? P : qvar ? 40000 : 1000, offsets)) return rc;   // utils/mgf_pricer.py:13, :44
+  if (expansion_order != B200SV_ORDER_FIRST && expansion_order != B200SV_ORDER_SECOND)
+    return fail(-4, "expansion_order not implemented");                    // affine_expansion.py:680-681
+  return c.build(params, ttms, forwards, discfactors, offsets, strikes, types, is_spot_measure != 0,
+                 qvar ? ChainTypes::kQvar : ChainTypes::kFourier, vol_scaler);
+}
+
+static int prepare_heston_chain(FourierChain& c, const b200sv_heston_params* params, int M, const double* ttms, const double* forwards,
+                                const double* discfactors, const int* offsets, const double* strikes, const int8_t* types, int variable_type,
+                                double vol_scaler, int P) {
+  if (variable_type != B200SV_LOG_RETURN && variable_type != B200SV_Q_VAR) return fail(-4, "variable_type not implemented");   // heston_pricer.py:276-277
+  const bool qvar = variable_type == B200SV_Q_VAR;
+  if (int rc = c.init(false, 1, M, P > 0 ? P : qvar ? 40000 : 1000, offsets)) return rc;
+  return c.build(params, ttms, forwards, discfactors, offsets, strikes, types, true, qvar ? ChainTypes::kQvar : ChainTypes::kFourier,
+                 vol_scaler);
+}
+
+// The LogSV pricing launches of a prepared chain (single, greeks and batch routes): logsv_mgf_kernel over the B sets, then the sums.
+static int queue_logsv_prices(ChainDev& d, const FourierChain& c, const b200sv_logsv_params* params, const double* etas, int N,
+                              double* prices_out, double* ivols_out) {
+  std::vector<ChainSpec> spec((size_t)c.B * c.M);
+  std::vector<double> yb(c.B);
+  for (int b = 0; b < c.B; ++b) {
+    yb[b] = params[b].sigma0 - params[b].theta;
+    for (int m = 0; m < c.M; ++m)
+      spec[(size_t)b * c.M + m] = ChainSpec{c.dtaus[m], make_model(params[b], etas ? etas[(size_t)b * c.M + m] : 1.0, c.spot)};
+  }
+  DevBuf d_y(d.st);
+  if (int rc = d.upload(c)) return rc;
+  B200SV_CUDA(d.spec.upload(spec.data(), spec.size()));
+  if (c.batch) B200SV_CUDA(d_y.upload(yb.data(), yb.size()));
+  B200SV_CUDA(d.a.alloc(sizeof(cd) * (size_t)c.B * c.M * c.P * N));
+  launch_logsv_mgf(N, d.st, d.phi.as<cd>(), d.psi.as<cd>(), c.P, c.M, d.spec.as<ChainSpec>(), nullptr, d.a.as<cd>(), d.lm.as<cd>(),
+                   c.batch ? 0.0 : yb[0], c.B, d_y.as<double>(), c.batch && c.per_set_grid ? c.P : 0);
+  if (int rc = check_launch("logsv_mgf_kernel")) return rc;
+  return d.sums(c, prices_out, ivols_out);
+}
+
+// The Heston pricing launches of a prepared chain: heston_mgf_kernel (blockIdx.y = set), then the sums.
+static int queue_heston_prices(ChainDev& d, const FourierChain& c, const b200sv_heston_params* params, double* prices_out, double* ivols_out) {
+  DevBuf d_hp(d.st);
+  if (int rc = d.upload(c)) return rc;
+  B200SV_CUDA(d.dt.upload(c.dtaus.data(), c.dtaus.size()));
+  if (c.batch) B200SV_CUDA(d_hp.upload(params, c.B));
+  const int tpb = c.batch ? 64 : mgf_block_threads(c.P);
+  heston_mgf_kernel<<<dim3((c.P + tpb - 1) / tpb, c.B), tpb, 0, d.st>>>(d.phi.as<cd>(), d.psi.as<cd>(), c.P, c.M, d.dt.as<double>(), params[0],
+                                                                        nullptr, nullptr, nullptr, nullptr, d.lm.as<cd>(),
+                                                                        d_hp.as<b200sv_heston_params>(), c.per_set_grid && c.batch ? c.P : 0);
+  if (int rc = check_launch("heston_mgf_kernel")) return rc;
+  return d.sums(c, prices_out, ivols_out);
+}
+
+// Plumbing of the single-grid entry points: phi [P], psi [P] (when given) and a_in [P][n] (when given) go up, `launch` queues its
+// kernel(s) on them and returns check_launch's code, then a_out [P][n] and log_mgf_out [P] (when given) come back.
+template <class Launch>
+static int run_grid(const double* phi, const double* psi, int P, const double* a_in, int n, double* a_out, double* log_mgf_out, Launch launch) {
+  HostCall call;
+  const cudaStream_t st = call.st;
+  DevBuf d_phi(st), d_psi(st), d_a0(st), d_a1(st), d_lm(st);
+  const size_t na = (size_t)P * n;
+  B200SV_CUDA(d_phi.upload(cplx(phi), P));
+  if (psi) B200SV_CUDA(d_psi.upload(cplx(psi), P));
+  if (a_in) B200SV_CUDA(d_a0.upload(cplx(a_in), na));
+  if (a_out) B200SV_CUDA(d_a1.alloc(sizeof(cd) * na));
+  if (log_mgf_out) B200SV_CUDA(d_lm.alloc(sizeof(cd) * P));
+  if (int rc = launch(st, d_phi.as<cd>(), d_psi.as<cd>(), d_a0.as<cd>(), d_a1.as<cd>(), d_lm.as<cd>())) return rc;
+  B200SV_CUDA(d_a1.download(cplx(a_out), na));
+  B200SV_CUDA(d_lm.download(cplx(log_mgf_out), P));
+  return call.sync.done();
+}
+
+// One CTA per strike over a caller-supplied log-MGF and grid (b200sv_fourier_*): log_mgf, grid and the rows go up, `launch` queues the sum
+// kernel and returns check_launch's code, the J results come back.
+template <class Row, class Launch>
+static int run_sums(const double* log_mgf, const double* grid, int P, const std::vector<Row>& rows, double* out, Launch launch) {
+  HostCall call;
+  const cudaStream_t st = call.st;
+  DevBuf d_g(st), d_lm(st), d_rows(st), d_out(st);
+  B200SV_CUDA(d_g.upload(cplx(grid), P));
+  B200SV_CUDA(d_lm.upload(cplx(log_mgf), P));
+  B200SV_CUDA(d_rows.upload(rows.data(), rows.size()));
+  B200SV_CUDA(d_out.alloc(sizeof(double) * rows.size()));
+  if (int rc = launch(st, (unsigned)rows.size(), d_lm.as<cd>(), d_g.as<cd>(), d_rows.as<Row>(), d_out.as<double>())) return rc;
+  B200SV_CUDA(d_out.download(out, rows.size()));
+  return call.sync.done();
+}
+
+static int fourier_sum_host(const double* log_mgf, const double* grid, int P, const std::vector<SumSpec>& specs, int mode, int all_calls,
+                            double* out) {
+  return run_sums(log_mgf, grid, P, specs, out, [&](cudaStream_t st, unsigned J, const cd* lm, const cd* g, const SumSpec* ss, double* pr) {
+    fourier_sum_kernel<<<J, kFourierThreads, 0, st>>>(lm, g, P, ss, mode, all_calls, pr);
+    return check_launch("fourier_sum_kernel");
+  });
+}
+
+static int check_expansion_order(int expansion_order) {
+  if (expansion_order != B200SV_ORDER_FIRST && expansion_order != B200SV_ORDER_SECOND) return fail(-4, "expansion_order not implemented");
+  return 0;
 }
 
 }  // namespace b200sv
@@ -1831,170 +2103,33 @@ int b200sv_logsv_price_chain(const b200sv_logsv_params* params, int M, const dou
                              const int8_t* types, int is_spot_measure, int variable_type, int expansion_order,
                              double vol_scaler, int P, double* prices_out, double* a_out, double* log_mgf_out) {
   B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out, "null pointer");
-  if (variable_type != B200SV_LOG_RETURN && variable_type != B200SV_Q_VAR) return fail(-4, "variable_type not implemented");   // logsv_pricer.py:733-734
-  const bool qvar = variable_type == B200SV_Q_VAR;
-  if (P <= 0) P = qvar ? 40000 : 1000;                                     // utils/mgf_pricer.py:13, :44
-  B200SV_REQUIRE(M >= 1 && P >= 3, "M >= 1, P >= 3");
-  if (expansion_order != B200SV_ORDER_FIRST && expansion_order != B200SV_ORDER_SECOND)
-    return fail(-4, "expansion_order not implemented");                    // affine_expansion.py:680-681
-  const bool spot = is_spot_measure != 0;
-  const int Jtot = offsets[M] - offsets[0];
-  if (int rc = qvar ? check_qvar_types(types + offsets[0], Jtot) : check_fourier_types(types + offsets[0], Jtot, spot)) return rc;
-  double t0 = 0.0, tmin = ttms[0];
-  for (int m = 0; m < M; ++m) {
-    B200SV_REQUIRE(ttms[m] > t0, "ttms must be positive and strictly increasing");
-    t0 = ttms[m];
-    tmin = std::min(tmin, ttms[m]);
-  }
-  if (!(vol_scaler > 0.0)) vol_scaler = params->sigma0 * std::sqrt(std::min(tmin, 0.5 / 12.0));   // logsv_pricer.py:664-666
+  FourierChain c;
+  if (int rc = prepare_logsv_chain(c, params, M, ttms, forwards, discfactors, offsets, strikes, types, is_spot_measure, variable_type,
+                                   expansion_order, vol_scaler, P))
+    return rc;
   const int N = expansion_order == B200SV_ORDER_FIRST ? 3 : 5;
-  std::vector<double> phi, psi;
-  if (!qvar) {
-    build_phi(vol_scaler, spot, P, phi);
-  } else {                                                                 // utils/mgf_pricer.py:79-85: psi grid, phi = 0 (MMA) | 1 (inverse)
-    build_grid(-0.5, 4000.0, P, psi);
-    phi.assign(2 * (size_t)P, 0.0);
-    if (!spot)
-      for (int i = 0; i < P; ++i) phi[2 * i] = 1.0;
-  }
-  std::vector<ChainSpec> spec(M);
-  t0 = 0.0;
-  for (int m = 0; m < M; ++m) {
-    spec[m].dtau = ttms[m] - t0;
-    spec[m].model = make_model(*params, etas ? etas[m] : 1.0, spot);
-    t0 = ttms[m];
-  }
-  std::vector<StrikeSpec> ss(std::max(Jtot, 1));
-  std::vector<SumSpec> qs(std::max(Jtot, 1));
-  for (int m = 0; m < M; ++m)
-    for (int j = offsets[m]; j < offsets[m + 1]; ++j) {
-      B200SV_REQUIRE(strikes[j] > 0.0, "strikes must be positive");
-      ss[j - offsets[0]] = StrikeSpec{strikes[j], forwards[m], discfactors[m], (int)types[j], m, ttms[m], 0};
-      qs[j - offsets[0]] = SumSpec{strikes[j] * ttms[m], discfactors[m], ttms[m], (int)types[j], m};
-    }
-  cudaStream_t st = current_stream();
-  ensure_pool_threshold();
-  StreamSync sync(st);
-  DevBuf d_phi(st), d_psi(st), d_spec(st), d_a(st), d_lm(st), d_ss(st), d_pr(st), d_stat(st);
-  B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_psi.alloc(sizeof(cd) * P));
-  if (qvar) B200SV_CUDA(cudaMemcpyAsync(d_psi.p, psi.data(), sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(d_spec.alloc(sizeof(ChainSpec) * M));
-  B200SV_CUDA(d_a.alloc(sizeof(cd) * (size_t)M * P * N));
-  B200SV_CUDA(d_lm.alloc(sizeof(cd) * (size_t)M * P));
-  B200SV_CUDA(d_ss.alloc(std::max(sizeof(StrikeSpec), sizeof(SumSpec)) * ss.size()));
-  B200SV_CUDA(d_pr.alloc(sizeof(double) * ss.size()));
-  B200SV_CUDA(d_stat.alloc(sizeof(int) * P));
-  B200SV_CUDA(cudaMemcpyAsync(d_phi.p, phi.data(), sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_spec.p, spec.data(), sizeof(ChainSpec) * M, cudaMemcpyHostToDevice, st));
-  if (qvar)
-    B200SV_CUDA(cudaMemcpyAsync(d_ss.p, qs.data(), sizeof(SumSpec) * qs.size(), cudaMemcpyHostToDevice, st));
-  else
-    B200SV_CUDA(cudaMemcpyAsync(d_ss.p, ss.data(), sizeof(StrikeSpec) * ss.size(), cudaMemcpyHostToDevice, st));
-  const int tpb = mgf_block_threads(P), nb = (P + tpb - 1) / tpb;
-  const double y = params->sigma0 - params->theta;
-  const cd* dpsi = qvar ? d_psi.as<cd>() : nullptr;
-  if (N == 5)
-    launch_logsv_mgf<5>(tpb, nb, st, d_phi.as<cd>(), dpsi, P, M, d_spec.as<ChainSpec>(), nullptr, d_a.as<cd>(), d_lm.as<cd>(), y, d_stat.as<int>());
-  else
-    launch_logsv_mgf<3>(tpb, nb, st, d_phi.as<cd>(), dpsi, P, M, d_spec.as<ChainSpec>(), nullptr, d_a.as<cd>(), d_lm.as<cd>(), y, d_stat.as<int>());
-  if (int rc = check_launch("logsv_mgf_kernel")) return rc;
-  if (Jtot > 0) {
-    if (qvar)
-      fourier_sum_kernel<<<Jtot, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_psi.as<cd>(), P, d_ss.as<SumSpec>(), kModeQvar, 0, d_pr.as<double>());
-    else
-      fourier_vanilla_kernel<<<Jtot, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_phi.as<cd>(), P, d_ss.as<StrikeSpec>(), spot ? 1 : 0, 1, d_pr.as<double>());
-    if (int rc = check_launch("fourier_vanilla_kernel")) return rc;
-    B200SV_CUDA(cudaMemcpyAsync(prices_out, d_pr.p, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st));
-  }
-  if (a_out) B200SV_CUDA(cudaMemcpyAsync(a_out, d_a.p, sizeof(cd) * (size_t)M * P * N, cudaMemcpyDeviceToHost, st));
-  if (log_mgf_out) B200SV_CUDA(cudaMemcpyAsync(log_mgf_out, d_lm.p, sizeof(cd) * (size_t)M * P, cudaMemcpyDeviceToHost, st));
-  return sync.done();
+  ChainDev d;
+  if (int rc = queue_logsv_prices(d, c, params, etas, N, prices_out, nullptr)) return rc;
+  B200SV_CUDA(d.a.download(cplx(a_out), (size_t)M * c.P * N));
+  B200SV_CUDA(d.lm.download(cplx(log_mgf_out), (size_t)M * c.P));
+  return d.sync.done();
 }
 
 int b200sv_heston_price_chain(const b200sv_heston_params* params, int M, const double* ttms, const double* forwards,
                               const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
                               int variable_type, double vol_scaler, int P, double* prices_out, double* log_mgf_out) {
   B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out, "null pointer");
-  if (variable_type != B200SV_LOG_RETURN && variable_type != B200SV_Q_VAR) return fail(-4, "variable_type not implemented");   // heston_pricer.py:276-277
-  const bool qvar = variable_type == B200SV_Q_VAR;
-  if (P <= 0) P = qvar ? 40000 : 1000;
-  B200SV_REQUIRE(M >= 1 && P >= 3, "M >= 1, P >= 3");
-  const int Jtot = offsets[M] - offsets[0];
-  if (int rc = qvar ? check_qvar_types(types + offsets[0], Jtot) : check_fourier_types(types + offsets[0], Jtot, true)) return rc;
-  if (!(vol_scaler > 0.0)) vol_scaler = std::min(0.3, std::sqrt(params->v0 * ttms[0]));   // heston_pricer.py:234-235
-  std::vector<double> phi, psi;
-  if (!qvar) {
-    build_phi(vol_scaler, true, P, phi);
-  } else {
-    build_grid(-0.5, 4000.0, P, psi);
-    phi.assign(2 * (size_t)P, 0.0);
-  }
-  std::vector<double> dtaus(M);
-  double t0 = 0.0;
-  for (int m = 0; m < M; ++m) {
-    B200SV_REQUIRE(ttms[m] > t0, "ttms must be positive and strictly increasing");
-    dtaus[m] = ttms[m] - t0;
-    t0 = ttms[m];
-  }
-  std::vector<StrikeSpec> ss(std::max(Jtot, 1));
-  std::vector<SumSpec> qs(std::max(Jtot, 1));
-  for (int m = 0; m < M; ++m)
-    for (int j = offsets[m]; j < offsets[m + 1]; ++j) {
-      B200SV_REQUIRE(strikes[j] > 0.0, "strikes must be positive");
-      ss[j - offsets[0]] = StrikeSpec{strikes[j], forwards[m], discfactors[m], (int)types[j], m, ttms[m], 0};
-      qs[j - offsets[0]] = SumSpec{strikes[j] * ttms[m], discfactors[m], ttms[m], (int)types[j], m};
-    }
-  cudaStream_t st = current_stream();
-  ensure_pool_threshold();
-  StreamSync sync(st);
-  DevBuf d_phi(st), d_psi(st), d_dt(st), d_lm(st), d_ss(st), d_pr(st);
-  B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_psi.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_dt.alloc(sizeof(double) * M));
-  B200SV_CUDA(d_lm.alloc(sizeof(cd) * (size_t)M * P));
-  B200SV_CUDA(d_ss.alloc(std::max(sizeof(StrikeSpec), sizeof(SumSpec)) * ss.size()));
-  B200SV_CUDA(d_pr.alloc(sizeof(double) * ss.size()));
-  B200SV_CUDA(cudaMemcpyAsync(d_phi.p, phi.data(), sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  if (qvar) B200SV_CUDA(cudaMemcpyAsync(d_psi.p, psi.data(), sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_dt.p, dtaus.data(), sizeof(double) * M, cudaMemcpyHostToDevice, st));
-  if (qvar)
-    B200SV_CUDA(cudaMemcpyAsync(d_ss.p, qs.data(), sizeof(SumSpec) * qs.size(), cudaMemcpyHostToDevice, st));
-  else
-    B200SV_CUDA(cudaMemcpyAsync(d_ss.p, ss.data(), sizeof(StrikeSpec) * ss.size(), cudaMemcpyHostToDevice, st));
-  const int tpb = mgf_block_threads(P), nb = (P + tpb - 1) / tpb;
-  heston_mgf_kernel<<<nb, tpb, 0, st>>>(d_phi.as<cd>(), qvar ? d_psi.as<cd>() : nullptr, P, M, d_dt.as<double>(), *params, nullptr, nullptr,
-                                        nullptr, nullptr, d_lm.as<cd>());
-  if (int rc = check_launch("heston_mgf_kernel")) return rc;
-  if (Jtot > 0) {
-    if (qvar)
-      fourier_sum_kernel<<<Jtot, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_psi.as<cd>(), P, d_ss.as<SumSpec>(), kModeQvar, 0, d_pr.as<double>());
-    else
-      fourier_vanilla_kernel<<<Jtot, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_phi.as<cd>(), P, d_ss.as<StrikeSpec>(), 1, 1, d_pr.as<double>());
-    if (int rc = check_launch("fourier_vanilla_kernel")) return rc;
-    B200SV_CUDA(cudaMemcpyAsync(prices_out, d_pr.p, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st));
-  }
-  if (log_mgf_out) B200SV_CUDA(cudaMemcpyAsync(log_mgf_out, d_lm.p, sizeof(cd) * (size_t)M * P, cudaMemcpyDeviceToHost, st));
-  return sync.done();
+  FourierChain c;
+  if (int rc = prepare_heston_chain(c, params, M, ttms, forwards, discfactors, offsets, strikes, types, variable_type, vol_scaler, P)) return rc;
+  ChainDev d;
+  if (int rc = queue_heston_prices(d, c, params, prices_out, nullptr)) return rc;
+  B200SV_CUDA(d.lm.download(cplx(log_mgf_out), (size_t)M * c.P));
+  return d.sync.done();
 }
 
 /* ---- forward-mode sensitivities of the two Fourier chain pricers (DESIGN.md §4.2) ----
- * The prices come from b200sv_*_price_chain itself (same launches, bit-identical); the tangent kernel then re-runs the primal next to
- * one tangent per thread and fourier_vanilla_greeks_kernel assembles delta, gamma and the parameter rows. */
-static int greeks_strike_specs(int M, const double* ttms, const double* forwards, const double* discfactors, const int* offsets,
-                               const double* strikes, std::vector<StrikeSpec>& ss, std::vector<double>& dtaus) {
-  const int Jtot = offsets[M] - offsets[0];
-  ss.resize(std::max(Jtot, 1));
-  dtaus.resize(M);
-  double t0 = 0.0;
-  for (int m = 0; m < M; ++m) {
-    dtaus[m] = ttms[m] - t0;
-    t0 = ttms[m];
-    for (int j = offsets[m]; j < offsets[m + 1]; ++j) ss[j - offsets[0]] = StrikeSpec{strikes[j], forwards[m], discfactors[m], 0, m, ttms[m], 0};
-  }
-  return Jtot;
-}
-
+ * One prepared chain: the pricing launches of b200sv_*_price_chain (same function, so bit-identical prices), then the tangent kernel and
+ * fourier_vanilla_greeks_kernel, which assembles delta, gamma and the parameter rows; one synchronisation at the end. */
 int b200sv_logsv_price_chain_greeks(const b200sv_logsv_params* params, int M, const double* ttms, const double* forwards,
                                     const double* discfactors, const double* etas, const int* offsets, const double* strikes,
                                     const int8_t* types, int is_spot_measure, int variable_type, int expansion_order,
@@ -2002,60 +2137,42 @@ int b200sv_logsv_price_chain_greeks(const b200sv_logsv_params* params, int M, co
                                     int* nfev_out) {
   B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && greeks_out, "null pointer");
   if (variable_type != B200SV_LOG_RETURN) return fail(-4, "variable_type not implemented: sensitivities cover LOG_RETURN only");
-  if (int rc = b200sv_logsv_price_chain(params, M, ttms, forwards, discfactors, etas, offsets, strikes, types, is_spot_measure, variable_type,
-                                        expansion_order, vol_scaler, P, prices_out, nullptr, nullptr))
-    return rc;                                                             // validates every argument the two routes share
-  if (P <= 0) P = 1000;
-  const bool spot = is_spot_measure != 0;
+  FourierChain c;
+  if (int rc = prepare_logsv_chain(c, params, M, ttms, forwards, discfactors, offsets, strikes, types, is_spot_measure, variable_type,
+                                   expansion_order, vol_scaler, P))
+    return rc;
   const int N = expansion_order == B200SV_ORDER_FIRST ? 3 : 5, NP = 1 + kLogsvOdeDirs;
-  if (!(vol_scaler > 0.0)) vol_scaler = params->sigma0 * std::sqrt(std::min(*std::min_element(ttms, ttms + M), 0.5 / 12.0));
-  std::vector<double> phi, dtaus;
-  build_phi(vol_scaler, spot, P, phi);
-  std::vector<StrikeSpec> ss;
-  const int Jtot = greeks_strike_specs(M, ttms, forwards, discfactors, offsets, strikes, ss, dtaus);
-  for (int j = 0; j < Jtot; ++j) ss[j].type = types[offsets[0] + j];
-  std::vector<ChainSpec> spec(M);
+  P = c.P;
   std::vector<LogsvModelTangent> dspec((size_t)M * kLogsvOdeDirs);
   for (int m = 0; m < M; ++m) {
-    const double eta = etas ? etas[m] : 1.0;
-    spec[m] = ChainSpec{dtaus[m], make_model(*params, eta, spot)};
-    LogsvModelTangent d[kLogsvOdeDirs];
-    make_model_tangents(*params, eta, spot, d);
-    std::copy(d, d + kLogsvOdeDirs, dspec.begin() + (size_t)m * kLogsvOdeDirs);
+    LogsvModelTangent t[kLogsvOdeDirs];
+    make_model_tangents(*params, etas ? etas[m] : 1.0, c.spot, t);
+    std::copy(t, t + kLogsvOdeDirs, dspec.begin() + (size_t)m * kLogsvOdeDirs);
   }
-  cudaStream_t st = current_stream();
-  StreamSync sync(st);
-  DevBuf d_phi(st), d_spec(st), d_dspec(st), d_dlm(st), d_lm(st), d_nfev(st), d_ss(st), d_g(st);
-  B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_spec.alloc(sizeof(ChainSpec) * M));
-  B200SV_CUDA(d_dspec.alloc(sizeof(LogsvModelTangent) * dspec.size()));
+  ChainDev d;
+  if (int rc = queue_logsv_prices(d, c, params, etas, N, prices_out, nullptr)) return rc;
+  DevBuf d_dspec(d.st), d_dlm(d.st), d_lm(d.st), d_nfev(d.st), d_g(d.st);
+  B200SV_CUDA(d_dspec.upload(dspec.data(), dspec.size()));
   B200SV_CUDA(d_dlm.alloc(sizeof(cd) * (size_t)NP * M * P));
   B200SV_CUDA(d_lm.alloc(sizeof(cd) * (size_t)M * P));
   B200SV_CUDA(d_nfev.alloc(sizeof(int) * P));
-  B200SV_CUDA(d_ss.alloc(sizeof(StrikeSpec) * ss.size()));
-  B200SV_CUDA(d_g.alloc(sizeof(double) * (size_t)(2 + NP) * ss.size()));
-  B200SV_CUDA(cudaMemcpyAsync(d_phi.p, phi.data(), sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_spec.p, spec.data(), sizeof(ChainSpec) * M, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_dspec.p, dspec.data(), sizeof(LogsvModelTangent) * dspec.size(), cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_ss.p, ss.data(), sizeof(StrikeSpec) * ss.size(), cudaMemcpyHostToDevice, st));
-  const int nb = (P * kLogsvOdeDirs + kTangentTPB - 1) / kTangentTPB;
-  const double y = params->sigma0 - params->theta;
-  if (N == 5)
-    logsv_mgf_tangent_kernel<5><<<nb, kTangentTPB, 0, st>>>(d_phi.as<cd>(), P, M, d_spec.as<ChainSpec>(), d_dspec.as<LogsvModelTangent>(), y,
-                                                            d_dlm.as<cd>(), d_lm.as<cd>(), nullptr, d_nfev.as<int>());
-  else
-    logsv_mgf_tangent_kernel<3><<<nb, kTangentTPB, 0, st>>>(d_phi.as<cd>(), P, M, d_spec.as<ChainSpec>(), d_dspec.as<LogsvModelTangent>(), y,
-                                                            d_dlm.as<cd>(), d_lm.as<cd>(), nullptr, d_nfev.as<int>());
+  B200SV_CUDA(d_g.alloc(sizeof(double) * (size_t)(2 + NP) * c.ss.size()));
+  const auto tangent = N == 5 ? logsv_mgf_tangent_kernel<5> : logsv_mgf_tangent_kernel<3>;
+  tangent<<<(P * kLogsvOdeDirs + kTangentTPB - 1) / kTangentTPB, kTangentTPB, 0, d.st>>>(d.phi.as<cd>(), P, M, d.spec.as<ChainSpec>(),
+                                                                                       d_dspec.as<LogsvModelTangent>(),
+                                                                                       params->sigma0 - params->theta, d_dlm.as<cd>(),
+                                                                                       d_lm.as<cd>(), nullptr, d_nfev.as<int>());
   if (int rc = check_launch("logsv_mgf_tangent_kernel")) return rc;
-  if (Jtot > 0) {
-    fourier_vanilla_greeks_kernel<1 + kLogsvOdeDirs><<<Jtot, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_dlm.as<cd>(), d_phi.as<cd>(), P, M,
-                                                                                       d_ss.as<StrikeSpec>(), spot ? 1 : 0, d_g.as<double>());
+  if (c.Jtot > 0) {       // the tangent kernel's own primal log-MGF (DESIGN.md §4.2)
+    fourier_vanilla_greeks_kernel<1 + kLogsvOdeDirs><<<c.Jtot, kFourierThreads, 0, d.st>>>(d_lm.as<cd>(), d_dlm.as<cd>(), d.phi.as<cd>(), P, M,
+                                                                                         d.rows.as<StrikeSpec>(), c.spot ? 1 : 0,
+                                                                                         d_g.as<double>());
     if (int rc = check_launch("fourier_vanilla_greeks_kernel")) return rc;
-    B200SV_CUDA(cudaMemcpyAsync(greeks_out, d_g.p, sizeof(double) * (size_t)(2 + NP) * Jtot, cudaMemcpyDeviceToHost, st));
+    B200SV_CUDA(d_g.download(greeks_out, (size_t)(2 + NP) * c.Jtot));
   }
-  if (dlog_mgf_out) B200SV_CUDA(cudaMemcpyAsync(dlog_mgf_out, d_dlm.p, sizeof(cd) * (size_t)NP * M * P, cudaMemcpyDeviceToHost, st));
-  if (nfev_out) B200SV_CUDA(cudaMemcpyAsync(nfev_out, d_nfev.p, sizeof(int) * P, cudaMemcpyDeviceToHost, st));
-  return sync.done();
+  B200SV_CUDA(d_dlm.download(cplx(dlog_mgf_out), (size_t)NP * M * P));
+  B200SV_CUDA(d_nfev.download(nfev_out, P));
+  return d.sync.done();
 }
 
 int b200sv_heston_price_chain_greeks(const b200sv_heston_params* params, int M, const double* ttms, const double* forwards,
@@ -2064,172 +2181,54 @@ int b200sv_heston_price_chain_greeks(const b200sv_heston_params* params, int M, 
                                      double* dlog_mgf_out) {
   B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && greeks_out, "null pointer");
   if (variable_type != B200SV_LOG_RETURN) return fail(-4, "variable_type not implemented: sensitivities cover LOG_RETURN only");
-  if (int rc = b200sv_heston_price_chain(params, M, ttms, forwards, discfactors, offsets, strikes, types, variable_type, vol_scaler, P,
-                                         prices_out, nullptr))
-    return rc;
-  if (P <= 0) P = 1000;
+  FourierChain c;
+  if (int rc = prepare_heston_chain(c, params, M, ttms, forwards, discfactors, offsets, strikes, types, variable_type, vol_scaler, P)) return rc;
   const int NP = 1 + kHestonOdeDirs;
-  if (!(vol_scaler > 0.0)) vol_scaler = std::min(0.3, std::sqrt(params->v0 * ttms[0]));
-  std::vector<double> phi, dtaus;
-  build_phi(vol_scaler, true, P, phi);
-  std::vector<StrikeSpec> ss;
-  const int Jtot = greeks_strike_specs(M, ttms, forwards, discfactors, offsets, strikes, ss, dtaus);
-  for (int j = 0; j < Jtot; ++j) ss[j].type = types[offsets[0] + j];
-  cudaStream_t st = current_stream();
-  StreamSync sync(st);
-  DevBuf d_phi(st), d_dt(st), d_dlm(st), d_lm(st), d_ss(st), d_g(st);
-  B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_dt.alloc(sizeof(double) * M));
+  P = c.P;
+  ChainDev d;
+  if (int rc = queue_heston_prices(d, c, params, prices_out, nullptr)) return rc;
+  DevBuf d_dlm(d.st), d_g(d.st);
   B200SV_CUDA(d_dlm.alloc(sizeof(cd) * (size_t)NP * M * P));
-  B200SV_CUDA(d_lm.alloc(sizeof(cd) * (size_t)M * P));
-  B200SV_CUDA(d_ss.alloc(sizeof(StrikeSpec) * ss.size()));
-  B200SV_CUDA(d_g.alloc(sizeof(double) * (size_t)(2 + NP) * ss.size()));
-  B200SV_CUDA(cudaMemcpyAsync(d_phi.p, phi.data(), sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_dt.p, dtaus.data(), sizeof(double) * M, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_ss.p, ss.data(), sizeof(StrikeSpec) * ss.size(), cudaMemcpyHostToDevice, st));
-  const int tpb = 64;
-  heston_mgf_kernel<<<(P + tpb - 1) / tpb, tpb, 0, st>>>(d_phi.as<cd>(), nullptr, P, M, d_dt.as<double>(), *params, nullptr, nullptr, nullptr,
-                                                        nullptr, d_lm.as<cd>());
-  if (int rc = check_launch("heston_mgf_kernel")) return rc;
-  heston_mgf_tangent_kernel<<<(P * kHestonOdeDirs + tpb - 1) / tpb, tpb, 0, st>>>(d_phi.as<cd>(), P, M, d_dt.as<double>(), *params, d_dlm.as<cd>());
+  B200SV_CUDA(d_g.alloc(sizeof(double) * (size_t)(2 + NP) * c.ss.size()));
+  heston_mgf_tangent_kernel<<<(P * kHestonOdeDirs + 63) / 64, 64, 0, d.st>>>(d.phi.as<cd>(), P, M, d.dt.as<double>(), *params, d_dlm.as<cd>());
   if (int rc = check_launch("heston_mgf_tangent_kernel")) return rc;
-  if (Jtot > 0) {
-    fourier_vanilla_greeks_kernel<1 + kHestonOdeDirs><<<Jtot, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_dlm.as<cd>(), d_phi.as<cd>(), P, M,
-                                                                                        d_ss.as<StrikeSpec>(), 1, d_g.as<double>());
+  if (c.Jtot > 0) {       // the pricing launch's log-MGF: heston_mgf_kernel is a per-thread closed form, the same for any block size
+    fourier_vanilla_greeks_kernel<1 + kHestonOdeDirs><<<c.Jtot, kFourierThreads, 0, d.st>>>(d.lm.as<cd>(), d_dlm.as<cd>(), d.phi.as<cd>(), P, M,
+                                                                                          d.rows.as<StrikeSpec>(), 1, d_g.as<double>());
     if (int rc = check_launch("fourier_vanilla_greeks_kernel")) return rc;
-    B200SV_CUDA(cudaMemcpyAsync(greeks_out, d_g.p, sizeof(double) * (size_t)(2 + NP) * Jtot, cudaMemcpyDeviceToHost, st));
+    B200SV_CUDA(d_g.download(greeks_out, (size_t)(2 + NP) * c.Jtot));
   }
-  if (dlog_mgf_out) B200SV_CUDA(cudaMemcpyAsync(dlog_mgf_out, d_dlm.p, sizeof(cd) * (size_t)NP * M * P, cudaMemcpyDeviceToHost, st));
-  return sync.done();
+  B200SV_CUDA(d_dlm.download(cplx(dlog_mgf_out), (size_t)NP * M * P));
+  return d.sync.done();
 }
 
-/* ---- batched chain pricers: B parameter sets on one chain in one pass (calibration objective + its finite-difference gradient) ---- */
-static int chain_batch_common(int B, int M, const double* ttms, const double* forwards, const double* discfactors, const int* offsets,
-                              const double* strikes, const int8_t* types, bool spot, int P, std::vector<double>& dtaus,
-                              std::vector<StrikeSpec>& ss, bool per_set_grid) {
-  B200SV_REQUIRE(B >= 1 && B <= 65535 && M >= 1 && P >= 3, "1 <= B <= 65535, M >= 1, P >= 3");
-  const int Jtot = offsets[M] - offsets[0];
-  B200SV_REQUIRE(Jtot >= 1, "the chain has no strikes");
-  if (int rc = check_fourier_types(types + offsets[0], Jtot, spot)) return rc;
-  dtaus.resize(M);
-  double t0 = 0.0;
-  for (int m = 0; m < M; ++m) {
-    B200SV_REQUIRE(ttms[m] > t0, "ttms must be positive and strictly increasing");
-    dtaus[m] = ttms[m] - t0;
-    t0 = ttms[m];
-  }
-  ss.resize((size_t)B * Jtot);
-  for (int b = 0; b < B; ++b)
-    for (int m = 0; m < M; ++m)
-      for (int j = offsets[m]; j < offsets[m + 1]; ++j) {
-        B200SV_REQUIRE(strikes[j] > 0.0, "strikes must be positive");
-        ss[(size_t)b * Jtot + (j - offsets[0])] = StrikeSpec{strikes[j], forwards[m], discfactors[m], (int)types[j], b * M + m, ttms[m], per_set_grid ? b : 0};
-      }
-  return 0;
-}
-
+/* ---- batched chain pricers: B parameter sets on one chain in one pass (calibration objective + its finite-difference gradient) ----
+ * vol_scaler <= 0: each set gets its own grid from its default scaler */
 int b200sv_logsv_price_chain_batch(const b200sv_logsv_params* params, int B, int M, const double* ttms, const double* forwards,
                                    const double* discfactors, const double* etas, const int* offsets, const double* strikes,
                                    const int8_t* types, int is_spot_measure, int expansion_order, double vol_scaler, int P,
                                    double* prices_out, double* ivols_out) {
   B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && strikes && types && prices_out, "null pointer");
-  if (P <= 0) P = 1000;
   if (expansion_order != B200SV_ORDER_FIRST && expansion_order != B200SV_ORDER_SECOND) return fail(-4, "expansion_order not implemented");
-  const bool spot = is_spot_measure != 0;
-  const bool per_set_grid = !(vol_scaler > 0.0);      // default scaler depends on sigma0 of each set (logsv_pricer.py:664-666)
-  std::vector<double> dtaus;
-  std::vector<StrikeSpec> ss;
-  if (int rc = chain_batch_common(B, M, ttms, forwards, discfactors, offsets, strikes, types, spot, P, dtaus, ss, per_set_grid)) return rc;
-  const int Jtot = offsets[M] - offsets[0], N = expansion_order == B200SV_ORDER_FIRST ? 3 : 5;
-  const double tmin = *std::min_element(ttms, ttms + M);
-  const int G = per_set_grid ? B : 1;
-  std::vector<double> phi, one;
-  for (int g = 0; g < G; ++g) {
-    build_phi(per_set_grid ? params[g].sigma0 * std::sqrt(std::min(tmin, 0.5 / 12.0)) : vol_scaler, spot, P, one);
-    phi.insert(phi.end(), one.begin(), one.end());
-  }
-  std::vector<ChainSpec> spec((size_t)B * M);
-  std::vector<double> yb(B);
-  for (int b = 0; b < B; ++b) {
-    yb[b] = params[b].sigma0 - params[b].theta;
-    for (int m = 0; m < M; ++m) spec[(size_t)b * M + m] = ChainSpec{dtaus[m], make_model(params[b], etas ? etas[(size_t)b * M + m] : 1.0, spot)};
-  }
-  cudaStream_t st = current_stream();
-  ensure_pool_threshold();
-  StreamSync sync(st);
-  DevBuf d_phi(st), d_spec(st), d_y(st), d_a(st), d_lm(st), d_ss(st), d_pr(st), d_iv(st);
-  const size_t nq = (size_t)B * Jtot;
-  B200SV_CUDA(d_phi.alloc(sizeof(cd) * (size_t)G * P));
-  B200SV_CUDA(d_spec.alloc(sizeof(ChainSpec) * spec.size()));
-  B200SV_CUDA(d_y.alloc(sizeof(double) * B));
-  B200SV_CUDA(d_a.alloc(sizeof(cd) * (size_t)B * M * P * N));
-  B200SV_CUDA(d_lm.alloc(sizeof(cd) * (size_t)B * M * P));
-  B200SV_CUDA(d_ss.alloc(sizeof(StrikeSpec) * nq));
-  B200SV_CUDA(d_pr.alloc(sizeof(double) * nq));
-  B200SV_CUDA(d_iv.alloc(sizeof(double) * nq));
-  B200SV_CUDA(cudaMemcpyAsync(d_phi.p, phi.data(), sizeof(cd) * (size_t)G * P, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_spec.p, spec.data(), sizeof(ChainSpec) * spec.size(), cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_y.p, yb.data(), sizeof(double) * B, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_ss.p, ss.data(), sizeof(StrikeSpec) * nq, cudaMemcpyHostToDevice, st));
-  const long long threads = (long long)B * P;
-  const int tpb = mgf_block_threads((int)std::min<long long>(threads, 1 << 30)), nb = (P + tpb - 1) / tpb;
-  if (N == 5)
-    launch_logsv_mgf<5>(tpb, nb, st, d_phi.as<cd>(), nullptr, P, M, d_spec.as<ChainSpec>(), nullptr, d_a.as<cd>(), d_lm.as<cd>(), 0.0, nullptr, B,
-                        d_y.as<double>(), per_set_grid ? P : 0);
-  else
-    launch_logsv_mgf<3>(tpb, nb, st, d_phi.as<cd>(), nullptr, P, M, d_spec.as<ChainSpec>(), nullptr, d_a.as<cd>(), d_lm.as<cd>(), 0.0, nullptr, B,
-                        d_y.as<double>(), per_set_grid ? P : 0);
-  if (int rc = check_launch("logsv_mgf_kernel")) return rc;
-  fourier_vanilla_kernel<<<(unsigned)nq, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_phi.as<cd>(), P, d_ss.as<StrikeSpec>(), spot ? 1 : 0, 1,
-                                                                    d_pr.as<double>(), ivols_out ? d_iv.as<double>() : nullptr);
-  if (int rc = check_launch("fourier_vanilla_kernel")) return rc;
-  B200SV_CUDA(cudaMemcpyAsync(prices_out, d_pr.p, sizeof(double) * nq, cudaMemcpyDeviceToHost, st));
-  if (ivols_out) B200SV_CUDA(cudaMemcpyAsync(ivols_out, d_iv.p, sizeof(double) * nq, cudaMemcpyDeviceToHost, st));
-  return sync.done();
+  FourierChain c;
+  if (int rc = c.init(true, B, M, P > 0 ? P : 1000, offsets)) return rc;
+  if (int rc = c.build(params, ttms, forwards, discfactors, offsets, strikes, types, is_spot_measure != 0, ChainTypes::kFourier, vol_scaler))
+    return rc;
+  ChainDev d;
+  if (int rc = queue_logsv_prices(d, c, params, etas, expansion_order == B200SV_ORDER_FIRST ? 3 : 5, prices_out, ivols_out)) return rc;
+  return d.sync.done();
 }
 
 int b200sv_heston_price_chain_batch(const b200sv_heston_params* params, int B, int M, const double* ttms, const double* forwards,
                                     const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
                                     double vol_scaler, int P, double* prices_out, double* ivols_out) {
   B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && strikes && types && prices_out, "null pointer");
-  if (P <= 0) P = 1000;
-  const bool per_set_grid = !(vol_scaler > 0.0);      // default scaler depends on v0 of each set (heston_pricer.py:234-235)
-  std::vector<double> dtaus;
-  std::vector<StrikeSpec> ss;
-  if (int rc = chain_batch_common(B, M, ttms, forwards, discfactors, offsets, strikes, types, true, P, dtaus, ss, per_set_grid)) return rc;
-  const int Jtot = offsets[M] - offsets[0];
-  const int G = per_set_grid ? B : 1;
-  std::vector<double> phi, one;
-  for (int g = 0; g < G; ++g) {
-    build_phi(per_set_grid ? std::min(0.3, std::sqrt(params[g].v0 * ttms[0])) : vol_scaler, true, P, one);
-    phi.insert(phi.end(), one.begin(), one.end());
-  }
-  cudaStream_t st = current_stream();
-  ensure_pool_threshold();
-  StreamSync sync(st);
-  DevBuf d_phi(st), d_hp(st), d_dt(st), d_lm(st), d_ss(st), d_pr(st), d_iv(st);
-  const size_t nq = (size_t)B * Jtot;
-  B200SV_CUDA(d_phi.alloc(sizeof(cd) * (size_t)G * P));
-  B200SV_CUDA(d_hp.alloc(sizeof(b200sv_heston_params) * B));
-  B200SV_CUDA(d_dt.alloc(sizeof(double) * M));
-  B200SV_CUDA(d_lm.alloc(sizeof(cd) * (size_t)B * M * P));
-  B200SV_CUDA(d_ss.alloc(sizeof(StrikeSpec) * nq));
-  B200SV_CUDA(d_pr.alloc(sizeof(double) * nq));
-  B200SV_CUDA(d_iv.alloc(sizeof(double) * nq));
-  B200SV_CUDA(cudaMemcpyAsync(d_phi.p, phi.data(), sizeof(cd) * (size_t)G * P, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_hp.p, params, sizeof(b200sv_heston_params) * B, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_dt.p, dtaus.data(), sizeof(double) * M, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_ss.p, ss.data(), sizeof(StrikeSpec) * nq, cudaMemcpyHostToDevice, st));
-  const int tpb = 64, nb = (P + tpb - 1) / tpb;
-  heston_mgf_kernel<<<dim3(nb, B), tpb, 0, st>>>(d_phi.as<cd>(), nullptr, P, M, d_dt.as<double>(), params[0], nullptr, nullptr, nullptr, nullptr,
-                                                 d_lm.as<cd>(), d_hp.as<b200sv_heston_params>(), per_set_grid ? P : 0);
-  if (int rc = check_launch("heston_mgf_kernel")) return rc;
-  fourier_vanilla_kernel<<<(unsigned)nq, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_phi.as<cd>(), P, d_ss.as<StrikeSpec>(), 1, 1, d_pr.as<double>(),
-                                                                    ivols_out ? d_iv.as<double>() : nullptr);
-  if (int rc = check_launch("fourier_vanilla_kernel")) return rc;
-  B200SV_CUDA(cudaMemcpyAsync(prices_out, d_pr.p, sizeof(double) * nq, cudaMemcpyDeviceToHost, st));
-  if (ivols_out) B200SV_CUDA(cudaMemcpyAsync(ivols_out, d_iv.p, sizeof(double) * nq, cudaMemcpyDeviceToHost, st));
-  return sync.done();
+  FourierChain c;
+  if (int rc = c.init(true, B, M, P > 0 ? P : 1000, offsets)) return rc;
+  if (int rc = c.build(params, ttms, forwards, discfactors, offsets, strikes, types, true, ChainTypes::kFourier, vol_scaler)) return rc;
+  ChainDev d;
+  if (int rc = queue_heston_prices(d, c, params, prices_out, ivols_out)) return rc;
+  return d.sync.done();
 }
 
 /* Hawkes jump-diffusion Fourier chain (hawkesjd_chain_pricer / hawkesjd_chain_pricer_with_risk_premia, hawkes_jd_pricer.py:365-515).
@@ -2241,93 +2240,53 @@ int b200sv_hawkesjd_price_chain(const b200sv_hawkes_params* params, int M, const
                                 double risk_premia_gamma, double* prices_out, double* a_out, double* log_mgf_out, double* normalizers_out,
                                 double* gamma_forwards_out) {
   B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out, "null pointer");
-  if (P <= 0) P = 500;                                                        // MAX_PHI, hawkes_jd_pricer.py:37
-  B200SV_REQUIRE(M >= 1 && P >= 3, "M >= 1, P >= 3");
   const bool with_gamma = risk_premia_gamma == risk_premia_gamma;
-  const bool spot = is_spot_measure != 0;
-  const int Jtot = offsets[M] - offsets[0];
-  if (with_gamma) {                                                            // utils/mgf_pricer.py:310-318: 'C' / 'P' under the spot measure only
-    if (!spot) return fail(-5, "not implemented");
-    for (int j = offsets[0]; j < offsets[M]; ++j)
-      if (types[j] != B200SV_CALL && types[j] != B200SV_PUT) return fail(-5, "not implemented");
-  } else if (int rc = check_fourier_types(types + offsets[0], Jtot, spot)) {
+  FourierChain c;
+  if (int rc = c.init(false, 1, M, P > 0 ? P : 500, offsets)) return rc;     // MAX_PHI, hawkes_jd_pricer.py:37
+  if (int rc = c.build(params, ttms, forwards, discfactors, offsets, strikes, types, is_spot_measure != 0,
+                       with_gamma ? ChainTypes::kGamma : ChainTypes::kFourier, vol_scaler))
     return rc;
-  }
-  std::vector<double> dtaus(M);
-  double t0 = 0.0, tmin = ttms[0];
-  for (int m = 0; m < M; ++m) {
-    B200SV_REQUIRE(ttms[m] > t0, "ttms must be positive and strictly increasing");
-    dtaus[m] = ttms[m] - t0;
-    t0 = ttms[m];
-    tmin = std::min(tmin, ttms[m]);
-  }
-  if (!(vol_scaler > 0.0)) vol_scaler = std::min(std::max(params->sigma, 0.2), 0.5) * std::sqrt(std::min(tmin, 1.0 / 12.0));   // :360-362
-  std::vector<double> phi;
-  build_phi(vol_scaler, true, P, phi);                                         // get_transform_var_grid default is_spot_measure=True (:385)
-  if (with_gamma)
-    for (int i = 0; i < P; ++i) phi[2 * i] = -0.5 - risk_premia_gamma;           // real_phi (:451)
-  const HawkesMgfConsts c = make_hawkes_mgf_consts(*params);
-  cudaStream_t st = current_stream();
-  ensure_pool_threshold();
-  StreamSync sync(st);
-  DevBuf d_phi(st), d_dt(st), d_a(st), d_lm(st), d_ss(st), d_pr(st), d_g(st);
-  B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_dt.alloc(sizeof(double) * 2 * M));
-  B200SV_CUDA(d_a.alloc(sizeof(cd) * (size_t)M * P * 3));
-  B200SV_CUDA(d_lm.alloc(sizeof(cd) * (size_t)M * P));
-  B200SV_CUDA(cudaMemcpyAsync(d_phi.p, phi.data(), sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  std::vector<double> dts(dtaus);
+  P = c.P;
+  for (int i = 0; i < P; ++i)        // get_transform_var_grid default is_spot_measure=True (:385); real_phi (:451)
+    c.phi[2 * i] = with_gamma ? -0.5 - risk_premia_gamma : -0.5;
+  const HawkesMgfConsts k = make_hawkes_mgf_consts(*params);
+  ChainDev d;
+  std::vector<double> dts(c.dtaus);
   dts.insert(dts.end(), ttms, ttms + M);                                        // [increments | full maturities]
-  B200SV_CUDA(cudaMemcpyAsync(d_dt.p, dts.data(), sizeof(double) * 2 * M, cudaMemcpyHostToDevice, st));
+  B200SV_CUDA(d.dt.upload(dts.data(), dts.size()));
   std::vector<double> normalizers(M, 1.0), gamma_forwards(M, 1.0);
   if (with_gamma) {                                                            // hawkesjd_forwards_under_risk_kernel (:487-515)
     const double two[4] = {-risk_premia_gamma, 0.0, -risk_premia_gamma - 1.0, 0.0};
-    B200SV_CUDA(d_g.alloc(sizeof(cd) * (2 + 2 * (size_t)M)));
-    B200SV_CUDA(cudaMemcpyAsync(d_g.p, two, sizeof(two), cudaMemcpyHostToDevice, st));
-    hawkes_mgf_kernel<4><<<1, 4, 0, st>>>(d_g.as<cd>(), nullptr, 2, M, d_dt.as<double>() + M, c, nullptr, nullptr, d_g.as<cd>() + 2, 1, nullptr);
+    DevBuf d_two(d.st), d_lm2(d.st);
+    B200SV_CUDA(d_two.upload(cplx(two), 2));
+    B200SV_CUDA(d_lm2.alloc(sizeof(cd) * 2 * (size_t)M));
+    launch_hawkes_mgf(d.st, d_two.as<cd>(), nullptr, 2, M, d.dt.as<double>() + M, k, nullptr, nullptr, d_lm2.as<cd>(), 1);
     if (int rc = check_launch("hawkes_mgf_kernel")) return rc;
     std::vector<double> lm2(4 * (size_t)M);
-    B200SV_CUDA(cudaMemcpyAsync(lm2.data(), d_g.as<cd>() + 2, sizeof(cd) * 2 * M, cudaMemcpyDeviceToHost, st));
-    B200SV_CUDA(cudaStreamSynchronize(st));
+    B200SV_CUDA(cudaMemcpyAsync(lm2.data(), d_lm2.p, sizeof(cd) * 2 * M, cudaMemcpyDeviceToHost, d.st));
+    B200SV_CUDA(cudaStreamSynchronize(d.st));
     for (int m = 0; m < M; ++m) {                                              // log_mgf layout [m][point]
       normalizers[m] = 1.0 / std::exp(lm2[2 * (2 * (size_t)m + 0)]);
       gamma_forwards[m] = forwards[m] * std::exp(lm2[2 * (2 * (size_t)m + 1)]) * normalizers[m];
     }
-  }
-  std::vector<StrikeSpec> ss(std::max(Jtot, 1));
-  for (int m = 0; m < M; ++m)
-    for (int j = offsets[m]; j < offsets[m + 1]; ++j) {
-      B200SV_REQUIRE(strikes[j] > 0.0, "strikes must be positive");
-      ss[j - offsets[0]] = with_gamma ? StrikeSpec{strikes[j], forwards[m], normalizers[m], (int)types[j], m, gamma_forwards[m], 0}
-                                      : StrikeSpec{strikes[j], forwards[m], discfactors[m], (int)types[j], m, ttms[m], 0};
+    for (int j = 0; j < c.Jtot; ++j) {                                          // the gamma slice pricer's discfactor / forward slots
+      c.ss[j].discfactor = normalizers[c.ss[j].slice];
+      c.ss[j].ttm = gamma_forwards[c.ss[j].slice];
     }
-  B200SV_CUDA(d_ss.alloc(sizeof(StrikeSpec) * ss.size()));
-  B200SV_CUDA(d_pr.alloc(sizeof(double) * ss.size()));
-  B200SV_CUDA(cudaMemcpyAsync(d_ss.p, ss.data(), sizeof(StrikeSpec) * ss.size(), cudaMemcpyHostToDevice, st));
-  const int tpb = mgf_block_threads(P), nb = (P + tpb - 1) / tpb;
-  switch (tpb) {
-    case 4: hawkes_mgf_kernel<4><<<nb, 4, 0, st>>>(d_phi.as<cd>(), nullptr, P, M, d_dt.as<double>(), c, nullptr, d_a.as<cd>(), d_lm.as<cd>(), 0, nullptr); break;
-    case 8: hawkes_mgf_kernel<8><<<nb, 8, 0, st>>>(d_phi.as<cd>(), nullptr, P, M, d_dt.as<double>(), c, nullptr, d_a.as<cd>(), d_lm.as<cd>(), 0, nullptr); break;
-    case 16: hawkes_mgf_kernel<16><<<nb, 16, 0, st>>>(d_phi.as<cd>(), nullptr, P, M, d_dt.as<double>(), c, nullptr, d_a.as<cd>(), d_lm.as<cd>(), 0, nullptr); break;
-    case 32: hawkes_mgf_kernel<32><<<nb, 32, 0, st>>>(d_phi.as<cd>(), nullptr, P, M, d_dt.as<double>(), c, nullptr, d_a.as<cd>(), d_lm.as<cd>(), 0, nullptr); break;
-    default: hawkes_mgf_kernel<64><<<nb, 64, 0, st>>>(d_phi.as<cd>(), nullptr, P, M, d_dt.as<double>(), c, nullptr, d_a.as<cd>(), d_lm.as<cd>(), 0, nullptr); break;
   }
+  if (int rc = d.upload(c)) return rc;
+  B200SV_CUDA(d.a.alloc(sizeof(cd) * (size_t)M * P * 3));
+  launch_hawkes_mgf(d.st, d.phi.as<cd>(), nullptr, P, M, d.dt.as<double>(), k, nullptr, d.a.as<cd>(), d.lm.as<cd>(), 0);
   if (int rc = check_launch("hawkes_mgf_kernel")) return rc;
-  if (Jtot > 0) {
-    if (with_gamma)
-      fourier_gamma_kernel<<<Jtot, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_phi.as<cd>(), P, d_ss.as<StrikeSpec>(), risk_premia_gamma, d_pr.as<double>());
-    else
-      fourier_vanilla_kernel<<<Jtot, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_phi.as<cd>(), P, d_ss.as<StrikeSpec>(), spot ? 1 : 0, 1, d_pr.as<double>());
-    if (int rc = check_launch("fourier kernel")) return rc;
-    B200SV_CUDA(cudaMemcpyAsync(prices_out, d_pr.p, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st));
-  }
-  if (a_out) B200SV_CUDA(cudaMemcpyAsync(a_out, d_a.p, sizeof(cd) * (size_t)M * P * 3, cudaMemcpyDeviceToHost, st));
-  if (log_mgf_out) B200SV_CUDA(cudaMemcpyAsync(log_mgf_out, d_lm.p, sizeof(cd) * (size_t)M * P, cudaMemcpyDeviceToHost, st));
-  if (int rc = sync.done()) return rc;
+  if (int rc = d.sums(c, prices_out, nullptr, risk_premia_gamma)) return rc;
+  B200SV_CUDA(d.a.download(cplx(a_out), (size_t)M * P * 3));
+  B200SV_CUDA(d.lm.download(cplx(log_mgf_out), (size_t)M * P));
+  if (int rc = d.sync.done()) return rc;
   if (normalizers_out) std::copy(normalizers.begin(), normalizers.end(), normalizers_out);
   if (gamma_forwards_out) std::copy(gamma_forwards.begin(), gamma_forwards.end(), gamma_forwards_out);
   return 0;
 }
+
 
 /* compute_hawkes_a_mgf_grid (hawkes_jd_pricer.py:518-547) on caller-supplied grids: A(0) = a_inout [P][3] -> A(dtau) in place, log_mgf_out [P] */
 int b200sv_hawkesjd_mgf_grid(const double* phi, const double* psi, int P, double dtau, double* a_inout, const b200sv_hawkes_params* params,
@@ -2335,33 +2294,12 @@ int b200sv_hawkesjd_mgf_grid(const double* phi, const double* psi, int P, double
   B200SV_REQUIRE(phi && a_inout && params && log_mgf_out, "null pointer");
   B200SV_REQUIRE(P >= 1 && dtau > 0.0, "P >= 1, dtau > 0");
   const HawkesMgfConsts c = make_hawkes_mgf_consts(*params);
-  cudaStream_t st = current_stream();
-  ensure_pool_threshold();
-  StreamSync sync(st);
-  DevBuf d_phi(st), d_psi(st), d_dt(st), d_a0(st), d_a1(st), d_lm(st);
-  B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_psi.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_dt.alloc(sizeof(double)));
-  B200SV_CUDA(d_a0.alloc(sizeof(cd) * (size_t)P * 3));
-  B200SV_CUDA(d_a1.alloc(sizeof(cd) * (size_t)P * 3));
-  B200SV_CUDA(d_lm.alloc(sizeof(cd) * P));
-  B200SV_CUDA(cudaMemcpyAsync(d_phi.p, phi, sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  if (psi) B200SV_CUDA(cudaMemcpyAsync(d_psi.p, psi, sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_dt.p, &dtau, sizeof(double), cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_a0.p, a_inout, sizeof(cd) * (size_t)P * 3, cudaMemcpyHostToDevice, st));
-  const cd* dpsi = psi ? d_psi.as<cd>() : nullptr;
-  const int tpb = mgf_block_threads(P), nb = (P + tpb - 1) / tpb;
-  switch (tpb) {
-    case 4: hawkes_mgf_kernel<4><<<nb, 4, 0, st>>>(d_phi.as<cd>(), dpsi, P, 1, d_dt.as<double>(), c, d_a0.as<cd>(), d_a1.as<cd>(), d_lm.as<cd>(), 0, nullptr); break;
-    case 8: hawkes_mgf_kernel<8><<<nb, 8, 0, st>>>(d_phi.as<cd>(), dpsi, P, 1, d_dt.as<double>(), c, d_a0.as<cd>(), d_a1.as<cd>(), d_lm.as<cd>(), 0, nullptr); break;
-    case 16: hawkes_mgf_kernel<16><<<nb, 16, 0, st>>>(d_phi.as<cd>(), dpsi, P, 1, d_dt.as<double>(), c, d_a0.as<cd>(), d_a1.as<cd>(), d_lm.as<cd>(), 0, nullptr); break;
-    case 32: hawkes_mgf_kernel<32><<<nb, 32, 0, st>>>(d_phi.as<cd>(), dpsi, P, 1, d_dt.as<double>(), c, d_a0.as<cd>(), d_a1.as<cd>(), d_lm.as<cd>(), 0, nullptr); break;
-    default: hawkes_mgf_kernel<64><<<nb, 64, 0, st>>>(d_phi.as<cd>(), dpsi, P, 1, d_dt.as<double>(), c, d_a0.as<cd>(), d_a1.as<cd>(), d_lm.as<cd>(), 0, nullptr); break;
-  }
-  if (int rc = check_launch("hawkes_mgf_kernel")) return rc;
-  B200SV_CUDA(cudaMemcpyAsync(a_inout, d_a1.p, sizeof(cd) * (size_t)P * 3, cudaMemcpyDeviceToHost, st));
-  B200SV_CUDA(cudaMemcpyAsync(log_mgf_out, d_lm.p, sizeof(cd) * P, cudaMemcpyDeviceToHost, st));
-  return sync.done();
+  return run_grid(phi, psi, P, a_inout, 3, a_inout, log_mgf_out, [&](cudaStream_t st, const cd* ph, const cd* ps, const cd* a0, cd* a1, cd* lm) {
+    DevBuf d_dt(st);
+    B200SV_CUDA(d_dt.upload(&dtau, 1));
+    launch_hawkes_mgf(st, ph, ps, P, 1, d_dt.as<double>(), c, a0, a1, lm, 0);
+    return check_launch("hawkes_mgf_kernel");
+  });
 }
 
 int b200sv_logsv_mgf_grid(const double* phi, const double* psi, int P, double dtau, double* a_inout,
@@ -2369,35 +2307,15 @@ int b200sv_logsv_mgf_grid(const double* phi, const double* psi, int P, double dt
                           double* log_mgf_out) {
   B200SV_REQUIRE(phi && a_inout && params && log_mgf_out, "null pointer");
   B200SV_REQUIRE(P >= 1 && dtau > 0.0, "P >= 1, dtau > 0");
-  if (expansion_order != B200SV_ORDER_FIRST && expansion_order != B200SV_ORDER_SECOND)
-    return fail(-4, "expansion_order not implemented");
+  if (int rc = check_expansion_order(expansion_order)) return rc;
   const int N = expansion_order == B200SV_ORDER_FIRST ? 3 : 5;
-  ChainSpec spec{dtau, make_model(*params, eta, is_spot_measure != 0)};
-  cudaStream_t st = current_stream();
-  ensure_pool_threshold();
-  StreamSync sync(st);
-  DevBuf d_phi(st), d_psi(st), d_spec(st), d_a0(st), d_a1(st), d_lm(st);
-  B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_psi.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_spec.alloc(sizeof(ChainSpec)));
-  B200SV_CUDA(d_a0.alloc(sizeof(cd) * (size_t)P * N));
-  B200SV_CUDA(d_a1.alloc(sizeof(cd) * (size_t)P * N));
-  B200SV_CUDA(d_lm.alloc(sizeof(cd) * P));
-  B200SV_CUDA(cudaMemcpyAsync(d_phi.p, phi, sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  if (psi) B200SV_CUDA(cudaMemcpyAsync(d_psi.p, psi, sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_spec.p, &spec, sizeof(ChainSpec), cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_a0.p, a_inout, sizeof(cd) * (size_t)P * N, cudaMemcpyHostToDevice, st));
-  const int tpb = mgf_block_threads(P), nb = (P + tpb - 1) / tpb;
-  const double y = params->sigma0 - params->theta;
-  const cd* dpsi = psi ? d_psi.as<cd>() : nullptr;
-  if (N == 5)
-    launch_logsv_mgf<5>(tpb, nb, st, d_phi.as<cd>(), dpsi, P, 1, d_spec.as<ChainSpec>(), d_a0.as<cd>(), d_a1.as<cd>(), d_lm.as<cd>(), y, nullptr);
-  else
-    launch_logsv_mgf<3>(tpb, nb, st, d_phi.as<cd>(), dpsi, P, 1, d_spec.as<ChainSpec>(), d_a0.as<cd>(), d_a1.as<cd>(), d_lm.as<cd>(), y, nullptr);
-  if (int rc = check_launch("logsv_mgf_kernel")) return rc;
-  B200SV_CUDA(cudaMemcpyAsync(a_inout, d_a1.p, sizeof(cd) * (size_t)P * N, cudaMemcpyDeviceToHost, st));
-  B200SV_CUDA(cudaMemcpyAsync(log_mgf_out, d_lm.p, sizeof(cd) * P, cudaMemcpyDeviceToHost, st));
-  return sync.done();
+  const ChainSpec spec{dtau, make_model(*params, eta, is_spot_measure != 0)};
+  return run_grid(phi, psi, P, a_inout, N, a_inout, log_mgf_out, [&](cudaStream_t st, const cd* ph, const cd* ps, const cd* a0, cd* a1, cd* lm) {
+    DevBuf d_spec(st);
+    B200SV_CUDA(d_spec.upload(&spec, 1));
+    launch_logsv_mgf(N, st, ph, ps, P, 1, d_spec.as<ChainSpec>(), a0, a1, lm, params->sigma0 - params->theta);
+    return check_launch("logsv_mgf_kernel");
+  });
 }
 
 // func_a_ode_quadratic_terms (pricers/logsv/affine_expansion.py:67-184) for a grid of transform points: the dense tensors the reference
@@ -2408,81 +2326,54 @@ int b200sv_logsv_ode_terms(const double* phi, const double* psi, int P, const b2
                            int expansion_order, double* M_out, double* L_out, double* H_out) {
   B200SV_REQUIRE(phi && params && M_out && L_out && H_out, "null pointer");
   B200SV_REQUIRE(P >= 1, "P >= 1");
-  if (expansion_order != B200SV_ORDER_FIRST && expansion_order != B200SV_ORDER_SECOND) return fail(-4, "expansion_order not implemented");
+  if (int rc = check_expansion_order(expansion_order)) return rc;
   const int N = expansion_order == B200SV_ORDER_FIRST ? 3 : 5;
   const LogsvModel model = make_model(*params, eta, is_spot_measure != 0);
-  cudaStream_t st = current_stream();
-  ensure_pool_threshold();
-  StreamSync sync(st);
-  DevBuf d_phi(st), d_psi(st), d_M(st), d_L(st), d_H(st);
-  const size_t nM = (size_t)P * N * N * N, nL = (size_t)P * N * N, nH = (size_t)P * N;
-  B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_psi.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_M.alloc(sizeof(cd) * nM));
-  B200SV_CUDA(d_L.alloc(sizeof(cd) * nL));
-  B200SV_CUDA(d_H.alloc(sizeof(cd) * nH));
-  B200SV_CUDA(cudaMemcpyAsync(d_phi.p, phi, sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  if (psi) B200SV_CUDA(cudaMemcpyAsync(d_psi.p, psi, sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  const cd* dpsi = psi ? d_psi.as<cd>() : nullptr;
-  if (N == 5)
-    logsv_ode_terms_kernel<5><<<(P + 63) / 64, 64, 0, st>>>(d_phi.as<cd>(), dpsi, P, model, d_M.as<cd>(), d_L.as<cd>(), d_H.as<cd>());
-  else
-    logsv_ode_terms_kernel<3><<<(P + 63) / 64, 64, 0, st>>>(d_phi.as<cd>(), dpsi, P, model, d_M.as<cd>(), d_L.as<cd>(), d_H.as<cd>());
-  if (int rc = check_launch("logsv_ode_terms_kernel")) return rc;
-  B200SV_CUDA(cudaMemcpyAsync(M_out, d_M.p, sizeof(cd) * nM, cudaMemcpyDeviceToHost, st));
-  B200SV_CUDA(cudaMemcpyAsync(L_out, d_L.p, sizeof(cd) * nL, cudaMemcpyDeviceToHost, st));
-  B200SV_CUDA(cudaMemcpyAsync(H_out, d_H.p, sizeof(cd) * nH, cudaMemcpyDeviceToHost, st));
-  return sync.done();
+  return run_grid(phi, psi, P, nullptr, 0, nullptr, nullptr, [&](cudaStream_t st, const cd* ph, const cd* ps, const cd*, cd*, cd*) {
+    const size_t nM = (size_t)P * N * N * N, nL = (size_t)P * N * N, nH = (size_t)P * N;
+    DevBuf d_M(st), d_L(st), d_H(st);
+    B200SV_CUDA(d_M.alloc(sizeof(cd) * nM));
+    B200SV_CUDA(d_L.alloc(sizeof(cd) * nL));
+    B200SV_CUDA(d_H.alloc(sizeof(cd) * nH));
+    const auto terms = N == 5 ? logsv_ode_terms_kernel<5> : logsv_ode_terms_kernel<3>;
+    terms<<<(P + 63) / 64, 64, 0, st>>>(ph, ps, P, model, d_M.as<cd>(), d_L.as<cd>(), d_H.as<cd>());
+    if (int rc = check_launch("logsv_ode_terms_kernel")) return rc;
+    B200SV_CUDA(d_M.download(cplx(M_out), nM));
+    B200SV_CUDA(d_L.download(cplx(L_out), nL));
+    B200SV_CUDA(d_H.download(cplx(H_out), nH));
+    return 0;
+  });
 }
 
 int b200sv_logsv_ode_rhs(const double* phi, const double* psi, int P, const double* A, const b200sv_logsv_params* params, double eta,
                          int is_spot_measure, int expansion_order, double* rhs_out) {
   B200SV_REQUIRE(phi && A && params && rhs_out, "null pointer");
   B200SV_REQUIRE(P >= 1, "P >= 1");
-  if (expansion_order != B200SV_ORDER_FIRST && expansion_order != B200SV_ORDER_SECOND) return fail(-4, "expansion_order not implemented");
+  if (int rc = check_expansion_order(expansion_order)) return rc;
   const int N = expansion_order == B200SV_ORDER_FIRST ? 3 : 5;
   const LogsvModel model = make_model(*params, eta, is_spot_measure != 0);
-  cudaStream_t st = current_stream();
-  ensure_pool_threshold();
-  StreamSync sync(st);
-  DevBuf d_phi(st), d_psi(st), d_A(st), d_R(st);
-  B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_psi.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_A.alloc(sizeof(cd) * (size_t)P * N));
-  B200SV_CUDA(d_R.alloc(sizeof(cd) * (size_t)P * N));
-  B200SV_CUDA(cudaMemcpyAsync(d_phi.p, phi, sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  if (psi) B200SV_CUDA(cudaMemcpyAsync(d_psi.p, psi, sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_A.p, A, sizeof(cd) * (size_t)P * N, cudaMemcpyHostToDevice, st));
-  const cd* dpsi = psi ? d_psi.as<cd>() : nullptr;
-  if (N == 5)
-    logsv_ode_rhs_kernel<5><<<(P + 63) / 64, 64, 0, st>>>(d_phi.as<cd>(), dpsi, P, model, d_A.as<cd>(), d_R.as<cd>());
-  else
-    logsv_ode_rhs_kernel<3><<<(P + 63) / 64, 64, 0, st>>>(d_phi.as<cd>(), dpsi, P, model, d_A.as<cd>(), d_R.as<cd>());
-  if (int rc = check_launch("logsv_ode_rhs_kernel")) return rc;
-  B200SV_CUDA(cudaMemcpyAsync(rhs_out, d_R.p, sizeof(cd) * (size_t)P * N, cudaMemcpyDeviceToHost, st));
-  return sync.done();
+  return run_grid(phi, psi, P, A, N, rhs_out, nullptr, [&](cudaStream_t st, const cd* ph, const cd* ps, const cd* a, cd* r, cd*) {
+    const auto rhs = N == 5 ? logsv_ode_rhs_kernel<5> : logsv_ode_rhs_kernel<3>;
+    rhs<<<(P + 63) / 64, 64, 0, st>>>(ph, ps, P, model, a, r);
+    return check_launch("logsv_ode_rhs_kernel");
+  });
 }
 
 int b200sv_ode_rhs_dense(const double* A, int P, int n, const double* M, const double* L, const double* H, double* rhs_out) {
   B200SV_REQUIRE(A && M && L && H && rhs_out, "null pointer");
   B200SV_REQUIRE(P >= 1 && n >= 1 && n <= 16, "P >= 1, 1 <= n <= 16");
-  cudaStream_t st = current_stream();
-  ensure_pool_threshold();
-  StreamSync sync(st);
+  HostCall call;
+  const cudaStream_t st = call.st;
   DevBuf d_A(st), d_M(st), d_L(st), d_H(st), d_R(st);
-  B200SV_CUDA(d_A.alloc(sizeof(cd) * (size_t)P * n));
-  B200SV_CUDA(d_M.alloc(sizeof(cd) * (size_t)n * n * n));
-  B200SV_CUDA(d_L.alloc(sizeof(cd) * (size_t)n * n));
-  B200SV_CUDA(d_H.alloc(sizeof(cd) * n));
+  B200SV_CUDA(d_A.upload(cplx(A), (size_t)P * n));
+  B200SV_CUDA(d_M.upload(cplx(M), (size_t)n * n * n));
+  B200SV_CUDA(d_L.upload(cplx(L), (size_t)n * n));
+  B200SV_CUDA(d_H.upload(cplx(H), n));
   B200SV_CUDA(d_R.alloc(sizeof(cd) * (size_t)P * n));
-  B200SV_CUDA(cudaMemcpyAsync(d_A.p, A, sizeof(cd) * (size_t)P * n, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_M.p, M, sizeof(cd) * (size_t)n * n * n, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_L.p, L, sizeof(cd) * (size_t)n * n, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_H.p, H, sizeof(cd) * n, cudaMemcpyHostToDevice, st));
   ode_rhs_dense_kernel<<<(P * n + 127) / 128, 128, 0, st>>>(d_A.as<cd>(), P, n, d_M.as<cd>(), d_L.as<cd>(), d_H.as<cd>(), d_R.as<cd>());
   if (int rc = check_launch("ode_rhs_dense_kernel")) return rc;
-  B200SV_CUDA(cudaMemcpyAsync(rhs_out, d_R.p, sizeof(cd) * (size_t)P * n, cudaMemcpyDeviceToHost, st));
-  return sync.done();
+  B200SV_CUDA(d_R.download(cplx(rhs_out), (size_t)P * n));
+  return call.sync.done();
 }
 
 // compute_logsv_a_mgf_grid(is_analytic=True): the semi-analytic branch over a transform grid (affine_expansion.py:388-470 -> :306-384)
@@ -2490,31 +2381,14 @@ int b200sv_logsv_mgf_grid_analytic(const double* phi, const double* psi, int P, 
                                    int is_spot_measure, int expansion_order, int year_days, double* log_mgf_out) {
   B200SV_REQUIRE(phi && a_inout && params && log_mgf_out, "null pointer");
   B200SV_REQUIRE(P >= 1 && dtau > 0.0 && year_days >= 1, "P >= 1, dtau > 0, year_days >= 1");
-  if (expansion_order != B200SV_ORDER_FIRST && expansion_order != B200SV_ORDER_SECOND) return fail(-4, "expansion_order not implemented");
+  if (int rc = check_expansion_order(expansion_order)) return rc;
   const int N = expansion_order == B200SV_ORDER_FIRST ? 3 : 5;
   const LogsvModel model = make_model(*params, 1.0, is_spot_measure != 0);      // eta is ignored on this branch (reference :340-348)
-  cudaStream_t st = current_stream();
-  ensure_pool_threshold();
-  StreamSync sync(st);
-  DevBuf d_phi(st), d_psi(st), d_a0(st), d_a1(st), d_lm(st);
-  B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_psi.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_a0.alloc(sizeof(cd) * (size_t)P * N));
-  B200SV_CUDA(d_a1.alloc(sizeof(cd) * (size_t)P * N));
-  B200SV_CUDA(d_lm.alloc(sizeof(cd) * P));
-  B200SV_CUDA(cudaMemcpyAsync(d_phi.p, phi, sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  if (psi) B200SV_CUDA(cudaMemcpyAsync(d_psi.p, psi, sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_a0.p, a_inout, sizeof(cd) * (size_t)P * N, cudaMemcpyHostToDevice, st));
-  const cd* dpsi = psi ? d_psi.as<cd>() : nullptr;
-  const double y = params->sigma0 - params->theta;
-  if (N == 5)
-    logsv_mgf_analytic_kernel<5><<<(P + 63) / 64, 64, 0, st>>>(d_phi.as<cd>(), dpsi, P, model, dtau, year_days, d_a0.as<cd>(), d_a1.as<cd>(), d_lm.as<cd>(), y);
-  else
-    logsv_mgf_analytic_kernel<3><<<(P + 63) / 64, 64, 0, st>>>(d_phi.as<cd>(), dpsi, P, model, dtau, year_days, d_a0.as<cd>(), d_a1.as<cd>(), d_lm.as<cd>(), y);
-  if (int rc = check_launch("logsv_mgf_analytic_kernel")) return rc;
-  B200SV_CUDA(cudaMemcpyAsync(a_inout, d_a1.p, sizeof(cd) * (size_t)P * N, cudaMemcpyDeviceToHost, st));
-  B200SV_CUDA(cudaMemcpyAsync(log_mgf_out, d_lm.p, sizeof(cd) * P, cudaMemcpyDeviceToHost, st));
-  return sync.done();
+  return run_grid(phi, psi, P, a_inout, N, a_inout, log_mgf_out, [&](cudaStream_t st, const cd* ph, const cd* ps, const cd* a0, cd* a1, cd* lm) {
+    const auto analytic = N == 5 ? logsv_mgf_analytic_kernel<5> : logsv_mgf_analytic_kernel<3>;
+    analytic<<<(P + 63) / 64, 64, 0, st>>>(ph, ps, P, model, dtau, year_days, a0, a1, lm, params->sigma0 - params->theta);
+    return check_launch("logsv_mgf_analytic_kernel");
+  });
 }
 
 // compute_logsv_a_mgf_grid(is_stiff_solver=True): SciPy's BDF control law per grid point (affine_expansion.py:229-303)
@@ -2522,62 +2396,32 @@ int b200sv_logsv_mgf_grid_bdf(const double* phi, const double* psi, int P, doubl
                               double eta, int is_spot_measure, int expansion_order, double* log_mgf_out) {
   B200SV_REQUIRE(phi && a_inout && params && log_mgf_out, "null pointer");
   B200SV_REQUIRE(P >= 1 && dtau > 0.0, "P >= 1, dtau > 0");
-  if (expansion_order != B200SV_ORDER_FIRST && expansion_order != B200SV_ORDER_SECOND) return fail(-4, "expansion_order not implemented");
+  if (int rc = check_expansion_order(expansion_order)) return rc;
   const int N = expansion_order == B200SV_ORDER_FIRST ? 3 : 5;
   const LogsvModel model = make_model(*params, eta, is_spot_measure != 0);
-  cudaStream_t st = current_stream();
-  ensure_pool_threshold();
-  StreamSync sync(st);
-  DevBuf d_phi(st), d_psi(st), d_a0(st), d_a1(st), d_lm(st);
-  B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_psi.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_a0.alloc(sizeof(cd) * (size_t)P * N));
-  B200SV_CUDA(d_a1.alloc(sizeof(cd) * (size_t)P * N));
-  B200SV_CUDA(d_lm.alloc(sizeof(cd) * P));
-  B200SV_CUDA(cudaMemcpyAsync(d_phi.p, phi, sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  if (psi) B200SV_CUDA(cudaMemcpyAsync(d_psi.p, psi, sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_a0.p, a_inout, sizeof(cd) * (size_t)P * N, cudaMemcpyHostToDevice, st));
-  const cd* dpsi = psi ? d_psi.as<cd>() : nullptr;
-  const double y = params->sigma0 - params->theta;
-  if (N == 5)
-    logsv_mgf_bdf_kernel<5><<<(P + 63) / 64, 64, 0, st>>>(d_phi.as<cd>(), dpsi, P, model, dtau, d_a0.as<cd>(), d_a1.as<cd>(), d_lm.as<cd>(), y, nullptr);
-  else
-    logsv_mgf_bdf_kernel<3><<<(P + 63) / 64, 64, 0, st>>>(d_phi.as<cd>(), dpsi, P, model, dtau, d_a0.as<cd>(), d_a1.as<cd>(), d_lm.as<cd>(), y, nullptr);
-  if (int rc = check_launch("logsv_mgf_bdf_kernel")) return rc;
-  B200SV_CUDA(cudaMemcpyAsync(a_inout, d_a1.p, sizeof(cd) * (size_t)P * N, cudaMemcpyDeviceToHost, st));
-  B200SV_CUDA(cudaMemcpyAsync(log_mgf_out, d_lm.p, sizeof(cd) * P, cudaMemcpyDeviceToHost, st));
-  return sync.done();
+  return run_grid(phi, psi, P, a_inout, N, a_inout, log_mgf_out, [&](cudaStream_t st, const cd* ph, const cd* ps, const cd* a0, cd* a1, cd* lm) {
+    const auto bdf = N == 5 ? logsv_mgf_bdf_kernel<5> : logsv_mgf_bdf_kernel<3>;
+    bdf<<<(P + 63) / 64, 64, 0, st>>>(ph, ps, P, model, dtau, a0, a1, lm, params->sigma0 - params->theta, nullptr);
+    return check_launch("logsv_mgf_bdf_kernel");
+  });
 }
 
 int b200sv_heston_mgf_grid(const double* phi, const double* psi, int P, double dtau, double* a_inout, double* b_inout,
                            const b200sv_heston_params* params, double* log_mgf_out) {
   B200SV_REQUIRE(phi && a_inout && b_inout && params && log_mgf_out, "null pointer");
   B200SV_REQUIRE(P >= 1 && dtau > 0.0, "P >= 1, dtau > 0");
-  cudaStream_t st = current_stream();
-  ensure_pool_threshold();
-  StreamSync sync(st);
-  DevBuf d_phi(st), d_psi(st), d_dt(st), d_a(st), d_b(st), d_a1(st), d_b1(st), d_lm(st);
-  B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_psi.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_dt.alloc(sizeof(double)));
-  B200SV_CUDA(d_a.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_b.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_a1.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_b1.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_lm.alloc(sizeof(cd) * P));
-  B200SV_CUDA(cudaMemcpyAsync(d_phi.p, phi, sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  if (psi) B200SV_CUDA(cudaMemcpyAsync(d_psi.p, psi, sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_dt.p, &dtau, sizeof(double), cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_a.p, a_inout, sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_b.p, b_inout, sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  const int tpb = mgf_block_threads(P), nb = (P + tpb - 1) / tpb;
-  heston_mgf_kernel<<<nb, tpb, 0, st>>>(d_phi.as<cd>(), psi ? d_psi.as<cd>() : nullptr, P, 1, d_dt.as<double>(), *params,
-                                        d_a.as<cd>(), d_b.as<cd>(), d_a1.as<cd>(), d_b1.as<cd>(), d_lm.as<cd>());
-  if (int rc = check_launch("heston_mgf_kernel")) return rc;
-  B200SV_CUDA(cudaMemcpyAsync(a_inout, d_a1.p, sizeof(cd) * P, cudaMemcpyDeviceToHost, st));
-  B200SV_CUDA(cudaMemcpyAsync(b_inout, d_b1.p, sizeof(cd) * P, cudaMemcpyDeviceToHost, st));
-  B200SV_CUDA(cudaMemcpyAsync(log_mgf_out, d_lm.p, sizeof(cd) * P, cudaMemcpyDeviceToHost, st));
-  return sync.done();
+  return run_grid(phi, psi, P, a_inout, 1, a_inout, log_mgf_out, [&](cudaStream_t st, const cd* ph, const cd* ps, const cd* a0, cd* a1, cd* lm) {
+    DevBuf d_dt(st), d_b(st), d_b1(st);
+    B200SV_CUDA(d_dt.upload(&dtau, 1));
+    B200SV_CUDA(d_b.upload(cplx(b_inout), P));
+    B200SV_CUDA(d_b1.alloc(sizeof(cd) * P));
+    const int tpb = mgf_block_threads(P);
+    heston_mgf_kernel<<<(P + tpb - 1) / tpb, tpb, 0, st>>>(ph, ps, P, 1, d_dt.as<double>(), *params, a0, d_b.as<cd>(), a1, d_b1.as<cd>(), lm,
+                                                           nullptr, 0);
+    if (int rc = check_launch("heston_mgf_kernel")) return rc;
+    B200SV_CUDA(d_b1.download(cplx(b_inout), P));
+    return 0;
+  });
 }
 
 int b200sv_fourier_vanilla(const double* log_mgf, const double* phi, int P, double forward, const double* strikes,
@@ -2588,22 +2432,11 @@ int b200sv_fourier_vanilla(const double* log_mgf, const double* phi, int P, doub
   if (int rc = check_fourier_types(types, J, spot)) return rc;
   std::vector<StrikeSpec> ss(J);
   for (int j = 0; j < J; ++j) ss[j] = StrikeSpec{strikes[j], forward, discfactor, (int)types[j], 0, 1.0, 0};
-  cudaStream_t st = current_stream();
-  ensure_pool_threshold();
-  StreamSync sync(st);
-  DevBuf d_phi(st), d_lm(st), d_ss(st), d_pr(st);
-  B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_lm.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_ss.alloc(sizeof(StrikeSpec) * J));
-  B200SV_CUDA(d_pr.alloc(sizeof(double) * J));
-  B200SV_CUDA(cudaMemcpyAsync(d_phi.p, phi, sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_lm.p, log_mgf, sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_ss.p, ss.data(), sizeof(StrikeSpec) * J, cudaMemcpyHostToDevice, st));
-  fourier_vanilla_kernel<<<J, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_phi.as<cd>(), P, d_ss.as<StrikeSpec>(), spot ? 1 : 0,
-                                                        all_half_re(phi, P) ? 1 : 0, d_pr.as<double>());
-  if (int rc = check_launch("fourier_vanilla_kernel")) return rc;
-  B200SV_CUDA(cudaMemcpyAsync(prices_out, d_pr.p, sizeof(double) * J, cudaMemcpyDeviceToHost, st));
-  return sync.done();
+  const int half_re = all_half_re(phi, P) ? 1 : 0;
+  return run_sums(log_mgf, phi, P, ss, prices_out, [&](cudaStream_t st, unsigned n, const cd* lm, const cd* g, const StrikeSpec* s, double* pr) {
+    fourier_vanilla_kernel<<<n, kFourierThreads, 0, st>>>(lm, g, P, s, spot ? 1 : 0, half_re, pr, nullptr);
+    return check_launch("fourier_vanilla_kernel");
+  });
 }
 
 /* slice_pricer_with_mgf_grid_with_gamma (utils/mgf_pricer.py:273-320) on caller-supplied log-MGF / transform grids: 'C' / 'P' under the spot
@@ -2612,48 +2445,13 @@ int b200sv_fourier_gamma(const double* log_mgf, const double* phi, int P, double
                          double gamma_forward, const double* strikes, const int8_t* types, int J, int is_spot_measure, double* prices_out) {
   B200SV_REQUIRE(log_mgf && phi && strikes && types && prices_out, "null pointer");
   B200SV_REQUIRE(P >= 3 && J >= 1, "P >= 3, J >= 1");
-  if (!is_spot_measure) return fail(-5, "not implemented");
+  if (int rc = check_gamma_types(types, J, is_spot_measure != 0)) return rc;
   std::vector<StrikeSpec> ss(J);
-  for (int j = 0; j < J; ++j) {
-    if (types[j] != B200SV_CALL && types[j] != B200SV_PUT) return fail(-5, "not implemented");
-    ss[j] = StrikeSpec{strikes[j], forward, normalizer, (int)types[j], 0, gamma_forward, 0};
-  }
-  cudaStream_t st = current_stream();
-  ensure_pool_threshold();
-  StreamSync sync(st);
-  DevBuf d_phi(st), d_lm(st), d_ss(st), d_pr(st);
-  B200SV_CUDA(d_phi.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_lm.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_ss.alloc(sizeof(StrikeSpec) * J));
-  B200SV_CUDA(d_pr.alloc(sizeof(double) * J));
-  B200SV_CUDA(cudaMemcpyAsync(d_phi.p, phi, sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_lm.p, log_mgf, sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_ss.p, ss.data(), sizeof(StrikeSpec) * J, cudaMemcpyHostToDevice, st));
-  fourier_gamma_kernel<<<J, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_phi.as<cd>(), P, d_ss.as<StrikeSpec>(), risk_premia_gamma, d_pr.as<double>());
-  if (int rc = check_launch("fourier_gamma_kernel")) return rc;
-  B200SV_CUDA(cudaMemcpyAsync(prices_out, d_pr.p, sizeof(double) * J, cudaMemcpyDeviceToHost, st));
-  return sync.done();
-}
-
-// shared driver of the generic sums
-static int fourier_sum_host(const double* log_mgf, const double* grid, int P, const std::vector<SumSpec>& specs, int mode, int all_calls,
-                            double* out) {
-  const int J = (int)specs.size();
-  cudaStream_t st = current_stream();
-  ensure_pool_threshold();
-  StreamSync sync(st);
-  DevBuf d_g(st), d_lm(st), d_ss(st), d_pr(st);
-  B200SV_CUDA(d_g.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_lm.alloc(sizeof(cd) * P));
-  B200SV_CUDA(d_ss.alloc(sizeof(SumSpec) * J));
-  B200SV_CUDA(d_pr.alloc(sizeof(double) * J));
-  B200SV_CUDA(cudaMemcpyAsync(d_g.p, grid, sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_lm.p, log_mgf, sizeof(cd) * P, cudaMemcpyHostToDevice, st));
-  B200SV_CUDA(cudaMemcpyAsync(d_ss.p, specs.data(), sizeof(SumSpec) * J, cudaMemcpyHostToDevice, st));
-  fourier_sum_kernel<<<J, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_g.as<cd>(), P, d_ss.as<SumSpec>(), mode, all_calls, d_pr.as<double>());
-  if (int rc = check_launch("fourier_sum_kernel")) return rc;
-  B200SV_CUDA(cudaMemcpyAsync(out, d_pr.p, sizeof(double) * J, cudaMemcpyDeviceToHost, st));
-  return sync.done();
+  for (int j = 0; j < J; ++j) ss[j] = StrikeSpec{strikes[j], forward, normalizer, (int)types[j], 0, gamma_forward, 0};
+  return run_sums(log_mgf, phi, P, ss, prices_out, [&](cudaStream_t st, unsigned n, const cd* lm, const cd* g, const StrikeSpec* s, double* pr) {
+    fourier_gamma_kernel<<<n, kFourierThreads, 0, st>>>(lm, g, P, s, risk_premia_gamma, pr);
+    return check_launch("fourier_gamma_kernel");
+  });
 }
 
 int b200sv_fourier_qvar(const double* log_mgf, const double* psi, int P, double ttm, const double* strikes, const int8_t* types, int J,
