@@ -281,6 +281,16 @@ int b200sv_hawkesjd_price_chain(const b200sv_hawkes_params* params, int M, const
                                 const int* offsets, const double* strikes, const int8_t* types, int is_spot_measure, double vol_scaler, int P,
                                 double risk_premia_gamma, double* prices_out, double* a_out, double* log_mgf_out, double* normalizers_out,
                                 double* gamma_forwards_out);
+/* prices and forward-mode sensitivities of the Hawkes Fourier chain without a risk kernel (DESIGN.md §4.3).  Arguments as in
+ * b200sv_hawkesjd_price_chain; prices_out is bit-identical to it.  greeks_out [2 + 15][J], J = offsets[M]-offsets[0]: d price / d forwards[m],
+ * d^2 price / d forwards[m]^2, then d price / d parameter in the order sigma, shift_p, mean_p, shift_m, mean_m, lambda_p, theta_p, kappa_p,
+ * beta1_p, beta2_p, lambda_m, theta_m, kappa_m, beta1_m, beta2_m (mu does not enter the Fourier route; the compensators are differentiated
+ * through shift and mean; vol_scaler and discount factors held fixed).  Optional outputs (may be NULL): dlog_mgf_out [15][M][P] complex128
+ * interleaved; nfev_out [P], right-hand-side evaluations per grid point over the chain (the mesh the tangents were stepped on). */
+int b200sv_hawkesjd_price_chain_greeks(const b200sv_hawkes_params* params, int M, const double* ttms, const double* forwards,
+                                       const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
+                                       int is_spot_measure, double vol_scaler, int P, double* prices_out, double* greeks_out,
+                                       double* dlog_mgf_out, int* nfev_out);
 /* compute_hawkes_a_mgf_grid / solve_a_ode_grid (pricers/hawkes_jd_pricer.py:518-579) on caller-supplied transform grids (complex128 as interleaved
  * doubles; psi may be NULL = zeros): a_inout [P][3] holds A(0) on entry and A(dtau) on return, log_mgf_out [P] = a0 + a_p lambda_p + a_m lambda_m */
 int b200sv_hawkesjd_mgf_grid(const double* phi, const double* psi, int P, double dtau, double* a_inout, const b200sv_hawkes_params* params,

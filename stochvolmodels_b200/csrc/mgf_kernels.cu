@@ -986,18 +986,17 @@ __device__ __forceinline__ void rhs_tangent(const cd (&A)[N], const cd (&dA)[N],
 // The tangent of one parameter direction stepped on rk45_generic's attempts: dY_s = dy + h sum_j a_sj dK_j, dK_s = d f(Y_s), accepted
 // steps commit dy <- dy + h sum_j b_j dK_j and dK_0 <- dK_6 (FSAL).  dK: 8 "stages" in shared memory, 0..6 the stage tangents, 7 the
 // candidate dy of the current attempt.  dy stays in registers and carries over maturities like A.
-template <int N, int TPB>
-struct LogsvTangentHook {
-  const LogsvModel* m;
-  const CoefView<TPB>* c;
-  LogsvModelTangent dm;
-  CoefView<TPB> dc;
+// TanRhs: functor ``void operator()(const cd (&Y)[N], const cd (&dY)[N], cd (&out)[N]) const`` = J(Y) dY + d_p f(Y) of one direction
+// (LogsvTanRhsFn, HawkesTanRhsFn); the bookkeeping does not depend on it.
+template <int N, int TPB, typename TanRhs>
+struct TangentHook {
+  TanRhs f;
   StageStore<N, TPB> dK;        // StageStore indexes (stage * N + k) * TPB: 8 stages fit in 8 * N * TPB entries
   cd dy[N];
 
   __device__ __forceinline__ void eval(int s, const cd (&Y)[N], const cd (&dY)[N]) {
     cd o[N];
-    rhs_tangent<N, TPB>(Y, dY, *m, *c, dm, dc, o);
+    f(Y, dY, o);
 #pragma unroll
     for (int k = 0; k < N; ++k) dK.at(s, k) = o[k];
   }
@@ -1035,6 +1034,19 @@ struct LogsvTangentHook {
   }
 };
 
+template <int N, int TPB>
+struct LogsvTanRhsFn {
+  const LogsvModel* m;
+  const CoefView<TPB>* c;
+  LogsvModelTangent dm;
+  CoefView<TPB> dc;
+  __device__ __forceinline__ void operator()(const cd (&Y)[N], const cd (&dY)[N], cd (&out)[N]) const {
+    rhs_tangent<N, TPB>(Y, dY, *m, *c, dm, dc, out);
+  }
+};
+template <int N, int TPB>
+using LogsvTangentHook = TangentHook<N, TPB, LogsvTanRhsFn<N, TPB>>;
+
 constexpr int kTangentTPB = 16;      // shared memory per thread: 6N primal stages + 8N tangent stages + 2 x 14 coefficients
 
 // One thread = one (grid point, parameter direction): the primal integration of logsv_mgf_kernel (same rk45_generic, same mesh) plus one
@@ -1060,8 +1072,8 @@ __global__ void __launch_bounds__(kTangentTPB) logsv_mgf_tangent_kernel(const cd
   StageStore<N, TPB> K{stage_smem + threadIdx.x};
   const CoefView<TPB> c{coef_smem + threadIdx.x};
   LogsvTangentHook<N, TPB> tan;
-  tan.c = &c;
-  tan.dc = CoefView<TPB>{dcoef_smem + threadIdx.x};
+  tan.f.c = &c;
+  tan.f.dc = CoefView<TPB>{dcoef_smem + threadIdx.x};
   tan.dK = StageStore<N, TPB>{tan_smem + threadIdx.x};
   cd A[N];
 #pragma unroll
@@ -1078,9 +1090,9 @@ __global__ void __launch_bounds__(kTangentTPB) logsv_mgf_tangent_kernel(const cd
   for (int mm = 0; mm < M; ++mm) {
     const LogsvModel model = spec[mm].model;
     store_coef<TPB>(coef_smem + threadIdx.x, make_coef(model, ph, ps));
-    tan.m = &model;
-    tan.dm = dspec[mm * D + dir];
-    store_coef<TPB>(dcoef_smem + threadIdx.x, make_dcoef(model, tan.dm, ph, ps));
+    tan.f.m = &model;
+    tan.f.dm = dspec[mm * D + dir];
+    store_coef<TPB>(dcoef_smem + threadIdx.x, make_dcoef(model, tan.f.dm, ph, ps));
     int nfe = 0;
     st |= rk45_generic<N, TPB>(A, spec[mm].dtau, LogsvRhsFn<N, TPB>{model, c}, K, &nfe, &tan);
     nf += nfe;
@@ -1156,6 +1168,105 @@ __global__ void heston_mgf_tangent_kernel(const cd* __restrict__ phi, int P, int
     b = b_new;
     dlog_mgf[((size_t)(1 + dir) * M + mm) * P + p] = a.d + b.d * hp.v0;
     if (dir == 0) dlog_mgf[(size_t)mm * P + p] = b.v;
+  }
+}
+
+// ---- Hawkes jump-diffusion (DESIGN.md §4.3) ----
+// 15 parameters (HAWKES_GREEK_PARAMS: the HawkesJDParams fields without mu, which the Fourier route never reads, and risk_premia_gamma);
+// lambda_p / lambda_m enter only through log_mgf = a0 + a_p lambda_p + a_m lambda_m, the other 13 are ODE directions.
+constexpr int kHawkesGreekParams = 15;
+constexpr int kHawkesOdeDirs = 13;
+// row of dlog_mgf / greeks of ODE direction d (the two lambda rows, 5 and 10, are a_p and a_m)
+__host__ __device__ constexpr int hawkes_dir_row(int d) { return d < 5 ? d : d < 9 ? d + 1 : d + 2; }
+
+// d(HawkesMgfConsts field) / d(each ODE direction), built on the host: each direction is a HawkesMgfConsts of field derivatives.
+// comp = e^shift / (1 - mean) - 1 is derived: d comp / d shift = e^shift / (1 - mean), d comp / d mean = e^shift / (1 - mean)^2.
+struct HawkesTangentDirs {
+  HawkesMgfConsts d[kHawkesOdeDirs];
+};
+
+static HawkesTangentDirs make_hawkes_tangents(const b200sv_hawkes_params& p) {
+  HawkesTangentDirs t;
+  for (auto& d : t.d) d = HawkesMgfConsts{0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+  const double ep = std::exp(p.shift_p) / (1.0 - p.mean_p), em = std::exp(p.shift_m) / (1.0 - p.mean_m);
+  t.d[0].sigma2 = 2.0 * p.sigma;                                     // sigma
+  t.d[1].shift_p = 1.0, t.d[1].comp_p = ep;                          // shift_p
+  t.d[2].mean_p = 1.0, t.d[2].comp_p = ep / (1.0 - p.mean_p);        // mean_p
+  t.d[3].shift_m = 1.0, t.d[3].comp_m = em;                          // shift_m
+  t.d[4].mean_m = 1.0, t.d[4].comp_m = em / (1.0 - p.mean_m);        // mean_m
+  t.d[5].kt_p = p.kappa_p;                                           // theta_p
+  t.d[6].kappa_p = 1.0, t.d[6].kt_p = p.theta_p;                     // kappa_p
+  t.d[7].beta1_p = 1.0;                                              // beta1_p
+  t.d[8].beta2_p = 1.0;                                              // beta2_p
+  t.d[9].kt_m = p.kappa_m;                                           // theta_m
+  t.d[10].kappa_m = 1.0, t.d[10].kt_m = p.theta_m;                   // kappa_m
+  t.d[11].beta1_m = 1.0;                                             // beta1_m
+  t.d[12].beta2_m = 1.0;                                             // beta2_m
+  return t;
+}
+
+// d E(z) of the jump-size MGF E(z) = e^{-s z} / (1 + m z) along (dz, ds, dm):  E (-(s + m / (1 + m z)) dz - z ds - z / (1 + m z) dm)
+__device__ __forceinline__ cd hawkes_djump(cd z, cd dz, double s, double m, double ds, double dm) {
+  const cd r = mk(1.0) / (mk(1.0) + m * z);
+  const cd e = cexp_(-s * z) * r;
+  return e * (-((mk(s) + m * r) * dz) - z * (mk(ds) + dm * r));
+}
+
+// d f(A) = J(A) dA + d_p f(A) of HawkesRhsFn for one direction, d = d(consts)/d(direction)
+struct HawkesTanRhsFn {
+  const HawkesMgfConsts& c;
+  HawkesMgfConsts d;
+  cd phi, h0;              // h0 = (phi + 1) phi / 2 - psi: drift0 = sigma^2 h0
+  __device__ __forceinline__ void operator()(const cd (&A)[3], const cd (&dA)[3], cd (&out)[3]) const {
+    const cd zp = (phi - c.beta1_p * A[1]) - c.beta1_m * A[2], zm = (phi - c.beta2_p * A[1]) - c.beta2_m * A[2];
+    const cd dzp = -(((c.beta1_p * dA[1] + c.beta1_m * dA[2]) + d.beta1_p * A[1]) + d.beta1_m * A[2]);
+    const cd dzm = -(((c.beta2_p * dA[1] + c.beta2_m * dA[2]) + d.beta2_p * A[1]) + d.beta2_m * A[2]);
+    out[0] = (((c.kt_p * dA[1] + c.kt_m * dA[2]) + d.kt_p * A[1]) + d.kt_m * A[2]) + d.sigma2 * h0;
+    out[1] = (hawkes_djump(zp, dzp, c.shift_p, c.mean_p, d.shift_p, d.mean_p) - (c.kappa_p * dA[1] + d.kappa_p * A[1])) + d.comp_p * phi;
+    out[2] = (hawkes_djump(zm, dzm, c.shift_m, c.mean_m, d.shift_m, d.mean_m) - (c.kappa_m * dA[2] + d.kappa_m * A[2])) + d.comp_m * phi;
+  }
+};
+
+// hawkes_mgf_kernel in forward mode: one thread = one (grid point, ODE direction), the primal integration of hawkes_mgf_kernel (same
+// rk45_generic, same mesh) plus one tangent, A and dA carried over the maturities.  The 13 directions of a point are neighbouring threads,
+// so a warp runs few meshes.  Outputs: dlog_mgf [15][M][P] (HAWKES_GREEK_PARAMS order; rows 5 / 10 = a_p / a_m), log_mgf [M][P],
+// status [P], nfev [P] (each optional but dlog_mgf).
+template <int TPB>
+__global__ void __launch_bounds__(TPB) hawkes_mgf_tangent_kernel(const cd* __restrict__ phi, int P, int M, const double* __restrict__ dtaus,
+                                                                 HawkesMgfConsts c, HawkesTangentDirs dirs, cd* __restrict__ dlog_mgf,
+                                                                 cd* __restrict__ log_mgf, int* __restrict__ status, int* __restrict__ nfev) {
+  constexpr int D = kHawkesOdeDirs;
+  __shared__ cd stage_smem[6 * 3 * TPB];
+  __shared__ cd tan_smem[8 * 3 * TPB];
+  const int t = blockIdx.x * TPB + threadIdx.x;
+  if (t >= P * D) return;
+  const int p = t / D, dir = t % D;
+#pragma unroll
+  for (int i = 0; i < 18; ++i) stage_smem[threadIdx.x + i * TPB] = mk(0.0);
+#pragma unroll
+  for (int i = 0; i < 24; ++i) tan_smem[threadIdx.x + i * TPB] = mk(0.0);
+  StageStore<3, TPB> K{stage_smem + threadIdx.x};
+  const cd ph = phi[p];
+  const cd h0 = 0.5 * ((ph + mk(1.0)) * ph);
+  const HawkesRhsFn f{c, ph, c.sigma2 * h0};
+  TangentHook<3, TPB, HawkesTanRhsFn> tan{HawkesTanRhsFn{c, dirs.d[dir], ph, h0}, StageStore<3, TPB>{tan_smem + threadIdx.x}, {}};   // dy = 0
+  cd A[3] = {mk(0.0), mk(0.0), mk(0.0)};
+  const int row = hawkes_dir_row(dir);
+  int st = 0, nf = 0;
+  for (int m = 0; m < M; ++m) {
+    int nfe = 0;
+    st |= rk45_generic<3, TPB>(A, dtaus[m], f, K, &nfe, &tan);
+    nf += nfe;
+    dlog_mgf[((size_t)row * M + m) * P + p] = (tan.dy[0] + tan.dy[1] * c.lambda_p) + tan.dy[2] * c.lambda_m;
+    if (dir == 0) {
+      dlog_mgf[((size_t)5 * M + m) * P + p] = A[1];
+      dlog_mgf[((size_t)10 * M + m) * P + p] = A[2];
+      if (log_mgf) log_mgf[(size_t)m * P + p] = (A[0] + A[1] * c.lambda_p) + A[2] * c.lambda_m;
+    }
+  }
+  if (dir == 0) {
+    if (status) status[p] = st;
+    if (nfev) nfev[p] = nf;
   }
 }
 
@@ -1857,6 +1968,22 @@ static void launch_hawkes_mgf(cudaStream_t st, const cd* phi, const cd* psi, int
   k<<<(P + tpb - 1) / tpb, tpb, 0, st>>>(phi, psi, P, M, dtaus, c, a_in, a_out, lm, restart, nullptr);
 }
 
+// hawkes_mgf_tangent_kernel over the P * 13 (point, direction) threads; block size as for hawkes_mgf_kernel, from the threads in flight
+using HawkesTangentKernel = decltype(&hawkes_mgf_tangent_kernel<64>);
+static void launch_hawkes_mgf_tangent(cudaStream_t st, const cd* phi, int P, int M, const double* dtaus, const HawkesMgfConsts& c,
+                                      const HawkesTangentDirs& dirs, cd* dlm, cd* lm, int* nfev) {
+  const int n = P * kHawkesOdeDirs, tpb = mgf_block_threads(n);
+  HawkesTangentKernel k;
+  switch (tpb) {
+    case 4: k = hawkes_mgf_tangent_kernel<4>; break;
+    case 8: k = hawkes_mgf_tangent_kernel<8>; break;
+    case 16: k = hawkes_mgf_tangent_kernel<16>; break;
+    case 32: k = hawkes_mgf_tangent_kernel<32>; break;
+    default: k = hawkes_mgf_tangent_kernel<64>;
+  }
+  k<<<(n + tpb - 1) / tpb, tpb, 0, st>>>(phi, P, M, dtaus, c, dirs, dlm, lm, nullptr, nfev);
+}
+
 // ---- chain preparation ----
 // Default transform-grid scale when the caller passes vol_scaler <= 0; t0 is the first (shortest) maturity.
 static double default_vol_scaler(const b200sv_logsv_params& p, double t0) {      // logsv_pricer.py:664-666
@@ -2042,6 +2169,30 @@ static int queue_heston_prices(ChainDev& d, const FourierChain& c, const b200sv_
                                                                         d_hp.as<b200sv_heston_params>(), c.per_set_grid && c.batch ? c.P : 0);
   if (int rc = check_launch("heston_mgf_kernel")) return rc;
   return d.sums(c, prices_out, ivols_out);
+}
+
+// Validation of b200sv_hawkesjd_price_chain and its greeks: sizes, then the chain; the grid sits on Re = -1/2 - gamma (gamma = 0 without
+// the risk kernel) under both measures -- get_transform_var_grid's default is_spot_measure=True (hawkes_jd_pricer.py:385), real_phi (:451).
+static int prepare_hawkes_chain(FourierChain& c, const b200sv_hawkes_params* params, int M, const double* ttms, const double* forwards,
+                                const double* discfactors, const int* offsets, const double* strikes, const int8_t* types, int is_spot_measure,
+                                double vol_scaler, int P, double risk_premia_gamma) {
+  const bool with_gamma = risk_premia_gamma == risk_premia_gamma;
+  if (int rc = c.init(false, 1, M, P > 0 ? P : 500, offsets)) return rc;     // MAX_PHI, hawkes_jd_pricer.py:37
+  if (int rc = c.build(params, ttms, forwards, discfactors, offsets, strikes, types, is_spot_measure != 0,
+                       with_gamma ? ChainTypes::kGamma : ChainTypes::kFourier, vol_scaler))
+    return rc;
+  for (int i = 0; i < c.P; ++i) c.phi[2 * i] = with_gamma ? -0.5 - risk_premia_gamma : -0.5;
+  return 0;
+}
+
+// The Hawkes pricing launches of a prepared chain whose maturity increments are in d.dt (price and greeks routes): hawkes_mgf_kernel with
+// A carried over the maturities, then the sums (the gamma slice pricer when gamma is finite; c.ss then holds its normalisers / forwards).
+static int queue_hawkes_prices(ChainDev& d, const FourierChain& c, const HawkesMgfConsts& k, double* prices_out, double gamma = NAN) {
+  if (int rc = d.upload(c)) return rc;
+  B200SV_CUDA(d.a.alloc(sizeof(cd) * (size_t)c.M * c.P * 3));
+  launch_hawkes_mgf(d.st, d.phi.as<cd>(), nullptr, c.P, c.M, d.dt.as<double>(), k, nullptr, d.a.as<cd>(), d.lm.as<cd>(), 0);
+  if (int rc = check_launch("hawkes_mgf_kernel")) return rc;
+  return d.sums(c, prices_out, nullptr, gamma);
 }
 
 // Plumbing of the single-grid entry points: phi [P], psi [P] (when given) and a_in [P][n] (when given) go up, `launch` queues its
@@ -2242,13 +2393,10 @@ int b200sv_hawkesjd_price_chain(const b200sv_hawkes_params* params, int M, const
   B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out, "null pointer");
   const bool with_gamma = risk_premia_gamma == risk_premia_gamma;
   FourierChain c;
-  if (int rc = c.init(false, 1, M, P > 0 ? P : 500, offsets)) return rc;     // MAX_PHI, hawkes_jd_pricer.py:37
-  if (int rc = c.build(params, ttms, forwards, discfactors, offsets, strikes, types, is_spot_measure != 0,
-                       with_gamma ? ChainTypes::kGamma : ChainTypes::kFourier, vol_scaler))
+  if (int rc = prepare_hawkes_chain(c, params, M, ttms, forwards, discfactors, offsets, strikes, types, is_spot_measure, vol_scaler, P,
+                                    risk_premia_gamma))
     return rc;
   P = c.P;
-  for (int i = 0; i < P; ++i)        // get_transform_var_grid default is_spot_measure=True (:385); real_phi (:451)
-    c.phi[2 * i] = with_gamma ? -0.5 - risk_premia_gamma : -0.5;
   const HawkesMgfConsts k = make_hawkes_mgf_consts(*params);
   ChainDev d;
   std::vector<double> dts(c.dtaus);
@@ -2274,17 +2422,49 @@ int b200sv_hawkesjd_price_chain(const b200sv_hawkes_params* params, int M, const
       c.ss[j].ttm = gamma_forwards[c.ss[j].slice];
     }
   }
-  if (int rc = d.upload(c)) return rc;
-  B200SV_CUDA(d.a.alloc(sizeof(cd) * (size_t)M * P * 3));
-  launch_hawkes_mgf(d.st, d.phi.as<cd>(), nullptr, P, M, d.dt.as<double>(), k, nullptr, d.a.as<cd>(), d.lm.as<cd>(), 0);
-  if (int rc = check_launch("hawkes_mgf_kernel")) return rc;
-  if (int rc = d.sums(c, prices_out, nullptr, risk_premia_gamma)) return rc;
+  if (int rc = queue_hawkes_prices(d, c, k, prices_out, risk_premia_gamma)) return rc;
   B200SV_CUDA(d.a.download(cplx(a_out), (size_t)M * P * 3));
   B200SV_CUDA(d.lm.download(cplx(log_mgf_out), (size_t)M * P));
   if (int rc = d.sync.done()) return rc;
   if (normalizers_out) std::copy(normalizers.begin(), normalizers.end(), normalizers_out);
   if (gamma_forwards_out) std::copy(gamma_forwards.begin(), gamma_forwards.end(), gamma_forwards_out);
   return 0;
+}
+
+/* Forward-mode sensitivities of the Hawkes Fourier chain without a risk kernel (DESIGN.md §4.3): the pricing launches of
+ * b200sv_hawkesjd_price_chain (same function, so bit-identical prices), hawkes_mgf_tangent_kernel, then fourier_vanilla_greeks_kernel on the
+ * tangent kernel's own primal log-MGF; one synchronisation at the end. */
+int b200sv_hawkesjd_price_chain_greeks(const b200sv_hawkes_params* params, int M, const double* ttms, const double* forwards,
+                                       const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
+                                       int is_spot_measure, double vol_scaler, int P, double* prices_out, double* greeks_out,
+                                       double* dlog_mgf_out, int* nfev_out) {
+  B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && greeks_out, "null pointer");
+  FourierChain c;
+  if (int rc = prepare_hawkes_chain(c, params, M, ttms, forwards, discfactors, offsets, strikes, types, is_spot_measure, vol_scaler, P, NAN))
+    return rc;
+  constexpr int NP = kHawkesGreekParams;
+  P = c.P;
+  const HawkesMgfConsts k = make_hawkes_mgf_consts(*params);
+  ChainDev d;
+  B200SV_CUDA(d.dt.upload(c.dtaus.data(), c.dtaus.size()));
+  if (int rc = queue_hawkes_prices(d, c, k, prices_out)) return rc;
+  DevBuf d_dlm(d.st), d_lm(d.st), d_nfev(d.st), d_g(d.st);
+  B200SV_CUDA(d_dlm.alloc(sizeof(cd) * (size_t)NP * M * P));
+  B200SV_CUDA(d_lm.alloc(sizeof(cd) * (size_t)M * P));
+  B200SV_CUDA(d_nfev.alloc(sizeof(int) * P));
+  B200SV_CUDA(d_g.alloc(sizeof(double) * (size_t)(2 + NP) * c.ss.size()));
+  launch_hawkes_mgf_tangent(d.st, d.phi.as<cd>(), P, M, d.dt.as<double>(), k, make_hawkes_tangents(*params), d_dlm.as<cd>(), d_lm.as<cd>(),
+                            d_nfev.as<int>());
+  if (int rc = check_launch("hawkes_mgf_tangent_kernel")) return rc;
+  if (c.Jtot > 0) {       // the tangent kernel's own primal log-MGF, on the mesh the tangents were stepped on
+    fourier_vanilla_greeks_kernel<NP><<<c.Jtot, kFourierThreads, 0, d.st>>>(d_lm.as<cd>(), d_dlm.as<cd>(), d.phi.as<cd>(), P, M,
+                                                                            d.rows.as<StrikeSpec>(), c.spot ? 1 : 0, d_g.as<double>());
+    if (int rc = check_launch("fourier_vanilla_greeks_kernel")) return rc;
+    B200SV_CUDA(d_g.download(greeks_out, (size_t)(2 + NP) * c.Jtot));
+  }
+  B200SV_CUDA(d_dlm.download(cplx(dlog_mgf_out), (size_t)NP * M * P));
+  B200SV_CUDA(d_nfev.download(nfev_out, P));
+  return d.sync.done();
 }
 
 

@@ -97,6 +97,9 @@ def heston_mc_chain(params: C.HestonParamsC, ttms, forwards, discfactors, strike
 
 LOGSV_GREEK_PARAMS = ("sigma0", "theta", "kappa1", "kappa2", "beta", "volvol")
 HESTON_GREEK_PARAMS = ("v0", "theta", "kappa", "rho", "volvol")
+# HawkesJDParams fields in dataclass order without mu (the Fourier route never reads it) and risk_premia_gamma (not covered)
+HAWKES_GREEK_PARAMS = ("sigma", "shift_p", "mean_p", "shift_m", "mean_m", "lambda_p", "theta_p", "kappa_p", "beta1_p", "beta2_p",
+                       "lambda_m", "theta_m", "kappa_m", "beta1_m", "beta2_m")
 
 
 def _greeks_result(prices, stds, greeks, greeks_se, offsets):
@@ -487,6 +490,25 @@ def heston_price_chain_greeks(params: C.HestonParamsC, ttms, forwards, discfacto
            C.dptr(greeks), dlm.ctypes.data_as(C._dp) if return_grids else None)
     out = (C.split_chain(prices, offsets), greeks, offsets)
     return out + (dlm,) if return_grids else out
+
+
+def hawkesjd_price_chain_greeks(params: C.HawkesParamsC, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms,
+                                is_spot_measure: bool = True, vol_scaler: Optional[float] = None, max_phi: Optional[int] = None,
+                                return_grids: bool = False):
+    """Hawkes twin of logsv_price_chain_greeks without a risk kernel (b200sv_hawkesjd_price_chain_greeks): greeks rows = delta, gamma, then
+    HAWKES_GREEK_PARAMS; ``return_grids`` adds (dlog_mgf [15, M, P], nfev [P]).  P defaults to the route's 500 points."""
+    _check_fourier_types(optiontypes_ttms, is_spot_measure)
+    max_phi = int(max_phi) if max_phi else 500
+    M, ttms, forwards, discfactors, offsets, strikes, types = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
+    n = len(HAWKES_GREEK_PARAMS)
+    prices, greeks = np.empty(strikes.shape[0]), np.empty((2 + n, strikes.shape[0]))
+    dlm = np.empty((n, M, max_phi), dtype=np.complex128) if return_grids else None
+    nfev = np.empty(max_phi, dtype=np.int32) if return_grids else None
+    C.call("b200sv_hawkesjd_price_chain_greeks", byref(params), M, C.dptr(ttms), C.dptr(forwards), C.dptr(discfactors), C.iptr(offsets),
+           C.dptr(strikes), C.i8ptr(types), int(bool(is_spot_measure)), float(vol_scaler) if vol_scaler is not None else 0.0, max_phi,
+           C.dptr(prices), C.dptr(greeks), dlm.ctypes.data_as(C._dp) if return_grids else None, C.iptr(nfev) if return_grids else None)
+    out = (C.split_chain(prices, offsets), greeks, offsets)
+    return out + (dlm, nfev) if return_grids else out
 
 
 def logsv_price_chain_batch(params_list: Sequence[C.LogsvParamsC], ttms, forwards, discfactors, etas, strikes_ttms, optiontypes_ttms,

@@ -1,5 +1,5 @@
-"""Forward-mode sensitivities of the LogSV / Heston Fourier chain pricers (DESIGN.md §4.2): the result type and the checks shared by
-``LogSVPricer.price_chain_greeks`` and ``HestonPricer.price_chain_greeks``.
+"""Forward-mode sensitivities of the LogSV / Heston / Hawkes Fourier chain pricers (DESIGN.md §4.2, §4.3): the result type and the checks
+shared by ``LogSVPricer.price_chain_greeks``, ``HestonPricer.price_chain_greeks`` and ``HawkesJDPricer.price_chain_greeks``.
 
 One call returns, for every strike and maturity, the price (bit-identical to ``price_chain`` with the same arguments), delta and gamma
 with respect to the slice forward, and the derivative with respect to every model parameter.  The parameter sensitivities are the exact

@@ -1,11 +1,13 @@
 """Wall-clock of the forward-mode Fourier sensitivities against the alternative they replace: median of repeated calls after warm-up of
 price_chain, price_chain_greeks and the (2n + 1)-set central-difference batch (engine.*_price_chain_batch, grid pinned) on the BTC chain
-and BASELINE config 3 (5 maturities x 21 strikes), LogSV and Heston.  Prints the card and its power limit with the times.
+and BASELINE config 3 (5 maturities x 21 strikes), LogSV and Heston; Hawkes on the hawkes_fourier.npz and BTC chains against the 31
+sequential price_chain calls of central differences (grid pinned).  Prints the card and its power limit with the times.
 usage: python tools/bench_fourier_greeks.py [--reps 30]"""
 import argparse, os, subprocess, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
-from stochvolmodels_b200 import HestonParams, HestonPricer, LogSvParams, LogSVPricer, LOGSV_BTC_PARAMS, OptionChain, engine, get_btc_test_chain_data
+from stochvolmodels_b200 import (HawkesJDParams, HawkesJDPricer, HestonParams, HestonPricer, LogSvParams, LogSVPricer, LOGSV_BTC_PARAMS,
+                                 OptionChain, engine, get_btc_test_chain_data)
 
 ap = argparse.ArgumentParser()
 ap.add_argument("--reps", type=int, default=30)
@@ -70,4 +72,19 @@ for name, chain in (("heston btc 4x49", btc), ("heston c3 5x21", c3)):
     t_g = timed(lambda: pricer.price_chain_greeks(chain, hp))
     t_b = timed(batch)
     print(f"{name:16s} price_chain {t_p:7.3f} ms   price_chain_greeks {t_g:7.3f} ms   {len(sets)}-set central-difference batch {t_b:7.3f} ms",
+          flush=True)
+# Hawkes: there is no batch pricer, so the alternative is 2 x 15 + 1 sequential price_chain calls with vol_scaler pinned
+g = np.load(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden", "hawkes_fourier.npz"))
+hk_chain = OptionChain(ttms=g["ttms"], forwards=g["forwards"], strikes_ttms=[g["strikes"]] * 3, optiontypes_ttms=[g["types"]] * 3,
+                       discfactors=g["discfactors"])
+for name, chain in (("hawkes npz 3x5", hk_chain), ("hawkes btc 4x49", btc)):
+    pricer, kp = HawkesJDPricer(), HawkesJDParams()
+    vs = float(np.clip(kp.sigma, 0.2, 0.5) * np.sqrt(min(np.min(chain.ttms), 1.0 / 12.0)))
+    names = engine.HAWKES_GREEK_PARAMS
+    sets = [HawkesJDParams(**dict(zip(names, s)), mu=kp.mu) for s in bumped_sets([getattr(kp, n) for n in names])]
+    loop = lambda: [pricer.price_chain(chain, s, vol_scaler=vs) for s in sets]
+    t_p = timed(lambda: pricer.price_chain(chain, kp))
+    t_g = timed(lambda: pricer.price_chain_greeks(chain, kp))
+    t_b = timed(loop)
+    print(f"{name:16s} price_chain {t_p:7.3f} ms   price_chain_greeks {t_g:7.3f} ms   {len(sets)}-call central-difference loop {t_b:7.3f} ms",
           flush=True)
