@@ -186,15 +186,46 @@ def c128(a) -> np.ndarray:
 
 
 def dptr(a: np.ndarray):
+    """double* of a float64 array, or of a complex128 one (interleaved re, im); None -> NULL"""
     return a.ctypes.data_as(_dp) if a is not None else None
 
 
 def iptr(a: np.ndarray):
-    return a.ctypes.data_as(_ip)
+    """int* of an int32 array; None -> NULL"""
+    return a.ctypes.data_as(_ip) if a is not None else None
 
 
 def i8ptr(a: np.ndarray):
     return a.ctypes.data_as(_i8p)
+
+
+def seed64(seed) -> int:
+    """a Philox key as the library's uint64: Python ints of any sign or size wrap modulo 2^64"""
+    return int(seed) & 0xFFFFFFFFFFFFFFFF
+
+
+DEFAULT_VOL_SCALER = -1.0       # the Fourier chain entry points read every vol_scaler <= 0 as "the model's default transform grid"
+
+
+def vol_scaler_arg(vol_scaler) -> float:
+    return DEFAULT_VOL_SCALER if vol_scaler is None else float(vol_scaler)
+
+
+def batch_etas(etas, B: int, M: int):
+    """per-set vol backbones [B, M] as float64, or None (the library then uses ones)"""
+    if etas is None:
+        return None
+    etas = np.ascontiguousarray(etas, dtype=np.float64)
+    if etas.shape != (B, M):
+        raise ValueError(f"etas must have shape ({B}, {M})")
+    return etas
+
+
+def chain_ptrs(chain, *etas):
+    """the chain block of a chain entry point, (M, ttms, forwards, discfactors, [etas,] offsets, strikes, types), from engine._chain_arrays;
+    the LogSV entry points take their etas array (None -> NULL) between the discount factors and the offsets"""
+    return (chain.M, dptr(chain.ttms), dptr(chain.forwards), dptr(chain.discfactors), *(dptr(e) for e in etas), iptr(chain.offsets),
+            dptr(chain.strikes), i8ptr(chain.types))
 
 
 def encode_types(optiontypes) -> np.ndarray:

@@ -8,7 +8,7 @@ from __future__ import annotations
 import ctypes
 import os
 from ctypes import byref
-from typing import List, Optional, Sequence, Tuple
+from typing import List, NamedTuple, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -60,39 +60,66 @@ def heston_params_c(v0, theta, kappa, rho, volvol) -> C.HestonParamsC:
     return C.HestonParamsC(float(v0), float(theta), float(kappa), float(rho), float(volvol))
 
 
-def _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms):
+class _Chain(NamedTuple):
+    M: int
+    ttms: np.ndarray
+    forwards: np.ndarray
+    discfactors: np.ndarray
+    offsets: np.ndarray
+    strikes: np.ndarray
+    types: np.ndarray
+
+
+def _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms) -> _Chain:
     ttms, forwards, discfactors = C.f64(ttms), C.f64(forwards), C.f64(discfactors)
     M = ttms.shape[0]
     if not (forwards.shape[0] == discfactors.shape[0] == len(strikes_ttms) == len(optiontypes_ttms) == M):
         raise ValueError("ttms, forwards, discfactors, strikes_ttms, and optiontypes_ttms must have the same length")
     offsets, strikes, types = C.flatten_chain(strikes_ttms, optiontypes_ttms)
-    return M, ttms, forwards, discfactors, offsets, strikes, types
+    return _Chain(M, ttms, forwards, discfactors, offsets, strikes, types)
+
+
+def _backbone(etas, M: int):
+    """the etas slot of a single-set chain call: [vol backbone [M], ones when None] on the LogSV routes, [] (passed as ()) on the others"""
+    return [C.f64(np.ones(M) if e is None else e) for e in etas]
 
 
 # ---- Monte Carlo --------------------------------------------------------------------------------------------------------
+def _mc_chain(symbol: str, params, chain, etas, head, variable_type, seed: int, flags: int, tail=(), n_greeks: int = 0):
+    """the single-set chain MC entry points: C arguments (params, chain block, *head, variable type, seed, flags, *tail, prices, stds
+    [, greeks, greeks_se]).  ``etas`` = (LogSV vol backbone or None,) or ().  With ``n_greeks`` returns (prices, std errors,
+    greeks [1+P, J], greeks_se [1+P, J], offsets), else (prices, std errors)."""
+    vt = variable_code(variable_type)
+    ch = _chain_arrays(*chain)
+    etas = _backbone(etas, ch.M)
+    J = ch.strikes.shape[0]
+    prices, stds = np.empty(J), np.empty(J)
+    greeks = [np.empty((1 + n_greeks, J)), np.empty((1 + n_greeks, J))] if n_greeks else []
+    C.call(symbol, byref(params), *C.chain_ptrs(ch, *etas), *head, vt, C.seed64(seed), int(flags), *tail, C.dptr(prices), C.dptr(stds),
+           *map(C.dptr, greeks))
+    prices, stds = C.split_chain(prices, ch.offsets), C.split_chain(stds, ch.offsets)
+    return (prices, stds, *greeks, ch.offsets) if n_greeks else (prices, stds)
+
+
 def logsv_mc_chain(params: C.LogsvParamsC, ttms, forwards, discfactors, etas, strikes_ttms, optiontypes_ttms, nb_path: int,
                    nb_steps_per_year: int, is_spot_measure: bool, variable_type, seed: int, flags: int
                    ) -> Tuple[List[np.ndarray], List[np.ndarray]]:
-    vt = variable_code(variable_type)
-    M, ttms, forwards, discfactors, offsets, strikes, types = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
-    etas = C.f64(np.ones(M) if etas is None else etas)
-    prices, stds = np.empty(strikes.shape[0]), np.empty(strikes.shape[0])
-    C.call("b200sv_logsv_mc_chain", byref(params), M, C.dptr(ttms), C.dptr(forwards), C.dptr(discfactors), C.dptr(etas),
-           C.iptr(offsets), C.dptr(strikes), C.i8ptr(types), int(nb_path), int(nb_steps_per_year), int(bool(is_spot_measure)), vt,
-           int(seed) & 0xFFFFFFFFFFFFFFFF, int(flags), C.dptr(prices), C.dptr(stds))
-    return C.split_chain(prices, offsets), C.split_chain(stds, offsets)
+    return _mc_chain("b200sv_logsv_mc_chain", params, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms), (etas,),
+                     (int(nb_path), int(nb_steps_per_year), int(bool(is_spot_measure))), variable_type, seed, flags)
 
 
 def heston_mc_chain(params: C.HestonParamsC, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, nb_path: int,
                     nb_steps_per_year: int, variable_type, seed: int, flags: int, scheme: int = C.HESTON_EULER_FLOOR
                     ) -> Tuple[List[np.ndarray], List[np.ndarray]]:
-    vt = variable_code(variable_type)
-    M, ttms, forwards, discfactors, offsets, strikes, types = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
-    prices, stds = np.empty(strikes.shape[0]), np.empty(strikes.shape[0])
-    C.call("b200sv_heston_mc_chain", byref(params), M, C.dptr(ttms), C.dptr(forwards), C.dptr(discfactors), C.iptr(offsets),
-           C.dptr(strikes), C.i8ptr(types), int(nb_path), int(nb_steps_per_year), vt, int(seed) & 0xFFFFFFFFFFFFFFFF, int(flags),
-           int(scheme), C.dptr(prices), C.dptr(stds))
-    return C.split_chain(prices, offsets), C.split_chain(stds, offsets)
+    return _mc_chain("b200sv_heston_mc_chain", params, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms), (),
+                     (int(nb_path), int(nb_steps_per_year)), variable_type, seed, flags, (int(scheme),))
+
+
+def hawkesjd_mc_chain(params: C.HawkesParamsC, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, nb_path: int, variable_type,
+                      seed: int, flags: int) -> Tuple[List[np.ndarray], List[np.ndarray]]:
+    """chain MC of the Hawkes jump-diffusion (b200sv_hawkesjd_mc_chain; its time grid is fixed by the library)"""
+    return _mc_chain("b200sv_hawkesjd_mc_chain", params, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms), (), (int(nb_path),),
+                     variable_type, seed, flags)
 
 
 LOGSV_GREEK_PARAMS = ("sigma0", "theta", "kappa1", "kappa2", "beta", "volvol")
@@ -102,98 +129,69 @@ HAWKES_GREEK_PARAMS = ("sigma", "shift_p", "mean_p", "shift_m", "mean_m", "lambd
                        "lambda_m", "theta_m", "kappa_m", "beta1_m", "beta2_m")
 
 
-def _greeks_result(prices, stds, greeks, greeks_se, offsets):
-    """flat library outputs -> (prices, std errors, greeks [1+P, J], greeks_se [1+P, J], offsets)"""
-    return C.split_chain(prices, offsets), C.split_chain(stds, offsets), greeks, greeks_se, offsets
-
-
 def logsv_mc_chain_greeks(params: C.LogsvParamsC, ttms, forwards, discfactors, etas, strikes_ttms, optiontypes_ttms, nb_path: int,
                           nb_steps_per_year: int, is_spot_measure: bool, variable_type, seed: int, flags: int):
     """prices, std errors and pathwise sensitivities of the chain in one pass (b200sv_logsv_mc_chain_greeks).  Returns (prices, std errors,
     greeks [1+6, J], greeks_se [1+6, J], offsets): row 0 the forward delta, then LOGSV_GREEK_PARAMS; J runs over the flattened chain."""
-    vt = variable_code(variable_type)
-    M, ttms, forwards, discfactors, offsets, strikes, types = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
-    etas = C.f64(np.ones(M) if etas is None else etas)
-    J = strikes.shape[0]
-    prices, stds = np.empty(J), np.empty(J)
-    greeks, greeks_se = np.empty((1 + len(LOGSV_GREEK_PARAMS), J)), np.empty((1 + len(LOGSV_GREEK_PARAMS), J))
-    C.call("b200sv_logsv_mc_chain_greeks", byref(params), M, C.dptr(ttms), C.dptr(forwards), C.dptr(discfactors), C.dptr(etas),
-           C.iptr(offsets), C.dptr(strikes), C.i8ptr(types), int(nb_path), int(nb_steps_per_year), int(bool(is_spot_measure)), vt,
-           int(seed) & 0xFFFFFFFFFFFFFFFF, int(flags), C.dptr(prices), C.dptr(stds), C.dptr(greeks), C.dptr(greeks_se))
-    return _greeks_result(prices, stds, greeks, greeks_se, offsets)
+    return _mc_chain("b200sv_logsv_mc_chain_greeks", params, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms), (etas,),
+                     (int(nb_path), int(nb_steps_per_year), int(bool(is_spot_measure))), variable_type, seed, flags,
+                     n_greeks=len(LOGSV_GREEK_PARAMS))
 
 
 def heston_mc_chain_greeks(params: C.HestonParamsC, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, nb_path: int,
                            nb_steps_per_year: int, variable_type, seed: int, flags: int, scheme: int = C.HESTON_EULER_FLOOR):
     """Heston twin of logsv_mc_chain_greeks (b200sv_heston_mc_chain_greeks): greeks rows = forward delta, then HESTON_GREEK_PARAMS."""
-    vt = variable_code(variable_type)
-    M, ttms, forwards, discfactors, offsets, strikes, types = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
-    J = strikes.shape[0]
-    prices, stds = np.empty(J), np.empty(J)
-    greeks, greeks_se = np.empty((1 + len(HESTON_GREEK_PARAMS), J)), np.empty((1 + len(HESTON_GREEK_PARAMS), J))
-    C.call("b200sv_heston_mc_chain_greeks", byref(params), M, C.dptr(ttms), C.dptr(forwards), C.dptr(discfactors), C.iptr(offsets),
-           C.dptr(strikes), C.i8ptr(types), int(nb_path), int(nb_steps_per_year), vt, int(seed) & 0xFFFFFFFFFFFFFFFF, int(flags),
-           int(scheme), C.dptr(prices), C.dptr(stds), C.dptr(greeks), C.dptr(greeks_se))
-    return _greeks_result(prices, stds, greeks, greeks_se, offsets)
+    return _mc_chain("b200sv_heston_mc_chain_greeks", params, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms), (),
+                     (int(nb_path), int(nb_steps_per_year)), variable_type, seed, flags, (int(scheme),), n_greeks=len(HESTON_GREEK_PARAMS))
+
+
+def _tangent_terminal(symbol: str, params, ttm: float, nb_path: int, nb_steps_per_year: int, model_args, seed: int, flags: int,
+                      slice_index: int, path_offset: int, n_params: int):
+    out = [np.empty(nb_path) for _ in range(3)] + [np.empty((n_params, nb_path)) for _ in range(3)]
+    C.call(symbol, byref(params), float(ttm), int(nb_path), int(nb_steps_per_year), *model_args, C.seed64(seed), int(flags), int(slice_index),
+           int(path_offset), *map(C.dptr, out))
+    return tuple(out)
 
 
 def logsv_tangent_terminal(params: C.LogsvParamsC, ttm: float, nb_path: int, nb_steps_per_year: int, is_spot_measure: bool, eta: float,
                            seed: int, flags: int, slice_index: int = 0, path_offset: int = 0):
     """one slice of the tangent stepper from (0, sigma0, 0): (x, sigma, qvar, dx [6, n], dsigma [6, n], dqvar [6, n])"""
-    P = len(LOGSV_GREEK_PARAMS)
-    x, s, q = np.empty(nb_path), np.empty(nb_path), np.empty(nb_path)
-    dx, ds, dq = np.empty((P, nb_path)), np.empty((P, nb_path)), np.empty((P, nb_path))
-    C.call("b200sv_logsv_tangent_terminal", byref(params), float(ttm), int(nb_path), int(nb_steps_per_year), int(bool(is_spot_measure)),
-           float(eta), int(seed) & 0xFFFFFFFFFFFFFFFF, int(flags), int(slice_index), int(path_offset), C.dptr(x), C.dptr(s), C.dptr(q),
-           C.dptr(dx), C.dptr(ds), C.dptr(dq))
-    return x, s, q, dx, ds, dq
+    return _tangent_terminal("b200sv_logsv_tangent_terminal", params, ttm, nb_path, nb_steps_per_year, (int(bool(is_spot_measure)), float(eta)),
+                             seed, flags, slice_index, path_offset, len(LOGSV_GREEK_PARAMS))
 
 
 def heston_tangent_terminal(params: C.HestonParamsC, ttm: float, nb_path: int, nb_steps_per_year: int, seed: int, flags: int,
                             slice_index: int = 0, path_offset: int = 0):
     """one slice of the Heston tangent stepper from (0, v0, 0): (x, var, qvar, dx [5, n], dvar [5, n], dqvar [5, n])"""
-    P = len(HESTON_GREEK_PARAMS)
-    x, v, q = np.empty(nb_path), np.empty(nb_path), np.empty(nb_path)
-    dx, dv, dq = np.empty((P, nb_path)), np.empty((P, nb_path)), np.empty((P, nb_path))
-    C.call("b200sv_heston_tangent_terminal", byref(params), float(ttm), int(nb_path), int(nb_steps_per_year), int(seed) & 0xFFFFFFFFFFFFFFFF,
-           int(flags), int(slice_index), int(path_offset), C.dptr(x), C.dptr(v), C.dptr(q), C.dptr(dx), C.dptr(dv), C.dptr(dq))
-    return x, v, q, dx, dv, dq
+    return _tangent_terminal("b200sv_heston_tangent_terminal", params, ttm, nb_path, nb_steps_per_year, (), seed, flags, slice_index,
+                             path_offset, len(HESTON_GREEK_PARAMS))
+
+
+def _chain_batch(symbol: str, struct, params_list, chain, etas, args, n_out: int, with_ivols: bool):
+    """the batched chain entry points: C arguments (params [B], B, chain block with ``etas`` = (LogSV [B, M] or None,) or (), *args, n_out
+    outputs [B, J], ivols [B, J] | NULL) -> (*outputs, ivols | None)"""
+    ch = _chain_arrays(*chain)
+    B = len(params_list)
+    arr = (struct * B)(*params_list)
+    etas = [C.batch_etas(e, B, ch.M) for e in etas]
+    outs = [np.empty((B, ch.strikes.shape[0])) for _ in range(n_out)]
+    ivols = np.empty((B, ch.strikes.shape[0])) if with_ivols else None
+    C.call(symbol, arr, B, *C.chain_ptrs(ch, *etas), *args, *map(C.dptr, outs), C.dptr(ivols))
+    return (*outs, ivols)
 
 
 def logsv_mc_chain_batch(params_list: Sequence[C.LogsvParamsC], ttms, forwards, discfactors, etas, strikes_ttms, optiontypes_ttms,
                          nb_path: int, nb_steps_per_year: int, is_spot_measure: bool, seed: int, flags: int, with_ivols: bool = True):
     """B parameter sets through the fused chain MC on the SAME seed in one call -> (prices, std errors, ivols | None), each [B, J]."""
-    M, ttms, forwards, discfactors, offsets, strikes, types = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
-    B = len(params_list)
-    arr = (C.LogsvParamsC * B)(*params_list)
-    etas_c = None
-    if etas is not None:
-        etas_c = np.ascontiguousarray(etas, dtype=np.float64)
-        if etas_c.shape != (B, M):
-            raise ValueError(f"etas must have shape ({B}, {M})")
-    J = strikes.shape[0]
-    prices, stds = np.empty((B, J)), np.empty((B, J))
-    ivols = np.empty((B, J)) if with_ivols else None
-    C.call("b200sv_logsv_mc_chain_batch", arr, B, M, C.dptr(ttms), C.dptr(forwards), C.dptr(discfactors),
-           C.dptr(etas_c) if etas_c is not None else None, C.iptr(offsets), C.dptr(strikes), C.i8ptr(types), int(nb_path),
-           int(nb_steps_per_year), int(bool(is_spot_measure)), int(seed) & 0xFFFFFFFFFFFFFFFF, int(flags), C.dptr(prices), C.dptr(stds),
-           C.dptr(ivols) if with_ivols else None)
-    return prices, stds, ivols
+    return _chain_batch("b200sv_logsv_mc_chain_batch", C.LogsvParamsC, params_list, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms),
+                        (etas,), (int(nb_path), int(nb_steps_per_year), int(bool(is_spot_measure)), C.seed64(seed), int(flags)), 2, with_ivols)
 
 
 def heston_mc_chain_batch(params_list: Sequence[C.HestonParamsC], ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms,
                           nb_path: int, nb_steps_per_year: int, seed: int, flags: int, scheme: int = C.HESTON_EULER_FLOOR,
                           with_ivols: bool = True):
-    M, ttms, forwards, discfactors, offsets, strikes, types = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
-    B = len(params_list)
-    arr = (C.HestonParamsC * B)(*params_list)
-    J = strikes.shape[0]
-    prices, stds = np.empty((B, J)), np.empty((B, J))
-    ivols = np.empty((B, J)) if with_ivols else None
-    C.call("b200sv_heston_mc_chain_batch", arr, B, M, C.dptr(ttms), C.dptr(forwards), C.dptr(discfactors), C.iptr(offsets), C.dptr(strikes),
-           C.i8ptr(types), int(nb_path), int(nb_steps_per_year), int(seed) & 0xFFFFFFFFFFFFFFFF, int(flags), int(scheme), C.dptr(prices),
-           C.dptr(stds), C.dptr(ivols) if with_ivols else None)
-    return prices, stds, ivols
+    return _chain_batch("b200sv_heston_mc_chain_batch", C.HestonParamsC, params_list, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms),
+                        (), (int(nb_path), int(nb_steps_per_year), C.seed64(seed), int(flags), int(scheme)), 2, with_ivols)
 
 
 def rough_logsv_mc_chain(params_list, weights, nodes, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, nb_path: int, nsteps, hs,
@@ -202,7 +200,8 @@ def rough_logsv_mc_chain(params_list, weights, nodes, ttms, forwards, discfactor
     or [B, n]; ``Z0`` / ``Z1``: host unit normals [rows >= max(nsteps), nb_path] or None (in-kernel Philox draws).
     Returns (prices [B, J], std [B, J], ivols [B, J] | None, states [M, n + 2, nb_path] | None)."""
     vt = variable_code(variable_type)
-    M, ttms, forwards, discfactors, offsets, strikes, types = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
+    ch = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
+    M = ch.M
     B = len(params_list)
     arr = (C.LogsvParamsC * B)(*params_list)
     weights, nodes = np.atleast_2d(C.f64(weights)), np.atleast_2d(C.f64(nodes))
@@ -231,22 +230,20 @@ def rough_logsv_mc_chain(params_list, weights, nodes, ttms, forwards, discfactor
         if z_rows > int(nsteps.max()):          # the library uploads exactly max(nsteps) rows
             Z0, Z1 = np.ascontiguousarray(Z0[: int(nsteps.max())]), np.ascontiguousarray(Z1[: int(nsteps.max())])
             z_rows = int(nsteps.max())
-    J = strikes.shape[0]
+    J = ch.strikes.shape[0]
     prices, stds = np.empty((B, J)), np.empty((B, J))
     ivols = np.empty((B, J)) if with_ivols else None
     states = np.empty((M, n + 2, int(nb_path))) if return_states else None
-    C.call("b200sv_rough_logsv_mc_chain", arr, B, n, C.dptr(weights), C.dptr(nodes), M, C.dptr(ttms), C.dptr(forwards), C.dptr(discfactors),
-           C.iptr(offsets), C.dptr(strikes), C.i8ptr(types), int(nb_path), nsteps.ctypes.data_as(C._ip), C.dptr(hs),
-           C.dptr(Z0) if Z0 is not None else None, C.dptr(Z1) if Z1 is not None else None, int(z_rows), vt, int(seed) & 0xFFFFFFFFFFFFFFFF,
-           int(flags), C.dptr(prices), C.dptr(stds), C.dptr(ivols) if with_ivols else None, C.dptr(states) if return_states else None)
-    return prices, stds, ivols, states, offsets
+    C.call("b200sv_rough_logsv_mc_chain", arr, B, n, C.dptr(weights), C.dptr(nodes), *C.chain_ptrs(ch), int(nb_path), C.iptr(nsteps), C.dptr(hs),
+           C.dptr(Z0), C.dptr(Z1), int(z_rows), vt, C.seed64(seed), int(flags), C.dptr(prices), C.dptr(stds), C.dptr(ivols), C.dptr(states))
+    return prices, stds, ivols, states, ch.offsets
 
 
 def logsv_terminal(params: C.LogsvParamsC, ttm: float, nb_path: int, nb_steps_per_year: int, is_spot_measure: bool, eta: float,
                    seed: int, flags: int):
     x, s, q = np.empty(nb_path), np.empty(nb_path), np.empty(nb_path)
     C.call("b200sv_logsv_terminal", byref(params), float(ttm), int(nb_path), int(nb_steps_per_year), int(bool(is_spot_measure)),
-           float(eta), int(seed) & 0xFFFFFFFFFFFFFFFF, int(flags), C.dptr(x), C.dptr(s), C.dptr(q))
+           float(eta), C.seed64(seed), int(flags), C.dptr(x), C.dptr(s), C.dptr(q))
     return x, s, q
 
 
@@ -257,7 +254,7 @@ def logsv_terminal_from_state(params: C.LogsvParamsC, x0, sigma0, qvar0, ttm: fl
     if not (x.shape == s.shape == q.shape and x.ndim == 1):
         raise ValueError("x0, sigma0, qvar0 must be 1-d arrays of one length")
     C.call("b200sv_logsv_terminal_from_state", byref(params), float(ttm), int(x.shape[0]), int(nb_steps_per_year), int(bool(is_spot_measure)),
-           float(eta), int(seed) & 0xFFFFFFFFFFFFFFFF, int(flags), int(slice_index), C.dptr(x), C.dptr(s), C.dptr(q))
+           float(eta), C.seed64(seed), int(flags), int(slice_index), C.dptr(x), C.dptr(s), C.dptr(q))
     return x, s, q
 
 
@@ -271,8 +268,31 @@ def heston_terminal(params: C.HestonParamsC, ttm: float, nb_path: int, nb_steps_
                     scheme: int = C.HESTON_EULER_FLOOR):
     x, v, q = np.empty(nb_path), np.empty(nb_path), np.empty(nb_path)
     C.call("b200sv_heston_terminal", byref(params), float(ttm), int(nb_path), int(nb_steps_per_year),
-           int(seed) & 0xFFFFFFFFFFFFFFFF, int(flags), int(scheme), C.dptr(x), C.dptr(v), C.dptr(q))
+           C.seed64(seed), int(flags), int(scheme), C.dptr(x), C.dptr(v), C.dptr(q))
     return x, v, q
+
+
+def hawkesjd_terminal(params: C.HawkesParamsC, ttm: float, x, lambda_p, lambda_m, seed: int, flags: int, slice_index: int, per_path: bool):
+    """fused Philox stepper of the Hawkes jump-diffusion (b200sv_hawkesjd_terminal), in place on the float64 arrays (x, lambda_p, lambda_m);
+    without ``per_path`` every path starts from (0, params.lambda_p, params.lambda_m)"""
+    C.call("b200sv_hawkesjd_terminal", byref(params), float(ttm), int(x.shape[0]), C.seed64(seed), flags, int(slice_index), 1 if per_path else 0,
+           C.dptr(x), C.dptr(lambda_p), C.dptr(lambda_m))
+    return x, lambda_p, lambda_m
+
+
+def hawkesjd_step_fixed(x, lambda_p, lambda_m, blocks, nb_steps: int, nb_path: int, dt: float, params: C.HawkesParamsC):
+    """strict Hawkes stepper on caller-supplied draws ``blocks`` = (W0, U_P, U_M, J_P, J_M) (b200sv_hawkesjd_step_fixed), in place"""
+    C.call("b200sv_hawkesjd_step_fixed", C.dptr(x), C.dptr(lambda_p), C.dptr(lambda_m), *map(C.dptr, blocks), nb_steps, nb_path, dt,
+           byref(params))
+    return x, lambda_p, lambda_m
+
+
+def hawkesjd_device_draws(seed: int, path0: int, n: int, slice_index: int, nb_steps: int, dt: float, params: C.HawkesParamsC, flags: int):
+    """[W0, U_P, U_M, J_P, J_M], each [nb_steps, n]: what the Hawkes stepper draws in-kernel (b200sv_hawkesjd_device_draws)"""
+    out = [np.empty((nb_steps, n)) for _ in range(5)]
+    C.call("b200sv_hawkesjd_device_draws", C.seed64(seed), int(path0), int(n), int(slice_index), nb_steps, dt, byref(params), flags,
+           *map(C.dptr, out))
+    return out
 
 
 def _fixed_inputs(x0, v0, q0, W0, W1):
@@ -320,8 +340,7 @@ def mc_payoffs(x, qvar, ttm, forward, strikes, optiontypes, discfactor=1.0, vari
 
 def device_normals(seed: int, path0: int, n: int, slice_idx: int, nsteps: int, flags: int):
     z0, z1 = np.empty((nsteps, n)), np.empty((nsteps, n))
-    C.call("b200sv_device_normals", int(seed) & 0xFFFFFFFFFFFFFFFF, int(path0), int(n), int(slice_idx), int(nsteps), int(flags),
-           C.dptr(z0), C.dptr(z1))
+    C.call("b200sv_device_normals", C.seed64(seed), int(path0), int(n), int(slice_idx), int(nsteps), int(flags), C.dptr(z0), C.dptr(z1))
     return z0, z1
 
 
@@ -332,43 +351,36 @@ def debug_exp_pair(L):
     return out[0::2].copy(), out[1::2].copy()
 
 
-def _c128(a):
-    return np.ascontiguousarray(a, dtype=np.complex128)
-
-
 def logsv_ode_terms(phi_grid, psi_grid, params: C.LogsvParamsC, eta: float, is_spot_measure: bool, order: int):
     """dense (M [P,n,n,n], L [P,n,n], H [P,n]) of the coefficient ODEs over a transform grid (b200sv_logsv_ode_terms)."""
-    phi = _c128(np.atleast_1d(phi_grid))
-    psi = None if psi_grid is None else _c128(np.atleast_1d(psi_grid))
+    phi = C.c128(np.atleast_1d(phi_grid))
+    psi = None if psi_grid is None else C.c128(np.atleast_1d(psi_grid))
     P, n = phi.shape[0], (3 if order == 1 else 5)
     M, L, H = np.empty((P, n, n, n), np.complex128), np.empty((P, n, n), np.complex128), np.empty((P, n), np.complex128)
-    as_d = lambda a: a.view(np.float64).ctypes.data_as(C._dp)
-    C.call("b200sv_logsv_ode_terms", as_d(phi), as_d(psi) if psi is not None else None, P, byref(params), float(eta), int(bool(is_spot_measure)),
-           int(order), as_d(M), as_d(L), as_d(H))
+    C.call("b200sv_logsv_ode_terms", C.dptr(phi), C.dptr(psi), P, byref(params), float(eta), int(bool(is_spot_measure)),
+           int(order), C.dptr(M), C.dptr(L), C.dptr(H))
     return M, L, H
 
 
 def logsv_ode_rhs(phi_grid, psi_grid, A, params: C.LogsvParamsC, eta: float, is_spot_measure: bool, order: int):
     """right-hand side A'MA + LA + H at A [P, n] through the production device function (b200sv_logsv_ode_rhs)."""
-    phi, A = _c128(np.atleast_1d(phi_grid)), _c128(np.atleast_2d(A))
-    psi = None if psi_grid is None else _c128(np.atleast_1d(psi_grid))
+    phi, A = C.c128(np.atleast_1d(phi_grid)), C.c128(np.atleast_2d(A))
+    psi = None if psi_grid is None else C.c128(np.atleast_1d(psi_grid))
     out = np.empty_like(A)
-    as_d = lambda a: a.view(np.float64).ctypes.data_as(C._dp)
-    C.call("b200sv_logsv_ode_rhs", as_d(phi), as_d(psi) if psi is not None else None, phi.shape[0], as_d(A), byref(params), float(eta),
-           int(bool(is_spot_measure)), int(order), as_d(out))
+    C.call("b200sv_logsv_ode_rhs", C.dptr(phi), C.dptr(psi), phi.shape[0], C.dptr(A), byref(params), float(eta),
+           int(bool(is_spot_measure)), int(order), C.dptr(out))
     return out
 
 
 def ode_rhs_dense(A, M, L, H):
     """func_rhs with caller-supplied dense tensors: A [P, n] (or [n]) -> rhs of the same shape (b200sv_ode_rhs_dense)."""
-    A0 = _c128(A)
-    A2, M, L, H = np.atleast_2d(A0), _c128(M), _c128(L), _c128(H)
+    A0 = C.c128(A)
+    A2, M, L, H = np.atleast_2d(A0), C.c128(M), C.c128(L), C.c128(H)
     n = A2.shape[1]
     if M.shape != (n, n, n) or L.shape != (n, n) or H.shape != (n,):
         raise ValueError("M, L, H must have shapes (n, n, n), (n, n), (n,)")
     out = np.empty_like(A2)
-    as_d = lambda a: a.view(np.float64).ctypes.data_as(C._dp)
-    C.call("b200sv_ode_rhs_dense", as_d(A2), A2.shape[0], n, as_d(M), as_d(L), as_d(H), as_d(out))
+    C.call("b200sv_ode_rhs_dense", C.dptr(A2), A2.shape[0], n, C.dptr(M), C.dptr(L), C.dptr(H), C.dptr(out))
     return out.reshape(A0.shape)
 
 
@@ -413,44 +425,71 @@ def _check_qvar_types(optiontypes_ttms):
                 raise ValueError("not implemented")       # utils/mgf_pricer.py:349-358
 
 
+def _price_chain(symbol: str, params, chain, etas, is_spot_measure: bool, head, variable_type: int, vol_scaler, max_phi, return_grids: bool,
+                 coefs: Tuple[int, ...]):
+    """the fused Fourier chain entry points: C arguments (params, chain block, *head, vol_scaler, max_phi, prices[, a [M, P, n] for n in
+    ``coefs``], log_mgf [M, P])"""
+    if variable_type == C.Q_VAR:
+        _check_qvar_types(chain[4])
+    else:
+        _check_fourier_types(chain[4], is_spot_measure)
+    max_phi = int(max_phi) if max_phi else (40000 if variable_type == C.Q_VAR else 1000)
+    ch = _chain_arrays(*chain)
+    etas = _backbone(etas, ch.M)
+    prices = np.empty(ch.strikes.shape[0])
+    grids = [np.empty((ch.M, max_phi, n), dtype=np.complex128) if return_grids else None for n in coefs]
+    grids.append(np.empty((ch.M, max_phi), dtype=np.complex128) if return_grids else None)
+    C.call(symbol, byref(params), *C.chain_ptrs(ch, *etas), *head, C.vol_scaler_arg(vol_scaler), max_phi, C.dptr(prices), *map(C.dptr, grids))
+    out = C.split_chain(prices, ch.offsets)
+    return (out, *grids) if return_grids else out
+
+
 def logsv_price_chain(params: C.LogsvParamsC, ttms, forwards, discfactors, etas, strikes_ttms, optiontypes_ttms,
                       is_spot_measure: bool = True, expansion_order: int = C.ORDER_SECOND, vol_scaler: Optional[float] = None,
                       max_phi: Optional[int] = None, return_grids: bool = False, variable_type: int = C.LOG_RETURN):
-    if variable_type == C.Q_VAR:
-        _check_qvar_types(optiontypes_ttms)
-    else:
-        _check_fourier_types(optiontypes_ttms, is_spot_measure)
-    max_phi = int(max_phi) if max_phi else (40000 if variable_type == C.Q_VAR else 1000)
-    M, ttms, forwards, discfactors, offsets, strikes, types = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
-    etas = C.f64(np.ones(M) if etas is None else etas)
-    n = 3 if expansion_order == C.ORDER_FIRST else 5
-    prices = np.empty(strikes.shape[0])
-    a_out = np.empty((M, max_phi, n), dtype=np.complex128) if return_grids else None
-    lm_out = np.empty((M, max_phi), dtype=np.complex128) if return_grids else None
-    C.call("b200sv_logsv_price_chain", byref(params), M, C.dptr(ttms), C.dptr(forwards), C.dptr(discfactors), C.dptr(etas),
-           C.iptr(offsets), C.dptr(strikes), C.i8ptr(types), int(bool(is_spot_measure)), int(variable_type), int(expansion_order),
-           float(vol_scaler) if vol_scaler is not None else -1.0, int(max_phi), C.dptr(prices),
-           a_out.ctypes.data_as(C._dp) if return_grids else None, lm_out.ctypes.data_as(C._dp) if return_grids else None)
-    out = C.split_chain(prices, offsets)
-    return (out, a_out, lm_out) if return_grids else out
+    return _price_chain("b200sv_logsv_price_chain", params, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms), (etas,),
+                        is_spot_measure, (int(bool(is_spot_measure)), int(variable_type), int(expansion_order)), variable_type, vol_scaler,
+                        max_phi, return_grids, (3 if expansion_order == C.ORDER_FIRST else 5,))
 
 
 def heston_price_chain(params: C.HestonParamsC, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms,
                        vol_scaler: Optional[float] = None, max_phi: Optional[int] = None, return_grids: bool = False,
                        variable_type: int = C.LOG_RETURN):
-    if variable_type == C.Q_VAR:
-        _check_qvar_types(optiontypes_ttms)
-    else:
-        _check_fourier_types(optiontypes_ttms, True)
-    max_phi = int(max_phi) if max_phi else (40000 if variable_type == C.Q_VAR else 1000)
-    M, ttms, forwards, discfactors, offsets, strikes, types = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
-    prices = np.empty(strikes.shape[0])
-    lm_out = np.empty((M, max_phi), dtype=np.complex128) if return_grids else None
-    C.call("b200sv_heston_price_chain", byref(params), M, C.dptr(ttms), C.dptr(forwards), C.dptr(discfactors), C.iptr(offsets),
-           C.dptr(strikes), C.i8ptr(types), int(variable_type), float(vol_scaler) if vol_scaler is not None else -1.0, int(max_phi),
-           C.dptr(prices), lm_out.ctypes.data_as(C._dp) if return_grids else None)
-    out = C.split_chain(prices, offsets)
-    return (out, lm_out) if return_grids else out
+    return _price_chain("b200sv_heston_price_chain", params, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms), (), True,
+                        (int(variable_type),), variable_type, vol_scaler, max_phi, return_grids, ())
+
+
+def hawkesjd_price_chain(params: C.HawkesParamsC, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, is_spot_measure: bool,
+                         vol_scaler: Optional[float], max_phi: int, gamma: Optional[float], return_grids: bool = False):
+    """Fourier prices of the Hawkes chain (b200sv_hawkesjd_price_chain), under the risk kernel exp(-gamma x) unless ``gamma`` is None.
+    ``return_grids`` adds (a [M, P, 3], log_mgf [M, P], normalizers [M], gamma_forwards [M])."""
+    ch = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
+    prices = np.empty(ch.strikes.shape[0])
+    a = np.empty((ch.M, max_phi, 3), dtype=np.complex128) if return_grids else None
+    lm = np.empty((ch.M, max_phi), dtype=np.complex128) if return_grids else None
+    norm, gfw = np.empty(ch.M), np.empty(ch.M)
+    C.call("b200sv_hawkesjd_price_chain", byref(params), *C.chain_ptrs(ch), int(bool(is_spot_measure)), C.vol_scaler_arg(vol_scaler), max_phi,
+           float("nan") if gamma is None else float(gamma), C.dptr(prices), C.dptr(a), C.dptr(lm), C.dptr(norm), C.dptr(gfw))
+    out = C.split_chain(prices, ch.offsets)
+    return (out, a, lm, norm, gfw) if return_grids else out
+
+
+def _price_chain_greeks(symbol: str, params, chain, etas, is_spot_measure: bool, head, vol_scaler, max_phi: int, return_grids: bool, names,
+                        with_nfev: bool):
+    """the Fourier greeks entry points: C arguments (params, chain block, *head, vol_scaler, max_phi, prices, greeks [2 + P, J],
+    dlog_mgf [P, M, max_phi][, nfev [max_phi]]) -> (prices per maturity, greeks, offsets[, dlog_mgf[, nfev]])"""
+    _check_fourier_types(chain[4], is_spot_measure)
+    ch = _chain_arrays(*chain)
+    etas = _backbone(etas, ch.M)
+    n, J = len(names), ch.strikes.shape[0]
+    prices, greeks = np.empty(J), np.empty((2 + n, J))
+    grids = (np.empty((n, ch.M, max_phi), dtype=np.complex128) if return_grids else None,)
+    if with_nfev:
+        grids += (np.empty(max_phi, dtype=np.int32) if return_grids else None,)
+    C.call(symbol, byref(params), *C.chain_ptrs(ch, *etas), *head, C.vol_scaler_arg(vol_scaler), max_phi, C.dptr(prices), C.dptr(greeks),
+           C.dptr(grids[0]), *map(C.iptr, grids[1:]))
+    out = (C.split_chain(prices, ch.offsets), greeks, ch.offsets)
+    return out + grids if return_grids else out
 
 
 def logsv_price_chain_greeks(params: C.LogsvParamsC, ttms, forwards, discfactors, etas, strikes_ttms, optiontypes_ttms,
@@ -459,37 +498,17 @@ def logsv_price_chain_greeks(params: C.LogsvParamsC, ttms, forwards, discfactors
     """Fourier prices and forward-mode sensitivities of the chain (b200sv_logsv_price_chain_greeks).  Returns (prices per maturity,
     greeks [2 + 6, J], offsets) -- greeks rows: delta, gamma, then LOGSV_GREEK_PARAMS -- and with ``return_grids`` also
     (dlog_mgf [6, M, P], nfev [P])."""
-    _check_fourier_types(optiontypes_ttms, is_spot_measure)
-    max_phi = int(max_phi) if max_phi else 1000
-    M, ttms, forwards, discfactors, offsets, strikes, types = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
-    etas = C.f64(np.ones(M) if etas is None else etas)
-    n = len(LOGSV_GREEK_PARAMS)
-    prices, greeks = np.empty(strikes.shape[0]), np.empty((2 + n, strikes.shape[0]))
-    dlm = np.empty((n, M, max_phi), dtype=np.complex128) if return_grids else None
-    nfev = np.empty(max_phi, dtype=np.int32) if return_grids else None
-    C.call("b200sv_logsv_price_chain_greeks", byref(params), M, C.dptr(ttms), C.dptr(forwards), C.dptr(discfactors), C.dptr(etas),
-           C.iptr(offsets), C.dptr(strikes), C.i8ptr(types), int(bool(is_spot_measure)), C.LOG_RETURN, int(expansion_order),
-           float(vol_scaler) if vol_scaler is not None else -1.0, max_phi, C.dptr(prices), C.dptr(greeks),
-           dlm.ctypes.data_as(C._dp) if return_grids else None, C.iptr(nfev) if return_grids else None)
-    out = (C.split_chain(prices, offsets), greeks, offsets)
-    return out + (dlm, nfev) if return_grids else out
+    return _price_chain_greeks("b200sv_logsv_price_chain_greeks", params, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms), (etas,),
+                               is_spot_measure, (int(bool(is_spot_measure)), C.LOG_RETURN, int(expansion_order)), vol_scaler,
+                               int(max_phi or 1000), return_grids, LOGSV_GREEK_PARAMS, True)
 
 
 def heston_price_chain_greeks(params: C.HestonParamsC, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms,
                               vol_scaler: Optional[float] = None, max_phi: Optional[int] = None, return_grids: bool = False):
     """Heston twin of logsv_price_chain_greeks (b200sv_heston_price_chain_greeks): greeks rows = delta, gamma, then HESTON_GREEK_PARAMS;
     ``return_grids`` adds dlog_mgf [5, M, P]."""
-    _check_fourier_types(optiontypes_ttms, True)
-    max_phi = int(max_phi) if max_phi else 1000
-    M, ttms, forwards, discfactors, offsets, strikes, types = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
-    n = len(HESTON_GREEK_PARAMS)
-    prices, greeks = np.empty(strikes.shape[0]), np.empty((2 + n, strikes.shape[0]))
-    dlm = np.empty((n, M, max_phi), dtype=np.complex128) if return_grids else None
-    C.call("b200sv_heston_price_chain_greeks", byref(params), M, C.dptr(ttms), C.dptr(forwards), C.dptr(discfactors), C.iptr(offsets),
-           C.dptr(strikes), C.i8ptr(types), C.LOG_RETURN, float(vol_scaler) if vol_scaler is not None else -1.0, max_phi, C.dptr(prices),
-           C.dptr(greeks), dlm.ctypes.data_as(C._dp) if return_grids else None)
-    out = (C.split_chain(prices, offsets), greeks, offsets)
-    return out + (dlm,) if return_grids else out
+    return _price_chain_greeks("b200sv_heston_price_chain_greeks", params, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms), (),
+                               True, (C.LOG_RETURN,), vol_scaler, int(max_phi or 1000), return_grids, HESTON_GREEK_PARAMS, False)
 
 
 def hawkesjd_price_chain_greeks(params: C.HawkesParamsC, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms,
@@ -497,18 +516,9 @@ def hawkesjd_price_chain_greeks(params: C.HawkesParamsC, ttms, forwards, discfac
                                 return_grids: bool = False):
     """Hawkes twin of logsv_price_chain_greeks without a risk kernel (b200sv_hawkesjd_price_chain_greeks): greeks rows = delta, gamma, then
     HAWKES_GREEK_PARAMS; ``return_grids`` adds (dlog_mgf [15, M, P], nfev [P]).  P defaults to the route's 500 points."""
-    _check_fourier_types(optiontypes_ttms, is_spot_measure)
-    max_phi = int(max_phi) if max_phi else 500
-    M, ttms, forwards, discfactors, offsets, strikes, types = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
-    n = len(HAWKES_GREEK_PARAMS)
-    prices, greeks = np.empty(strikes.shape[0]), np.empty((2 + n, strikes.shape[0]))
-    dlm = np.empty((n, M, max_phi), dtype=np.complex128) if return_grids else None
-    nfev = np.empty(max_phi, dtype=np.int32) if return_grids else None
-    C.call("b200sv_hawkesjd_price_chain_greeks", byref(params), M, C.dptr(ttms), C.dptr(forwards), C.dptr(discfactors), C.iptr(offsets),
-           C.dptr(strikes), C.i8ptr(types), int(bool(is_spot_measure)), float(vol_scaler) if vol_scaler is not None else 0.0, max_phi,
-           C.dptr(prices), C.dptr(greeks), dlm.ctypes.data_as(C._dp) if return_grids else None, C.iptr(nfev) if return_grids else None)
-    out = (C.split_chain(prices, offsets), greeks, offsets)
-    return out + (dlm, nfev) if return_grids else out
+    return _price_chain_greeks("b200sv_hawkesjd_price_chain_greeks", params, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms), (),
+                               is_spot_measure, (int(bool(is_spot_measure)),), vol_scaler, int(max_phi or 500), return_grids,
+                               HAWKES_GREEK_PARAMS, True)
 
 
 def logsv_price_chain_batch(params_list: Sequence[C.LogsvParamsC], ttms, forwards, discfactors, etas, strikes_ttms, optiontypes_ttms,
@@ -516,39 +526,21 @@ def logsv_price_chain_batch(params_list: Sequence[C.LogsvParamsC], ttms, forward
                             max_phi: int = 1000, with_ivols: bool = True):
     """B parameter sets on one chain in one pass -> (prices [B, J], ivols [B, J] | None); ``etas`` is [B, M] or None."""
     _check_fourier_types(optiontypes_ttms, bool(is_spot_measure))
-    M, ttms, forwards, discfactors, offsets, strikes, types = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
-    B = len(params_list)
-    arr = (C.LogsvParamsC * B)(*params_list)
-    etas_c = None
-    if etas is not None:
-        etas_c = np.ascontiguousarray(etas, dtype=np.float64)
-        if etas_c.shape != (B, M):
-            raise ValueError(f"etas must have shape ({B}, {M})")
-    prices = np.empty((B, strikes.shape[0]))
-    ivols = np.empty((B, strikes.shape[0])) if with_ivols else None
-    C.call("b200sv_logsv_price_chain_batch", arr, B, M, C.dptr(ttms), C.dptr(forwards), C.dptr(discfactors),
-           C.dptr(etas_c) if etas_c is not None else None, C.iptr(offsets), C.dptr(strikes), C.i8ptr(types), int(bool(is_spot_measure)),
-           int(expansion_order), float(vol_scaler) if vol_scaler is not None else -1.0, int(max_phi), C.dptr(prices),
-           C.dptr(ivols) if with_ivols else None)
-    return prices, ivols
+    return _chain_batch("b200sv_logsv_price_chain_batch", C.LogsvParamsC, params_list, (ttms, forwards, discfactors, strikes_ttms,
+                        optiontypes_ttms), (etas,), (int(bool(is_spot_measure)), int(expansion_order), C.vol_scaler_arg(vol_scaler),
+                        int(max_phi)), 1, with_ivols)
 
 
 def heston_price_chain_batch(params_list: Sequence[C.HestonParamsC], ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms,
                              vol_scaler: Optional[float] = None, max_phi: int = 1000, with_ivols: bool = True):
     """B Heston parameter sets on one chain in one pass -> (prices [B, J], ivols [B, J] | None)."""
     _check_fourier_types(optiontypes_ttms, True)
-    M, ttms, forwards, discfactors, offsets, strikes, types = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
-    B = len(params_list)
-    arr = (C.HestonParamsC * B)(*params_list)
-    prices = np.empty((B, strikes.shape[0]))
-    ivols = np.empty((B, strikes.shape[0])) if with_ivols else None
-    C.call("b200sv_heston_price_chain_batch", arr, B, M, C.dptr(ttms), C.dptr(forwards), C.dptr(discfactors), C.iptr(offsets),
-           C.dptr(strikes), C.i8ptr(types), float(vol_scaler) if vol_scaler is not None else -1.0, int(max_phi), C.dptr(prices),
-           C.dptr(ivols) if with_ivols else None)
-    return prices, ivols
+    return _chain_batch("b200sv_heston_price_chain_batch", C.HestonParamsC, params_list, (ttms, forwards, discfactors, strikes_ttms,
+                        optiontypes_ttms), (), (C.vol_scaler_arg(vol_scaler), int(max_phi)), 1, with_ivols)
 
 
-def logsv_mgf_grid(phi, psi, dtau: float, a_t0, params: C.LogsvParamsC, eta: float, is_spot_measure: bool, expansion_order: int):
+def _logsv_mgf_grid(symbol: str, phi, psi, dtau: float, a_t0, params: C.LogsvParamsC, expansion_order: int, args):
+    """the three LogSV grid solvers: C arguments (phi, psi, P, dtau, a, params, *args, log_mgf) -> (a_t1 [P, n], log_mgf [P])"""
     phi = C.c128(phi)
     psi = C.c128(psi) if psi is not None else None
     P = phi.shape[0]
@@ -557,39 +549,25 @@ def logsv_mgf_grid(phi, psi, dtau: float, a_t0, params: C.LogsvParamsC, eta: flo
     if a.shape != (P, n):
         raise ValueError(f"a_t0 must have shape ({P}, {n})")
     lm = np.empty(P, dtype=np.complex128)
-    C.call("b200sv_logsv_mgf_grid", phi.ctypes.data_as(C._dp), psi.ctypes.data_as(C._dp) if psi is not None else None, P, float(dtau),
-           a.ctypes.data_as(C._dp), byref(params), float(eta), int(bool(is_spot_measure)), int(expansion_order), lm.ctypes.data_as(C._dp))
+    C.call(symbol, C.dptr(phi), C.dptr(psi), P, float(dtau), C.dptr(a), byref(params), *args, C.dptr(lm))
     return a, lm
+
+
+def logsv_mgf_grid(phi, psi, dtau: float, a_t0, params: C.LogsvParamsC, eta: float, is_spot_measure: bool, expansion_order: int):
+    return _logsv_mgf_grid("b200sv_logsv_mgf_grid", phi, psi, dtau, a_t0, params, expansion_order,
+                           (float(eta), int(bool(is_spot_measure)), int(expansion_order)))
 
 
 def logsv_mgf_grid_bdf(phi, psi, dtau: float, a_t0, params: C.LogsvParamsC, eta: float, is_spot_measure: bool, expansion_order: int):
     """stiff branch (is_stiff_solver=True: SciPy's BDF control law) over a transform grid: (a_t1 [P, n], log_mgf [P])"""
-    phi = C.c128(phi)
-    psi = C.c128(psi) if psi is not None else None
-    P = phi.shape[0]
-    n = 3 if expansion_order == C.ORDER_FIRST else 5
-    a = np.array(C.c128(a_t0), copy=True)
-    if a.shape != (P, n):
-        raise ValueError(f"a_t0 must have shape ({P}, {n})")
-    lm = np.empty(P, dtype=np.complex128)
-    C.call("b200sv_logsv_mgf_grid_bdf", phi.ctypes.data_as(C._dp), psi.ctypes.data_as(C._dp) if psi is not None else None, P, float(dtau),
-           a.ctypes.data_as(C._dp), byref(params), float(eta), int(bool(is_spot_measure)), int(expansion_order), lm.ctypes.data_as(C._dp))
-    return a, lm
+    return _logsv_mgf_grid("b200sv_logsv_mgf_grid_bdf", phi, psi, dtau, a_t0, params, expansion_order,
+                           (float(eta), int(bool(is_spot_measure)), int(expansion_order)))
 
 
 def logsv_mgf_grid_analytic(phi, psi, dtau: float, a_t0, params: C.LogsvParamsC, is_spot_measure: bool, expansion_order: int, year_days: int = 260):
     """semi-analytic branch (is_analytic=True) over a transform grid: (a_t1 [P, n], log_mgf [P])"""
-    phi = C.c128(phi)
-    psi = C.c128(psi) if psi is not None else None
-    P = phi.shape[0]
-    n = 3 if expansion_order == C.ORDER_FIRST else 5
-    a = np.array(C.c128(a_t0), copy=True)
-    if a.shape != (P, n):
-        raise ValueError(f"a_t0 must have shape ({P}, {n})")
-    lm = np.empty(P, dtype=np.complex128)
-    C.call("b200sv_logsv_mgf_grid_analytic", phi.ctypes.data_as(C._dp), psi.ctypes.data_as(C._dp) if psi is not None else None, P, float(dtau),
-           a.ctypes.data_as(C._dp), byref(params), int(bool(is_spot_measure)), int(expansion_order), int(year_days), lm.ctypes.data_as(C._dp))
-    return a, lm
+    return _logsv_mgf_grid("b200sv_logsv_mgf_grid_analytic", phi, psi, dtau, a_t0, params, expansion_order,
+                           (int(bool(is_spot_measure)), int(expansion_order), int(year_days)))
 
 
 def heston_mgf_grid(phi, psi, dtau: float, a_t0, b_t0, params: C.HestonParamsC):
@@ -599,9 +577,16 @@ def heston_mgf_grid(phi, psi, dtau: float, a_t0, b_t0, params: C.HestonParamsC):
     a = np.array(C.c128(a_t0), copy=True) if a_t0 is not None else np.zeros(P, dtype=np.complex128)
     b = np.array(C.c128(b_t0), copy=True) if b_t0 is not None else np.zeros(P, dtype=np.complex128)
     lm = np.empty(P, dtype=np.complex128)
-    C.call("b200sv_heston_mgf_grid", phi.ctypes.data_as(C._dp), psi.ctypes.data_as(C._dp) if psi is not None else None, P, float(dtau),
-           a.ctypes.data_as(C._dp), b.ctypes.data_as(C._dp), byref(params), lm.ctypes.data_as(C._dp))
+    C.call("b200sv_heston_mgf_grid", C.dptr(phi), C.dptr(psi), P, float(dtau), C.dptr(a), C.dptr(b), byref(params), C.dptr(lm))
     return lm, a, b
+
+
+def hawkesjd_mgf_grid(phi, psi, dtau: float, a, params: C.HawkesParamsC):
+    """Hawkes log-MGF over a transform grid (b200sv_hawkesjd_mgf_grid): complex128 ``a`` [P, 3] holds A(0) and receives A(dtau);
+    returns log_mgf [P]"""
+    lm = np.empty(phi.shape[0], dtype=np.complex128)
+    C.call("b200sv_hawkesjd_mgf_grid", C.dptr(phi), C.dptr(psi), phi.shape[0], float(dtau), C.dptr(a), byref(params), C.dptr(lm))
+    return lm
 
 
 def fourier_vanilla(log_mgf, phi, forward, strikes, optiontypes, discfactor=1.0, is_spot_measure=True):
@@ -610,7 +595,7 @@ def fourier_vanilla(log_mgf, phi, forward, strikes, optiontypes, discfactor=1.0,
     types = C.encode_types(optiontypes)
     J = strikes.shape[0]
     prices = np.empty(J)
-    C.call("b200sv_fourier_vanilla", log_mgf.ctypes.data_as(C._dp), phi.ctypes.data_as(C._dp), phi.shape[0], float(forward),
+    C.call("b200sv_fourier_vanilla", C.dptr(log_mgf), C.dptr(phi), phi.shape[0], float(forward),
            C.dptr(strikes), C.i8ptr(types), J, float(discfactor), int(bool(is_spot_measure)), C.dptr(prices))
     return prices
 
@@ -621,7 +606,7 @@ def fourier_gamma(log_mgf, phi, risk_premia_gamma, forward, normalizer, gamma_fo
     log_mgf, phi, strikes = C.c128(log_mgf), C.c128(phi), C.f64(strikes)
     types = C.encode_types(optiontypes)
     prices = np.empty(strikes.shape[0])
-    C.call("b200sv_fourier_gamma", log_mgf.ctypes.data_as(C._dp), phi.ctypes.data_as(C._dp), phi.shape[0], float(risk_premia_gamma), float(forward),
+    C.call("b200sv_fourier_gamma", C.dptr(log_mgf), C.dptr(phi), phi.shape[0], float(risk_premia_gamma), float(forward),
            float(normalizer), float(gamma_forward), C.dptr(strikes), C.i8ptr(types), strikes.shape[0], 1, C.dptr(prices))
     return prices
 
@@ -631,7 +616,7 @@ def fourier_qvar(log_mgf, psi, ttm, strikes, optiontypes, discfactor=1.0):
     log_mgf, psi, strikes = C.c128(log_mgf), C.c128(psi), C.f64(strikes)
     types = C.encode_types(optiontypes)
     prices = np.empty(strikes.shape[0])
-    C.call("b200sv_fourier_qvar", log_mgf.ctypes.data_as(C._dp), psi.ctypes.data_as(C._dp), psi.shape[0], float(ttm), C.dptr(strikes),
+    C.call("b200sv_fourier_qvar", C.dptr(log_mgf), C.dptr(psi), psi.shape[0], float(ttm), C.dptr(strikes),
            C.i8ptr(types), strikes.shape[0], float(discfactor), C.dptr(prices))
     return prices
 
@@ -639,7 +624,7 @@ def fourier_qvar(log_mgf, psi, ttm, strikes, optiontypes, discfactor=1.0):
 def fourier_pdf_sums(log_mgf, grid, z):
     log_mgf, grid, z = C.c128(log_mgf), C.c128(grid), C.f64(z)
     out = np.empty(z.shape[0])
-    C.call("b200sv_fourier_pdf", log_mgf.ctypes.data_as(C._dp), grid.ctypes.data_as(C._dp), grid.shape[0], C.dptr(z), z.shape[0], C.dptr(out))
+    C.call("b200sv_fourier_pdf", C.dptr(log_mgf), C.dptr(grid), grid.shape[0], C.dptr(z), z.shape[0], C.dptr(out))
     return out
 
 
@@ -650,21 +635,20 @@ def fourier_digital(log_mgf, phi, forward, strikes, optiontypes, discfactor=1.0)
     log_mgf, phi, strikes = C.c128(log_mgf), C.c128(phi), C.f64(strikes)
     types = C.encode_types(optiontypes)
     prices = np.empty(strikes.shape[0])
-    C.call("b200sv_fourier_digital", log_mgf.ctypes.data_as(C._dp), phi.ctypes.data_as(C._dp), phi.shape[0], float(forward), C.dptr(strikes),
+    C.call("b200sv_fourier_digital", C.dptr(log_mgf), C.dptr(phi), phi.shape[0], float(forward), C.dptr(strikes),
            C.i8ptr(types), strikes.shape[0], float(discfactor), C.dptr(prices))
     return prices
 
 
 def bsm_implied_vols(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, prices_ttms):
     """Black-76 implied vols of a whole chain in one kernel launch."""
-    M, ttms, forwards, discfactors, offsets, strikes, types = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
+    ch = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
     prices = C.f64(np.concatenate([np.asarray(p, dtype=np.float64).ravel() for p in prices_ttms]))
-    if prices.shape[0] != strikes.shape[0]:
+    if prices.shape[0] != ch.strikes.shape[0]:
         raise ValueError("model prices and strikes must have the same length")
-    ivols = np.empty(strikes.shape[0])
-    C.call("b200sv_bsm_implied_vols", M, C.dptr(ttms), C.dptr(forwards), C.dptr(discfactors), C.iptr(offsets), C.dptr(strikes),
-           C.i8ptr(types), C.dptr(prices), C.dptr(ivols))
-    return C.split_chain(ivols, offsets)
+    ivols = np.empty(ch.strikes.shape[0])
+    C.call("b200sv_bsm_implied_vols", *C.chain_ptrs(ch), C.dptr(prices), C.dptr(ivols))
+    return C.split_chain(ivols, ch.offsets)
 
 
 def infer_bsm_ivols_from_model_chain_prices(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, model_prices_ttms):
@@ -689,5 +673,5 @@ def logsv_vol_paths(params: C.LogsvParamsC, ttm: float, nb_path: int, nb_steps_p
             raise ValueError(f"brownians must have shape ({nb_steps}, {nb_path})")
     sigma_t = np.empty((nb_steps + 1, nb_path))
     C.call("b200sv_logsv_vol_paths", byref(params), float(ttm), int(nb_path), int(nb_steps_per_year), int(bool(is_spot_measure)),
-           int(seed) & 0xFFFFFFFFFFFFFFFF, C.dptr(brownians) if brownians is not None else None, C.dptr(sigma_t))
+           C.seed64(seed), C.dptr(brownians), C.dptr(sigma_t))
     return sigma_t, grid_t

@@ -22,6 +22,7 @@ from typing import Callable, List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import _capi as C
+from . import engine
 from .utils.funcs import set_time_grid
 
 
@@ -31,6 +32,52 @@ def shard_paths(nb_path: int, world_size: int, rank: int) -> Tuple[int, int]:
     n_local = base + (1 if rank < rem else 0)
     offset = rank * base + min(rank, rem)
     return n_local, offset
+
+
+def _shared_seed(seed) -> int:
+    """the Philox key of an MC call: the caller's ``seed``, or a fresh one -- which under a torch.distributed world must be the SAME on every rank
+    (sharded: one stream over all paths; replicated: identical prices everywhere), so rank 0 draws it and broadcasts"""
+    if seed is not None:
+        return int(seed)
+    value = engine.fresh_seed()
+    try:
+        import torch
+        import torch.distributed as dist
+    except Exception:
+        return value
+    if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+        device = "cuda" if dist.get_backend() == "nccl" else "cpu"
+        box = torch.tensor([value & 0x7FFFFFFFFFFFFFFF], dtype=torch.int64, device=device)
+        dist.broadcast(box, src=0)
+        value = int(box.item())
+    return value
+
+
+SHARD_MIN_PATHS = 500_000      # below this a chain call is launch-bound: one GPU prices it faster than N GPUs exchanging moments (r02 profile)
+
+
+def _use_distributed(kwargs) -> bool:
+    """shard this Monte Carlo call over the ranks of the initialised torch.distributed world?  Small calls (``nb_path`` < SHARD_MIN_PATHS, env
+    B200SV_SHARD_MIN_PATHS) are priced REPLICATED instead -- every rank runs all the paths on its own GPU through the single-launch chain
+    kernel and gets bit-identical prices (the Philox counter is the global path id), 0.17 ms against 0.53 ms sharded at 1e4 paths on 2 GPUs
+    (`profiles/r02_multi_gpu_latency.txt`).  Naming an ``exchange`` forces the sharded route."""
+    if not kwargs.get("distributed", True):
+        return False
+    try:
+        import torch.distributed as dist
+    except Exception:       # torch absent: single-process only
+        return False
+    if not (dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1):
+        return False
+    nb_path = kwargs.get("nb_path")
+    if nb_path is not None and kwargs.get("exchange") is None:
+        return int(nb_path) >= int(os.environ.get("B200SV_SHARD_MIN_PATHS", SHARD_MIN_PATHS))
+    return True
+
+
+def payoff_kinds(types: np.ndarray) -> int:
+    """the payoff-kind mask of one slice's int8 type codes that b200sv_dev_payoff_sums takes: 1 = a call or put, 2 = an inverse option"""
+    return int(np.bitwise_or.reduce(np.where(types >= 2, 2, 1)))
 
 
 # (group id, device index) -> (ctx, capacity): mailboxes are created once per process group and reused by every chain call, so that the
@@ -224,21 +271,22 @@ class CudaMcEngine:
             if self.p2p is not None:      # a rank without paths still takes part in the exchange
                 C.call("b200sv_dev_p2p_publish", self.p2p, c_void_p(self.moments.data_ptr()), 2, self._stream())
             return self.moments
+        seed = C.seed64(seed)
         if self.model == "logsv":
             C.call("b200sv_dev_logsv_slice", x, v, q, self.n_local, self.path_offset, int(init), byref(self.params_c), float(eta),
-                   int(bool(is_spot)), int(nsteps), float(dt), int(m), float(forward), int(seed) & 0xFFFFFFFFFFFFFFFF, self.flags,
+                   int(bool(is_spot)), int(nsteps), float(dt), int(m), float(forward), seed, self.flags,
                    c_void_p(self.moments.data_ptr()), self.p2p, self._stream())
         elif self.model == "hawkes":
             C.call("b200sv_dev_hawkesjd_slice", x, v, q, self.n_local, self.path_offset, int(init), byref(self.params_c), int(nsteps), float(dt),
-                   int(m), float(forward), int(seed) & 0xFFFFFFFFFFFFFFFF, self.flags, c_void_p(self.moments.data_ptr()), self.p2p, self._stream())
+                   int(m), float(forward), seed, self.flags, c_void_p(self.moments.data_ptr()), self.p2p, self._stream())
         elif self.model == "rough":       # every maturity restarts at t = 0 on its own grid: `init` and `m` do not enter
             w, nodes = self.factors
             C.call("b200sv_dev_rough_logsv_slice", x, c_void_p(self.state[1].data_ptr()), c_void_p(self.state[self.qrow].data_ptr()), self.n_local,
                    self.path_offset, byref(self.params_c), int(w.shape[0]), C.dptr(w), C.dptr(nodes), int(nsteps), float(dt), float(forward),
-                   int(seed) & 0xFFFFFFFFFFFFFFFF, self.flags, c_void_p(self.moments.data_ptr()), self.p2p, self._stream())
+                   seed, self.flags, c_void_p(self.moments.data_ptr()), self.p2p, self._stream())
         else:
             C.call("b200sv_dev_heston_slice", x, v, q, self.n_local, self.path_offset, int(init), byref(self.params_c), int(nsteps),
-                   float(dt), int(m), float(forward), int(seed) & 0xFFFFFFFFFFFFFFFF, self.flags, self.scheme,
+                   float(dt), int(m), float(forward), seed, self.flags, self.scheme,
                    c_void_p(self.moments.data_ptr()), self.p2p, self._stream())
         return self.moments
 
@@ -345,8 +393,8 @@ def mc_chain_distributed(model: str, params_c, ttms, forwards, discfactors, etas
             results.append((None, None))
             continue
         jo = int(offsets[m])
-        kinds = int(np.bitwise_or.reduce(np.where(types[jo: jo + J] >= 2, 2, 1)))
-        sums = eng.payoff_sums(float(ttms[m]), float(forwards[m]), strikes_dev[jo: jo + J], types_dev[jo: jo + J], J, variable_type, kinds)
+        sums = eng.payoff_sums(float(ttms[m]), float(forwards[m]), strikes_dev[jo: jo + J], types_dev[jo: jo + J], J, variable_type,
+                               payoff_kinds(types[jo: jo + J]))
         if world > 1 and not use_p2p:
             dist.all_reduce(sums, op=dist.ReduceOp.SUM, group=group)                 # exchange (2): 24*J bytes
         if chain_out:
@@ -380,3 +428,38 @@ def mc_chain_distributed(model: str, params_c, ttms, forwards, discfactors, etas
     if return_engine:
         return prices_out, stds_out, eng
     return prices_out, stds_out
+
+
+def _fixed_randoms_chain_device(rnd, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, params_c, etas,
+                                is_spot_measure, variable_type, fast=True):
+    """chain MC on the fixed unit normals of ``rnd`` (a logsv_pricer.DeviceRandoms, resident in HBM): strict stepper reading W from HBM,
+    re-centring moments, payoff sums, finalisation -- one stream, no host round trip until the prices are copied back."""
+    import torch
+    dev = rnd.device
+    n = rnd.nb_path
+    vt = engine.variable_code(variable_type)
+    offsets, strikes, types = C.flatten_chain(strikes_ttms, optiontypes_ttms)
+    with torch.cuda.device(dev):
+        state = torch.zeros((3, n), dtype=torch.float64, device=dev)
+        state[1].fill_(params_c.sigma0)
+        mom = torch.zeros(2, dtype=torch.float64, device=dev)
+        J_tot = int(offsets[-1])
+        sums = torch.zeros(3 * max(J_tot, 1), dtype=torch.float64, device=dev)
+        out = torch.zeros((2, max(J_tot, 1)), dtype=torch.float64, device=dev)
+        strikes_dev = torch.as_tensor(strikes).to(dev)
+        types_dev = torch.as_tensor(types).to(dev)
+        stream = c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        ptr = lambda t: c_void_p(t.data_ptr())
+        for m, ttm in enumerate(ttms):
+            W0, W1 = rnd.W0s[m], rnd.W1s[m]
+            C.call("b200sv_dev_logsv_step_fixed", ptr(state[0]), ptr(state[1]), ptr(state[2]), ptr(W0), ptr(W1), int(W0.shape[0]), n,
+                   rnd.dts[m], byref(params_c), float(etas[m]), int(bool(is_spot_measure)), int(bool(fast)), stream)
+            J, jo = int(offsets[m + 1] - offsets[m]), int(offsets[m])
+            if J == 0:
+                continue
+            C.call("b200sv_dev_spot_moments", ptr(state[0]), n, float(forwards[m]), ptr(mom), stream)
+            C.call("b200sv_dev_payoff_sums", ptr(state[0]), ptr(state[2]), n, 0, float(ttm), float(forwards[m]), ptr(strikes_dev[jo:]),
+                   ptr(types_dev[jo:]), J, vt, payoff_kinds(types[jo: jo + J]), ptr(mom), ptr(sums[3 * jo:]), None, stream)
+            C.call("b200sv_dev_payoff_finalize", ptr(sums[3 * jo:]), J, float(discfactors[m]), n, ptr(out[0, jo:]), ptr(out[1, jo:]), None, stream)
+        host = out.cpu().numpy()
+    return C.split_chain(host[0], offsets), C.split_chain(host[1], offsets)

@@ -234,7 +234,8 @@ def calibrate_logsv(pricer, option_chain, params0, params_min, params_max, is_ve
                     model_calibration_type: LogsvModelCalibrationType, constraints_type: ConstraintsType,
                     calibration_engine: CalibrationEngine, nb_path: int, nb_steps: int, seed: int, is_spot_measure: bool = True,
                     disp: bool = False, return_info: bool = False, fd_step: Optional[float] = None, mc_randoms: str = "numpy"):
-    from .logsv_pricer import (DeviceRandoms, _fixed_randoms_chain_device, _params_c, get_randoms_for_chain_valuation)
+    from ..multi_gpu import _fixed_randoms_chain_device
+    from .logsv_pricer import DeviceRandoms, _params_c, get_randoms_for_chain_valuation
     vol_scaler = pricer.set_vol_scaler(option_chain=option_chain)
     _, market_vols_ttms = option_chain.get_chain_data_as_xy()
     market_vols = to_flat_np_array(market_vols_ttms)

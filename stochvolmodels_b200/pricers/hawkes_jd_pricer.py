@@ -16,7 +16,6 @@ Fourier: the 3-equation Riccati system per transform point goes through the same
 """
 from __future__ import annotations
 
-from ctypes import byref
 from dataclasses import asdict, dataclass
 from typing import Any, Dict, List, Optional, Tuple
 
@@ -25,6 +24,7 @@ import numpy as np
 from .. import _capi as C
 from .. import engine
 from ..data.option_chain import OptionChain
+from ..multi_gpu import _shared_seed, _use_distributed, mc_chain_distributed
 from ..utils.config import VariableType
 from ..utils.funcs import set_time_grid, timer
 from .model_pricer import ModelParams, ModelPricer
@@ -199,19 +199,11 @@ def hawkesjd_mc_chain_pricer(ttms, forwards, discfactors, strikes_ttms, optionty
     the TOTAL path count, sharded over the ranks by global path id (the LogSV chain's two exchanges per maturity, multi_gpu.py)."""
     vt = engine.variable_code(variable_type)
     pc = _params_c(**locals())
-    from .logsv_pricer import _shared_seed, _use_distributed
     seed = _shared_seed(seed)
-    from .logsv_pricer import _use_distributed
     if _use_distributed({"distributed": distributed, "nb_path": nb_path, "exchange": exchange}):
-        from ..multi_gpu import mc_chain_distributed
-        C.encode_types(np.concatenate([np.asarray(t) for t in optiontypes_ttms]))
         return mc_chain_distributed("hawkes", pc, ttms, forwards, discfactors, None, strikes_ttms, optiontypes_ttms, nb_path, STEPS_PER_YEAR,
                                     True, vt, seed, engine.mc_flags("fp64", gauss), exchange=exchange)
-    M, ttms, forwards, discfactors, offsets, strikes, types = engine._chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
-    prices, stds = np.empty(strikes.shape[0]), np.empty(strikes.shape[0])
-    C.call("b200sv_hawkesjd_mc_chain", byref(pc), M, C.dptr(ttms), C.dptr(forwards), C.dptr(discfactors), C.iptr(offsets), C.dptr(strikes),
-           C.i8ptr(types), int(nb_path), vt, seed & 0xFFFFFFFFFFFFFFFF, engine.mc_flags("fp64", gauss), C.dptr(prices), C.dptr(stds))
-    return C.split_chain(prices, offsets), C.split_chain(stds, offsets)
+    return engine.hawkesjd_mc_chain(pc, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, nb_path, vt, seed, engine.mc_flags("fp64", gauss))
 
 
 def simulate_hawkesjd_terminal(ttm: float, x0: np.ndarray, lambda_p0: np.ndarray, lambda_m0: np.ndarray, mu: float, sigma: float, shift_p: float,
@@ -234,12 +226,10 @@ def simulate_hawkesjd_terminal(ttm: float, x0: np.ndarray, lambda_p0: np.ndarray
         blocks = [C.f64(b) for b in inputs]
         if len(blocks) != 5 or any(b.shape != (nb_steps, nb_path) for b in blocks):
             raise ValueError(f"inputs must be five arrays of shape ({nb_steps}, {nb_path})")
-        C.call("b200sv_hawkesjd_step_fixed", C.dptr(x), C.dptr(lp), C.dptr(lm), *[C.dptr(b) for b in blocks], nb_steps, nb_path, dt, byref(pc))
-        return x, lp, lm
+        return engine.hawkesjd_step_fixed(x, lp, lm, blocks, nb_steps, nb_path, dt, pc)
     const_start = x0.shape[0] == 1 and lambda_p0.shape[0] == 1 and lambda_m0.shape[0] == 1
-    C.call("b200sv_hawkesjd_terminal", byref(pc), float(ttm), int(nb_path), (engine.fresh_seed() if seed is None else int(seed)) & 0xFFFFFFFFFFFFFFFF,
-           engine.mc_flags("fp64", gauss), int(slice_index), 0 if const_start else 1, C.dptr(x), C.dptr(lp), C.dptr(lm))
-    return x, lp, lm
+    return engine.hawkesjd_terminal(pc, ttm, x, lp, lm, engine.fresh_seed() if seed is None else int(seed), engine.mc_flags("fp64", gauss),
+                                    slice_index, not const_start)
 
 
 def hawkesjd_device_draws(seed: int, path0: int, n: int, slice_index: int, ttm: float, gauss: str = "fp32", **params):
@@ -247,10 +237,7 @@ def hawkesjd_device_draws(seed: int, path0: int, n: int, slice_index: int, ttm: 
     reference's form (test / diagnostics hook)."""
     pc = _params_c(**{**{k: 0.0 for k in _KEYS}, **params})
     S, dt, _ = set_time_grid(ttm=ttm, nb_steps_per_year=STEPS_PER_YEAR)
-    out = [np.empty((S, n)) for _ in range(5)]
-    C.call("b200sv_hawkesjd_device_draws", int(seed) & 0xFFFFFFFFFFFFFFFF, int(path0), int(n), int(slice_index), S, dt, byref(pc),
-           engine.mc_flags("fp64", gauss), *[C.dptr(o) for o in out])
-    return (*out, dt)
+    return (*engine.hawkesjd_device_draws(seed, path0, n, slice_index, S, dt, pc, engine.mc_flags("fp64", gauss)), dt)
 
 
 MAX_PHI = 500           # transform grid size of the Fourier route (reference :37)
@@ -271,20 +258,10 @@ def _fourier_chain(model_params: HawkesJDParams, ttms, forwards, discfactors, st
         engine._check_fourier_types(optiontypes_ttms, bool(is_spot_measure))
     elif not is_spot_measure or any(str(t) not in ("C", "P") for types in optiontypes_ttms for t in types):
         raise ValueError("not implemented")           # utils/mgf_pricer.py:310-318
-    M, ttms, forwards, discfactors, offsets, strikes, types = engine._chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
     d = model_params.to_dict()
     d.pop("risk_premia_gamma", None)
-    pc = _params_c(**d)
-    prices = np.empty(strikes.shape[0])
-    a = np.empty((M, MAX_PHI, 3), dtype=np.complex128) if return_grids else None
-    lm = np.empty((M, MAX_PHI), dtype=np.complex128) if return_grids else None
-    norm, gfw = np.empty(M), np.empty(M)
-    cptr = lambda arr: None if arr is None else arr.ctypes.data_as(C._dp)
-    C.call("b200sv_hawkesjd_price_chain", byref(pc), M, C.dptr(ttms), C.dptr(forwards), C.dptr(discfactors), C.iptr(offsets), C.dptr(strikes),
-           C.i8ptr(types), int(bool(is_spot_measure)), float(vol_scaler) if vol_scaler is not None else 0.0, MAX_PHI,
-           float("nan") if gamma is None else float(gamma), C.dptr(prices), cptr(a), cptr(lm), C.dptr(norm), C.dptr(gfw))
-    out = C.split_chain(prices, offsets)
-    return (out, a, lm, norm, gfw) if return_grids else out
+    return engine.hawkesjd_price_chain(_params_c(**d), ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, is_spot_measure, vol_scaler,
+                                       MAX_PHI, gamma, return_grids)
 
 
 def hawkesjd_chain_pricer(model_params: HawkesJDParams, ttms: np.ndarray, forwards: np.ndarray, discfactors: np.ndarray, strikes_ttms, optiontypes_ttms,
@@ -330,10 +307,7 @@ def compute_hawkes_a_mgf_grid(ttm: float, phi_grid: np.ndarray, model_params: Ha
         raise ValueError("a_t0 must have shape (len(phi_grid), 3)")
     d = model_params.to_dict()
     d.pop("risk_premia_gamma", None)
-    lm = np.empty(phi.shape[0], dtype=np.complex128)
-    cp = lambda arr: None if arr is None else arr.ctypes.data_as(C._dp)
-    C.call("b200sv_hawkesjd_mgf_grid", cp(phi), cp(psi), phi.shape[0], float(ttm), cp(a), byref(_params_c(**d)), cp(lm))
-    return a, lm
+    return a, engine.hawkesjd_mgf_grid(phi, psi, ttm, a, _params_c(**d))
 
 
 def solve_a_ode_grid(phi_grid: np.ndarray, ttm: float, model_params: HawkesJDParams, psi_grid: Optional[np.ndarray] = None,

@@ -17,6 +17,7 @@ import numpy as np
 from .. import _capi as C
 from .. import engine
 from ..data.option_chain import OptionChain
+from ..multi_gpu import _shared_seed, _use_distributed, mc_chain_distributed
 from ..utils.config import VariableType
 from ..utils.funcs import timer
 from .model_pricer import ModelParams, ModelPricer
@@ -100,7 +101,6 @@ class HestonPricer(ModelPricer):
             raise NotImplementedError("model_mc_chain_greeks needs scheme='euler_floor'")
         vt = engine.variable_code(variable_type)
         flags = engine.mc_flags("fp64", kwargs.get("gauss", "fp32"))
-        from .logsv_pricer import _shared_seed
         res = engine.heston_mc_chain_greeks(_params_c(params.v0, params.theta, params.kappa, params.rho, params.volvol), option_chain.ttms,
                                             option_chain.forwards, option_chain.discfactors, option_chain.strikes_ttms,
                                             option_chain.optiontypes_ttms, nb_path, kwargs.get("nb_steps_per_year", 360), vt,
@@ -140,14 +140,10 @@ def heston_mc_chain_pricer(ttms, forwards, discfactors, strikes_ttms, optiontype
                            nb_steps_per_year: int = 360, seed: Optional[int] = None, precision: str = "fp64", gauss: str = "fp32",
                            distributed: bool = True, scheme="euler_floor", exchange: Optional[str] = None) -> Tuple[List[np.ndarray], List[np.ndarray]]:
     """chain MC under Heston (reference :285-331)."""
-    from .logsv_pricer import _use_distributed
     params_c = _params_c(v0, theta, kappa, rho, volvol)
     flags = engine.mc_flags(precision, gauss)
-    from .logsv_pricer import _shared_seed
     seed = _shared_seed(seed)
     if _use_distributed({"distributed": distributed, "nb_path": nb_path, "exchange": exchange}):
-        from ..multi_gpu import mc_chain_distributed
-        C.encode_types(np.concatenate([np.asarray(t) for t in optiontypes_ttms]))
         return mc_chain_distributed("heston", params_c, ttms, forwards, discfactors, None, strikes_ttms, optiontypes_ttms, nb_path,
                                     nb_steps_per_year, True, engine.variable_code(variable_type), seed, flags, scheme=_scheme_code(scheme), exchange=exchange)
     return engine.heston_mc_chain(params_c, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, nb_path, nb_steps_per_year,

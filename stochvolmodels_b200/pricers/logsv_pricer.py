@@ -26,6 +26,8 @@ import numpy as np
 from .. import _capi as C
 from .. import engine
 from ..data.option_chain import OptionChain
+from ..multi_gpu import CudaMcEngine, _fixed_randoms_chain_device, _shared_seed, _use_distributed, mc_chain_distributed, shard_paths
+from ..multi_gpu import SHARD_MIN_PATHS  # noqa: F401  (the MC routing policy lives in multi_gpu; this name stays importable from here)
 from ..utils.config import VariableType
 from ..utils.funcs import set_time_grid, timer
 from .calibration import CalibrationEngine, ConstraintsType, LogsvModelCalibrationType, calibrate_logsv
@@ -158,48 +160,6 @@ def _params_c(params) -> C.LogsvParamsC:
     return engine.logsv_params_c(params.sigma0, params.theta, params.kappa1, kappa2, params.beta, params.volvol)
 
 
-def _shared_seed(seed) -> int:
-    """the Philox key of an MC call: the caller's ``seed``, or a fresh one -- which under a torch.distributed world must be the SAME on every rank
-    (sharded: one stream over all paths; replicated: identical prices everywhere), so rank 0 draws it and broadcasts"""
-    if seed is not None:
-        return int(seed)
-    value = engine.fresh_seed()
-    try:
-        import torch
-        import torch.distributed as dist
-    except Exception:
-        return value
-    if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
-        device = "cuda" if dist.get_backend() == "nccl" else "cpu"
-        box = torch.tensor([value & 0x7FFFFFFFFFFFFFFF], dtype=torch.int64, device=device)
-        dist.broadcast(box, src=0)
-        value = int(box.item())
-    return value
-
-
-SHARD_MIN_PATHS = 500_000      # below this a chain call is launch-bound: one GPU prices it faster than N GPUs exchanging moments (r02 profile)
-
-
-def _use_distributed(kwargs) -> bool:
-    """shard this Monte Carlo call over the ranks of the initialised torch.distributed world?  Small calls (``nb_path`` < SHARD_MIN_PATHS, env
-    B200SV_SHARD_MIN_PATHS) are priced REPLICATED instead -- every rank runs all the paths on its own GPU through the single-launch chain
-    kernel and gets bit-identical prices (the Philox counter is the global path id), 0.17 ms against 0.53 ms sharded at 1e4 paths on 2 GPUs
-    (`profiles/r02_multi_gpu_latency.txt`).  Naming an ``exchange`` forces the sharded route."""
-    if not kwargs.get("distributed", True):
-        return False
-    try:
-        import torch.distributed as dist
-    except Exception:       # torch absent: single-process only
-        return False
-    if not (dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1):
-        return False
-    nb_path = kwargs.get("nb_path")
-    if nb_path is not None and kwargs.get("exchange") is None:
-        import os
-        return int(nb_path) >= int(os.environ.get("B200SV_SHARD_MIN_PATHS", SHARD_MIN_PATHS))
-    return True
-
-
 class LogSVPricer(ModelPricer):
     """ModelPricer for the log-normal SV model, Fourier + Monte Carlo routes on the GPU."""
 
@@ -322,7 +282,6 @@ class LogSVPricer(ModelPricer):
         path_range = kwargs.get("path_range")
         if path_range is None and _use_distributed(kwargs):
             import torch.distributed as dist
-            from ..multi_gpu import shard_paths
             n_local, offset = shard_paths(nb_path, dist.get_world_size(), dist.get_rank())
             path_range = (offset, n_local)
         if path_range is not None:
@@ -440,8 +399,6 @@ def logsv_mc_chain_pricer(ttms: np.ndarray, forwards: np.ndarray, discfactors: n
     flags = engine.mc_flags(precision, gauss)
     seed = _shared_seed(seed)
     if _use_distributed({"distributed": distributed, "nb_path": nb_path, "exchange": exchange}):
-        from ..multi_gpu import mc_chain_distributed
-        C.encode_types(np.concatenate([np.asarray(t) for t in optiontypes_ttms]))
         return mc_chain_distributed("logsv", params_c, ttms, forwards, discfactors, vol_backbone_etas, strikes_ttms,
                                     optiontypes_ttms, nb_path, nb_steps_per_year, is_spot_measure,
                                     engine.variable_code(variable_type), seed, flags, exchange=exchange)
@@ -460,7 +417,6 @@ def simulate_vol_paths(ttm: float, v0: float, theta: float, kappa1: float, kappa
 
 def _terminal_values_shard(params, ttm, offset, n_local, is_spot_measure, nb_steps_per_year, seed, gauss):
     """paths [offset, offset + n_local) of the global Philox stream on the current CUDA device (device-level slice call, state copied back)"""
-    from ..multi_gpu import CudaMcEngine
     if seed is None:
         raise ValueError("a sharded simulation needs an explicit seed (every rank must draw from the same stream)")
     if n_local == 0:
@@ -580,8 +536,6 @@ def rough_logsv_mc_chain_pricer_fixed_randoms(ttms, forwards, discfactors, strik
     hs = [float(np.asarray(g)[1] - np.asarray(g)[0]) for g in timegrids]             # split_simulation.py:346
     params_c = engine.logsv_params_c(sigma0, theta, kappa1, kappa2, beta, orthog_vol)
     if Z0 is None and not (return_states or debug) and _use_distributed({"distributed": distributed, "nb_path": nb_path, "exchange": exchange}):
-        from ..multi_gpu import mc_chain_distributed
-        C.encode_types(np.concatenate([np.asarray(t) for t in optiontypes_ttms]))
         return mc_chain_distributed("rough", params_c, ttms, forwards, discfactors, None, strikes_ttms, optiontypes_ttms, nb_path, 0, True,
                                     engine.variable_code(variable_type), _shared_seed(seed),
                                     engine.mc_flags("fp64", gauss), exchange=exchange, grid=list(zip(nsteps, hs)), factors=(weights, nodes),
@@ -597,43 +551,6 @@ def rough_logsv_mc_chain_pricer_fixed_randoms(ttms, forwards, discfactors, strik
             print(f"Mean spot Strand: {np.mean(np.exp(states[m, 0]))}, nan spots: {np.count_nonzero(np.isnan(states[m, 0]))}")
     out = (C.split_chain(prices[0], offsets), C.split_chain(stds[0], offsets))
     return out + (states,) if return_states else out
-
-
-def _fixed_randoms_chain_device(rnd: DeviceRandoms, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, params_c, etas,
-                                is_spot_measure, variable_type, fast=True):
-    """device-resident variant: strict stepper reading W from HBM, re-centring moments, payoff sums, finalisation -- one stream,
-    no host round trip until the prices are copied back."""
-    import torch
-    from ctypes import byref, c_void_p
-    dev = rnd.device
-    n = rnd.nb_path
-    vt = engine.variable_code(variable_type)
-    offsets, strikes, types = C.flatten_chain(strikes_ttms, optiontypes_ttms)
-    with torch.cuda.device(dev):
-        state = torch.zeros((3, n), dtype=torch.float64, device=dev)
-        state[1].fill_(params_c.sigma0)
-        mom = torch.zeros(2, dtype=torch.float64, device=dev)
-        J_tot = int(offsets[-1])
-        sums = torch.zeros(3 * max(J_tot, 1), dtype=torch.float64, device=dev)
-        out = torch.zeros((2, max(J_tot, 1)), dtype=torch.float64, device=dev)
-        strikes_dev = torch.as_tensor(strikes).to(dev)
-        types_dev = torch.as_tensor(types).to(dev)
-        stream = c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-        ptr = lambda t: c_void_p(t.data_ptr())
-        for m, ttm in enumerate(ttms):
-            W0, W1 = rnd.W0s[m], rnd.W1s[m]
-            C.call("b200sv_dev_logsv_step_fixed", ptr(state[0]), ptr(state[1]), ptr(state[2]), ptr(W0), ptr(W1), int(W0.shape[0]), n,
-                   rnd.dts[m], byref(params_c), float(etas[m]), int(bool(is_spot_measure)), int(bool(fast)), stream)
-            J, jo = int(offsets[m + 1] - offsets[m]), int(offsets[m])
-            if J == 0:
-                continue
-            C.call("b200sv_dev_spot_moments", ptr(state[0]), n, float(forwards[m]), ptr(mom), stream)
-            kinds = int(np.bitwise_or.reduce(np.where(types[jo: jo + J] >= 2, 2, 1)))
-            C.call("b200sv_dev_payoff_sums", ptr(state[0]), ptr(state[2]), n, 0, float(ttm), float(forwards[m]), ptr(strikes_dev[jo:]),
-                   ptr(types_dev[jo:]), J, vt, kinds, ptr(mom), ptr(sums[3 * jo:]), None, stream)
-            C.call("b200sv_dev_payoff_finalize", ptr(sums[3 * jo:]), J, float(discfactors[m]), n, ptr(out[0, jo:]), ptr(out[1, jo:]), None, stream)
-        host = out.cpu().numpy()
-    return C.split_chain(host[0], offsets), C.split_chain(host[1], offsets)
 
 
 def logsv_mc_chain_pricer_fixed_randoms(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, W0s, W1s=None, dts=None,

@@ -55,3 +55,17 @@ def test_product_never_imports_the_oracle():
             if f.endswith((".py", ".cu", ".cuh", ".h")):
                 text = open(os.path.join(dirpath, f)).read()
                 assert not re.search(r"^\s*(from|import)\s+oracle\b", text, flags=re.M), os.path.join(dirpath, f)
+
+
+def test_library_calls_stay_in_their_abi_modules():
+    """engine.py marshals the host-level entry points and multi_gpu.py the device-level ones; no other product module calls the library
+    or builds raw pointers."""
+    pkg = os.path.join(ROOT, "stochvolmodels_b200")
+    allowed = {os.path.join(pkg, f) for f in ("engine.py", "multi_gpu.py", "_capi.py")}
+    for dirpath, _, files in os.walk(pkg):
+        for f in files:
+            path = os.path.join(dirpath, f)
+            if f.endswith(".py") and path not in allowed:
+                text = open(path).read()
+                for pattern in ("C.call(", "_capi.call(", ".ctypes.data_as("):
+                    assert pattern not in text, f"{pattern} in {path}"

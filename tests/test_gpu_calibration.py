@@ -190,7 +190,8 @@ def test_logsv_calibration_mc_engine_recovers_own_market(cuda_lib):
     """MC engine with fixed device-resident normals (reference :251-266): calibrating to vols produced by the same normals recovers
     the generating beta / volvol."""
     from stochvolmodels_b200 import CalibrationEngine, LogSvParams, LogSVPricer, LogsvModelCalibrationType, OptionChain
-    from stochvolmodels_b200.pricers.logsv_pricer import (_fixed_randoms_chain_device, _params_c, get_randoms_for_chain_valuation)
+    from stochvolmodels_b200.multi_gpu import _fixed_randoms_chain_device
+    from stochvolmodels_b200.pricers.logsv_pricer import _params_c, get_randoms_for_chain_valuation
     ttms, fw = np.array([1.0 / 12.0, 0.25]), np.ones(2)
     truth = LogSvParams(sigma0=0.9, theta=1.0, kappa1=4.0, kappa2=4.0, beta=0.3, volvol=1.5)
     flat = OptionChain(ttms=ttms, forwards=fw, strikes_ttms=[K5, K5], optiontypes_ttms=[T5, T5], ids=np.array(["a", "b"]))

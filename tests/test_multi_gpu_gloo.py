@@ -150,11 +150,37 @@ def test_sharded_rough_chain_equals_unsharded_under_gloo():
             np.testing.assert_allclose(e[m], ee[m], rtol=1e-9, atol=1e-14)
 
 
+def _bad_code_worker(rank, world, port, out):
+    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
+    dist.init_process_group("gloo", rank=rank, world_size=world)
+    try:
+        from stochvolmodels_b200 import _capi as C, engine
+        from stochvolmodels_b200.multi_gpu import mc_chain_distributed
+        c, built = CASES["logsv"], []
+        try:
+            mc_chain_distributed("logsv", engine.logsv_params_c(*c["params"]), c["ttms"], c["fw"], c["df"], c["etas"], [K5, K5],
+                                 [c["types"][0], np.array(["P", "P", "X", "C", "C"])], N, NPY, c["spot"], C.LOG_RETURN, SEED, C.GAUSS_F64,
+                                 engine_factory=lambda *a, **k: built.append(a))
+            out[rank] = "accepted"
+        except ValueError as e:
+            out[rank] = (str(e), len(built))
+    finally:
+        dist.destroy_process_group()
+
+
+def test_unknown_payoff_code_raises_on_every_rank_before_any_engine():
+    """the sharded route validates the option types before it builds an engine (the pricers rely on it and do not check them first)"""
+    world, port = 2, _free_port()
+    out = mp.Manager().dict()
+    mp.spawn(_bad_code_worker, args=(world, port, out), nprocs=world, join=True)
+    assert dict(out) == {r: ("unknown option payoff code", 0) for r in range(world)}
+
+
 def _policy_worker(rank, world, port, out):
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
     dist.init_process_group("gloo", rank=rank, world_size=world)
     try:
-        from stochvolmodels_b200.pricers.logsv_pricer import SHARD_MIN_PATHS, _shared_seed, _use_distributed
+        from stochvolmodels_b200.multi_gpu import SHARD_MIN_PATHS, _shared_seed, _use_distributed
         out[rank] = dict(seed=_shared_seed(None), given=_shared_seed(42),
                          small=_use_distributed({"nb_path": SHARD_MIN_PATHS - 1}), large=_use_distributed({"nb_path": SHARD_MIN_PATHS}),
                          forced=_use_distributed({"nb_path": 10, "exchange": "collective"}), off=_use_distributed({"distributed": False, "nb_path": 10 ** 9}),
@@ -172,5 +198,5 @@ def test_shard_or_replicate_policy_and_shared_seed_under_gloo():
     assert out[0]["seed"] == out[1]["seed"] and out[0]["given"] == out[1]["given"] == 42
     for r in range(world):
         assert out[r]["small"] is False and out[r]["large"] is True and out[r]["forced"] is True and out[r]["off"] is False and out[r]["unknown"] is True
-    from stochvolmodels_b200.pricers.logsv_pricer import _use_distributed
+    from stochvolmodels_b200.multi_gpu import _use_distributed
     assert _use_distributed({"nb_path": 10 ** 9}) is False          # no process group: never sharded
