@@ -259,6 +259,21 @@ int b200sv_rough_logsv_mc_chain(const b200sv_logsv_params* params, int B, int n_
                                 long long z_rows, int variable_type, uint64_t seed, int flags, double* prices_out, double* stderr_out,
                                 double* ivols_out, double* states_out);
 
+/* The rough chain above for ONE parameter set, plus pathwise sensitivities in the same pass (DESIGN.md §3.10): prices and "std errors"
+ * as b200sv_rough_logsv_mc_chain on the same normals (discfactor * nanstd(payoff)), and greeks_out / greeks_se_out [1 + 6][J_total]: row 0
+ * the forward delta, then d price / d (sigma0, theta, kappa1, kappa2, beta, volvol) in struct field order (volvol = the orthogonal
+ * vol-of-vol), with real standard errors discfactor * std(g) / sqrt(nb_path).  weights / nodes [n_factors] are inputs, not differentiated.
+ * Optional (may be NULL): states_out [M][n_factors + 2][nb_path] as above, tangents_out [M][6][n_factors + 2][nb_path] = the same rows
+ * differentiated per parameter, resets_out [M] = the number of paths that took the reset-to-1e-6 branch at any step of maturity m's grid
+ * (the pathwise rows omit the mass such paths move across that switch).  fp64 state only (B200SV_STATE_F32 is rejected); synchronous on
+ * the library stream. */
+int b200sv_rough_logsv_mc_chain_greeks(const b200sv_logsv_params* params, int n_factors, const double* weights, const double* nodes, int M,
+                                       const double* ttms, const double* forwards, const double* discfactors, const int* offsets,
+                                       const double* strikes, const int8_t* types, long long nb_path, const int* nsteps, const double* hs,
+                                       const double* Z0, const double* Z1, long long z_rows, int variable_type, uint64_t seed, int flags,
+                                       double* prices_out, double* stderr_out, double* greeks_out, double* greeks_se_out, double* states_out,
+                                       double* tangents_out, double* resets_out);
+
 /* Hawkes jump-diffusion Monte Carlo (pricers/hawkes_jd_pricer.py): 1800 steps per year (:752), state (x, lambda_p, lambda_m).
  * b200sv_hawkesjd_mc_chain   = hawkesjd_mc_chain_pricer (:644-715): chained slices, forward-recentred payoffs on x; in-kernel draws (Philox;
  *                              flags = B200SV_GAUSS_* for the normals, the jump clocks and sizes come from 32-bit uniforms through fp64 logs).

@@ -1203,9 +1203,10 @@ __global__ void __launch_bounds__(kThreads) payoff_greeks_kernel(const double* _
   }
 }
 
-// prices / std errors exactly as payoff_finalize_kernel, plus greeks_out[k][Jtot] = df * mean(g_k), greeks_se = df * std(g_k) / sqrt(N)
-__global__ void greeks_finalize_kernel(const double* __restrict__ sums, int KV, int J, int Jtot, double discfactor, double total_paths,
-                                       double* __restrict__ prices, double* __restrict__ stderrs, double* __restrict__ greeks,
+// prices / std errors exactly as payoff_finalize_kernel (std / sqrt(price_paths)), plus greeks_out[k][Jtot] = df * mean(g_k),
+// greeks_se = df * std(g_k) / sqrt(total_paths).  The rough-vol route passes price_paths = 1 (its prices carry the plain std).
+__global__ void greeks_finalize_kernel(const double* __restrict__ sums, int KV, int J, int Jtot, double discfactor, double price_paths,
+                                       double total_paths, double* __restrict__ prices, double* __restrict__ stderrs, double* __restrict__ greeks,
                                        double* __restrict__ greeks_se) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= J) return;
@@ -1216,7 +1217,7 @@ __global__ void greeks_finalize_kernel(const double* __restrict__ sums, int KV, 
     const double mean = s1 / cnt;
     double var = s2 / cnt - mean * mean;
     var = var > 0.0 ? var : 0.0;
-    const double m = discfactor * mean, e = discfactor * sqrt(var) / sqrt(total_paths);
+    const double m = discfactor * mean, e = discfactor * sqrt(var) / sqrt(k < 0 ? price_paths : total_paths);
     if (k < 0) {
       prices[j] = m;
       stderrs[j] = e;
@@ -1875,8 +1876,8 @@ static int mc_chain_greeks_host(const Params& p, int M, const double* ttms, cons
     if (int rc = check_launch("payoff_greeks_kernel")) return rc;
     reduce_partials_kernel<<<1, 256, 0, st>>>(partials.as<double>(), g.blocks, Kpad, KV * J, d_sums.as<double>(), P2pPublish{});
     if (int rc = check_launch("reduce_partials_kernel")) return rc;
-    greeks_finalize_kernel<<<(J + 127) / 128, 128, 0, st>>>(d_sums.as<double>(), KV, J, Jalloc, discfactors[m], (double)nb_path, o_price + jo,
-                                                            o_se + jo, o_g + jo, o_gse + jo);
+    greeks_finalize_kernel<<<(J + 127) / 128, 128, 0, st>>>(d_sums.as<double>(), KV, J, Jalloc, discfactors[m], (double)nb_path, (double)nb_path,
+                                                            o_price + jo, o_se + jo, o_g + jo, o_gse + jo);
     if (int rc = check_launch("greeks_finalize_kernel")) return rc;
   }
   if (Jtot > 0) {
@@ -2365,6 +2366,20 @@ int b200sv_rough_logsv_mc_chain(const b200sv_logsv_params* params, int B, int n_
   B200SV_REQUIRE(params && weights && nodes && ttms && forwards && discfactors && offsets && nsteps && hs && prices_out && stderr_out, "null pointer");
   return rough_chain_host(params, B, n_factors, weights, nodes, M, ttms, forwards, discfactors, offsets, strikes, types, nb_path, nsteps, hs, Z0, Z1,
                           z_rows, variable_type, seed, flags, prices_out, stderr_out, ivols_out, states_out);
+}
+
+int b200sv_rough_logsv_mc_chain_greeks(const b200sv_logsv_params* params, int n_factors, const double* weights, const double* nodes, int M,
+                                       const double* ttms, const double* forwards, const double* discfactors, const int* offsets,
+                                       const double* strikes, const int8_t* types, long long nb_path, const int* nsteps, const double* hs,
+                                       const double* Z0, const double* Z1, long long z_rows, int variable_type, uint64_t seed, int flags,
+                                       double* prices_out, double* stderr_out, double* greeks_out, double* greeks_se_out, double* states_out,
+                                       double* tangents_out, double* resets_out) {
+  B200SV_REQUIRE(params && weights && nodes && ttms && forwards && discfactors && offsets && nsteps && hs && prices_out && stderr_out && greeks_out &&
+                     greeks_se_out,
+                 "null pointer");
+  return rough_chain_greeks_host(*params, n_factors, weights, nodes, M, ttms, forwards, discfactors, offsets, strikes, types, nb_path, nsteps, hs, Z0,
+                                 Z1, z_rows, variable_type, seed, flags, prices_out, stderr_out, greeks_out, greeks_se_out, states_out, tangents_out,
+                                 resets_out);
 }
 
 // ---- Hawkes jump-diffusion MC (hawkes_kernels.cuh) ---------------------------------------------------------------------------

@@ -14,6 +14,10 @@
 // normals per step in the fixed-random mode (16 B / path-step, coalesced [S][P] rows) or nothing at all in the Philox mode, plus the
 // terminal state.  ~160 fp64 instructions per step at n = 3 (8 RK4 slopes, one table exponential, one MUFU-seeded sqrt): fp64-pipe bound.
 // The reference kernels are compiled fastmath=True, so its own evaluation order is not fixed; agreement with it is 1e-12.
+//
+// Pathwise sensitivities (DESIGN.md §3.10): rough_logsv_tangent_kernel steps the same RoughPath through a hook that records the
+// intermediates its tangent needs, and carries per path dv[6][N], dls[6], dy[6] for (sigma0, theta, kappa1, kappa2, beta, orthog_vol);
+// the chain reuses payoff_greeks_kernel / greeks_finalize_kernel of mc_kernels.cu.  With the default hook the pricing kernel is unchanged.
 #pragma once
 
 namespace b200sv {
@@ -58,8 +62,18 @@ static RoughConsts make_rough_consts(const b200sv_logsv_params& p, int n, const 
   return c;
 }
 
+// Observer of RoughPath::step: receives the intermediates of the primal step that its tangent needs (rough_logsv_tangent_kernel).
+// The default observes nothing and compiles away, so the pricing kernel is the same machine code with or without this hook.
+struct RoughNoHook {
+  __device__ __forceinline__ void stage(int, double) {}                          // <w, z> at RK4 stage point k (0..3 first drift, 4..7 second)
+  __device__ __forceinline__ void diffusion(double, double, double, double) {}   // <w, u>, the log-normal exponent before / after clamp_log, e^ex
+  __device__ __forceinline__ void reset() {}                                     // the step took the reset-to-1e-6 branch
+  __device__ __forceinline__ void spot(double, double, double, double) {}        // vw, volw_h, term1, term2 of the log-spot increment
+};
+
 template <int N>
 struct RoughPath {
+  static constexpr bool kRedrawPair = false;     // rough_run_path keeps the second normal pair of a float-draw call in registers
   double v[N];
   double ls, y;
 
@@ -70,25 +84,28 @@ struct RoughPath {
     return s;
   }
   // slope of the drift ODE at z (split_simulation.py:100-103)
-  __device__ __forceinline__ static void slope(const RoughConsts& c, const double (&z)[N], double (&s)[N]) {
+  template <class Hook>
+  __device__ __forceinline__ static void slope(const RoughConsts& c, const double (&z)[N], double (&s)[N], Hook& hk, int k) {
     const double zw = wsum_of(c, z);
+    hk.stage(k, zw);
     const double g = (c.kappa1 + c.kappa2 * zw) * (c.theta - zw);
 #pragma unroll
     for (int i = 0; i < N; ++i) s[i] = fma(-c.nodes[i], z[i] - c.v0, g);
   }
-  // classical RK4 over a step of size hh (drift_ode_solve2, :76-124)
-  __device__ __forceinline__ static void drift(const RoughConsts& c, double (&z)[N], double hh) {
+  // classical RK4 over a step of size hh (drift_ode_solve2, :76-124); stages k0 .. k0 + 3 for the hook
+  template <class Hook>
+  __device__ __forceinline__ static void drift(const RoughConsts& c, double (&z)[N], double hh, Hook& hk, int k0) {
     double s1[N], s2[N], s3[N], s4[N], t[N];
-    slope(c, z, s1);
+    slope(c, z, s1, hk, k0);
 #pragma unroll
     for (int i = 0; i < N; ++i) t[i] = fma(0.5 * hh, s1[i], z[i]);
-    slope(c, t, s2);
+    slope(c, t, s2, hk, k0 + 1);
 #pragma unroll
     for (int i = 0; i < N; ++i) t[i] = fma(0.5 * hh, s2[i], z[i]);
-    slope(c, t, s3);
+    slope(c, t, s3, hk, k0 + 2);
 #pragma unroll
     for (int i = 0; i < N; ++i) t[i] = fma(hh, s3[i], z[i]);
-    slope(c, t, s4);
+    slope(c, t, s4, hk, k0 + 3);
 #pragma unroll
     for (int i = 0; i < N; ++i) z[i] = fma(hh / 6.0, (s1[i] + 2.0 * s2[i]) + (2.0 * s3[i] + s4[i]), z[i]);
   }
@@ -100,6 +117,11 @@ struct RoughPath {
   }
   // one time step (log_spot_full_solve2_f64, :287-337): z0 drives the volatility, z1 the orthogonal part of the spot
   __device__ __forceinline__ void step(const RoughConsts& c, double z0, double z1) {
+    RoughNoHook none;
+    step(c, z0, z1, none);
+  }
+  template <class Hook>
+  __device__ __forceinline__ void step(const RoughConsts& c, double z0, double z1, Hook& hk) {
     const double vw = wsum_of(c, v);
     double w_lam_vol = 0.0;
 #pragma unroll
@@ -108,19 +130,23 @@ struct RoughPath {
     double u[N];
 #pragma unroll
     for (int i = 0; i < N; ++i) u[i] = v[i];
-    drift(c, u, c.half_h);
+    drift(c, u, c.half_h, hk, 0);
     const double yw = wsum_of(c, u);
-    const double ex = clamp_log(fma(c.vv, z0 * c.sqrt_h, -0.5 * c.vv * c.vv * c.h));
-    const double Yh = yw * exp_table(ex);                                               // diffus_sde_solve_f64 (:240-243)
+    const double ex_raw = fma(c.vv, z0 * c.sqrt_h, -0.5 * c.vv * c.vv * c.h);
+    const double ex = clamp_log(ex_raw);
+    const double e = exp_table(ex);
+    hk.diffusion(yw, ex_raw, ex, e);
+    const double Yh = yw * e;                                                           // diffus_sde_solve_f64 (:240-243)
     const double Q = c.w_inv * (Yh - yw);
 #pragma unroll
     for (int i = 0; i < N; ++i) u[i] += Q;
-    drift(c, u, c.half_h);
+    drift(c, u, c.half_h, hk, 4);
     double volw_h = wsum_of(c, u);
     if (!(volw_h > 0.0)) {          // NaN or <= 0: the reference resets every factor of that path to 1e-6 (:310-312)
 #pragma unroll
       for (int i = 0; i < N; ++i) u[i] = 1e-6;
       volw_h = wsum_of(c, u);
+      hk.reset();
     }
     double w_lam_vol_h = 0.0;
 #pragma unroll
@@ -131,6 +157,7 @@ struct RoughPath {
                           (c.kappa1 - c.kappa2 * c.theta) * (0.5 * vw + 0.5 * volw_h) + c.kappa2 * (0.5 * sq_vw + 0.5 * sq_vhw)) *
                          c.h;
     const double term2 = 0.5 * c.h * sq_vw + 0.5 * c.h * sq_vhw;
+    hk.spot(vw, volw_h, term1, term2);
     ls = ls - 0.5 * term2 + c.rho * term1 + c.rho_comp * (term2 > 0.0 ? fast_sqrt(term2) : sqrt(term2)) * z1;
     y = fma(0.5 * c.h, sq_vw + sq_vhw, y);
 #pragma unroll
@@ -140,7 +167,36 @@ struct RoughPath {
 
 // Z0 / Z1 != nullptr: caller-supplied unit normals, row-major [S][P] (device); else in-kernel Philox draws (stream of philox.cuh with
 // slice = 0 for EVERY maturity, so that maturity m consumes the first S_m steps of one fixed stream per path, as the reference does with
-// the rows of Z0 / Z1).  vol_out: [N][P] factor values (may be nullptr), log_spot_out / qv_out: [P].
+// the rows of Z0 / Z1).  Path: RoughPath or RoughTangentPath, anything with step(c, z0, z1).
+template <int GAUSS, class Path>
+__device__ __forceinline__ void rough_run_path(Path& p, const RoughConsts& c, const double* __restrict__ Z0, const double* __restrict__ Z1, int S,
+                                               long long P, long long i, unsigned long long seed, unsigned long long path_offset) {
+  if (Z0) {
+    for (int s = 0; s < S; ++s) p.step(c, __ldg(Z0 + (size_t)s * P + i), __ldg(Z1 + (size_t)s * P + i));
+  } else {
+    StepNormals<double, GAUSS> rng(seed, path_offset + (unsigned long long)i, 0u);
+    if constexpr (GAUSS == kGaussF64) {
+      for (int s = 0; s < S; ++s) {
+        double z0, z1;
+        rng.get((uint32_t)s, z0, z1);
+        p.step(c, z0, z1);
+      }
+    } else {
+      for (int cidx = 0; 2 * cidx < S; ++cidx) {
+        double a0, a1, b0, b1;
+        rng.get2((uint32_t)cidx, a0, a1, b0, b1);
+        p.step(c, a0, a1);
+        if (2 * cidx + 1 < S) {
+          // a register-bound path draws the pair again instead of holding the second normals across the first step (same words)
+          if constexpr (Path::kRedrawPair) rng.get2((uint32_t)cidx, a0, a1, b0, b1);
+          p.step(c, b0, b1);
+        }
+      }
+    }
+  }
+}
+
+// vol_out: [N][P] factor values (may be nullptr), log_spot_out / qv_out: [P].
 template <int N, int GAUSS>
 __global__ void __launch_bounds__(kThreads) rough_logsv_kernel(double* __restrict__ log_spot_out, double* __restrict__ vol_out,
                                                               double* __restrict__ qv_out, const double* __restrict__ Z0,
@@ -152,25 +208,7 @@ __global__ void __launch_bounds__(kThreads) rough_logsv_kernel(double* __restric
   for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < P; i += stride) {
     RoughPath<N> p;
     p.init(c);
-    if (Z0) {
-      for (int s = 0; s < S; ++s) p.step(c, __ldg(Z0 + (size_t)s * P + i), __ldg(Z1 + (size_t)s * P + i));
-    } else {
-      StepNormals<double, GAUSS> rng(seed, path_offset + (unsigned long long)i, 0u);
-      if constexpr (GAUSS == kGaussF64) {
-        for (int s = 0; s < S; ++s) {
-          double z0, z1;
-          rng.get((uint32_t)s, z0, z1);
-          p.step(c, z0, z1);
-        }
-      } else {
-        for (int cidx = 0; 2 * cidx < S; ++cidx) {
-          double a0, a1, b0, b1;
-          rng.get2((uint32_t)cidx, a0, a1, b0, b1);
-          p.step(c, a0, a1);
-          if (2 * cidx + 1 < S) p.step(c, b0, b1);
-        }
-      }
-    }
+    rough_run_path<GAUSS>(p, c, Z0, Z1, S, P, i, seed, path_offset);
     log_spot_out[i] = p.ls;
     qv_out[i] = p.y;
     if (vol_out) {
@@ -203,6 +241,263 @@ static int launch_rough(int n, double* ls, double* vol, double* qv, const double
     case 7: return launch_rough_n<7>(ls, vol, qv, Z0, Z1, S, P, c, seed, path_offset, gauss, st);
     case 8: return launch_rough_n<8>(ls, vol, qv, Z0, Z1, S, P, c, seed, path_offset, gauss, st);
   }
+  return fail(-1, "invalid argument: the rough-vol kernel supports 1..8 factors");
+}
+
+// --------------------------------------------------------------------------------------------------------------------
+// pathwise (forward-mode) sensitivities of the rough chain, DESIGN.md §3.10
+// --------------------------------------------------------------------------------------------------------------------
+// Directions in LOGSV_GREEK_PARAMS order: sigma0, theta, kappa1, kappa2, beta, volvol (the ORTHOGONAL vol-of-vol on this route).
+// Per direction the derivatives of the RoughConsts entries the step reads; weights and nodes are inputs, not directions.
+constexpr int kRoughParams = 6;
+
+struct RoughTangentConsts {
+  double dv0[kRoughParams];        // d v0 = d sigma0 / W
+  double dtheta[kRoughParams], dk1[kRoughParams], dk2[kRoughParams];
+  double dvv[kRoughParams];        // d (vartheta W)
+  double drho[kRoughParams], drho_comp[kRoughParams];
+  double dlog_vt[kRoughParams];    // d vartheta / vartheta  (d (1/vartheta) = -dlog_vt / vartheta)
+  double dwlv0[kRoughParams];      // d sum w_i x_i v0
+  unsigned long long* reset_count; // device counter of the paths that took the reset-to-1e-6 branch at any step
+};
+
+static RoughTangentConsts make_rough_tangent_consts(const b200sv_logsv_params& p, const RoughConsts& c) {
+  RoughTangentConsts k{};
+  double wlam = 0.0;
+  for (int i = 0; i < kMaxRoughFactors; ++i) wlam += c.wlam[i];      // unused factors are zero in RoughConsts
+  const double vt = c.volvol;
+  const double dvt[kRoughParams] = {0.0, 0.0, 0.0, 0.0, p.beta / vt, p.volvol / vt};
+  const double dbeta[kRoughParams] = {0.0, 0.0, 0.0, 0.0, 1.0, 0.0};
+  for (int q = 0; q < kRoughParams; ++q) {
+    k.dv0[q] = q == 0 ? c.w_inv : 0.0;
+    k.dtheta[q] = q == 1 ? 1.0 : 0.0;
+    k.dk1[q] = q == 2 ? 1.0 : 0.0;
+    k.dk2[q] = q == 3 ? 1.0 : 0.0;
+    k.dvv[q] = c.wsum * dvt[q];
+    k.drho[q] = (dbeta[q] - c.rho * dvt[q]) / vt;
+    k.drho_comp[q] = c.rho_comp > 0.0 ? -c.rho * k.drho[q] / c.rho_comp : 0.0;
+    k.dlog_vt[q] = dvt[q] / vt;
+    k.dwlv0[q] = wlam * k.dv0[q];
+  }
+  return k;
+}
+
+// The production RoughPath steps the primal; this object is its hook, records the stage sums <w, z> and the other intermediates, and then
+// advances the tangents dv[q][N], dls[q], dy[q] of every direction q with the linearised step (exact derivative of the discrete map).
+template <int N>
+struct RoughTangentPath {
+  static constexpr bool kRedrawPair = true;      // 6 (N + 2) tangent doubles: no room for two normals across a step
+  RoughPath<N> p;
+  double dv[kRoughParams][N], dls[kRoughParams], dy[kRoughParams];
+  double zw[8], yw, ex_raw, ex, e, vw, vhw, term1, term2;
+  bool was_reset, any_reset;      // this step / any step of the path took the reset-to-1e-6 branch
+  const RoughTangentConsts& k;     // the kernel's __grid_constant__ parameter
+  __device__ __forceinline__ explicit RoughTangentPath(const RoughTangentConsts& k_) : k(k_) {}
+
+  __device__ __forceinline__ void stage(int s, double z) { zw[s] = z; }
+  __device__ __forceinline__ void diffusion(double yw_, double ex_raw_, double ex_, double e_) {
+    yw = yw_;
+    ex_raw = ex_raw_;
+    ex = ex_;
+    e = e_;
+  }
+  __device__ __forceinline__ void reset() {
+    was_reset = true;
+    any_reset = true;
+  }
+  __device__ __forceinline__ void spot(double vw_, double vhw_, double t1, double t2) {
+    vw = vw_;
+    vhw = vhw_;
+    term1 = t1;
+    term2 = t2;
+  }
+
+  __device__ __forceinline__ void init(const RoughConsts& c) {
+    p.init(c);
+    any_reset = false;
+#pragma unroll
+    for (int q = 0; q < kRoughParams; ++q) {
+#pragma unroll
+      for (int i = 0; i < N; ++i) dv[q][i] = k.dv0[q];
+      dls[q] = 0.0;
+      dy[q] = 0.0;
+    }
+  }
+  // tangent of the drift slope at a stage point with <w, z> = zw_s: ds_i = -x_i (dz_i - dv0) + dg
+  __device__ __forceinline__ void slope_t(const RoughConsts& c, int q, double zs, const double (&dz)[N], double (&ds)[N]) const {
+    const double dzw = RoughPath<N>::wsum_of(c, dz);
+    const double dg = fma(k.dk2[q], zs, fma(c.kappa2, dzw, k.dk1[q])) * (c.theta - zs) + fma(c.kappa2, zs, c.kappa1) * (k.dtheta[q] - dzw);
+#pragma unroll
+    for (int i = 0; i < N; ++i) ds[i] = fma(-c.nodes[i], dz[i] - k.dv0[q], dg);
+  }
+  // tangent of RoughPath::drift: the same RK4 stage combination applied to the stage tangents
+  __device__ __forceinline__ void drift_t(const RoughConsts& c, int q, double (&dz)[N], double hh, int s0) const {
+    double acc[N], t[N], s[N];
+    slope_t(c, q, zw[s0], dz, s);
+#pragma unroll
+    for (int i = 0; i < N; ++i) {
+      acc[i] = s[i];
+      t[i] = fma(0.5 * hh, s[i], dz[i]);
+    }
+    slope_t(c, q, zw[s0 + 1], t, s);
+#pragma unroll
+    for (int i = 0; i < N; ++i) {
+      acc[i] = fma(2.0, s[i], acc[i]);
+      t[i] = fma(0.5 * hh, s[i], dz[i]);
+    }
+    slope_t(c, q, zw[s0 + 2], t, s);
+#pragma unroll
+    for (int i = 0; i < N; ++i) {
+      acc[i] = fma(2.0, s[i], acc[i]);
+      t[i] = fma(hh, s[i], dz[i]);
+    }
+    slope_t(c, q, zw[s0 + 3], t, s);
+#pragma unroll
+    for (int i = 0; i < N; ++i) dz[i] = fma(hh / 6.0, acc[i] + s[i], dz[i]);
+  }
+
+  __device__ __forceinline__ void step(const RoughConsts& c, double z0, double z1) {
+    was_reset = false;
+    p.step(c, z0, z1, *this);
+    const bool clamped = ex != ex_raw;
+    const double sq = term2 > 0.0 ? sqrt(term2) : 0.0, half_inv_sq = term2 > 0.0 ? 0.5 / sq : 0.0;
+    const double a_mean = 0.5 * vw + 0.5 * vhw, a_sq = 0.5 * vw * vw + 0.5 * vhw * vhw;
+    const double dex_unit = fma(c.sqrt_h, z0, -c.vv * c.h);                 // d ex / d vv
+#pragma unroll
+    for (int q = 0; q < kRoughParams; ++q) {
+      double du[N];
+      double dvw = 0.0, dwlv = 0.0;
+#pragma unroll
+      for (int i = 0; i < N; ++i) {
+        du[i] = dv[q][i];
+        dvw = fma(c.weight[i], du[i], dvw);
+        dwlv = fma(c.wlam[i], du[i], dwlv);
+      }
+      drift_t(c, q, du, c.half_h, 0);
+      // exact log-normal step of <w, u>: dYh = e^ex (dyw + yw dex), the shift dQ = (dYh - dyw) / W added to every factor
+      const double dyw = RoughPath<N>::wsum_of(c, du);
+      const double dex = clamped ? 0.0 : k.dvv[q] * dex_unit;
+      const double dQ = c.w_inv * (e * fma(yw, dex, dyw) - dyw);
+#pragma unroll
+      for (int i = 0; i < N; ++i) du[i] += dQ;
+      drift_t(c, q, du, c.half_h, 4);
+      double dvhw = 0.0, dwlvh = 0.0;
+#pragma unroll
+      for (int i = 0; i < N; ++i) {
+        if (was_reset) du[i] = 0.0;
+        dvhw = fma(c.weight[i], du[i], dvhw);
+        dwlvh = fma(c.wlam[i], du[i], dwlvh);
+        dv[q][i] = du[i];
+      }
+      // log-spot increment: term1 = h / vartheta * A, term2 = h / 2 (vw^2 + volw_h^2)
+      const double dsum = fma(vw, dvw, vhw * dvhw);
+      const double dterm2 = c.h * dsum;
+      const double dA = (((dvhw - dvw) * c.inv_h + 0.5 * dwlv + 0.5 * dwlvh) - k.dwlv0[q]) * c.w_inv -
+                        fma(k.dk1[q], c.theta, c.kappa1 * k.dtheta[q]) +
+                        (k.dk1[q] - fma(k.dk2[q], c.theta, c.kappa2 * k.dtheta[q])) * a_mean +
+                        (c.kappa1 - c.kappa2 * c.theta) * (0.5 * dvw + 0.5 * dvhw) + fma(k.dk2[q], a_sq, c.kappa2 * dsum);
+      const double dterm1 = fma(-k.dlog_vt[q], term1, c.h * c.inv_volvol * dA);
+      const double dsq = fma(k.drho_comp[q], sq, c.rho_comp * dterm2 * half_inv_sq);
+      dls[q] += fma(dsq, z1, fma(-0.5, dterm2, fma(k.drho[q], term1, c.rho * dterm1)));
+      dy[q] += dterm2;
+    }
+  }
+};
+
+// rough_logsv_kernel with tangents: same persistent grid-stride loop and normals (rough_run_path), same restart at t = 0.  Writes the state
+// like rough_logsv_kernel, dls_out / dqv_out [6][P], dvol_out [6][N][P] (may be nullptr), and per-CTA partials [gridDim.x][2 + 6]:
+// sum F e^ls, count, sum F e^ls dls_q over the non-NaN spots (the moments payoff_greeks_kernel re-centres with).  *k.reset_count += the
+// number of paths that took the reset branch at ANY step of the grid (their mass across the switch is what the pathwise rows omit, DESIGN.md
+// §3.10): one atomic per such path after its last step, so that no counter is held in registers across the path loop.
+template <int N, int GAUSS>
+__global__ void __launch_bounds__(kThreads) rough_logsv_tangent_kernel(double* __restrict__ log_spot_out, double* __restrict__ vol_out,
+                                                                      double* __restrict__ qv_out, double* __restrict__ dls_out,
+                                                                      double* __restrict__ dvol_out, double* __restrict__ dqv_out,
+                                                                      const double* __restrict__ Z0, const double* __restrict__ Z1, int S, long long P,
+                                                                      RoughConsts c, const __grid_constant__ RoughTangentConsts k,
+                                                                      unsigned long long seed, double forward, double* __restrict__ partials) {
+  constexpr int K = 2 + kRoughParams;
+  __shared__ double red[K * kThreads / 32];
+  exp_table_init();
+  if constexpr (GAUSS != kGaussF32) gauss64_table_init();
+  double acc[K];
+#pragma unroll
+  for (int j = 0; j < K; ++j) acc[j] = 0.0;
+  const long long stride = (long long)gridDim.x * kThreads;
+  for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < P; i += stride) {
+    RoughTangentPath<N> t(k);
+    t.init(c);
+    rough_run_path<GAUSS>(t, c, Z0, Z1, S, P, i, seed, 0ull);
+    log_spot_out[i] = t.p.ls;
+    qv_out[i] = t.p.y;
+    if (vol_out) {
+#pragma unroll
+      for (int f = 0; f < N; ++f) vol_out[(size_t)f * P + i] = t.p.v[f];
+    }
+    const double spot = forward * exp(t.p.ls);
+#pragma unroll
+    for (int q = 0; q < kRoughParams; ++q) {
+      dls_out[(size_t)q * P + i] = t.dls[q];
+      dqv_out[(size_t)q * P + i] = t.dy[q];
+      if (dvol_out) {
+#pragma unroll
+        for (int f = 0; f < N; ++f) dvol_out[((size_t)q * N + f) * P + i] = t.dv[q][f];
+      }
+      if (spot == spot) acc[2 + q] = fma(spot, t.dls[q], acc[2 + q]);
+    }
+    if (spot == spot) {
+      acc[0] += spot;
+      acc[1] += 1.0;
+    }
+    if (t.any_reset) atomicAdd(k.reset_count, 1ull);
+  }
+  block_sum<K, kThreads>(acc, red);
+  if (threadIdx.x == 0) {
+#pragma unroll
+    for (int j = 0; j < K; ++j) partials[K * blockIdx.x + j] = acc[j];
+  }
+}
+
+template <int N>
+static int launch_rough_tangent_n(double* ls, double* vol, double* qv, double* dls, double* dvol, double* dqv, const double* Z0, const double* Z1,
+                                  int S, long long P, const RoughConsts& c, const RoughTangentConsts& k, uint64_t seed, int gauss, double forward,
+                                  double* partials, int blocks, cudaStream_t st) {
+  if (gauss == kGaussF64)
+    rough_logsv_tangent_kernel<N, kGaussF64><<<blocks, kThreads, 0, st>>>(ls, vol, qv, dls, dvol, dqv, Z0, Z1, S, P, c, k, seed, forward, partials);
+  else
+    rough_logsv_tangent_kernel<N, kGaussF32><<<blocks, kThreads, 0, st>>>(ls, vol, qv, dls, dvol, dqv, Z0, Z1, S, P, c, k, seed, forward, partials);
+  return check_launch("rough_logsv_tangent_kernel");
+}
+
+template <int N>
+static int rough_tangent_blocks(long long P) {
+  return persistent_grid(rough_logsv_tangent_kernel<N, kGaussF32>, kThreads, P).blocks;
+}
+
+static int rough_tangent_grid(int n, long long P) {
+  switch (n) {
+    case 1: return rough_tangent_blocks<1>(P);
+    case 2: return rough_tangent_blocks<2>(P);
+    case 3: return rough_tangent_blocks<3>(P);
+    case 4: return rough_tangent_blocks<4>(P);
+    case 5: return rough_tangent_blocks<5>(P);
+    case 6: return rough_tangent_blocks<6>(P);
+    case 7: return rough_tangent_blocks<7>(P);
+    case 8: return rough_tangent_blocks<8>(P);
+  }
+  return 0;
+}
+
+static int launch_rough_tangent(int n, double* ls, double* vol, double* qv, double* dls, double* dvol, double* dqv, const double* Z0,
+                                const double* Z1, int S, long long P, const RoughConsts& c, const RoughTangentConsts& k, uint64_t seed, int gauss,
+                                double forward, double* partials, int blocks, cudaStream_t st) {
+#define B200SV_ROUGH_TANGENT_CASE(NF) \
+  case NF: return launch_rough_tangent_n<NF>(ls, vol, qv, dls, dvol, dqv, Z0, Z1, S, P, c, k, seed, gauss, forward, partials, blocks, st);
+  switch (n) {
+    B200SV_ROUGH_TANGENT_CASE(1) B200SV_ROUGH_TANGENT_CASE(2) B200SV_ROUGH_TANGENT_CASE(3) B200SV_ROUGH_TANGENT_CASE(4)
+    B200SV_ROUGH_TANGENT_CASE(5) B200SV_ROUGH_TANGENT_CASE(6) B200SV_ROUGH_TANGENT_CASE(7) B200SV_ROUGH_TANGENT_CASE(8)
+  }
+#undef B200SV_ROUGH_TANGENT_CASE
   return fail(-1, "invalid argument: the rough-vol kernel supports 1..8 factors");
 }
 
@@ -253,6 +548,117 @@ static int rough_chain_host(const b200sv_logsv_params* params, int B, int n, con
     }
   }
   return io.copy_back(sync, prices_out, stderr_out, ivols_out);
+}
+
+// chain driver with pathwise sensitivities, one parameter set: per maturity tangent kernel -> moments -> payoff_greeks_kernel<6> ->
+// greeks_finalize_kernel.  Prices / "std errors" keep the route's convention (discfactor * nanstd(payoff)); greeks_se is df * std / sqrt(P).
+// greeks_out / greeks_se_out [1 + 6][Jtot] (row 0 = forward delta); states_out [M][n + 2][P], tangents_out [M][6][n + 2][P], resets_out [M]
+// (paths that took the reset branch at any step of maturity m's grid) may be NULL.
+static int rough_chain_greeks_host(const b200sv_logsv_params& p, int n, const double* weights, const double* nodes, int M, const double* ttms,
+                                   const double* forwards, const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
+                                   long long nb_path, const int* nsteps, const double* hs, const double* Z0, const double* Z1, long long z_rows,
+                                   int variable_type, uint64_t seed, int flags, double* prices_out, double* stderr_out, double* greeks_out,
+                                   double* greeks_se_out, double* states_out, double* tangents_out, double* resets_out) {
+  constexpr int NP = kRoughParams, K = 2 + NP, KV = 3 + 2 * (1 + NP);
+  B200SV_REQUIRE(n >= 1 && n <= kMaxRoughFactors, "1 <= n_factors <= 8");
+  B200SV_REQUIRE(nb_path >= 1, "nb_path must be >= 1");
+  B200SV_REQUIRE((Z0 == nullptr) == (Z1 == nullptr), "Z0 and Z1 must be supplied together");
+  if (int rc = validate_chain(M, ttms, offsets, types, variable_type)) return rc;
+  const int g = gauss_mode(flags);
+  B200SV_REQUIRE(g == kGaussF32 || g == kGaussF64, "gauss flags");
+  B200SV_REQUIRE(!(flags & B200SV_STATE_F32), "the rough-vol route is float64 only");
+  int Smax = 0;
+  for (int m = 0; m < M; ++m) {
+    B200SV_REQUIRE(nsteps[m] >= 1 && hs[m] > 0.0, "nsteps / h must be positive");
+    Smax = std::max(Smax, nsteps[m]);
+  }
+  B200SV_REQUIRE(!Z0 || z_rows >= Smax, "Z0 / Z1 have fewer rows than the longest grid");
+  const int Jtot = offsets[M] - offsets[0], Jalloc = std::max(Jtot, 1);
+  cudaStream_t st = current_stream();
+  ensure_pool_threshold();
+  StreamSync sync(st);
+  const size_t P = (size_t)nb_path;
+  const int blocks = rough_tangent_grid(n, nb_path);
+  DevBuf d_state(st), d_tan(st), d_dvol(st), d_z(st), d_strikes(st), d_types(st), d_out(st), d_mom(st), d_sums(st), d_part(st), d_gpart(st),
+      d_resets(st);
+  B200SV_CUDA(d_state.alloc(sizeof(double) * (size_t)(n + 2) * P));
+  B200SV_CUDA(d_tan.alloc(sizeof(double) * 2 * NP * P));
+  if (tangents_out) B200SV_CUDA(d_dvol.alloc(sizeof(double) * (size_t)NP * n * P));
+  B200SV_CUDA(d_strikes.alloc(sizeof(double) * Jalloc));
+  B200SV_CUDA(d_types.alloc(Jalloc));
+  B200SV_CUDA(d_out.alloc(sizeof(double) * 2 * (size_t)Jalloc * (2 + NP)));
+  B200SV_CUDA(d_mom.alloc(sizeof(double) * K));
+  B200SV_CUDA(d_sums.alloc(sizeof(double) * KV * Jalloc));
+  B200SV_CUDA(d_part.alloc(sizeof(double) * K * (size_t)blocks));
+  B200SV_CUDA(d_resets.alloc(sizeof(unsigned long long) * M));
+  B200SV_CUDA(cudaMemsetAsync(d_resets.p, 0, sizeof(unsigned long long) * M, st));
+  // payoff_greeks_kernel: one grid shape per chunk count, partials sized for the widest slice
+  int Jmax = 0;
+  for (int m = 0; m < M; ++m) Jmax = std::max(Jmax, offsets[m + 1] - offsets[m]);
+  const int max_chunks = std::max(1, (Jmax + kGreeksStrikeChunk - 1) / kGreeksStrikeChunk);
+  const Grid gp = persistent_grid(payoff_greeks_kernel<NP>, kThreads, nb_path);
+  B200SV_CUDA(d_gpart.alloc(sizeof(double) * (size_t)KV * kGreeksStrikeChunk * max_chunks * gp.blocks));
+  if (Z0) {
+    B200SV_CUDA(d_z.alloc(sizeof(double) * 2 * (size_t)Smax * P));
+    B200SV_CUDA(cudaMemcpyAsync(d_z.p, Z0, sizeof(double) * (size_t)Smax * P, cudaMemcpyHostToDevice, st));
+    B200SV_CUDA(cudaMemcpyAsync(d_z.as<double>() + (size_t)Smax * P, Z1, sizeof(double) * (size_t)Smax * P, cudaMemcpyHostToDevice, st));
+  }
+  if (Jtot > 0) {
+    B200SV_CUDA(cudaMemcpyAsync(d_strikes.p, strikes + offsets[0], sizeof(double) * Jtot, cudaMemcpyHostToDevice, st));
+    B200SV_CUDA(cudaMemcpyAsync(d_types.p, types + offsets[0], Jtot, cudaMemcpyHostToDevice, st));
+  }
+  double *d_ls = d_state.as<double>(), *d_vol = d_ls + P, *d_qv = d_ls + (size_t)(n + 1) * P;
+  double *d_dls = d_tan.as<double>(), *d_dqv = d_dls + NP * P, *d_dv = d_dvol.as<double>();
+  const double *z0 = d_z.as<double>(), *z1 = Z0 ? z0 + (size_t)Smax * P : nullptr;
+  double *o_price = d_out.as<double>(), *o_se = o_price + Jalloc, *o_g = o_se + Jalloc, *o_gse = o_g + (size_t)(1 + NP) * Jalloc;
+  for (int m = 0; m < M; ++m) {
+    const RoughConsts c = make_rough_consts(p, n, weights, nodes, hs[m]);
+    RoughTangentConsts k = make_rough_tangent_consts(p, c);
+    k.reset_count = d_resets.as<unsigned long long>() + m;
+    if (int rc = launch_rough_tangent(n, d_ls, d_vol, d_qv, d_dls, tangents_out ? d_dv : nullptr, d_dqv, z0, z1, nsteps[m], nb_path, c, k, seed, g,
+                                      forwards[m], d_part.as<double>(), blocks, st))
+      return rc;
+    reduce_partials_kernel<<<1, 64, 0, st>>>(d_part.as<double>(), blocks, K, K, d_mom.as<double>(), P2pPublish{});
+    if (int rc = check_launch("reduce_partials_kernel")) return rc;
+    if (states_out)
+      B200SV_CUDA(cudaMemcpyAsync(states_out + (size_t)m * (n + 2) * P, d_ls, sizeof(double) * (size_t)(n + 2) * P, cudaMemcpyDeviceToHost, st));
+    if (tangents_out) {
+      for (int q = 0; q < NP; ++q) {
+        double* o = tangents_out + ((size_t)m * NP + q) * (n + 2) * P;
+        B200SV_CUDA(cudaMemcpyAsync(o, d_dls + q * P, sizeof(double) * P, cudaMemcpyDeviceToHost, st));
+        B200SV_CUDA(cudaMemcpyAsync(o + P, d_dv + (size_t)q * n * P, sizeof(double) * n * P, cudaMemcpyDeviceToHost, st));
+        B200SV_CUDA(cudaMemcpyAsync(o + (size_t)(n + 1) * P, d_dqv + q * P, sizeof(double) * P, cudaMemcpyDeviceToHost, st));
+      }
+    }
+    const int J = offsets[m + 1] - offsets[m], jo = offsets[m] - offsets[0];
+    if (J == 0) continue;
+    const int chunks = (J + kGreeksStrikeChunk - 1) / kGreeksStrikeChunk;
+    const int Kpad = KV * kGreeksStrikeChunk * chunks;
+    const int gblocks = std::max(1, gp.blocks / chunks);
+    payoff_greeks_kernel<NP><<<dim3(gblocks, chunks), gp.threads, 0, st>>>(d_ls, d_qv, d_dls, d_dqv, nb_path, ttms[m], forwards[m],
+                                                                           d_strikes.as<double>() + jo, d_types.as<int8_t>() + jo, J, variable_type,
+                                                                           d_mom.as<double>(), d_gpart.as<double>(), Kpad);
+    if (int rc = check_launch("payoff_greeks_kernel")) return rc;
+    reduce_partials_kernel<<<1, 256, 0, st>>>(d_gpart.as<double>(), gblocks, Kpad, KV * J, d_sums.as<double>(), P2pPublish{});
+    if (int rc = check_launch("reduce_partials_kernel")) return rc;
+    // the price row keeps the route's un-normalised std (total_paths = 1), the sensitivity rows are standard errors
+    greeks_finalize_kernel<<<(J + 127) / 128, 128, 0, st>>>(d_sums.as<double>(), KV, J, Jalloc, discfactors[m], 1.0, (double)nb_path,
+                                                            o_price + jo, o_se + jo, o_g + jo, o_gse + jo);
+    if (int rc = check_launch("greeks_finalize_kernel")) return rc;
+  }
+  if (Jtot > 0) {
+    B200SV_CUDA(cudaMemcpyAsync(prices_out, o_price, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st));
+    B200SV_CUDA(cudaMemcpyAsync(stderr_out, o_se, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st));
+    for (int q = 0; q < 1 + NP; ++q) {
+      B200SV_CUDA(cudaMemcpyAsync(greeks_out + (size_t)q * Jtot, o_g + (size_t)q * Jalloc, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st));
+      B200SV_CUDA(cudaMemcpyAsync(greeks_se_out + (size_t)q * Jtot, o_gse + (size_t)q * Jalloc, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st));
+    }
+  }
+  std::vector<unsigned long long> h_resets(M);
+  B200SV_CUDA(cudaMemcpyAsync(h_resets.data(), d_resets.p, sizeof(unsigned long long) * M, cudaMemcpyDeviceToHost, st));
+  if (int rc = sync.done()) return rc;
+  for (int m = 0; m < M && resets_out; ++m) resets_out[m] = (double)h_resets[m];
+  return 0;
 }
 
 }  // namespace b200sv

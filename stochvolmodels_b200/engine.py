@@ -194,6 +194,54 @@ def heston_mc_chain_batch(params_list: Sequence[C.HestonParamsC], ttms, forwards
                         (), (int(nb_path), int(nb_steps_per_year), C.seed64(seed), int(flags), int(scheme)), 2, with_ivols)
 
 
+def _rough_grid_normals(M: int, nb_path: int, nsteps, hs, Z0, Z1):
+    """the per-maturity grids and the optional host normals of the rough-vol entry points -> (nsteps, hs, Z0, Z1, z_rows)"""
+    nsteps = np.ascontiguousarray(nsteps, dtype=np.int32)
+    hs = C.f64(hs)
+    if nsteps.shape[0] != M or hs.shape[0] != M:
+        raise ValueError("nsteps and hs must have one entry per maturity")
+    z_rows = 0
+    if Z0 is not None or Z1 is not None:
+        if Z0 is None or Z1 is None:
+            raise ValueError("Z0 and Z1 must be supplied together")
+        Z0, Z1 = C.f64(Z0), C.f64(Z1)
+        if Z0.ndim != 2 or Z0.shape != Z1.shape or Z0.shape[1] != nb_path:
+            raise ValueError("Z0 and Z1 must be 2-d arrays [nb_steps, nb_path] of the same shape")
+        z_rows = Z0.shape[0]
+        if z_rows < int(nsteps.max()):
+            raise ValueError("Z0 / Z1 have fewer rows than the longest time grid")
+        if z_rows > int(nsteps.max()):          # the library uploads exactly max(nsteps) rows
+            Z0, Z1 = np.ascontiguousarray(Z0[: int(nsteps.max())]), np.ascontiguousarray(Z1[: int(nsteps.max())])
+            z_rows = int(nsteps.max())
+    return nsteps, hs, Z0, Z1, z_rows
+
+
+def rough_logsv_mc_chain_greeks(params: C.LogsvParamsC, weights, nodes, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms,
+                                nb_path: int, nsteps, hs, Z0=None, Z1=None, variable_type=1, seed: int = 0, flags: int = 0,
+                                return_states: bool = False, return_tangents: bool = False):
+    """one parameter set through the rough-LogSV chain MC with pathwise sensitivities (b200sv_rough_logsv_mc_chain_greeks).  Arguments as
+    rough_logsv_mc_chain with ``weights`` / ``nodes`` [n].  Returns (prices, std errors, greeks [1+6, J], greeks_se [1+6, J], offsets,
+    states [M, n + 2, nb_path] | None, tangents [M, 6, n + 2, nb_path] | None, resets [M]): greeks row 0 the forward delta, then
+    LOGSV_GREEK_PARAMS; resets[m] = the number of paths that took the reset-to-1e-6 branch at any step of maturity m's grid."""
+    vt = variable_code(variable_type)
+    ch = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
+    weights, nodes = C.f64(weights), C.f64(nodes)
+    if weights.shape != nodes.shape or weights.ndim != 1:
+        raise ValueError("weights and nodes must be 1-d arrays of the same length")
+    n = weights.shape[0]
+    nsteps, hs, Z0, Z1, z_rows = _rough_grid_normals(ch.M, nb_path, nsteps, hs, Z0, Z1)
+    J, P = ch.strikes.shape[0], len(LOGSV_GREEK_PARAMS)
+    prices, stds, greeks, greeks_se = np.empty(J), np.empty(J), np.empty((1 + P, J)), np.empty((1 + P, J))
+    states = np.empty((ch.M, n + 2, int(nb_path))) if return_states else None
+    tangents = np.empty((ch.M, P, n + 2, int(nb_path))) if return_tangents else None
+    resets = np.empty(ch.M)
+    C.call("b200sv_rough_logsv_mc_chain_greeks", byref(params), n, C.dptr(weights), C.dptr(nodes), *C.chain_ptrs(ch), int(nb_path), C.iptr(nsteps),
+           C.dptr(hs), C.dptr(Z0), C.dptr(Z1), int(z_rows), vt, C.seed64(seed), int(flags), C.dptr(prices), C.dptr(stds), C.dptr(greeks),
+           C.dptr(greeks_se), C.dptr(states), C.dptr(tangents), C.dptr(resets))
+    return (C.split_chain(prices, ch.offsets), C.split_chain(stds, ch.offsets), greeks, greeks_se, ch.offsets, states, tangents,
+            resets.astype(np.int64))
+
+
 def rough_logsv_mc_chain(params_list, weights, nodes, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, nb_path: int, nsteps, hs,
                          Z0=None, Z1=None, variable_type=1, seed: int = 0, flags: int = 0, with_ivols: bool = False, return_states: bool = False):
     """B parameter sets through the rough-LogSV multi-factor chain MC (b200sv_rough_logsv_mc_chain).  ``weights`` / ``nodes``: [n] (shared)
@@ -213,23 +261,7 @@ def rough_logsv_mc_chain(params_list, weights, nodes, ttms, forwards, discfactor
     if weights.shape[0] != B:
         raise ValueError(f"weights / nodes must have {B} rows")
     weights, nodes = np.ascontiguousarray(weights), np.ascontiguousarray(nodes)
-    nsteps = np.ascontiguousarray(nsteps, dtype=np.int32)
-    hs = C.f64(hs)
-    if nsteps.shape[0] != M or hs.shape[0] != M:
-        raise ValueError("nsteps and hs must have one entry per maturity")
-    z_rows = 0
-    if Z0 is not None or Z1 is not None:
-        if Z0 is None or Z1 is None:
-            raise ValueError("Z0 and Z1 must be supplied together")
-        Z0, Z1 = C.f64(Z0), C.f64(Z1)
-        if Z0.ndim != 2 or Z0.shape != Z1.shape or Z0.shape[1] != nb_path:
-            raise ValueError("Z0 and Z1 must be 2-d arrays [nb_steps, nb_path] of the same shape")
-        z_rows = Z0.shape[0]
-        if z_rows < int(nsteps.max()):
-            raise ValueError("Z0 / Z1 have fewer rows than the longest time grid")
-        if z_rows > int(nsteps.max()):          # the library uploads exactly max(nsteps) rows
-            Z0, Z1 = np.ascontiguousarray(Z0[: int(nsteps.max())]), np.ascontiguousarray(Z1[: int(nsteps.max())])
-            z_rows = int(nsteps.max())
+    nsteps, hs, Z0, Z1, z_rows = _rough_grid_normals(M, nb_path, nsteps, hs, Z0, Z1)
     J = ch.strikes.shape[0]
     prices, stds = np.empty((B, J)), np.empty((B, J))
     ivols = np.empty((B, J)) if with_ivols else None

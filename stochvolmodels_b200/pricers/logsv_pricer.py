@@ -250,7 +250,7 @@ class LogSVPricer(ModelPricer):
         """MC prices and standard errors as ``model_mc_price_chain`` (same defaults, ``seed`` / ``gauss`` kwargs, same numbers on the same
         seed) plus pathwise sensitivities in the same pass: the forward delta and d price / d (sigma0, theta, kappa1, kappa2, beta, volvol),
         each with its standard error -> ``McChainGreeks``.  ``kappa2`` is the value after ``__post_init__`` and is held fixed when kappa1 or
-        theta moves; the vol backbone and discount factors are not differentiated.  fp64 state only; no rough-vol route, no ``exchange``.
+        theta moves; the vol backbone and discount factors are not differentiated.  fp64 state only; no ``exchange``; the rough-vol route has its own ``rough_mc_chain_greeks``.
         Under torch.distributed every rank prices all paths (replicated, bit-identical results)."""
         from .mc_greeks import check_greeks_kwargs, to_mc_chain_greeks
         check_greeks_kwargs(kwargs)
@@ -261,6 +261,35 @@ class LogSVPricer(ModelPricer):
                                            option_chain.optiontypes_ttms, nb_path, nb_steps or int(360 * np.max(option_chain.ttms)) + 1,
                                            is_spot_measure, vt, _shared_seed(kwargs.get("seed")), flags)
         return to_mc_chain_greeks(res, engine.LOGSV_GREEK_PARAMS)
+
+    @timer
+    def rough_mc_chain_greeks(self, option_chain: OptionChain, params: LogSvParams, nb_path: int = 100000, nb_steps: Optional[int] = None,
+                              variable_type: VariableType = VariableType.LOG_RETURN, **kwargs):
+        """pathwise sensitivities of the rough-vol route (DESIGN.md §3.10): prices and "std errors" equal to
+        ``model_mc_price_chain(use_rough_mc=True)`` with the same arguments (``seed`` required; ``gauss=None`` the RandomState normals of
+        get_randoms_for_rough_vol_chain_valuation, 'fp32' / 'fp64' in-kernel Philox; ``nb_steps`` passed through as given), plus the forward
+        delta and d price / d (sigma0, theta, kappa1, kappa2, beta, volvol) with standard errors -> ``McChainGreeks``.  ``volvol`` is the
+        orthogonal vol-of-vol, as on the price route; ``params.weights`` / ``params.nodes`` are inputs, not differentiated.  ``reset_paths``
+        counts, per maturity, the paths that hit the reset-to-1e-6 branch (their mass across it is not in the rows).  fp64 only, no
+        ``exchange``; under torch.distributed every rank prices all paths (replicated, bit-identical results)."""
+        from .mc_greeks import check_rough_greeks_kwargs, to_mc_chain_greeks
+        check_rough_greeks_kwargs(kwargs)
+        vt = engine.variable_code(variable_type)
+        gauss, seed = kwargs.get("gauss"), int(kwargs["seed"])
+        if gauss is None:
+            Z0, Z1, grids = get_randoms_for_rough_vol_chain_valuation(ttms=option_chain.ttms, nb_path=nb_path, nb_steps_per_year=nb_steps, seed=seed)
+        else:
+            Z0 = Z1 = None
+            grids = [set_time_grid(ttm, nb_steps)[2] for ttm in option_chain.ttms]
+        weights, nodes = np.asarray(params.weights, dtype=np.float64), np.asarray(params.nodes, dtype=np.float64)
+        res = engine.rough_logsv_mc_chain_greeks(engine.logsv_params_c(params.sigma0, params.theta, params.kappa1, params.kappa2, params.beta,
+                                                                       params.volvol), weights, nodes, option_chain.ttms, option_chain.forwards,
+                                                 option_chain.discfactors, option_chain.strikes_ttms, option_chain.optiontypes_ttms, nb_path,
+                                                 [g.size - 1 for g in grids], [float(g[1] - g[0]) for g in grids], Z0, Z1, vt, seed,
+                                                 engine.mc_flags("fp64", gauss or "fp32"))
+        out = to_mc_chain_greeks(res[:5], engine.LOGSV_GREEK_PARAMS)
+        out.reset_paths = res[7]
+        return out
 
     @timer
     def simulate_vol_paths(self, params: LogSvParams, brownians: np.ndarray = None, ttm: float = 1.0, nb_path: int = 100000,

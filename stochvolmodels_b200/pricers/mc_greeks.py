@@ -11,7 +11,7 @@ GPU.  The Philox counter is the global path id, so every rank returns bit-identi
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import Dict, List, Sequence
+from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 
@@ -21,13 +21,16 @@ from .. import _capi as C
 @dataclass
 class McChainGreeks:
     """prices / std errors / delta / delta_se: one array per maturity.  ``params`` / ``params_se``: parameter name (dataclass field,
-    after ``__post_init__``) -> one array per maturity of d price / d parameter and its standard error."""
+    after ``__post_init__``) -> one array per maturity of d price / d parameter and its standard error.  ``reset_paths`` (rough-vol route
+    only, else None): per maturity, the number of paths that took the reset-to-1e-6 branch at any step; the pathwise rows omit the price
+    mass such paths move across that switch, so they are unbiased for the scheme only where it is 0."""
     prices: List[np.ndarray]
     std_errors: List[np.ndarray]
     delta: List[np.ndarray]
     delta_se: List[np.ndarray]
     params: Dict[str, List[np.ndarray]]
     params_se: Dict[str, List[np.ndarray]]
+    reset_paths: Optional[np.ndarray] = None
 
 
 def check_greeks_kwargs(kwargs, precision_default: str = "fp64") -> None:
@@ -35,11 +38,23 @@ def check_greeks_kwargs(kwargs, precision_default: str = "fp64") -> None:
     if kwargs.get("precision", precision_default) != "fp64":
         raise NotImplementedError("model_mc_chain_greeks needs precision='fp64'")
     if kwargs.get("use_rough_mc"):
-        raise NotImplementedError("model_mc_chain_greeks does not cover the rough-vol route (use_rough_mc)")
+        raise NotImplementedError("model_mc_chain_greeks does not cover the rough-vol route (use_rough_mc): use LogSVPricer.rough_mc_chain_greeks")
     if kwargs.get("exchange") is not None:
         raise NotImplementedError("model_mc_chain_greeks is single-GPU per rank (replicated under torch.distributed): no exchange")
     if kwargs.get("gauss", "fp32") not in ("fp32", "fp64"):
         raise NotImplementedError("model_mc_chain_greeks supports gauss='fp32' or 'fp64'")
+
+
+def check_rough_greeks_kwargs(kwargs) -> None:
+    """what LogSVPricer.rough_mc_chain_greeks rejects before any GPU work"""
+    if kwargs.get("precision", "fp64") != "fp64":
+        raise NotImplementedError("rough_mc_chain_greeks needs precision='fp64'")
+    if kwargs.get("exchange") is not None:
+        raise NotImplementedError("rough_mc_chain_greeks is single-GPU per rank (replicated under torch.distributed): no exchange")
+    if kwargs.get("gauss") not in (None, "fp32", "fp64"):
+        raise NotImplementedError("rough_mc_chain_greeks supports gauss=None (RandomState normals), 'fp32' or 'fp64'")
+    if kwargs.get("seed") is None:
+        raise ValueError("rough_mc_chain_greeks needs a seed, like model_mc_price_chain(use_rough_mc=True)")
 
 
 def to_mc_chain_greeks(result, names: Sequence[str]) -> McChainGreeks:
