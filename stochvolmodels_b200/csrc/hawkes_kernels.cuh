@@ -291,7 +291,7 @@ static int hawkes_chain_host(const b200sv_hawkes_params* p, int M, const double*
                              int flags, double* prices_out, double* stderr_out) {
   B200SV_REQUIRE(nb_path >= 1, "nb_path must be >= 1");
   B200SV_REQUIRE(!(flags & B200SV_STATE_F32), "the Hawkes route is float64 only");
-  if (int rc = validate_chain(M, ttms, offsets, types, variable_type)) return rc;
+  if (int rc = validate_chain(M, ttms, offsets, strikes, types, variable_type)) return rc;
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
   StreamSync sync(st);

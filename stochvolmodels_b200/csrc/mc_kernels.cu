@@ -1515,7 +1515,7 @@ static int payoff_kinds(const int8_t* types, int J) {
   return k;
 }
 
-static int validate_chain(int M, const double* ttms, const int* offsets, const int8_t* types, int variable_type) {
+static int validate_chain(int M, const double* ttms, const int* offsets, const double* strikes, const int8_t* types, int variable_type) {
   B200SV_REQUIRE(M >= 1, "M must be >= 1");
   double t0 = 0.0;
   for (int m = 0; m < M; ++m) {
@@ -1523,6 +1523,7 @@ static int validate_chain(int M, const double* ttms, const int* offsets, const i
     B200SV_REQUIRE(offsets[m + 1] >= offsets[m], "offsets must be non-decreasing");
     t0 = ttms[m];
   }
+  B200SV_REQUIRE(offsets[M] == offsets[0] || (strikes && types), "null pointer");
   for (int j = offsets[0]; j < offsets[M]; ++j)
     if (types[j] < 0 || types[j] > 3) return fail(-3, "unknown option payoff code");      // utils/mc_payoffs.py:83-84
   if (variable_type != B200SV_LOG_RETURN && variable_type != B200SV_Q_VAR)
@@ -1564,16 +1565,14 @@ struct ChainIO {
         forwards(forwards_), discfactors(discfactors_), offsets(offsets_), types(types_), st(s), d_strikes(s), d_types(s), d_out(s), d_mom(s),
         d_sums(s) {}
 
-  int upload(const double* strikes) {
-    B200SV_CUDA(d_strikes.alloc(sizeof(double) * Jalloc));
-    B200SV_CUDA(d_types.alloc(Jalloc));
-    B200SV_CUDA(d_out.alloc(sizeof(double) * 3 * Jalloc * B));
-    B200SV_CUDA(d_mom.alloc(sizeof(double) * 2));
-    B200SV_CUDA(d_sums.alloc(sizeof(double) * 3 * Jalloc));
-    if (Jtot > 0) {
-      B200SV_CUDA(cudaMemcpyAsync(d_strikes.p, strikes + offsets[0], sizeof(double) * Jtot, cudaMemcpyHostToDevice, st));
-      B200SV_CUDA(cudaMemcpyAsync(d_types.p, types + offsets[0], Jtot, cudaMemcpyHostToDevice, st));
-    }
+  // K moments, KV payoff sums per strike and R result rows per parameter set: the pricing layout by default, GreeksChainIO's otherwise
+  int upload(const double* strikes, int K = 2, int KV = 3, int R = 3) {
+    B200SV_CUDA(d_out.alloc(sizeof(double) * R * Jalloc * B));
+    B200SV_CUDA(d_mom.alloc(sizeof(double) * K));
+    B200SV_CUDA(d_sums.alloc(sizeof(double) * KV * Jalloc));
+    if (Jtot == 0) return 0;
+    B200SV_CUDA(d_strikes.upload(strikes + offsets[0], Jtot));
+    B200SV_CUDA(d_types.upload(types + offsets[0], Jtot));
     return 0;
   }
   double* moments() const { return d_mom.as<double>(); }
@@ -1602,8 +1601,67 @@ struct ChainIO {
   }
 };
 
-// The [3][n] fp64 path state (x, vol, qvar) of a host-level call on the device, and the caller's three arrays it is uploaded from
-// (alloc(true)) and copied back to (download).
+// The chain of a sensitivity driver over nb_path paths and NP parameter directions: ChainIO with the [2 + NP] moments its tangent launch reduces
+// into, per-strike sums of the payoff and its sensitivities, their partials (sized once for the widest slice), and the result block
+// [prices | std errors | greeks [1 + NP] | greeks_se [1 + NP]][Jalloc].
+template <int NP>
+struct GreeksChainIO : ChainIO {
+  static constexpr int KV = 3 + 2 * (1 + NP);
+  long long n;
+  Grid gp;      // payoff_greeks_kernel's persistent grid, its blocks split across the strike chunks of a slice
+  DevBuf d_part;
+
+  GreeksChainIO(int M_, const double* ttms_, const double* forwards_, const double* discfactors_, const int* offsets_, const int8_t* types_,
+                int variable_type_, long long nb_path, cudaStream_t s)
+      : ChainIO(1, M_, ttms_, forwards_, discfactors_, offsets_, types_, variable_type_, s), n(nb_path),
+        gp(persistent_grid(payoff_greeks_kernel<NP>, kThreads, nb_path)), d_part(s) {}
+
+  int upload(const double* strikes) {
+    int Jmax = 0;
+    for (int m = 0; m < M; ++m) Jmax = std::max(Jmax, offsets[m + 1] - offsets[m]);
+    const int max_chunks = std::max(1, (Jmax + kGreeksStrikeChunk - 1) / kGreeksStrikeChunk);
+    B200SV_CUDA(d_part.alloc(sizeof(double) * (size_t)KV * kGreeksStrikeChunk * max_chunks * gp.blocks));
+    return ChainIO::upload(strikes, 2 + NP, KV, 2 * (2 + NP));
+  }
+
+  // maturity m: per-strike payoff and sensitivity sums over the state (x, q) and its tangents (dx, dq) [NP][n] -> prices, price-row std
+  // errors (/ sqrt(price_paths)) and the 1 + NP sensitivity rows with their standard errors (/ sqrt(n)) into the result block
+  int payoff(int m, const double* x, const double* q, const double* dx, const double* dq, double price_paths) {
+    const int J = offsets[m + 1] - offsets[m], jo = offsets[m] - offsets[0];
+    if (J == 0) return 0;
+    const int chunks = (J + kGreeksStrikeChunk - 1) / kGreeksStrikeChunk;
+    const int Kpad = KV * kGreeksStrikeChunk * chunks;
+    const int blocks = std::max(1, gp.blocks / chunks);
+    payoff_greeks_kernel<NP><<<dim3(blocks, chunks), gp.threads, 0, st>>>(x, q, dx, dq, n, ttms[m], forwards[m], d_strikes.as<double>() + jo,
+                                                                          d_types.as<int8_t>() + jo, J, variable_type, moments(),
+                                                                          d_part.as<double>(), Kpad);
+    if (int rc = check_launch("payoff_greeks_kernel")) return rc;
+    reduce_partials_kernel<<<1, 256, 0, st>>>(d_part.as<double>(), blocks, Kpad, KV * J, d_sums.as<double>(), P2pPublish{});
+    if (int rc = check_launch("reduce_partials_kernel")) return rc;
+    double* o = d_out.as<double>() + jo;
+    greeks_finalize_kernel<<<(J + 127) / 128, 128, 0, st>>>(d_sums.as<double>(), KV, J, Jalloc, discfactors[m], price_paths, (double)n, o,
+                                                            o + Jalloc, o + 2 * Jalloc, o + (size_t)(3 + NP) * Jalloc);
+    return check_launch("greeks_finalize_kernel");
+  }
+
+  // one device-to-host copy of the result block, the synchronisation that ends the call, then the scatter into prices_out, stderr_out [Jtot]
+  // and greeks_out, greeks_se_out [1 + NP][Jtot] (a non-empty chain has Jalloc == Jtot, so the block's rows are already the caller's)
+  int copy_back(StreamSync& sync, double* prices_out, double* stderr_out, double* greeks_out, double* greeks_se_out) const {
+    const size_t J = (size_t)Jtot, G = (size_t)(1 + NP) * J;
+    std::vector<double> h(2 * J + 2 * G);
+    if (J > 0) B200SV_CUDA(d_out.download(h.data(), h.size()));
+    if (int rc = sync.done()) return rc;
+    if (J == 0) return 0;
+    memcpy(prices_out, h.data(), sizeof(double) * J);
+    memcpy(stderr_out, h.data() + J, sizeof(double) * J);
+    memcpy(greeks_out, h.data() + 2 * J, sizeof(double) * G);
+    memcpy(greeks_se_out, h.data() + 2 * J + G, sizeof(double) * G);
+    return 0;
+  }
+};
+
+// The [3][n] fp64 path state (x, vol, qvar) of a host-level call on the device, or its tangents ([3][NP * n]), and the caller's three arrays
+// it is uploaded from (alloc(true)) and copied back to (download).
 struct HostState {
   double* h[3];
   size_t n;
@@ -1741,7 +1799,7 @@ static int mc_chain_host(const Params* params, int M, const double* ttms, const 
   B200SV_REQUIRE(B >= 1, "B must be >= 1");
   B200SV_REQUIRE(nb_path >= 1, "nb_path must be >= 1");
   B200SV_REQUIRE(nb_steps_per_year >= 1, "nb_steps_per_year must be >= 1");
-  if (int rc = validate_chain(M, ttms, offsets, types, variable_type)) return rc;
+  if (int rc = validate_chain(M, ttms, offsets, strikes, types, variable_type)) return rc;
   if (use_coop_chain(flags, nb_path, std::is_same<Params, b200sv_heston_params>::value))
     return mc_chain_host_coop(params, M, ttms, forwards, discfactors, etas, offsets, strikes, types, nb_path, nb_steps_per_year, is_spot,
                               variable_type, seed, flags, prices_out, stderr_out, scheme, B, ivols_out);
@@ -1827,33 +1885,22 @@ static int mc_chain_greeks_host(const Params& p, int M, const double* ttms, cons
                                 int is_spot, int variable_type, uint64_t seed, int flags, double* prices_out, double* stderr_out,
                                 double* greeks_out, double* greeks_se_out) {
   using TConsts = decltype(tangent_consts(p, 1.0, false, 1.0));
-  constexpr int NP = TangentPathOf<TConsts>::NP, KV = 3 + 2 * (1 + NP);
+  constexpr int NP = TangentPathOf<TConsts>::NP;
   B200SV_REQUIRE(nb_path >= 1, "nb_path must be >= 1");
   B200SV_REQUIRE(nb_steps_per_year >= 1, "nb_steps_per_year must be >= 1");
-  if (int rc = validate_chain(M, ttms, offsets, types, variable_type)) return rc;
+  if (int rc = validate_chain(M, ttms, offsets, strikes, types, variable_type)) return rc;
   const int gauss = greeks_gauss(flags);
   if (gauss < 0) return gauss;
-  const int Jtot = offsets[M] - offsets[0], Jalloc = std::max(Jtot, 1);
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
   StreamSync sync(st);
   const size_t n = (size_t)nb_path;
-  const size_t state_doubles = 3 * n + 3 * (size_t)NP * n;
-  const size_t out_doubles = 2 * (size_t)Jalloc * (2 + NP);        // prices, std errors, greeks [1+P][J], greeks_se [1+P][J]
-  DevBuf d_state(st), d_strikes(st), d_types(st), d_out(st), d_mom(st), d_sums(st);
-  B200SV_CUDA(d_state.alloc(sizeof(double) * state_doubles));
-  B200SV_CUDA(d_strikes.alloc(sizeof(double) * Jalloc));
-  B200SV_CUDA(d_types.alloc(Jalloc));
-  B200SV_CUDA(d_out.alloc(sizeof(double) * out_doubles));
-  B200SV_CUDA(d_mom.alloc(sizeof(double) * (2 + NP)));
-  B200SV_CUDA(d_sums.alloc(sizeof(double) * KV * Jalloc));
-  if (Jtot > 0) {
-    B200SV_CUDA(cudaMemcpyAsync(d_strikes.p, strikes + offsets[0], sizeof(double) * Jtot, cudaMemcpyHostToDevice, st));
-    B200SV_CUDA(cudaMemcpyAsync(d_types.p, types + offsets[0], Jtot, cudaMemcpyHostToDevice, st));
-  }
+  DevBuf d_state(st);
+  GreeksChainIO<NP> io(M, ttms, forwards, discfactors, offsets, types, variable_type, nb_path, st);
+  B200SV_CUDA(d_state.alloc(sizeof(double) * (3 * n + 3 * (size_t)NP * n)));
+  if (int rc = io.upload(strikes)) return rc;
   double *x = d_state.as<double>(), *v = x + n, *q = v + n;
   const TangentState t{q + n, q + n + NP * n, q + n + 2 * NP * n};
-  double *o_price = d_out.as<double>(), *o_se = o_price + Jalloc, *o_g = o_se + Jalloc, *o_gse = o_g + (size_t)(1 + NP) * Jalloc;
   double t0 = 0.0;
   for (int m = 0; m < M; ++m) {
     int S;
@@ -1861,34 +1908,10 @@ static int mc_chain_greeks_host(const Params& p, int M, const double* ttms, cons
     time_grid(ttms[m] - t0, nb_steps_per_year, &S, &dt);
     t0 = ttms[m];
     const TConsts c = tangent_consts(p, etas ? etas[m] : 1.0, is_spot != 0, dt);
-    if (int rc = launch_tangent_slice(gauss, x, v, q, t, nb_path, 0, m == 0, v_init(p), S, m, forwards[m], seed, c, d_mom.as<double>(), st)) return rc;
-    const int J = offsets[m + 1] - offsets[m], jo = offsets[m] - offsets[0];
-    if (J == 0) continue;
-    const int chunks = (J + kGreeksStrikeChunk - 1) / kGreeksStrikeChunk;
-    const int Kpad = KV * kGreeksStrikeChunk * chunks;
-    Grid g = persistent_grid(payoff_greeks_kernel<NP>, kThreads, nb_path);
-    g.blocks = std::max(1, g.blocks / chunks);
-    DevBuf partials(st);
-    B200SV_CUDA(partials.alloc(sizeof(double) * (size_t)Kpad * g.blocks));
-    payoff_greeks_kernel<NP><<<dim3(g.blocks, chunks), g.threads, 0, st>>>(x, q, t.dx, t.dq, nb_path, ttms[m], forwards[m], d_strikes.as<double>() + jo,
-                                                                           d_types.as<int8_t>() + jo, J, variable_type, d_mom.as<double>(),
-                                                                           partials.as<double>(), Kpad);
-    if (int rc = check_launch("payoff_greeks_kernel")) return rc;
-    reduce_partials_kernel<<<1, 256, 0, st>>>(partials.as<double>(), g.blocks, Kpad, KV * J, d_sums.as<double>(), P2pPublish{});
-    if (int rc = check_launch("reduce_partials_kernel")) return rc;
-    greeks_finalize_kernel<<<(J + 127) / 128, 128, 0, st>>>(d_sums.as<double>(), KV, J, Jalloc, discfactors[m], (double)nb_path, (double)nb_path,
-                                                            o_price + jo, o_se + jo, o_g + jo, o_gse + jo);
-    if (int rc = check_launch("greeks_finalize_kernel")) return rc;
+    if (int rc = launch_tangent_slice(gauss, x, v, q, t, nb_path, 0, m == 0, v_init(p), S, m, forwards[m], seed, c, io.moments(), st)) return rc;
+    if (int rc = io.payoff(m, x, q, t.dx, t.dq, (double)nb_path)) return rc;
   }
-  if (Jtot > 0) {
-    B200SV_CUDA(cudaMemcpyAsync(prices_out, o_price, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st));
-    B200SV_CUDA(cudaMemcpyAsync(stderr_out, o_se, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st));
-    for (int k = 0; k < 1 + NP; ++k) {
-      B200SV_CUDA(cudaMemcpyAsync(greeks_out + (size_t)k * Jtot, o_g + (size_t)k * Jalloc, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st));
-      B200SV_CUDA(cudaMemcpyAsync(greeks_se_out + (size_t)k * Jtot, o_gse + (size_t)k * Jalloc, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st));
-    }
-  }
-  return sync.done();
+  return io.copy_back(sync, prices_out, stderr_out, greeks_out, greeks_se_out);
 }
 
 // one slice from the initial state (0, v_init, 0) with initial tangents, for paths [path_offset, path_offset + n) of Philox slice
@@ -1907,12 +1930,12 @@ static int tangent_terminal_host(const Params& p, double ttm, long long nb_path,
   ensure_pool_threshold();
   StreamSync sync(st);
   const size_t n = (size_t)nb_path;
-  HostState s(x, v, q, nb_path, st);
-  DevBuf d_tan(st), d_mom(st);
+  HostState s(x, v, q, nb_path, st), ds(dx, dv, dq, NP * nb_path, st);
+  DevBuf d_mom(st);
   if (int rc = s.alloc(false)) return rc;
-  B200SV_CUDA(d_tan.alloc(sizeof(double) * 3 * (size_t)NP * n));
+  if (int rc = ds.alloc(false)) return rc;
   B200SV_CUDA(d_mom.alloc(sizeof(double) * (2 + NP)));
-  const TangentState t{d_tan.as<double>(), d_tan.as<double>() + NP * n, d_tan.as<double>() + 2 * NP * n};
+  const TangentState t{ds.dev(0), ds.dev(1), ds.dev(2)};
   int S;
   double dt;
   time_grid(ttm, nb_steps_per_year, &S, &dt);
@@ -1921,9 +1944,7 @@ static int tangent_terminal_host(const Params& p, double ttm, long long nb_path,
                                     d_mom.as<double>(), st))
     return rc;
   if (int rc = s.download()) return rc;
-  double* dst[3] = {dx, dv, dq};
-  const double* src[3] = {t.dx, t.dv, t.dq};
-  for (int k = 0; k < 3; ++k) B200SV_CUDA(cudaMemcpyAsync(dst[k], src[k], sizeof(double) * NP * n, cudaMemcpyDeviceToHost, st));
+  if (int rc = ds.download()) return rc;
   if (int rc = sync.done()) return rc;
   if (std::is_same<Params, b200sv_logsv_params>::value)
     for (size_t k = 0; k < (size_t)NP; ++k)

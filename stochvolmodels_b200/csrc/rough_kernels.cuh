@@ -218,30 +218,25 @@ __global__ void __launch_bounds__(kThreads) rough_logsv_kernel(double* __restric
   }
 }
 
-template <int N>
-static int launch_rough_n(double* ls, double* vol, double* qv, const double* Z0, const double* Z1, int S, long long P, const RoughConsts& c,
-                          uint64_t seed, long long path_offset, int gauss, cudaStream_t st) {
-  Grid g = persistent_grid(rough_logsv_kernel<N, kGaussF32>, kThreads, P);
-  if (gauss == kGaussF64)
-    rough_logsv_kernel<N, kGaussF64><<<g.blocks, g.threads, 0, st>>>(ls, vol, qv, Z0, Z1, S, P, c, seed, (unsigned long long)path_offset);
+// the factor count n picks the template instantiation: f(std::integral_constant<int, n>{}) for n in 1..8
+template <int N = 1, class F>
+static int with_factors(int n, F&& f) {
+  if constexpr (N > kMaxRoughFactors)
+    return fail(-1, "invalid argument: the rough-vol kernel supports 1..8 factors");
   else
-    rough_logsv_kernel<N, kGaussF32><<<g.blocks, g.threads, 0, st>>>(ls, vol, qv, Z0, Z1, S, P, c, seed, (unsigned long long)path_offset);
-  return check_launch("rough_logsv_kernel");
+    return n == N ? f(std::integral_constant<int, N>{}) : with_factors<N + 1>(n, f);
 }
 
+// Both Gauss modes launch on the grid of the fp32-draw instantiation.
 static int launch_rough(int n, double* ls, double* vol, double* qv, const double* Z0, const double* Z1, int S, long long P, const RoughConsts& c,
                         uint64_t seed, long long path_offset, int gauss, cudaStream_t st) {
-  switch (n) {
-    case 1: return launch_rough_n<1>(ls, vol, qv, Z0, Z1, S, P, c, seed, path_offset, gauss, st);
-    case 2: return launch_rough_n<2>(ls, vol, qv, Z0, Z1, S, P, c, seed, path_offset, gauss, st);
-    case 3: return launch_rough_n<3>(ls, vol, qv, Z0, Z1, S, P, c, seed, path_offset, gauss, st);
-    case 4: return launch_rough_n<4>(ls, vol, qv, Z0, Z1, S, P, c, seed, path_offset, gauss, st);
-    case 5: return launch_rough_n<5>(ls, vol, qv, Z0, Z1, S, P, c, seed, path_offset, gauss, st);
-    case 6: return launch_rough_n<6>(ls, vol, qv, Z0, Z1, S, P, c, seed, path_offset, gauss, st);
-    case 7: return launch_rough_n<7>(ls, vol, qv, Z0, Z1, S, P, c, seed, path_offset, gauss, st);
-    case 8: return launch_rough_n<8>(ls, vol, qv, Z0, Z1, S, P, c, seed, path_offset, gauss, st);
-  }
-  return fail(-1, "invalid argument: the rough-vol kernel supports 1..8 factors");
+  return with_factors(n, [&](auto nf) {
+    constexpr int N = decltype(nf)::value;
+    const Grid g = persistent_grid(rough_logsv_kernel<N, kGaussF32>, kThreads, P);
+    const auto kernel = gauss == kGaussF64 ? rough_logsv_kernel<N, kGaussF64> : rough_logsv_kernel<N, kGaussF32>;
+    kernel<<<g.blocks, g.threads, 0, st>>>(ls, vol, qv, Z0, Z1, S, P, c, seed, (unsigned long long)path_offset);
+    return check_launch("rough_logsv_kernel");
+  });
 }
 
 // --------------------------------------------------------------------------------------------------------------------
@@ -458,48 +453,54 @@ __global__ void __launch_bounds__(kThreads) rough_logsv_tangent_kernel(double* _
   }
 }
 
-template <int N>
-static int launch_rough_tangent_n(double* ls, double* vol, double* qv, double* dls, double* dvol, double* dqv, const double* Z0, const double* Z1,
-                                  int S, long long P, const RoughConsts& c, const RoughTangentConsts& k, uint64_t seed, int gauss, double forward,
-                                  double* partials, int blocks, cudaStream_t st) {
-  if (gauss == kGaussF64)
-    rough_logsv_tangent_kernel<N, kGaussF64><<<blocks, kThreads, 0, st>>>(ls, vol, qv, dls, dvol, dqv, Z0, Z1, S, P, c, k, seed, forward, partials);
-  else
-    rough_logsv_tangent_kernel<N, kGaussF32><<<blocks, kThreads, 0, st>>>(ls, vol, qv, dls, dvol, dqv, Z0, Z1, S, P, c, k, seed, forward, partials);
-  return check_launch("rough_logsv_tangent_kernel");
-}
-
-template <int N>
-static int rough_tangent_blocks(long long P) {
-  return persistent_grid(rough_logsv_tangent_kernel<N, kGaussF32>, kThreads, P).blocks;
-}
-
-static int rough_tangent_grid(int n, long long P) {
-  switch (n) {
-    case 1: return rough_tangent_blocks<1>(P);
-    case 2: return rough_tangent_blocks<2>(P);
-    case 3: return rough_tangent_blocks<3>(P);
-    case 4: return rough_tangent_blocks<4>(P);
-    case 5: return rough_tangent_blocks<5>(P);
-    case 6: return rough_tangent_blocks<6>(P);
-    case 7: return rough_tangent_blocks<7>(P);
-    case 8: return rough_tangent_blocks<8>(P);
-  }
-  return 0;
-}
-
+// one maturity of the rough chain with tangents, then moments_out[2 + 6] = (sum F e^ls, count, sum F e^ls dls_q).  Both Gauss modes launch on
+// the grid of the fp32-draw instantiation: the block count fixes the order of the moments' reduction.
 static int launch_rough_tangent(int n, double* ls, double* vol, double* qv, double* dls, double* dvol, double* dqv, const double* Z0,
                                 const double* Z1, int S, long long P, const RoughConsts& c, const RoughTangentConsts& k, uint64_t seed, int gauss,
-                                double forward, double* partials, int blocks, cudaStream_t st) {
-#define B200SV_ROUGH_TANGENT_CASE(NF) \
-  case NF: return launch_rough_tangent_n<NF>(ls, vol, qv, dls, dvol, dqv, Z0, Z1, S, P, c, k, seed, gauss, forward, partials, blocks, st);
-  switch (n) {
-    B200SV_ROUGH_TANGENT_CASE(1) B200SV_ROUGH_TANGENT_CASE(2) B200SV_ROUGH_TANGENT_CASE(3) B200SV_ROUGH_TANGENT_CASE(4)
-    B200SV_ROUGH_TANGENT_CASE(5) B200SV_ROUGH_TANGENT_CASE(6) B200SV_ROUGH_TANGENT_CASE(7) B200SV_ROUGH_TANGENT_CASE(8)
-  }
-#undef B200SV_ROUGH_TANGENT_CASE
-  return fail(-1, "invalid argument: the rough-vol kernel supports 1..8 factors");
+                                double forward, double* moments_out, cudaStream_t st) {
+  constexpr int K = 2 + kRoughParams;
+  return with_factors(n, [&](auto nf) {
+    constexpr int N = decltype(nf)::value;
+    const int blocks = persistent_grid(rough_logsv_tangent_kernel<N, kGaussF32>, kThreads, P).blocks;
+    const auto kernel = gauss == kGaussF64 ? rough_logsv_tangent_kernel<N, kGaussF64> : rough_logsv_tangent_kernel<N, kGaussF32>;
+    DevBuf partials(st);
+    B200SV_CUDA(partials.alloc(sizeof(double) * K * (size_t)blocks));
+    kernel<<<blocks, kThreads, 0, st>>>(ls, vol, qv, dls, dvol, dqv, Z0, Z1, S, P, c, k, seed, forward, partials.as<double>());
+    if (int rc = check_launch("rough_logsv_tangent_kernel")) return rc;
+    reduce_partials_kernel<<<1, 64, 0, st>>>(partials.as<double>(), blocks, K, K, moments_out, P2pPublish{});
+    return check_launch("reduce_partials_kernel");
+  });
 }
+
+// The argument checks both rough chain drivers make after their own factor-count check, and the caller's normals: the Gauss mode, the longest
+// grid Smax, and Z0 / Z1 [Smax][P] on the device (left null with in-kernel Philox draws).
+struct RoughChainArgs {
+  int gauss = 0, Smax = 0;
+  DevBuf z0, z1;
+  explicit RoughChainArgs(cudaStream_t st) : z0(st), z1(st) {}
+
+  int check(long long nb_path, const double* Z0, const double* Z1, long long z_rows, int M, const double* ttms, const int* offsets,
+            const double* strikes, const int8_t* types, int variable_type, int flags, const int* nsteps, const double* hs) {
+    B200SV_REQUIRE(nb_path >= 1, "nb_path must be >= 1");
+    B200SV_REQUIRE((Z0 == nullptr) == (Z1 == nullptr), "Z0 and Z1 must be supplied together");
+    if (int rc = validate_chain(M, ttms, offsets, strikes, types, variable_type)) return rc;
+    gauss = gauss_mode(flags);
+    B200SV_REQUIRE(gauss == kGaussF32 || gauss == kGaussF64, "gauss flags");
+    B200SV_REQUIRE(!(flags & B200SV_STATE_F32), "the rough-vol route is float64 only");
+    for (int m = 0; m < M; ++m) {
+      B200SV_REQUIRE(nsteps[m] >= 1 && hs[m] > 0.0, "nsteps / h must be positive");
+      Smax = std::max(Smax, nsteps[m]);
+    }
+    B200SV_REQUIRE(!Z0 || z_rows >= Smax, "Z0 / Z1 have fewer rows than the longest grid");
+    return 0;
+  }
+  int upload(const double* Z0, const double* Z1, long long nb_path) {
+    if (!Z0) return 0;
+    B200SV_CUDA(z0.upload(Z0, (size_t)Smax * nb_path));
+    B200SV_CUDA(z1.upload(Z1, (size_t)Smax * nb_path));
+    return 0;
+  }
+};
 
 // host-level chain driver: B parameter sets x M maturities on ONE upload of the normals (or none at all with Philox draws)
 static int rough_chain_host(const b200sv_logsv_params* params, int B, int n, const double* weights /*[B][n]*/, const double* nodes /*[B][n]*/, int M,
@@ -508,38 +509,23 @@ static int rough_chain_host(const b200sv_logsv_params* params, int B, int n, con
                             const double* Z1, long long z_rows, int variable_type, uint64_t seed, int flags, double* prices_out,
                             double* stderr_out, double* ivols_out, double* states_out /* B == 1: [M][(n+2)][P] log_spot, vol[n], qv */) {
   B200SV_REQUIRE(B >= 1 && n >= 1 && n <= kMaxRoughFactors, "B >= 1 and 1 <= n_factors <= 8");
-  B200SV_REQUIRE(nb_path >= 1, "nb_path must be >= 1");
-  B200SV_REQUIRE((Z0 == nullptr) == (Z1 == nullptr), "Z0 and Z1 must be supplied together");
   B200SV_REQUIRE(!states_out || B == 1, "terminal states are returned for a single parameter set");
-  if (int rc = validate_chain(M, ttms, offsets, types, variable_type)) return rc;
-  const int g = gauss_mode(flags);
-  B200SV_REQUIRE(g == kGaussF32 || g == kGaussF64, "gauss flags");
-  B200SV_REQUIRE(!(flags & B200SV_STATE_F32), "the rough-vol route is float64 only");
-  int Smax = 0;
-  for (int m = 0; m < M; ++m) {
-    B200SV_REQUIRE(nsteps[m] >= 1 && hs[m] > 0.0, "nsteps / h must be positive");
-    Smax = std::max(Smax, nsteps[m]);
-  }
-  B200SV_REQUIRE(!Z0 || z_rows >= Smax, "Z0 / Z1 have fewer rows than the longest grid");
   cudaStream_t st = current_stream();
+  RoughChainArgs a(st);
+  if (int rc = a.check(nb_path, Z0, Z1, z_rows, M, ttms, offsets, strikes, types, variable_type, flags, nsteps, hs)) return rc;
   ensure_pool_threshold();
   StreamSync sync(st);
   const size_t P = (size_t)nb_path;
-  DevBuf d_state(st), d_z(st);
+  DevBuf d_state(st);
   ChainIO io(B, M, ttms, forwards, discfactors, offsets, types, variable_type, st);
   B200SV_CUDA(d_state.alloc(sizeof(double) * (size_t)(n + 2) * P));
-  if (Z0) {
-    B200SV_CUDA(d_z.alloc(sizeof(double) * 2 * (size_t)Smax * P));
-    B200SV_CUDA(cudaMemcpyAsync(d_z.p, Z0, sizeof(double) * (size_t)Smax * P, cudaMemcpyHostToDevice, st));
-    B200SV_CUDA(cudaMemcpyAsync(d_z.as<double>() + (size_t)Smax * P, Z1, sizeof(double) * (size_t)Smax * P, cudaMemcpyHostToDevice, st));
-  }
+  if (int rc = a.upload(Z0, Z1, nb_path)) return rc;
   if (int rc = io.upload(strikes)) return rc;
   double *d_ls = d_state.as<double>(), *d_vol = d_ls + P, *d_qv = d_ls + (size_t)(n + 1) * P;
-  const double *z0 = d_z.as<double>(), *z1 = Z0 ? z0 + (size_t)Smax * P : nullptr;
   for (int b = 0; b < B; ++b) {
     for (int m = 0; m < M; ++m) {
       const RoughConsts c = make_rough_consts(params[b], n, weights + (size_t)b * n, nodes + (size_t)b * n, hs[m]);
-      if (int rc = launch_rough(n, d_ls, d_vol, d_qv, z0, z1, nsteps[m], nb_path, c, seed, 0, g, st)) return rc;
+      if (int rc = launch_rough(n, d_ls, d_vol, d_qv, a.z0.as<double>(), a.z1.as<double>(), nsteps[m], nb_path, c, seed, 0, a.gauss, st)) return rc;
       if (states_out)
         B200SV_CUDA(cudaMemcpyAsync(states_out + (size_t)m * (n + 2) * P, d_ls, sizeof(double) * (size_t)(n + 2) * P, cudaMemcpyDeviceToHost, st));
       // the reference hands (1, nb_path)-shaped arrays to compute_mc_vars_payoff, whose "/ sqrt(x0.shape[0])" is then "/ 1":
@@ -559,67 +545,32 @@ static int rough_chain_greeks_host(const b200sv_logsv_params& p, int n, const do
                                    long long nb_path, const int* nsteps, const double* hs, const double* Z0, const double* Z1, long long z_rows,
                                    int variable_type, uint64_t seed, int flags, double* prices_out, double* stderr_out, double* greeks_out,
                                    double* greeks_se_out, double* states_out, double* tangents_out, double* resets_out) {
-  constexpr int NP = kRoughParams, K = 2 + NP, KV = 3 + 2 * (1 + NP);
+  constexpr int NP = kRoughParams;
   B200SV_REQUIRE(n >= 1 && n <= kMaxRoughFactors, "1 <= n_factors <= 8");
-  B200SV_REQUIRE(nb_path >= 1, "nb_path must be >= 1");
-  B200SV_REQUIRE((Z0 == nullptr) == (Z1 == nullptr), "Z0 and Z1 must be supplied together");
-  if (int rc = validate_chain(M, ttms, offsets, types, variable_type)) return rc;
-  const int g = gauss_mode(flags);
-  B200SV_REQUIRE(g == kGaussF32 || g == kGaussF64, "gauss flags");
-  B200SV_REQUIRE(!(flags & B200SV_STATE_F32), "the rough-vol route is float64 only");
-  int Smax = 0;
-  for (int m = 0; m < M; ++m) {
-    B200SV_REQUIRE(nsteps[m] >= 1 && hs[m] > 0.0, "nsteps / h must be positive");
-    Smax = std::max(Smax, nsteps[m]);
-  }
-  B200SV_REQUIRE(!Z0 || z_rows >= Smax, "Z0 / Z1 have fewer rows than the longest grid");
-  const int Jtot = offsets[M] - offsets[0], Jalloc = std::max(Jtot, 1);
   cudaStream_t st = current_stream();
+  RoughChainArgs a(st);
+  if (int rc = a.check(nb_path, Z0, Z1, z_rows, M, ttms, offsets, strikes, types, variable_type, flags, nsteps, hs)) return rc;
   ensure_pool_threshold();
   StreamSync sync(st);
   const size_t P = (size_t)nb_path;
-  const int blocks = rough_tangent_grid(n, nb_path);
-  DevBuf d_state(st), d_tan(st), d_dvol(st), d_z(st), d_strikes(st), d_types(st), d_out(st), d_mom(st), d_sums(st), d_part(st), d_gpart(st),
-      d_resets(st);
+  DevBuf d_state(st), d_tan(st), d_dvol(st), d_resets(st);
+  GreeksChainIO<NP> io(M, ttms, forwards, discfactors, offsets, types, variable_type, nb_path, st);
   B200SV_CUDA(d_state.alloc(sizeof(double) * (size_t)(n + 2) * P));
   B200SV_CUDA(d_tan.alloc(sizeof(double) * 2 * NP * P));
   if (tangents_out) B200SV_CUDA(d_dvol.alloc(sizeof(double) * (size_t)NP * n * P));
-  B200SV_CUDA(d_strikes.alloc(sizeof(double) * Jalloc));
-  B200SV_CUDA(d_types.alloc(Jalloc));
-  B200SV_CUDA(d_out.alloc(sizeof(double) * 2 * (size_t)Jalloc * (2 + NP)));
-  B200SV_CUDA(d_mom.alloc(sizeof(double) * K));
-  B200SV_CUDA(d_sums.alloc(sizeof(double) * KV * Jalloc));
-  B200SV_CUDA(d_part.alloc(sizeof(double) * K * (size_t)blocks));
   B200SV_CUDA(d_resets.alloc(sizeof(unsigned long long) * M));
   B200SV_CUDA(cudaMemsetAsync(d_resets.p, 0, sizeof(unsigned long long) * M, st));
-  // payoff_greeks_kernel: one grid shape per chunk count, partials sized for the widest slice
-  int Jmax = 0;
-  for (int m = 0; m < M; ++m) Jmax = std::max(Jmax, offsets[m + 1] - offsets[m]);
-  const int max_chunks = std::max(1, (Jmax + kGreeksStrikeChunk - 1) / kGreeksStrikeChunk);
-  const Grid gp = persistent_grid(payoff_greeks_kernel<NP>, kThreads, nb_path);
-  B200SV_CUDA(d_gpart.alloc(sizeof(double) * (size_t)KV * kGreeksStrikeChunk * max_chunks * gp.blocks));
-  if (Z0) {
-    B200SV_CUDA(d_z.alloc(sizeof(double) * 2 * (size_t)Smax * P));
-    B200SV_CUDA(cudaMemcpyAsync(d_z.p, Z0, sizeof(double) * (size_t)Smax * P, cudaMemcpyHostToDevice, st));
-    B200SV_CUDA(cudaMemcpyAsync(d_z.as<double>() + (size_t)Smax * P, Z1, sizeof(double) * (size_t)Smax * P, cudaMemcpyHostToDevice, st));
-  }
-  if (Jtot > 0) {
-    B200SV_CUDA(cudaMemcpyAsync(d_strikes.p, strikes + offsets[0], sizeof(double) * Jtot, cudaMemcpyHostToDevice, st));
-    B200SV_CUDA(cudaMemcpyAsync(d_types.p, types + offsets[0], Jtot, cudaMemcpyHostToDevice, st));
-  }
+  if (int rc = a.upload(Z0, Z1, nb_path)) return rc;
+  if (int rc = io.upload(strikes)) return rc;
   double *d_ls = d_state.as<double>(), *d_vol = d_ls + P, *d_qv = d_ls + (size_t)(n + 1) * P;
-  double *d_dls = d_tan.as<double>(), *d_dqv = d_dls + NP * P, *d_dv = d_dvol.as<double>();
-  const double *z0 = d_z.as<double>(), *z1 = Z0 ? z0 + (size_t)Smax * P : nullptr;
-  double *o_price = d_out.as<double>(), *o_se = o_price + Jalloc, *o_g = o_se + Jalloc, *o_gse = o_g + (size_t)(1 + NP) * Jalloc;
+  double *d_dls = d_tan.as<double>(), *d_dqv = d_dls + NP * P, *d_dv = d_dvol.as<double>();      // d_dv: null without tangents_out
   for (int m = 0; m < M; ++m) {
     const RoughConsts c = make_rough_consts(p, n, weights, nodes, hs[m]);
     RoughTangentConsts k = make_rough_tangent_consts(p, c);
     k.reset_count = d_resets.as<unsigned long long>() + m;
-    if (int rc = launch_rough_tangent(n, d_ls, d_vol, d_qv, d_dls, tangents_out ? d_dv : nullptr, d_dqv, z0, z1, nsteps[m], nb_path, c, k, seed, g,
-                                      forwards[m], d_part.as<double>(), blocks, st))
+    if (int rc = launch_rough_tangent(n, d_ls, d_vol, d_qv, d_dls, d_dv, d_dqv, a.z0.as<double>(), a.z1.as<double>(), nsteps[m], nb_path, c, k, seed,
+                                      a.gauss, forwards[m], io.moments(), st))
       return rc;
-    reduce_partials_kernel<<<1, 64, 0, st>>>(d_part.as<double>(), blocks, K, K, d_mom.as<double>(), P2pPublish{});
-    if (int rc = check_launch("reduce_partials_kernel")) return rc;
     if (states_out)
       B200SV_CUDA(cudaMemcpyAsync(states_out + (size_t)m * (n + 2) * P, d_ls, sizeof(double) * (size_t)(n + 2) * P, cudaMemcpyDeviceToHost, st));
     if (tangents_out) {
@@ -630,33 +581,12 @@ static int rough_chain_greeks_host(const b200sv_logsv_params& p, int n, const do
         B200SV_CUDA(cudaMemcpyAsync(o + (size_t)(n + 1) * P, d_dqv + q * P, sizeof(double) * P, cudaMemcpyDeviceToHost, st));
       }
     }
-    const int J = offsets[m + 1] - offsets[m], jo = offsets[m] - offsets[0];
-    if (J == 0) continue;
-    const int chunks = (J + kGreeksStrikeChunk - 1) / kGreeksStrikeChunk;
-    const int Kpad = KV * kGreeksStrikeChunk * chunks;
-    const int gblocks = std::max(1, gp.blocks / chunks);
-    payoff_greeks_kernel<NP><<<dim3(gblocks, chunks), gp.threads, 0, st>>>(d_ls, d_qv, d_dls, d_dqv, nb_path, ttms[m], forwards[m],
-                                                                           d_strikes.as<double>() + jo, d_types.as<int8_t>() + jo, J, variable_type,
-                                                                           d_mom.as<double>(), d_gpart.as<double>(), Kpad);
-    if (int rc = check_launch("payoff_greeks_kernel")) return rc;
-    reduce_partials_kernel<<<1, 256, 0, st>>>(d_gpart.as<double>(), gblocks, Kpad, KV * J, d_sums.as<double>(), P2pPublish{});
-    if (int rc = check_launch("reduce_partials_kernel")) return rc;
     // the price row keeps the route's un-normalised std (total_paths = 1), the sensitivity rows are standard errors
-    greeks_finalize_kernel<<<(J + 127) / 128, 128, 0, st>>>(d_sums.as<double>(), KV, J, Jalloc, discfactors[m], 1.0, (double)nb_path,
-                                                            o_price + jo, o_se + jo, o_g + jo, o_gse + jo);
-    if (int rc = check_launch("greeks_finalize_kernel")) return rc;
-  }
-  if (Jtot > 0) {
-    B200SV_CUDA(cudaMemcpyAsync(prices_out, o_price, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st));
-    B200SV_CUDA(cudaMemcpyAsync(stderr_out, o_se, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st));
-    for (int q = 0; q < 1 + NP; ++q) {
-      B200SV_CUDA(cudaMemcpyAsync(greeks_out + (size_t)q * Jtot, o_g + (size_t)q * Jalloc, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st));
-      B200SV_CUDA(cudaMemcpyAsync(greeks_se_out + (size_t)q * Jtot, o_gse + (size_t)q * Jalloc, sizeof(double) * Jtot, cudaMemcpyDeviceToHost, st));
-    }
+    if (int rc = io.payoff(m, d_ls, d_qv, d_dls, d_dqv, 1.0)) return rc;
   }
   std::vector<unsigned long long> h_resets(M);
-  B200SV_CUDA(cudaMemcpyAsync(h_resets.data(), d_resets.p, sizeof(unsigned long long) * M, cudaMemcpyDeviceToHost, st));
-  if (int rc = sync.done()) return rc;
+  B200SV_CUDA(d_resets.download(h_resets.data(), M));
+  if (int rc = io.copy_back(sync, prices_out, stderr_out, greeks_out, greeks_se_out)) return rc;
   for (int m = 0; m < M && resets_out; ++m) resets_out[m] = (double)h_resets[m];
   return 0;
 }
