@@ -286,6 +286,19 @@ int b200sv_rough_logsv_mc_chain_greeks(const b200sv_logsv_params* params, int n_
 int b200sv_hawkesjd_mc_chain(const b200sv_hawkes_params* params, int M, const double* ttms, const double* forwards, const double* discfactors,
                              const int* offsets, const double* strikes, const int8_t* types, long long nb_path, int variable_type, uint64_t seed,
                              int flags, double* prices_out, double* stderr_out);
+/* b200sv_hawkesjd_mc_chain with Monte Carlo sensitivities (DESIGN.md §3.11): arguments as b200sv_hawkesjd_mc_chain, then
+ * greeks_out / greeks_se_out [1 + 15][J]: the forward delta, then d price / d parameter in the order sigma, shift_p, mean_p, shift_m, mean_m,
+ * lambda_p, theta_p, kappa_p, beta1_p, beta2_p, lambda_m, theta_m, kappa_m, beta1_m, beta2_m, each with its standard error df std(g) / sqrt(N).
+ * Pathwise through the diffusion, the jump sizes and the intensities with the firing decisions frozen, plus the likelihood-ratio score of
+ * the decisions; unbiased for the discretised scheme.  prices_out / stderr_out are bit-identical to b200sv_hawkesjd_mc_chain on the same
+ * nb_path, seed and flags.  LOG_RETURN only (Q_VAR returns -4), fp64 state, B200SV_GAUSS_F32 or B200SV_GAUSS_F64, mean_p != 0 and
+ * mean_m != 0 (dJ/dmean = (J - shift)/mean).
+ * Optional per-path outputs for paths [0, n_paths_out) (test hook; each may be NULL): states_out [M][3][n_paths_out] = (x, lambda_p,
+ * lambda_m) after maturity m; tangents_out [M][4][15][n_paths_out] = (dx, dlambda_p, dlambda_m, accumulated score) per direction. */
+int b200sv_hawkesjd_mc_chain_greeks(const b200sv_hawkes_params* params, int M, const double* ttms, const double* forwards,
+                                    const double* discfactors, const int* offsets, const double* strikes, const int8_t* types, long long nb_path,
+                                    int variable_type, uint64_t seed, int flags, double* prices_out, double* stderr_out, double* greeks_out,
+                                    double* greeks_se_out, long long n_paths_out, double* states_out, double* tangents_out);
 /* Hawkes jump-diffusion, Fourier route.  Replaces hawkesjd_chain_pricer (pricers/hawkes_jd_pricer.py:365-417) and, with a finite
  * risk_premia_gamma, hawkesjd_chain_pricer_with_risk_premia (:420-484) incl. hawkesjd_forwards_under_risk_kernel (:487-515),
  * compute_hawkes_a_mgf_grid / solve_ode_for_a (:518-641: SciPy RK45 per transform point) and the slice pricers of utils/mgf_pricer.py

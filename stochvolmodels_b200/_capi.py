@@ -81,6 +81,8 @@ SIGNATURES = {
     "b200sv_rough_logsv_mc_chain_greeks": [_lp, c_int, _dp, _dp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_longlong, _ip, _dp, _dp, _dp, c_longlong,
                                            c_int, c_uint64, c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp],
     "b200sv_hawkesjd_mc_chain": [_kp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_longlong, c_int, c_uint64, c_int, _dp, _dp],
+    "b200sv_hawkesjd_mc_chain_greeks": [_kp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_longlong, c_int, c_uint64, c_int, _dp, _dp, _dp, _dp,
+                                        c_longlong, _dp, _dp],
     "b200sv_hawkesjd_price_chain": [_kp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_double, c_int, c_double, _dp, _dp, _dp, _dp, _dp],
     "b200sv_hawkesjd_mgf_grid": [_dp, _dp, c_int, c_double, _dp, _kp, _dp],
     "b200sv_fourier_gamma": [_dp, _dp, c_int, c_double, c_double, c_double, c_double, _dp, _i8p, c_int, c_int, _dp],

@@ -139,13 +139,84 @@ __device__ __noinline__ double2 hawkes_two_sizes(uint32_t wx, uint32_t wy, doubl
 #ifndef B200SV_HAWKES_MINBLOCKS
 #define B200SV_HAWKES_MINBLOCKS 2
 #endif
+// Observer of the stepper (DESIGN.md §3.11).  step() sees every step after the primal update with the intensities the firing test read,
+// the normal, the two firing decisions and the jump sizes.  The default observes nothing and compiles away, so hawkes_slice_kernel is the
+// same machine code with or without this hook.
+struct HawkesNoHook {
+  __device__ __forceinline__ void step(double, double, double, bool, bool, double, double) {}
+};
+
+// the S steps of one path of one slice from (xi, lp, lm): the draws and the update of hawkes_slice_kernel
+template <int GAUSS, class Hook>
+__device__ __forceinline__ void hawkes_path_steps(double& xi, double& lp, double& lm, const HawkesSliceArgs& a, const HawkesConsts& c,
+                                                  const HawkesFast& f, uint2 key, uint32_t plo, uint32_t phi, StepNormals<double, GAUSS>& rng,
+                                                  Hook& hk) {
+  auto one_step = [&](double z, uint32_t rp, uint32_t rm, uint32_t step) {
+    const double lp0 = lp, lm0 = lm;
+    const uint32_t tp = __double2uint_rd(fma(-lp, f.thr, 4294967296.0)), tm = __double2uint_rd(fma(-lm, f.thr, 4294967296.0));
+    const bool cand_p = rp >= max(tp, 1u) - 1u, cand_m = rm >= max(tm, 1u) - 1u;
+    double jp = 0.0, jm = 0.0;
+    bool fp_ = false, fm_ = false;
+    if (cand_p || cand_m) {                                                     // ~1 % of the lane-steps: a clock may fire
+      fp_ = cand_p && hawkes_fires(lp, rp, c.dt, f.dt_lo);
+      fm_ = cand_m && hawkes_fires(lm, rm, c.dt, f.dt_lo);
+      if (fp_ || fm_) {
+        const uint4 w = hawkes_size_words(key, plo, phi, step, a.slice);
+        if (fp_ && fm_) {
+          const double2 jj = hawkes_two_sizes(w.x, w.y, c.shift_p, c.mean_p, c.shift_m, c.mean_m);
+          jp = jj.x;
+          jm = jj.y;
+        } else {                                                                // one logarithm serves whichever clock fired
+          const double l = -log(hawkes_uniform(fp_ ? w.x : w.y));
+          if (fp_) jp = __dadd_rn(c.shift_p, __dmul_rn(c.mean_p, l));            // = hawkes_size_p
+          else jm = __dadd_rn(c.shift_m, -__dmul_rn(-c.mean_m, l));              // = hawkes_size_m
+        }
+      }
+    }
+    double d = fma(-c.comp_p, lp, c.drift_dt);
+    d = fma(-c.comp_m, lm, d);
+    d = fma(f.ssd, z, d);
+    xi += d;
+    lp = fma(f.kdt_p, c.theta_p - lp, lp);
+    lm = fma(f.kdt_m, c.theta_m - lm, lm);
+    if (jp != 0.0 || jm != 0.0) {
+      xi += jp + jm;
+      lp += fma(c.beta1_p, jp, c.beta2_p * jm);
+      lm += fma(c.beta1_m, jp, c.beta2_m * jm);
+    }
+    hk.step(lp0, lm0, z, fp_, fm_, jp, jm);
+  };
+  const int S = a.nsteps;
+  for (int s = 0; s < S; s += 4) {                  // four steps: one (float) or two (fp64) calls of normals, two calls of clocks
+    double z[4];
+    if constexpr (GAUSS == kGaussF64) {
+      rng.get((uint32_t)(s >> 1), z[0], z[1]);
+      if (s + 2 < S) rng.get((uint32_t)(s >> 1) + 1u, z[2], z[3]);
+    } else {
+      rng.get2((uint32_t)(s >> 2), z[0], z[1], z[2], z[3]);
+    }
+    const uint4 c0 = hawkes_clock_words(key, plo, phi, (uint32_t)(s >> 1), a.slice);
+    one_step(z[0], c0.x, c0.y, (uint32_t)s);
+    if (s + 1 < S) one_step(z[1], c0.z, c0.w, (uint32_t)s + 1u);
+    if (s + 2 < S) {
+      const uint4 c1 = hawkes_clock_words(key, plo, phi, (uint32_t)(s >> 1) + 1u, a.slice);
+      one_step(z[2], c1.x, c1.y, (uint32_t)s + 2u);
+      if (s + 3 < S) one_step(z[3], c1.z, c1.w, (uint32_t)s + 3u);
+    }
+  }
+}
+
+__device__ __forceinline__ HawkesFast hawkes_fast(const HawkesConsts& c) {
+  return HawkesFast{c.sigma * c.sqrt_dt, c.kappa_p * c.dt, c.kappa_m * c.dt, c.dt * (1.0 + 1e-9) * 4294967296.0, c.dt * (1.0 - 1e-9)};
+}
+
 template <int GAUSS>
 __global__ void __launch_bounds__(kThreads, B200SV_HAWKES_MINBLOCKS) hawkes_slice_kernel(HawkesSliceArgs a, HawkesConsts c) {
   __shared__ double red[2 * kThreads / 32];
   if constexpr (GAUSS != kGaussF32) gauss64_table_init();
   double acc[2] = {0.0, 0.0};
   const uint2 key = make_uint2((uint32_t)a.seed, (uint32_t)(a.seed >> 32));
-  const HawkesFast f{c.sigma * c.sqrt_dt, c.kappa_p * c.dt, c.kappa_m * c.dt, c.dt * (1.0 + 1e-9) * 4294967296.0, c.dt * (1.0 - 1e-9)};
+  const HawkesFast f = hawkes_fast(c);
   const long long stride = (long long)gridDim.x * kThreads;
   for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < a.n; i += stride) {
     double xi = 0.0, lp = a.lam_p0, lm = a.lam_m0;
@@ -157,55 +228,8 @@ __global__ void __launch_bounds__(kThreads, B200SV_HAWKES_MINBLOCKS) hawkes_slic
     const unsigned long long path = a.path_offset + (unsigned long long)i;
     const uint32_t plo = (uint32_t)path, phi = (uint32_t)(path >> 32);
     StepNormals<double, GAUSS> rng(a.seed, path, a.slice);
-    auto one_step = [&](double z, uint32_t rp, uint32_t rm, uint32_t step) {
-      const uint32_t tp = __double2uint_rd(fma(-lp, f.thr, 4294967296.0)), tm = __double2uint_rd(fma(-lm, f.thr, 4294967296.0));
-      const bool cand_p = rp >= max(tp, 1u) - 1u, cand_m = rm >= max(tm, 1u) - 1u;
-      double jp = 0.0, jm = 0.0;
-      if (cand_p || cand_m) {                                                     // ~1 % of the lane-steps: a clock may fire
-        const bool fp_ = cand_p && hawkes_fires(lp, rp, c.dt, f.dt_lo), fm_ = cand_m && hawkes_fires(lm, rm, c.dt, f.dt_lo);
-        if (fp_ || fm_) {
-          const uint4 w = hawkes_size_words(key, plo, phi, step, a.slice);
-          if (fp_ && fm_) {
-            const double2 jj = hawkes_two_sizes(w.x, w.y, c.shift_p, c.mean_p, c.shift_m, c.mean_m);
-            jp = jj.x;
-            jm = jj.y;
-          } else {                                                                // one logarithm serves whichever clock fired
-            const double l = -log(hawkes_uniform(fp_ ? w.x : w.y));
-            if (fp_) jp = __dadd_rn(c.shift_p, __dmul_rn(c.mean_p, l));            // = hawkes_size_p
-            else jm = __dadd_rn(c.shift_m, -__dmul_rn(-c.mean_m, l));              // = hawkes_size_m
-          }
-        }
-      }
-      double d = fma(-c.comp_p, lp, c.drift_dt);
-      d = fma(-c.comp_m, lm, d);
-      d = fma(f.ssd, z, d);
-      xi += d;
-      lp = fma(f.kdt_p, c.theta_p - lp, lp);
-      lm = fma(f.kdt_m, c.theta_m - lm, lm);
-      if (jp != 0.0 || jm != 0.0) {
-        xi += jp + jm;
-        lp += fma(c.beta1_p, jp, c.beta2_p * jm);
-        lm += fma(c.beta1_m, jp, c.beta2_m * jm);
-      }
-    };
-    const int S = a.nsteps;
-    for (int s = 0; s < S; s += 4) {                  // four steps: one (float) or two (fp64) calls of normals, two calls of clocks
-      double z[4];
-      if constexpr (GAUSS == kGaussF64) {
-        rng.get((uint32_t)(s >> 1), z[0], z[1]);
-        if (s + 2 < S) rng.get((uint32_t)(s >> 1) + 1u, z[2], z[3]);
-      } else {
-        rng.get2((uint32_t)(s >> 2), z[0], z[1], z[2], z[3]);
-      }
-      const uint4 c0 = hawkes_clock_words(key, plo, phi, (uint32_t)(s >> 1), a.slice);
-      one_step(z[0], c0.x, c0.y, (uint32_t)s);
-      if (s + 1 < S) one_step(z[1], c0.z, c0.w, (uint32_t)s + 1u);
-      if (s + 2 < S) {
-        const uint4 c1 = hawkes_clock_words(key, plo, phi, (uint32_t)(s >> 1) + 1u, a.slice);
-        one_step(z[2], c1.x, c1.y, (uint32_t)s + 2u);
-        if (s + 3 < S) one_step(z[3], c1.z, c1.w, (uint32_t)s + 3u);
-      }
-    }
+    HawkesNoHook none;
+    hawkes_path_steps<GAUSS>(xi, lp, lm, a, c, f, key, plo, phi, rng, none);
     a.x[i] = xi;
     a.lam_p[i] = lp;
     a.lam_m[i] = lm;
@@ -219,6 +243,176 @@ __global__ void __launch_bounds__(kThreads, B200SV_HAWKES_MINBLOCKS) hawkes_slic
   if (threadIdx.x == 0) {
     a.partials[2 * blockIdx.x + 0] = acc[0];
     a.partials[2 * blockIdx.x + 1] = acc[1];
+  }
+}
+// ---- Monte Carlo sensitivities (DESIGN.md §3.11) -----------------------------------------------------------------------------
+// Directions in HAWKES_GREEK_PARAMS order: 0 sigma, 1 shift_p, 2 mean_p, 3 shift_m, 4 mean_m, 5..9 (lambda, theta, kappa, beta1, beta2)_p,
+// 10..14 the same for the minus intensity.  With the firing decisions frozen, sigma moves only x, the five own parameters of an intensity
+// move only that intensity, and the shifts and means move both through the jump loads: each intensity carries 9 tangents, q = 0..3 the
+// shift / mean directions, q = 4..8 its own five.
+constexpr int kHawkesParams = 15;
+constexpr int kHawkesLamDirs = 9;
+__host__ __device__ constexpr int hawkes_dir_p(int q) { return q + 1; }
+__host__ __device__ constexpr int hawkes_dir_m(int q) { return q < 4 ? q + 1 : q + 6; }
+
+// the chain's tangent state between maturities, SoA [rows][n]: dx [15], dlambda_p [9], dlambda_m [9], accumulated score [15] (row 0 is 0)
+struct HawkesTangentArgs {
+  double *dx, *dlp, *dlm, *score;
+};
+
+// Pathwise tangents with frozen decisions plus the likelihood-ratio score of the decisions.  dx and the no-jump score are linear in the
+// step-start intensity tangents, so the hook keeps their running sums rp / rm over the slice and forms dx and the score once at the end:
+//   dx_p    += -comp_p rp_p - comp_m rm_p  (+ sqrt(dt) sum z - sigma dt S for sigma, + firings - dcomp/dshift sum lambda for the shifts,
+//              + sum E - dcomp/dmean sum lambda for the means, E = (J - shift) / mean the unit exponential of a jump)
+//   score_p += -dt (rp_p + rm_p) + fire_p,  fire_p = sum over firing steps of dlambda (dt + dt / expm1(lambda dt)), plus dt dlambda on steps
+//              with lambda <= 0 (the clock cannot fire there: no score)
+struct HawkesTangentHook {
+  const HawkesConsts& c;
+  double a_p, a_m;                            // 1 - kappa dt: d lambda' / d lambda between jumps
+  double dlp[kHawkesLamDirs], dlm[kHawkesLamDirs];
+  double rp[kHawkesLamDirs], rm[kHawkesLamDirs];
+  double fire[kHawkesParams];                 // index = direction; fire[0] stays 0
+  double sp, sm, np_, nm_, ep, em, zs;        // sums of the step-start intensities, firing counts, sums of E, sum of z
+
+  __device__ __forceinline__ HawkesTangentHook(const HawkesConsts& c_, const HawkesFast& f) : c(c_), a_p(1.0 - f.kdt_p), a_m(1.0 - f.kdt_m) {}
+
+  __device__ __forceinline__ void load(const HawkesTangentArgs& t, long long i, long long n, bool init) {
+#pragma unroll
+    for (int q = 0; q < kHawkesLamDirs; ++q) {
+      dlp[q] = init ? (q == 4 ? 1.0 : 0.0) : t.dlp[q * n + i];          // d lambda_p(0) / d lambda_p = 1
+      dlm[q] = init ? (q == 4 ? 1.0 : 0.0) : t.dlm[q * n + i];
+      rp[q] = rm[q] = 0.0;
+    }
+#pragma unroll
+    for (int p = 0; p < kHawkesParams; ++p) fire[p] = 0.0;
+    sp = sm = np_ = nm_ = ep = em = zs = 0.0;
+  }
+
+  __device__ __forceinline__ void step(double lp0, double lm0, double z, bool fp, bool fm, double jp, double jm) {
+    zs += z;
+    sp += lp0;
+    sm += lm0;
+    if (fp || fm || !(lp0 > 0.0) || !(lm0 > 0.0)) {           // score terms at the step-start tangents (~1 % of the lane-steps)
+      const double wp = fp ? c.dt + c.dt / expm1(lp0 * c.dt) : (lp0 > 0.0 ? 0.0 : c.dt);
+      const double wm = fm ? c.dt + c.dt / expm1(lm0 * c.dt) : (lm0 > 0.0 ? 0.0 : c.dt);
+#pragma unroll
+      for (int q = 0; q < kHawkesLamDirs; ++q) {
+        fire[hawkes_dir_p(q)] = fma(wp, dlp[q], fire[hawkes_dir_p(q)]);
+        fire[hawkes_dir_m(q)] = fma(wm, dlm[q], fire[hawkes_dir_m(q)]);
+      }
+    }
+    const double kp = c.dt * (c.theta_p - lp0), km = c.dt * (c.theta_m - lm0);
+#pragma unroll
+    for (int q = 0; q < kHawkesLamDirs; ++q) {
+      rp[q] += dlp[q];
+      rm[q] += dlm[q];
+      const double bp = q == 5 ? c.kappa_p * c.dt : q == 6 ? kp : 0.0;   // theta: kappa dt, kappa: dt (theta - lambda)
+      const double bm = q == 5 ? c.kappa_m * c.dt : q == 6 ? km : 0.0;
+      dlp[q] = fma(a_p, dlp[q], bp);
+      dlm[q] = fma(a_m, dlm[q], bm);
+    }
+    if (fp || fm) {                                           // the jump loads: dJ/dshift = 1, dJ/dmean = E; beta rows take J itself
+      const double up = fp ? 1.0 : 0.0, um = fm ? 1.0 : 0.0;
+      const double eep = fp ? (jp - c.shift_p) / c.mean_p : 0.0, eem = fm ? (jm - c.shift_m) / c.mean_m : 0.0;
+      np_ += up;
+      nm_ += um;
+      ep += eep;
+      em += eem;
+      dlp[0] = fma(c.beta1_p, up, dlp[0]);
+      dlp[1] = fma(c.beta1_p, eep, dlp[1]);
+      dlp[2] = fma(c.beta2_p, um, dlp[2]);
+      dlp[3] = fma(c.beta2_p, eem, dlp[3]);
+      dlp[7] += jp;
+      dlp[8] += jm;
+      dlm[0] = fma(c.beta1_m, up, dlm[0]);
+      dlm[1] = fma(c.beta1_m, eep, dlm[1]);
+      dlm[2] = fma(c.beta2_m, um, dlm[2]);
+      dlm[3] = fma(c.beta2_m, eem, dlm[3]);
+      dlm[7] += jp;
+      dlm[8] += jm;
+    }
+  }
+
+  // end of the slice (S steps): dx and the score from their values at the slice start, into the SoA state
+  __device__ __forceinline__ void finish(const HawkesTangentArgs& t, long long i, long long n, bool init, int S, double (&dx)[kHawkesParams],
+                                         double (&sc)[kHawkesParams]) const {
+#pragma unroll
+    for (int p = 0; p < kHawkesParams; ++p) {
+      dx[p] = init ? 0.0 : t.dx[p * n + i];
+      sc[p] = init ? 0.0 : t.score[p * n + i];
+    }
+    dx[0] += fma(c.sqrt_dt, zs, -c.sigma * c.dt * (double)S);
+    const double gp = c.dt * exp(c.shift_p) / (1.0 - c.mean_p), gm = c.dt * exp(c.shift_m) / (1.0 - c.mean_m);   // dcomp / dshift
+    dx[1] += fma(-gp, sp, np_);
+    dx[2] += fma(-gp / (1.0 - c.mean_p), sp, ep);                                                                   // dcomp / dmean
+    dx[3] += fma(-gm, sm, nm_);
+    dx[4] += fma(-gm / (1.0 - c.mean_m), sm, em);
+#pragma unroll
+    for (int q = 0; q < kHawkesLamDirs; ++q) {
+      dx[hawkes_dir_p(q)] = fma(-c.comp_p, rp[q], dx[hawkes_dir_p(q)]);
+      dx[hawkes_dir_m(q)] = fma(-c.comp_m, rm[q], dx[hawkes_dir_m(q)]);
+      sc[hawkes_dir_p(q)] = fma(-c.dt, rp[q], sc[hawkes_dir_p(q)]);
+      sc[hawkes_dir_m(q)] = fma(-c.dt, rm[q], sc[hawkes_dir_m(q)]);
+    }
+#pragma unroll
+    for (int p = 1; p < kHawkesParams; ++p) sc[p] += fire[p];
+#pragma unroll
+    for (int q = 0; q < kHawkesLamDirs; ++q) {
+      t.dlp[q * n + i] = dlp[q];
+      t.dlm[q * n + i] = dlm[q];
+    }
+#pragma unroll
+    for (int p = 0; p < kHawkesParams; ++p) {
+      t.dx[p * n + i] = dx[p];
+      t.score[p * n + i] = sc[p];
+    }
+  }
+};
+
+// hawkes_slice_kernel with tangents and scores: the same primal steps (bit-identical state), the same Philox streams, launched on the
+// pricing kernel's grid so that the re-centring moments (first two partials) are the pricing route's.  Per-CTA partials [gridDim.x][2 + 15]:
+// sum F e^x, count, sum F e^x (dx_p + score_p) over the non-NaN spots.
+template <int GAUSS>
+__global__ void __launch_bounds__(kThreads) hawkes_tangent_slice_kernel(HawkesSliceArgs a, HawkesConsts c, HawkesTangentArgs t) {
+  constexpr int K = 2 + kHawkesParams;
+  __shared__ double red[K * kThreads / 32];
+  if constexpr (GAUSS != kGaussF32) gauss64_table_init();
+  double acc[K];
+#pragma unroll
+  for (int k = 0; k < K; ++k) acc[k] = 0.0;
+  const uint2 key = make_uint2((uint32_t)a.seed, (uint32_t)(a.seed >> 32));
+  const HawkesFast f = hawkes_fast(c);
+  const long long stride = (long long)gridDim.x * kThreads;
+  for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < a.n; i += stride) {
+    double xi = 0.0, lp = a.lam_p0, lm = a.lam_m0;
+    if (!a.init) {
+      xi = a.x[i];
+      lp = a.lam_p[i];
+      lm = a.lam_m[i];
+    }
+    const unsigned long long path = a.path_offset + (unsigned long long)i;
+    const uint32_t plo = (uint32_t)path, phi = (uint32_t)(path >> 32);
+    StepNormals<double, GAUSS> rng(a.seed, path, a.slice);
+    HawkesTangentHook h(c, f);
+    h.load(t, i, a.n, a.init != 0);
+    hawkes_path_steps<GAUSS>(xi, lp, lm, a, c, f, key, plo, phi, rng, h);
+    a.x[i] = xi;
+    a.lam_p[i] = lp;
+    a.lam_m[i] = lm;
+    double dx[kHawkesParams], sc[kHawkesParams];
+    h.finish(t, i, a.n, a.init != 0, a.nsteps, dx, sc);
+    const double spot = a.forward * exp(xi);
+    if (spot == spot) {
+      acc[0] += spot;
+      acc[1] += 1.0;
+#pragma unroll
+      for (int k = 0; k < kHawkesParams; ++k) acc[2 + k] = fma(spot, dx[k] + sc[k], acc[2 + k]);
+    }
+  }
+  block_sum<K, kThreads>(acc, red);
+  if (threadIdx.x == 0) {
+#pragma unroll
+    for (int k = 0; k < K; ++k) a.partials[K * blockIdx.x + k] = acc[k];
   }
 }
 
@@ -251,9 +445,10 @@ __global__ void hawkes_device_draws_kernel(unsigned long long seed, unsigned lon
   }
 }
 
+// one slice of the pricing kernel, or with `tan` of the tangent kernel on the same grid (moments_out then holds 2 + 15 values)
 static int launch_hawkes_slice(double* x, double* lp, double* lm, long long n, long long path_offset, int init, const b200sv_hawkes_params& p,
                                int nsteps, double dt, int slice_index, double forward, uint64_t seed, int flags, double* moments_out,
-                               cudaStream_t st, P2pCtx* p2p = nullptr) {
+                               cudaStream_t st, P2pCtx* p2p = nullptr, const HawkesTangentArgs* tan = nullptr) {
   const int g = gauss_mode(flags);
   if (g != kGaussF32 && g != kGaussF64) return fail(-1, "invalid argument: gauss flags");
   HawkesSliceArgs a;
@@ -271,16 +466,25 @@ static int launch_hawkes_slice(double* x, double* lp, double* lm, long long n, l
   a.forward = forward;
   const HawkesConsts c = make_hawkes_consts(p, dt);
   Grid grid = persistent_grid(hawkes_slice_kernel<kGaussF32>, kThreads, n);
+  const int K = tan ? 2 + kHawkesParams : 2;
   ensure_pool_threshold();
   DevBuf partials(st);
-  B200SV_CUDA(partials.alloc(sizeof(double) * 2 * grid.blocks));
+  B200SV_CUDA(partials.alloc(sizeof(double) * K * grid.blocks));
   a.partials = partials.as<double>();
-  if (g == kGaussF64)
-    hawkes_slice_kernel<kGaussF64><<<grid.blocks, grid.threads, 0, st>>>(a, c);
-  else
-    hawkes_slice_kernel<kGaussF32><<<grid.blocks, grid.threads, 0, st>>>(a, c);
-  if (int rc = check_launch("hawkes_slice_kernel")) return rc;
-  reduce_partials_kernel<<<1, 64, 0, st>>>(a.partials, grid.blocks, 2, 2, moments_out, make_publish(p2p, st));   // exchange #1 (producer)
+  if (tan) {
+    if (g == kGaussF64)
+      hawkes_tangent_slice_kernel<kGaussF64><<<grid.blocks, grid.threads, 0, st>>>(a, c, *tan);
+    else
+      hawkes_tangent_slice_kernel<kGaussF32><<<grid.blocks, grid.threads, 0, st>>>(a, c, *tan);
+    if (int rc = check_launch("hawkes_tangent_slice_kernel")) return rc;
+  } else {
+    if (g == kGaussF64)
+      hawkes_slice_kernel<kGaussF64><<<grid.blocks, grid.threads, 0, st>>>(a, c);
+    else
+      hawkes_slice_kernel<kGaussF32><<<grid.blocks, grid.threads, 0, st>>>(a, c);
+    if (int rc = check_launch("hawkes_slice_kernel")) return rc;
+  }
+  reduce_partials_kernel<<<1, 64, 0, st>>>(a.partials, grid.blocks, K, K, moments_out, make_publish(p2p, st));   // exchange #1 (producer)
   return check_launch("reduce_partials_kernel");
 }
 
@@ -312,6 +516,65 @@ static int hawkes_chain_host(const b200sv_hawkes_params* p, int M, const double*
     if (int rc = io.payoff(0, m, x, x, false, nb_path, (double)nb_path, false)) return rc;
   }
   return io.copy_back(sync, prices_out, stderr_out, nullptr);
+}
+
+// Chain with Monte Carlo sensitivities (DESIGN.md §3.11): per maturity the tangent slice, the sensitivity rows from the score-aware payoff
+// kernel and the price rows from the pricing route's own payoff launches on the same state, so prices and std errors are bit-identical to
+// hawkes_chain_host.  The device state is [3 + 15 + 9 + 9 + 15][N] rows (x, lambda_p, lambda_m, dx, dlambda_p, dlambda_m, score); the first
+// n_paths_out columns are copied out per maturity when states_out [M][3][n_out] or tangents_out [M][4][15][n_out] is given.
+static int hawkes_chain_greeks_host(const b200sv_hawkes_params* p, int M, const double* ttms, const double* forwards, const double* discfactors,
+                                    const int* offsets, const double* strikes, const int8_t* types, long long nb_path, int variable_type,
+                                    uint64_t seed, int flags, double* prices_out, double* stderr_out, double* greeks_out, double* greeks_se_out,
+                                    long long n_paths_out, double* states_out, double* tangents_out) {
+  constexpr int NP = kHawkesParams, L = kHawkesLamDirs, R = 3 + NP + 2 * L + NP;
+  B200SV_REQUIRE(nb_path >= 1, "nb_path must be >= 1");
+  B200SV_REQUIRE(n_paths_out >= 0 && n_paths_out <= nb_path, "n_paths_out must be in [0, nb_path]");
+  // d J / d mean = (J - shift) / mean, the jump's unit exponential: undefined for a degenerate jump size
+  B200SV_REQUIRE(p && p->mean_p != 0.0 && p->mean_m != 0.0, "the Hawkes sensitivities need mean_p != 0 and mean_m != 0");
+  if (int rc = validate_chain(M, ttms, offsets, strikes, types, variable_type)) return rc;
+  if (variable_type != B200SV_LOG_RETURN) return fail(-4, "variable_type not implemented: the Hawkes sensitivities cover LOG_RETURN");
+  const int gauss = greeks_gauss(flags);
+  if (gauss < 0) return gauss;
+  cudaStream_t st = current_stream();
+  ensure_pool_threshold();
+  StreamSync sync(st);
+  const size_t N = (size_t)nb_path, no = (states_out || tangents_out) ? (size_t)n_paths_out : 0;
+  DevBuf d(st);
+  GreeksChainIO<NP, true> io(M, ttms, forwards, discfactors, offsets, types, variable_type, nb_path, st);
+  B200SV_CUDA(d.alloc(sizeof(double) * R * N));
+  if (int rc = io.upload(strikes)) return rc;
+  double* x = d.as<double>();
+  const HawkesTangentArgs t{x + 3 * N, x + (3 + NP) * N, x + (3 + NP + L) * N, x + (3 + NP + 2 * L) * N};
+  std::vector<double> h_paths(no * R * M);
+  double t0 = 0.0;
+  for (int m = 0; m < M; ++m) {
+    int S;
+    double dt;
+    time_grid(ttms[m] - t0, kHawkesStepsPerYear, &S, &dt);
+    t0 = ttms[m];
+    if (int rc = launch_hawkes_slice(x, x + N, x + 2 * N, nb_path, 0, m == 0, *p, S, dt, m, forwards[m], seed, flags, io.moments(), st, nullptr, &t))
+      return rc;
+    if (int rc = io.payoff(m, x, x, t.dx, t.dx, (double)nb_path, t.score)) return rc;
+    if (int rc = io.ChainIO::payoff(0, m, x, x, false, nb_path, (double)nb_path, false)) return rc;
+    if (no)
+      B200SV_CUDA(cudaMemcpy2DAsync(h_paths.data() + no * R * m, sizeof(double) * no, x, sizeof(double) * N, sizeof(double) * no, R,
+                                    cudaMemcpyDeviceToHost, st));
+  }
+  if (int rc = io.copy_back(sync, prices_out, stderr_out, greeks_out, greeks_se_out)) return rc;
+  for (size_t m = 0; m < (size_t)M && no; ++m) {
+    const double* h = h_paths.data() + no * R * m;
+    if (states_out) memcpy(states_out + 3 * no * m, h, sizeof(double) * 3 * no);
+    if (!tangents_out) continue;
+    double* o = tangents_out + 4 * NP * no * m;                      // [4][15][n_out]: dx, dlambda_p, dlambda_m, score
+    memset(o, 0, sizeof(double) * 4 * NP * no);
+    memcpy(o, h + 3 * no, sizeof(double) * NP * no);
+    for (int q = 0; q < L; ++q) {
+      memcpy(o + (NP + hawkes_dir_p(q)) * no, h + (3 + NP + q) * no, sizeof(double) * no);
+      memcpy(o + (2 * NP + hawkes_dir_m(q)) * no, h + (3 + NP + L + q) * no, sizeof(double) * no);
+    }
+    memcpy(o + 3 * NP * no, h + (3 + NP + 2 * L) * no, sizeof(double) * NP * no);
+  }
+  return 0;
 }
 
 }  // namespace b200sv

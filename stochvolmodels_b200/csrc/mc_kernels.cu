@@ -1132,13 +1132,14 @@ __global__ void __launch_bounds__(kSliceThreads, B200SV_SLICE_MINBLOCKS) mc_tang
 // dS_p = F e^x dx_p - mean(F e^x dx_p) over the nanmean's set, dS/dF = S/F; dU_p = dq_p/ttm, dU/dF = 0 under Q_VAR.
 // pay = h(U) (C/P) or h(U)/S (IC/IP) with h = (U-K)^+ or (K-U)^+; g = h'(U) dU or (h'(U) dU - pay dS)/S.  A path whose payoff is NaN
 // is skipped for every sum.  Row layout per strike: (sum pay, sum pay^2, count, then (sum g, sum g^2) for delta and every parameter).
+// SCORE (the Hawkes route, DESIGN.md §3.11): every parameter row also carries the likelihood-ratio term pay * score_p, score [NP][n].
 constexpr int kGreeksStrikeChunk = 2;
-template <int NP>
-__global__ void __launch_bounds__(kThreads) payoff_greeks_kernel(const double* __restrict__ x, const double* __restrict__ q,
-                                                                const double* __restrict__ dx, const double* __restrict__ dq, long long n,
-                                                                double ttm, double forward, const double* __restrict__ strikes,
-                                                                const int8_t* __restrict__ types, int J, int variable_type,
-                                                                const double* __restrict__ moments, double* __restrict__ partials, int Kpad) {
+template <int NP, bool SCORE>
+__device__ __forceinline__ void payoff_greeks_body(const double* __restrict__ x, const double* __restrict__ q, const double* __restrict__ dx,
+                                                   const double* __restrict__ dq, const double* __restrict__ score, long long n, double ttm,
+                                                   double forward, const double* __restrict__ strikes, const int8_t* __restrict__ types, int J,
+                                                   int variable_type, const double* __restrict__ moments, double* __restrict__ partials,
+                                                   int Kpad) {
   constexpr int KV = 3 + 2 * (1 + NP), KC = KV * kGreeksStrikeChunk;
   __shared__ double red[KC * kThreads / 32];
   __shared__ double sh_mom[2 + NP];
@@ -1174,6 +1175,11 @@ __global__ void __launch_bounds__(kThreads) payoff_greeks_kernel(const double* _
       dU[1 + k] = is_qvar ? dq[k * n + i] * inv_ttm : dS[1 + k];
     }
     const double under = is_qvar ? q[i] * inv_ttm : spot;
+    double sc[SCORE ? NP : 1];
+    if constexpr (SCORE) {
+#pragma unroll
+      for (int k = 0; k < NP; ++k) sc[k] = score[k * n + i];
+    }
 #pragma unroll
     for (int c = 0; c < kGreeksStrikeChunk; ++c) {
       if (ty[c] < 0) continue;
@@ -1191,6 +1197,9 @@ __global__ void __launch_bounds__(kThreads) payoff_greeks_kernel(const double* _
       for (int k = 0; k < 1 + NP; ++k) {
         double g = itm ? hp * dU[k] : 0.0;
         if (inverse) g = (g - pay * dS[k]) / spot;
+        if constexpr (SCORE) {
+          if (k > 0) g = fma(pay, sc[k - 1], g);
+        }
         a[3 + 2 * k] += g;
         a[4 + 2 * k] = fma(g, g, a[4 + 2 * k]);
       }
@@ -1201,6 +1210,21 @@ __global__ void __launch_bounds__(kThreads) payoff_greeks_kernel(const double* _
 #pragma unroll
     for (int c = 0; c < KC; ++c) partials[(size_t)blockIdx.x * Kpad + KV * j0 + c] = acc[c];
   }
+}
+template <int NP>
+__global__ void __launch_bounds__(kThreads) payoff_greeks_kernel(const double* __restrict__ x, const double* __restrict__ q,
+                                                                const double* __restrict__ dx, const double* __restrict__ dq, long long n,
+                                                                double ttm, double forward, const double* __restrict__ strikes,
+                                                                const int8_t* __restrict__ types, int J, int variable_type,
+                                                                const double* __restrict__ moments, double* __restrict__ partials, int Kpad) {
+  payoff_greeks_body<NP, false>(x, q, dx, dq, nullptr, n, ttm, forward, strikes, types, J, variable_type, moments, partials, Kpad);
+}
+template <int NP>
+__global__ void __launch_bounds__(kThreads) payoff_score_greeks_kernel(const double* __restrict__ x, const double* __restrict__ dx,
+                                                                      const double* __restrict__ score, long long n, double ttm, double forward,
+                                                                      const double* __restrict__ strikes, const int8_t* __restrict__ types, int J,
+                                                                      const double* __restrict__ moments, double* __restrict__ partials, int Kpad) {
+  payoff_greeks_body<NP, true>(x, x, dx, dx, score, n, ttm, forward, strikes, types, J, B200SV_LOG_RETURN, moments, partials, Kpad);
 }
 
 // prices / std errors exactly as payoff_finalize_kernel (std / sqrt(price_paths)), plus greeks_out[k][Jtot] = df * mean(g_k),
@@ -1604,7 +1628,8 @@ struct ChainIO {
 // The chain of a sensitivity driver over nb_path paths and NP parameter directions: ChainIO with the [2 + NP] moments its tangent launch reduces
 // into, per-strike sums of the payoff and its sensitivities, their partials (sized once for the widest slice), and the result block
 // [prices | std errors | greeks [1 + NP] | greeks_se [1 + NP]][Jalloc].
-template <int NP>
+// SCORE: the payoff launches add the likelihood-ratio term of a score array (payoff_score_greeks_kernel, LOG_RETURN only)
+template <int NP, bool SCORE = false>
 struct GreeksChainIO : ChainIO {
   static constexpr int KV = 3 + 2 * (1 + NP);
   long long n;
@@ -1614,7 +1639,12 @@ struct GreeksChainIO : ChainIO {
   GreeksChainIO(int M_, const double* ttms_, const double* forwards_, const double* discfactors_, const int* offsets_, const int8_t* types_,
                 int variable_type_, long long nb_path, cudaStream_t s)
       : ChainIO(1, M_, ttms_, forwards_, discfactors_, offsets_, types_, variable_type_, s), n(nb_path),
-        gp(persistent_grid(payoff_greeks_kernel<NP>, kThreads, nb_path)), d_part(s) {}
+        gp(payoff_grid(nb_path)), d_part(s) {}
+
+  static Grid payoff_grid(long long nb_path) {
+    if constexpr (SCORE) return persistent_grid(payoff_score_greeks_kernel<NP>, kThreads, nb_path);
+    else return persistent_grid(payoff_greeks_kernel<NP>, kThreads, nb_path);
+  }
 
   int upload(const double* strikes) {
     int Jmax = 0;
@@ -1625,16 +1655,22 @@ struct GreeksChainIO : ChainIO {
   }
 
   // maturity m: per-strike payoff and sensitivity sums over the state (x, q) and its tangents (dx, dq) [NP][n] -> prices, price-row std
-  // errors (/ sqrt(price_paths)) and the 1 + NP sensitivity rows with their standard errors (/ sqrt(n)) into the result block
-  int payoff(int m, const double* x, const double* q, const double* dx, const double* dq, double price_paths) {
+  // errors (/ sqrt(price_paths)) and the 1 + NP sensitivity rows with their standard errors (/ sqrt(n)) into the result block.  SCORE: the
+  // rows add the likelihood-ratio term pay * score_p, score [NP][n].
+  int payoff(int m, const double* x, const double* q, const double* dx, const double* dq, double price_paths, const double* score = nullptr) {
     const int J = offsets[m + 1] - offsets[m], jo = offsets[m] - offsets[0];
     if (J == 0) return 0;
     const int chunks = (J + kGreeksStrikeChunk - 1) / kGreeksStrikeChunk;
     const int Kpad = KV * kGreeksStrikeChunk * chunks;
     const int blocks = std::max(1, gp.blocks / chunks);
-    payoff_greeks_kernel<NP><<<dim3(blocks, chunks), gp.threads, 0, st>>>(x, q, dx, dq, n, ttms[m], forwards[m], d_strikes.as<double>() + jo,
-                                                                          d_types.as<int8_t>() + jo, J, variable_type, moments(),
-                                                                          d_part.as<double>(), Kpad);
+    const double* ks = d_strikes.as<double>() + jo;
+    const int8_t* ts = d_types.as<int8_t>() + jo;
+    if constexpr (SCORE)
+      payoff_score_greeks_kernel<NP><<<dim3(blocks, chunks), gp.threads, 0, st>>>(x, dx, score, n, ttms[m], forwards[m], ks, ts, J, moments(),
+                                                                                  d_part.as<double>(), Kpad);
+    else
+      payoff_greeks_kernel<NP><<<dim3(blocks, chunks), gp.threads, 0, st>>>(x, q, dx, dq, n, ttms[m], forwards[m], ks, ts, J, variable_type,
+                                                                            moments(), d_part.as<double>(), Kpad);
     if (int rc = check_launch("payoff_greeks_kernel")) return rc;
     reduce_partials_kernel<<<1, 256, 0, st>>>(d_part.as<double>(), blocks, Kpad, KV * J, d_sums.as<double>(), P2pPublish{});
     if (int rc = check_launch("reduce_partials_kernel")) return rc;
@@ -2410,6 +2446,15 @@ int b200sv_hawkesjd_mc_chain(const b200sv_hawkes_params* params, int M, const do
   B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && stderr_out, "null pointer");
   return hawkes_chain_host(params, M, ttms, forwards, discfactors, offsets, strikes, types, nb_path, variable_type, seed, flags, prices_out,
                            stderr_out);
+}
+
+int b200sv_hawkesjd_mc_chain_greeks(const b200sv_hawkes_params* params, int M, const double* ttms, const double* forwards,
+                                    const double* discfactors, const int* offsets, const double* strikes, const int8_t* types, long long nb_path,
+                                    int variable_type, uint64_t seed, int flags, double* prices_out, double* stderr_out, double* greeks_out,
+                                    double* greeks_se_out, long long n_paths_out, double* states_out, double* tangents_out) {
+  B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && stderr_out && greeks_out && greeks_se_out, "null pointer");
+  return hawkes_chain_greeks_host(params, M, ttms, forwards, discfactors, offsets, strikes, types, nb_path, variable_type, seed, flags,
+                                  prices_out, stderr_out, greeks_out, greeks_se_out, n_paths_out, states_out, tangents_out);
 }
 
 int b200sv_hawkesjd_terminal(const b200sv_hawkes_params* params, double ttm, long long nb_path, uint64_t seed, int flags, int slice_index,

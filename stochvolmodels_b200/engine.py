@@ -85,9 +85,9 @@ def _backbone(etas, M: int):
 
 
 # ---- Monte Carlo --------------------------------------------------------------------------------------------------------
-def _mc_chain(symbol: str, params, chain, etas, head, variable_type, seed: int, flags: int, tail=(), n_greeks: int = 0):
+def _mc_chain(symbol: str, params, chain, etas, head, variable_type, seed: int, flags: int, tail=(), n_greeks: int = 0, post=()):
     """the single-set chain MC entry points: C arguments (params, chain block, *head, variable type, seed, flags, *tail, prices, stds
-    [, greeks, greeks_se]).  ``etas`` = (LogSV vol backbone or None,) or ().  With ``n_greeks`` returns (prices, std errors,
+    [, greeks, greeks_se], *post).  ``etas`` = (LogSV vol backbone or None,) or ().  With ``n_greeks`` returns (prices, std errors,
     greeks [1+P, J], greeks_se [1+P, J], offsets), else (prices, std errors)."""
     vt = variable_code(variable_type)
     ch = _chain_arrays(*chain)
@@ -96,7 +96,7 @@ def _mc_chain(symbol: str, params, chain, etas, head, variable_type, seed: int, 
     prices, stds = np.empty(J), np.empty(J)
     greeks = [np.empty((1 + n_greeks, J)), np.empty((1 + n_greeks, J))] if n_greeks else []
     C.call(symbol, byref(params), *C.chain_ptrs(ch, *etas), *head, vt, C.seed64(seed), int(flags), *tail, C.dptr(prices), C.dptr(stds),
-           *map(C.dptr, greeks))
+           *map(C.dptr, greeks), *post)
     prices, stds = C.split_chain(prices, ch.offsets), C.split_chain(stds, ch.offsets)
     return (prices, stds, *greeks, ch.offsets) if n_greeks else (prices, stds)
 
@@ -143,6 +143,20 @@ def heston_mc_chain_greeks(params: C.HestonParamsC, ttms, forwards, discfactors,
     """Heston twin of logsv_mc_chain_greeks (b200sv_heston_mc_chain_greeks): greeks rows = forward delta, then HESTON_GREEK_PARAMS."""
     return _mc_chain("b200sv_heston_mc_chain_greeks", params, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms), (),
                      (int(nb_path), int(nb_steps_per_year)), variable_type, seed, flags, (int(scheme),), n_greeks=len(HESTON_GREEK_PARAMS))
+
+
+def hawkesjd_mc_chain_greeks(params: C.HawkesParamsC, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, nb_path: int, variable_type,
+                             seed: int, flags: int, n_paths_out: int = 0):
+    """chain MC of the Hawkes jump-diffusion with Monte Carlo sensitivities (b200sv_hawkesjd_mc_chain_greeks; DESIGN.md §3.11).  Returns
+    (prices, std errors, greeks [1+15, J], greeks_se [1+15, J], offsets, states, tangents): greeks row 0 the forward delta, then
+    HAWKES_GREEK_PARAMS.  With ``n_paths_out`` > 0, states [M, 3, n_paths_out] = (x, lambda_p, lambda_m) and tangents [M, 4, 15, n_paths_out]
+    = (dx, dlambda_p, dlambda_m, accumulated score) of the first paths after each maturity, else None."""
+    M, P, n_out = C.f64(ttms).shape[0], len(HAWKES_GREEK_PARAMS), int(n_paths_out)
+    states = np.empty((M, 3, n_out)) if n_out else None
+    tangents = np.empty((M, 4, P, n_out)) if n_out else None
+    res = _mc_chain("b200sv_hawkesjd_mc_chain_greeks", params, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms), (), (int(nb_path),),
+                    variable_type, seed, flags, n_greeks=P, post=(n_out, C.dptr(states), C.dptr(tangents)))
+    return (*res, states, tangents)
 
 
 def _tangent_terminal(symbol: str, params, ttm: float, nb_path: int, nb_steps_per_year: int, model_args, seed: int, flags: int,

@@ -1,7 +1,8 @@
 """HawkesJDPricer on H100: the reference's ``pricers/hawkes_jd_pricer.py`` (SURVEY.md §8f #4), Monte Carlo and Fourier routes.
 
 * ``HawkesJDParams``                          (hawkes_jd_pricer.py:41-119)
-* ``HawkesJDPricer.model_mc_price_chain``     (:156-171) -> ``hawkesjd_mc_chain_pricer`` (:644-715)
+* ``HawkesJDPricer.model_mc_price_chain``     (:156-171) -> ``hawkesjd_mc_chain_pricer`` (:644-715); ``model_mc_chain_greeks`` adds Monte Carlo
+  sensitivities (DESIGN.md §3.11)
 * ``HawkesJDPricer.simulate_terminal_values`` (:193-224) -> ``simulate_hawkesjd_terminal`` (:718-779)
 * ``HawkesJDPricer.price_chain``              (:125-155) -> ``hawkesjd_chain_pricer`` (:365-417) / ``hawkesjd_chain_pricer_with_risk_premia`` (:420-484),
   ``hawkesjd_forwards_under_risk_kernel`` (:487-515), ``compute_hawkes_a_mgf_grid`` / ``solve_a_ode_grid`` (:518-579)
@@ -120,6 +121,24 @@ class HawkesJDPricer(ModelPricer):
                                         seed=kwargs.get("seed"), gauss=kwargs.get("gauss", "fp32"),
                                         variable_type=kwargs.get("variable_type", VariableType.LOG_RETURN),
                                         distributed=kwargs.get("distributed", True), exchange=kwargs.get("exchange"), **d)
+
+    @timer
+    def model_mc_chain_greeks(self, option_chain: OptionChain, params: HawkesJDParams, nb_path: int = 100000, seed: Optional[int] = None,
+                              gauss: str = "fp32", **kwargs):
+        """MC prices and standard errors bit-identical to ``model_mc_price_chain`` with the same ``nb_path`` / ``seed`` / ``gauss`` (one GPU),
+        plus the forward delta and d price / d HAWKES_GREEK_PARAMS (the Fourier route's 15 names and order; ``mu`` is excluded there too),
+        each with its standard error df std(g) / sqrt(N) -> ``McChainGreeks``.  Pathwise with the firing decisions frozen plus the
+        likelihood-ratio score of the decisions (DESIGN.md §3.11): unbiased for the discretised scheme the pricer simulates.  LOG_RETURN,
+        fp64 state, ``gauss`` 'fp32' / 'fp64'; Q_VAR, ``exchange``, another ``precision`` or a set ``risk_premia_gamma`` raise
+        NotImplementedError, ``mean_p == 0`` or ``mean_m == 0`` (degenerate jump sizes) ValueError.  Under torch.distributed every rank prices all paths (replicated, bit-identical results)."""
+        from .mc_greeks import check_hawkes_mc_greeks_kwargs, to_mc_chain_greeks
+        check_hawkes_mc_greeks_kwargs(kwargs, gauss, params)
+        d = params.to_dict()
+        d.pop("risk_premia_gamma", None)
+        res = engine.hawkesjd_mc_chain_greeks(_params_c(**d), option_chain.ttms, option_chain.forwards, option_chain.discfactors,
+                                              option_chain.strikes_ttms, option_chain.optiontypes_ttms, nb_path, C.LOG_RETURN, _shared_seed(seed),
+                                              engine.mc_flags("fp64", gauss))
+        return to_mc_chain_greeks(res[:5], engine.HAWKES_GREEK_PARAMS)
 
     # ---- calibration drivers (reference :230-357): SLSQP on the host around the GPU Fourier chain pricer -----------------------------
     def _vol_objective(self, option_chain: OptionChain, unpack, is_vega_weighted: bool, is_unit_ttm_vega: bool, scale: float = 1.0):

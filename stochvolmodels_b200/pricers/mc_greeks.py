@@ -1,5 +1,6 @@
-"""Pathwise Monte Carlo sensitivities of the LogSV / Heston chain pricers (DESIGN.md §3.9): the result type and the checks shared by
-``LogSVPricer.model_mc_chain_greeks`` and ``HestonPricer.model_mc_chain_greeks``.
+"""Monte Carlo sensitivities of the chain pricers (DESIGN.md §3.9-3.11): the result type and the argument checks of
+``LogSVPricer.model_mc_chain_greeks``, ``HestonPricer.model_mc_chain_greeks``, ``LogSVPricer.rough_mc_chain_greeks`` and
+``HawkesJDPricer.model_mc_chain_greeks``.
 
 One GPU pass returns, for every strike and maturity, the price and its standard error (identical to ``model_mc_price_chain`` on the same
 seed), the forward delta and the derivative with respect to every model parameter, each with its own standard error.  The estimators are
@@ -55,6 +56,24 @@ def check_rough_greeks_kwargs(kwargs) -> None:
         raise NotImplementedError("rough_mc_chain_greeks supports gauss=None (RandomState normals), 'fp32' or 'fp64'")
     if kwargs.get("seed") is None:
         raise ValueError("rough_mc_chain_greeks needs a seed, like model_mc_price_chain(use_rough_mc=True)")
+
+
+def check_hawkes_mc_greeks_kwargs(kwargs, gauss, params) -> None:
+    """what HawkesJDPricer.model_mc_chain_greeks rejects before any GPU work"""
+    if kwargs.get("precision", "fp64") != "fp64":
+        raise NotImplementedError("model_mc_chain_greeks needs precision='fp64'")
+    if kwargs.get("exchange") is not None:
+        raise NotImplementedError("model_mc_chain_greeks is single-GPU per rank (replicated under torch.distributed): no exchange")
+    if gauss not in ("fp32", "fp64"):
+        raise NotImplementedError("model_mc_chain_greeks supports gauss='fp32' or 'fp64'")
+    vt = kwargs.get("variable_type", C.LOG_RETURN)
+    if getattr(vt, "value", vt) != C.LOG_RETURN:
+        raise NotImplementedError("the Hawkes Monte Carlo sensitivities cover variable_type=LOG_RETURN only")
+    if params.risk_premia_gamma is not None:
+        raise NotImplementedError("the Hawkes Monte Carlo sensitivities do not cover a risk kernel (risk_premia_gamma)")
+    if params.mean_p == 0.0 or params.mean_m == 0.0:
+        # d J / d mean is the jump's unit exponential, recovered as (J - shift) / mean: undefined for a degenerate jump size
+        raise ValueError("the Hawkes Monte Carlo sensitivities need mean_p != 0 and mean_m != 0")
 
 
 def to_mc_chain_greeks(result, names: Sequence[str]) -> McChainGreeks:
