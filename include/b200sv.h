@@ -129,6 +129,22 @@ int b200sv_heston_mc_chain_greeks(const b200sv_heston_params* params, int M, con
                                   const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
                                   long long nb_path, int nb_steps_per_year, int variable_type, uint64_t seed, int flags, int scheme,
                                   double* prices_out, double* stderr_out, double* greeks_out, double* greeks_se_out);
+/* The two calls above plus the Monte Carlo gamma d^2 price / d forwards[m]^2 of every strike, by conditional smoothing of the log-spot's
+ * last step (DESIGN.md §3.9): gamma_out and gamma_se_out [J], the standard error with the greeks' convention.  Unbiased for the
+ * discretised scheme at the given nb_path.  Every other output is bit-identical to the _greeks call with the same arguments; the same
+ * flags and schemes are rejected.  Optional test hook (laststep_out may be NULL): laststep_out [M][2][n_paths_out] = (s, mu) of paths
+ * [0, n_paths_out) after maturity m, where the last step is x = mu + s z0 given the state before it. */
+int b200sv_logsv_mc_chain_greeks_gamma(const b200sv_logsv_params* params, int M, const double* ttms, const double* forwards,
+                                       const double* discfactors, const double* etas, const int* offsets, const double* strikes,
+                                       const int8_t* types, long long nb_path, int nb_steps_per_year, int is_spot_measure, int variable_type,
+                                       uint64_t seed, int flags, double* prices_out, double* stderr_out, double* greeks_out,
+                                       double* greeks_se_out, double* gamma_out, double* gamma_se_out, long long n_paths_out,
+                                       double* laststep_out);
+int b200sv_heston_mc_chain_greeks_gamma(const b200sv_heston_params* params, int M, const double* ttms, const double* forwards,
+                                        const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
+                                        long long nb_path, int nb_steps_per_year, int variable_type, uint64_t seed, int flags, int scheme,
+                                        double* prices_out, double* stderr_out, double* greeks_out, double* greeks_se_out, double* gamma_out,
+                                        double* gamma_se_out, long long n_paths_out, double* laststep_out);
 
 /* test entry points of the tangent stepper: one slice of ttm from (0, sigma0 | v0, 0) for the global paths [path_offset, path_offset + nb_path)
  * of Philox slice `slice_index`.  x, sigma | var, qvar: nb_path doubles; dx, dsigma | dvar, dqvar: [P][nb_path] tangents in the parameter

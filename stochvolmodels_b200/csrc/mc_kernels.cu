@@ -963,6 +963,7 @@ static HestonTangentConsts make_heston_tangent_consts(const b200sv_heston_params
 struct LogsvTangentPath {
   static constexpr int NP = kLogsvParams;
   static constexpr bool kPrefetch = false;   // 18 tangent registers leave no room for a second set of normals in flight
+  static constexpr bool kRecordsLastStep = false;
   using Consts = LogsvTangentConsts;
   LogsvPath<double> b;
   double dx[NP], dL[NP], dq[NP];
@@ -1019,6 +1020,9 @@ struct LogsvTangentPath {
   __device__ __forceinline__ double tx(int p) const { return dx[p]; }
   __device__ __forceinline__ double tq(int p) const { return fma(-2.0 * k.c.cq * b.s * b.s, dL[p], dq[p]); }
   __device__ __forceinline__ double tv(int p) const { return dL[p]; }
+  // the vol state a step reads (old sigma) and the standard deviation ce sigma of that step's log-spot increment
+  __device__ __forceinline__ double step_vol() const { return b.s; }
+  __device__ __forceinline__ double step_sd(double vol) const { return b.ce * vol; }
 };
 
 // Heston floor-Euler: dv' = 0 where the floor binds, else dv (1 - kappa dt) + dv (c0 z0 + c1 z1)/(2 sqrt v) + d(kappa dt) (theta - v)
@@ -1026,6 +1030,7 @@ struct LogsvTangentPath {
 struct HestonTangentPath {
   static constexpr int NP = kHestonParams;
   static constexpr bool kPrefetch = B200SV_SLICE_PREFETCH != 0;
+  static constexpr bool kRecordsLastStep = false;
   using Consts = HestonTangentConsts;
   HestonPath<double, false> b;
   double dx[NP], dv[NP], dq[NP];
@@ -1073,6 +1078,39 @@ struct HestonTangentPath {
   __device__ __forceinline__ double tx(int p) const { return dx[p]; }
   __device__ __forceinline__ double tq(int p) const { return dq[p]; }
   __device__ __forceinline__ double tv(int p) const { return dv[p]; }
+  // the vol state a step reads (old variance) and the standard deviation sqrt(v dt) of that step's log-spot increment
+  __device__ __forceinline__ double step_vol() const { return b.v; }
+  __device__ __forceinline__ double step_sd(double vol) const { return b.sdt * sqrt(vol); }
+};
+
+// Monte Carlo gamma (DESIGN.md §3.9): TPath that also keeps the vol state and z0 of the step in flight, so that after the slice the
+// conditional law of the last log-spot step is known -- x_S = mu + s z0_S with s = step_sd(vol_{S-1}) -- and writes (s, mu) to
+// laststep [2][n].  z0 is the value the step consumed (after the float-to-double conversion of the fp32 stream); the overflow re-run
+// replays every step, so the recorded step is the clamped one where the path was re-run.
+template <typename TPath>
+struct LastStepConsts {
+  typename TPath::Consts c;
+  double* laststep;
+};
+
+template <typename TPath>
+struct LastStepPath : TPath {
+  using Consts = LastStepConsts<TPath>;
+  static constexpr bool kRecordsLastStep = true;
+  double vol_last, z_last;
+  double* out;
+  __device__ __forceinline__ LastStepPath(const Consts& k_) : TPath(k_.c), out(k_.laststep) {}
+  template <bool SAFE>
+  __device__ __forceinline__ void step(double z0, double z1) {
+    vol_last = TPath::step_vol();
+    z_last = z0;
+    TPath::template step<SAFE>(z0, z1);
+  }
+  __device__ __forceinline__ void record_last_step(long long i, long long n, double xT) const {
+    const double s = TPath::step_sd(vol_last);
+    out[i] = s;
+    out[n + i] = fma(-s, z_last, xT);
+  }
 };
 
 // mc_slice_kernel with tangents: same persistent grid-stride loop, same Philox stream (counter = global path id, slice), same
@@ -1107,6 +1145,7 @@ __global__ void __launch_bounds__(kSliceThreads, B200SV_SLICE_MINBLOCKS) mc_tang
     a.x[i] = xT;
     a.v[i] = p.sigma();
     a.q[i] = p.q();
+    if constexpr (TPath::kRecordsLastStep) p.record_last_step(i, a.n, xT);
     const double spot = a.forward * exp(xT);
 #pragma unroll
     for (int k = 0; k < NP; ++k) {
@@ -1250,6 +1289,91 @@ __global__ void greeks_finalize_kernel(const double* __restrict__ sums, int KV, 
       greeks_se[(size_t)k * Jtot + j] = e;
     }
   }
+}
+
+// Per-strike (sum g, sum g^2) of the smoothed gamma (DESIGN.md §3.9).  With the other paths held fixed, path i's re-centred spot is
+// S_i = (1 - 1/n) F e^{mu_i + s_i Z} - c_i, c_i = (sum_{j != i} Y_j)/n - F = corr - Y_i/n (Y = F e^x, n = the nanmean's count), whose density
+// at k is f_i(k) = phi(d) / ((k + c_i) s_i), d = ln((k + c_i) / A_i) / s_i, A_i = (1 - 1/n) F e^{mu_i}, and 0 where k + c_i <= 0.  Per path:
+//   LOG_RETURN  C, P: (K/F)^2 f_i(K)     IC: (K/F^2) f_i(K) - 2K/(F^2 S_i) 1{S_i > K}     IP: (K/F^2) f_i(K) + 2K/(F^2 S_i) 1{S_i < K}
+//   Q_VAR       C, P: 0                   IC, IP: 2 pay_i / F^2
+// A path whose payoff is NaN is skipped, as in the price row.  laststep [2][n] = (s, mu) of mc_tangent_slice_kernel<LastStepPath<.>>.
+constexpr int kGammaStrikeChunk = 8;
+__global__ void __launch_bounds__(kThreads) payoff_gamma_kernel(const double* __restrict__ x, const double* __restrict__ q,
+                                                               const double* __restrict__ laststep, long long n, double ttm, double forward,
+                                                               const double* __restrict__ strikes, const int8_t* __restrict__ types, int J,
+                                                               int variable_type, const double* __restrict__ moments,
+                                                               double* __restrict__ partials, int Kpad) {
+  constexpr int KC = 2 * kGammaStrikeChunk;
+  __shared__ double red[KC * kThreads / 32];
+  __shared__ double sh_mom[2];
+  if (threadIdx.x < 2) sh_mom[threadIdx.x] = moments[threadIdx.x];
+  __syncthreads();
+  const double corr = sh_mom[0] / sh_mom[1] - forward, inv_cnt = 1.0 / sh_mom[1];
+  const double log_a0 = log((1.0 - inv_cnt) * forward);       // ln A_i = log_a0 + mu_i
+  const int j0 = blockIdx.y * kGammaStrikeChunk;
+  double kk[kGammaStrikeChunk];
+  int ty[kGammaStrikeChunk];
+#pragma unroll
+  for (int c = 0; c < kGammaStrikeChunk; ++c) {
+    kk[c] = j0 + c < J ? strikes[j0 + c] : 0.0;
+    ty[c] = j0 + c < J ? (int)types[j0 + c] : -1;
+  }
+  const bool is_qvar = variable_type == B200SV_Q_VAR;
+  const double inv_f = 1.0 / forward, inv_f2 = inv_f * inv_f, inv_ttm = 1.0 / ttm;
+  constexpr double kInvSqrt2Pi = 0.3989422804014326779;
+  double acc[KC];
+#pragma unroll
+  for (int c = 0; c < KC; ++c) acc[c] = 0.0;
+  const long long stride = (long long)gridDim.x * kThreads;
+  for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < n; i += stride) {
+    const double fe = forward * exp(x[i]);
+    const double spot = fe - corr;
+    const double under = is_qvar ? q[i] * inv_ttm : spot;
+    const double s = laststep[i], log_a = log_a0 + laststep[n + i], cshift = fma(-fe, inv_cnt, corr);
+#pragma unroll
+    for (int c = 0; c < kGammaStrikeChunk; ++c) {
+      if (ty[c] < 0) continue;
+      const bool is_put = ty[c] & 1, inverse = ty[c] >= 2;
+      const bool itm = is_put ? under < kk[c] : under > kk[c];
+      const double h = itm ? (is_put ? kk[c] - under : under - kk[c]) : 0.0;
+      const double pay = inverse ? h / spot : h;
+      if (pay != pay) continue;
+      double g;
+      if (is_qvar) {
+        g = inverse ? 2.0 * pay * inv_f2 : 0.0;
+      } else {
+        const double kc = kk[c] + cshift;
+        double dens = 0.0;
+        if (kc > 0.0) {
+          const double d = (log(kc) - log_a) / s;
+          dens = kInvSqrt2Pi * exp(-0.5 * d * d) / (kc * s);
+        }
+        g = inverse ? kk[c] * inv_f2 * dens : kk[c] * kk[c] * inv_f2 * dens;
+        if (inverse && itm) g += (is_put ? 2.0 : -2.0) * kk[c] * inv_f2 / spot;
+      }
+      acc[2 * c] += g;
+      acc[2 * c + 1] = fma(g, g, acc[2 * c + 1]);
+    }
+  }
+  block_sum<KC, kThreads>(acc, red);
+  if (threadIdx.x == 0) {
+#pragma unroll
+    for (int c = 0; c < KC; ++c) partials[(size_t)blockIdx.x * Kpad + 2 * j0 + c] = acc[c];
+  }
+}
+
+// gamma[Jtot] = df * mean(g), gamma_se = df * std(g) / sqrt(total_paths): the sensitivity rows' convention, over the price row's count
+// (column 2 of the KV-wide payoff sums: the gamma sums skip the same paths)
+__global__ void gamma_finalize_kernel(const double* __restrict__ gsums, const double* __restrict__ sums, int KV, int J, double discfactor,
+                                      double total_paths, double* __restrict__ gamma, double* __restrict__ gamma_se) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= J) return;
+  const double cnt = sums[(size_t)KV * j + 2];
+  const double mean = gsums[2 * j] / cnt;
+  double var = gsums[2 * j + 1] / cnt - mean * mean;
+  var = var > 0.0 ? var : 0.0;
+  gamma[j] = discfactor * mean;
+  gamma_se[j] = discfactor * sqrt(var) / sqrt(total_paths);
 }
 
 // --------------------------------------------------------------------------------------------------------------------
@@ -1629,17 +1753,21 @@ struct ChainIO {
 // into, per-strike sums of the payoff and its sensitivities, their partials (sized once for the widest slice), and the result block
 // [prices | std errors | greeks [1 + NP] | greeks_se [1 + NP]][Jalloc].
 // SCORE: the payoff launches add the likelihood-ratio term of a score array (payoff_score_greeks_kernel, LOG_RETURN only)
+// with_gamma: two more result rows [gamma | gamma_se][Jalloc] after those, filled by payoff_gamma().
 template <int NP, bool SCORE = false>
 struct GreeksChainIO : ChainIO {
   static constexpr int KV = 3 + 2 * (1 + NP);
   long long n;
+  bool with_gamma;
   Grid gp;      // payoff_greeks_kernel's persistent grid, its blocks split across the strike chunks of a slice
-  DevBuf d_part;
+  Grid gg;      // payoff_gamma_kernel's, likewise
+  DevBuf d_part, d_gpart, d_gsums;
 
   GreeksChainIO(int M_, const double* ttms_, const double* forwards_, const double* discfactors_, const int* offsets_, const int8_t* types_,
-                int variable_type_, long long nb_path, cudaStream_t s)
-      : ChainIO(1, M_, ttms_, forwards_, discfactors_, offsets_, types_, variable_type_, s), n(nb_path),
-        gp(payoff_grid(nb_path)), d_part(s) {}
+                int variable_type_, long long nb_path, cudaStream_t s, bool with_gamma_ = false)
+      : ChainIO(1, M_, ttms_, forwards_, discfactors_, offsets_, types_, variable_type_, s), n(nb_path), with_gamma(with_gamma_),
+        gp(payoff_grid(nb_path)), gg(with_gamma_ ? persistent_grid(payoff_gamma_kernel, kThreads, nb_path) : Grid{}), d_part(s), d_gpart(s),
+        d_gsums(s) {}
 
   static Grid payoff_grid(long long nb_path) {
     if constexpr (SCORE) return persistent_grid(payoff_score_greeks_kernel<NP>, kThreads, nb_path);
@@ -1651,7 +1779,32 @@ struct GreeksChainIO : ChainIO {
     for (int m = 0; m < M; ++m) Jmax = std::max(Jmax, offsets[m + 1] - offsets[m]);
     const int max_chunks = std::max(1, (Jmax + kGreeksStrikeChunk - 1) / kGreeksStrikeChunk);
     B200SV_CUDA(d_part.alloc(sizeof(double) * (size_t)KV * kGreeksStrikeChunk * max_chunks * gp.blocks));
-    return ChainIO::upload(strikes, 2 + NP, KV, 2 * (2 + NP));
+    if (with_gamma) {
+      const int gamma_chunks = std::max(1, (Jmax + kGammaStrikeChunk - 1) / kGammaStrikeChunk);
+      B200SV_CUDA(d_gpart.alloc(sizeof(double) * (size_t)2 * kGammaStrikeChunk * gamma_chunks * gg.blocks));
+      B200SV_CUDA(d_gsums.alloc(sizeof(double) * 2 * (size_t)Jalloc));
+    }
+    return ChainIO::upload(strikes, 2 + NP, KV, 2 * (2 + NP) + (with_gamma ? 2 : 0));
+  }
+
+  // maturity m, after payoff(): per-strike sums of the smoothed gamma over the state (x, q) and the last step's laststep [2][n] = (s, mu)
+  // -> the gamma rows of the result block, over the count payoff() left in the payoff sums
+  int payoff_gamma(int m, const double* x, const double* q, const double* laststep) {
+    const int J = offsets[m + 1] - offsets[m], jo = offsets[m] - offsets[0];
+    if (J == 0) return 0;
+    const int chunks = (J + kGammaStrikeChunk - 1) / kGammaStrikeChunk;
+    const int Kpad = 2 * kGammaStrikeChunk * chunks;
+    const int blocks = std::max(1, gg.blocks / chunks);
+    payoff_gamma_kernel<<<dim3(blocks, chunks), gg.threads, 0, st>>>(x, q, laststep, n, ttms[m], forwards[m], d_strikes.as<double>() + jo,
+                                                                     d_types.as<int8_t>() + jo, J, variable_type, moments(), d_gpart.as<double>(),
+                                                                     Kpad);
+    if (int rc = check_launch("payoff_gamma_kernel")) return rc;
+    reduce_partials_kernel<<<1, 256, 0, st>>>(d_gpart.as<double>(), blocks, Kpad, 2 * J, d_gsums.as<double>(), P2pPublish{});
+    if (int rc = check_launch("reduce_partials_kernel")) return rc;
+    double* o = d_out.as<double>() + (size_t)2 * (2 + NP) * Jalloc + jo;
+    gamma_finalize_kernel<<<(J + 127) / 128, 128, 0, st>>>(d_gsums.as<double>(), d_sums.as<double>(), KV, J, discfactors[m], (double)n, o,
+                                                           o + Jalloc);
+    return check_launch("gamma_finalize_kernel");
   }
 
   // maturity m: per-strike payoff and sensitivity sums over the state (x, q) and its tangents (dx, dq) [NP][n] -> prices, price-row std
@@ -1681,10 +1834,12 @@ struct GreeksChainIO : ChainIO {
   }
 
   // one device-to-host copy of the result block, the synchronisation that ends the call, then the scatter into prices_out, stderr_out [Jtot]
-  // and greeks_out, greeks_se_out [1 + NP][Jtot] (a non-empty chain has Jalloc == Jtot, so the block's rows are already the caller's)
-  int copy_back(StreamSync& sync, double* prices_out, double* stderr_out, double* greeks_out, double* greeks_se_out) const {
+  // and greeks_out, greeks_se_out [1 + NP][Jtot] (a non-empty chain has Jalloc == Jtot, so the block's rows are already the caller's);
+  // with_gamma also gamma_out, gamma_se_out [Jtot]
+  int copy_back(StreamSync& sync, double* prices_out, double* stderr_out, double* greeks_out, double* greeks_se_out, double* gamma_out = nullptr,
+                double* gamma_se_out = nullptr) const {
     const size_t J = (size_t)Jtot, G = (size_t)(1 + NP) * J;
-    std::vector<double> h(2 * J + 2 * G);
+    std::vector<double> h(2 * J + 2 * G + (with_gamma ? 2 * J : 0));
     if (J > 0) B200SV_CUDA(d_out.download(h.data(), h.size()));
     if (int rc = sync.done()) return rc;
     if (J == 0) return 0;
@@ -1692,6 +1847,10 @@ struct GreeksChainIO : ChainIO {
     memcpy(stderr_out, h.data() + J, sizeof(double) * J);
     memcpy(greeks_out, h.data() + 2 * J, sizeof(double) * G);
     memcpy(greeks_se_out, h.data() + 2 * J + G, sizeof(double) * G);
+    if (with_gamma) {
+      memcpy(gamma_out, h.data() + 2 * J + 2 * G, sizeof(double) * J);
+      memcpy(gamma_se_out, h.data() + 3 * J + 2 * G, sizeof(double) * J);
+    }
     return 0;
   }
 };
@@ -1894,12 +2053,15 @@ static int greeks_gauss(int flags) {
   return g;
 }
 
-// one maturity slice with tangents; moments_out[2 + P] = (sum F e^x, count, sum F e^x dx_p)
+// one maturity slice with tangents; moments_out[2 + P] = (sum F e^x, count, sum F e^x dx_p).  laststep != nullptr: the recording variant,
+// which also writes (s, mu) of every path's last step to laststep [2][n].  Both variants take the grid of the plain kernel, so the
+// moments' reduction order -- and every number the plain kernel produces -- is the same.
 template <typename TConsts>
 static int launch_tangent_slice(int gauss, double* x, double* v, double* q, const TangentState& t, long long n, long long path_offset, int init,
                                 double v_init, int nsteps, int slice_index, double forward, uint64_t seed, const TConsts& c, double* moments_out,
-                                cudaStream_t st) {
+                                cudaStream_t st, double* laststep = nullptr) {
   using TPath = TangentPathOf<TConsts>;
+  using RPath = LastStepPath<TPath>;
   constexpr int K = 2 + TPath::NP;
   const auto kernel = gauss == kGaussF64 ? mc_tangent_slice_kernel<TPath, kGaussF64> : mc_tangent_slice_kernel<TPath, kGaussF32>;
   const Grid g = persistent_grid(kernel, kSliceThreads, n);
@@ -1907,36 +2069,47 @@ static int launch_tangent_slice(int gauss, double* x, double* v, double* q, cons
   B200SV_CUDA(partials.alloc(sizeof(double) * K * g.blocks));
   const SliceArgs<double> a{x, v, q, n, (unsigned long long)path_offset, init, v_init, nsteps, (unsigned int)slice_index, seed, forward,
                             partials.as<double>()};
-  kernel<<<g.blocks, g.threads, 0, st>>>(a, t, c);
+  if (laststep) {
+    const auto rkernel = gauss == kGaussF64 ? mc_tangent_slice_kernel<RPath, kGaussF64> : mc_tangent_slice_kernel<RPath, kGaussF32>;
+    rkernel<<<g.blocks, g.threads, 0, st>>>(a, t, LastStepConsts<TPath>{c, laststep});
+  } else {
+    kernel<<<g.blocks, g.threads, 0, st>>>(a, t, c);
+  }
   if (int rc = check_launch("mc_tangent_slice_kernel")) return rc;
   reduce_partials_kernel<<<1, 64, 0, st>>>(a.partials, g.blocks, K, K, moments_out, P2pPublish{});
   return check_launch("reduce_partials_kernel");
 }
 
 // chain driver: per maturity tangent slice -> moments -> per-strike payoff / sensitivity sums -> finalize (stand-alone launches, fixed-order
-// reductions).  greeks_out / greeks_se_out: [1 + P][Jtot], row 0 = forward delta.
+// reductions).  greeks_out / greeks_se_out: [1 + P][Jtot], row 0 = forward delta.  gamma_out != nullptr: the slices record their last
+// step and the smoothed gamma rows gamma_out / gamma_se_out [Jtot] are added (DESIGN.md §3.9), the other outputs unchanged; laststep_out
+// [M][2][n_paths_out] (test hook, may be NULL) receives (s, mu) of paths [0, n_paths_out) after every maturity.
 template <typename Params>
 static int mc_chain_greeks_host(const Params& p, int M, const double* ttms, const double* forwards, const double* discfactors, const double* etas,
                                 const int* offsets, const double* strikes, const int8_t* types, long long nb_path, int nb_steps_per_year,
                                 int is_spot, int variable_type, uint64_t seed, int flags, double* prices_out, double* stderr_out,
-                                double* greeks_out, double* greeks_se_out) {
+                                double* greeks_out, double* greeks_se_out, double* gamma_out = nullptr, double* gamma_se_out = nullptr,
+                                long long n_paths_out = 0, double* laststep_out = nullptr) {
   using TConsts = decltype(tangent_consts(p, 1.0, false, 1.0));
   constexpr int NP = TangentPathOf<TConsts>::NP;
+  const bool with_gamma = gamma_out != nullptr;
   B200SV_REQUIRE(nb_path >= 1, "nb_path must be >= 1");
   B200SV_REQUIRE(nb_steps_per_year >= 1, "nb_steps_per_year must be >= 1");
+  B200SV_REQUIRE(n_paths_out >= 0 && n_paths_out <= nb_path, "n_paths_out must be in [0, nb_path]");
   if (int rc = validate_chain(M, ttms, offsets, strikes, types, variable_type)) return rc;
   const int gauss = greeks_gauss(flags);
   if (gauss < 0) return gauss;
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
   StreamSync sync(st);
-  const size_t n = (size_t)nb_path;
+  const size_t n = (size_t)nb_path, no = laststep_out ? (size_t)n_paths_out : 0;
   DevBuf d_state(st);
-  GreeksChainIO<NP> io(M, ttms, forwards, discfactors, offsets, types, variable_type, nb_path, st);
-  B200SV_CUDA(d_state.alloc(sizeof(double) * (3 * n + 3 * (size_t)NP * n)));
+  GreeksChainIO<NP> io(M, ttms, forwards, discfactors, offsets, types, variable_type, nb_path, st, with_gamma);
+  B200SV_CUDA(d_state.alloc(sizeof(double) * (3 * n + 3 * (size_t)NP * n + (with_gamma ? 2 * n : 0))));
   if (int rc = io.upload(strikes)) return rc;
   double *x = d_state.as<double>(), *v = x + n, *q = v + n;
   const TangentState t{q + n, q + n + NP * n, q + n + 2 * NP * n};
+  double* laststep = with_gamma ? q + n + 3 * NP * n : nullptr;     // [2][n], reused across maturities
   double t0 = 0.0;
   for (int m = 0; m < M; ++m) {
     int S;
@@ -1944,10 +2117,16 @@ static int mc_chain_greeks_host(const Params& p, int M, const double* ttms, cons
     time_grid(ttms[m] - t0, nb_steps_per_year, &S, &dt);
     t0 = ttms[m];
     const TConsts c = tangent_consts(p, etas ? etas[m] : 1.0, is_spot != 0, dt);
-    if (int rc = launch_tangent_slice(gauss, x, v, q, t, nb_path, 0, m == 0, v_init(p), S, m, forwards[m], seed, c, io.moments(), st)) return rc;
+    if (int rc = launch_tangent_slice(gauss, x, v, q, t, nb_path, 0, m == 0, v_init(p), S, m, forwards[m], seed, c, io.moments(), st, laststep))
+      return rc;
     if (int rc = io.payoff(m, x, q, t.dx, t.dq, (double)nb_path)) return rc;
+    if (!with_gamma) continue;
+    if (int rc = io.payoff_gamma(m, x, q, laststep)) return rc;
+    if (no)
+      B200SV_CUDA(cudaMemcpy2DAsync(laststep_out + 2 * no * m, sizeof(double) * no, laststep, sizeof(double) * n, sizeof(double) * no, 2,
+                                    cudaMemcpyDeviceToHost, st));
   }
-  return io.copy_back(sync, prices_out, stderr_out, greeks_out, greeks_se_out);
+  return io.copy_back(sync, prices_out, stderr_out, greeks_out, greeks_se_out, gamma_out, gamma_se_out);
 }
 
 // one slice from the initial state (0, v_init, 0) with initial tangents, for paths [path_offset, path_offset + n) of Philox slice
@@ -2085,6 +2264,34 @@ int b200sv_heston_mc_chain_greeks(const b200sv_heston_params* params, int M, con
   B200SV_REQUIRE(scheme == B200SV_HESTON_EULER_FLOOR, "pathwise sensitivities need scheme = B200SV_HESTON_EULER_FLOOR");
   return mc_chain_greeks_host(*params, M, ttms, forwards, discfactors, nullptr, offsets, strikes, types, nb_path, nb_steps_per_year, 1,
                               variable_type, seed, flags, prices_out, stderr_out, greeks_out, greeks_se_out);
+}
+
+int b200sv_logsv_mc_chain_greeks_gamma(const b200sv_logsv_params* params, int M, const double* ttms, const double* forwards,
+                                       const double* discfactors, const double* etas, const int* offsets, const double* strikes,
+                                       const int8_t* types, long long nb_path, int nb_steps_per_year, int is_spot_measure, int variable_type,
+                                       uint64_t seed, int flags, double* prices_out, double* stderr_out, double* greeks_out,
+                                       double* greeks_se_out, double* gamma_out, double* gamma_se_out, long long n_paths_out,
+                                       double* laststep_out) {
+  B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && stderr_out && greeks_out && greeks_se_out && gamma_out &&
+                     gamma_se_out,
+                 "null pointer");
+  return mc_chain_greeks_host(*params, M, ttms, forwards, discfactors, etas, offsets, strikes, types, nb_path, nb_steps_per_year, is_spot_measure,
+                              variable_type, seed, flags, prices_out, stderr_out, greeks_out, greeks_se_out, gamma_out, gamma_se_out, n_paths_out,
+                              laststep_out);
+}
+
+int b200sv_heston_mc_chain_greeks_gamma(const b200sv_heston_params* params, int M, const double* ttms, const double* forwards,
+                                        const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
+                                        long long nb_path, int nb_steps_per_year, int variable_type, uint64_t seed, int flags, int scheme,
+                                        double* prices_out, double* stderr_out, double* greeks_out, double* greeks_se_out, double* gamma_out,
+                                        double* gamma_se_out, long long n_paths_out, double* laststep_out) {
+  B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && stderr_out && greeks_out && greeks_se_out && gamma_out &&
+                     gamma_se_out,
+                 "null pointer");
+  B200SV_REQUIRE(scheme == B200SV_HESTON_EULER_FLOOR, "pathwise sensitivities need scheme = B200SV_HESTON_EULER_FLOOR");
+  return mc_chain_greeks_host(*params, M, ttms, forwards, discfactors, nullptr, offsets, strikes, types, nb_path, nb_steps_per_year, 1,
+                              variable_type, seed, flags, prices_out, stderr_out, greeks_out, greeks_se_out, gamma_out, gamma_se_out, n_paths_out,
+                              laststep_out);
 }
 
 int b200sv_logsv_tangent_terminal(const b200sv_logsv_params* params, double ttm, long long nb_path, int nb_steps_per_year, int is_spot_measure,

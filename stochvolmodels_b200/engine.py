@@ -145,6 +145,36 @@ def heston_mc_chain_greeks(params: C.HestonParamsC, ttms, forwards, discfactors,
                      (int(nb_path), int(nb_steps_per_year)), variable_type, seed, flags, (int(scheme),), n_greeks=len(HESTON_GREEK_PARAMS))
 
 
+def _mc_chain_greeks_gamma(symbol: str, params, chain, etas, head, variable_type, seed: int, flags: int, tail, n_greeks: int,
+                           n_paths_out: int):
+    M, J, n_out = len(chain[3]), sum(len(s) for s in chain[3]), int(n_paths_out)
+    gamma, gamma_se = np.empty(J), np.empty(J)
+    laststep = np.empty((M, 2, n_out)) if n_out else None
+    res = _mc_chain(symbol, params, chain, etas, head, variable_type, seed, flags, tail, n_greeks=n_greeks,
+                    post=(C.dptr(gamma), C.dptr(gamma_se), n_out, C.dptr(laststep)))
+    return (*res, gamma, gamma_se, laststep)
+
+
+def logsv_mc_chain_greeks_gamma(params: C.LogsvParamsC, ttms, forwards, discfactors, etas, strikes_ttms, optiontypes_ttms, nb_path: int,
+                                nb_steps_per_year: int, is_spot_measure: bool, variable_type, seed: int, flags: int, n_paths_out: int = 0):
+    """logsv_mc_chain_greeks plus the Monte Carlo gamma by conditional smoothing of the last step (b200sv_logsv_mc_chain_greeks_gamma;
+    DESIGN.md §3.9).  Returns (prices, std errors, greeks [1+6, J], greeks_se [1+6, J], offsets, gamma [J], gamma_se [J], laststep): the
+    first five bit-identical to logsv_mc_chain_greeks; with ``n_paths_out`` > 0, laststep [M, 2, n_paths_out] = (s, mu) of the first paths'
+    last step after each maturity (x = mu + s z0), else None."""
+    return _mc_chain_greeks_gamma("b200sv_logsv_mc_chain_greeks_gamma", params, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms),
+                                  (etas,), (int(nb_path), int(nb_steps_per_year), int(bool(is_spot_measure))), variable_type, seed, flags, (),
+                                  len(LOGSV_GREEK_PARAMS), n_paths_out)
+
+
+def heston_mc_chain_greeks_gamma(params: C.HestonParamsC, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, nb_path: int,
+                                 nb_steps_per_year: int, variable_type, seed: int, flags: int, scheme: int = C.HESTON_EULER_FLOOR,
+                                 n_paths_out: int = 0):
+    """Heston twin of logsv_mc_chain_greeks_gamma (b200sv_heston_mc_chain_greeks_gamma)."""
+    return _mc_chain_greeks_gamma("b200sv_heston_mc_chain_greeks_gamma", params, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms),
+                                  (), (int(nb_path), int(nb_steps_per_year)), variable_type, seed, flags, (int(scheme),),
+                                  len(HESTON_GREEK_PARAMS), n_paths_out)
+
+
 def hawkesjd_mc_chain_greeks(params: C.HawkesParamsC, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, nb_path: int, variable_type,
                              seed: int, flags: int, n_paths_out: int = 0):
     """chain MC of the Hawkes jump-diffusion with Monte Carlo sensitivities (b200sv_hawkesjd_mc_chain_greeks; DESIGN.md §3.11).  Returns

@@ -246,20 +246,22 @@ class LogSVPricer(ModelPricer):
     @timer
     def model_mc_chain_greeks(self, option_chain: OptionChain, params: LogSvParams, is_spot_measure: bool = True,
                               variable_type: VariableType = VariableType.LOG_RETURN, nb_path: int = 100000,
-                              nb_steps: Optional[int] = None, **kwargs):
+                              nb_steps: Optional[int] = None, with_gamma: bool = False, **kwargs):
         """MC prices and standard errors as ``model_mc_price_chain`` (same defaults, ``seed`` / ``gauss`` kwargs, same numbers on the same
         seed) plus pathwise sensitivities in the same pass: the forward delta and d price / d (sigma0, theta, kappa1, kappa2, beta, volvol),
         each with its standard error -> ``McChainGreeks``.  ``kappa2`` is the value after ``__post_init__`` and is held fixed when kappa1 or
         theta moves; the vol backbone and discount factors are not differentiated.  fp64 state only; no ``exchange``; the rough-vol route has its own ``rough_mc_chain_greeks``.
+        ``with_gamma=True`` also fills ``gamma`` / ``gamma_se`` (d^2 price / d forward^2 by conditional smoothing of the last step,
+        DESIGN.md §3.9) and leaves every other number unchanged.
         Under torch.distributed every rank prices all paths (replicated, bit-identical results)."""
         from .mc_greeks import check_greeks_kwargs, to_mc_chain_greeks
         check_greeks_kwargs(kwargs)
         vt = engine.variable_code(variable_type)
         flags = engine.mc_flags("fp64", kwargs.get("gauss", "fp32"))
-        res = engine.logsv_mc_chain_greeks(_params_c(params), option_chain.ttms, option_chain.forwards, option_chain.discfactors,
-                                           params.get_vol_backbone_etas(ttms=option_chain.ttms), option_chain.strikes_ttms,
-                                           option_chain.optiontypes_ttms, nb_path, nb_steps or int(360 * np.max(option_chain.ttms)) + 1,
-                                           is_spot_measure, vt, _shared_seed(kwargs.get("seed")), flags)
+        route = engine.logsv_mc_chain_greeks_gamma if with_gamma else engine.logsv_mc_chain_greeks
+        res = route(_params_c(params), option_chain.ttms, option_chain.forwards, option_chain.discfactors,
+                    params.get_vol_backbone_etas(ttms=option_chain.ttms), option_chain.strikes_ttms, option_chain.optiontypes_ttms, nb_path,
+                    nb_steps or int(360 * np.max(option_chain.ttms)) + 1, is_spot_measure, vt, _shared_seed(kwargs.get("seed")), flags)
         return to_mc_chain_greeks(res, engine.LOGSV_GREEK_PARAMS)
 
     @timer
@@ -272,7 +274,8 @@ class LogSVPricer(ModelPricer):
         orthogonal vol-of-vol, as on the price route; ``params.weights`` / ``params.nodes`` are inputs, not differentiated.  ``reset_paths``
         counts, per maturity, the paths that hit the reset-to-1e-6 branch (their mass across it is not in the rows).  fp64 only, no
         ``exchange``; under torch.distributed every rank prices all paths (replicated, bit-identical results)."""
-        from .mc_greeks import check_rough_greeks_kwargs, to_mc_chain_greeks
+        from .mc_greeks import check_no_gamma, check_rough_greeks_kwargs, to_mc_chain_greeks
+        check_no_gamma(kwargs, "rough_mc_chain_greeks")
         check_rough_greeks_kwargs(kwargs)
         vt = engine.variable_code(variable_type)
         gauss, seed = kwargs.get("gauss"), int(kwargs["seed"])

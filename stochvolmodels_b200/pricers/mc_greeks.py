@@ -24,7 +24,9 @@ class McChainGreeks:
     """prices / std errors / delta / delta_se: one array per maturity.  ``params`` / ``params_se``: parameter name (dataclass field,
     after ``__post_init__``) -> one array per maturity of d price / d parameter and its standard error.  ``reset_paths`` (rough-vol route
     only, else None): per maturity, the number of paths that took the reset-to-1e-6 branch at any step; the pathwise rows omit the price
-    mass such paths move across that switch, so they are unbiased for the scheme only where it is 0."""
+    mass such paths move across that switch, so they are unbiased for the scheme only where it is 0.  ``gamma`` / ``gamma_se`` (LogSV and
+    Heston with ``with_gamma=True``, else None): one array per maturity of d^2 price / d forward^2 by conditional smoothing of the
+    last step (DESIGN.md §3.9) and its standard error."""
     prices: List[np.ndarray]
     std_errors: List[np.ndarray]
     delta: List[np.ndarray]
@@ -32,6 +34,8 @@ class McChainGreeks:
     params: Dict[str, List[np.ndarray]]
     params_se: Dict[str, List[np.ndarray]]
     reset_paths: Optional[np.ndarray] = None
+    gamma: Optional[List[np.ndarray]] = None
+    gamma_se: Optional[List[np.ndarray]] = None
 
 
 def check_greeks_kwargs(kwargs, precision_default: str = "fp64") -> None:
@@ -76,10 +80,20 @@ def check_hawkes_mc_greeks_kwargs(kwargs, gauss, params) -> None:
         raise ValueError("the Hawkes Monte Carlo sensitivities need mean_p != 0 and mean_m != 0")
 
 
+def check_no_gamma(kwargs, method: str) -> None:
+    """the routes without a Monte Carlo gamma reject ``with_gamma=True`` before any GPU work"""
+    if kwargs.get("with_gamma"):
+        raise NotImplementedError(f"{method} has no Monte Carlo gamma: with_gamma=True covers LogSVPricer and HestonPricer.model_mc_chain_greeks")
+
+
 def to_mc_chain_greeks(result, names: Sequence[str]) -> McChainGreeks:
-    """engine.*_mc_chain_greeks output -> McChainGreeks"""
-    prices, stds, greeks, greeks_se, offsets = result
+    """engine.*_mc_chain_greeks output -> McChainGreeks; engine.*_mc_chain_greeks_gamma output (gamma and gamma_se after the offsets) fills
+    ``gamma`` / ``gamma_se`` as well"""
+    prices, stds, greeks, greeks_se, offsets = result[:5]
     split = lambda row: C.split_chain(row, offsets)
-    return McChainGreeks(prices=prices, std_errors=stds, delta=split(greeks[0]), delta_se=split(greeks_se[0]),
-                         params={n: split(greeks[1 + k]) for k, n in enumerate(names)},
-                         params_se={n: split(greeks_se[1 + k]) for k, n in enumerate(names)})
+    out = McChainGreeks(prices=prices, std_errors=stds, delta=split(greeks[0]), delta_se=split(greeks_se[0]),
+                        params={n: split(greeks[1 + k]) for k, n in enumerate(names)},
+                        params_se={n: split(greeks_se[1 + k]) for k, n in enumerate(names)})
+    if len(result) > 5:
+        out.gamma, out.gamma_se = split(result[5]), split(result[6])
+    return out
