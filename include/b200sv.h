@@ -491,6 +491,9 @@ int b200sv_fourier_digital(const double* log_mgf, const double* phi, int P, doub
  * (offsets[M]-offsets[0] entries).  'IC'/'IP' quotes are inverted like 'C'/'P'; prices outside the no-arbitrage bounds give NaN. */
 int b200sv_bsm_implied_vols(int M, const double* ttms, const double* forwards, const double* discfactors, const int* offsets,
                             const double* strikes, const int8_t* types, const double* prices, double* ivols_out);
+/* test hook: b200sv_bsm_implied_vols plus iterations_out[] = the Newton iterations each quote took (0 for a NaN verdict) */
+int b200sv_debug_bsm_implied_vols(int M, const double* ttms, const double* forwards, const double* discfactors, const int* offsets,
+                                  const double* strikes, const int8_t* types, const double* prices, double* ivols_out, int* iterations_out);
 
 #ifdef __cplusplus
 }

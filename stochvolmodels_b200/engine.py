@@ -727,6 +727,17 @@ def bsm_implied_vols(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms
     return C.split_chain(ivols, ch.offsets)
 
 
+def debug_bsm_implied_vols(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, prices_ttms):
+    """bsm_implied_vols through the debug twin of its kernel -> (ivols, iterations), both flat in chain order (b200sv_debug_bsm_implied_vols)"""
+    ch = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
+    prices = C.f64(np.concatenate([np.asarray(p, dtype=np.float64).ravel() for p in prices_ttms]))
+    if prices.shape[0] != ch.strikes.shape[0]:
+        raise ValueError("model prices and strikes must have the same length")
+    ivols, iterations = np.empty(ch.strikes.shape[0]), np.empty(ch.strikes.shape[0], dtype=np.int32)
+    C.call("b200sv_debug_bsm_implied_vols", *C.chain_ptrs(ch), C.dptr(prices), C.dptr(ivols), C.iptr(iterations))
+    return ivols, iterations
+
+
 def infer_bsm_ivols_from_model_chain_prices(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, model_prices_ttms):
     """the chain inversion the reference delegates to its third-party Black package (data/option_chain.py:340-345), keyword for keyword"""
     return bsm_implied_vols(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, model_prices_ttms)

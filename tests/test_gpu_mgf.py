@@ -179,7 +179,7 @@ def test_heston_qvar_and_digitals_vs_reference_golden(cuda_lib):
 
 
 def test_gpu_black_implied_vols(cuda_lib):
-    """the chain inversion kernel == the host checker (same bisection) and the reference's pinned quickstart vols; round trips."""
+    """the chain inversion kernel and the host bisection both within the exact-reference bar, and the reference's pinned quickstart vols; round trips."""
     from oracle import bsm
     from stochvolmodels_b200 import OptionChain, engine
     K = np.array([0.6, 0.9, 1.0, 1.1, 1.6])
@@ -189,11 +189,18 @@ def test_gpu_black_implied_vols(cuda_lib):
     prices = [bsm.compute_bsm_vanilla_price(fw[m], K, ttms[m], vols[m], types, df[m]) for m in range(3)]
     iv = engine.bsm_implied_vols(ttms, fw, df, [K] * 3, [types] * 3, prices)
     host = bsm.infer_bsm_ivols_from_model_chain_prices(ttms, fw, df, [K] * 3, [types] * 3, prices)
+    import ivol_cases as ic
+    pytest.importorskip("mpmath")
     for m in range(3):
-        good = prices[m] > 1e-8            # far-OTM quotes (price ~1e-12) are ill-conditioned: 1 ulp of price = 1e-5 of vol
+        # every quote against the exact implied vol of the fp64 quote as given (tests/ivol_cases.py), the far-OTM ones (~1e-12) included;
+        # the host bisection meets the same bar
+        c = dict(F=np.full(5, fw[m]), K=K, T=np.full(5, ttms[m]), D=np.full(5, df[m]), type=types, price=prices[m], vol=np.full(5, vols[m]))
+        iv_star, bar = ic.reference(c)
+        for got in (iv[m], host[m]):
+            ratio, nan_mismatch, bad = ic.check(got, iv_star, bar)
+            assert nan_mismatch.size == 0 and bad.size == 0, (m, ratio, got, iv_star)
+        good = prices[m] > 1e-8
         np.testing.assert_allclose(iv[m][good], vols[m], rtol=1e-8)
-        np.testing.assert_allclose(iv[m][good], host[m][good], rtol=1e-10)     # same bisection; normcdf vs scipy ndtr differ by ulps
-        assert np.all(np.isfinite(iv[m]) == np.isfinite(host[m]))
     chain = OptionChain.slice_to_chain(0.25, 1.0, np.array([1.0, 1.0]), np.array(["C", "C"]))
     out = chain.compute_model_ivols_from_chain_data([np.array([0.197330882838064, 1.5])])[0]
     np.testing.assert_allclose(out[0], 0.999577, rtol=5e-6)            # examples/getting_started/quickstart.py:44
