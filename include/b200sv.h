@@ -435,6 +435,18 @@ int b200sv_heston_price_chain_batch(const b200sv_heston_params* params, int B, i
                                     const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
                                     double vol_scaler, int P, double* prices_out, double* ivols_out);
 
+/* same for the Hawkes jump-diffusion: the objectives of HawkesJDPricer.calibrate_model_params_to_chain and
+ * calibrate_risk_premia_gamma_to_chain (pricers/hawkes_jd_pricer.py:230-357).  B Hawkes parameter sets on one chain in one pass.
+ * gammas: NULL = no risk kernel, else [B] finite risk_premia_gamma per set (all sets on the risk-kernel route: 'C' / 'P' under the spot
+ * measure only, else -5).  vol_scaler <= 0: per-set default grid clip(sigma_b, 0.2, 0.5) sqrt(min(min ttm, 1/12)); with gammas every set
+ * has its own grid (Re phi = -1/2 - gamma_b) either way.  P <= 0: 500 grid points.  prices_out [B][J], ivols_out [B][J] (NULL = skip the
+ * fused Black-76 inversion), row b in chain order.  Row b equals b200sv_hawkesjd_price_chain(params[b], gammas ? gammas[b] : NaN)
+ * (+ b200sv_bsm_implied_vols on the chain's forwards / discfactors) bit for bit. */
+int b200sv_hawkesjd_price_chain_batch(const b200sv_hawkes_params* params, int B, int M, const double* ttms, const double* forwards,
+                                      const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
+                                      int is_spot_measure, double vol_scaler, int P, const double* gammas,
+                                      double* prices_out, double* ivols_out);
+
 /* replaces compute_logsv_a_mgf_grid, non-analytic branch (pricers/logsv/affine_expansion.py:570-685 -> solve_a_ode_grid
  * :492-529): phi, psi, a (in: A(0), out: A(dtau)), log_mgf_out are complex128 interleaved host arrays of P, P, P*n, P. */
 int b200sv_logsv_mgf_grid(const double* phi, const double* psi, int P, double dtau, double* a_inout,

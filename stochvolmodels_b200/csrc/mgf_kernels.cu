@@ -876,6 +876,41 @@ __global__ void __launch_bounds__(kFourierThreads) fourier_gamma_kernel(const cd
   }
 }
 
+// fourier_gamma_kernel over the rows of a batch (b200sv_hawkesjd_price_chain_batch), with the Black inversion of fourier_vanilla_kernel
+// fused: row grid sp.grid sits on Re phi = -1/2 - gammas[sp.grid]; norm_gfwd[2 sp.slice + {0, 1}] = that slice's normaliser and forward under
+// the risk kernel.  spec.forward / discfactor / ttm are the chain's own: the calibration objective inverts the (undiscounted) gamma price
+// with the chain's forward, discount factor and maturity (compute_model_ivols_from_chain_data, as in the reference).
+__global__ void __launch_bounds__(kFourierThreads) fourier_gamma_batch_kernel(const cd* __restrict__ log_mgf, const cd* __restrict__ phi, int P,
+                                                                             const StrikeSpec* __restrict__ specs, const double* __restrict__ gammas,
+                                                                             const double* __restrict__ norm_gfwd, double* __restrict__ prices,
+                                                                             double* __restrict__ ivols) {
+  __shared__ double red[kFourierThreads / 32];
+  const StrikeSpec sp = specs[blockIdx.x];
+  const double gamma = gammas[sp.grid];
+  const cd* lm = log_mgf + (size_t)sp.slice * P;
+  phi += (size_t)sp.grid * P;
+  const double x = log(sp.forward / sp.strike);
+  const double h3 = (phi[1].im - phi[0].im) / 3.0;
+  const bool fast = fabs(phi[0].re - (0.5 + gamma)) < 1e-10;
+  double acc[1] = {0.0};
+  for (int j = threadIdx.x; j < P; j += kFourierThreads) {
+    const double wq = (j & 1) ? 4.0 : ((j == 0 || j == P - 1) ? 1.0 : 2.0);
+    const double dp = h3 * wq;
+    const cd ph = phi[j];
+    const cd pg = ph + mk(gamma);
+    const cd w = fast ? mk((dp / M_PI) / (ph.im * ph.im + 0.25)) : -(mk(dp / M_PI) / ((pg + mk(1.0)) * pg));
+    const cd term = w * cexp_(lm[j] - x * ph);
+    if (term.re == term.re) acc[0] += term.re;
+  }
+  block_sum<1, kFourierThreads>(acc, red);
+  if (threadIdx.x == 0) {
+    const double gk = pow(sp.strike, 1.0 + gamma), normalizer = norm_gfwd[2 * (size_t)sp.slice], gamma_forward = norm_gfwd[2 * (size_t)sp.slice + 1];
+    const double price = (sp.type == B200SV_CALL ? gamma_forward : sp.strike) - normalizer * gk * acc[0];
+    prices[blockIdx.x] = price;
+    if (ivols) ivols[blockIdx.x] = black_implied_vol(sp.forward, sp.strike, sp.ttm, sp.discfactor, price, sp.type);
+  }
+}
+
 // --------------------------------------------------------------------------------------------------------------------
 // Forward-mode sensitivities of the Fourier chain pricers (DESIGN.md §4.2)
 // --------------------------------------------------------------------------------------------------------------------
@@ -2195,6 +2230,29 @@ static int queue_hawkes_prices(ChainDev& d, const FourierChain& c, const HawkesM
   return d.sums(c, prices_out, nullptr, gamma);
 }
 
+// Validation of b200sv_hawkesjd_price_chain_batch: sizes, the risk-premia gammas (all finite), then the chain.  The grids follow
+// prepare_hawkes_chain set by set: Re phi = -1/2 - gamma_b under both measures.  With gammas every set needs its own grid even when
+// vol_scaler pins the imaginary parts, since the real parts differ.
+static int prepare_hawkes_batch(FourierChain& c, const b200sv_hawkes_params* params, int B, int M, const double* ttms, const double* forwards,
+                                const double* discfactors, const int* offsets, const double* strikes, const int8_t* types, int is_spot_measure,
+                                double vol_scaler, int P, const double* gammas) {
+  if (int rc = c.init(true, B, M, P > 0 ? P : 500, offsets)) return rc;     // MAX_PHI, hawkes_jd_pricer.py:37
+  if (gammas)
+    for (int b = 0; b < B; ++b) B200SV_REQUIRE(std::isfinite(gammas[b]), "gammas must be finite (NULL: no risk kernel)");
+  if (int rc = c.build(params, ttms, forwards, discfactors, offsets, strikes, types, is_spot_measure != 0,
+                       gammas ? ChainTypes::kGamma : ChainTypes::kFourier, vol_scaler))
+    return rc;
+  if (gammas && !c.per_set_grid) {
+    const std::vector<double> one(c.phi);
+    for (int b = 1; b < B; ++b) c.phi.insert(c.phi.end(), one.begin(), one.end());
+    for (size_t i = 0; i < c.ss.size(); ++i) c.ss[i].grid = (int)(i / c.Jtot);
+    c.per_set_grid = true;
+  }
+  for (int g = 0; g < (c.per_set_grid ? B : 1); ++g)
+    for (int i = 0; i < c.P; ++i) c.phi[2 * ((size_t)g * c.P + i)] = gammas ? -0.5 - gammas[g] : -0.5;
+  return 0;
+}
+
 // Plumbing of the single-grid entry points: phi [P], psi [P] (when given) and a_in [P][n] (when given) go up, `launch` queues its
 // kernel(s) on them and returns check_launch's code, then a_out [P][n] and log_mgf_out [P] (when given) come back.
 template <class Launch>
@@ -2464,6 +2522,74 @@ int b200sv_hawkesjd_price_chain_greeks(const b200sv_hawkes_params* params, int M
   }
   B200SV_CUDA(d_dlm.download(cplx(dlog_mgf_out), (size_t)NP * M * P));
   B200SV_CUDA(d_nfev.download(nfev_out, P));
+  return d.sync.done();
+}
+
+/* B Hawkes parameter sets on one chain in one pass (the calibration drivers' objective and its finite-difference neighbours).  The Riccati
+ * grids run through the single-set hawkes_mgf_kernel, one launch per set queued back to back: a kernel of its own that read the constants
+ * per set from memory contracts its fp64 arithmetic into different fused multiply-adds and moves prices by an ulp (DESIGN.md §9), and the
+ * rows must equal b200sv_hawkesjd_price_chain bit for bit.  With gammas, the two restarted single-point solves per (set, maturity) come
+ * first and ONE copy back feeds the host-side normalisers / forwards (the same host arithmetic as there).  Then all sets' Fourier sums
+ * (vanilla or gamma) in one launch, the Black inversion fused, and one copy back. */
+int b200sv_hawkesjd_price_chain_batch(const b200sv_hawkes_params* params, int B, int M, const double* ttms, const double* forwards,
+                                      const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
+                                      int is_spot_measure, double vol_scaler, int P, const double* gammas, double* prices_out,
+                                      double* ivols_out) {
+  B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && strikes && types && prices_out, "null pointer");
+  FourierChain c;
+  if (int rc = prepare_hawkes_batch(c, params, B, M, ttms, forwards, discfactors, offsets, strikes, types, is_spot_measure, vol_scaler, P,
+                                    gammas))
+    return rc;
+  P = c.P;
+  std::vector<HawkesMgfConsts> k(B);
+  for (int b = 0; b < B; ++b) k[b] = make_hawkes_mgf_consts(params[b]);
+  ChainDev d;
+  DevBuf d_gam(d.st), d_ng(d.st);
+  std::vector<double> dts(c.dtaus);
+  dts.insert(dts.end(), ttms, ttms + M);                                        // [increments | full maturities]
+  B200SV_CUDA(d.dt.upload(dts.data(), dts.size()));
+  if (gammas) {                                                                // hawkesjd_forwards_under_risk_kernel (:487-515), per set
+    std::vector<double> two(4 * (size_t)B, 0.0), lm2(4 * (size_t)B * M), ng(2 * (size_t)B * M);
+    for (int b = 0; b < B; ++b) {
+      two[4 * (size_t)b] = -gammas[b];
+      two[4 * (size_t)b + 2] = -gammas[b] - 1.0;
+    }
+    DevBuf d_two(d.st), d_lm2(d.st);
+    B200SV_CUDA(d_two.upload(cplx(two.data()), 2 * (size_t)B));
+    B200SV_CUDA(d_lm2.alloc(sizeof(cd) * 2 * (size_t)B * M));
+    for (int b = 0; b < B; ++b) {
+      launch_hawkes_mgf(d.st, d_two.as<cd>() + 2 * b, nullptr, 2, M, d.dt.as<double>() + M, k[b], nullptr, nullptr, d_lm2.as<cd>() + 2 * (size_t)M * b, 1);
+      if (int rc = check_launch("hawkes_mgf_kernel")) return rc;
+    }
+    B200SV_CUDA(d_lm2.download(cplx(lm2.data()), 2 * (size_t)B * M));
+    B200SV_CUDA(cudaStreamSynchronize(d.st));
+    for (int b = 0; b < B; ++b)
+      for (int m = 0; m < M; ++m) {                                            // log_mgf layout [b][m][point]
+        const size_t s = (size_t)b * M + m;
+        ng[2 * s] = 1.0 / std::exp(lm2[2 * (2 * s + 0)]);
+        ng[2 * s + 1] = forwards[m] * std::exp(lm2[2 * (2 * s + 1)]) * ng[2 * s];
+      }
+    B200SV_CUDA(d_ng.upload(ng.data(), ng.size()));
+    B200SV_CUDA(d_gam.upload(gammas, (size_t)B));
+  }
+  if (int rc = d.upload(c)) return rc;
+  for (int b = 0; b < B; ++b) {
+    launch_hawkes_mgf(d.st, d.phi.as<cd>() + (c.per_set_grid ? (size_t)b * P : 0), nullptr, P, M, d.dt.as<double>(), k[b], nullptr, nullptr,
+                      d.lm.as<cd>() + (size_t)b * M * P, 0);
+    if (int rc = check_launch("hawkes_mgf_kernel")) return rc;
+  }
+  if (!gammas) {
+    if (int rc = d.sums(c, prices_out, ivols_out)) return rc;
+    return d.sync.done();
+  }
+  const size_t nq = (size_t)B * c.Jtot;
+  if (ivols_out) B200SV_CUDA(d.iv.alloc(sizeof(double) * nq));
+  fourier_gamma_batch_kernel<<<(unsigned)nq, kFourierThreads, 0, d.st>>>(d.lm.as<cd>(), d.phi.as<cd>(), P, d.rows.as<StrikeSpec>(),
+                                                                         d_gam.as<double>(), d_ng.as<double>(), d.pr.as<double>(),
+                                                                         d.iv.as<double>());
+  if (int rc = check_launch("fourier_gamma_batch_kernel")) return rc;
+  B200SV_CUDA(d.pr.download(prices_out, nq));
+  B200SV_CUDA(d.iv.download(ivols_out, nq));
   return d.sync.done();
 }
 

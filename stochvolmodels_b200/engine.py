@@ -615,6 +615,24 @@ def heston_price_chain_batch(params_list: Sequence[C.HestonParamsC], ttms, forwa
                         optiontypes_ttms), (), (C.vol_scaler_arg(vol_scaler), int(max_phi)), 1, with_ivols)
 
 
+def hawkesjd_price_chain_batch(params_list: Sequence[C.HawkesParamsC], ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms,
+                               is_spot_measure: bool = True, vol_scaler: Optional[float] = None, max_phi: int = 500, gammas=None,
+                               with_ivols: bool = True):
+    """B Hawkes parameter sets on one chain in one pass -> (prices [B, J], ivols [B, J] | None).  ``gammas``: None (no risk kernel) or [B]
+    risk_premia_gamma per set, every set then priced under its risk kernel.  Row b is bit-identical to hawkesjd_price_chain of set b."""
+    if gammas is None:
+        _check_fourier_types(optiontypes_ttms, bool(is_spot_measure))
+    else:
+        if not is_spot_measure or any(str(t) not in ("C", "P") for types in optiontypes_ttms for t in types):
+            raise ValueError("not implemented")           # utils/mgf_pricer.py:310-318
+        gammas = C.f64(gammas)
+        if gammas.shape != (len(params_list),):
+            raise ValueError(f"gammas must have shape ({len(params_list)},)")
+    return _chain_batch("b200sv_hawkesjd_price_chain_batch", C.HawkesParamsC, params_list, (ttms, forwards, discfactors, strikes_ttms,
+                        optiontypes_ttms), (), (int(bool(is_spot_measure)), C.vol_scaler_arg(vol_scaler), int(max_phi), C.dptr(gammas)), 1,
+                        with_ivols)
+
+
 def _logsv_mgf_grid(symbol: str, phi, psi, dtau: float, a_t0, params: C.LogsvParamsC, expansion_order: int, args):
     """the three LogSV grid solvers: C arguments (phi, psi, P, dtau, a, params, *args, log_mgf) -> (a_t1 [P, n], log_mgf [P])"""
     phi = C.c128(phi)

@@ -150,6 +150,84 @@ class BatchedObjective:
         return self._g.copy()
 
 
+def scipy_difference_steps(x: np.ndarray, eps: float, bounds) -> np.ndarray:
+    """the steps h of scipy's 2-point ``approx_derivative(abs_step=eps, bounds=bounds)`` -- what SLSQP differences an objective with when it
+    is given no ``jac``: eps, a relative step sqrt(machine eps) sign(x) max(1, |x|) where x + eps == x, then the one-sided bound handling of
+    ``_adjust_scheme_to_bounds``: flipped where x + h leaves the box and -h fits, else the distance to the farther bound."""
+    lb = np.array([-np.inf if b[0] is None else b[0] for b in bounds], dtype=float)
+    ub = np.array([np.inf if b[1] is None else b[1] for b in bounds], dtype=float)
+    sign = (x >= 0).astype(x.dtype) * 2 - 1
+    h = np.where(((x + eps) - x) == 0, SLSQP_EPS * sign * np.maximum(1.0, np.abs(x)), eps).astype(x.dtype)
+    if np.all((lb == -np.inf) & (ub == np.inf)):
+        return h
+    lower, upper = x - lb, ub - x
+    xh = x + h
+    fitting = np.abs(h) <= np.maximum(lower, upper)
+    h[((xh < lb) | (xh > ub)) & fitting] *= -1
+    forward = (upper >= lower) & ~fitting
+    h[forward] = upper[forward]
+    backward = (upper < lower) & ~fitting
+    h[backward] = -lower[backward]
+    return h
+
+
+@dataclass
+class ScipyDifferenceObjective:
+    """objective + the gradient scipy would difference from it (scipy_difference_steps), memoised on the last point.  ``fun(x)`` prices x
+    alone; ``jac(x)`` prices its n neighbours x + h_i e_i together in ONE batch, so a point SLSQP only asks the value of (a line-search
+    trial) costs one set, and every set is priced once.  Each row is reduced with the sequential objective's own expression
+    (``nansum(weights * (vols - market)^2)``, ``weights`` with any scale folded in), the neighbours are built as scipy builds them (a copy of
+    x with one coordinate moved) and the divisor is dx = (x + h) - x, so ``fun`` / ``jac`` return bit for bit what SLSQP computes from a
+    one-set-at-a-time objective.  ``on_point(x)``, if given, sees the points in the order that objective would have been evaluated: x on
+    ``fun``, its neighbours on ``jac``.  ``batch_vols(points [B, n]) -> model vols [B, J]``; ``nb_batches`` counts its calls."""
+    batch_vols: Callable[[np.ndarray], np.ndarray]
+    market_vols: np.ndarray
+    weights: np.ndarray
+    bounds: Sequence[Tuple[float, float]]
+    eps: float = SLSQP_EPS
+    on_point: Optional[Callable[[np.ndarray], None]] = None
+    nb_batches: int = 0
+    nan_quotes: int = 0          # quotes without an implied vol at the LAST point priced by fun (dropped there by nansum, as in the reference)
+    _x: Optional[np.ndarray] = None
+    _f: float = np.nan
+    _g: Optional[np.ndarray] = None
+
+    def _values(self, pts: np.ndarray) -> np.ndarray:
+        vols = self.batch_vols(pts)
+        self.nb_batches += 1
+        return vols, [float(np.nansum(self.weights * np.square(v - self.market_vols))) for v in vols]
+
+    def _value(self, x: np.ndarray) -> None:
+        if self._x is not None and np.array_equal(x, self._x):
+            return
+        vols, f = self._values(x[None, :].copy())
+        self.nan_quotes = int(np.count_nonzero(np.isnan(vols[0])))
+        self._x, self._f, self._g = x.copy(), f[0], None
+
+    def fun(self, x: np.ndarray, *args) -> float:
+        x = np.asarray(x, dtype=float)
+        self._value(x)
+        if self.on_point is not None:
+            self.on_point(x)
+        return self._f
+
+    def jac(self, x: np.ndarray, *args) -> np.ndarray:
+        x = np.asarray(x, dtype=float)
+        if self._x is None or not np.array_equal(x, self._x):
+            self.fun(x)                                          # the one-set objective evaluates x before differencing at it
+        if self._g is None:
+            h = scipy_difference_steps(x, self.eps, self.bounds)
+            pts = np.repeat(x[None, :], x.size, axis=0)
+            for i in range(x.size):
+                pts[i, i] = x[i] + h[i]
+            if self.on_point is not None:
+                for p in pts:
+                    self.on_point(p)
+            _, f = self._values(pts)
+            self._g = np.array([(f[i] - self._f) / ((x[i] + h[i]) - x[i]) for i in range(x.size)])
+        return self._g.copy()
+
+
 def run_slsqp(objective: BatchedObjective, p0: np.ndarray, bounds, constraints=None, disp: bool = False):
     """``scipy.optimize.minimize(method='SLSQP', options={'ftol': 1e-8})`` as in the reference (:543-555), with the batched gradient."""
     from scipy.optimize import minimize      # host-side optimizer; scipy is already a dependency of the reference

@@ -7,7 +7,7 @@
 * ``HawkesJDPricer.price_chain``              (:125-155) -> ``hawkesjd_chain_pricer`` (:365-417) / ``hawkesjd_chain_pricer_with_risk_premia`` (:420-484),
   ``hawkesjd_forwards_under_risk_kernel`` (:487-515), ``compute_hawkes_a_mgf_grid`` / ``solve_a_ode_grid`` (:518-579)
 * ``HawkesJDPricer.calibrate_model_params_to_chain`` (:230-300), ``calibrate_risk_premia_gamma_to_chain`` (:303-357): host SLSQP loops around the
-  GPU chain pricer
+  batched GPU chain pricer (``b200sv_hawkesjd_price_chain_batch``), fits bit-identical to SLSQP differencing the one-set objective
 
 Monte Carlo: the reference draws every random input from numpy's process-global generator; here they are drawn in-kernel from the Philox
 stream keyed by an explicit ``seed`` (default: the ``set_seed`` stream or OS entropy).  ``simulate_hawkesjd_terminal`` additionally accepts the five
@@ -28,6 +28,7 @@ from ..data.option_chain import OptionChain
 from ..multi_gpu import _shared_seed, _use_distributed, mc_chain_distributed
 from ..utils.config import VariableType
 from ..utils.funcs import set_time_grid, timer
+from .calibration import SLSQP_EPS, ScipyDifferenceObjective
 from .model_pricer import ModelParams, ModelPricer
 
 _KEYS = tuple(k for k, _ in C.HawkesParamsC._fields_)
@@ -141,27 +142,16 @@ class HawkesJDPricer(ModelPricer):
                                               engine.mc_flags("fp64", gauss))
         return to_mc_chain_greeks(res[:5], engine.HAWKES_GREEK_PARAMS)
 
-    # ---- calibration drivers (reference :230-357): SLSQP on the host around the GPU Fourier chain pricer -----------------------------
-    def _vol_objective(self, option_chain: OptionChain, unpack, is_vega_weighted: bool, is_unit_ttm_vega: bool, scale: float = 1.0):
-        """weighted squared difference of model and mid implied vols (nansum: quotes whose model price leaves the no-arbitrage bounds drop out)"""
-        market = np.concatenate([np.asarray(v, dtype=float) for v in option_chain.get_mid_vols()])
-        if is_vega_weighted:
-            weights = np.concatenate([v / np.sum(v) for v in option_chain.get_chain_vegas(is_unit_ttm_vega=is_unit_ttm_vega)])
-        else:
-            weights = np.ones_like(market)
-
-        def objective(pars: np.ndarray, *_) -> float:
-            model = np.concatenate(self.compute_model_ivols_for_chain(option_chain=option_chain, params=unpack(pars)))
-            return float(np.nansum(scale * weights * np.square(model - market)))
-        return objective
-
+    # ---- calibration drivers (reference :230-357): SLSQP on the host around the batched GPU Fourier chain pricer ---------------------
     @timer
     def calibrate_model_params_to_chain(self, option_chain: OptionChain, params0: HawkesJDParams, is_vega_weighted: bool = True,
-                                        is_unit_ttm_vega: bool = False, **kwargs) -> HawkesJDParams:
+                                        is_unit_ttm_vega: bool = False, return_info: bool = False, **kwargs):
         """fit (sigma, mean_p, mean_m, theta_p, theta_m, kappa, beta_p, beta_m) to the chain's mid vols with shifts and initial intensities
         fixed at ``params0``'s; kappa is shared by the two intensities and beta_p / beta_m enter as +beta / -beta pairs (reference :230-300, same
         start vector -- including its beta_m start 0.5 (beta2_p - beta2_m) --, bounds, stationarity constraint and SLSQP options).
-        ``disp`` / ``maxiter`` (extras) are handed to SLSQP."""
+        ``disp`` / ``maxiter`` (extras) are handed to SLSQP.  The 8 difference neighbours of a point whose gradient SLSQP asks for are priced
+        in one ``hawkesjd_price_chain_batch`` call; objective and gradient are bit for bit what SLSQP differences from the one-set objective,
+        so the fit is too.  ``return_info``: (fit, {"fun", "nit", "nb_batches", "x", "nan_quotes"})."""
         from scipy.optimize import minimize
         p0 = np.array([params0.sigma, params0.mean_p, params0.mean_m, params0.theta_p, params0.theta_m, 0.5 * (params0.kappa_p + params0.kappa_m),
                        0.5 * (params0.beta1_p - params0.beta2_p), 0.5 * (params0.beta2_p - params0.beta2_m)])
@@ -176,29 +166,46 @@ class HawkesJDPricer(ModelPricer):
         options = {"disp": bool(kwargs.get("disp", False)), "ftol": 1e-8}
         if "maxiter" in kwargs:
             options["maxiter"] = int(kwargs["maxiter"])
-        res = minimize(self._vol_objective(option_chain, unpack, is_vega_weighted, is_unit_ttm_vega), p0, args=None, method="SLSQP",
-                       constraints=stationary, bounds=bounds, options=options)
-        return unpack(res.x)
+        objective = _batched_vol_objective(option_chain, unpack, is_vega_weighted, is_unit_ttm_vega, bounds, SLSQP_EPS)
+        res = minimize(objective.fun, p0, args=None, method="SLSQP", jac=objective.jac, constraints=stationary, bounds=bounds, options=options)
+        fit = unpack(res.x)
+        if return_info:
+            return fit, {"fun": float(res.fun), "nit": int(res.nit), "nb_batches": objective.nb_batches, "x": res.x,
+                         "nan_quotes": objective.nan_quotes}
+        return fit
 
     @timer
     def calibrate_risk_premia_gamma_to_chain(self, option_chain: OptionChain, params0: HawkesJDParams, is_vega_weighted: bool = True,
-                                             is_unit_ttm_vega: bool = False, maxiter: int = 100, print_iter: bool = True, **kwargs) -> HawkesJDParams:
+                                             is_unit_ttm_vega: bool = False, maxiter: int = 100, print_iter: bool = True, return_info: bool = False,
+                                             **kwargs):
         """fit (sigma, risk_premia_gamma) with every other parameter of ``params0`` fixed (reference :303-357: gamma scaled by 8 into (-1, 1),
-        weights x 1e4, SLSQP with finite-difference step 0.025, ftol = tol = 1e-16).  Returns a new object; the reference mutates ``params0``."""
+        weights x 1e4, SLSQP with finite-difference step 0.025, ftol = tol = 1e-16).  Returns a new object; the reference mutates ``params0``.
+        The 2 difference neighbours of a point whose gradient SLSQP asks for are priced in one risk-kernel ``hawkesjd_price_chain_batch``
+        call, with the fit of the one-set objective bit for bit; ``print_iter`` prints a line per point in the order that objective would (the neighbours
+        only when SLSQP asks for the gradient).  ``return_info``: (fit, {"fun", "nit", "nb_batches", "x", "nan_quotes"})."""
         from scipy.optimize import minimize
         gamma_scaler = 8.0
         fixed = {k: v for k, v in params0.to_dict().items() if k in _KEYS}
+        bounds = ((0.01, 1.5), (-1.0, 1.0))
 
-        def unpack(x: np.ndarray) -> HawkesJDParams:
-            if print_iter:
-                print(f"unpack_pars: sigma={x[0]}, gamma={gamma_scaler * x[1]}")
+        def announce(x: np.ndarray) -> None:
+            print(f"unpack_pars: sigma={x[0]}, gamma={gamma_scaler * x[1]}")
+
+        def to_params(x: np.ndarray) -> HawkesJDParams:
             return HawkesJDParams(**{**fixed, "sigma": float(x[0])}, risk_premia_gamma=float(gamma_scaler * x[1]))
 
         p0 = np.array([params0.sigma, (params0.risk_premia_gamma or 0.0) / gamma_scaler])
-        res = minimize(self._vol_objective(option_chain, unpack, is_vega_weighted, is_unit_ttm_vega, scale=10000.0), p0, args=None, method="SLSQP",
-                       bounds=((0.01, 1.5), (-1.0, 1.0)), options={"disp": bool(kwargs.get("disp", False)), "ftol": 1e-16, "maxiter": maxiter, "eps": 0.025},
-                       tol=1e-16)
-        return unpack(res.x)
+        objective = _batched_vol_objective(option_chain, to_params, is_vega_weighted, is_unit_ttm_vega, bounds, 0.025, scale=10000.0,
+                                           on_point=announce if print_iter else None)
+        res = minimize(objective.fun, p0, args=None, method="SLSQP", jac=objective.jac, bounds=bounds,
+                       options={"disp": bool(kwargs.get("disp", False)), "ftol": 1e-16, "maxiter": maxiter, "eps": 0.025}, tol=1e-16)
+        if print_iter:
+            announce(res.x)
+        fit = to_params(res.x)
+        if return_info:
+            return fit, {"fun": float(res.fun), "nit": int(res.nit), "nb_batches": objective.nb_batches, "x": res.x,
+                         "nan_quotes": objective.nan_quotes}
+        return fit
 
     @timer
     def simulate_terminal_values(self, params: HawkesJDParams, ttm: float = 1.0, nb_path: int = 100000, is_spot_measure: bool = True, **kwargs
@@ -282,6 +289,29 @@ def _fourier_chain(model_params: HawkesJDParams, ttms, forwards, discfactors, st
     d.pop("risk_premia_gamma", None)
     return engine.hawkesjd_price_chain(_params_c(**d), ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, is_spot_measure, vol_scaler,
                                        MAX_PHI, gamma, return_grids)
+
+
+def _batched_vol_objective(option_chain: OptionChain, to_params, is_vega_weighted: bool, is_unit_ttm_vega: bool, bounds, eps: float,
+                           scale: float = 1.0, on_point=None) -> ScipyDifferenceObjective:
+    """the drivers' objective: weighted squared difference of model and mid implied vols, nansum over the chain (quotes whose model price
+    leaves the no-arbitrage bounds drop out), with the weights of the reference (per-slice normalised vegas, times ``scale``).  The model vols
+    of a point, and of its difference neighbours together, come from hawkesjd_price_chain_batch, on the risk-kernel route when the
+    parameter sets carry a risk_premia_gamma -- the same prices and vols as compute_model_ivols_for_chain per set."""
+    market = np.concatenate([np.asarray(v, dtype=float) for v in option_chain.get_mid_vols()])
+    if is_vega_weighted:
+        weights = np.concatenate([v / np.sum(v) for v in option_chain.get_chain_vegas(is_unit_ttm_vega=is_unit_ttm_vega)])
+    else:
+        weights = np.ones_like(market)
+
+    def batch_vols(points: np.ndarray) -> np.ndarray:
+        sets = [to_params(p) for p in points]
+        gammas = None if sets[0].risk_premia_gamma is None else [s.risk_premia_gamma for s in sets]
+        _, ivols = engine.hawkesjd_price_chain_batch([_params_c(**s.to_dict()) for s in sets], option_chain.ttms, option_chain.forwards,
+                                                     option_chain.discfactors, option_chain.strikes_ttms, option_chain.optiontypes_ttms,
+                                                     max_phi=MAX_PHI, gammas=gammas)
+        return ivols
+    return ScipyDifferenceObjective(batch_vols=batch_vols, market_vols=market, weights=scale * weights, bounds=bounds, eps=eps,
+                                    on_point=on_point)
 
 
 def hawkesjd_chain_pricer(model_params: HawkesJDParams, ttms: np.ndarray, forwards: np.ndarray, discfactors: np.ndarray, strikes_ttms, optiontypes_ttms,
