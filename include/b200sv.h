@@ -419,6 +419,21 @@ int b200sv_heston_price_chain_greeks(const b200sv_heston_params* params, int M, 
                                      int variable_type, double vol_scaler, int P, double* prices_out, double* greeks_out,
                                      double* dlog_mgf_out);
 
+/* second-order forward-mode sensitivities of the two Fourier chain pricers (DESIGN.md §4.4), LOG_RETURN only (else -4).  The arguments
+ * and outputs of b200sv_*_price_chain_greeks (bit-identical to it), then vanna_out [n][J]: d^2 price / d forwards[m] d parameter, and
+ * hessian_out [n(n+1)/2][J]: d^2 price / d p d q for p <= q, the upper triangle row-major in struct field order ((0,0), (0,1), ..,
+ * (0,n-1), (1,1), ..).  Optional (may be NULL): d2log_mgf_out [n(n+1)/2][M][P] complex128 interleaved, the second parameter
+ * derivatives of the log-MGF grid in the same order.  Exact derivatives of the scheme on the first-order route's mesh. */
+int b200sv_logsv_price_chain_hessian(const b200sv_logsv_params* params, int M, const double* ttms, const double* forwards,
+                                     const double* discfactors, const double* etas, const int* offsets, const double* strikes,
+                                     const int8_t* types, int is_spot_measure, int variable_type, int expansion_order,
+                                     double vol_scaler, int P, double* prices_out, double* greeks_out, double* dlog_mgf_out,
+                                     int* nfev_out, double* vanna_out, double* hessian_out, double* d2log_mgf_out);
+int b200sv_heston_price_chain_hessian(const b200sv_heston_params* params, int M, const double* ttms, const double* forwards,
+                                      const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
+                                      int variable_type, double vol_scaler, int P, double* prices_out, double* greeks_out,
+                                      double* dlog_mgf_out, double* vanna_out, double* hessian_out, double* d2log_mgf_out);
+
 /* B parameter sets on ONE chain in one pass -- the objective of the calibration drivers and its finite-difference gradient:
  * _LogSvCalibrationObjective.__call__ (pricers/logsv_pricer.py:234-294: compute_model_ivols_for_chain = logsv_chain_pricer +
  * option_chain.compute_model_ivols_from_chain_data), which scipy SLSQP evaluates n+1 times per iteration, one parameter set at a time.

@@ -1360,6 +1360,390 @@ __global__ void __launch_bounds__(kFourierThreads) fourier_vanilla_greeks_kernel
 }
 
 // --------------------------------------------------------------------------------------------------------------------
+// Second-order forward-mode sensitivities of the Fourier chain pricers (DESIGN.md §4.4)
+// --------------------------------------------------------------------------------------------------------------------
+// row of the pair (p, q), p <= q < n, in the row-major upper triangle [n (n + 1) / 2]
+__host__ __device__ constexpr int tri_index(int p, int q, int n) { return p * n - p * (p - 1) / 2 + (q - p); }
+// the pair of row r of that triangle
+__device__ __forceinline__ void tri_pair(int r, int n, int& p, int& q) {
+  p = 0;
+  while (r >= n - p) r -= n - p++;
+  q = p + r;
+}
+
+constexpr int kLogsvOdePairs = kLogsvOdeDirs * (kLogsvOdeDirs + 1) / 2;     // 15 pairs over (theta, kappa1, kappa2, beta, volvol)
+constexpr int kHestonOdePairs = kHestonOdeDirs * (kHestonOdeDirs + 1) / 2;  // 10 pairs over (theta, kappa, rho, volvol)
+
+// d2(LogsvModel field) / d(direction p) d(direction q) for the kLogsvOdePairs pairs (tri_index order over the ODE directions); the fields
+// are polynomials of degree <= 3 in the parameters, kappa2 held fixed when kappa1 or theta moves as in make_model_tangents
+static void make_model_hessian(const b200sv_logsv_params& p, double eta, bool spot, LogsvModelTangent (&h)[kLogsvOdePairs]) {
+  for (auto& t : h) t = LogsvModelTangent{0, 0, 0, 0, 0, 0, 0, 0, 0};
+  const double v2 = p.beta * p.beta + p.volvol * p.volvol, th2 = p.theta * p.theta;
+  constexpr int D = kLogsvOdeDirs;
+  LogsvModelTangent& tt = h[tri_index(0, 0, D)];     // theta theta
+  tt.th2 = 2.0;
+  tt.qv2 = 2.0 * v2;
+  tt.lam = spot ? 0.0 : 2.0 * p.beta * eta;
+  h[tri_index(0, 2, D)].kp = 1.0;                    // theta kappa2
+  LogsvModelTangent& tb = h[tri_index(0, 3, D)];     // theta beta
+  tb.qv = 2.0 * p.beta;
+  tb.qv2 = 4.0 * p.theta * p.beta;
+  tb.lam = spot ? 0.0 : 2.0 * p.theta * eta;
+  tb.kp = spot ? 0.0 : -2.0 * eta;
+  LogsvModelTangent& tv = h[tri_index(0, 4, D)];     // theta volvol
+  tv.qv = 2.0 * p.volvol;
+  tv.qv2 = 4.0 * p.theta * p.volvol;
+  for (int d : {3, 4}) {                             // beta beta, volvol volvol
+    LogsvModelTangent& s = h[tri_index(d, d, D)];
+    s.v2 = 2.0;
+    s.qv = 2.0 * p.theta;
+    s.qv2 = 2.0 * th2;
+  }
+}
+
+// make_coef differentiated twice: linear in the fields except the products th2 b, theta b (b = beta_eta phi) and th2 eta2, theta eta2,
+// which take the second-order product rule
+__device__ __forceinline__ Coef make_d2coef(const LogsvModel& m, const LogsvModelTangent& dp, const LogsvModelTangent& dq,
+                                            const LogsvModelTangent& d2, cd phi, cd psi) {
+  Coef c;
+  const cd b = m.beta_eta * phi, bp = dp.beta_eta * phi, bq = dq.beta_eta * phi, b2 = d2.beta_eta * phi;
+  const cd dtb = ((d2.th2 * b + dp.th2 * bq) + dq.th2 * bp) + m.th2 * b2;          // d2(th2 b)
+  const cd d1b = ((d2.theta * b + dp.theta * bq) + dq.theta * bp) + m.theta * b2;  // d2(theta b)
+  c.l01 = mk(d2.lam) - dtb;
+  c.l11 = mk(-d2.kp) - 2.0 * d1b;
+  c.l12 = 2.0 * (mk(d2.lam + d2.qv) - dtb);
+  c.l21 = mk(-d2.k2p) - b2;
+  c.l22 = mk(d2.v2 - 2.0 * d2.kp) - 4.0 * d1b;
+  c.l23 = 3.0 * (mk(2.0 * d2.qv) - dtb);
+  c.l32 = -2.0 * (mk(d2.k2p) + b2);
+  c.l33 = 3.0 * (mk(d2.v2 - d2.kp) - 2.0 * d1b);
+  c.l34 = 4.0 * (mk(3.0 * d2.qv) - dtb);
+  c.l43 = -3.0 * (mk(d2.k2p) + b2);
+  c.l44 = 2.0 * (mk(d2.v2 - 2.0 * d2.kp) - 4.0 * d1b);
+  const cd r = m.spot ? phi * (phi + mk(1.0)) - 2.0 * psi : phi * (phi - mk(1.0)) - 2.0 * psi;
+  c.h0 = (0.5 * d2.th2 * m.eta2) * r;
+  c.h1 = (d2.theta * m.eta2) * r;
+  c.h2 = mk(0.0);
+  return c;
+}
+
+// the products X_i Y_j + Y_i X_j over the pairs q = {11, 12, 22, 13, 14, 23, 24, 33} of rhs_rows
+template <int N>
+__device__ __forceinline__ void sym_products(const cd (&X)[N], const cd (&Y)[N], cd (&out)[8]) {
+  constexpr int I[8] = {1, 1, 2, 1, 1, 2, 2, 3}, J[8] = {1, 2, 2, 3, 4, 3, 4, 3};
+#pragma unroll
+  for (int k = 0; k < 8; ++k) out[k] = (I[k] < N && J[k] < N) ? X[I[k]] * Y[J[k]] + Y[I[k]] * X[J[k]] : mk(0.0);
+}
+
+// The three right-hand sides of one parameter pair (p, q), f(A) = rows(q(A), A; F) with F = (v2, qv, qv2, Coef):
+//   d_p f   = rows(dq_p, dA_p; F) + rows(q, A; F_p, with H)                                  (rhs_tangent), the same for q
+//   d_pq f  = rows(d2q, d2A; F) + rows(dq_p, dA_p; F_q) + rows(dq_q, dA_q; F_p) + rows(q, A; F_pq, with H)
+// with dq_p = sym(A, dA_p) and d2q = sym(A, d2A) + sym(dA_p, dA_q): J(A) d2A + f_AA(dA_p, dA_q) + d_p J(A) dA_q + d_q J(A) dA_p + d_pq f(A).
+template <int N, int TPB>
+struct LogsvTan2RhsFn {
+  const LogsvModel* m;
+  const CoefView<TPB>* c;
+  LogsvModelTangent dmp, dmq, d2m;
+  CoefView<TPB> dcp, dcq, d2c;
+  __device__ __forceinline__ void operator()(const cd (&Y)[N], const cd (&dYp)[N], const cd (&dYq)[N], const cd (&d2Y)[N], cd (&op)[N],
+                                             cd (&oq)[N], cd (&opq)[N]) const {
+    rhs_tangent<N, TPB>(Y, dYp, *m, *c, dmp, dcp, op);
+    rhs_tangent<N, TPB>(Y, dYq, *m, *c, dmq, dcq, oq);
+    cd q[8], s[8], t[8], r[N];
+    sym_products<N>(Y, d2Y, q);
+    sym_products<N>(dYp, dYq, s);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) q[k] = q[k] + s[k];
+    rhs_rows<N, TPB, false>(q, d2Y, m->v2, m->qv, m->qv2, *c, opq);
+    sym_products<N>(Y, dYp, s);
+    rhs_rows<N, TPB, false>(s, dYp, dmq.v2, dmq.qv, dmq.qv2, dcq, r);
+#pragma unroll
+    for (int k = 0; k < N; ++k) opq[k] = opq[k] + r[k];
+    sym_products<N>(Y, dYq, s);
+    rhs_rows<N, TPB, false>(s, dYq, dmp.v2, dmp.qv, dmp.qv2, dcp, r);
+#pragma unroll
+    for (int k = 0; k < N; ++k) opq[k] = opq[k] + r[k];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) t[k] = mk(0.0);
+    t[0] = Y[1] * Y[1]; t[1] = Y[1] * Y[2]; t[2] = Y[2] * Y[2];
+    if constexpr (N == 5) {
+      t[3] = Y[1] * Y[3]; t[4] = Y[1] * Y[4]; t[5] = Y[2] * Y[3]; t[6] = Y[2] * Y[4]; t[7] = Y[3] * Y[3];
+    }
+    rhs_rows<N, TPB, true>(t, Y, d2m.v2, d2m.qv, d2m.qv2, d2c, r);
+#pragma unroll
+    for (int k = 0; k < N; ++k) opq[k] = opq[k] + r[k];
+  }
+};
+
+// Dormand-Prince stage combination of one tangent store: y + h sum_j a_sj K_j (stage s) ...
+template <int N, int TPB>
+__device__ __forceinline__ void tan_stage_input(StageStore<N, TPB> K, int s, const cd (&y)[N], double h, cd (&out)[N]) {
+#pragma unroll
+  for (int k = 0; k < N; ++k) {
+    cd acc = K.at(0, k) * c_A[s][0];
+#pragma unroll
+    for (int jj = 1; jj < 5; ++jj) acc = acc + K.at(jj, k) * c_A[s][jj];
+    out[k] = y[k] + acc * h;
+  }
+}
+// ... and the candidate y + h sum_j b_j K_j of the attempt, parked in stage 7
+template <int N, int TPB>
+__device__ __forceinline__ void tan_candidate(StageStore<N, TPB> K, const cd (&y)[N], double h, cd (&out)[N]) {
+  constexpr double B[6] = {35.0 / 384, 0, 500.0 / 1113, 125.0 / 192, -2187.0 / 6784, 11.0 / 84};
+#pragma unroll
+  for (int k = 0; k < N; ++k) {
+    cd acc = K.at(0, k) * B[0];
+#pragma unroll
+    for (int jj = 2; jj < 6; ++jj) acc = acc + K.at(jj, k) * B[jj];
+    out[k] = y[k] + h * acc;
+    K.at(7, k) = out[k];
+  }
+}
+
+// TangentHook one order higher: the tangents of directions p and q and the mixed second-order tangent of the pair, all stepped on
+// rk45_generic's attempts with the same bookkeeping (8 stages per store, 7 = the candidate; dy carried in registers over the maturities).
+// Tan2Rhs: ``void operator()(Y, dYp, dYq, d2Y, out_p, out_q, out_pq) const``.
+template <int N, int TPB, typename Tan2Rhs>
+struct Tangent2Hook {
+  Tan2Rhs f;
+  StageStore<N, TPB> dKp, dKq, d2K;
+  cd dyp[N], dyq[N], d2y[N];
+
+  __device__ __forceinline__ void eval(int s, const cd (&Y)[N], const cd (&dYp)[N], const cd (&dYq)[N], const cd (&d2Y)[N]) {
+    cd op[N], oq[N], opq[N];
+    f(Y, dYp, dYq, d2Y, op, oq, opq);
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+      dKp.at(s, k) = op[k];
+      dKq.at(s, k) = oq[k];
+      d2K.at(s, k) = opq[k];
+    }
+  }
+  __device__ __forceinline__ void start(const cd (&y)[N]) { eval(0, y, dyp, dyq, d2y); }
+  __device__ __forceinline__ void stage(int s, const cd (&yt)[N], double h) {
+    cd a[N], b[N], c[N];
+    tan_stage_input<N, TPB>(dKp, s, dyp, h, a);
+    tan_stage_input<N, TPB>(dKq, s, dyq, h, b);
+    tan_stage_input<N, TPB>(d2K, s, d2y, h, c);
+    eval(s, yt, a, b, c);
+  }
+  __device__ __forceinline__ void last(const cd (&yn)[N], double h) {
+    cd a[N], b[N], c[N];
+    tan_candidate<N, TPB>(dKp, dyp, h, a);
+    tan_candidate<N, TPB>(dKq, dyq, h, b);
+    tan_candidate<N, TPB>(d2K, d2y, h, c);
+    eval(6, yn, a, b, c);
+  }
+  __device__ __forceinline__ void accept() {
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+      dyp[k] = dKp.at(7, k);
+      dyq[k] = dKq.at(7, k);
+      d2y[k] = d2K.at(7, k);
+      dKp.at(0, k) = dKp.at(6, k);
+      dKq.at(0, k) = dKq.at(6, k);
+      d2K.at(0, k) = d2K.at(6, k);
+    }
+  }
+};
+
+constexpr int kHessianTPB = 8;   // shared memory per thread: 6N primal stages + 3 x 8N tangent stages + 4 x 14 coefficients
+
+// One thread = one (grid point, ODE pair p <= q): the primal integration of logsv_mgf_kernel (same rk45_generic, same mesh) plus the
+// tangents of p and q and their mixed second-order tangent.  The 15 pairs of a point are neighbouring threads.  lm = sum_k A_k y^k with
+// y = sigma0 - theta gives
+//   d2lm_pq = sum_k d2A_k y^k + (dA_p,k y_q + dA_q,k y_p) k y^(k-1) + A_k y_p y_q k (k-1) y^(k-2),   y_sigma0 = 1, y_theta = -1;
+// sigma0 has no ODE tangent, so the diagonal thread of direction p also writes the pair (sigma0, p) and pair 0 writes (sigma0, sigma0).
+// dspec [M][5], d2spec [M][15]: first and second field derivatives.  Output d2log_mgf [21][M][P] (tri_index over LOGSV_GREEK_PARAMS).
+template <int N>
+__global__ void __launch_bounds__(kHessianTPB) logsv_mgf_hessian_kernel(const cd* __restrict__ phi, int P, int M, const ChainSpec* __restrict__ spec,
+                                                                         const LogsvModelTangent* __restrict__ dspec,
+                                                                         const LogsvModelTangent* __restrict__ d2spec, double y,
+                                                                         cd* __restrict__ d2log_mgf) {
+  constexpr int TPB = kHessianTPB, D = kLogsvOdeDirs, NP = 1 + kLogsvOdeDirs;
+  __shared__ cd stage_smem[6 * N * TPB];
+  __shared__ cd tan_smem[3 * 8 * N * TPB];
+  __shared__ cd coef_smem[4 * 14 * TPB];
+  const int t = blockIdx.x * TPB + threadIdx.x;
+  if (t >= P * kLogsvOdePairs) return;
+  const int p = t / kLogsvOdePairs, pair = t % kLogsvOdePairs;
+  int dp, dq;
+  tri_pair(pair, D, dp, dq);
+#pragma unroll
+  for (int i = 0; i < 6 * N; ++i) stage_smem[threadIdx.x + i * TPB] = mk(0.0);
+#pragma unroll
+  for (int i = 0; i < 3 * 8 * N; ++i) tan_smem[threadIdx.x + i * TPB] = mk(0.0);
+  StageStore<N, TPB> K{stage_smem + threadIdx.x};
+  const CoefView<TPB> c{coef_smem + threadIdx.x};
+  Tangent2Hook<N, TPB, LogsvTan2RhsFn<N, TPB>> tan;
+  tan.f.c = &c;
+  tan.f.dcp = CoefView<TPB>{coef_smem + 14 * TPB + threadIdx.x};
+  tan.f.dcq = CoefView<TPB>{coef_smem + 28 * TPB + threadIdx.x};
+  tan.f.d2c = CoefView<TPB>{coef_smem + 42 * TPB + threadIdx.x};
+  tan.dKp = StageStore<N, TPB>{tan_smem + threadIdx.x};
+  tan.dKq = StageStore<N, TPB>{tan_smem + 8 * N * TPB + threadIdx.x};
+  tan.d2K = StageStore<N, TPB>{tan_smem + 16 * N * TPB + threadIdx.x};
+  cd A[N];
+#pragma unroll
+  for (int k = 0; k < N; ++k) {
+    A[k] = mk(0.0);
+    tan.dyp[k] = tan.dyq[k] = tan.d2y[k] = mk(0.0);
+  }
+  const cd ph = phi[p], ps = mk(0.0);
+  const double y2 = y * y;
+  const double ys[5] = {1.0, y, y2, y2 * y, y2 * y2};
+  const double dys[5] = {0.0, 1.0, 2.0 * y, 3.0 * y2, 4.0 * (y2 * y)};
+  const double d2ys[5] = {0.0, 0.0, 2.0, 6.0 * y, 12.0 * y2};
+  const double yp = dp == 0 ? -1.0 : 0.0, yq = dq == 0 ? -1.0 : 0.0;
+  for (int mm = 0; mm < M; ++mm) {
+    const LogsvModel model = spec[mm].model;
+    store_coef<TPB>(coef_smem + threadIdx.x, make_coef(model, ph, ps));
+    tan.f.m = &model;
+    tan.f.dmp = dspec[mm * D + dp];
+    tan.f.dmq = dspec[mm * D + dq];
+    tan.f.d2m = d2spec[mm * kLogsvOdePairs + pair];
+    store_coef<TPB>(coef_smem + 14 * TPB + threadIdx.x, make_dcoef(model, tan.f.dmp, ph, ps));
+    store_coef<TPB>(coef_smem + 28 * TPB + threadIdx.x, make_dcoef(model, tan.f.dmq, ph, ps));
+    store_coef<TPB>(coef_smem + 42 * TPB + threadIdx.x, make_d2coef(model, tan.f.dmp, tan.f.dmq, tan.f.d2m, ph, ps));
+    rk45_generic<N, TPB>(A, spec[mm].dtau, LogsvRhsFn<N, TPB>{model, c}, K, nullptr, &tan);
+    cd h = mk(0.0), hs = mk(0.0), hss = mk(0.0);
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+      h = h + (tan.d2y[k] * ys[k] + (tan.dyp[k] * yq + tan.dyq[k] * yp) * dys[k] + A[k] * (yp * yq * d2ys[k]));
+      hs = hs + (tan.dyp[k] * dys[k] + A[k] * (yp * d2ys[k]));      // (sigma0, p): y_sigma0 = 1, no ODE tangent
+      hss = hss + A[k] * d2ys[k];                                      // (sigma0, sigma0)
+    }
+    d2log_mgf[((size_t)tri_index(1 + dp, 1 + dq, NP) * M + mm) * P + p] = h;
+    if (dp == dq) d2log_mgf[((size_t)tri_index(0, 1 + dp, NP) * M + mm) * P + p] = hs;
+    if (pair == 0) d2log_mgf[(size_t)mm * P + p] = hss;
+  }
+}
+
+// hyper-dual complex numbers (value, derivative in p, derivative in q, mixed second derivative) for the Heston closed form, through the
+// same principal csqrt / cexp / clog and Smith division as dcd
+struct hcd {
+  cd v, d1, d2, d12;
+};
+__device__ __forceinline__ hcd hmk(cd v) { return hcd{v, mk(0.0), mk(0.0), mk(0.0)}; }
+__device__ __forceinline__ hcd operator+(hcd a, hcd b) { return hcd{a.v + b.v, a.d1 + b.d1, a.d2 + b.d2, a.d12 + b.d12}; }
+__device__ __forceinline__ hcd operator-(hcd a, hcd b) { return hcd{a.v - b.v, a.d1 - b.d1, a.d2 - b.d2, a.d12 - b.d12}; }
+__device__ __forceinline__ hcd operator-(hcd a) { return hcd{-a.v, -a.d1, -a.d2, -a.d12}; }
+__device__ __forceinline__ hcd operator*(double s, hcd a) { return hcd{s * a.v, s * a.d1, s * a.d2, s * a.d12}; }
+__device__ __forceinline__ hcd operator*(hcd a, hcd b) {
+  return hcd{a.v * b.v, a.d1 * b.v + a.v * b.d1, a.d2 * b.v + a.v * b.d2, ((a.d12 * b.v + a.d1 * b.d2) + a.d2 * b.d1) + a.v * b.d12};
+}
+__device__ __forceinline__ hcd operator/(hcd a, hcd b) {   // q = a / b from a = q b differentiated
+  const cd q = a.v / b.v, q1 = (a.d1 - q * b.d1) / b.v, q2 = (a.d2 - q * b.d2) / b.v;
+  return hcd{q, q1, q2, (((a.d12 - q1 * b.d2) - q2 * b.d1) - q * b.d12) / b.v};
+}
+__device__ __forceinline__ hcd hsqrt(hcd z) {              // s^2 = z differentiated
+  const cd s = csqrt_(z.v), s1 = z.d1 / (2.0 * s), s2 = z.d2 / (2.0 * s);
+  return hcd{s, s1, s2, (z.d12 - 2.0 * (s1 * s2)) / (2.0 * s)};
+}
+__device__ __forceinline__ hcd hexp(hcd z) {
+  const cd e = cexp_(z.v);
+  return hcd{e, e * z.d1, e * z.d2, e * (z.d12 + z.d1 * z.d2)};
+}
+__device__ __forceinline__ hcd hlog(hcd z) {
+  const cd l1 = z.d1 / z.v, l2 = z.d2 / z.v;
+  return hcd{clog_(z.v), l1, l2, (z.d12 - l1 * z.d2) / z.v};
+}
+
+// heston_mgf_kernel in second-order forward mode: one thread = one (grid point, pair p <= q of theta | kappa | rho | volvol), (a, b) as
+// hyper-dual numbers carried over the maturities.  log_mgf = a + b v0, so d2/dv0^2 = 0 and d2/dv0 dq = db/dq: the diagonal thread of q
+// writes the latter, pair 0 the former.  d2log_mgf [15][M][P] (tri_index over HESTON_GREEK_PARAMS).
+__global__ void heston_mgf_hessian_kernel(const cd* __restrict__ phi, int P, int M, const double* __restrict__ dtaus, b200sv_heston_params hp,
+                                          cd* __restrict__ d2log_mgf) {
+  constexpr int D = kHestonOdeDirs, NP = 1 + kHestonOdeDirs;
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= P * kHestonOdePairs) return;
+  const int p = t / kHestonOdePairs, pair = t % kHestonOdePairs;
+  int dp, dq;
+  tri_pair(pair, D, dp, dq);
+  const double x[D] = {hp.theta, hp.kappa, hp.rho, hp.volvol};
+  hcd par[D];
+#pragma unroll
+  for (int k = 0; k < D; ++k) par[k] = hcd{mk(x[k]), mk(k == dp ? 1.0 : 0.0), mk(k == dq ? 1.0 : 0.0), mk(0.0)};
+  const hcd th = par[0], ka = par[1], rho = par[2], vv = par[3];
+  const hcd ph = hmk(phi[p]);
+  const hcd vv2 = vv * vv;
+  const hcd b1 = ka + (rho * vv) * ph;
+  const hcd b0 = hmk((0.5 * ph.v) * (ph.v + mk(1.0)));
+  const hcd zeta = hsqrt(b1 * b1 - (2.0 * b0) * vv2);
+  const hcd psi_p = zeta - b1, psi_m = b1 + zeta;
+  const hcd two_zeta = 2.0 * zeta;
+  hcd a = hmk(mk(0.0)), b = hmk(mk(0.0));
+  for (int mm = 0; mm < M; ++mm) {
+    const double tau = dtaus[mm];
+    const hcd ez = hexp(-(tau * zeta));
+    const hcd c_p = (psi_p + vv2 * b) / two_zeta, c_m = (psi_m - vv2 * b) / two_zeta;
+    const hcd den = c_p * ez + c_m;
+    const hcd b_new = -((-(psi_m * c_p)) * ez + psi_p * c_m) / (vv2 * den);
+    const hcd a_new = (-((th * ka) / vv2)) * (tau * psi_p + 2.0 * hlog(den)) + a;
+    a = a_new;
+    b = b_new;
+    d2log_mgf[((size_t)tri_index(1 + dp, 1 + dq, NP) * M + mm) * P + p] = a.d12 + b.d12 * hp.v0;
+    if (dp == dq) d2log_mgf[((size_t)tri_index(0, 1 + dp, NP) * M + mm) * P + p] = b.d1;
+    if (pair == 0) d2log_mgf[(size_t)mm * P + p] = mk(0.0);
+  }
+}
+
+// The second-order Fourier sums next to fourier_vanilla_greeks_kernel's, one CTA per strike, fixed-order block_sum:
+//   S_p = sum w Re(e^z dlm_p),  S_xp = sum w Re(-phi e^z dlm_p),  S_pq = sum w Re(e^z (d2lm_pq + dlm_p dlm_q)),
+// z = lm - x phi, the same NaN-skipping.  Spot: vanna_p = -df K S_xp / F, hessian_pq = -df K S_pq;
+// inverse: vanna_p = -df (S_p + S_xp), hessian_pq = -F df S_pq.  vanna [NP][J], hessian [NP (NP + 1) / 2][J] (tri_index rows).
+template <int NP>
+__global__ void __launch_bounds__(kFourierThreads) fourier_vanilla_hessian_kernel(const cd* __restrict__ log_mgf, const cd* __restrict__ dlog_mgf,
+                                                                                 const cd* __restrict__ d2log_mgf, const cd* __restrict__ phi,
+                                                                                 int P, int M, const StrikeSpec* __restrict__ specs,
+                                                                                 int is_spot, double* __restrict__ vanna,
+                                                                                 double* __restrict__ hessian) {
+  constexpr int NH = NP * (NP + 1) / 2, NV = 2 * NP + NH;
+  __shared__ double red[NV * (kFourierThreads / 32)];
+  const StrikeSpec sp = specs[blockIdx.x];
+  const cd* lm = log_mgf + (size_t)sp.slice * P;
+  const double x = log(sp.forward / sp.strike);
+  const double h3 = (phi[1].im - phi[0].im) / 3.0;
+  double acc[NV];
+#pragma unroll
+  for (int i = 0; i < NV; ++i) acc[i] = 0.0;
+  for (int j = threadIdx.x; j < P; j += kFourierThreads) {
+    const double wq = (j & 1) ? 4.0 : ((j == 0 || j == P - 1) ? 1.0 : 2.0);
+    const double dp = h3 * wq;
+    const cd ph = phi[j];
+    const double w = (dp / M_PI) / (ph.im * ph.im + 0.25);
+    const cd e = cexp_(lm[j] - x * ph);
+    const cd term = mk(w) * e;
+    if (term.re == term.re) {
+      cd dl[NP];
+#pragma unroll
+      for (int k = 0; k < NP; ++k) {
+        dl[k] = dlog_mgf[((size_t)k * M + sp.slice) * P + j];
+        const cd ed = e * dl[k];
+        acc[k] += w * ed.re;
+        acc[NP + k] += w * (-(ph * ed)).re;
+      }
+      int r = 0;
+#pragma unroll
+      for (int p = 0; p < NP; ++p)
+#pragma unroll
+        for (int q = p; q < NP; ++q, ++r) acc[2 * NP + r] += w * (e * (d2log_mgf[((size_t)r * M + sp.slice) * P + j] + dl[p] * dl[q])).re;
+    }
+  }
+  block_sum<NV, kFourierThreads>(acc, red);
+  if (threadIdx.x == 0) {
+    const double F = sp.forward, K = sp.strike, df = sp.discfactor;
+    const int J = gridDim.x;
+#pragma unroll
+    for (int k = 0; k < NP; ++k)
+      vanna[(size_t)k * J + blockIdx.x] = is_spot ? -df * K * acc[NP + k] / F : -df * (acc[k] + acc[NP + k]);
+    const double scale = is_spot ? -df * K : -F * df;
+#pragma unroll
+    for (int r = 0; r < NH; ++r) hessian[(size_t)r * J + blockIdx.x] = scale * acc[2 * NP + r];
+  }
+}
+
+// --------------------------------------------------------------------------------------------------------------------
 // host side
 // --------------------------------------------------------------------------------------------------------------------
 // Latency regime (few grid points in total): lane-parallel kernel; throughput regime (batches, the 40000-point psi grid): one thread per
@@ -2296,6 +2680,80 @@ static int fourier_sum_host(const double* log_mgf, const double* grid, int P, co
   });
 }
 
+// The first-order sensitivity launches of a prepared LogSV chain (b200sv_logsv_price_chain_greeks and _hessian): the pricing launches,
+// logsv_mgf_tangent_kernel and, on a non-empty chain, fourier_vanilla_greeks_kernel.  dspec, the tangent kernel's primal log-MGF (lm), its
+// tangents (dlm), nfev and the greeks stay on the device for the launches that follow; download() queues the copies and synchronises.
+struct LogsvGreeksDev {
+  DevBuf dspec, dlm, lm, nfev, g;
+  explicit LogsvGreeksDev(cudaStream_t s) : dspec(s), dlm(s), lm(s), nfev(s), g(s) {}
+
+  int download(ChainDev& d, const FourierChain& c, double* greeks_out, double* dlog_mgf_out, int* nfev_out) {
+    constexpr int NP = 1 + kLogsvOdeDirs;
+    if (c.Jtot > 0) B200SV_CUDA(g.download(greeks_out, (size_t)(2 + NP) * c.Jtot));
+    B200SV_CUDA(dlm.download(cplx(dlog_mgf_out), (size_t)NP * c.M * c.P));
+    B200SV_CUDA(nfev.download(nfev_out, c.P));
+    return d.sync.done();
+  }
+};
+
+static int queue_logsv_greeks(ChainDev& d, LogsvGreeksDev& t, const FourierChain& c, const b200sv_logsv_params* params, const double* etas,
+                              int expansion_order, double* prices_out) {
+  const int N = expansion_order == B200SV_ORDER_FIRST ? 3 : 5, NP = 1 + kLogsvOdeDirs, M = c.M, P = c.P;
+  std::vector<LogsvModelTangent> dspec((size_t)M * kLogsvOdeDirs);
+  for (int m = 0; m < M; ++m) {
+    LogsvModelTangent tg[kLogsvOdeDirs];
+    make_model_tangents(*params, etas ? etas[m] : 1.0, c.spot, tg);
+    std::copy(tg, tg + kLogsvOdeDirs, dspec.begin() + (size_t)m * kLogsvOdeDirs);
+  }
+  if (int rc = queue_logsv_prices(d, c, params, etas, N, prices_out, nullptr)) return rc;
+  B200SV_CUDA(t.dspec.upload(dspec.data(), dspec.size()));
+  B200SV_CUDA(t.dlm.alloc(sizeof(cd) * (size_t)NP * M * P));
+  B200SV_CUDA(t.lm.alloc(sizeof(cd) * (size_t)M * P));
+  B200SV_CUDA(t.nfev.alloc(sizeof(int) * P));
+  B200SV_CUDA(t.g.alloc(sizeof(double) * (size_t)(2 + NP) * c.ss.size()));
+  const auto tangent = N == 5 ? logsv_mgf_tangent_kernel<5> : logsv_mgf_tangent_kernel<3>;
+  tangent<<<(P * kLogsvOdeDirs + kTangentTPB - 1) / kTangentTPB, kTangentTPB, 0, d.st>>>(d.phi.as<cd>(), P, M, d.spec.as<ChainSpec>(),
+                                                                                       t.dspec.as<LogsvModelTangent>(),
+                                                                                       params->sigma0 - params->theta, t.dlm.as<cd>(),
+                                                                                       t.lm.as<cd>(), nullptr, t.nfev.as<int>());
+  if (int rc = check_launch("logsv_mgf_tangent_kernel")) return rc;
+  if (c.Jtot > 0) {       // the tangent kernel's own primal log-MGF (DESIGN.md §4.2)
+    fourier_vanilla_greeks_kernel<1 + kLogsvOdeDirs><<<c.Jtot, kFourierThreads, 0, d.st>>>(t.lm.as<cd>(), t.dlm.as<cd>(), d.phi.as<cd>(), P, M,
+                                                                                         d.rows.as<StrikeSpec>(), c.spot ? 1 : 0,
+                                                                                         t.g.as<double>());
+    if (int rc = check_launch("fourier_vanilla_greeks_kernel")) return rc;
+  }
+  return 0;
+}
+
+// The Heston twin: the pricing launches, heston_mgf_tangent_kernel and fourier_vanilla_greeks_kernel; dlm and the greeks stay on the device.
+struct HestonGreeksDev {
+  DevBuf dlm, g;
+  explicit HestonGreeksDev(cudaStream_t s) : dlm(s), g(s) {}
+
+  int download(ChainDev& d, const FourierChain& c, double* greeks_out, double* dlog_mgf_out) {
+    constexpr int NP = 1 + kHestonOdeDirs;
+    if (c.Jtot > 0) B200SV_CUDA(g.download(greeks_out, (size_t)(2 + NP) * c.Jtot));
+    B200SV_CUDA(dlm.download(cplx(dlog_mgf_out), (size_t)NP * c.M * c.P));
+    return d.sync.done();
+  }
+};
+
+static int queue_heston_greeks(ChainDev& d, HestonGreeksDev& t, const FourierChain& c, const b200sv_heston_params* params, double* prices_out) {
+  const int NP = 1 + kHestonOdeDirs, M = c.M, P = c.P;
+  if (int rc = queue_heston_prices(d, c, params, prices_out, nullptr)) return rc;
+  B200SV_CUDA(t.dlm.alloc(sizeof(cd) * (size_t)NP * M * P));
+  B200SV_CUDA(t.g.alloc(sizeof(double) * (size_t)(2 + NP) * c.ss.size()));
+  heston_mgf_tangent_kernel<<<(P * kHestonOdeDirs + 63) / 64, 64, 0, d.st>>>(d.phi.as<cd>(), P, M, d.dt.as<double>(), *params, t.dlm.as<cd>());
+  if (int rc = check_launch("heston_mgf_tangent_kernel")) return rc;
+  if (c.Jtot > 0) {       // the pricing launch's log-MGF: heston_mgf_kernel is a per-thread closed form, the same for any block size
+    fourier_vanilla_greeks_kernel<1 + kHestonOdeDirs><<<c.Jtot, kFourierThreads, 0, d.st>>>(d.lm.as<cd>(), t.dlm.as<cd>(), d.phi.as<cd>(), P, M,
+                                                                                          d.rows.as<StrikeSpec>(), 1, t.g.as<double>());
+    if (int rc = check_launch("fourier_vanilla_greeks_kernel")) return rc;
+  }
+  return 0;
+}
+
 static int check_expansion_order(int expansion_order) {
   if (expansion_order != B200SV_ORDER_FIRST && expansion_order != B200SV_ORDER_SECOND) return fail(-4, "expansion_order not implemented");
   return 0;
@@ -2350,38 +2808,10 @@ int b200sv_logsv_price_chain_greeks(const b200sv_logsv_params* params, int M, co
   if (int rc = prepare_logsv_chain(c, params, M, ttms, forwards, discfactors, offsets, strikes, types, is_spot_measure, variable_type,
                                    expansion_order, vol_scaler, P))
     return rc;
-  const int N = expansion_order == B200SV_ORDER_FIRST ? 3 : 5, NP = 1 + kLogsvOdeDirs;
-  P = c.P;
-  std::vector<LogsvModelTangent> dspec((size_t)M * kLogsvOdeDirs);
-  for (int m = 0; m < M; ++m) {
-    LogsvModelTangent t[kLogsvOdeDirs];
-    make_model_tangents(*params, etas ? etas[m] : 1.0, c.spot, t);
-    std::copy(t, t + kLogsvOdeDirs, dspec.begin() + (size_t)m * kLogsvOdeDirs);
-  }
   ChainDev d;
-  if (int rc = queue_logsv_prices(d, c, params, etas, N, prices_out, nullptr)) return rc;
-  DevBuf d_dspec(d.st), d_dlm(d.st), d_lm(d.st), d_nfev(d.st), d_g(d.st);
-  B200SV_CUDA(d_dspec.upload(dspec.data(), dspec.size()));
-  B200SV_CUDA(d_dlm.alloc(sizeof(cd) * (size_t)NP * M * P));
-  B200SV_CUDA(d_lm.alloc(sizeof(cd) * (size_t)M * P));
-  B200SV_CUDA(d_nfev.alloc(sizeof(int) * P));
-  B200SV_CUDA(d_g.alloc(sizeof(double) * (size_t)(2 + NP) * c.ss.size()));
-  const auto tangent = N == 5 ? logsv_mgf_tangent_kernel<5> : logsv_mgf_tangent_kernel<3>;
-  tangent<<<(P * kLogsvOdeDirs + kTangentTPB - 1) / kTangentTPB, kTangentTPB, 0, d.st>>>(d.phi.as<cd>(), P, M, d.spec.as<ChainSpec>(),
-                                                                                       d_dspec.as<LogsvModelTangent>(),
-                                                                                       params->sigma0 - params->theta, d_dlm.as<cd>(),
-                                                                                       d_lm.as<cd>(), nullptr, d_nfev.as<int>());
-  if (int rc = check_launch("logsv_mgf_tangent_kernel")) return rc;
-  if (c.Jtot > 0) {       // the tangent kernel's own primal log-MGF (DESIGN.md §4.2)
-    fourier_vanilla_greeks_kernel<1 + kLogsvOdeDirs><<<c.Jtot, kFourierThreads, 0, d.st>>>(d_lm.as<cd>(), d_dlm.as<cd>(), d.phi.as<cd>(), P, M,
-                                                                                         d.rows.as<StrikeSpec>(), c.spot ? 1 : 0,
-                                                                                         d_g.as<double>());
-    if (int rc = check_launch("fourier_vanilla_greeks_kernel")) return rc;
-    B200SV_CUDA(d_g.download(greeks_out, (size_t)(2 + NP) * c.Jtot));
-  }
-  B200SV_CUDA(d_dlm.download(cplx(dlog_mgf_out), (size_t)NP * M * P));
-  B200SV_CUDA(d_nfev.download(nfev_out, P));
-  return d.sync.done();
+  LogsvGreeksDev g(d.st);
+  if (int rc = queue_logsv_greeks(d, g, c, params, etas, expansion_order, prices_out)) return rc;
+  return g.download(d, c, greeks_out, dlog_mgf_out, nfev_out);
 }
 
 int b200sv_heston_price_chain_greeks(const b200sv_heston_params* params, int M, const double* ttms, const double* forwards,
@@ -2392,23 +2822,88 @@ int b200sv_heston_price_chain_greeks(const b200sv_heston_params* params, int M, 
   if (variable_type != B200SV_LOG_RETURN) return fail(-4, "variable_type not implemented: sensitivities cover LOG_RETURN only");
   FourierChain c;
   if (int rc = prepare_heston_chain(c, params, M, ttms, forwards, discfactors, offsets, strikes, types, variable_type, vol_scaler, P)) return rc;
-  const int NP = 1 + kHestonOdeDirs;
-  P = c.P;
   ChainDev d;
-  if (int rc = queue_heston_prices(d, c, params, prices_out, nullptr)) return rc;
-  DevBuf d_dlm(d.st), d_g(d.st);
-  B200SV_CUDA(d_dlm.alloc(sizeof(cd) * (size_t)NP * M * P));
-  B200SV_CUDA(d_g.alloc(sizeof(double) * (size_t)(2 + NP) * c.ss.size()));
-  heston_mgf_tangent_kernel<<<(P * kHestonOdeDirs + 63) / 64, 64, 0, d.st>>>(d.phi.as<cd>(), P, M, d.dt.as<double>(), *params, d_dlm.as<cd>());
-  if (int rc = check_launch("heston_mgf_tangent_kernel")) return rc;
-  if (c.Jtot > 0) {       // the pricing launch's log-MGF: heston_mgf_kernel is a per-thread closed form, the same for any block size
-    fourier_vanilla_greeks_kernel<1 + kHestonOdeDirs><<<c.Jtot, kFourierThreads, 0, d.st>>>(d.lm.as<cd>(), d_dlm.as<cd>(), d.phi.as<cd>(), P, M,
-                                                                                          d.rows.as<StrikeSpec>(), 1, d_g.as<double>());
-    if (int rc = check_launch("fourier_vanilla_greeks_kernel")) return rc;
-    B200SV_CUDA(d_g.download(greeks_out, (size_t)(2 + NP) * c.Jtot));
+  HestonGreeksDev g(d.st);
+  if (int rc = queue_heston_greeks(d, g, c, params, prices_out)) return rc;
+  return g.download(d, c, greeks_out, dlog_mgf_out);
+}
+
+/* ---- second-order forward-mode sensitivities of the two Fourier chain pricers (DESIGN.md §4.4) ----
+ * The launches of b200sv_*_price_chain_greeks unchanged (bit-identical first-order outputs), then the Hessian kernel and
+ * fourier_vanilla_hessian_kernel; one synchronisation at the end. */
+int b200sv_logsv_price_chain_hessian(const b200sv_logsv_params* params, int M, const double* ttms, const double* forwards,
+                                     const double* discfactors, const double* etas, const int* offsets, const double* strikes,
+                                     const int8_t* types, int is_spot_measure, int variable_type, int expansion_order,
+                                     double vol_scaler, int P, double* prices_out, double* greeks_out, double* dlog_mgf_out,
+                                     int* nfev_out, double* vanna_out, double* hessian_out, double* d2log_mgf_out) {
+  B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && greeks_out && vanna_out && hessian_out, "null pointer");
+  if (variable_type != B200SV_LOG_RETURN) return fail(-4, "variable_type not implemented: sensitivities cover LOG_RETURN only");
+  FourierChain c;
+  if (int rc = prepare_logsv_chain(c, params, M, ttms, forwards, discfactors, offsets, strikes, types, is_spot_measure, variable_type,
+                                   expansion_order, vol_scaler, P))
+    return rc;
+  ChainDev d;
+  LogsvGreeksDev g(d.st);
+  if (int rc = queue_logsv_greeks(d, g, c, params, etas, expansion_order, prices_out)) return rc;
+  const int N = expansion_order == B200SV_ORDER_FIRST ? 3 : 5, NP = 1 + kLogsvOdeDirs, NH = NP * (NP + 1) / 2;
+  P = c.P;
+  std::vector<LogsvModelTangent> d2spec((size_t)M * kLogsvOdePairs);
+  for (int m = 0; m < M; ++m) {
+    LogsvModelTangent h[kLogsvOdePairs];
+    make_model_hessian(*params, etas ? etas[m] : 1.0, c.spot, h);
+    std::copy(h, h + kLogsvOdePairs, d2spec.begin() + (size_t)m * kLogsvOdePairs);
   }
-  B200SV_CUDA(d_dlm.download(cplx(dlog_mgf_out), (size_t)NP * M * P));
-  return d.sync.done();
+  DevBuf d_d2spec(d.st), d_d2lm(d.st), d_v(d.st), d_h(d.st);
+  B200SV_CUDA(d_d2spec.upload(d2spec.data(), d2spec.size()));
+  B200SV_CUDA(d_d2lm.alloc(sizeof(cd) * (size_t)NH * M * P));
+  B200SV_CUDA(d_v.alloc(sizeof(double) * (size_t)NP * c.ss.size()));
+  B200SV_CUDA(d_h.alloc(sizeof(double) * (size_t)NH * c.ss.size()));
+  const auto hessian = N == 5 ? logsv_mgf_hessian_kernel<5> : logsv_mgf_hessian_kernel<3>;
+  hessian<<<(P * kLogsvOdePairs + kHessianTPB - 1) / kHessianTPB, kHessianTPB, 0, d.st>>>(d.phi.as<cd>(), P, M, d.spec.as<ChainSpec>(),
+                                                                                        g.dspec.as<LogsvModelTangent>(),
+                                                                                        d_d2spec.as<LogsvModelTangent>(),
+                                                                                        params->sigma0 - params->theta, d_d2lm.as<cd>());
+  if (int rc = check_launch("logsv_mgf_hessian_kernel")) return rc;
+  if (c.Jtot > 0) {       // the tangent kernel's primal log-MGF and tangents, as for the first-order rows
+    fourier_vanilla_hessian_kernel<NP><<<c.Jtot, kFourierThreads, 0, d.st>>>(g.lm.as<cd>(), g.dlm.as<cd>(), d_d2lm.as<cd>(), d.phi.as<cd>(), P,
+                                                                             M, d.rows.as<StrikeSpec>(), c.spot ? 1 : 0, d_v.as<double>(),
+                                                                             d_h.as<double>());
+    if (int rc = check_launch("fourier_vanilla_hessian_kernel")) return rc;
+    B200SV_CUDA(d_v.download(vanna_out, (size_t)NP * c.Jtot));
+    B200SV_CUDA(d_h.download(hessian_out, (size_t)NH * c.Jtot));
+  }
+  B200SV_CUDA(d_d2lm.download(cplx(d2log_mgf_out), (size_t)NH * M * P));
+  return g.download(d, c, greeks_out, dlog_mgf_out, nfev_out);
+}
+
+int b200sv_heston_price_chain_hessian(const b200sv_heston_params* params, int M, const double* ttms, const double* forwards,
+                                      const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
+                                      int variable_type, double vol_scaler, int P, double* prices_out, double* greeks_out,
+                                      double* dlog_mgf_out, double* vanna_out, double* hessian_out, double* d2log_mgf_out) {
+  B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && greeks_out && vanna_out && hessian_out, "null pointer");
+  if (variable_type != B200SV_LOG_RETURN) return fail(-4, "variable_type not implemented: sensitivities cover LOG_RETURN only");
+  FourierChain c;
+  if (int rc = prepare_heston_chain(c, params, M, ttms, forwards, discfactors, offsets, strikes, types, variable_type, vol_scaler, P)) return rc;
+  ChainDev d;
+  HestonGreeksDev g(d.st);
+  if (int rc = queue_heston_greeks(d, g, c, params, prices_out)) return rc;
+  const int NP = 1 + kHestonOdeDirs, NH = NP * (NP + 1) / 2;
+  P = c.P;
+  DevBuf d_d2lm(d.st), d_v(d.st), d_h(d.st);
+  B200SV_CUDA(d_d2lm.alloc(sizeof(cd) * (size_t)NH * M * P));
+  B200SV_CUDA(d_v.alloc(sizeof(double) * (size_t)NP * c.ss.size()));
+  B200SV_CUDA(d_h.alloc(sizeof(double) * (size_t)NH * c.ss.size()));
+  heston_mgf_hessian_kernel<<<(P * kHestonOdePairs + 63) / 64, 64, 0, d.st>>>(d.phi.as<cd>(), P, M, d.dt.as<double>(), *params, d_d2lm.as<cd>());
+  if (int rc = check_launch("heston_mgf_hessian_kernel")) return rc;
+  if (c.Jtot > 0) {
+    fourier_vanilla_hessian_kernel<NP><<<c.Jtot, kFourierThreads, 0, d.st>>>(d.lm.as<cd>(), g.dlm.as<cd>(), d_d2lm.as<cd>(), d.phi.as<cd>(), P,
+                                                                             M, d.rows.as<StrikeSpec>(), 1, d_v.as<double>(), d_h.as<double>());
+    if (int rc = check_launch("fourier_vanilla_hessian_kernel")) return rc;
+    B200SV_CUDA(d_v.download(vanna_out, (size_t)NP * c.Jtot));
+    B200SV_CUDA(d_h.download(hessian_out, (size_t)NH * c.Jtot));
+  }
+  B200SV_CUDA(d_d2lm.download(cplx(d2log_mgf_out), (size_t)NH * M * P));
+  return g.download(d, c, greeks_out, dlog_mgf_out);
 }
 
 /* ---- batched chain pricers: B parameter sets on one chain in one pass (calibration objective + its finite-difference gradient) ----

@@ -587,6 +587,44 @@ def heston_price_chain_greeks(params: C.HestonParamsC, ttms, forwards, discfacto
                                True, (C.LOG_RETURN,), vol_scaler, int(max_phi or 1000), return_grids, HESTON_GREEK_PARAMS, False)
 
 
+def _price_chain_hessian(symbol: str, params, chain, etas, is_spot_measure: bool, head, vol_scaler, max_phi: int, return_grids: bool, names,
+                         with_nfev: bool):
+    """the second-order Fourier entry points: the arguments of _price_chain_greeks, then vanna [P, J], hessian [P(P+1)/2, J],
+    d2log_mgf [P(P+1)/2, M, max_phi] -> (prices per maturity, greeks, vanna, hessian, offsets[, dlog_mgf, d2log_mgf])"""
+    _check_fourier_types(chain[4], is_spot_measure)
+    ch = _chain_arrays(*chain)
+    etas = _backbone(etas, ch.M)
+    n, J = len(names), ch.strikes.shape[0]
+    nh = n * (n + 1) // 2
+    prices, greeks, vanna, hessian = np.empty(J), np.empty((2 + n, J)), np.empty((n, J)), np.empty((nh, J))
+    dlm = np.empty((n, ch.M, max_phi), dtype=np.complex128) if return_grids else None
+    d2lm = np.empty((nh, ch.M, max_phi), dtype=np.complex128) if return_grids else None
+    C.call(symbol, byref(params), *C.chain_ptrs(ch, *etas), *head, C.vol_scaler_arg(vol_scaler), max_phi, C.dptr(prices), C.dptr(greeks),
+           C.dptr(dlm), *((None,) if with_nfev else ()), C.dptr(vanna), C.dptr(hessian), C.dptr(d2lm))
+    out = (C.split_chain(prices, ch.offsets), greeks, vanna, hessian, ch.offsets)
+    return out + (dlm, d2lm) if return_grids else out
+
+
+def logsv_price_chain_hessian(params: C.LogsvParamsC, ttms, forwards, discfactors, etas, strikes_ttms, optiontypes_ttms,
+                              is_spot_measure: bool = True, expansion_order: int = C.ORDER_SECOND, vol_scaler: Optional[float] = None,
+                              max_phi: Optional[int] = None, return_grids: bool = False):
+    """logsv_price_chain_greeks plus the second-order sensitivities (b200sv_logsv_price_chain_hessian).  Returns (prices per maturity,
+    greeks [2 + 6, J], vanna [6, J], hessian [21, J], offsets): greeks as logsv_price_chain_greeks (bit for bit), vanna rows in
+    LOGSV_GREEK_PARAMS order, hessian rows the upper triangle (p <= q) row-major in that order; ``return_grids`` adds
+    (dlog_mgf [6, M, P], d2log_mgf [21, M, P])."""
+    return _price_chain_hessian("b200sv_logsv_price_chain_hessian", params, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms),
+                                (etas,), is_spot_measure, (int(bool(is_spot_measure)), C.LOG_RETURN, int(expansion_order)), vol_scaler,
+                                int(max_phi or 1000), return_grids, LOGSV_GREEK_PARAMS, True)
+
+
+def heston_price_chain_hessian(params: C.HestonParamsC, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms,
+                               vol_scaler: Optional[float] = None, max_phi: Optional[int] = None, return_grids: bool = False):
+    """Heston twin of logsv_price_chain_hessian (b200sv_heston_price_chain_hessian): vanna [5, J], hessian [15, J] over
+    HESTON_GREEK_PARAMS; ``return_grids`` adds (dlog_mgf [5, M, P], d2log_mgf [15, M, P])."""
+    return _price_chain_hessian("b200sv_heston_price_chain_hessian", params, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms),
+                                (), True, (C.LOG_RETURN,), vol_scaler, int(max_phi or 1000), return_grids, HESTON_GREEK_PARAMS, False)
+
+
 def hawkesjd_price_chain_greeks(params: C.HawkesParamsC, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms,
                                 is_spot_measure: bool = True, vol_scaler: Optional[float] = None, max_phi: Optional[int] = None,
                                 return_grids: bool = False):

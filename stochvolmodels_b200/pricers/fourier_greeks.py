@@ -26,17 +26,35 @@ class FourierChainGreeks:
     params: Dict[str, List[np.ndarray]]
 
 
-def check_fourier_greeks_kwargs(kwargs) -> None:
-    """reject what the forward-mode route does not cover before any GPU work"""
+@dataclass
+class FourierChainHessian(FourierChainGreeks):
+    """``FourierChainGreeks`` (bit-identical to ``price_chain_greeks``) plus the second order, one array per maturity:
+    ``vanna``: parameter name -> d^2 price / d forward d parameter; ``hessian``: name -> name -> d^2 price / d p d q, symmetric
+    (``hessian[p][q]`` and ``hessian[q][p]`` are the same arrays)."""
+    vanna: Dict[str, List[np.ndarray]]
+    hessian: Dict[str, Dict[str, List[np.ndarray]]]
+
+
+def _check_fourier_kwargs(kwargs, method: str) -> None:
     if kwargs.get("is_analytic"):
-        raise NotImplementedError("price_chain_greeks does not cover the semi-analytic branch (is_analytic)")
+        raise NotImplementedError(f"{method} does not cover the semi-analytic branch (is_analytic)")
     if kwargs.get("is_stiff_solver"):
-        raise NotImplementedError("price_chain_greeks does not cover the BDF branch (is_stiff_solver)")
+        raise NotImplementedError(f"{method} does not cover the BDF branch (is_stiff_solver)")
     if kwargs.get("use_rough_mc"):
-        raise NotImplementedError("price_chain_greeks does not cover the rough-vol route (use_rough_mc)")
+        raise NotImplementedError(f"{method} does not cover the rough-vol route (use_rough_mc)")
     vt = kwargs.get("variable_type")
     if vt is not None and getattr(vt, "value", vt) != C.LOG_RETURN:
-        raise NotImplementedError("price_chain_greeks covers variable_type=LOG_RETURN only")
+        raise NotImplementedError(f"{method} covers variable_type=LOG_RETURN only")
+
+
+def check_fourier_greeks_kwargs(kwargs) -> None:
+    """reject what the forward-mode route does not cover before any GPU work"""
+    _check_fourier_kwargs(kwargs, "price_chain_greeks")
+
+
+def check_fourier_hessian_kwargs(kwargs) -> None:
+    """the same rejections for ``price_chain_hessian``"""
+    _check_fourier_kwargs(kwargs, "price_chain_hessian")
 
 
 def to_fourier_chain_greeks(prices, greeks, offsets, names: Sequence[str]) -> FourierChainGreeks:
@@ -44,3 +62,17 @@ def to_fourier_chain_greeks(prices, greeks, offsets, names: Sequence[str]) -> Fo
     split = lambda row: C.split_chain(row, offsets)
     return FourierChainGreeks(prices=prices, delta=split(greeks[0]), gamma=split(greeks[1]),
                               params={n: split(greeks[2 + k]) for k, n in enumerate(names)})
+
+
+def to_fourier_chain_hessian(prices, greeks, vanna, hessian, offsets, names: Sequence[str]) -> FourierChainHessian:
+    """engine.*_price_chain_hessian output -> FourierChainHessian; hessian rows are the upper triangle p <= q, row-major in ``names``"""
+    split = lambda row: C.split_chain(row, offsets)
+    first = to_fourier_chain_greeks(prices, greeks, offsets, names)
+    hess: Dict[str, Dict[str, List[np.ndarray]]] = {n: {} for n in names}
+    r = 0
+    for i, p in enumerate(names):
+        for q in names[i:]:
+            hess[p][q] = hess[q][p] = split(hessian[r])
+            r += 1
+    return FourierChainHessian(prices=first.prices, delta=first.delta, gamma=first.gamma, params=first.params,
+                               vanna={n: split(vanna[k]) for k, n in enumerate(names)}, hessian=hess)

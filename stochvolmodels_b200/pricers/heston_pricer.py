@@ -69,6 +69,17 @@ class HestonPricer(ModelPricer):
             option_chain.discfactors, option_chain.strikes_ttms, option_chain.optiontypes_ttms, vol_scaler=kwargs.get("vol_scaler"))
         return to_fourier_chain_greeks(prices, greeks, offsets, engine.HESTON_GREEK_PARAMS)
 
+    def price_chain_hessian(self, option_chain: OptionChain, params: HestonParams, **kwargs):
+        """``price_chain_greeks`` (bit for bit) plus vanna and the symmetric Hessian over (v0, theta, kappa, rho, volvol) in one call ->
+        ``FourierChainHessian``: second derivatives of the closed form through hyper-dual numbers on a fixed transform grid.  Q_VAR
+        raises NotImplementedError."""
+        from .fourier_greeks import check_fourier_hessian_kwargs, to_fourier_chain_hessian
+        check_fourier_hessian_kwargs(kwargs)
+        prices, greeks, vanna, hessian, offsets = engine.heston_price_chain_hessian(
+            _params_c(params.v0, params.theta, params.kappa, params.rho, params.volvol), option_chain.ttms, option_chain.forwards,
+            option_chain.discfactors, option_chain.strikes_ttms, option_chain.optiontypes_ttms, vol_scaler=kwargs.get("vol_scaler"))
+        return to_fourier_chain_hessian(prices, greeks, vanna, hessian, offsets, engine.HESTON_GREEK_PARAMS)
+
     @timer
     def calibrate_model_params_to_chain(self, option_chain: OptionChain, params0: HestonParams = None, is_vega_weighted: bool = True,
                                         is_unit_ttm_vega: bool = False, **kwargs) -> HestonParams:

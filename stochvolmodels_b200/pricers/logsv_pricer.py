@@ -185,6 +185,20 @@ class LogSVPricer(ModelPricer):
             vol_scaler=kwargs.get("vol_scaler"), max_phi=kwargs.get("max_phi"))
         return to_fourier_chain_greeks(prices, greeks, offsets, engine.LOGSV_GREEK_PARAMS)
 
+    def price_chain_hessian(self, option_chain: OptionChain, params: LogSvParams, is_spot_measure: bool = True, **kwargs):
+        """``price_chain_greeks`` (bit for bit) plus the second-order sensitivities in one call -> ``FourierChainHessian``: vanna
+        d^2 price / d forward d p and the symmetric Hessian d^2 price / d p d q over (sigma0, theta, kappa1, kappa2, beta, volvol), exact
+        second derivatives of the scheme on the adaptive solver's accepted steps.  Same arguments, conventions and rejections as
+        ``price_chain_greeks``."""
+        from .fourier_greeks import check_fourier_hessian_kwargs, to_fourier_chain_hessian
+        check_fourier_hessian_kwargs(kwargs)
+        prices, greeks, vanna, hessian, offsets = engine.logsv_price_chain_hessian(
+            _params_c(params), option_chain.ttms, option_chain.forwards, option_chain.discfactors,
+            params.get_vol_backbone_etas(ttms=option_chain.ttms), option_chain.strikes_ttms, option_chain.optiontypes_ttms,
+            is_spot_measure=is_spot_measure, expansion_order=_order_code(kwargs.get("expansion_order", ExpansionOrder.SECOND)),
+            vol_scaler=kwargs.get("vol_scaler"), max_phi=kwargs.get("max_phi"))
+        return to_fourier_chain_hessian(prices, greeks, vanna, hessian, offsets, engine.LOGSV_GREEK_PARAMS)
+
     def set_vol_scaler(self, option_chain: OptionChain) -> float:
         """transform-grid scaler from the first slice's ATM vol (reference :436-439)."""
         return set_vol_scaler(sigma0=option_chain.get_chain_atm_vols()[0], ttm=option_chain.ttms[0])
