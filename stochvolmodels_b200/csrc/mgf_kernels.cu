@@ -49,19 +49,19 @@ __device__ __forceinline__ cd operator/(cd a, cd b) {
   const double r = b.re / b.im, d = b.re * r + b.im;
   return cd{(a.re * r + a.im) / d, (a.im * r - a.re) / d};
 }
-__device__ __forceinline__ cd csqrt_(cd z) {   // principal branch
+__device__ __forceinline__ cd sqrt_(cd z) {   // principal branch
   if (z.re == 0.0 && z.im == 0.0) return cd{0.0, z.im};
   const double t = sqrt(0.5 * (fabs(z.re) + hypot(z.re, z.im)));
   if (z.re >= 0.0) return cd{t, z.im / (2.0 * t)};
   return cd{fabs(z.im) / (2.0 * t), copysign(t, z.im)};
 }
-__device__ __forceinline__ cd cexp_(cd z) {
+__device__ __forceinline__ cd exp_(cd z) {
   double s, c;
   sincos(z.im, &s, &c);
   const double e = exp(z.re);
   return cd{e * c, e * s};
 }
-__device__ __forceinline__ cd clog_(cd z) { return cd{log(hypot(z.re, z.im)), atan2(z.im, z.re)}; }
+__device__ __forceinline__ cd log_(cd z) { return cd{log(hypot(z.re, z.im)), atan2(z.im, z.re)}; }
 
 // --------------------------------------------------------------------------------------------------------------------
 // LogSV affine expansion: per-grid-point coefficients of A' = A^T M A + L A + H (sparse, hand-expanded)
@@ -630,6 +630,43 @@ __global__ void __launch_bounds__(32 * kLaneWarpsPerBlock, 1) logsv_mgf_lanes_ke
 // --------------------------------------------------------------------------------------------------------------------
 // Heston closed form: pricers/heston_pricer.py:199-214, chained over maturities with (a, b) carried in registers
 // --------------------------------------------------------------------------------------------------------------------
+// Written once over the number type: T = cd for the prices, dcd (one direction) for the tangents, hcd (a pair) for the Hessian, with the
+// parameters in R = double, dcd, hcd and the overloads sqrt_ / exp_ / log_ of each type.  The constructor is the per-point set-up, step()
+// carries (a, b) over one maturity increment; operand order is part of the result (every kernel reproduces the fp64 of the others).
+template <class R, class T>
+struct HestonClosedForm {
+  struct AB {
+    T a, b;
+  };
+  R th, ka, vv2;
+  T psi_p, psi_m, zeta, two_zeta;
+
+  __device__ __forceinline__ HestonClosedForm(R theta, R kappa, R rho, R volvol, cd ph, cd ps)
+      : th(theta), ka(kappa), vv2(volvol * volvol) {
+    const T b1 = T{kappa} + (rho * volvol) * T{ph};
+    const T b0 = T{(0.5 * ph) * (ph + mk(1.0)) - ps};
+    zeta = sqrt_(b1 * b1 - (2.0 * b0) * vv2);
+    psi_p = zeta - b1;
+    psi_m = b1 + zeta;
+    two_zeta = 2.0 * zeta;
+  }
+  __device__ __forceinline__ void step(double tau, T& a, T& b) const {
+    const T ez = exp_(-(tau * zeta));
+    const T c_p = (psi_p + vv2 * b) / two_zeta, c_m = (psi_m - vv2 * b) / two_zeta;
+    const T den = c_p * ez + c_m;
+    const T b_new = -((-(psi_m * c_p)) * ez + psi_p * c_m) / (vv2 * den);
+    const T a_new = (-((th * ka) / vv2)) * (tau * psi_p + 2.0 * log_(den)) + a;
+    a = a_new;
+    b = b_new;
+  }
+  // step() on copies of (a, b), returned: what heston_mgf_kernel calls, since stepping its own (a, b) in place gives the same arithmetic on
+  // differently allocated registers
+  __device__ __forceinline__ AB stepped(double tau, T a, T b) const {
+    step(tau, a, b);
+    return AB{a, b};
+  }
+};
+
 __global__ void heston_mgf_kernel(const cd* __restrict__ phi, const cd* __restrict__ psi, int P, int M,
                                   const double* __restrict__ dtaus, b200sv_heston_params hp, const cd* __restrict__ a_in,
                                   const cd* __restrict__ b_in, cd* __restrict__ a_out, cd* __restrict__ b_out,
@@ -644,21 +681,11 @@ __global__ void heston_mgf_kernel(const cd* __restrict__ phi, const cd* __restri
   }
   const cd ph = phi[p], ps = psi ? psi[p] : mk(0.0);
   cd a = a_in ? a_in[p] : mk(0.0), b = b_in ? b_in[p] : mk(0.0);
-  const double vv2 = hp.volvol * hp.volvol;
-  const cd b1 = mk(hp.kappa) + (hp.rho * hp.volvol) * ph;
-  const cd b0 = (0.5 * ph) * (ph + mk(1.0)) - ps;
-  const cd zeta = csqrt_(b1 * b1 - (2.0 * b0) * vv2);
-  const cd psi_p = zeta - b1, psi_m = b1 + zeta;
-  const cd two_zeta = 2.0 * zeta;
+  const HestonClosedForm<double, cd> cf(hp.theta, hp.kappa, hp.rho, hp.volvol, ph, ps);
   for (int mm = 0; mm < M; ++mm) {
-    const double tau = dtaus[mm];
-    const cd ez = cexp_(-(zeta * tau));
-    const cd c_p = (psi_p + vv2 * b) / two_zeta, c_m = (psi_m - vv2 * b) / two_zeta;
-    const cd den = c_p * ez + c_m;
-    const cd b_new = -((-(psi_m * c_p)) * ez + psi_p * c_m) / (vv2 * den);
-    const cd a_new = (-(hp.theta * hp.kappa / vv2)) * (psi_p * tau + 2.0 * clog_(den)) + a;
-    a = a_new;
-    b = b_new;
+    const auto ab = cf.stepped(dtaus[mm], a, b);
+    a = ab.a;
+    b = ab.b;
     if (a_out) a_out[(size_t)mm * P + p] = a;
     if (b_out) b_out[(size_t)mm * P + p] = b;
     log_mgf[(size_t)mm * P + p] = a + b * hp.v0;
@@ -668,7 +695,7 @@ __global__ void heston_mgf_kernel(const cd* __restrict__ phi, const cd* __restri
 // --------------------------------------------------------------------------------------------------------------------
 // Fourier sums: utils/mgf_pricer.py:190-219.  One CTA per strike.
 // --------------------------------------------------------------------------------------------------------------------
-struct StrikeSpec {
+struct StrikeSpec {   // one strike of the chain, with its maturity's forward, discount factor and maturity
   double strike, forward, discfactor;
   int type;     // B200SV_CALL ..
   int slice;    // which log_mgf row
@@ -678,22 +705,30 @@ struct StrikeSpec {
 
 constexpr int kFourierThreads = 256;
 
+// The strike sum of one CTA: the quadrature step dp = h3 w_j of every grid point j (the block's threads strided over the P points) goes to
+// term(j, dp, phi_j), which adds the point's terms into the zeroed acc[NV] and skips the point itself when its price term is NaN
+// (np.nansum); then the fixed-order block_sum leaves the sums in thread 0's acc.
+template <int NV, class Term>
+__device__ __forceinline__ void strike_sum(const cd* __restrict__ phi, int P, double (&acc)[NV], Term term) {
+  __shared__ double red[NV * (kFourierThreads / 32)];
+  const double h3 = (phi[1].im - phi[0].im) / 3.0;
+  for (int j = threadIdx.x; j < P; j += kFourierThreads) {
+    // legacy Simpson weights (utils/mgf_pricer.py:163-170): 1,4,2,4,... with first/last = 1 and THEN every odd index = 4
+    const double wq = (j & 1) ? 4.0 : ((j == 0 || j == P - 1) ? 1.0 : 2.0);
+    term(j, h3 * wq, phi[j]);
+  }
+  block_sum<NV, kFourierThreads>(acc, red);
+}
+
 __global__ void __launch_bounds__(kFourierThreads) fourier_vanilla_kernel(const cd* __restrict__ log_mgf, const cd* __restrict__ phi,
                                                                          int P, const StrikeSpec* __restrict__ specs,
                                                                          int is_spot, int half_re, double* __restrict__ prices,
                                                                          double* __restrict__ ivols = nullptr) {
-  __shared__ double red[kFourierThreads / 32];
   const StrikeSpec sp = specs[blockIdx.x];
   const cd* lm = log_mgf + (size_t)sp.slice * P;
-  phi += (size_t)sp.grid * P;
   const double x = log(sp.forward / sp.strike);
-  const double h3 = (phi[1].im - phi[0].im) / 3.0;
-  double acc[1] = {0.0};
-  for (int j = threadIdx.x; j < P; j += kFourierThreads) {
-    // legacy Simpson weights (utils/mgf_pricer.py:163-170): 1,4,2,4,... with first/last = 1 and THEN every odd index = 4
-    double wq = (j & 1) ? 4.0 : ((j == 0 || j == P - 1) ? 1.0 : 2.0);
-    const double dp = h3 * wq;
-    const cd ph = phi[j];
+  double acc[1] = {};
+  strike_sum(phi + (size_t)sp.grid * P, P, acc, [&](int j, double dp, cd ph) {
     cd w;
     if (half_re) {
       w = mk((dp / M_PI) / (ph.im * ph.im + 0.25));
@@ -701,11 +736,9 @@ __global__ void __launch_bounds__(kFourierThreads) fourier_vanilla_kernel(const 
       const cd den = is_spot ? (ph + mk(1.0)) * ph : (ph - mk(1.0)) * ph;
       w = -(mk(dp / M_PI) / den);
     }
-    const cd z = lm[j] - x * ph;
-    const cd term = w * cexp_(z);
-    if (term.re == term.re) acc[0] += term.re;     // np.nansum(np.real(...))
-  }
-  block_sum<1, kFourierThreads>(acc, red);
+    const cd term = w * exp_(lm[j] - x * ph);
+    if (term.re == term.re) acc[0] += term.re;
+  });
   if (threadIdx.x == 0) {
     const double capped = acc[0], F = sp.forward, K = sp.strike, df = sp.discfactor;
     double price;
@@ -731,15 +764,10 @@ struct SumSpec {
 __global__ void __launch_bounds__(kFourierThreads) fourier_sum_kernel(const cd* __restrict__ log_mgf, const cd* __restrict__ grid, int P,
                                                                      const SumSpec* __restrict__ specs, int mode, int all_calls,
                                                                      double* __restrict__ out) {
-  __shared__ double red[kFourierThreads / 32];
   const SumSpec sp = specs[blockIdx.x];
   const cd* lm = log_mgf + (size_t)sp.slice * P;
-  const double h3 = (grid[1].im - grid[0].im) / 3.0;
-  double acc[1] = {0.0};
-  for (int j = threadIdx.x; j < P; j += kFourierThreads) {
-    const double wq = (j & 1) ? 4.0 : ((j == 0 || j == P - 1) ? 1.0 : 2.0);   // legacy Simpson, mgf_pricer.py:163-170
-    const double dp = h3 * wq;
-    const cd g = grid[j];
+  double acc[1] = {};
+  strike_sum(grid, P, acc, [&](int j, double dp, cd g) {
     cd w;
     if (mode == kModeQvar)
       w = mk(dp / M_PI) / (g * g);                              // (dp/pi)/(psi*psi), :344
@@ -747,10 +775,9 @@ __global__ void __launch_bounds__(kFourierThreads) fourier_sum_kernel(const cd* 
       w = mk(dp / M_PI);                                        // dp/pi, :374-376
     else
       w = all_calls ? -(mk(dp / M_PI) / g) : (mk(dp / M_PI) / g);   // -/+ (dp/pi)/phi, :241-246
-    const cd term = w * cexp_(sp.coef * g + lm[j]);
+    const cd term = w * exp_(sp.coef * g + lm[j]);
     if (term.re == term.re) acc[0] += term.re;
-  }
-  block_sum<1, kFourierThreads>(acc, red);
+  });
   if (threadIdx.x == 0) {
     const double S = acc[0];
     double r;
@@ -806,8 +833,8 @@ struct HawkesRhsFn {
   cd phi, drift0;          // drift0 = sigma^2 ((phi + 1) phi / 2 - psi)
   __device__ __forceinline__ void operator()(const cd (&A)[3], cd (&out)[3]) const {
     const cd zp = (phi - c.beta1_p * A[1]) - c.beta1_m * A[2], zm = (phi - c.beta2_p * A[1]) - c.beta2_m * A[2];
-    const cd jp = cexp_(-c.shift_p * zp) / (mk(1.0) + c.mean_p * zp) - mk(1.0);
-    const cd jm = cexp_(-c.shift_m * zm) / (mk(1.0) + c.mean_m * zm) - mk(1.0);
+    const cd jp = exp_(-c.shift_p * zp) / (mk(1.0) + c.mean_p * zp) - mk(1.0);
+    const cd jm = exp_(-c.shift_m * zm) / (mk(1.0) + c.mean_m * zm) - mk(1.0);
     out[0] = (c.kt_p * A[1] + c.kt_m * A[2]) + drift0;
     out[1] = (jp - c.kappa_p * A[1]) + c.comp_p * phi;
     out[2] = (jm - c.kappa_m * A[2]) + c.comp_m * phi;
@@ -849,37 +876,10 @@ __global__ void __launch_bounds__(TPB) hawkes_mgf_kernel(const cd* __restrict__ 
 
 // slice_pricer_with_mgf_grid_with_gamma (utils/mgf_pricer.py:273-320): general weights -(dp/pi) / ((phi + g + 1)(phi + g)) (its fast branch
 // compares Re(phi) with +(1/2 + g) while the grid sits on -(1/2 + g), so it never runs), calls gamma_forward - n K^(1+g) S, puts K - n K^(1+g) S;
-// no discount factor (both as in the reference).  spec.forward = forward, spec.discfactor = normalizer n, spec.ttm = gamma_forward.
-__global__ void __launch_bounds__(kFourierThreads) fourier_gamma_kernel(const cd* __restrict__ log_mgf, const cd* __restrict__ phi, int P,
-                                                                       const StrikeSpec* __restrict__ specs, double gamma,
-                                                                       double* __restrict__ prices) {
-  __shared__ double red[kFourierThreads / 32];
-  const StrikeSpec sp = specs[blockIdx.x];
-  const cd* lm = log_mgf + (size_t)sp.slice * P;
-  const double x = log(sp.forward / sp.strike);
-  const double h3 = (phi[1].im - phi[0].im) / 3.0;
-  const bool fast = fabs(phi[0].re - (0.5 + gamma)) < 1e-10;
-  double acc[1] = {0.0};
-  for (int j = threadIdx.x; j < P; j += kFourierThreads) {
-    const double wq = (j & 1) ? 4.0 : ((j == 0 || j == P - 1) ? 1.0 : 2.0);
-    const double dp = h3 * wq;
-    const cd ph = phi[j];
-    const cd pg = ph + mk(gamma);
-    const cd w = fast ? mk((dp / M_PI) / (ph.im * ph.im + 0.25)) : -(mk(dp / M_PI) / ((pg + mk(1.0)) * pg));
-    const cd term = w * cexp_(lm[j] - x * ph);
-    if (term.re == term.re) acc[0] += term.re;
-  }
-  block_sum<1, kFourierThreads>(acc, red);
-  if (threadIdx.x == 0) {
-    const double gk = pow(sp.strike, 1.0 + gamma);
-    prices[blockIdx.x] = (sp.type == B200SV_CALL ? sp.ttm : sp.strike) - sp.discfactor * gk * acc[0];
-  }
-}
-
-// fourier_gamma_kernel over the rows of a batch (b200sv_hawkesjd_price_chain_batch), with the Black inversion of fourier_vanilla_kernel
-// fused: row grid sp.grid sits on Re phi = -1/2 - gammas[sp.grid]; norm_gfwd[2 sp.slice + {0, 1}] = that slice's normaliser and forward under
-// the risk kernel.  spec.forward / discfactor / ttm are the chain's own: the calibration objective inverts the (undiscounted) gamma price
-// with the chain's forward, discount factor and maturity (compute_model_ivols_from_chain_data, as in the reference).
+// no discount factor (both as in the reference).  Row grid sp.grid sits on Re phi = -1/2 - gammas[sp.grid]; norm_gfwd[2 sp.slice + {0, 1}] =
+// that slice's normaliser n and forward under the risk kernel (b200sv_fourier_gamma: one grid and one slice).  ivols (optional): the Black
+// inversion of fourier_vanilla_kernel fused for the batch -- spec.forward / discfactor / ttm are the chain's own, and the calibration
+// objective inverts the (undiscounted) gamma price with them (compute_model_ivols_from_chain_data, as in the reference).
 __global__ void __launch_bounds__(kFourierThreads) fourier_gamma_batch_kernel(const cd* __restrict__ log_mgf, const cd* __restrict__ phi, int P,
                                                                              const StrikeSpec* __restrict__ specs, const double* __restrict__ gammas,
                                                                              const double* __restrict__ norm_gfwd, double* __restrict__ prices,
@@ -899,7 +899,7 @@ __global__ void __launch_bounds__(kFourierThreads) fourier_gamma_batch_kernel(co
     const cd ph = phi[j];
     const cd pg = ph + mk(gamma);
     const cd w = fast ? mk((dp / M_PI) / (ph.im * ph.im + 0.25)) : -(mk(dp / M_PI) / ((pg + mk(1.0)) * pg));
-    const cd term = w * cexp_(lm[j] - x * ph);
+    const cd term = w * exp_(lm[j] - x * ph);
     if (term.re == term.re) acc[0] += term.re;
   }
   block_sum<1, kFourierThreads>(acc, red);
@@ -1018,55 +1018,74 @@ __device__ __forceinline__ void rhs_tangent(const cd (&A)[N], const cd (&dA)[N],
   for (int k = 0; k < N; ++k) out[k] = jv[k] + pv[k];
 }
 
-// The tangent of one parameter direction stepped on rk45_generic's attempts: dY_s = dy + h sum_j a_sj dK_j, dK_s = d f(Y_s), accepted
-// steps commit dy <- dy + h sum_j b_j dK_j and dK_0 <- dK_6 (FSAL).  dK: 8 "stages" in shared memory, 0..6 the stage tangents, 7 the
-// candidate dy of the current attempt.  dy stays in registers and carries over maturities like A.
-// TanRhs: functor ``void operator()(const cd (&Y)[N], const cd (&dY)[N], cd (&out)[N]) const`` = J(Y) dY + d_p f(Y) of one direction
-// (LogsvTanRhsFn, HawkesTanRhsFn); the bookkeeping does not depend on it.
-template <int N, int TPB, typename TanRhs>
-struct TangentHook {
-  TanRhs f;
-  StageStore<N, TPB> dK;        // StageStore indexes (stage * N + k) * TPB: 8 stages fit in 8 * N * TPB entries
+// One tangent stepped on rk45_generic's attempts: dY_s = dy + h sum_j a_sj dK_j, dK_s = d f(Y_s), accepted steps commit
+// dy <- dy + h sum_j b_j dK_j and dK_0 <- dK_6 (FSAL).  dK: 8 "stages" in shared memory (StageStore indexes (stage * N + k) * TPB, so 8
+// stages fit in 8 * N * TPB entries), 0..6 the stage tangents, 7 the candidate dy of the current attempt.  dy stays in registers and
+// carries over maturities like A.
+template <int N, int TPB>
+struct TangentStore {
+  StageStore<N, TPB> dK;
   cd dy[N];
 
-  __device__ __forceinline__ void eval(int s, const cd (&Y)[N], const cd (&dY)[N]) {
-    cd o[N];
-    f(Y, dY, o);
-#pragma unroll
-    for (int k = 0; k < N; ++k) dK.at(s, k) = o[k];
-  }
-  __device__ __forceinline__ void start(const cd (&y)[N]) { eval(0, y, dy); }
-  __device__ __forceinline__ void stage(int s, const cd (&yt)[N], double h) {
-    cd dyt[N];
+  // the input dy + h sum_j a_sj dK_j of stage s
+  __device__ __forceinline__ void stage_input(int s, double h, cd (&out)[N]) {
 #pragma unroll
     for (int k = 0; k < N; ++k) {
       cd acc = dK.at(0, k) * c_A[s][0];
 #pragma unroll
       for (int jj = 1; jj < 5; ++jj) acc = acc + dK.at(jj, k) * c_A[s][jj];
-      dyt[k] = dy[k] + acc * h;
+      out[k] = dy[k] + acc * h;
     }
-    eval(s, yt, dyt);
   }
-  __device__ __forceinline__ void last(const cd (&yn)[N], double h) {
+  // the candidate dy + h sum_j b_j dK_j of the attempt, also parked in stage 7
+  __device__ __forceinline__ void candidate(double h, cd (&out)[N]) {
     constexpr double B[6] = {35.0 / 384, 0, 500.0 / 1113, 125.0 / 192, -2187.0 / 6784, 11.0 / 84};
-    cd dyn[N];
 #pragma unroll
     for (int k = 0; k < N; ++k) {
       cd acc = dK.at(0, k) * B[0];
 #pragma unroll
       for (int jj = 2; jj < 6; ++jj) acc = acc + dK.at(jj, k) * B[jj];
-      dyn[k] = dy[k] + h * acc;
-      dK.at(7, k) = dyn[k];
+      out[k] = dy[k] + h * acc;
+      dK.at(7, k) = out[k];
     }
+  }
+};
+
+// The accept step of the tangent stores of one attempt: dy <- the candidate, dK_0 <- dK_6 (FSAL), component by component across the stores.
+template <int N, int TPB, class... Store>
+__device__ __forceinline__ void accept_tangents(Store&... s) {
+#pragma unroll
+  for (int k = 0; k < N; ++k) {
+    ((s.dy[k] = s.dK.at(7, k)), ...);
+    ((s.dK.at(0, k) = s.dK.at(6, k)), ...);
+  }
+}
+
+// The tangent of one parameter direction.  TanRhs: functor ``void operator()(const cd (&Y)[N], const cd (&dY)[N], cd (&out)[N]) const``
+// = J(Y) dY + d_p f(Y) of one direction (LogsvTanRhsFn, HawkesTanRhsFn); the bookkeeping does not depend on it.
+template <int N, int TPB, typename TanRhs>
+struct TangentHook {
+  TanRhs f;
+  TangentStore<N, TPB> t;
+
+  __device__ __forceinline__ void eval(int s, const cd (&Y)[N], const cd (&dY)[N]) {
+    cd o[N];
+    f(Y, dY, o);
+#pragma unroll
+    for (int k = 0; k < N; ++k) t.dK.at(s, k) = o[k];
+  }
+  __device__ __forceinline__ void start(const cd (&y)[N]) { eval(0, y, t.dy); }
+  __device__ __forceinline__ void stage(int s, const cd (&yt)[N], double h) {
+    cd dyt[N];
+    t.stage_input(s, h, dyt);
+    eval(s, yt, dyt);
+  }
+  __device__ __forceinline__ void last(const cd (&yn)[N], double h) {
+    cd dyn[N];
+    t.candidate(h, dyn);
     eval(6, yn, dyn);
   }
-  __device__ __forceinline__ void accept() {
-#pragma unroll
-    for (int k = 0; k < N; ++k) {
-      dy[k] = dK.at(7, k);
-      dK.at(0, k) = dK.at(6, k);
-    }
-  }
+  __device__ __forceinline__ void accept() { accept_tangents<N, TPB>(t); }
 };
 
 template <int N, int TPB>
@@ -1109,12 +1128,12 @@ __global__ void __launch_bounds__(kTangentTPB) logsv_mgf_tangent_kernel(const cd
   LogsvTangentHook<N, TPB> tan;
   tan.f.c = &c;
   tan.f.dc = CoefView<TPB>{dcoef_smem + threadIdx.x};
-  tan.dK = StageStore<N, TPB>{tan_smem + threadIdx.x};
+  tan.t.dK = StageStore<N, TPB>{tan_smem + threadIdx.x};
   cd A[N];
 #pragma unroll
   for (int k = 0; k < N; ++k) {
     A[k] = mk(0.0);
-    tan.dy[k] = mk(0.0);
+    tan.t.dy[k] = mk(0.0);
   }
   const cd ph = phi[p], ps = mk(0.0);
   const double y2 = y * y;
@@ -1135,7 +1154,7 @@ __global__ void __launch_bounds__(kTangentTPB) logsv_mgf_tangent_kernel(const cd
 #pragma unroll
     for (int k = 0; k < N; ++k) {
       lm = lm + A[k] * ys[k];
-      dlm = dlm + (tan.dy[k] * ys[k] + A[k] * (dys[k] * dy_dp));
+      dlm = dlm + (tan.t.dy[k] * ys[k] + A[k] * (dys[k] * dy_dp));
       dls = dls + A[k] * dys[k];
     }
     dlog_mgf[((size_t)(1 + dir) * M + mm) * P + p] = dlm;
@@ -1164,15 +1183,15 @@ __device__ __forceinline__ dcd operator/(dcd a, dcd b) {
   const cd q = a.v / b.v;
   return dcd{q, (a.d - q * b.d) / b.v};
 }
-__device__ __forceinline__ dcd dsqrt(dcd z) {
-  const cd s = csqrt_(z.v);
+__device__ __forceinline__ dcd sqrt_(dcd z) {
+  const cd s = sqrt_(z.v);
   return dcd{s, z.d / (2.0 * s)};
 }
-__device__ __forceinline__ dcd dexp(dcd z) {
-  const cd e = cexp_(z.v);
+__device__ __forceinline__ dcd exp_(dcd z) {
+  const cd e = exp_(z.v);
   return dcd{e, e * z.d};
 }
-__device__ __forceinline__ dcd dlog(dcd z) { return dcd{clog_(z.v), z.d / z.v}; }
+__device__ __forceinline__ dcd log_(dcd z) { return dcd{log_(z.v), z.d / z.v}; }
 
 // heston_mgf_kernel in forward mode: one thread = one (grid point, direction theta | kappa | rho | volvol), (a, b) and their tangents
 // carried over the maturities.  dlog_mgf [5][M][P]: row 0 d/dv0 = b, rows 1.. the directions (HESTON_GREEK_PARAMS order).
@@ -1184,23 +1203,10 @@ __global__ void heston_mgf_tangent_kernel(const cd* __restrict__ phi, int P, int
   const int p = t / D, dir = t % D;
   const dcd th = dmk(mk(hp.theta), mk(dir == 0 ? 1.0 : 0.0)), ka = dmk(mk(hp.kappa), mk(dir == 1 ? 1.0 : 0.0));
   const dcd rho = dmk(mk(hp.rho), mk(dir == 2 ? 1.0 : 0.0)), vv = dmk(mk(hp.volvol), mk(dir == 3 ? 1.0 : 0.0));
-  const dcd ph = dmk(phi[p]);
-  const dcd vv2 = vv * vv;
-  const dcd b1 = ka + (rho * vv) * ph;
-  const dcd b0 = dmk((0.5 * ph.v) * (ph.v + mk(1.0)));
-  const dcd zeta = dsqrt(b1 * b1 - (2.0 * b0) * vv2);
-  const dcd psi_p = zeta - b1, psi_m = b1 + zeta;
-  const dcd two_zeta = 2.0 * zeta;
+  const HestonClosedForm<dcd, dcd> cf(th, ka, rho, vv, phi[p], mk(0.0));
   dcd a = dmk(mk(0.0)), b = dmk(mk(0.0));
   for (int mm = 0; mm < M; ++mm) {
-    const double tau = dtaus[mm];
-    const dcd ez = dexp(-(tau * zeta));
-    const dcd c_p = (psi_p + vv2 * b) / two_zeta, c_m = (psi_m - vv2 * b) / two_zeta;
-    const dcd den = c_p * ez + c_m;
-    const dcd b_new = -((-(psi_m * c_p)) * ez + psi_p * c_m) / (vv2 * den);
-    const dcd a_new = (-((th * ka) / vv2)) * (tau * psi_p + 2.0 * dlog(den)) + a;
-    a = a_new;
-    b = b_new;
+    cf.step(dtaus[mm], a, b);
     dlog_mgf[((size_t)(1 + dir) * M + mm) * P + p] = a.d + b.d * hp.v0;
     if (dir == 0) dlog_mgf[(size_t)mm * P + p] = b.v;
   }
@@ -1243,7 +1249,7 @@ static HawkesTangentDirs make_hawkes_tangents(const b200sv_hawkes_params& p) {
 // d E(z) of the jump-size MGF E(z) = e^{-s z} / (1 + m z) along (dz, ds, dm):  E (-(s + m / (1 + m z)) dz - z ds - z / (1 + m z) dm)
 __device__ __forceinline__ cd hawkes_djump(cd z, cd dz, double s, double m, double ds, double dm) {
   const cd r = mk(1.0) / (mk(1.0) + m * z);
-  const cd e = cexp_(-s * z) * r;
+  const cd e = exp_(-s * z) * r;
   return e * (-((mk(s) + m * r) * dz) - z * (mk(ds) + dm * r));
 }
 
@@ -1284,7 +1290,7 @@ __global__ void __launch_bounds__(TPB) hawkes_mgf_tangent_kernel(const cd* __res
   const cd ph = phi[p];
   const cd h0 = 0.5 * ((ph + mk(1.0)) * ph);
   const HawkesRhsFn f{c, ph, c.sigma2 * h0};
-  TangentHook<3, TPB, HawkesTanRhsFn> tan{HawkesTanRhsFn{c, dirs.d[dir], ph, h0}, StageStore<3, TPB>{tan_smem + threadIdx.x}, {}};   // dy = 0
+  TangentHook<3, TPB, HawkesTanRhsFn> tan{HawkesTanRhsFn{c, dirs.d[dir], ph, h0}, {StageStore<3, TPB>{tan_smem + threadIdx.x}, {}}};   // dy = 0
   cd A[3] = {mk(0.0), mk(0.0), mk(0.0)};
   const int row = hawkes_dir_row(dir);
   int st = 0, nf = 0;
@@ -1292,7 +1298,7 @@ __global__ void __launch_bounds__(TPB) hawkes_mgf_tangent_kernel(const cd* __res
     int nfe = 0;
     st |= rk45_generic<3, TPB>(A, dtaus[m], f, K, &nfe, &tan);
     nf += nfe;
-    dlog_mgf[((size_t)row * M + m) * P + p] = (tan.dy[0] + tan.dy[1] * c.lambda_p) + tan.dy[2] * c.lambda_m;
+    dlog_mgf[((size_t)row * M + m) * P + p] = (tan.t.dy[0] + tan.t.dy[1] * c.lambda_p) + tan.t.dy[2] * c.lambda_m;
     if (dir == 0) {
       dlog_mgf[((size_t)5 * M + m) * P + p] = A[1];
       dlog_mgf[((size_t)10 * M + m) * P + p] = A[2];
@@ -1313,21 +1319,13 @@ __global__ void __launch_bounds__(kFourierThreads) fourier_vanilla_greeks_kernel
                                                                                 const cd* __restrict__ phi, int P, int M,
                                                                                 const StrikeSpec* __restrict__ specs, int is_spot,
                                                                                 double* __restrict__ greeks) {
-  constexpr int NV = 3 + NP;
-  __shared__ double red[NV * (kFourierThreads / 32)];
   const StrikeSpec sp = specs[blockIdx.x];
   const cd* lm = log_mgf + (size_t)sp.slice * P;
   const double x = log(sp.forward / sp.strike);
-  const double h3 = (phi[1].im - phi[0].im) / 3.0;
-  double acc[NV];
-#pragma unroll
-  for (int i = 0; i < NV; ++i) acc[i] = 0.0;
-  for (int j = threadIdx.x; j < P; j += kFourierThreads) {
-    const double wq = (j & 1) ? 4.0 : ((j == 0 || j == P - 1) ? 1.0 : 2.0);
-    const double dp = h3 * wq;
-    const cd ph = phi[j];
+  double acc[3 + NP] = {};
+  strike_sum(phi, P, acc, [&](int j, double dp, cd ph) {
     const double w = (dp / M_PI) / (ph.im * ph.im + 0.25);
-    const cd e = cexp_(lm[j] - x * ph);
+    const cd e = exp_(lm[j] - x * ph);
     const cd term = mk(w) * e;
     if (term.re == term.re) {
       acc[0] += term.re;
@@ -1336,8 +1334,7 @@ __global__ void __launch_bounds__(kFourierThreads) fourier_vanilla_greeks_kernel
 #pragma unroll
       for (int k = 0; k < NP; ++k) acc[3 + k] += w * (e * dlog_mgf[((size_t)k * M + sp.slice) * P + j]).re;
     }
-  }
-  block_sum<NV, kFourierThreads>(acc, red);
+  });
   if (threadIdx.x == 0) {
     const double S = acc[0], Sx = acc[1], Sxx = acc[2], F = sp.forward, K = sp.strike, df = sp.discfactor;
     const int J = gridDim.x;
@@ -1475,76 +1472,39 @@ struct LogsvTan2RhsFn {
   }
 };
 
-// Dormand-Prince stage combination of one tangent store: y + h sum_j a_sj K_j (stage s) ...
-template <int N, int TPB>
-__device__ __forceinline__ void tan_stage_input(StageStore<N, TPB> K, int s, const cd (&y)[N], double h, cd (&out)[N]) {
-#pragma unroll
-  for (int k = 0; k < N; ++k) {
-    cd acc = K.at(0, k) * c_A[s][0];
-#pragma unroll
-    for (int jj = 1; jj < 5; ++jj) acc = acc + K.at(jj, k) * c_A[s][jj];
-    out[k] = y[k] + acc * h;
-  }
-}
-// ... and the candidate y + h sum_j b_j K_j of the attempt, parked in stage 7
-template <int N, int TPB>
-__device__ __forceinline__ void tan_candidate(StageStore<N, TPB> K, const cd (&y)[N], double h, cd (&out)[N]) {
-  constexpr double B[6] = {35.0 / 384, 0, 500.0 / 1113, 125.0 / 192, -2187.0 / 6784, 11.0 / 84};
-#pragma unroll
-  for (int k = 0; k < N; ++k) {
-    cd acc = K.at(0, k) * B[0];
-#pragma unroll
-    for (int jj = 2; jj < 6; ++jj) acc = acc + K.at(jj, k) * B[jj];
-    out[k] = y[k] + h * acc;
-    K.at(7, k) = out[k];
-  }
-}
-
-// TangentHook one order higher: the tangents of directions p and q and the mixed second-order tangent of the pair, all stepped on
-// rk45_generic's attempts with the same bookkeeping (8 stages per store, 7 = the candidate; dy carried in registers over the maturities).
-// Tan2Rhs: ``void operator()(Y, dYp, dYq, d2Y, out_p, out_q, out_pq) const``.
+// TangentHook one order higher: the tangents of directions p and q and the mixed second-order tangent of the pair, three TangentStores
+// stepped on rk45_generic's attempts.  Tan2Rhs: ``void operator()(Y, dYp, dYq, d2Y, out_p, out_q, out_pq) const``.
 template <int N, int TPB, typename Tan2Rhs>
 struct Tangent2Hook {
   Tan2Rhs f;
-  StageStore<N, TPB> dKp, dKq, d2K;
-  cd dyp[N], dyq[N], d2y[N];
+  TangentStore<N, TPB> p, q, pq;
 
   __device__ __forceinline__ void eval(int s, const cd (&Y)[N], const cd (&dYp)[N], const cd (&dYq)[N], const cd (&d2Y)[N]) {
     cd op[N], oq[N], opq[N];
     f(Y, dYp, dYq, d2Y, op, oq, opq);
 #pragma unroll
     for (int k = 0; k < N; ++k) {
-      dKp.at(s, k) = op[k];
-      dKq.at(s, k) = oq[k];
-      d2K.at(s, k) = opq[k];
+      p.dK.at(s, k) = op[k];
+      q.dK.at(s, k) = oq[k];
+      pq.dK.at(s, k) = opq[k];
     }
   }
-  __device__ __forceinline__ void start(const cd (&y)[N]) { eval(0, y, dyp, dyq, d2y); }
+  __device__ __forceinline__ void start(const cd (&y)[N]) { eval(0, y, p.dy, q.dy, pq.dy); }
   __device__ __forceinline__ void stage(int s, const cd (&yt)[N], double h) {
     cd a[N], b[N], c[N];
-    tan_stage_input<N, TPB>(dKp, s, dyp, h, a);
-    tan_stage_input<N, TPB>(dKq, s, dyq, h, b);
-    tan_stage_input<N, TPB>(d2K, s, d2y, h, c);
+    p.stage_input(s, h, a);
+    q.stage_input(s, h, b);
+    pq.stage_input(s, h, c);
     eval(s, yt, a, b, c);
   }
   __device__ __forceinline__ void last(const cd (&yn)[N], double h) {
     cd a[N], b[N], c[N];
-    tan_candidate<N, TPB>(dKp, dyp, h, a);
-    tan_candidate<N, TPB>(dKq, dyq, h, b);
-    tan_candidate<N, TPB>(d2K, d2y, h, c);
+    p.candidate(h, a);
+    q.candidate(h, b);
+    pq.candidate(h, c);
     eval(6, yn, a, b, c);
   }
-  __device__ __forceinline__ void accept() {
-#pragma unroll
-    for (int k = 0; k < N; ++k) {
-      dyp[k] = dKp.at(7, k);
-      dyq[k] = dKq.at(7, k);
-      d2y[k] = d2K.at(7, k);
-      dKp.at(0, k) = dKp.at(6, k);
-      dKq.at(0, k) = dKq.at(6, k);
-      d2K.at(0, k) = d2K.at(6, k);
-    }
-  }
+  __device__ __forceinline__ void accept() { accept_tangents<N, TPB>(p, q, pq); }
 };
 
 constexpr int kHessianTPB = 8;   // shared memory per thread: 6N primal stages + 3 x 8N tangent stages + 4 x 14 coefficients
@@ -1580,14 +1540,14 @@ __global__ void __launch_bounds__(kHessianTPB) logsv_mgf_hessian_kernel(const cd
   tan.f.dcp = CoefView<TPB>{coef_smem + 14 * TPB + threadIdx.x};
   tan.f.dcq = CoefView<TPB>{coef_smem + 28 * TPB + threadIdx.x};
   tan.f.d2c = CoefView<TPB>{coef_smem + 42 * TPB + threadIdx.x};
-  tan.dKp = StageStore<N, TPB>{tan_smem + threadIdx.x};
-  tan.dKq = StageStore<N, TPB>{tan_smem + 8 * N * TPB + threadIdx.x};
-  tan.d2K = StageStore<N, TPB>{tan_smem + 16 * N * TPB + threadIdx.x};
+  tan.p.dK = StageStore<N, TPB>{tan_smem + threadIdx.x};
+  tan.q.dK = StageStore<N, TPB>{tan_smem + 8 * N * TPB + threadIdx.x};
+  tan.pq.dK = StageStore<N, TPB>{tan_smem + 16 * N * TPB + threadIdx.x};
   cd A[N];
 #pragma unroll
   for (int k = 0; k < N; ++k) {
     A[k] = mk(0.0);
-    tan.dyp[k] = tan.dyq[k] = tan.d2y[k] = mk(0.0);
+    tan.p.dy[k] = tan.q.dy[k] = tan.pq.dy[k] = mk(0.0);
   }
   const cd ph = phi[p], ps = mk(0.0);
   const double y2 = y * y;
@@ -1609,8 +1569,8 @@ __global__ void __launch_bounds__(kHessianTPB) logsv_mgf_hessian_kernel(const cd
     cd h = mk(0.0), hs = mk(0.0), hss = mk(0.0);
 #pragma unroll
     for (int k = 0; k < N; ++k) {
-      h = h + (tan.d2y[k] * ys[k] + (tan.dyp[k] * yq + tan.dyq[k] * yp) * dys[k] + A[k] * (yp * yq * d2ys[k]));
-      hs = hs + (tan.dyp[k] * dys[k] + A[k] * (yp * d2ys[k]));      // (sigma0, p): y_sigma0 = 1, no ODE tangent
+      h = h + (tan.pq.dy[k] * ys[k] + (tan.p.dy[k] * yq + tan.q.dy[k] * yp) * dys[k] + A[k] * (yp * yq * d2ys[k]));
+      hs = hs + (tan.p.dy[k] * dys[k] + A[k] * (yp * d2ys[k]));      // (sigma0, p): y_sigma0 = 1, no ODE tangent
       hss = hss + A[k] * d2ys[k];                                      // (sigma0, sigma0)
     }
     d2log_mgf[((size_t)tri_index(1 + dp, 1 + dq, NP) * M + mm) * P + p] = h;
@@ -1636,17 +1596,17 @@ __device__ __forceinline__ hcd operator/(hcd a, hcd b) {   // q = a / b from a =
   const cd q = a.v / b.v, q1 = (a.d1 - q * b.d1) / b.v, q2 = (a.d2 - q * b.d2) / b.v;
   return hcd{q, q1, q2, (((a.d12 - q1 * b.d2) - q2 * b.d1) - q * b.d12) / b.v};
 }
-__device__ __forceinline__ hcd hsqrt(hcd z) {              // s^2 = z differentiated
-  const cd s = csqrt_(z.v), s1 = z.d1 / (2.0 * s), s2 = z.d2 / (2.0 * s);
+__device__ __forceinline__ hcd sqrt_(hcd z) {              // s^2 = z differentiated
+  const cd s = sqrt_(z.v), s1 = z.d1 / (2.0 * s), s2 = z.d2 / (2.0 * s);
   return hcd{s, s1, s2, (z.d12 - 2.0 * (s1 * s2)) / (2.0 * s)};
 }
-__device__ __forceinline__ hcd hexp(hcd z) {
-  const cd e = cexp_(z.v);
+__device__ __forceinline__ hcd exp_(hcd z) {
+  const cd e = exp_(z.v);
   return hcd{e, e * z.d1, e * z.d2, e * (z.d12 + z.d1 * z.d2)};
 }
-__device__ __forceinline__ hcd hlog(hcd z) {
+__device__ __forceinline__ hcd log_(hcd z) {
   const cd l1 = z.d1 / z.v, l2 = z.d2 / z.v;
-  return hcd{clog_(z.v), l1, l2, (z.d12 - l1 * z.d2) / z.v};
+  return hcd{log_(z.v), l1, l2, (z.d12 - l1 * z.d2) / z.v};
 }
 
 // heston_mgf_kernel in second-order forward mode: one thread = one (grid point, pair p <= q of theta | kappa | rho | volvol), (a, b) as
@@ -1664,24 +1624,10 @@ __global__ void heston_mgf_hessian_kernel(const cd* __restrict__ phi, int P, int
   hcd par[D];
 #pragma unroll
   for (int k = 0; k < D; ++k) par[k] = hcd{mk(x[k]), mk(k == dp ? 1.0 : 0.0), mk(k == dq ? 1.0 : 0.0), mk(0.0)};
-  const hcd th = par[0], ka = par[1], rho = par[2], vv = par[3];
-  const hcd ph = hmk(phi[p]);
-  const hcd vv2 = vv * vv;
-  const hcd b1 = ka + (rho * vv) * ph;
-  const hcd b0 = hmk((0.5 * ph.v) * (ph.v + mk(1.0)));
-  const hcd zeta = hsqrt(b1 * b1 - (2.0 * b0) * vv2);
-  const hcd psi_p = zeta - b1, psi_m = b1 + zeta;
-  const hcd two_zeta = 2.0 * zeta;
+  const HestonClosedForm<hcd, hcd> cf(par[0], par[1], par[2], par[3], phi[p], mk(0.0));
   hcd a = hmk(mk(0.0)), b = hmk(mk(0.0));
   for (int mm = 0; mm < M; ++mm) {
-    const double tau = dtaus[mm];
-    const hcd ez = hexp(-(tau * zeta));
-    const hcd c_p = (psi_p + vv2 * b) / two_zeta, c_m = (psi_m - vv2 * b) / two_zeta;
-    const hcd den = c_p * ez + c_m;
-    const hcd b_new = -((-(psi_m * c_p)) * ez + psi_p * c_m) / (vv2 * den);
-    const hcd a_new = (-((th * ka) / vv2)) * (tau * psi_p + 2.0 * hlog(den)) + a;
-    a = a_new;
-    b = b_new;
+    cf.step(dtaus[mm], a, b);
     d2log_mgf[((size_t)tri_index(1 + dp, 1 + dq, NP) * M + mm) * P + p] = a.d12 + b.d12 * hp.v0;
     if (dp == dq) d2log_mgf[((size_t)tri_index(0, 1 + dp, NP) * M + mm) * P + p] = b.d1;
     if (pair == 0) d2log_mgf[(size_t)mm * P + p] = mk(0.0);
@@ -1698,21 +1644,14 @@ __global__ void __launch_bounds__(kFourierThreads) fourier_vanilla_hessian_kerne
                                                                                  int P, int M, const StrikeSpec* __restrict__ specs,
                                                                                  int is_spot, double* __restrict__ vanna,
                                                                                  double* __restrict__ hessian) {
-  constexpr int NH = NP * (NP + 1) / 2, NV = 2 * NP + NH;
-  __shared__ double red[NV * (kFourierThreads / 32)];
+  constexpr int NH = NP * (NP + 1) / 2;
   const StrikeSpec sp = specs[blockIdx.x];
   const cd* lm = log_mgf + (size_t)sp.slice * P;
   const double x = log(sp.forward / sp.strike);
-  const double h3 = (phi[1].im - phi[0].im) / 3.0;
-  double acc[NV];
-#pragma unroll
-  for (int i = 0; i < NV; ++i) acc[i] = 0.0;
-  for (int j = threadIdx.x; j < P; j += kFourierThreads) {
-    const double wq = (j & 1) ? 4.0 : ((j == 0 || j == P - 1) ? 1.0 : 2.0);
-    const double dp = h3 * wq;
-    const cd ph = phi[j];
+  double acc[2 * NP + NH] = {};
+  strike_sum(phi, P, acc, [&](int j, double dp, cd ph) {
     const double w = (dp / M_PI) / (ph.im * ph.im + 0.25);
-    const cd e = cexp_(lm[j] - x * ph);
+    const cd e = exp_(lm[j] - x * ph);
     const cd term = mk(w) * e;
     if (term.re == term.re) {
       cd dl[NP];
@@ -1729,8 +1668,7 @@ __global__ void __launch_bounds__(kFourierThreads) fourier_vanilla_hessian_kerne
 #pragma unroll
         for (int q = p; q < NP; ++q, ++r) acc[2 * NP + r] += w * (e * (d2log_mgf[((size_t)r * M + sp.slice) * P + j] + dl[p] * dl[q])).re;
     }
-  }
-  block_sum<NV, kFourierThreads>(acc, red);
+  });
   if (threadIdx.x == 0) {
     const double F = sp.forward, K = sp.strike, df = sp.discfactor;
     const int J = gridDim.x;
@@ -2494,9 +2432,10 @@ struct HostCall {
 };
 
 // A prepared chain on the device: upload() queues the grid(s), psi and strike rows; the model routes add their per-maturity inputs
-// (spec or dt), write the [B][M][P] log-MGF into lm (and A into a), and sums() prices every strike and copies the prices back.
+// (spec and the LogSV model tangents dspec, or dt), write the [B][M][P] log-MGF into lm (and A into a), and sums() prices every strike and
+// copies the prices back.
 struct ChainDev : HostCall {
-  DevBuf phi{st}, psi{st}, rows{st}, spec{st}, dt{st}, a{st}, lm{st}, pr{st}, iv{st};
+  DevBuf phi{st}, psi{st}, rows{st}, spec{st}, dspec{st}, dt{st}, a{st}, lm{st}, pr{st}, iv{st};
 
   int upload(const FourierChain& c) {
     B200SV_CUDA(phi.upload(c.phi.data(), c.phi.size()));
@@ -2511,17 +2450,18 @@ struct ChainDev : HostCall {
     return 0;
   }
 
-  // vanilla (or Q_VAR, or with a risk-premia gamma the gamma) Fourier sum, one CTA per strike; no launch on an empty chain
-  int sums(const FourierChain& c, double* prices_out, double* ivols_out, double gamma = NAN) {
+  // vanilla (or Q_VAR, or with risk-premia gammas the gamma) Fourier sum, one CTA per strike; no launch on an empty chain.  gammas [G] and
+  // norm_gfwd [B][M][2] (device, both or neither): the gamma of each grid and the (normaliser, gamma forward) of each slice.
+  int sums(const FourierChain& c, double* prices_out, double* ivols_out, const double* gammas = nullptr, const double* norm_gfwd = nullptr) {
     if (c.Jtot == 0) return 0;
     const size_t nq = (size_t)c.B * c.Jtot;
     if (ivols_out) B200SV_CUDA(iv.alloc(sizeof(double) * nq));
     if (c.qvar)
       fourier_sum_kernel<<<(unsigned)nq, kFourierThreads, 0, st>>>(lm.as<cd>(), psi.as<cd>(), c.P, rows.as<SumSpec>(), kModeQvar, 0,
                                                                     pr.as<double>());
-    else if (gamma == gamma)
-      fourier_gamma_kernel<<<(unsigned)nq, kFourierThreads, 0, st>>>(lm.as<cd>(), phi.as<cd>(), c.P, rows.as<StrikeSpec>(), gamma,
-                                                                      pr.as<double>());
+    else if (gammas)
+      fourier_gamma_batch_kernel<<<(unsigned)nq, kFourierThreads, 0, st>>>(lm.as<cd>(), phi.as<cd>(), c.P, rows.as<StrikeSpec>(), gammas,
+                                                                            norm_gfwd, pr.as<double>(), iv.as<double>());
     else
       fourier_vanilla_kernel<<<(unsigned)nq, kFourierThreads, 0, st>>>(lm.as<cd>(), phi.as<cd>(), c.P, rows.as<StrikeSpec>(), c.spot ? 1 : 0,
                                                                         1, pr.as<double>(), iv.as<double>());
@@ -2604,14 +2544,51 @@ static int prepare_hawkes_chain(FourierChain& c, const b200sv_hawkes_params* par
   return 0;
 }
 
-// The Hawkes pricing launches of a prepared chain whose maturity increments are in d.dt (price and greeks routes): hawkes_mgf_kernel with
-// A carried over the maturities, then the sums (the gamma slice pricer when gamma is finite; c.ss then holds its normalisers / forwards).
-static int queue_hawkes_prices(ChainDev& d, const FourierChain& c, const HawkesMgfConsts& k, double* prices_out, double gamma = NAN) {
+// The Hawkes pricing launches of a prepared chain (price, greeks and batch routes): the maturity increments go to d.dt, then
+// hawkes_mgf_kernel carries A over the maturities, one launch per set queued back to back (a kernel of its own that read the constants per
+// set from memory contracts its fp64 arithmetic into different fused multiply-adds and moves prices by an ulp, DESIGN.md §9), keeping A in
+// d.a for a single set only; then the sums, the gamma slice pricer when gammas / norm_gfwd (device, see ChainDev::sums) are given.
+static int queue_hawkes_prices(ChainDev& d, const FourierChain& c, const HawkesMgfConsts* k, double* prices_out, double* ivols_out = nullptr,
+                               const double* gammas = nullptr, const double* norm_gfwd = nullptr) {
   if (int rc = d.upload(c)) return rc;
-  B200SV_CUDA(d.a.alloc(sizeof(cd) * (size_t)c.M * c.P * 3));
-  launch_hawkes_mgf(d.st, d.phi.as<cd>(), nullptr, c.P, c.M, d.dt.as<double>(), k, nullptr, d.a.as<cd>(), d.lm.as<cd>(), 0);
-  if (int rc = check_launch("hawkes_mgf_kernel")) return rc;
-  return d.sums(c, prices_out, nullptr, gamma);
+  B200SV_CUDA(d.dt.upload(c.dtaus.data(), c.dtaus.size()));
+  if (!c.batch) B200SV_CUDA(d.a.alloc(sizeof(cd) * (size_t)c.M * c.P * 3));
+  for (int b = 0; b < c.B; ++b) {
+    launch_hawkes_mgf(d.st, d.phi.as<cd>() + (c.per_set_grid ? (size_t)b * c.P : 0), nullptr, c.P, c.M, d.dt.as<double>(), k[b], nullptr,
+                      d.a.as<cd>(), d.lm.as<cd>() + (size_t)b * c.M * c.P, 0);
+    if (int rc = check_launch("hawkes_mgf_kernel")) return rc;
+  }
+  return d.sums(c, prices_out, ivols_out, gammas, norm_gfwd);
+}
+
+// hawkesjd_forwards_under_risk_kernel (:487-515) for B parameter sets k[B] under gammas[B]: two single-point solves per (set, maturity) at
+// phi = -gamma and -gamma - 1, each restarted from A = 0 and integrated over the full maturity ttms[m]; one copy back, then on the host
+// ng [B][M][2] = (normaliser, gamma forward) = (1 / e^{lm(-gamma)}, forwards[m] e^{lm(-gamma - 1)} / e^{lm(-gamma)}).
+static int risk_kernel_normalizers(cudaStream_t st, const HawkesMgfConsts* k, const double* gammas, int B, int M, const double* ttms,
+                                   const double* forwards, std::vector<double>& ng) {
+  std::vector<double> two(4 * (size_t)B, 0.0), lm2(4 * (size_t)B * M);
+  for (int b = 0; b < B; ++b) {
+    two[4 * (size_t)b] = -gammas[b];
+    two[4 * (size_t)b + 2] = -gammas[b] - 1.0;
+  }
+  DevBuf d_ttm(st), d_two(st), d_lm2(st);
+  B200SV_CUDA(d_ttm.upload(ttms, M));
+  B200SV_CUDA(d_two.upload(cplx(two.data()), 2 * (size_t)B));
+  B200SV_CUDA(d_lm2.alloc(sizeof(cd) * 2 * (size_t)B * M));
+  for (int b = 0; b < B; ++b) {
+    launch_hawkes_mgf(st, d_two.as<cd>() + 2 * b, nullptr, 2, M, d_ttm.as<double>(), k[b], nullptr, nullptr, d_lm2.as<cd>() + 2 * (size_t)M * b, 1);
+    if (int rc = check_launch("hawkes_mgf_kernel")) return rc;
+  }
+  B200SV_CUDA(d_lm2.download(cplx(lm2.data()), 2 * (size_t)B * M));
+  B200SV_CUDA(cudaStreamSynchronize(st));
+  ng.resize(2 * (size_t)B * M);
+  for (int b = 0; b < B; ++b)
+    for (int m = 0; m < M; ++m) {                                            // log_mgf layout [b][m][point]
+      const size_t s = (size_t)b * M + m;
+      ng[2 * s] = 1.0 / std::exp(lm2[2 * (2 * s + 0)]);
+      ng[2 * s + 1] = forwards[m] * std::exp(lm2[2 * (2 * s + 1)]) * ng[2 * s];
+    }
+  return 0;
 }
 
 // Validation of b200sv_hawkesjd_price_chain_batch: sizes, the risk-premia gammas (all finite), then the chain.  The grids follow
@@ -2680,15 +2657,32 @@ static int fourier_sum_host(const double* log_mgf, const double* grid, int P, co
   });
 }
 
-// The first-order sensitivity launches of a prepared LogSV chain (b200sv_logsv_price_chain_greeks and _hessian): the pricing launches,
-// logsv_mgf_tangent_kernel and, on a non-empty chain, fourier_vanilla_greeks_kernel.  dspec, the tangent kernel's primal log-MGF (lm), its
-// tangents (dlm), nfev and the greeks stay on the device for the launches that follow; download() queues the copies and synchronises.
-struct LogsvGreeksDev {
-  DevBuf dspec, dlm, lm, nfev, g;
-  explicit LogsvGreeksDev(cudaStream_t s) : dspec(s), dlm(s), lm(s), nfev(s), g(s) {}
+// The first-order Fourier sums of a prepared chain (b200sv_*_price_chain_greeks, and the LogSV / Heston _hessian): the tangent kernel
+// writes dlm [NP][M][P] (and, for LogSV and Hawkes, its own primal log-MGF lm [M][P] and nfev [P]); sums() queues
+// fourier_vanilla_greeks_kernel on the log-MGF it is given, and dlm and the greeks [2 + NP][J] stay on the device for the launches that
+// follow; download() queues the copies and synchronises.
+template <int NP>
+struct GreeksDev {
+  DevBuf dlm, lm, nfev, g;
+  explicit GreeksDev(cudaStream_t s) : dlm(s), lm(s), nfev(s), g(s) {}
 
+  int alloc(const FourierChain& c, bool primal) {
+    B200SV_CUDA(dlm.alloc(sizeof(cd) * (size_t)NP * c.M * c.P));
+    if (primal) {
+      B200SV_CUDA(lm.alloc(sizeof(cd) * (size_t)c.M * c.P));
+      B200SV_CUDA(nfev.alloc(sizeof(int) * c.P));
+    }
+    B200SV_CUDA(g.alloc(sizeof(double) * (size_t)(2 + NP) * c.ss.size()));
+    return 0;
+  }
+  // no launch on an empty chain
+  int sums(const ChainDev& d, const FourierChain& c, const cd* log_mgf) {
+    if (c.Jtot == 0) return 0;
+    fourier_vanilla_greeks_kernel<NP><<<c.Jtot, kFourierThreads, 0, d.st>>>(log_mgf, dlm.as<cd>(), d.phi.as<cd>(), c.P, c.M,
+                                                                            d.rows.as<StrikeSpec>(), c.spot ? 1 : 0, g.as<double>());
+    return check_launch("fourier_vanilla_greeks_kernel");
+  }
   int download(ChainDev& d, const FourierChain& c, double* greeks_out, double* dlog_mgf_out, int* nfev_out) {
-    constexpr int NP = 1 + kLogsvOdeDirs;
     if (c.Jtot > 0) B200SV_CUDA(g.download(greeks_out, (size_t)(2 + NP) * c.Jtot));
     B200SV_CUDA(dlm.download(cplx(dlog_mgf_out), (size_t)NP * c.M * c.P));
     B200SV_CUDA(nfev.download(nfev_out, c.P));
@@ -2696,9 +2690,11 @@ struct LogsvGreeksDev {
   }
 };
 
-static int queue_logsv_greeks(ChainDev& d, LogsvGreeksDev& t, const FourierChain& c, const b200sv_logsv_params* params, const double* etas,
-                              int expansion_order, double* prices_out) {
-  const int N = expansion_order == B200SV_ORDER_FIRST ? 3 : 5, NP = 1 + kLogsvOdeDirs, M = c.M, P = c.P;
+// The first-order sensitivity launches of a prepared LogSV chain: the pricing launches, logsv_mgf_tangent_kernel on the model tangents
+// d.dspec (which the Hessian kernel reads too), then the sums on the tangent kernel's own primal log-MGF (DESIGN.md §4.2).
+static int queue_logsv_greeks(ChainDev& d, GreeksDev<1 + kLogsvOdeDirs>& t, const FourierChain& c, const b200sv_logsv_params* params,
+                              const double* etas, int expansion_order, double* prices_out) {
+  const int N = expansion_order == B200SV_ORDER_FIRST ? 3 : 5, M = c.M, P = c.P;
   std::vector<LogsvModelTangent> dspec((size_t)M * kLogsvOdeDirs);
   for (int m = 0; m < M; ++m) {
     LogsvModelTangent tg[kLogsvOdeDirs];
@@ -2706,51 +2702,48 @@ static int queue_logsv_greeks(ChainDev& d, LogsvGreeksDev& t, const FourierChain
     std::copy(tg, tg + kLogsvOdeDirs, dspec.begin() + (size_t)m * kLogsvOdeDirs);
   }
   if (int rc = queue_logsv_prices(d, c, params, etas, N, prices_out, nullptr)) return rc;
-  B200SV_CUDA(t.dspec.upload(dspec.data(), dspec.size()));
-  B200SV_CUDA(t.dlm.alloc(sizeof(cd) * (size_t)NP * M * P));
-  B200SV_CUDA(t.lm.alloc(sizeof(cd) * (size_t)M * P));
-  B200SV_CUDA(t.nfev.alloc(sizeof(int) * P));
-  B200SV_CUDA(t.g.alloc(sizeof(double) * (size_t)(2 + NP) * c.ss.size()));
+  B200SV_CUDA(d.dspec.upload(dspec.data(), dspec.size()));
+  if (int rc = t.alloc(c, true)) return rc;
   const auto tangent = N == 5 ? logsv_mgf_tangent_kernel<5> : logsv_mgf_tangent_kernel<3>;
   tangent<<<(P * kLogsvOdeDirs + kTangentTPB - 1) / kTangentTPB, kTangentTPB, 0, d.st>>>(d.phi.as<cd>(), P, M, d.spec.as<ChainSpec>(),
-                                                                                       t.dspec.as<LogsvModelTangent>(),
+                                                                                       d.dspec.as<LogsvModelTangent>(),
                                                                                        params->sigma0 - params->theta, t.dlm.as<cd>(),
                                                                                        t.lm.as<cd>(), nullptr, t.nfev.as<int>());
   if (int rc = check_launch("logsv_mgf_tangent_kernel")) return rc;
-  if (c.Jtot > 0) {       // the tangent kernel's own primal log-MGF (DESIGN.md §4.2)
-    fourier_vanilla_greeks_kernel<1 + kLogsvOdeDirs><<<c.Jtot, kFourierThreads, 0, d.st>>>(t.lm.as<cd>(), t.dlm.as<cd>(), d.phi.as<cd>(), P, M,
-                                                                                         d.rows.as<StrikeSpec>(), c.spot ? 1 : 0,
-                                                                                         t.g.as<double>());
-    if (int rc = check_launch("fourier_vanilla_greeks_kernel")) return rc;
-  }
-  return 0;
+  return t.sums(d, c, t.lm.as<cd>());
 }
 
-// The Heston twin: the pricing launches, heston_mgf_tangent_kernel and fourier_vanilla_greeks_kernel; dlm and the greeks stay on the device.
-struct HestonGreeksDev {
-  DevBuf dlm, g;
-  explicit HestonGreeksDev(cudaStream_t s) : dlm(s), g(s) {}
-
-  int download(ChainDev& d, const FourierChain& c, double* greeks_out, double* dlog_mgf_out) {
-    constexpr int NP = 1 + kHestonOdeDirs;
-    if (c.Jtot > 0) B200SV_CUDA(g.download(greeks_out, (size_t)(2 + NP) * c.Jtot));
-    B200SV_CUDA(dlm.download(cplx(dlog_mgf_out), (size_t)NP * c.M * c.P));
-    return d.sync.done();
-  }
-};
-
-static int queue_heston_greeks(ChainDev& d, HestonGreeksDev& t, const FourierChain& c, const b200sv_heston_params* params, double* prices_out) {
-  const int NP = 1 + kHestonOdeDirs, M = c.M, P = c.P;
+// The Heston twin: the pricing launches, heston_mgf_tangent_kernel, then the sums on the pricing launch's log-MGF (heston_mgf_kernel is a
+// per-thread closed form, the same for any block size).
+static int queue_heston_greeks(ChainDev& d, GreeksDev<1 + kHestonOdeDirs>& t, const FourierChain& c, const b200sv_heston_params* params,
+                               double* prices_out) {
   if (int rc = queue_heston_prices(d, c, params, prices_out, nullptr)) return rc;
-  B200SV_CUDA(t.dlm.alloc(sizeof(cd) * (size_t)NP * M * P));
-  B200SV_CUDA(t.g.alloc(sizeof(double) * (size_t)(2 + NP) * c.ss.size()));
-  heston_mgf_tangent_kernel<<<(P * kHestonOdeDirs + 63) / 64, 64, 0, d.st>>>(d.phi.as<cd>(), P, M, d.dt.as<double>(), *params, t.dlm.as<cd>());
+  if (int rc = t.alloc(c, false)) return rc;
+  heston_mgf_tangent_kernel<<<(c.P * kHestonOdeDirs + 63) / 64, 64, 0, d.st>>>(d.phi.as<cd>(), c.P, c.M, d.dt.as<double>(), *params,
+                                                                               t.dlm.as<cd>());
   if (int rc = check_launch("heston_mgf_tangent_kernel")) return rc;
-  if (c.Jtot > 0) {       // the pricing launch's log-MGF: heston_mgf_kernel is a per-thread closed form, the same for any block size
-    fourier_vanilla_greeks_kernel<1 + kHestonOdeDirs><<<c.Jtot, kFourierThreads, 0, d.st>>>(d.lm.as<cd>(), t.dlm.as<cd>(), d.phi.as<cd>(), P, M,
-                                                                                          d.rows.as<StrikeSpec>(), 1, t.g.as<double>());
-    if (int rc = check_launch("fourier_vanilla_greeks_kernel")) return rc;
+  return t.sums(d, c, d.lm.as<cd>());
+}
+
+// The second-order sums of b200sv_*_price_chain_hessian after its Hessian kernel wrote d2lm [NH][M][P]: fourier_vanilla_hessian_kernel on
+// log_mgf and the first-order tangents dlm [NP][M][P] (no launch on an empty chain), then vanna, the Hessian rows and d2lm come back; the
+// first-order outputs follow with GreeksDev::download().
+template <int NP>
+static int queue_hessian_sums(ChainDev& d, const FourierChain& c, const cd* log_mgf, const cd* dlm, const DevBuf& d2lm, double* vanna_out,
+                              double* hessian_out, double* d2log_mgf_out) {
+  constexpr int NH = NP * (NP + 1) / 2;
+  DevBuf d_v(d.st), d_h(d.st);
+  if (c.Jtot > 0) {
+    B200SV_CUDA(d_v.alloc(sizeof(double) * (size_t)NP * c.Jtot));
+    B200SV_CUDA(d_h.alloc(sizeof(double) * (size_t)NH * c.Jtot));
+    fourier_vanilla_hessian_kernel<NP><<<c.Jtot, kFourierThreads, 0, d.st>>>(log_mgf, dlm, d2lm.as<cd>(), d.phi.as<cd>(), c.P, c.M,
+                                                                             d.rows.as<StrikeSpec>(), c.spot ? 1 : 0, d_v.as<double>(),
+                                                                             d_h.as<double>());
+    if (int rc = check_launch("fourier_vanilla_hessian_kernel")) return rc;
+    B200SV_CUDA(d_v.download(vanna_out, (size_t)NP * c.Jtot));
+    B200SV_CUDA(d_h.download(hessian_out, (size_t)NH * c.Jtot));
   }
+  B200SV_CUDA(d2lm.download(cplx(d2log_mgf_out), (size_t)NH * c.M * c.P));
   return 0;
 }
 
@@ -2809,7 +2802,7 @@ int b200sv_logsv_price_chain_greeks(const b200sv_logsv_params* params, int M, co
                                    expansion_order, vol_scaler, P))
     return rc;
   ChainDev d;
-  LogsvGreeksDev g(d.st);
+  GreeksDev<1 + kLogsvOdeDirs> g(d.st);
   if (int rc = queue_logsv_greeks(d, g, c, params, etas, expansion_order, prices_out)) return rc;
   return g.download(d, c, greeks_out, dlog_mgf_out, nfev_out);
 }
@@ -2823,9 +2816,9 @@ int b200sv_heston_price_chain_greeks(const b200sv_heston_params* params, int M, 
   FourierChain c;
   if (int rc = prepare_heston_chain(c, params, M, ttms, forwards, discfactors, offsets, strikes, types, variable_type, vol_scaler, P)) return rc;
   ChainDev d;
-  HestonGreeksDev g(d.st);
+  GreeksDev<1 + kHestonOdeDirs> g(d.st);
   if (int rc = queue_heston_greeks(d, g, c, params, prices_out)) return rc;
-  return g.download(d, c, greeks_out, dlog_mgf_out);
+  return g.download(d, c, greeks_out, dlog_mgf_out, nullptr);
 }
 
 /* ---- second-order forward-mode sensitivities of the two Fourier chain pricers (DESIGN.md §4.4) ----
@@ -2843,7 +2836,7 @@ int b200sv_logsv_price_chain_hessian(const b200sv_logsv_params* params, int M, c
                                    expansion_order, vol_scaler, P))
     return rc;
   ChainDev d;
-  LogsvGreeksDev g(d.st);
+  GreeksDev<1 + kLogsvOdeDirs> g(d.st);
   if (int rc = queue_logsv_greeks(d, g, c, params, etas, expansion_order, prices_out)) return rc;
   const int N = expansion_order == B200SV_ORDER_FIRST ? 3 : 5, NP = 1 + kLogsvOdeDirs, NH = NP * (NP + 1) / 2;
   P = c.P;
@@ -2853,26 +2846,17 @@ int b200sv_logsv_price_chain_hessian(const b200sv_logsv_params* params, int M, c
     make_model_hessian(*params, etas ? etas[m] : 1.0, c.spot, h);
     std::copy(h, h + kLogsvOdePairs, d2spec.begin() + (size_t)m * kLogsvOdePairs);
   }
-  DevBuf d_d2spec(d.st), d_d2lm(d.st), d_v(d.st), d_h(d.st);
+  DevBuf d_d2spec(d.st), d_d2lm(d.st);
   B200SV_CUDA(d_d2spec.upload(d2spec.data(), d2spec.size()));
   B200SV_CUDA(d_d2lm.alloc(sizeof(cd) * (size_t)NH * M * P));
-  B200SV_CUDA(d_v.alloc(sizeof(double) * (size_t)NP * c.ss.size()));
-  B200SV_CUDA(d_h.alloc(sizeof(double) * (size_t)NH * c.ss.size()));
   const auto hessian = N == 5 ? logsv_mgf_hessian_kernel<5> : logsv_mgf_hessian_kernel<3>;
   hessian<<<(P * kLogsvOdePairs + kHessianTPB - 1) / kHessianTPB, kHessianTPB, 0, d.st>>>(d.phi.as<cd>(), P, M, d.spec.as<ChainSpec>(),
-                                                                                        g.dspec.as<LogsvModelTangent>(),
+                                                                                        d.dspec.as<LogsvModelTangent>(),
                                                                                         d_d2spec.as<LogsvModelTangent>(),
                                                                                         params->sigma0 - params->theta, d_d2lm.as<cd>());
   if (int rc = check_launch("logsv_mgf_hessian_kernel")) return rc;
-  if (c.Jtot > 0) {       // the tangent kernel's primal log-MGF and tangents, as for the first-order rows
-    fourier_vanilla_hessian_kernel<NP><<<c.Jtot, kFourierThreads, 0, d.st>>>(g.lm.as<cd>(), g.dlm.as<cd>(), d_d2lm.as<cd>(), d.phi.as<cd>(), P,
-                                                                             M, d.rows.as<StrikeSpec>(), c.spot ? 1 : 0, d_v.as<double>(),
-                                                                             d_h.as<double>());
-    if (int rc = check_launch("fourier_vanilla_hessian_kernel")) return rc;
-    B200SV_CUDA(d_v.download(vanna_out, (size_t)NP * c.Jtot));
-    B200SV_CUDA(d_h.download(hessian_out, (size_t)NH * c.Jtot));
-  }
-  B200SV_CUDA(d_d2lm.download(cplx(d2log_mgf_out), (size_t)NH * M * P));
+  // the tangent kernel's primal log-MGF and tangents, as for the first-order rows
+  if (int rc = queue_hessian_sums<NP>(d, c, g.lm.as<cd>(), g.dlm.as<cd>(), d_d2lm, vanna_out, hessian_out, d2log_mgf_out)) return rc;
   return g.download(d, c, greeks_out, dlog_mgf_out, nfev_out);
 }
 
@@ -2885,25 +2869,16 @@ int b200sv_heston_price_chain_hessian(const b200sv_heston_params* params, int M,
   FourierChain c;
   if (int rc = prepare_heston_chain(c, params, M, ttms, forwards, discfactors, offsets, strikes, types, variable_type, vol_scaler, P)) return rc;
   ChainDev d;
-  HestonGreeksDev g(d.st);
+  GreeksDev<1 + kHestonOdeDirs> g(d.st);
   if (int rc = queue_heston_greeks(d, g, c, params, prices_out)) return rc;
   const int NP = 1 + kHestonOdeDirs, NH = NP * (NP + 1) / 2;
   P = c.P;
-  DevBuf d_d2lm(d.st), d_v(d.st), d_h(d.st);
+  DevBuf d_d2lm(d.st);
   B200SV_CUDA(d_d2lm.alloc(sizeof(cd) * (size_t)NH * M * P));
-  B200SV_CUDA(d_v.alloc(sizeof(double) * (size_t)NP * c.ss.size()));
-  B200SV_CUDA(d_h.alloc(sizeof(double) * (size_t)NH * c.ss.size()));
   heston_mgf_hessian_kernel<<<(P * kHestonOdePairs + 63) / 64, 64, 0, d.st>>>(d.phi.as<cd>(), P, M, d.dt.as<double>(), *params, d_d2lm.as<cd>());
   if (int rc = check_launch("heston_mgf_hessian_kernel")) return rc;
-  if (c.Jtot > 0) {
-    fourier_vanilla_hessian_kernel<NP><<<c.Jtot, kFourierThreads, 0, d.st>>>(d.lm.as<cd>(), g.dlm.as<cd>(), d_d2lm.as<cd>(), d.phi.as<cd>(), P,
-                                                                             M, d.rows.as<StrikeSpec>(), 1, d_v.as<double>(), d_h.as<double>());
-    if (int rc = check_launch("fourier_vanilla_hessian_kernel")) return rc;
-    B200SV_CUDA(d_v.download(vanna_out, (size_t)NP * c.Jtot));
-    B200SV_CUDA(d_h.download(hessian_out, (size_t)NH * c.Jtot));
-  }
-  B200SV_CUDA(d_d2lm.download(cplx(d2log_mgf_out), (size_t)NH * M * P));
-  return g.download(d, c, greeks_out, dlog_mgf_out);
+  if (int rc = queue_hessian_sums<NP>(d, c, d.lm.as<cd>(), g.dlm.as<cd>(), d_d2lm, vanna_out, hessian_out, d2log_mgf_out)) return rc;
+  return g.download(d, c, greeks_out, dlog_mgf_out, nullptr);
 }
 
 /* ---- batched chain pricers: B parameter sets on one chain in one pass (calibration objective + its finite-difference gradient) ----
@@ -2952,35 +2927,21 @@ int b200sv_hawkesjd_price_chain(const b200sv_hawkes_params* params, int M, const
   P = c.P;
   const HawkesMgfConsts k = make_hawkes_mgf_consts(*params);
   ChainDev d;
-  std::vector<double> dts(c.dtaus);
-  dts.insert(dts.end(), ttms, ttms + M);                                        // [increments | full maturities]
-  B200SV_CUDA(d.dt.upload(dts.data(), dts.size()));
-  std::vector<double> normalizers(M, 1.0), gamma_forwards(M, 1.0);
-  if (with_gamma) {                                                            // hawkesjd_forwards_under_risk_kernel (:487-515)
-    const double two[4] = {-risk_premia_gamma, 0.0, -risk_premia_gamma - 1.0, 0.0};
-    DevBuf d_two(d.st), d_lm2(d.st);
-    B200SV_CUDA(d_two.upload(cplx(two), 2));
-    B200SV_CUDA(d_lm2.alloc(sizeof(cd) * 2 * (size_t)M));
-    launch_hawkes_mgf(d.st, d_two.as<cd>(), nullptr, 2, M, d.dt.as<double>() + M, k, nullptr, nullptr, d_lm2.as<cd>(), 1);
-    if (int rc = check_launch("hawkes_mgf_kernel")) return rc;
-    std::vector<double> lm2(4 * (size_t)M);
-    B200SV_CUDA(cudaMemcpyAsync(lm2.data(), d_lm2.p, sizeof(cd) * 2 * M, cudaMemcpyDeviceToHost, d.st));
-    B200SV_CUDA(cudaStreamSynchronize(d.st));
-    for (int m = 0; m < M; ++m) {                                              // log_mgf layout [m][point]
-      normalizers[m] = 1.0 / std::exp(lm2[2 * (2 * (size_t)m + 0)]);
-      gamma_forwards[m] = forwards[m] * std::exp(lm2[2 * (2 * (size_t)m + 1)]) * normalizers[m];
-    }
-    for (int j = 0; j < c.Jtot; ++j) {                                          // the gamma slice pricer's discfactor / forward slots
-      c.ss[j].discfactor = normalizers[c.ss[j].slice];
-      c.ss[j].ttm = gamma_forwards[c.ss[j].slice];
-    }
+  DevBuf d_gam(d.st), d_ng(d.st);
+  std::vector<double> ng(2 * (size_t)M, 1.0);                                   // [M][2] (normaliser, gamma forward), 1 without the kernel
+  if (with_gamma) {
+    if (int rc = risk_kernel_normalizers(d.st, &k, &risk_premia_gamma, 1, M, ttms, forwards, ng)) return rc;
+    B200SV_CUDA(d_gam.upload(&risk_premia_gamma, 1));
+    B200SV_CUDA(d_ng.upload(ng.data(), ng.size()));
   }
-  if (int rc = queue_hawkes_prices(d, c, k, prices_out, risk_premia_gamma)) return rc;
+  if (int rc = queue_hawkes_prices(d, c, &k, prices_out, nullptr, d_gam.as<double>(), d_ng.as<double>())) return rc;
   B200SV_CUDA(d.a.download(cplx(a_out), (size_t)M * P * 3));
   B200SV_CUDA(d.lm.download(cplx(log_mgf_out), (size_t)M * P));
   if (int rc = d.sync.done()) return rc;
-  if (normalizers_out) std::copy(normalizers.begin(), normalizers.end(), normalizers_out);
-  if (gamma_forwards_out) std::copy(gamma_forwards.begin(), gamma_forwards.end(), gamma_forwards_out);
+  for (int m = 0; m < M; ++m) {
+    if (normalizers_out) normalizers_out[m] = ng[2 * (size_t)m];
+    if (gamma_forwards_out) gamma_forwards_out[m] = ng[2 * (size_t)m + 1];
+  }
   return 0;
 }
 
@@ -2995,29 +2956,16 @@ int b200sv_hawkesjd_price_chain_greeks(const b200sv_hawkes_params* params, int M
   FourierChain c;
   if (int rc = prepare_hawkes_chain(c, params, M, ttms, forwards, discfactors, offsets, strikes, types, is_spot_measure, vol_scaler, P, NAN))
     return rc;
-  constexpr int NP = kHawkesGreekParams;
-  P = c.P;
   const HawkesMgfConsts k = make_hawkes_mgf_consts(*params);
   ChainDev d;
-  B200SV_CUDA(d.dt.upload(c.dtaus.data(), c.dtaus.size()));
-  if (int rc = queue_hawkes_prices(d, c, k, prices_out)) return rc;
-  DevBuf d_dlm(d.st), d_lm(d.st), d_nfev(d.st), d_g(d.st);
-  B200SV_CUDA(d_dlm.alloc(sizeof(cd) * (size_t)NP * M * P));
-  B200SV_CUDA(d_lm.alloc(sizeof(cd) * (size_t)M * P));
-  B200SV_CUDA(d_nfev.alloc(sizeof(int) * P));
-  B200SV_CUDA(d_g.alloc(sizeof(double) * (size_t)(2 + NP) * c.ss.size()));
-  launch_hawkes_mgf_tangent(d.st, d.phi.as<cd>(), P, M, d.dt.as<double>(), k, make_hawkes_tangents(*params), d_dlm.as<cd>(), d_lm.as<cd>(),
-                            d_nfev.as<int>());
+  if (int rc = queue_hawkes_prices(d, c, &k, prices_out)) return rc;
+  GreeksDev<kHawkesGreekParams> g(d.st);
+  if (int rc = g.alloc(c, true)) return rc;
+  launch_hawkes_mgf_tangent(d.st, d.phi.as<cd>(), c.P, M, d.dt.as<double>(), k, make_hawkes_tangents(*params), g.dlm.as<cd>(), g.lm.as<cd>(),
+                            g.nfev.as<int>());
   if (int rc = check_launch("hawkes_mgf_tangent_kernel")) return rc;
-  if (c.Jtot > 0) {       // the tangent kernel's own primal log-MGF, on the mesh the tangents were stepped on
-    fourier_vanilla_greeks_kernel<NP><<<c.Jtot, kFourierThreads, 0, d.st>>>(d_lm.as<cd>(), d_dlm.as<cd>(), d.phi.as<cd>(), P, M,
-                                                                            d.rows.as<StrikeSpec>(), c.spot ? 1 : 0, d_g.as<double>());
-    if (int rc = check_launch("fourier_vanilla_greeks_kernel")) return rc;
-    B200SV_CUDA(d_g.download(greeks_out, (size_t)(2 + NP) * c.Jtot));
-  }
-  B200SV_CUDA(d_dlm.download(cplx(dlog_mgf_out), (size_t)NP * M * P));
-  B200SV_CUDA(d_nfev.download(nfev_out, P));
-  return d.sync.done();
+  if (int rc = g.sums(d, c, g.lm.as<cd>())) return rc;     // the tangent kernel's own primal log-MGF, on the mesh the tangents were stepped on
+  return g.download(d, c, greeks_out, dlog_mgf_out, nfev_out);
 }
 
 /* B Hawkes parameter sets on one chain in one pass (the calibration drivers' objective and its finite-difference neighbours).  The Riccati
@@ -3035,56 +2983,17 @@ int b200sv_hawkesjd_price_chain_batch(const b200sv_hawkes_params* params, int B,
   if (int rc = prepare_hawkes_batch(c, params, B, M, ttms, forwards, discfactors, offsets, strikes, types, is_spot_measure, vol_scaler, P,
                                     gammas))
     return rc;
-  P = c.P;
   std::vector<HawkesMgfConsts> k(B);
   for (int b = 0; b < B; ++b) k[b] = make_hawkes_mgf_consts(params[b]);
   ChainDev d;
   DevBuf d_gam(d.st), d_ng(d.st);
-  std::vector<double> dts(c.dtaus);
-  dts.insert(dts.end(), ttms, ttms + M);                                        // [increments | full maturities]
-  B200SV_CUDA(d.dt.upload(dts.data(), dts.size()));
-  if (gammas) {                                                                // hawkesjd_forwards_under_risk_kernel (:487-515), per set
-    std::vector<double> two(4 * (size_t)B, 0.0), lm2(4 * (size_t)B * M), ng(2 * (size_t)B * M);
-    for (int b = 0; b < B; ++b) {
-      two[4 * (size_t)b] = -gammas[b];
-      two[4 * (size_t)b + 2] = -gammas[b] - 1.0;
-    }
-    DevBuf d_two(d.st), d_lm2(d.st);
-    B200SV_CUDA(d_two.upload(cplx(two.data()), 2 * (size_t)B));
-    B200SV_CUDA(d_lm2.alloc(sizeof(cd) * 2 * (size_t)B * M));
-    for (int b = 0; b < B; ++b) {
-      launch_hawkes_mgf(d.st, d_two.as<cd>() + 2 * b, nullptr, 2, M, d.dt.as<double>() + M, k[b], nullptr, nullptr, d_lm2.as<cd>() + 2 * (size_t)M * b, 1);
-      if (int rc = check_launch("hawkes_mgf_kernel")) return rc;
-    }
-    B200SV_CUDA(d_lm2.download(cplx(lm2.data()), 2 * (size_t)B * M));
-    B200SV_CUDA(cudaStreamSynchronize(d.st));
-    for (int b = 0; b < B; ++b)
-      for (int m = 0; m < M; ++m) {                                            // log_mgf layout [b][m][point]
-        const size_t s = (size_t)b * M + m;
-        ng[2 * s] = 1.0 / std::exp(lm2[2 * (2 * s + 0)]);
-        ng[2 * s + 1] = forwards[m] * std::exp(lm2[2 * (2 * s + 1)]) * ng[2 * s];
-      }
+  if (gammas) {
+    std::vector<double> ng;
+    if (int rc = risk_kernel_normalizers(d.st, k.data(), gammas, B, M, ttms, forwards, ng)) return rc;
     B200SV_CUDA(d_ng.upload(ng.data(), ng.size()));
     B200SV_CUDA(d_gam.upload(gammas, (size_t)B));
   }
-  if (int rc = d.upload(c)) return rc;
-  for (int b = 0; b < B; ++b) {
-    launch_hawkes_mgf(d.st, d.phi.as<cd>() + (c.per_set_grid ? (size_t)b * P : 0), nullptr, P, M, d.dt.as<double>(), k[b], nullptr, nullptr,
-                      d.lm.as<cd>() + (size_t)b * M * P, 0);
-    if (int rc = check_launch("hawkes_mgf_kernel")) return rc;
-  }
-  if (!gammas) {
-    if (int rc = d.sums(c, prices_out, ivols_out)) return rc;
-    return d.sync.done();
-  }
-  const size_t nq = (size_t)B * c.Jtot;
-  if (ivols_out) B200SV_CUDA(d.iv.alloc(sizeof(double) * nq));
-  fourier_gamma_batch_kernel<<<(unsigned)nq, kFourierThreads, 0, d.st>>>(d.lm.as<cd>(), d.phi.as<cd>(), P, d.rows.as<StrikeSpec>(),
-                                                                         d_gam.as<double>(), d_ng.as<double>(), d.pr.as<double>(),
-                                                                         d.iv.as<double>());
-  if (int rc = check_launch("fourier_gamma_batch_kernel")) return rc;
-  B200SV_CUDA(d.pr.download(prices_out, nq));
-  B200SV_CUDA(d.iv.download(ivols_out, nq));
+  if (int rc = queue_hawkes_prices(d, c, k.data(), prices_out, ivols_out, d_gam.as<double>(), d_ng.as<double>())) return rc;
   return d.sync.done();
 }
 
@@ -3248,10 +3157,14 @@ int b200sv_fourier_gamma(const double* log_mgf, const double* phi, int P, double
   B200SV_REQUIRE(P >= 3 && J >= 1, "P >= 3, J >= 1");
   if (int rc = check_gamma_types(types, J, is_spot_measure != 0)) return rc;
   std::vector<StrikeSpec> ss(J);
-  for (int j = 0; j < J; ++j) ss[j] = StrikeSpec{strikes[j], forward, normalizer, (int)types[j], 0, gamma_forward, 0};
+  for (int j = 0; j < J; ++j) ss[j] = StrikeSpec{strikes[j], forward, 1.0, (int)types[j], 0, 1.0, 0};
+  const double ng[2] = {normalizer, gamma_forward};
   return run_sums(log_mgf, phi, P, ss, prices_out, [&](cudaStream_t st, unsigned n, const cd* lm, const cd* g, const StrikeSpec* s, double* pr) {
-    fourier_gamma_kernel<<<n, kFourierThreads, 0, st>>>(lm, g, P, s, risk_premia_gamma, pr);
-    return check_launch("fourier_gamma_kernel");
+    DevBuf d_gam(st), d_ng(st);
+    B200SV_CUDA(d_gam.upload(&risk_premia_gamma, 1));
+    B200SV_CUDA(d_ng.upload(ng, 2));
+    fourier_gamma_batch_kernel<<<n, kFourierThreads, 0, st>>>(lm, g, P, s, d_gam.as<double>(), d_ng.as<double>(), pr, nullptr);
+    return check_launch("fourier_gamma_batch_kernel");
   });
 }
 
