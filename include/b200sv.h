@@ -335,6 +335,15 @@ int b200sv_hawkesjd_price_chain_greeks(const b200sv_hawkes_params* params, int M
                                        const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
                                        int is_spot_measure, double vol_scaler, int P, double* prices_out, double* greeks_out,
                                        double* dlog_mgf_out, int* nfev_out);
+/* second-order sensitivities of the Hawkes Fourier chain without a risk kernel (DESIGN.md §4.5).  The arguments and outputs of
+ * b200sv_hawkesjd_price_chain_greeks (bit-identical to it), then vanna_out [15][J]: d^2 price / d forwards[m] d parameter, and
+ * hessian_out [120][J]: d^2 price / d p d q for p <= q, the upper triangle row-major in that parameter order ((0,0), (0,1), .., (0,14),
+ * (1,1), ..).  Optional (may be NULL): d2log_mgf_out [120][M][P] complex128 interleaved, the second parameter derivatives of the log-MGF
+ * grid in the same order.  Exact derivatives of the scheme on the first-order route's mesh. */
+int b200sv_hawkesjd_price_chain_hessian(const b200sv_hawkes_params* params, int M, const double* ttms, const double* forwards,
+                                        const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
+                                        int is_spot_measure, double vol_scaler, int P, double* prices_out, double* greeks_out,
+                                        double* dlog_mgf_out, int* nfev_out, double* vanna_out, double* hessian_out, double* d2log_mgf_out);
 /* compute_hawkes_a_mgf_grid / solve_a_ode_grid (pricers/hawkes_jd_pricer.py:518-579) on caller-supplied transform grids (complex128 as interleaved
  * doubles; psi may be NULL = zeros): a_inout [P][3] holds A(0) on entry and A(dtau) on return, log_mgf_out [P] = a0 + a_p lambda_p + a_m lambda_m */
 int b200sv_hawkesjd_mgf_grid(const double* phi, const double* psi, int P, double dtau, double* a_inout, const b200sv_hawkes_params* params,

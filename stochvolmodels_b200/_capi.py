@@ -129,6 +129,8 @@ SIGNATURES = {
     "b200sv_logsv_price_chain_hessian": [_lp, c_int, _dp, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_int, c_int, c_double, c_int, _dp, _dp, _dp, _ip,
                                          _dp, _dp, _dp],
     "b200sv_heston_price_chain_hessian": [_hp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_double, c_int, _dp, _dp, _dp, _dp, _dp, _dp],
+    "b200sv_hawkesjd_price_chain_hessian": [_kp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_double, c_int, _dp, _dp, _dp, _ip, _dp, _dp,
+                                            _dp],
     "b200sv_logsv_price_chain_batch": [_lp, c_int, c_int, _dp, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_int, c_double, c_int, _dp, _dp],
     "b200sv_heston_price_chain_batch": [_hp, c_int, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_double, c_int, _dp, _dp],
     "b200sv_hawkesjd_price_chain_batch": [_kp, c_int, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_double, c_int, _dp, _dp, _dp],

@@ -1681,6 +1681,166 @@ __global__ void __launch_bounds__(kFourierThreads) fourier_vanilla_hessian_kerne
   }
 }
 
+// fourier_vanilla_hessian_kernel for many parameters: at NP = 15 its 2NP + NP(NP+1)/2 = 150 sums per thread do not stay in registers, so
+// a strike's rows are split over the CTAs blockIdx.y = 0 .. NH / NP, every CTA recomputing e^z.  blockIdx.y = 0: the 2NP vanna sums S_p,
+// S_xp; blockIdx.y = c > 0: the NP Hessian rows [(c - 1) NP, c NP).  Each row is the same fixed-order block_sum, NaN-skipping and
+// assembly as there.
+template <int NP>
+__global__ void __launch_bounds__(kFourierThreads) fourier_vanilla_hessian_split_kernel(const cd* __restrict__ log_mgf,
+                                                                                       const cd* __restrict__ dlog_mgf,
+                                                                                       const cd* __restrict__ d2log_mgf,
+                                                                                       const cd* __restrict__ phi, int P, int M,
+                                                                                       const StrikeSpec* __restrict__ specs, int is_spot,
+                                                                                       double* __restrict__ vanna, double* __restrict__ hessian) {
+  constexpr int NH = NP * (NP + 1) / 2, R = NP;       // Hessian rows per CTA
+  const StrikeSpec sp = specs[blockIdx.x];
+  const cd* lm = log_mgf + (size_t)sp.slice * P;
+  const double x = log(sp.forward / sp.strike);
+  const size_t rs = (size_t)M * P;                     // the row stride of dlog_mgf / d2log_mgf
+  const cd* dl = dlog_mgf + (size_t)sp.slice * P;
+  const cd* d2l = d2log_mgf + (size_t)sp.slice * P;
+  const bool vanna_rows = blockIdx.y == 0;
+  const int r0 = vanna_rows ? 0 : ((int)blockIdx.y - 1) * R;
+  int p0 = 0, q0 = 0;
+  if (!vanna_rows) tri_pair(r0, NP, p0, q0);
+  double acc[2 * NP] = {};
+  strike_sum(phi, P, acc, [&](int j, double dp, cd ph) {
+    const double w = (dp / M_PI) / (ph.im * ph.im + 0.25);
+    const cd e = exp_(lm[j] - x * ph);
+    const cd term = mk(w) * e;
+    if (term.re == term.re) {
+      if (vanna_rows) {
+#pragma unroll
+        for (int k = 0; k < NP; ++k) {
+          const cd ed = e * dl[k * rs + j];
+          acc[k] += w * ed.re;
+          acc[NP + k] += w * (-(ph * ed)).re;
+        }
+      } else {
+        int p = p0, q = q0;
+#pragma unroll
+        for (int i = 0; i < R; ++i) {
+          const int r = r0 + i;
+          if (r < NH) acc[i] += w * (e * (d2l[r * rs + j] + dl[p * rs + j] * dl[q * rs + j])).re;
+          if (++q == NP) q = ++p;
+        }
+      }
+    }
+  });
+  if (threadIdx.x == 0) {
+    const double F = sp.forward, K = sp.strike, df = sp.discfactor;
+    const int J = gridDim.x;
+    if (vanna_rows) {
+#pragma unroll
+      for (int k = 0; k < NP; ++k) vanna[(size_t)k * J + blockIdx.x] = is_spot ? -df * K * acc[NP + k] / F : -df * (acc[k] + acc[NP + k]);
+    } else {
+      const double scale = is_spot ? -df * K : -F * df;
+#pragma unroll
+      for (int i = 0; i < R; ++i)
+        if (r0 + i < NH) hessian[(size_t)(r0 + i) * J + blockIdx.x] = scale * acc[i];
+    }
+  }
+}
+
+// ---- Hawkes jump-diffusion, second order (DESIGN.md §4.5) ----
+constexpr int kHawkesOdePairs = kHawkesOdeDirs * (kHawkesOdeDirs + 1) / 2;  // 91 pairs over the 13 ODE directions
+
+// d2(HawkesMgfConsts field) / d(direction p) d(direction q) for the kHawkesOdePairs pairs (tri_index order over the ODE directions of
+// make_hawkes_tangents).  Nonzero: sigma2 = sigma^2, kt = kappa theta and comp = e^shift / (1 - mean) - 1.
+static void make_hawkes_hessian(const b200sv_hawkes_params& p, HawkesMgfConsts (&h)[kHawkesOdePairs]) {
+  for (auto& t : h) t = HawkesMgfConsts{0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+  constexpr int D = kHawkesOdeDirs;
+  const double ep = std::exp(p.shift_p) / (1.0 - p.mean_p), em = std::exp(p.shift_m) / (1.0 - p.mean_m);
+  h[tri_index(0, 0, D)].sigma2 = 2.0;                                                  // sigma sigma
+  h[tri_index(5, 6, D)].kt_p = 1.0;                                                    // theta_p kappa_p
+  h[tri_index(9, 10, D)].kt_m = 1.0;                                                   // theta_m kappa_m
+  h[tri_index(1, 1, D)].comp_p = ep;                                                   // shift_p shift_p
+  h[tri_index(1, 2, D)].comp_p = ep / (1.0 - p.mean_p);                                // shift_p mean_p
+  h[tri_index(2, 2, D)].comp_p = 2.0 * ep / ((1.0 - p.mean_p) * (1.0 - p.mean_p));     // mean_p mean_p
+  h[tri_index(3, 3, D)].comp_m = em;                                                   // shift_m shift_m
+  h[tri_index(3, 4, D)].comp_m = em / (1.0 - p.mean_m);                                // shift_m mean_m
+  h[tri_index(4, 4, D)].comp_m = 2.0 * em / ((1.0 - p.mean_m) * (1.0 - p.mean_m));     // mean_m mean_m
+}
+
+// The three right-hand sides of one ODE pair (p, q) in one hyper-dual evaluation of HawkesRhsFn's arithmetic: with A_k = (A, dA_p, dA_q,
+// d2A_pq) and every HawkesMgfConsts field f = (f, df/dp, df/dq, d2f/dp dq), the parts .d1 / .d2 are the tangent right-hand sides
+// J(A) dA_p + d_p f(A) (HawkesTanRhsFn) and J(A) dA_q + d_q f(A), and .d12 is
+//   J(A) d2A + f_AA(dA_p, dA_q) + d_p J(A) dA_q + d_q J(A) dA_p + d_pq f(A).
+// The jump-size MGF E(z; s, m) = e^{-s z} / (1 + m z) goes through hcd's exp_ and Smith division jointly in (z, s, m); the constant -1 of
+// E - 1 has no derivative and is left out.
+struct HawkesTan2RhsFn {
+  const HawkesMgfConsts& c;
+  HawkesMgfConsts dp, dq, d2;
+  cd phi, h0;              // h0 = (phi + 1) phi / 2 - psi: drift0 = sigma^2 h0
+  __device__ __forceinline__ hcd k(double HawkesMgfConsts::*f) const { return hcd{mk(c.*f), mk(dp.*f), mk(dq.*f), mk(d2.*f)}; }
+  __device__ __forceinline__ void operator()(const cd (&Y)[3], const cd (&dYp)[3], const cd (&dYq)[3], const cd (&d2Y)[3], cd (&op)[3],
+                                             cd (&oq)[3], cd (&opq)[3]) const {
+    using H = HawkesMgfConsts;
+    const hcd a1{Y[1], dYp[1], dYq[1], d2Y[1]}, a2{Y[2], dYp[2], dYq[2], d2Y[2]}, ph = hmk(phi), one = hmk(mk(1.0));
+    const hcd zp = (ph - k(&H::beta1_p) * a1) - k(&H::beta1_m) * a2, zm = (ph - k(&H::beta2_p) * a1) - k(&H::beta2_m) * a2;
+    const hcd jp = exp_(-(k(&H::shift_p) * zp)) / (one + k(&H::mean_p) * zp);
+    const hcd jm = exp_(-(k(&H::shift_m) * zm)) / (one + k(&H::mean_m) * zm);
+    const hcd o[3] = {(k(&H::kt_p) * a1 + k(&H::kt_m) * a2) + k(&H::sigma2) * hmk(h0), (jp - k(&H::kappa_p) * a1) + k(&H::comp_p) * ph,
+                      (jm - k(&H::kappa_m) * a2) + k(&H::comp_m) * ph};
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+      op[i] = o[i].d1;
+      oq[i] = o[i].d2;
+      opq[i] = o[i].d12;
+    }
+  }
+};
+
+constexpr int kHawkesHessianTPB = 32;   // static shared memory per thread: 6 x 3 primal + 3 x 8 x 3 tangent stages = 1 440 B, 45 KB per CTA
+
+// One thread = one (grid point, ODE pair p <= q): the primal integration of hawkes_mgf_kernel (same rk45_generic, same mesh) plus the
+// tangents of p and q and their mixed second-order tangent (Tangent2Hook), carried over the maturities like A.  The 91 pairs of a point are
+// neighbouring threads.  lm = a0 + a_p lambda_p + a_m lambda_m is linear in the lambdas and they have no ODE tangent, so
+//   d2lm_pq = d2a0 + d2a_p lambda_p + d2a_m lambda_m,  d2lm / dlambda_p dq = da_p / dq,  d2lm / dlambda_m dq = da_m / dq,  d2lm / dlambda dlambda = 0:
+// the diagonal thread of direction d also writes (lambda_p, d) and (lambda_m, d), pair 0 the three lambda-lambda rows.  dirs: the first
+// field derivatives (make_hawkes_tangents), d2c [91]: the second (make_hawkes_hessian).  Output d2log_mgf [120][M][P] (tri_index over
+// HAWKES_GREEK_PARAMS).
+__global__ void __launch_bounds__(kHawkesHessianTPB) hawkes_mgf_hessian_kernel(const cd* __restrict__ phi, int P, int M,
+                                                                               const double* __restrict__ dtaus, HawkesMgfConsts c,
+                                                                               HawkesTangentDirs dirs, const HawkesMgfConsts* __restrict__ d2c,
+                                                                               cd* __restrict__ d2log_mgf) {
+  constexpr int TPB = kHawkesHessianTPB, D = kHawkesOdeDirs, NP = kHawkesGreekParams;
+  __shared__ cd stage_smem[6 * 3 * TPB];
+  __shared__ cd tan_smem[3 * 8 * 3 * TPB];
+  const int t = blockIdx.x * TPB + threadIdx.x;
+  if (t >= P * kHawkesOdePairs) return;
+  const int p = t / kHawkesOdePairs, pair = t % kHawkesOdePairs;
+  int dp, dq;
+  tri_pair(pair, D, dp, dq);
+#pragma unroll
+  for (int i = 0; i < 18; ++i) stage_smem[threadIdx.x + i * TPB] = mk(0.0);
+#pragma unroll
+  for (int i = 0; i < 72; ++i) tan_smem[threadIdx.x + i * TPB] = mk(0.0);
+  StageStore<3, TPB> K{stage_smem + threadIdx.x};
+  const cd ph = phi[p];
+  const cd h0 = 0.5 * ((ph + mk(1.0)) * ph);
+  const HawkesRhsFn f{c, ph, c.sigma2 * h0};
+  Tangent2Hook<3, TPB, HawkesTan2RhsFn> tan{HawkesTan2RhsFn{c, dirs.d[dp], dirs.d[dq], d2c[pair], ph, h0},
+                                            {StageStore<3, TPB>{tan_smem + threadIdx.x}, {}},
+                                            {StageStore<3, TPB>{tan_smem + 24 * TPB + threadIdx.x}, {}},
+                                            {StageStore<3, TPB>{tan_smem + 48 * TPB + threadIdx.x}, {}}};   // dy = 0
+  cd A[3] = {mk(0.0), mk(0.0), mk(0.0)};
+  const int rp = hawkes_dir_row(dp), rq = hawkes_dir_row(dq);
+  for (int m = 0; m < M; ++m) {
+    rk45_generic<3, TPB>(A, dtaus[m], f, K, nullptr, &tan);
+    d2log_mgf[((size_t)tri_index(rp, rq, NP) * M + m) * P + p] = (tan.pq.dy[0] + tan.pq.dy[1] * c.lambda_p) + tan.pq.dy[2] * c.lambda_m;
+    if (dp == dq) {
+      d2log_mgf[((size_t)tri_index(min(5, rp), max(5, rp), NP) * M + m) * P + p] = tan.p.dy[1];
+      d2log_mgf[((size_t)tri_index(min(10, rp), max(10, rp), NP) * M + m) * P + p] = tan.p.dy[2];
+    }
+    if (pair == 0) {
+      d2log_mgf[((size_t)tri_index(5, 5, NP) * M + m) * P + p] = mk(0.0);
+      d2log_mgf[((size_t)tri_index(5, 10, NP) * M + m) * P + p] = mk(0.0);
+      d2log_mgf[((size_t)tri_index(10, 10, NP) * M + m) * P + p] = mk(0.0);
+    }
+  }
+}
+
 // --------------------------------------------------------------------------------------------------------------------
 // host side
 // --------------------------------------------------------------------------------------------------------------------
@@ -2725,9 +2885,21 @@ static int queue_heston_greeks(ChainDev& d, GreeksDev<1 + kHestonOdeDirs>& t, co
   return t.sums(d, c, d.lm.as<cd>());
 }
 
-// The second-order sums of b200sv_*_price_chain_hessian after its Hessian kernel wrote d2lm [NH][M][P]: fourier_vanilla_hessian_kernel on
-// log_mgf and the first-order tangents dlm [NP][M][P] (no launch on an empty chain), then vanna, the Hessian rows and d2lm come back; the
-// first-order outputs follow with GreeksDev::download().
+// The Hawkes twin, without a risk kernel: the pricing launches, hawkes_mgf_tangent_kernel on the constants k, then the sums on the tangent
+// kernel's own primal log-MGF, on the mesh the tangents were stepped on (DESIGN.md §4.3).
+static int queue_hawkes_greeks(ChainDev& d, GreeksDev<kHawkesGreekParams>& t, const FourierChain& c, const b200sv_hawkes_params& params,
+                               const HawkesMgfConsts& k, double* prices_out) {
+  if (int rc = queue_hawkes_prices(d, c, &k, prices_out)) return rc;
+  if (int rc = t.alloc(c, true)) return rc;
+  launch_hawkes_mgf_tangent(d.st, d.phi.as<cd>(), c.P, c.M, d.dt.as<double>(), k, make_hawkes_tangents(params), t.dlm.as<cd>(), t.lm.as<cd>(),
+                            t.nfev.as<int>());
+  if (int rc = check_launch("hawkes_mgf_tangent_kernel")) return rc;
+  return t.sums(d, c, t.lm.as<cd>());
+}
+
+// The second-order sums of b200sv_*_price_chain_hessian after its Hessian kernel wrote d2lm [NH][M][P]: fourier_vanilla_hessian_kernel
+// (fourier_vanilla_hessian_split_kernel for Hawkes' 15 parameters) on log_mgf and the first-order tangents dlm [NP][M][P] (no launch on an
+// empty chain), then vanna, the Hessian rows and d2lm come back; the first-order outputs follow with GreeksDev::download().
 template <int NP>
 static int queue_hessian_sums(ChainDev& d, const FourierChain& c, const cd* log_mgf, const cd* dlm, const DevBuf& d2lm, double* vanna_out,
                               double* hessian_out, double* d2log_mgf_out) {
@@ -2736,10 +2908,18 @@ static int queue_hessian_sums(ChainDev& d, const FourierChain& c, const cd* log_
   if (c.Jtot > 0) {
     B200SV_CUDA(d_v.alloc(sizeof(double) * (size_t)NP * c.Jtot));
     B200SV_CUDA(d_h.alloc(sizeof(double) * (size_t)NH * c.Jtot));
-    fourier_vanilla_hessian_kernel<NP><<<c.Jtot, kFourierThreads, 0, d.st>>>(log_mgf, dlm, d2lm.as<cd>(), d.phi.as<cd>(), c.P, c.M,
-                                                                             d.rows.as<StrikeSpec>(), c.spot ? 1 : 0, d_v.as<double>(),
-                                                                             d_h.as<double>());
-    if (int rc = check_launch("fourier_vanilla_hessian_kernel")) return rc;
+    if constexpr (NP <= 6) {      // LogSV, Heston: every row of a strike in one CTA
+      fourier_vanilla_hessian_kernel<NP><<<c.Jtot, kFourierThreads, 0, d.st>>>(log_mgf, dlm, d2lm.as<cd>(), d.phi.as<cd>(), c.P, c.M,
+                                                                               d.rows.as<StrikeSpec>(), c.spot ? 1 : 0, d_v.as<double>(),
+                                                                               d_h.as<double>());
+      if (int rc = check_launch("fourier_vanilla_hessian_kernel")) return rc;
+    } else {                      // Hawkes: the vanna CTA and NH / NP Hessian CTAs per strike
+      const dim3 grid(c.Jtot, 1 + (NH + NP - 1) / NP);
+      fourier_vanilla_hessian_split_kernel<NP><<<grid, kFourierThreads, 0, d.st>>>(log_mgf, dlm, d2lm.as<cd>(), d.phi.as<cd>(), c.P, c.M,
+                                                                                   d.rows.as<StrikeSpec>(), c.spot ? 1 : 0, d_v.as<double>(),
+                                                                                   d_h.as<double>());
+      if (int rc = check_launch("fourier_vanilla_hessian_split_kernel")) return rc;
+    }
     B200SV_CUDA(d_v.download(vanna_out, (size_t)NP * c.Jtot));
     B200SV_CUDA(d_h.download(hessian_out, (size_t)NH * c.Jtot));
   }
@@ -2958,13 +3138,39 @@ int b200sv_hawkesjd_price_chain_greeks(const b200sv_hawkes_params* params, int M
     return rc;
   const HawkesMgfConsts k = make_hawkes_mgf_consts(*params);
   ChainDev d;
-  if (int rc = queue_hawkes_prices(d, c, &k, prices_out)) return rc;
   GreeksDev<kHawkesGreekParams> g(d.st);
-  if (int rc = g.alloc(c, true)) return rc;
-  launch_hawkes_mgf_tangent(d.st, d.phi.as<cd>(), c.P, M, d.dt.as<double>(), k, make_hawkes_tangents(*params), g.dlm.as<cd>(), g.lm.as<cd>(),
-                            g.nfev.as<int>());
-  if (int rc = check_launch("hawkes_mgf_tangent_kernel")) return rc;
-  if (int rc = g.sums(d, c, g.lm.as<cd>())) return rc;     // the tangent kernel's own primal log-MGF, on the mesh the tangents were stepped on
+  if (int rc = queue_hawkes_greeks(d, g, c, *params, k, prices_out)) return rc;
+  return g.download(d, c, greeks_out, dlog_mgf_out, nfev_out);
+}
+
+/* Second-order sensitivities of the Hawkes Fourier chain without a risk kernel (DESIGN.md §4.5): the launches of
+ * b200sv_hawkesjd_price_chain_greeks unchanged (bit-identical first-order outputs), then hawkes_mgf_hessian_kernel and the split
+ * second-order sums; one synchronisation at the end. */
+int b200sv_hawkesjd_price_chain_hessian(const b200sv_hawkes_params* params, int M, const double* ttms, const double* forwards,
+                                        const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
+                                        int is_spot_measure, double vol_scaler, int P, double* prices_out, double* greeks_out,
+                                        double* dlog_mgf_out, int* nfev_out, double* vanna_out, double* hessian_out, double* d2log_mgf_out) {
+  B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && greeks_out && vanna_out && hessian_out, "null pointer");
+  FourierChain c;
+  if (int rc = prepare_hawkes_chain(c, params, M, ttms, forwards, discfactors, offsets, strikes, types, is_spot_measure, vol_scaler, P, NAN))
+    return rc;
+  const HawkesMgfConsts k = make_hawkes_mgf_consts(*params);
+  ChainDev d;
+  GreeksDev<kHawkesGreekParams> g(d.st);
+  if (int rc = queue_hawkes_greeks(d, g, c, *params, k, prices_out)) return rc;
+  constexpr int NP = kHawkesGreekParams, NH = NP * (NP + 1) / 2, TPB = kHawkesHessianTPB;
+  P = c.P;
+  HawkesMgfConsts h[kHawkesOdePairs];
+  make_hawkes_hessian(*params, h);
+  DevBuf d_d2c(d.st), d_d2lm(d.st);
+  B200SV_CUDA(d_d2c.upload(h, kHawkesOdePairs));
+  B200SV_CUDA(d_d2lm.alloc(sizeof(cd) * (size_t)NH * M * P));
+  hawkes_mgf_hessian_kernel<<<(P * kHawkesOdePairs + TPB - 1) / TPB, TPB, 0, d.st>>>(d.phi.as<cd>(), P, M, d.dt.as<double>(), k,
+                                                                                     make_hawkes_tangents(*params),
+                                                                                     d_d2c.as<HawkesMgfConsts>(), d_d2lm.as<cd>());
+  if (int rc = check_launch("hawkes_mgf_hessian_kernel")) return rc;
+  // the tangent kernel's primal log-MGF and tangents, as for the first-order rows
+  if (int rc = queue_hessian_sums<NP>(d, c, g.lm.as<cd>(), g.dlm.as<cd>(), d_d2lm, vanna_out, hessian_out, d2log_mgf_out)) return rc;
   return g.download(d, c, greeks_out, dlog_mgf_out, nfev_out);
 }
 

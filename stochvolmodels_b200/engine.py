@@ -635,6 +635,17 @@ def hawkesjd_price_chain_greeks(params: C.HawkesParamsC, ttms, forwards, discfac
                                HAWKES_GREEK_PARAMS, True)
 
 
+def hawkesjd_price_chain_hessian(params: C.HawkesParamsC, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms,
+                                 is_spot_measure: bool = True, vol_scaler: Optional[float] = None, max_phi: Optional[int] = None,
+                                 return_grids: bool = False):
+    """hawkesjd_price_chain_greeks plus the second-order sensitivities (b200sv_hawkesjd_price_chain_hessian): vanna [15, J], hessian
+    [120, J] over HAWKES_GREEK_PARAMS (upper triangle, row-major); ``return_grids`` adds (dlog_mgf [15, M, P], d2log_mgf [120, M, P]).
+    P defaults to the route's 500 points."""
+    return _price_chain_hessian("b200sv_hawkesjd_price_chain_hessian", params, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms),
+                                (), is_spot_measure, (int(bool(is_spot_measure)),), vol_scaler, int(max_phi or 500), return_grids,
+                                HAWKES_GREEK_PARAMS, True)
+
+
 def logsv_price_chain_batch(params_list: Sequence[C.LogsvParamsC], ttms, forwards, discfactors, etas, strikes_ttms, optiontypes_ttms,
                             is_spot_measure: bool = True, expansion_order: int = C.ORDER_SECOND, vol_scaler: Optional[float] = None,
                             max_phi: int = 1000, with_ivols: bool = True):

@@ -112,6 +112,21 @@ class HawkesJDPricer(ModelPricer):
             option_chain.optiontypes_ttms, is_spot_measure=is_spot_measure, vol_scaler=kwargs.get("vol_scaler"), max_phi=MAX_PHI)
         return to_fourier_chain_greeks(prices, greeks, offsets, engine.HAWKES_GREEK_PARAMS)
 
+    def price_chain_hessian(self, option_chain: OptionChain, params: HawkesJDParams, is_spot_measure: bool = True, **kwargs):
+        """``price_chain_greeks`` (bit for bit) plus the second order in one call -> ``FourierChainHessian``: vanna (d^2 price / d forward
+        d parameter) and the symmetric Hessian d^2 price / d p d q over HAWKES_GREEK_PARAMS, the exact second derivatives of the scheme on
+        the adaptive solver's own mesh (DESIGN.md §4.5).  Same conventions and the same rejections as ``price_chain_greeks``."""
+        from .fourier_greeks import check_fourier_hessian_kwargs, to_fourier_chain_hessian
+        if params.risk_premia_gamma is not None:
+            raise NotImplementedError("price_chain_hessian does not cover the risk-kernel pricer (risk_premia_gamma)")
+        check_fourier_hessian_kwargs(kwargs)
+        d = params.to_dict()
+        d.pop("risk_premia_gamma", None)
+        prices, greeks, vanna, hessian, offsets = engine.hawkesjd_price_chain_hessian(
+            _params_c(**d), option_chain.ttms, option_chain.forwards, option_chain.discfactors, option_chain.strikes_ttms,
+            option_chain.optiontypes_ttms, is_spot_measure=is_spot_measure, vol_scaler=kwargs.get("vol_scaler"), max_phi=MAX_PHI)
+        return to_fourier_chain_hessian(prices, greeks, vanna, hessian, offsets, engine.HAWKES_GREEK_PARAMS)
+
     @timer
     def model_mc_price_chain(self, option_chain: OptionChain, params: HawkesJDParams, nb_path: int = 100000, **kwargs
                              ) -> Tuple[List[np.ndarray], List[np.ndarray]]:
