@@ -530,6 +530,17 @@ int b200sv_bsm_implied_vols(int M, const double* ttms, const double* forwards, c
 /* test hook: b200sv_bsm_implied_vols plus iterations_out[] = the Newton iterations each quote took (0 for a NaN verdict) */
 int b200sv_debug_bsm_implied_vols(int M, const double* ttms, const double* forwards, const double* discfactors, const int* offsets,
                                   const double* strikes, const int8_t* types, const double* prices, double* ivols_out, int* iterations_out);
+/* implied-vol sensitivities of model prices, for any model (DESIGN.md §4.6).  The chain and prices[] as b200sv_bsm_implied_vols; NP
+ * (1..15, else -1) model parameters; greeks [2+NP][J] = d price / d forwards[m], d^2 price / d forwards[m]^2, d price / d p, in exactly the
+ * layout b200sv_*_price_chain_greeks return; optional vanna [NP][J] and hessian [NP(NP+1)/2][J] (upper triangle, row-major) in the layout of
+ * b200sv_*_price_chain_hessian, given together or not at all (else -1), each with its output (else -1).  Outputs: ivols_out [J], bit-identical
+ * to b200sv_bsm_implied_vols on the same prices; ivol_greeks_out [2+NP][J], ivol_vanna_out [NP][J], ivol_hessian_out [NP(NP+1)/2][J]: the
+ * same derivatives of the implied vol (sticky strike: the forward moves the model price and Black's forward).  A NaN ivol gives NaN rows; an
+ * ivol at an end of the inversion bracket (1e-8 or 10) gives zero rows.  Unknown type codes: -3. */
+int b200sv_bsm_implied_vol_sensitivities(int M, const double* ttms, const double* forwards, const double* discfactors, const int* offsets,
+                                         const double* strikes, const int8_t* types, const double* prices, int NP, const double* greeks,
+                                         const double* vanna, const double* hessian, double* ivols_out, double* ivol_greeks_out,
+                                         double* ivol_vanna_out, double* ivol_hessian_out);
 
 #ifdef __cplusplus
 }

@@ -5,7 +5,7 @@ from .data.option_chain import OptionChain, OptionSlice, get_btc_test_chain_data
 from .engine import HAWKES_GREEK_PARAMS, infer_bsm_ivols_from_model_chain_prices, infer_bsm_ivols_from_slice_prices
 from .pricers.calibration import CalibrationEngine, CalibrationError, ConstraintsType, LogsvModelCalibrationType
 from .pricers.hawkes_jd_pricer import HawkesJDParams, HawkesJDPricer
-from .pricers.fourier_greeks import FourierChainGreeks, FourierChainHessian
+from .pricers.fourier_greeks import ChainIvolGreeks, ChainIvolHessian, FourierChainGreeks, FourierChainHessian
 from .pricers.heston_pricer import BTC_HESTON_PARAMS, HestonParams, HestonPricer
 from .pricers.logsv.affine_expansion import ExpansionOrder
 from .pricers.logsv.vol_moments import compute_analytic_qvar
@@ -21,4 +21,4 @@ __all__ = ["HawkesJDParams", "HawkesJDPricer", "OptionChain", "get_btc_test_chai
            "LogSvParams", "LogSVPricer", "CalibrationEngine", "CalibrationError", "ConstraintsType", "LogsvModelCalibrationType", "LOGSV_BTC_PARAMS", "ModelParams", "ModelPricer", "OptionType", "VariableType", "set_seed", "set_time_grid",
            "compute_integration_weights", "OptionSlice", "compute_analytic_qvar", "infer_bsm_ivols_from_slice_prices",
            "infer_bsm_ivols_from_model_chain_prices", "McChainGreeks", "FourierChainGreeks", "FourierChainHessian",
-           "HAWKES_GREEK_PARAMS"]
+           "ChainIvolGreeks", "ChainIvolHessian", "HAWKES_GREEK_PARAMS"]

@@ -85,4 +85,35 @@ __device__ __forceinline__ double black_implied_vol(double forward, double strik
   return s / srt;
 }
 
+// True where black_implied_vol returned an end of its bracket [1e-8, 10] (to the rounding of s / sqrt T, with a 1e-10 relative margin):
+// the root lies outside it, so the returned vol does not move with the price.
+__device__ __forceinline__ bool black_vol_at_bracket_end(double vol) {
+  return vol <= 1e-8 * (1.0 + 1e-10) || vol >= 10.0 * (1.0 - 1e-10);
+}
+
+// Partial derivatives of the discounted Black-76 price B(F, vol) of one quote, in vol (not total vol): s = vol sqrt T,
+// d1 = ln(F/K) / s + s / 2, d2 = d1 - s, n = phi(d1), D the discount factor.  Calls and puts differ only in B_F; IC / IP are priced as
+// C / P, as in black_implied_vol.
+struct BlackPartials {
+  double vega;   // B_vol     = D F n sqrt T
+  double dF;     // B_F       = D N(d1) (call), D (N(d1) - 1) (put)
+  double dFF;    // B_FF      = D n / (F s)
+  double dFv;    // B_F,vol   = -D n d2 / vol
+  double dvv;    // B_vol,vol = B_vol d1 d2 / vol
+};
+
+__device__ __forceinline__ BlackPartials black_partials(double forward, double strike, double ttm, double discfactor, double vol, int type) {
+  const bool is_call = (type == B200SV_CALL || type == B200SV_INV_CALL);
+  const double srt = sqrt(ttm), s = vol * srt;
+  const double d1 = log(forward / strike) / s + 0.5 * s, d2 = d1 - s;
+  const double n = 0.3989422804014327 * exp(-0.5 * d1 * d1);
+  BlackPartials b;
+  b.vega = discfactor * forward * n * srt;
+  b.dF = discfactor * (is_call ? normcdf(d1) : -normcdf(-d1));
+  b.dFF = discfactor * n / (forward * s);
+  b.dFv = -discfactor * n * d2 / vol;
+  b.dvv = b.vega * d1 * d2 / vol;
+  return b;
+}
+
 }  // namespace b200sv

@@ -39,6 +39,78 @@ __global__ void black_ivol_count_kernel(const QuoteSpec* __restrict__ q, int n, 
   iterations[i] = it;
 }
 
+// Implied-vol sensitivities of model prices (DESIGN.md §4.6).  The model ivol sigma(F, p) is defined by B(F, sigma) = P(F, p), B the
+// discounted Black-76 price, P the model price, F the slice forward (sticky strike: it moves both P and Black's F), p the NP model
+// parameters.  One thread per quote inverts the price with black_implied_vol -- the same function on the same doubles as
+// b200sv_bsm_implied_vols and the fused batch pricers, so the ivols are bit-identical to theirs -- and applies the implicit-function rule
+//   sigma_p  = P_p / B_s                                   sigma_F  = (P_F - B_F) / B_s
+//   sigma_FF = (P_FF - B_FF - 2 B_Fs sigma_F - B_ss sigma_F^2) / B_s
+//   sigma_Fp = (P_Fp - B_Fs sigma_p - B_ss sigma_F sigma_p) / B_s          (SECOND only)
+//   sigma_pq = (P_pq - B_ss sigma_p sigma_q) / B_s                          (SECOND only)
+// rows: [2 + NP][n] = (P_F, P_FF, P_p) then, when SECOND, vanna [NP][n] = P_Fp and hessian [NP(NP+1)/2][n] = P_pq (p <= q, row-major).
+// out:  [n] ivols, then the sigma rows in the same layout.  Row-major [row][n], so a warp's loads and stores of one row are coalesced.
+// Where the ivol is NaN every row is NaN.  Where it is an end of the inversion bracket (1e-8 or 10) the ivol does not move with the
+// price and every row is 0: a calibration objective that still counts the quote then gets the gradient of what it counts.
+template <int NP, bool SECOND>
+__global__ void __launch_bounds__(64) black_ivol_sensitivities_kernel(const QuoteSpec* __restrict__ q, int n, const double* __restrict__ rows,
+                                                                      double* __restrict__ out) {
+  constexpr int NH = NP * (NP + 1) / 2;
+  constexpr int NROWS = 2 + NP + (SECOND ? NP + NH : 0);
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const QuoteSpec s = q[i];
+  const double vol = black_implied_vol(s.forward, s.strike, s.ttm, s.discfactor, s.price, s.type);
+  out[i] = vol;
+  double* sig = out + n;
+  if (vol != vol || black_vol_at_bracket_end(vol)) {
+    const double fill = vol != vol ? vol : 0.0;
+#pragma unroll 4
+    for (int r = 0; r < NROWS; ++r) sig[(size_t)r * n + i] = fill;
+    return;
+  }
+  const BlackPartials b = black_partials(s.forward, s.strike, s.ttm, s.discfactor, vol, s.type);
+  const double sF = (rows[i] - b.dF) / b.vega;
+  sig[i] = sF;
+  sig[(size_t)n + i] = (rows[(size_t)n + i] - b.dFF - 2.0 * b.dFv * sF - b.dvv * sF * sF) / b.vega;
+  double sp[NP];
+#pragma unroll
+  for (int k = 0; k < NP; ++k) {
+    sp[k] = rows[(size_t)(2 + k) * n + i] / b.vega;
+    sig[(size_t)(2 + k) * n + i] = sp[k];
+  }
+  if constexpr (SECOND) {
+    const double cF = b.dFv + b.dvv * sF;
+#pragma unroll
+    for (int k = 0; k < NP; ++k) {
+      const size_t r = (size_t)(2 + NP + k) * n + i;
+      sig[r] = (rows[r] - cF * sp[k]) / b.vega;
+    }
+    int h = 2 + 2 * NP;
+#pragma unroll
+    for (int a = 0; a < NP; ++a)
+#pragma unroll
+      for (int c = a; c < NP; ++c, ++h) {
+        const size_t r = (size_t)h * n + i;
+        sig[r] = (rows[r] - b.dvv * sp[a] * sp[c]) / b.vega;
+      }
+  }
+}
+
+constexpr int IVOL_SENS_MAX_NP = 15;     // the Hawkes parameter count, the largest of the Fourier chain pricers
+
+template <int NP>
+static int launch_ivol_sensitivities(int np, bool second, int n, const QuoteSpec* q, const double* rows, double* out, cudaStream_t st) {
+  if constexpr (NP > IVOL_SENS_MAX_NP) {
+    return fail(-1, "invalid argument: NP must be in 1..15");
+  } else {
+    if (np != NP) return launch_ivol_sensitivities<NP + 1>(np, second, n, q, rows, out, st);
+    const int blocks = (n + 63) / 64;
+    if (second) black_ivol_sensitivities_kernel<NP, true><<<blocks, 64, 0, st>>>(q, n, rows, out);
+    else black_ivol_sensitivities_kernel<NP, false><<<blocks, 64, 0, st>>>(q, n, rows, out);
+    return check_launch("black_ivol_sensitivities_kernel");
+  }
+}
+
 }  // namespace b200sv
 
 using namespace b200sv;
@@ -85,4 +157,52 @@ extern "C" int b200sv_debug_bsm_implied_vols(int M, const double* ttms, const do
                                              int* iterations_out) {
   B200SV_REQUIRE(iterations_out, "null pointer");
   return bsm_implied_vols(M, ttms, forwards, discfactors, offsets, strikes, types, prices, ivols_out, iterations_out);
+}
+
+extern "C" int b200sv_bsm_implied_vol_sensitivities(int M, const double* ttms, const double* forwards, const double* discfactors,
+                                                    const int* offsets, const double* strikes, const int8_t* types, const double* prices,
+                                                    int NP, const double* greeks, const double* vanna, const double* hessian,
+                                                    double* ivols_out, double* ivol_greeks_out, double* ivol_vanna_out,
+                                                    double* ivol_hessian_out) {
+  B200SV_REQUIRE(ttms && forwards && discfactors && offsets && strikes && types && prices && greeks && ivols_out && ivol_greeks_out,
+                 "null pointer");
+  B200SV_REQUIRE(M >= 1, "M >= 1");
+  B200SV_REQUIRE(NP >= 1 && NP <= IVOL_SENS_MAX_NP, "NP must be in 1..15");
+  B200SV_REQUIRE(!vanna == !hessian, "vanna and hessian are given together or not at all");
+  B200SV_REQUIRE(!vanna == !ivol_vanna_out && !hessian == !ivol_hessian_out, "every second-order input needs its output and vice versa");
+  const bool second = vanna != nullptr;
+  const int n = offsets[M] - offsets[0];
+  if (n <= 0) return 0;
+  std::vector<QuoteSpec> q(n);
+  for (int m = 0; m < M; ++m)
+    for (int j = offsets[m]; j < offsets[m + 1]; ++j) {
+      if (types[j] < 0 || types[j] > 3) return fail(-3, "unknown option payoff code");
+      q[j - offsets[0]] = QuoteSpec{forwards[m], strikes[j], ttms[m], discfactors[m], prices[j - offsets[0]], (int)types[j]};
+    }
+  const size_t nh = (size_t)NP * (NP + 1) / 2, n1 = 2 + NP, nrows = n1 + (second ? NP + nh : 0);
+  std::vector<double> rows(nrows * n);                      // the input rows packed as the kernel reads them: one upload
+  std::memcpy(rows.data(), greeks, sizeof(double) * n1 * n);
+  if (second) {
+    std::memcpy(rows.data() + n1 * n, vanna, sizeof(double) * NP * n);
+    std::memcpy(rows.data() + (n1 + NP) * n, hessian, sizeof(double) * nh * n);
+  }
+  cudaStream_t st = current_stream();
+  ensure_pool_threshold();
+  StreamSync sync(st);
+  DevBuf dq(st), drows(st), dout(st);
+  B200SV_CUDA(dq.upload(q.data(), n));
+  B200SV_CUDA(drows.upload(rows.data(), rows.size()));
+  B200SV_CUDA(dout.alloc(sizeof(double) * (1 + nrows) * n));
+  if (int rc = launch_ivol_sensitivities<1>(NP, second, n, dq.as<QuoteSpec>(), drows.as<double>(), dout.as<double>(), st)) return rc;
+  std::vector<double> out((1 + nrows) * n);
+  B200SV_CUDA(dout.download(out.data(), out.size()));
+  if (int rc = sync.done()) return rc;
+  const double* o = out.data();
+  std::memcpy(ivols_out, o, sizeof(double) * n);
+  std::memcpy(ivol_greeks_out, o + n, sizeof(double) * n1 * n);
+  if (second) {
+    std::memcpy(ivol_vanna_out, o + (1 + n1) * n, sizeof(double) * NP * n);
+    std::memcpy(ivol_hessian_out, o + (1 + n1 + NP) * n, sizeof(double) * nh * n);
+  }
+  return 0;
 }

@@ -805,6 +805,36 @@ def debug_bsm_implied_vols(ttms, forwards, discfactors, strikes_ttms, optiontype
     return ivols, iterations
 
 
+def bsm_implied_vol_sensitivities(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, prices_ttms, greeks, vanna=None, hessian=None):
+    """implied vols of the model prices and their sensitivities in one kernel launch (b200sv_bsm_implied_vol_sensitivities; DESIGN.md
+    §4.6).  ``greeks`` [2 + P, J]: d price / d forward, d^2 price / d forward^2, d price / d p, as the *_price_chain_greeks entry points
+    return it; ``vanna`` [P, J] and ``hessian`` [P(P+1)/2, J] as the *_price_chain_hessian ones do, both or neither.  Returns (ivols per
+    maturity, ivol_greeks [2 + P, J], ivol_vanna [P, J] | None, ivol_hessian [P(P+1)/2, J] | None) -- the same derivatives of the implied
+    vol; the ivols bit-identical to bsm_implied_vols."""
+    ch = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
+    prices = C.f64(np.concatenate([np.asarray(p, dtype=np.float64).ravel() for p in prices_ttms]))
+    J = ch.strikes.shape[0]
+    if prices.shape[0] != J:
+        raise ValueError("model prices and strikes must have the same length")
+    greeks = C.f64(greeks)
+    if greeks.ndim != 2 or greeks.shape[1] != J or not 1 <= greeks.shape[0] - 2 <= 15:
+        raise ValueError(f"greeks must have shape (2 + P, {J}) with P in 1..15")
+    P = greeks.shape[0] - 2
+    if (vanna is None) != (hessian is None):
+        raise ValueError("vanna and hessian are given together or not at all")
+    second = vanna is not None
+    if second:
+        vanna, hessian = C.f64(vanna), C.f64(hessian)
+        if vanna.shape != (P, J) or hessian.shape != (P * (P + 1) // 2, J):
+            raise ValueError(f"vanna must have shape ({P}, {J}) and hessian ({P * (P + 1) // 2}, {J})")
+    ivols, ivol_greeks = np.empty(J), np.empty((2 + P, J))
+    ivol_vanna = np.empty((P, J)) if second else None
+    ivol_hessian = np.empty((P * (P + 1) // 2, J)) if second else None
+    C.call("b200sv_bsm_implied_vol_sensitivities", *C.chain_ptrs(ch), C.dptr(prices), P, C.dptr(greeks), C.dptr(vanna), C.dptr(hessian),
+           C.dptr(ivols), C.dptr(ivol_greeks), C.dptr(ivol_vanna), C.dptr(ivol_hessian))
+    return C.split_chain(ivols, ch.offsets), ivol_greeks, ivol_vanna, ivol_hessian
+
+
 def infer_bsm_ivols_from_model_chain_prices(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, model_prices_ttms):
     """the chain inversion the reference delegates to its third-party Black package (data/option_chain.py:340-345), keyword for keyword"""
     return bsm_implied_vols(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, model_prices_ttms)

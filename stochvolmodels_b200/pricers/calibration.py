@@ -228,6 +228,64 @@ class ScipyDifferenceObjective:
         return self._g.copy()
 
 
+GRADIENTS = ("difference", "exact")
+
+
+def check_gradient(gradient: str) -> str:
+    """the ``gradient`` argument of the calibration drivers: 'difference' (default: SLSQP's forward difference, priced as one batch) or
+    'exact' (ExactGradientObjective)"""
+    if gradient not in GRADIENTS:
+        raise ValueError("gradient must be 'difference' or 'exact'")
+    return gradient
+
+
+@dataclass
+class ExactGradientObjective:
+    """objective and its exact gradient from ONE implied-vol sensitivity evaluation, memoised on the last point so that SLSQP's ``fun(x)``
+    and ``jac(x)`` share it (DESIGN.md §4.6).  ``ivol_greeks(x) -> (vols [J], dvols [F, J])``: the model vols at x and their derivatives
+    in the pricer's F model fields (ModelPricer.compute_chain_ivol_greeks on a pinned transform grid); ``field_jacobian(x) -> D [F, n]``:
+    d fields / d x of the parameter codec.  fun(x) = nansum(w (vol - market)^2); jac(x) = sum over the quotes with a finite vol of
+    2 w (vol - market) D^T dvols.  ``nb_batches`` counts library calls (two per evaluation: the price sensitivities and their
+    implied-vol transform)."""
+    ivol_greeks: Callable[[np.ndarray], Tuple[np.ndarray, np.ndarray]]
+    field_jacobian: Callable[[np.ndarray], np.ndarray]
+    market_vols: np.ndarray
+    weights: np.ndarray
+    nb_batches: int = 0
+    nan_quotes: int = 0          # quotes without an implied vol at the LAST evaluation point (dropped there by nansum, as in the reference)
+    _x: Optional[np.ndarray] = None
+    _f: float = np.nan
+    _g: Optional[np.ndarray] = None
+
+    CALLS_PER_EVALUATION = 2
+
+    def _evaluate(self, x: np.ndarray) -> None:
+        x = np.asarray(x, dtype=float)
+        if self._x is not None and np.array_equal(x, self._x):
+            return
+        vols, dvols = self.ivol_greeks(x)
+        self.nb_batches += self.CALLS_PER_EVALUATION
+        finite = np.isfinite(vols)
+        self.nan_quotes = int(np.count_nonzero(~finite))
+        resid = vols - self.market_vols
+        f = float(np.nansum(self.weights * np.square(resid)))
+        g_fields = dvols[:, finite] @ (2.0 * self.weights[finite] * resid[finite])
+        self._x, self._f, self._g = x.copy(), f, self.field_jacobian(x).T @ g_fields
+
+    def fun(self, x: np.ndarray, *args) -> float:
+        self._evaluate(x)
+        return self._f
+
+    def jac(self, x: np.ndarray, *args) -> np.ndarray:
+        self._evaluate(x)
+        return self._g.copy()
+
+
+def flat_ivol_rows(sens, names: Sequence[str]) -> Tuple[np.ndarray, np.ndarray]:
+    """ChainIvolGreeks -> (vols [J], d vols / d names [len(names), J]) flat in chain order"""
+    return (to_flat_np_array(sens.ivols), np.vstack([to_flat_np_array(sens.params[n]) for n in names]))
+
+
 def run_slsqp(objective: BatchedObjective, p0: np.ndarray, bounds, constraints=None, disp: bool = False):
     """``scipy.optimize.minimize(method='SLSQP', options={'ftol': 1e-8})`` as in the reference (:543-555), with the batched gradient."""
     from scipy.optimize import minimize      # host-side optimizer; scipy is already a dependency of the reference
@@ -280,6 +338,24 @@ class LogSvParameterCodec:
         return (np.array([getattr(p0, n) for n in names], dtype=float),
                 tuple((getattr(lo, n), getattr(hi, n)) for n in names))
 
+    def field_jacobian(self, pars: np.ndarray) -> np.ndarray:
+        """D [6, n] = d (sigma0, theta, kappa1, kappa2, beta, volvol) / d pars (engine.LOGSV_GREEK_PARAMS order), the chain rule of the
+        exact gradient.  PARAMS5 sets kappa2 = kappa1 / theta while the price sensitivities hold kappa2 fixed, so d/d theta picks up
+        -kappa1 / theta^2 d/d kappa2 and d/d kappa1 picks up d/d kappa2 / theta."""
+        D = np.zeros((6, len(pars)))
+        if self.calibration_type == LogsvModelCalibrationType.PARAMS4:
+            for col, field in enumerate((0, 1, 4, 5)):
+                D[field, col] = 1.0
+        elif self.calibration_type == LogsvModelCalibrationType.PARAMS5:
+            for col, field in enumerate((0, 1, 2, 4, 5)):
+                D[field, col] = 1.0
+            theta, kappa1 = pars[1], pars[2]
+            D[3, 1] = -kappa1 / (theta * theta)
+            D[3, 2] = 1.0 / theta
+        else:
+            raise NotImplementedError(f"exact gradient for {self.calibration_type}")
+        return D
+
 
 def build_logsv_constraints(codec: LogSvParameterCodec, constraints_type: ConstraintsType):
     """SLSQP inequality constraints of Theorem 3.7 (reference :297-330)."""
@@ -311,7 +387,14 @@ def build_logsv_constraints(codec: LogSvParameterCodec, constraints_type: Constr
 def calibrate_logsv(pricer, option_chain, params0, params_min, params_max, is_vega_weighted: bool, is_unit_ttm_vega: bool,
                     model_calibration_type: LogsvModelCalibrationType, constraints_type: ConstraintsType,
                     calibration_engine: CalibrationEngine, nb_path: int, nb_steps: int, seed: int, is_spot_measure: bool = True,
-                    disp: bool = False, return_info: bool = False, fd_step: Optional[float] = None, mc_randoms: str = "numpy"):
+                    disp: bool = False, return_info: bool = False, fd_step: Optional[float] = None, mc_randoms: str = "numpy",
+                    gradient: str = "difference"):
+    if check_gradient(gradient) == "exact":
+        if calibration_engine != CalibrationEngine.ANALYTIC:
+            raise NotImplementedError(f"gradient='exact' covers CalibrationEngine.ANALYTIC only, not {calibration_engine}")
+        if model_calibration_type not in (LogsvModelCalibrationType.PARAMS4, LogsvModelCalibrationType.PARAMS5):
+            raise NotImplementedError(f"gradient='exact' covers PARAMS4 and PARAMS5 only, not {model_calibration_type} (the eta backbone "
+                                      "of PARAMS_WITH_VARSWAP_FIT is refitted at every point and is not differentiated)")
     from ..multi_gpu import _fixed_randoms_chain_device
     from .logsv_pricer import DeviceRandoms, _params_c, get_randoms_for_chain_valuation
     vol_scaler = pricer.set_vol_scaler(option_chain=option_chain)
@@ -324,7 +407,15 @@ def calibrate_logsv(pricer, option_chain, params0, params_min, params_max, is_ve
     p0, bounds = codec.initial_and_bounds()
     ttms = option_chain.ttms
 
-    if calibration_engine == CalibrationEngine.ANALYTIC:
+    if gradient == "exact":
+        # one compute_chain_ivol_greeks call per point, on the grid the difference route pins too (set_vol_scaler above)
+        def ivol_greeks(x: np.ndarray):
+            sens = pricer.compute_chain_ivol_greeks(option_chain, codec.parse(x), is_spot_measure=is_spot_measure, vol_scaler=vol_scaler)
+            return flat_ivol_rows(sens, engine.LOGSV_GREEK_PARAMS)
+
+        objective = ExactGradientObjective(ivol_greeks=ivol_greeks, field_jacobian=codec.field_jacobian, market_vols=market_vols,
+                                           weights=weights)
+    elif calibration_engine == CalibrationEngine.ANALYTIC:
         def batch_vols(points: np.ndarray) -> np.ndarray:
             sets = [codec.parse(p) for p in points]
             etas = np.array([s.get_vol_backbone_etas(ttms=ttms) for s in sets], dtype=float)
@@ -381,7 +472,8 @@ def calibrate_logsv(pricer, option_chain, params0, params_min, params_max, is_ve
     else:
         raise NotImplementedError(f"{calibration_engine}")
 
-    objective = BatchedObjective(batch_vols=batch_vols, market_vols=market_vols, weights=weights, bounds=bounds, eps=fd_step or SLSQP_EPS)
+    if gradient == "difference":
+        objective = BatchedObjective(batch_vols=batch_vols, market_vols=market_vols, weights=weights, bounds=bounds, eps=fd_step or SLSQP_EPS)
     x, result = run_slsqp(objective, p0, bounds, build_logsv_constraints(codec, constraints_type), disp=disp)
     fit = codec.parse(x)
     if return_info:
@@ -394,14 +486,32 @@ def calibrate_logsv(pricer, option_chain, params0, params_min, params_max, is_ve
 HESTON_BOUNDS = ((0.01, 2.0), (0.01, 2.0), (0.1, 30.0), (-0.99, 0.99), (0.1, 5.0))      # heston_pricer.py:127
 
 
+def heston_default_vol_scaler(v0: float, ttm0: float) -> float:
+    """the transform-grid scaler the Heston chain pricers use when given none, min(0.3, sqrt(v0 T0)) with T0 the first maturity (the
+    library's default, to the bit)"""
+    return float(min(0.3, np.sqrt(v0 * ttm0)))
+
+
 def calibrate_heston(pricer, option_chain, params0, is_vega_weighted: bool, is_unit_ttm_vega: bool, disp: bool = False,
-                     return_info: bool = False, fd_step: Optional[float] = None):
+                     return_info: bool = False, fd_step: Optional[float] = None, gradient: str = "difference"):
     from .heston_pricer import HestonParams, _params_c
+    check_gradient(gradient)
     p0 = (np.array([params0.v0, params0.theta, params0.kappa, params0.rho, params0.volvol], dtype=float) if params0 is not None
           else np.array([0.1, 0.1, 2.0, -0.2, 1.0]))
     _, market_vols_ttms = option_chain.get_chain_data_as_xy()
     market_vols = to_flat_np_array(market_vols_ttms)
     weights = calibration_weights(option_chain, market_vols, is_vega_weighted, is_unit_ttm_vega)
+
+    if gradient == "exact":
+        # the grid is pinned at the start point's default scaler; the difference route re-grids every set (the default depends on v0)
+        vol_scaler = heston_default_vol_scaler(p0[0], float(option_chain.ttms[0]))
+
+        def ivol_greeks(x: np.ndarray):
+            sens = pricer.compute_chain_ivol_greeks(option_chain, HestonParams(*x), vol_scaler=vol_scaler)
+            return flat_ivol_rows(sens, engine.HESTON_GREEK_PARAMS)
+
+        objective = ExactGradientObjective(ivol_greeks=ivol_greeks, field_jacobian=lambda x: np.eye(5), market_vols=market_vols,
+                                           weights=weights)
 
     def batch_vols(points: np.ndarray) -> np.ndarray:
         sets = [_params_c(*p) for p in points]
@@ -412,7 +522,9 @@ def calibrate_heston(pricer, option_chain, params0, is_vega_weighted: bool, is_u
     def feller(pars):                     # 2 kappa theta - volvol^2 >= 0 (heston_pricer.py:152-160)
         return 2.0 * pars[2] * pars[1] - pars[4] * pars[4]
 
-    objective = BatchedObjective(batch_vols=batch_vols, market_vols=market_vols, weights=weights, bounds=HESTON_BOUNDS, eps=fd_step or SLSQP_EPS)
+    if gradient == "difference":
+        objective = BatchedObjective(batch_vols=batch_vols, market_vols=market_vols, weights=weights, bounds=HESTON_BOUNDS,
+                                     eps=fd_step or SLSQP_EPS)
     x, result = run_slsqp(objective, p0, HESTON_BOUNDS, {"type": "ineq", "fun": feller}, disp=disp)
     fit = HestonParams(v0=x[0], theta=x[1], kappa=x[2], rho=x[3], volvol=x[4])
     if return_info:

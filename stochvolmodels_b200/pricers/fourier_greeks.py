@@ -35,6 +35,58 @@ class FourierChainHessian(FourierChainGreeks):
     hessian: Dict[str, Dict[str, List[np.ndarray]]]
 
 
+@dataclass
+class ChainIvolGreeks:
+    """implied-vol sensitivities of a chain (DESIGN.md §4.6), one array per maturity: ``ivols`` (bit-identical to
+    ``compute_chain_prices_with_vols`` with the same arguments), ``delta`` / ``gamma`` (d ivol / d forward, d^2 ivol / d forward^2, sticky
+    strike) and ``params``: parameter name -> d ivol / d parameter.  NaN where the ivol is NaN, 0 where it is an end of the inversion
+    bracket (1e-8 or 10)."""
+    ivols: List[np.ndarray]
+    delta: List[np.ndarray]
+    gamma: List[np.ndarray]
+    params: Dict[str, List[np.ndarray]]
+
+
+@dataclass
+class ChainIvolHessian(ChainIvolGreeks):
+    """``ChainIvolGreeks`` plus ``vanna``: name -> d^2 ivol / d forward d parameter, and ``hessian``: name -> name -> d^2 ivol / d p d q,
+    symmetric (``hessian[p][q]`` and ``hessian[q][p]`` are the same arrays)."""
+    vanna: Dict[str, List[np.ndarray]]
+    hessian: Dict[str, Dict[str, List[np.ndarray]]]
+
+
+def _flat(rows_ttms) -> np.ndarray:
+    return np.concatenate([np.asarray(r, dtype=np.float64).ravel() for r in rows_ttms])
+
+
+def to_chain_ivol_sensitivities(option_chain, greeks: FourierChainGreeks):
+    """``FourierChainGreeks`` -> ``ChainIvolGreeks``, ``FourierChainHessian`` -> ``ChainIvolHessian``: the price rows mapped to implied-vol
+    rows on the chain's forwards and discount factors by one engine.bsm_implied_vol_sensitivities call"""
+    from .. import engine
+    names = list(greeks.params)
+    rows = np.vstack([_flat(greeks.delta), _flat(greeks.gamma), *(_flat(greeks.params[n]) for n in names)])
+    second = isinstance(greeks, FourierChainHessian)
+    vanna = np.vstack([_flat(greeks.vanna[n]) for n in names]) if second else None
+    hessian = np.vstack([_flat(greeks.hessian[p][q]) for i, p in enumerate(names) for q in names[i:]]) if second else None
+    ivols, g, v, h = engine.bsm_implied_vol_sensitivities(option_chain.ttms, option_chain.forwards, option_chain.discfactors,
+                                                          option_chain.strikes_ttms, option_chain.optiontypes_ttms, greeks.prices, rows,
+                                                          vanna, hessian)
+    offsets = np.zeros(len(ivols) + 1, dtype=np.int64)
+    offsets[1:] = np.cumsum([a.size for a in ivols])
+    split = lambda row: C.split_chain(row, offsets)
+    first = ChainIvolGreeks(ivols=ivols, delta=split(g[0]), gamma=split(g[1]), params={n: split(g[2 + k]) for k, n in enumerate(names)})
+    if not second:
+        return first
+    hess: Dict[str, Dict[str, List[np.ndarray]]] = {n: {} for n in names}
+    r = 0
+    for i, p in enumerate(names):
+        for q in names[i:]:
+            hess[p][q] = hess[q][p] = split(h[r])
+            r += 1
+    return ChainIvolHessian(ivols=first.ivols, delta=first.delta, gamma=first.gamma, params=first.params,
+                            vanna={n: split(v[k]) for k, n in enumerate(names)}, hessian=hess)
+
+
 def _check_fourier_kwargs(kwargs, method: str) -> None:
     if kwargs.get("is_analytic"):
         raise NotImplementedError(f"{method} does not cover the semi-analytic branch (is_analytic)")

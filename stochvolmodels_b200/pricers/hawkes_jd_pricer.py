@@ -28,7 +28,7 @@ from ..data.option_chain import OptionChain
 from ..multi_gpu import _shared_seed, _use_distributed, mc_chain_distributed
 from ..utils.config import VariableType
 from ..utils.funcs import set_time_grid, timer
-from .calibration import SLSQP_EPS, ScipyDifferenceObjective
+from .calibration import SLSQP_EPS, ExactGradientObjective, ScipyDifferenceObjective, check_gradient, flat_ivol_rows
 from .model_pricer import ModelParams, ModelPricer
 
 _KEYS = tuple(k for k, _ in C.HawkesParamsC._fields_)
@@ -166,8 +166,10 @@ class HawkesJDPricer(ModelPricer):
         start vector -- including its beta_m start 0.5 (beta2_p - beta2_m) --, bounds, stationarity constraint and SLSQP options).
         ``disp`` / ``maxiter`` (extras) are handed to SLSQP.  The 8 difference neighbours of a point whose gradient SLSQP asks for are priced
         in one ``hawkesjd_price_chain_batch`` call; objective and gradient are bit for bit what SLSQP differences from the one-set objective,
-        so the fit is too.  ``return_info``: (fit, {"fun", "nit", "nb_batches", "x", "nan_quotes"})."""
+        so the fit is too.  ``return_info``: (fit, {"fun", "nit", "nb_batches", "x", "nan_quotes"}).  ``gradient='exact'`` hands SLSQP the
+        exact gradient from one ``compute_chain_ivol_greeks`` call per point, on ``params0``'s default grid (DESIGN.md §4.6)."""
         from scipy.optimize import minimize
+        gradient = check_gradient(kwargs.get("gradient", "difference"))
         p0 = np.array([params0.sigma, params0.mean_p, params0.mean_m, params0.theta_p, params0.theta_m, 0.5 * (params0.kappa_p + params0.kappa_m),
                        0.5 * (params0.beta1_p - params0.beta2_p), 0.5 * (params0.beta2_p - params0.beta2_m)])
         bounds = ((0.10, 2.0), (0.01, 0.99), (-0.99, -0.01), (0.01, 100.0), (0.01, 100.0), (1.0, 100.0), (1.0, 100.0), (1.0, 100.0))
@@ -181,7 +183,11 @@ class HawkesJDPricer(ModelPricer):
         options = {"disp": bool(kwargs.get("disp", False)), "ftol": 1e-8}
         if "maxiter" in kwargs:
             options["maxiter"] = int(kwargs["maxiter"])
-        objective = _batched_vol_objective(option_chain, unpack, is_vega_weighted, is_unit_ttm_vega, bounds, SLSQP_EPS)
+        if gradient == "exact":
+            objective = _exact_vol_objective(self, option_chain, unpack, is_vega_weighted, is_unit_ttm_vega,
+                                             set_vol_scaler(params0.sigma, float(option_chain.ttms[0])))
+        else:
+            objective = _batched_vol_objective(option_chain, unpack, is_vega_weighted, is_unit_ttm_vega, bounds, SLSQP_EPS)
         res = minimize(objective.fun, p0, args=None, method="SLSQP", jac=objective.jac, constraints=stationary, bounds=bounds, options=options)
         fit = unpack(res.x)
         if return_info:
@@ -197,8 +203,12 @@ class HawkesJDPricer(ModelPricer):
         weights x 1e4, SLSQP with finite-difference step 0.025, ftol = tol = 1e-16).  Returns a new object; the reference mutates ``params0``.
         The 2 difference neighbours of a point whose gradient SLSQP asks for are priced in one risk-kernel ``hawkesjd_price_chain_batch``
         call, with the fit of the one-set objective bit for bit; ``print_iter`` prints a line per point in the order that objective would (the neighbours
-        only when SLSQP asks for the gradient).  ``return_info``: (fit, {"fun", "nit", "nb_batches", "x", "nan_quotes"})."""
+        only when SLSQP asks for the gradient).  ``return_info``: (fit, {"fun", "nit", "nb_batches", "x", "nan_quotes"}).  The risk kernel
+        has no sensitivities, so ``gradient='exact'`` raises NotImplementedError."""
         from scipy.optimize import minimize
+        if check_gradient(kwargs.get("gradient", "difference")) == "exact":
+            raise NotImplementedError("gradient='exact' does not cover calibrate_risk_premia_gamma_to_chain: the risk-kernel pricer has no "
+                                      "sensitivities")
         gamma_scaler = 8.0
         fixed = {k: v for k, v in params0.to_dict().items() if k in _KEYS}
         bounds = ((0.01, 1.5), (-1.0, 1.0))
@@ -306,17 +316,49 @@ def _fourier_chain(model_params: HawkesJDParams, ttms, forwards, discfactors, st
                                        MAX_PHI, gamma, return_grids)
 
 
+def _market_and_weights(option_chain: OptionChain, is_vega_weighted: bool, is_unit_ttm_vega: bool):
+    """(mid vols, objective weights) flat in chain order: per-slice normalised vegas, or ones"""
+    market = np.concatenate([np.asarray(v, dtype=float) for v in option_chain.get_mid_vols()])
+    if is_vega_weighted:
+        weights = np.concatenate([v / np.sum(v) for v in option_chain.get_chain_vegas(is_unit_ttm_vega=is_unit_ttm_vega)])
+    else:
+        weights = np.ones_like(market)
+    return market, weights
+
+
+# d HAWKES_GREEK_PARAMS / d x of calibrate_model_params_to_chain's x = (sigma, mean_p, mean_m, theta_p, theta_m, kappa, beta_p, beta_m):
+# kappa feeds kappa_p and kappa_m, beta_p feeds beta1_p = +x and beta2_p = -x, beta_m feeds beta1_m = +x and beta2_m = -x
+_HAWKES_FIT_FIELDS = ((("sigma", 1.0),), (("mean_p", 1.0),), (("mean_m", 1.0),), (("theta_p", 1.0),), (("theta_m", 1.0),),
+                      (("kappa_p", 1.0), ("kappa_m", 1.0)), (("beta1_p", 1.0), ("beta2_p", -1.0)), (("beta1_m", 1.0), ("beta2_m", -1.0)))
+
+
+def hawkes_fit_jacobian() -> np.ndarray:
+    D = np.zeros((len(engine.HAWKES_GREEK_PARAMS), len(_HAWKES_FIT_FIELDS)))
+    for col, fields in enumerate(_HAWKES_FIT_FIELDS):
+        for name, sign in fields:
+            D[engine.HAWKES_GREEK_PARAMS.index(name), col] = sign
+    return D
+
+
+def _exact_vol_objective(pricer, option_chain: OptionChain, to_params, is_vega_weighted: bool, is_unit_ttm_vega: bool,
+                         vol_scaler: float) -> ExactGradientObjective:
+    """the same objective with its exact gradient: one compute_chain_ivol_greeks call per point on the grid of ``vol_scaler``"""
+    market, weights = _market_and_weights(option_chain, is_vega_weighted, is_unit_ttm_vega)
+    D = hawkes_fit_jacobian()
+
+    def ivol_greeks(x: np.ndarray):
+        sens = pricer.compute_chain_ivol_greeks(option_chain, to_params(x), vol_scaler=vol_scaler)
+        return flat_ivol_rows(sens, engine.HAWKES_GREEK_PARAMS)
+    return ExactGradientObjective(ivol_greeks=ivol_greeks, field_jacobian=lambda x: D, market_vols=market, weights=weights)
+
+
 def _batched_vol_objective(option_chain: OptionChain, to_params, is_vega_weighted: bool, is_unit_ttm_vega: bool, bounds, eps: float,
                            scale: float = 1.0, on_point=None) -> ScipyDifferenceObjective:
     """the drivers' objective: weighted squared difference of model and mid implied vols, nansum over the chain (quotes whose model price
     leaves the no-arbitrage bounds drop out), with the weights of the reference (per-slice normalised vegas, times ``scale``).  The model vols
     of a point, and of its difference neighbours together, come from hawkesjd_price_chain_batch, on the risk-kernel route when the
     parameter sets carry a risk_premia_gamma -- the same prices and vols as compute_model_ivols_for_chain per set."""
-    market = np.concatenate([np.asarray(v, dtype=float) for v in option_chain.get_mid_vols()])
-    if is_vega_weighted:
-        weights = np.concatenate([v / np.sum(v) for v in option_chain.get_chain_vegas(is_unit_ttm_vega=is_unit_ttm_vega)])
-    else:
-        weights = np.ones_like(market)
+    market, weights = _market_and_weights(option_chain, is_vega_weighted, is_unit_ttm_vega)
 
     def batch_vols(points: np.ndarray) -> np.ndarray:
         sets = [to_params(p) for p in points]

@@ -84,10 +84,12 @@ class HestonPricer(ModelPricer):
     def calibrate_model_params_to_chain(self, option_chain: OptionChain, params0: HestonParams = None, is_vega_weighted: bool = True,
                                         is_unit_ttm_vega: bool = False, **kwargs) -> HestonParams:
         """fit (v0, theta, kappa, rho, volvol) to the chain's mid vols by SLSQP under the Feller constraint (reference :111-180); the
-        objective and its gradient are one batched GPU call per evaluation (pricers/calibration.py)."""
+        objective and its gradient are one batched GPU call per evaluation (pricers/calibration.py).  ``gradient='exact'`` hands SLSQP
+        the exact gradient from one ``compute_chain_ivol_greeks`` call per point, on the start point's default grid (DESIGN.md §4.6)."""
         from .calibration import calibrate_heston
         return calibrate_heston(self, option_chain, params0, is_vega_weighted, is_unit_ttm_vega, disp=bool(kwargs.get("disp", False)),
-                                return_info=bool(kwargs.get("return_info", False)), fd_step=kwargs.get("fd_step"))
+                                return_info=bool(kwargs.get("return_info", False)), fd_step=kwargs.get("fd_step"),
+                                gradient=kwargs.get("gradient", "difference"))
 
     def model_mc_price_chain(self, option_chain: OptionChain, params: HestonParams, nb_path: int = 100000,
                              variable_type: VariableType = VariableType.LOG_RETURN, **kwargs) -> Tuple[List[np.ndarray], List[np.ndarray]]:

@@ -214,14 +214,15 @@ class LogSVPricer(ModelPricer):
         """fit model parameters to the chain's mid implied vols: vega-weighted squared vol errors (Eq. (6.3)) minimised by SLSQP under
         ``constraints_type`` (reference :441-558; same arguments, bounds and return type).  The objective and its finite-difference
         gradient are ONE batched GPU call per optimizer evaluation (pricers/calibration.py).  ``return_info=True`` also returns
-        {fun, nit, nb_batches, x}."""
+        {fun, nit, nb_batches, x}.  ``gradient='exact'`` (ANALYTIC engine, PARAMS4 / PARAMS5) hands SLSQP the exact gradient of the
+        objective from one ``compute_chain_ivol_greeks`` call per point instead of the forward difference (DESIGN.md §4.6)."""
         params_min = params_min or LogSvParams(sigma0=0.1, theta=0.1, kappa1=0.25, kappa2=0.25, beta=-3.0, volvol=0.2)
         params_max = params_max or LogSvParams(sigma0=1.5, theta=1.5, kappa1=10.0, kappa2=10.0, beta=3.0, volvol=3.0)
         return calibrate_logsv(self, option_chain, params0, params_min, params_max, is_vega_weighted, is_unit_ttm_vega,
                                model_calibration_type, constraints_type, calibration_engine, nb_path, nb_steps, seed,
                                is_spot_measure=kwargs.get("is_spot_measure", True), disp=bool(kwargs.get("disp", False)),
                                return_info=bool(kwargs.get("return_info", False)), fd_step=kwargs.get("fd_step"),
-                               mc_randoms=kwargs.get("mc_randoms", "numpy"))
+                               mc_randoms=kwargs.get("mc_randoms", "numpy"), gradient=kwargs.get("gradient", "difference"))
 
     @timer
     def model_mc_price_chain(self, option_chain: OptionChain, params: LogSvParams, is_spot_measure: bool = True,
