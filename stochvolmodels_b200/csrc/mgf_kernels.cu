@@ -62,6 +62,13 @@ __device__ __forceinline__ cd exp_(cd z) {
   return cd{e * c, e * s};
 }
 __device__ __forceinline__ cd log_(cd z) { return cd{log(hypot(z.re, z.im)), atan2(z.im, z.re)}; }
+// exp_ with C99 cexp's exp(x ± 0i) = exp(x) ± 0i, which is numpy's: the summand of the strike sums at Im = 0 (grid point 0) whose exponent
+// overflows is then +inf, kept by np.nansum, instead of inf * sin(0) = NaN, skipped.  Used by the strike-sum kernels only; wherever exp_(z)
+// is finite the two agree bit for bit.
+__device__ __forceinline__ cd cexp_(cd z) {
+  const cd e = exp_(z);
+  return cd{e.re, z.im == 0.0 ? z.im : e.im};
+}
 
 // --------------------------------------------------------------------------------------------------------------------
 // LogSV affine expansion: per-grid-point coefficients of A' = A^T M A + L A + H (sparse, hand-expanded)
@@ -736,7 +743,7 @@ __global__ void __launch_bounds__(kFourierThreads) fourier_vanilla_kernel(const 
       const cd den = is_spot ? (ph + mk(1.0)) * ph : (ph - mk(1.0)) * ph;
       w = -(mk(dp / M_PI) / den);
     }
-    const cd term = w * exp_(lm[j] - x * ph);
+    const cd term = w * cexp_(lm[j] - x * ph);
     if (term.re == term.re) acc[0] += term.re;
   });
   if (threadIdx.x == 0) {
@@ -775,7 +782,7 @@ __global__ void __launch_bounds__(kFourierThreads) fourier_sum_kernel(const cd* 
       w = mk(dp / M_PI);                                        // dp/pi, :374-376
     else
       w = all_calls ? -(mk(dp / M_PI) / g) : (mk(dp / M_PI) / g);   // -/+ (dp/pi)/phi, :241-246
-    const cd term = w * exp_(sp.coef * g + lm[j]);
+    const cd term = w * cexp_(sp.coef * g + lm[j]);
     if (term.re == term.re) acc[0] += term.re;
   });
   if (threadIdx.x == 0) {
@@ -899,7 +906,7 @@ __global__ void __launch_bounds__(kFourierThreads) fourier_gamma_batch_kernel(co
     const cd ph = phi[j];
     const cd pg = ph + mk(gamma);
     const cd w = fast ? mk((dp / M_PI) / (ph.im * ph.im + 0.25)) : -(mk(dp / M_PI) / ((pg + mk(1.0)) * pg));
-    const cd term = w * exp_(lm[j] - x * ph);
+    const cd term = w * cexp_(lm[j] - x * ph);
     if (term.re == term.re) acc[0] += term.re;
   }
   block_sum<1, kFourierThreads>(acc, red);
@@ -1325,7 +1332,7 @@ __global__ void __launch_bounds__(kFourierThreads) fourier_vanilla_greeks_kernel
   double acc[3 + NP] = {};
   strike_sum(phi, P, acc, [&](int j, double dp, cd ph) {
     const double w = (dp / M_PI) / (ph.im * ph.im + 0.25);
-    const cd e = exp_(lm[j] - x * ph);
+    const cd e = cexp_(lm[j] - x * ph);
     const cd term = mk(w) * e;
     if (term.re == term.re) {
       acc[0] += term.re;
@@ -1651,7 +1658,7 @@ __global__ void __launch_bounds__(kFourierThreads) fourier_vanilla_hessian_kerne
   double acc[2 * NP + NH] = {};
   strike_sum(phi, P, acc, [&](int j, double dp, cd ph) {
     const double w = (dp / M_PI) / (ph.im * ph.im + 0.25);
-    const cd e = exp_(lm[j] - x * ph);
+    const cd e = cexp_(lm[j] - x * ph);
     const cd term = mk(w) * e;
     if (term.re == term.re) {
       cd dl[NP];
@@ -1706,7 +1713,7 @@ __global__ void __launch_bounds__(kFourierThreads) fourier_vanilla_hessian_split
   double acc[2 * NP] = {};
   strike_sum(phi, P, acc, [&](int j, double dp, cd ph) {
     const double w = (dp / M_PI) / (ph.im * ph.im + 0.25);
-    const cd e = exp_(lm[j] - x * ph);
+    const cd e = cexp_(lm[j] - x * ph);
     const cd term = mk(w) * e;
     if (term.re == term.re) {
       if (vanna_rows) {
