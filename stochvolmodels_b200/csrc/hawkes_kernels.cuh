@@ -212,9 +212,8 @@ __device__ __forceinline__ HawkesFast hawkes_fast(const HawkesConsts& c) {
 
 template <int GAUSS>
 __global__ void __launch_bounds__(kThreads, B200SV_HAWKES_MINBLOCKS) hawkes_slice_kernel(HawkesSliceArgs a, HawkesConsts c) {
-  __shared__ double red[2 * kThreads / 32];
   if constexpr (GAUSS != kGaussF32) gauss64_table_init();
-  double acc[2] = {0.0, 0.0};
+  SpotMoments<2, kThreads> mom;
   const uint2 key = make_uint2((uint32_t)a.seed, (uint32_t)(a.seed >> 32));
   const HawkesFast f = hawkes_fast(c);
   const long long stride = (long long)gridDim.x * kThreads;
@@ -233,17 +232,9 @@ __global__ void __launch_bounds__(kThreads, B200SV_HAWKES_MINBLOCKS) hawkes_slic
     a.x[i] = xi;
     a.lam_p[i] = lp;
     a.lam_m[i] = lm;
-    const double spot = a.forward * exp(xi);
-    if (spot == spot) {
-      acc[0] += spot;
-      acc[1] += 1.0;
-    }
+    mom.add(a.forward * exp(xi));
   }
-  block_sum<2, kThreads>(acc, red);
-  if (threadIdx.x == 0) {
-    a.partials[2 * blockIdx.x + 0] = acc[0];
-    a.partials[2 * blockIdx.x + 1] = acc[1];
-  }
+  mom.store(a.partials);
 }
 // ---- Monte Carlo sensitivities (DESIGN.md §3.11) -----------------------------------------------------------------------------
 // Directions in HAWKES_GREEK_PARAMS order: 0 sigma, 1 shift_p, 2 mean_p, 3 shift_m, 4 mean_m, 5..9 (lambda, theta, kappa, beta1, beta2)_p,
@@ -465,27 +456,21 @@ static int launch_hawkes_slice(double* x, double* lp, double* lm, long long n, l
   a.seed = seed;
   a.forward = forward;
   const HawkesConsts c = make_hawkes_consts(p, dt);
-  Grid grid = persistent_grid(hawkes_slice_kernel<kGaussF32>, kThreads, n);
-  const int K = tan ? 2 + kHawkesParams : 2;
-  ensure_pool_threshold();
-  DevBuf partials(st);
-  B200SV_CUDA(partials.alloc(sizeof(double) * K * grid.blocks));
-  a.partials = partials.as<double>();
-  if (tan) {
-    if (g == kGaussF64)
-      hawkes_tangent_slice_kernel<kGaussF64><<<grid.blocks, grid.threads, 0, st>>>(a, c, *tan);
-    else
-      hawkes_tangent_slice_kernel<kGaussF32><<<grid.blocks, grid.threads, 0, st>>>(a, c, *tan);
-    if (int rc = check_launch("hawkes_tangent_slice_kernel")) return rc;
-  } else {
-    if (g == kGaussF64)
-      hawkes_slice_kernel<kGaussF64><<<grid.blocks, grid.threads, 0, st>>>(a, c);
-    else
-      hawkes_slice_kernel<kGaussF32><<<grid.blocks, grid.threads, 0, st>>>(a, c);
-    if (int rc = check_launch("hawkes_slice_kernel")) return rc;
-  }
-  reduce_partials_kernel<<<1, 64, 0, st>>>(a.partials, grid.blocks, K, K, moments_out, make_publish(p2p, st));   // exchange #1 (producer)
-  return check_launch("reduce_partials_kernel");
+  const Grid grid = persistent_grid(hawkes_slice_kernel<kGaussF32>, kThreads, n);
+  return slice_moments(tan ? "hawkes_tangent_slice_kernel" : "hawkes_slice_kernel", tan ? 2 + kHawkesParams : 2, grid.blocks, moments_out, st, p2p,
+                       [&](double* partials) {
+                         a.partials = partials;
+                         if (tan) {
+                           if (g == kGaussF64)
+                             hawkes_tangent_slice_kernel<kGaussF64><<<grid.blocks, grid.threads, 0, st>>>(a, c, *tan);
+                           else
+                             hawkes_tangent_slice_kernel<kGaussF32><<<grid.blocks, grid.threads, 0, st>>>(a, c, *tan);
+                         } else if (g == kGaussF64) {
+                           hawkes_slice_kernel<kGaussF64><<<grid.blocks, grid.threads, 0, st>>>(a, c);
+                         } else {
+                           hawkes_slice_kernel<kGaussF32><<<grid.blocks, grid.threads, 0, st>>>(a, c);
+                         }
+                       });
 }
 
 constexpr int kHawkesStepsPerYear = 5 * 360;     // hawkes_jd_pricer.py:752
@@ -505,12 +490,8 @@ static int hawkes_chain_host(const b200sv_hawkes_params* p, int M, const double*
   B200SV_CUDA(d.alloc(sizeof(double) * 3 * N));
   if (int rc = io.upload(strikes)) return rc;
   double* x = d.as<double>();
-  double t0 = 0.0;
   for (int m = 0; m < M; ++m) {
-    int S;
-    double dt;
-    time_grid(ttms[m] - t0, kHawkesStepsPerYear, &S, &dt);
-    t0 = ttms[m];
+    const auto [S, dt] = maturity_grid(ttms, m, kHawkesStepsPerYear);
     if (int rc = launch_hawkes_slice(x, x + N, x + 2 * N, nb_path, 0, m == 0, *p, S, dt, m, forwards[m], seed, flags, io.moments(), st)) return rc;
     // compute_mc_vars_payoff(x0=x0, sigma0=x0, qvar0=x0, ...) (:703): the log-return array stands in for every argument
     if (int rc = io.payoff(0, m, x, x, false, nb_path, (double)nb_path, false)) return rc;
@@ -546,12 +527,8 @@ static int hawkes_chain_greeks_host(const b200sv_hawkes_params* p, int M, const 
   double* x = d.as<double>();
   const HawkesTangentArgs t{x + 3 * N, x + (3 + NP) * N, x + (3 + NP + L) * N, x + (3 + NP + 2 * L) * N};
   std::vector<double> h_paths(no * R * M);
-  double t0 = 0.0;
   for (int m = 0; m < M; ++m) {
-    int S;
-    double dt;
-    time_grid(ttms[m] - t0, kHawkesStepsPerYear, &S, &dt);
-    t0 = ttms[m];
+    const auto [S, dt] = maturity_grid(ttms, m, kHawkesStepsPerYear);
     if (int rc = launch_hawkes_slice(x, x + N, x + 2 * N, nb_path, 0, m == 0, *p, S, dt, m, forwards[m], seed, flags, io.moments(), st, nullptr, &t))
       return rc;
     if (int rc = io.payoff(m, x, x, t.dx, t.dx, (double)nb_path, t.score)) return rc;

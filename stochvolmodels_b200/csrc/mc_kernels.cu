@@ -311,7 +311,7 @@ struct SliceArgs {
   unsigned int slice;
   unsigned long long seed;
   double forward;
-  double* partials;   // [gridDim.x][2]
+  double* partials;   // [gridDim.x][K] re-centring moments (SpotMoments)
 };
 
 // advance one path through the slice, drawing its normals in the order philox.cuh defines.  SAFE = clamp the log-vol every step (re-run
@@ -379,44 +379,72 @@ __device__ __forceinline__ void run_slice_steps(Path& p, StepNormals<Real, GAUSS
   }
 }
 
-template <typename Path, typename Consts, typename Real, int GAUSS>
-__global__ void __launch_bounds__(kSliceThreads, B200SV_SLICE_MINBLOCKS) mc_slice_kernel(SliceArgs<Real> a, Consts consts) {
-  __shared__ double red[2 * kSliceThreads / 32];
-  exp_table_init();
-  if constexpr (GAUSS != kGaussF32) gauss64_table_init();
-  double acc[2] = {0.0, 0.0};
-  Path p(consts);
-  const long long stride = (long long)gridDim.x * kSliceThreads;
-  for (long long i = (long long)blockIdx.x * kSliceThreads + threadIdx.x; i < a.n; i += stride) {
-    Real xi = (Real)0, vi = (Real)a.v_init, qi = (Real)0;
-    if (!a.init) {
-      xi = a.x[i];
-      vi = a.v[i];
-      qi = a.q[i];
-    }
-    p.load(xi, vi, qi);
-    StepNormals<Real, GAUSS> rng(a.seed, a.path_offset + (unsigned long long)i, a.slice);
-    run_slice_steps<false>(p, rng, a.nsteps);
-    if (p.overflowed()) {      // rare: |log sigma| left [-700, 700] somewhere on this path -> redo it with the per-step clamp
-      p.load(xi, vi, qi);
-      run_slice_steps<true>(p, rng, a.nsteps);
-    }
-    const Real xT = p.x();
-    a.x[i] = xT;
-    a.v[i] = p.sigma();
-    a.q[i] = p.q();
-    // spots_t = forward*np.exp(x0); nanmean over all paths (utils/mc_payoffs.py:61-62)
-    const double spot = a.forward * exp((double)xT);
+// The re-centring moments of one CTA, row blockIdx.x of the partials [gridDim.x][K] that reduce_partials_kernel sums: (sum F e^x, count)
+// over the non-NaN spots (spots_t = forward*np.exp(x0), nanmean over all paths, utils/mc_payoffs.py:61-62) and, for K > 2, the K - 2
+// tangent terms sum F e^x d_k over the same spots.
+template <int K, int THREADS>
+struct SpotMoments {
+  double acc[K];
+  __device__ __forceinline__ SpotMoments() {
+#pragma unroll
+    for (int k = 0; k < K; ++k) acc[k] = 0.0;
+  }
+  __device__ __forceinline__ void add(double spot) {
     if (spot == spot) {
       acc[0] += spot;
       acc[1] += 1.0;
     }
   }
-  block_sum<2, kSliceThreads>(acc, red);
-  if (threadIdx.x == 0) {
-    a.partials[2 * blockIdx.x + 0] = acc[0];
-    a.partials[2 * blockIdx.x + 1] = acc[1];
+  // tangent term k, d = the path's k-th log-spot tangent.  A separate call per k: each kernel keeps its own order of the term and base
+  // updates (and of its tangent stores), which its SASS follows.
+  __device__ __forceinline__ void add_term(double spot, int k, double d) {
+    if (spot == spot) acc[2 + k] = fma(spot, d, acc[2 + k]);
   }
+  // block reduction, then thread 0 writes the CTA's row
+  __device__ __forceinline__ void store(double* __restrict__ partials) {
+    __shared__ double red[K * THREADS / 32];
+    block_sum<K, THREADS>(acc, red);
+    if (threadIdx.x == 0) {
+#pragma unroll
+      for (int k = 0; k < K; ++k) partials[K * blockIdx.x + k] = acc[k];
+    }
+  }
+};
+
+// One path of one slice: load the state (or start it from (0, v_init, 0)), step it, re-run it with the per-step clamp if the fast pass
+// left the representable log-vol range (rare: |log sigma| > 700 somewhere on the path), store it; returns the terminal x.
+template <typename Path, typename Real, int GAUSS>
+__device__ __forceinline__ Real slice_path(Path& p, const SliceArgs<Real>& a, long long i) {
+  Real xi = (Real)0, vi = (Real)a.v_init, qi = (Real)0;
+  if (!a.init) {
+    xi = a.x[i];
+    vi = a.v[i];
+    qi = a.q[i];
+  }
+  p.load(xi, vi, qi);
+  StepNormals<Real, GAUSS> rng(a.seed, a.path_offset + (unsigned long long)i, a.slice);
+  run_slice_steps<false>(p, rng, a.nsteps);
+  if (p.overflowed()) {
+    p.load(xi, vi, qi);
+    run_slice_steps<true>(p, rng, a.nsteps);
+  }
+  const Real xT = p.x();
+  a.x[i] = xT;
+  a.v[i] = p.sigma();
+  a.q[i] = p.q();
+  return xT;
+}
+
+template <typename Path, typename Consts, typename Real, int GAUSS>
+__global__ void __launch_bounds__(kSliceThreads, B200SV_SLICE_MINBLOCKS) mc_slice_kernel(SliceArgs<Real> a, Consts consts) {
+  exp_table_init();
+  if constexpr (GAUSS != kGaussF32) gauss64_table_init();
+  SpotMoments<2, kSliceThreads> mom;
+  Path p(consts);
+  const long long stride = (long long)gridDim.x * kSliceThreads;
+  for (long long i = (long long)blockIdx.x * kSliceThreads + threadIdx.x; i < a.n; i += stride)
+    mom.add(a.forward * exp((double)slice_path<Path, Real, GAUSS>(p, a, i)));
+  mom.store(a.partials);
 }
 
 // out[k] = sum_b partials[b*K + k] for k < K_out, fixed order: one warp per k, lanes stride over b, shuffle tree.
@@ -580,26 +608,27 @@ __global__ void __launch_bounds__(kThreads) logsv_vol_paths_kernel(double* __res
 // (sum F e^x over non-NaN, count) partials for externally supplied states (b200sv_mc_payoffs)
 __global__ void __launch_bounds__(kThreads) spot_moments_kernel(const double* __restrict__ x, long long n, double forward,
                                                                double* __restrict__ partials) {
-  __shared__ double red[2 * kThreads / 32];
-  double acc[2] = {0.0, 0.0};
+  SpotMoments<2, kThreads> mom;
   const long long stride = (long long)gridDim.x * kThreads;
-  for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < n; i += stride) {
-    const double spot = forward * exp(x[i]);
-    if (spot == spot) {
-      acc[0] += spot;
-      acc[1] += 1.0;
-    }
-  }
-  block_sum<2, kThreads>(acc, red);
-  if (threadIdx.x == 0) {
-    partials[2 * blockIdx.x + 0] = acc[0];
-    partials[2 * blockIdx.x + 1] = acc[1];
-  }
+  for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < n; i += stride) mom.add(forward * exp(x[i]));
+  mom.store(partials);
 }
 
 // --------------------------------------------------------------------------------------------------------------------
 // payoff sums: utils/mc_payoffs.py:61-88
 // --------------------------------------------------------------------------------------------------------------------
+// The strikes and payoff codes of the C strikes from j0 on; a slot past the slice's J strikes has ty = -1
+template <int C>
+__device__ __forceinline__ void load_strike_chunk(const double* __restrict__ strikes, const int8_t* __restrict__ types, int J, int j0,
+                                                  double (&kk)[C], int (&ty)[C]) {
+#pragma unroll
+  for (int c = 0; c < C; ++c) {
+    const int j = j0 + c;
+    kk[c] = j < J ? strikes[j] : 0.0;
+    ty[c] = j < J ? (int)types[j] : -1;
+  }
+}
+
 // General payoffs (any mix of C / P / IC / IP): per-strike NaN-skipping counts, IEEE division for the inverse payoffs.
 // payoff_general_block / payoff_vanilla_block: the work of ONE CTA for the strike chunk starting at j0 -- grid-stride over the paths with
 // `nblocks` CTAs, block-reduce, write this CTA's partial row.  Called by the stand-alone payoff kernels (blockIdx.y = chunk) and by the
@@ -611,12 +640,7 @@ __device__ __forceinline__ void payoff_general_block(const Real* __restrict__ x,
   __shared__ double red[3 * kStrikeChunk * kThreads / 32];
   double kk[kStrikeChunk];
   int ty[kStrikeChunk];
-#pragma unroll
-  for (int c = 0; c < kStrikeChunk; ++c) {
-    const int j = j0 + c;
-    kk[c] = j < J ? strikes[j] : 0.0;
-    ty[c] = j < J ? (int)types[j] : -1;
-  }
+  load_strike_chunk(strikes, types, J, j0, kk, ty);
   const bool is_qvar = variable_type == B200SV_Q_VAR;
   double acc[3 * kStrikeChunk];
 #pragma unroll
@@ -813,24 +837,9 @@ __global__ void __launch_bounds__(kSliceThreads, B200SV_SLICE_MINBLOCKS) mc_chai
     {
       double acc[2] = {0.0, 0.0};
       Path p(sp.c);
+      const SliceArgs<double> s{a.x, a.v, a.q, a.n, 0ull, m == 0, a.v_init, sp.nsteps, (unsigned int)m, a.seed, sp.forward, a.part_mom};
       for (long long i = (long long)blockIdx.x * kSliceThreads + threadIdx.x; i < a.n; i += stride) {
-        double xi = 0.0, vi = a.v_init, qi = 0.0;
-        if (m > 0) {
-          xi = a.x[i];
-          vi = a.v[i];
-          qi = a.q[i];
-        }
-        p.load(xi, vi, qi);
-        StepNormals<double, GAUSS> rng(a.seed, (unsigned long long)i, (unsigned int)m);
-        run_slice_steps<false>(p, rng, sp.nsteps);
-        if (p.overflowed()) {
-          p.load(xi, vi, qi);
-          run_slice_steps<true>(p, rng, sp.nsteps);
-        }
-        const double xT = p.x();
-        a.x[i] = xT;
-        a.v[i] = p.sigma();
-        a.q[i] = p.q();
+        const double xT = slice_path<Path, double, GAUSS>(p, s, i);
         const double spot = sp.forward * exp(xT);
         if (spot == spot) {
           acc[0] += spot;
@@ -1191,11 +1200,7 @@ __device__ __forceinline__ void payoff_greeks_body(const double* __restrict__ x,
   const int j0 = blockIdx.y * kGreeksStrikeChunk;
   double kk[kGreeksStrikeChunk];
   int ty[kGreeksStrikeChunk];
-#pragma unroll
-  for (int c = 0; c < kGreeksStrikeChunk; ++c) {
-    kk[c] = j0 + c < J ? strikes[j0 + c] : 0.0;
-    ty[c] = j0 + c < J ? (int)types[j0 + c] : -1;
-  }
+  load_strike_chunk(strikes, types, J, j0, kk, ty);
   const bool is_qvar = variable_type == B200SV_Q_VAR;
   const double inv_f = 1.0 / forward, inv_ttm = 1.0 / ttm;
   double acc[KC];
@@ -1313,11 +1318,7 @@ __global__ void __launch_bounds__(kThreads) payoff_gamma_kernel(const double* __
   const int j0 = blockIdx.y * kGammaStrikeChunk;
   double kk[kGammaStrikeChunk];
   int ty[kGammaStrikeChunk];
-#pragma unroll
-  for (int c = 0; c < kGammaStrikeChunk; ++c) {
-    kk[c] = j0 + c < J ? strikes[j0 + c] : 0.0;
-    ty[c] = j0 + c < J ? (int)types[j0 + c] : -1;
-  }
+  load_strike_chunk(strikes, types, J, j0, kk, ty);
   const bool is_qvar = variable_type == B200SV_Q_VAR;
   const double inv_f = 1.0 / forward, inv_f2 = inv_f * inv_f, inv_ttm = 1.0 / ttm;
   constexpr double kInvSqrt2Pi = 0.3989422804014326779;
@@ -1522,10 +1523,16 @@ static P2pGather make_gather(P2pCtx* c) {
 }
 
 // int(ttm * n) + 1 and dt = linspace(0, ttm, S+1)[1] - [0] (utils/funcs.py:44-47; numpy linspace: step = ttm / S, y[1] = 1*step)
-static void time_grid(double ttm, int n_per_year, int* S, double* dt) {
-  *S = (int)(ttm * (double)n_per_year) + 1;
-  *dt = (*S == 1) ? ttm : ttm / (double)(*S);   // linspace sets the LAST point to `stop` exactly; with S == 1 y[1] is that point
+struct StepGrid {
+  int S;
+  double dt;
+};
+static StepGrid time_grid(double ttm, int n_per_year) {
+  const int S = (int)(ttm * (double)n_per_year) + 1;
+  return {S, (S == 1) ? ttm : ttm / (double)S};   // linspace sets the LAST point to `stop` exactly; with S == 1 y[1] is that point
 }
+// the slice of maturity m of a chain: from ttms[m - 1] (0 for the first) to ttms[m]
+static StepGrid maturity_grid(const double* ttms, int m, int n_per_year) { return time_grid(ttms[m] - (m > 0 ? ttms[m - 1] : 0.0), n_per_year); }
 
 // B200SV_GAUSS_* bits -> GaussMode (philox.cuh); -1 = contradictory
 static int gauss_mode(int flags) {
@@ -1577,6 +1584,20 @@ static CoopKernel<HestonConsts> coop_kernel(const HestonConsts& c, int g) {
 }
 
 // ---- launchers ---------------------------------------------------------------------------------------------------------
+// The re-centring moments of a slice: launch(partials) enqueues the slice kernel on `blocks` CTAs, each writing its row of the partials
+// [blocks][K] (SpotMoments), then reduce_partials_kernel sums them in fixed order into moments_out[K] and, with a P2P context, publishes
+// them to the peers (exchange #1, producer).
+template <class Launch>
+static int slice_moments(const char* what, int K, int blocks, double* moments_out, cudaStream_t st, P2pCtx* p2p, Launch launch) {
+  ensure_pool_threshold();      // device-level callers too: a pool that trims at every synchronisation stalls the whole node (DESIGN.md 5)
+  DevBuf partials(st);
+  B200SV_CUDA(partials.alloc(sizeof(double) * K * (size_t)blocks));
+  launch(partials.as<double>());
+  if (int rc = check_launch(what)) return rc;
+  reduce_partials_kernel<<<1, 64, 0, st>>>(partials.as<double>(), blocks, K, K, moments_out, make_publish(p2p, st));
+  return check_launch("reduce_partials_kernel");
+}
+
 // one maturity slice on paths [path_offset, path_offset + n), then their re-centring moments (sum F e^x, count) into moments_out
 template <typename Real, typename Consts>
 static int launch_slice_k(SliceKernel<Real, Consts> kernel, void* x, void* v, void* q, long long n, long long path_offset, int init,
@@ -1595,15 +1616,11 @@ static int launch_slice_k(SliceKernel<Real, Consts> kernel, void* x, void* v, vo
     }
   }
 #endif
-  ensure_pool_threshold();      // device-level callers too: a pool that trims at every synchronisation stalls the whole node (DESIGN.md 5)
-  DevBuf partials(st);
-  B200SV_CUDA(partials.alloc(sizeof(double) * 2 * g.blocks));
-  const SliceArgs<Real> a{(Real*)x, (Real*)v, (Real*)q, n, (unsigned long long)path_offset, init, v_init, nsteps, (unsigned int)slice_index,
-                          seed, forward, partials.as<double>()};
-  kernel<<<g.blocks, g.threads, dyn_smem, st>>>(a, c);
-  if (int rc = check_launch("mc_slice_kernel")) return rc;
-  reduce_partials_kernel<<<1, 64, 0, st>>>(a.partials, g.blocks, 2, 2, moments_out, make_publish(p2p, st));   // exchange #1 (producer)
-  return check_launch("reduce_partials_kernel");
+  return slice_moments("mc_slice_kernel", 2, g.blocks, moments_out, st, p2p, [&](double* partials) {
+    const SliceArgs<Real> a{(Real*)x, (Real*)v, (Real*)q, n, (unsigned long long)path_offset, init, v_init, nsteps, (unsigned int)slice_index,
+                            seed, forward, partials};
+    kernel<<<g.blocks, g.threads, dyn_smem, st>>>(a, c);
+  });
 }
 
 template <typename Consts>
@@ -1647,14 +1664,10 @@ static int launch_payoff_t(const void* x, const void* q, long long n, double ttm
 }
 
 static int spot_moments_impl(const double* x, long long n, double forward, double* moments_out, cudaStream_t st, P2pCtx* p2p) {
-  Grid g = persistent_grid(spot_moments_kernel, kThreads, n);
-  ensure_pool_threshold();
-  DevBuf partials(st);
-  B200SV_CUDA(partials.alloc(sizeof(double) * 2 * g.blocks));
-  spot_moments_kernel<<<g.blocks, g.threads, 0, st>>>(x, n, forward, partials.as<double>());
-  if (int rc = check_launch("spot_moments_kernel")) return rc;
-  reduce_partials_kernel<<<1, 64, 0, st>>>(partials.as<double>(), g.blocks, 2, 2, moments_out, make_publish(p2p, st));
-  return check_launch("reduce_partials_kernel");
+  const Grid g = persistent_grid(spot_moments_kernel, kThreads, n);
+  return slice_moments("spot_moments_kernel", 2, g.blocks, moments_out, st, p2p, [&](double* partials) {
+    spot_moments_kernel<<<g.blocks, g.threads, 0, st>>>(x, n, forward, partials);
+  });
 }
 
 static int payoff_kinds(const int8_t* types, int J) {
@@ -1922,12 +1935,8 @@ static int mc_chain_host_coop(const Params* params, int M, const double* ttms, c
   }
   Spec* h_specs = (Spec*)(h_in.data() + sizeof(double) * Jalloc);
   for (int b = 0; b < B; ++b) {
-    double t0 = 0.0;
     for (int m = 0; m < M; ++m) {
-      int S;
-      double dt;
-      time_grid(ttms[m] - t0, nb_steps_per_year, &S, &dt);
-      t0 = ttms[m];
+      const auto [S, dt] = maturity_grid(ttms, m, nb_steps_per_year);
       const int J = offsets[m + 1] - offsets[m];
       Spec& sp = h_specs[(size_t)b * M + m];
       sp.c = slice_consts(params[b], etas ? etas[(size_t)b * M + m] : 1.0, is_spot != 0, dt, scheme);
@@ -2009,12 +2018,8 @@ static int mc_chain_host(const Params* params, int M, const double* ttms, const 
   if (int rc = io.upload(strikes)) return rc;
   char *x = state.as<char>(), *v = x + esz * (size_t)nb_path, *q = x + 2 * esz * (size_t)nb_path;
   for (int b = 0; b < B; ++b) {
-    double t0 = 0.0;
     for (int m = 0; m < M; ++m) {
-      int S;
-      double dt;
-      time_grid(ttms[m] - t0, nb_steps_per_year, &S, &dt);
-      t0 = ttms[m];
+      const auto [S, dt] = maturity_grid(ttms, m, nb_steps_per_year);
       const auto c = slice_consts(params[b], etas ? etas[(size_t)b * M + m] : 1.0, is_spot != 0, dt, scheme);
       if (int rc = launch_slice(x, v, q, nb_path, 0, m == 0, v_init(params[b]), S, m, forwards[m], seed, flags, c, io.moments(), st)) return rc;
       if (int rc = io.payoff(b, m, x, q, f32, nb_path, (double)nb_path, ivols_out != nullptr)) return rc;
@@ -2035,9 +2040,7 @@ static int terminal_host(const Params& p, double ttm, long long nb_path, int nb_
   DevBuf d_mom(st);
   if (int rc = s.alloc(false)) return rc;
   B200SV_CUDA(d_mom.alloc(sizeof(double) * 2));
-  int S;
-  double dt;
-  time_grid(ttm, nb_steps_per_year, &S, &dt);
+  const auto [S, dt] = time_grid(ttm, nb_steps_per_year);
   const auto c = slice_consts(p, eta, is_spot != 0, dt, scheme);
   if (int rc = launch_slice(s.dev(0), s.dev(1), s.dev(2), nb_path, 0, 1, v_init(p), S, 0, 1.0, seed, flags, c, d_mom.as<double>(), st)) return rc;
   if (int rc = s.download()) return rc;
@@ -2062,22 +2065,17 @@ static int launch_tangent_slice(int gauss, double* x, double* v, double* q, cons
                                 cudaStream_t st, double* laststep = nullptr) {
   using TPath = TangentPathOf<TConsts>;
   using RPath = LastStepPath<TPath>;
-  constexpr int K = 2 + TPath::NP;
   const auto kernel = gauss == kGaussF64 ? mc_tangent_slice_kernel<TPath, kGaussF64> : mc_tangent_slice_kernel<TPath, kGaussF32>;
   const Grid g = persistent_grid(kernel, kSliceThreads, n);
-  DevBuf partials(st);
-  B200SV_CUDA(partials.alloc(sizeof(double) * K * g.blocks));
-  const SliceArgs<double> a{x, v, q, n, (unsigned long long)path_offset, init, v_init, nsteps, (unsigned int)slice_index, seed, forward,
-                            partials.as<double>()};
-  if (laststep) {
-    const auto rkernel = gauss == kGaussF64 ? mc_tangent_slice_kernel<RPath, kGaussF64> : mc_tangent_slice_kernel<RPath, kGaussF32>;
-    rkernel<<<g.blocks, g.threads, 0, st>>>(a, t, LastStepConsts<TPath>{c, laststep});
-  } else {
-    kernel<<<g.blocks, g.threads, 0, st>>>(a, t, c);
-  }
-  if (int rc = check_launch("mc_tangent_slice_kernel")) return rc;
-  reduce_partials_kernel<<<1, 64, 0, st>>>(a.partials, g.blocks, K, K, moments_out, P2pPublish{});
-  return check_launch("reduce_partials_kernel");
+  return slice_moments("mc_tangent_slice_kernel", 2 + TPath::NP, g.blocks, moments_out, st, nullptr, [&](double* partials) {
+    const SliceArgs<double> a{x, v, q, n, (unsigned long long)path_offset, init, v_init, nsteps, (unsigned int)slice_index, seed, forward, partials};
+    if (laststep) {
+      const auto rkernel = gauss == kGaussF64 ? mc_tangent_slice_kernel<RPath, kGaussF64> : mc_tangent_slice_kernel<RPath, kGaussF32>;
+      rkernel<<<g.blocks, g.threads, 0, st>>>(a, t, LastStepConsts<TPath>{c, laststep});
+    } else {
+      kernel<<<g.blocks, g.threads, 0, st>>>(a, t, c);
+    }
+  });
 }
 
 // chain driver: per maturity tangent slice -> moments -> per-strike payoff / sensitivity sums -> finalize (stand-alone launches, fixed-order
@@ -2110,12 +2108,8 @@ static int mc_chain_greeks_host(const Params& p, int M, const double* ttms, cons
   double *x = d_state.as<double>(), *v = x + n, *q = v + n;
   const TangentState t{q + n, q + n + NP * n, q + n + 2 * NP * n};
   double* laststep = with_gamma ? q + n + 3 * NP * n : nullptr;     // [2][n], reused across maturities
-  double t0 = 0.0;
   for (int m = 0; m < M; ++m) {
-    int S;
-    double dt;
-    time_grid(ttms[m] - t0, nb_steps_per_year, &S, &dt);
-    t0 = ttms[m];
+    const auto [S, dt] = maturity_grid(ttms, m, nb_steps_per_year);
     const TConsts c = tangent_consts(p, etas ? etas[m] : 1.0, is_spot != 0, dt);
     if (int rc = launch_tangent_slice(gauss, x, v, q, t, nb_path, 0, m == 0, v_init(p), S, m, forwards[m], seed, c, io.moments(), st, laststep))
       return rc;
@@ -2151,9 +2145,7 @@ static int tangent_terminal_host(const Params& p, double ttm, long long nb_path,
   if (int rc = ds.alloc(false)) return rc;
   B200SV_CUDA(d_mom.alloc(sizeof(double) * (2 + NP)));
   const TangentState t{ds.dev(0), ds.dev(1), ds.dev(2)};
-  int S;
-  double dt;
-  time_grid(ttm, nb_steps_per_year, &S, &dt);
+  const auto [S, dt] = time_grid(ttm, nb_steps_per_year);
   const TConsts c = tangent_consts(p, eta, is_spot != 0, dt);
   if (int rc = launch_tangent_slice(gauss, s.dev(0), s.dev(1), s.dev(2), t, nb_path, path_offset, 1, v_init(p), S, slice_index, 1.0, seed, c,
                                     d_mom.as<double>(), st))
@@ -2332,9 +2324,7 @@ int b200sv_logsv_terminal_from_state(const b200sv_logsv_params* params, double t
   DevBuf d_mom(st);
   if (int rc = s.alloc(true)) return rc;
   B200SV_CUDA(d_mom.alloc(sizeof(double) * 2));
-  int S;
-  double dt;
-  time_grid(ttm, nb_steps_per_year, &S, &dt);
+  const auto [S, dt] = time_grid(ttm, nb_steps_per_year);
   const LogsvConsts c = make_logsv_consts(*params, eta, is_spot_measure != 0, dt);
   if (int rc = launch_slice(s.dev(0), s.dev(1), s.dev(2), nb_path, 0, 0, params->sigma0, S, slice_index, 1.0, seed, flags, c, d_mom.as<double>(), st))
     return rc;
@@ -2598,9 +2588,7 @@ int b200sv_logsv_vol_paths(const b200sv_logsv_params* params, double ttm, long l
                            uint64_t seed, const double* brownians, double* sigma_t_out) {
   B200SV_REQUIRE(params && sigma_t_out, "null pointer");
   B200SV_REQUIRE(nb_path >= 1 && ttm > 0.0 && nb_steps_per_year >= 1, "nb_path, ttm, nb_steps_per_year must be positive");
-  int S;
-  double dt;
-  time_grid(ttm, nb_steps_per_year, &S, &dt);
+  const auto [S, dt] = time_grid(ttm, nb_steps_per_year);
   // adj = beta under the inverse measure, no eta (pricers/logsv_pricer.py:929-932)
   LogsvRaw r{params->theta, params->kappa1, params->kappa2, params->beta, params->volvol, 1.0, is_spot_measure ? -1.0 : 1.0,
              is_spot_measure ? 0.0 : params->beta, dt};
@@ -2675,9 +2663,7 @@ int b200sv_hawkesjd_terminal(const b200sv_hawkes_params* params, double ttm, lon
   DevBuf d_mom(st);
   if (int rc = s.alloc(use_initial_arrays != 0)) return rc;
   B200SV_CUDA(d_mom.alloc(sizeof(double) * 2));
-  int S;
-  double dt;
-  time_grid(ttm, kHawkesStepsPerYear, &S, &dt);
+  const auto [S, dt] = time_grid(ttm, kHawkesStepsPerYear);
   if (int rc = launch_hawkes_slice(s.dev(0), s.dev(1), s.dev(2), nb_path, 0, use_initial_arrays ? 0 : 1, *params, S, dt, slice_index, 1.0, seed,
                                    flags, d_mom.as<double>(), st))
     return rc;

@@ -163,6 +163,16 @@ struct RoughPath {
 #pragma unroll
     for (int i = 0; i < N; ++i) v[i] = u[i];
   }
+  // path i's terminal state: log_spot_out / qv_out [P], vol_out [N][P] (may be nullptr)
+  __device__ __forceinline__ void store(double* __restrict__ log_spot_out, double* __restrict__ vol_out, double* __restrict__ qv_out, long long P,
+                                        long long i) const {
+    log_spot_out[i] = ls;
+    qv_out[i] = y;
+    if (vol_out) {
+#pragma unroll
+      for (int k = 0; k < N; ++k) vol_out[(size_t)k * P + i] = v[k];
+    }
+  }
 };
 
 // Z0 / Z1 != nullptr: caller-supplied unit normals, row-major [S][P] (device); else in-kernel Philox draws (stream of philox.cuh with
@@ -209,12 +219,7 @@ __global__ void __launch_bounds__(kThreads) rough_logsv_kernel(double* __restric
     RoughPath<N> p;
     p.init(c);
     rough_run_path<GAUSS>(p, c, Z0, Z1, S, P, i, seed, path_offset);
-    log_spot_out[i] = p.ls;
-    qv_out[i] = p.y;
-    if (vol_out) {
-#pragma unroll
-      for (int k = 0; k < N; ++k) vol_out[(size_t)k * P + i] = p.v[k];
-    }
+    p.store(log_spot_out, vol_out, qv_out, P, i);
   }
 }
 
@@ -411,24 +416,15 @@ __global__ void __launch_bounds__(kThreads) rough_logsv_tangent_kernel(double* _
                                                                       const double* __restrict__ Z0, const double* __restrict__ Z1, int S, long long P,
                                                                       RoughConsts c, const __grid_constant__ RoughTangentConsts k,
                                                                       unsigned long long seed, double forward, double* __restrict__ partials) {
-  constexpr int K = 2 + kRoughParams;
-  __shared__ double red[K * kThreads / 32];
   exp_table_init();
   if constexpr (GAUSS != kGaussF32) gauss64_table_init();
-  double acc[K];
-#pragma unroll
-  for (int j = 0; j < K; ++j) acc[j] = 0.0;
+  SpotMoments<2 + kRoughParams, kThreads> mom;
   const long long stride = (long long)gridDim.x * kThreads;
   for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < P; i += stride) {
     RoughTangentPath<N> t(k);
     t.init(c);
     rough_run_path<GAUSS>(t, c, Z0, Z1, S, P, i, seed, 0ull);
-    log_spot_out[i] = t.p.ls;
-    qv_out[i] = t.p.y;
-    if (vol_out) {
-#pragma unroll
-      for (int f = 0; f < N; ++f) vol_out[(size_t)f * P + i] = t.p.v[f];
-    }
+    t.p.store(log_spot_out, vol_out, qv_out, P, i);
     const double spot = forward * exp(t.p.ls);
 #pragma unroll
     for (int q = 0; q < kRoughParams; ++q) {
@@ -438,19 +434,12 @@ __global__ void __launch_bounds__(kThreads) rough_logsv_tangent_kernel(double* _
 #pragma unroll
         for (int f = 0; f < N; ++f) dvol_out[((size_t)q * N + f) * P + i] = t.dv[q][f];
       }
-      if (spot == spot) acc[2 + q] = fma(spot, t.dls[q], acc[2 + q]);
+      mom.add_term(spot, q, t.dls[q]);
     }
-    if (spot == spot) {
-      acc[0] += spot;
-      acc[1] += 1.0;
-    }
+    mom.add(spot);
     if (t.any_reset) atomicAdd(k.reset_count, 1ull);
   }
-  block_sum<K, kThreads>(acc, red);
-  if (threadIdx.x == 0) {
-#pragma unroll
-    for (int j = 0; j < K; ++j) partials[K * blockIdx.x + j] = acc[j];
-  }
+  mom.store(partials);
 }
 
 // one maturity of the rough chain with tangents, then moments_out[2 + 6] = (sum F e^ls, count, sum F e^ls dls_q).  Both Gauss modes launch on
@@ -458,17 +447,13 @@ __global__ void __launch_bounds__(kThreads) rough_logsv_tangent_kernel(double* _
 static int launch_rough_tangent(int n, double* ls, double* vol, double* qv, double* dls, double* dvol, double* dqv, const double* Z0,
                                 const double* Z1, int S, long long P, const RoughConsts& c, const RoughTangentConsts& k, uint64_t seed, int gauss,
                                 double forward, double* moments_out, cudaStream_t st) {
-  constexpr int K = 2 + kRoughParams;
   return with_factors(n, [&](auto nf) {
     constexpr int N = decltype(nf)::value;
     const int blocks = persistent_grid(rough_logsv_tangent_kernel<N, kGaussF32>, kThreads, P).blocks;
     const auto kernel = gauss == kGaussF64 ? rough_logsv_tangent_kernel<N, kGaussF64> : rough_logsv_tangent_kernel<N, kGaussF32>;
-    DevBuf partials(st);
-    B200SV_CUDA(partials.alloc(sizeof(double) * K * (size_t)blocks));
-    kernel<<<blocks, kThreads, 0, st>>>(ls, vol, qv, dls, dvol, dqv, Z0, Z1, S, P, c, k, seed, forward, partials.as<double>());
-    if (int rc = check_launch("rough_logsv_tangent_kernel")) return rc;
-    reduce_partials_kernel<<<1, 64, 0, st>>>(partials.as<double>(), blocks, K, K, moments_out, P2pPublish{});
-    return check_launch("reduce_partials_kernel");
+    return slice_moments("rough_logsv_tangent_kernel", 2 + kRoughParams, blocks, moments_out, st, nullptr, [&](double* partials) {
+      kernel<<<blocks, kThreads, 0, st>>>(ls, vol, qv, dls, dvol, dqv, Z0, Z1, S, P, c, k, seed, forward, partials);
+    });
   });
 }
 
