@@ -259,6 +259,19 @@ int b200sv_dev_logsv_step_fixed(double* x, double* sigma, double* qvar, const do
 int b200sv_dev_heston_step_fixed(double* x, double* var, double* qvar, const double* W0, const double* W1, int S,
                                  long long N, double dt, const b200sv_heston_params* params, void* stream);
 
+/* Pathwise sensitivities of the LogSV chain on fixed unit normals resident on the device (DESIGN.md §4.7): W0s[m], W1s[m] are device
+ * arrays [nsteps[m]][N] (row-major) of maturity m, stepped with dts[m] by the fast stepper above.  The chain block (ttms ... types, etas
+ * [M] or NULL for ones) is on the HOST, as for the host-level chain calls.  Outputs are DEVICE arrays: prices_out, stderr_out [J_total]
+ * bit-identical to b200sv_dev_logsv_step_fixed(fast = 1) + b200sv_dev_spot_moments + b200sv_dev_payoff_sums + b200sv_dev_payoff_finalize
+ * on the same normals, parameters, etas and measure, and greeks_out / greeks_se_out [1 + 6][J_total]: row 0 the forward delta, then
+ * d price / d (sigma0, theta, kappa1, kappa2, beta, volvol) in struct field order, with standard errors discfactor * std(g) / sqrt(N).
+ * Asynchronous on `stream`. */
+int b200sv_dev_logsv_mc_chain_greeks_fixed(const b200sv_logsv_params* params, int M, const double* ttms, const double* forwards,
+                                           const double* discfactors, const double* etas, const int* offsets, const double* strikes,
+                                           const int8_t* types, const double* const* W0s, const double* const* W1s, const int* nsteps,
+                                           const double* dts, long long N, int is_spot_measure, int variable_type, double* prices_out,
+                                           double* stderr_out, double* greeks_out, double* greeks_se_out, void* stream);
+
 /* Rough-LogSV multi-factor Monte Carlo chain (Markovian lift of the rough kernel, 1 <= n_factors <= 8):
  * rough_logsv_mc_chain_pricer_fixed_randoms (pricers/logsv_pricer.py:1164-1232) -> log_spot_full_combined
  * (pricers/rough_logsv/split_simulation.py:466-479, f64 branch :340-361).  params[b].volvol carries the ORTHOGONAL vol-of-vol of set b

@@ -112,6 +112,8 @@ SIGNATURES = {
     "b200sv_dev_logsv_step_fixed": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_double, _lp, c_double,
                                     c_int, c_int, c_void_p],
     "b200sv_dev_heston_step_fixed": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_longlong, c_double, _hp, c_void_p],
+    "b200sv_dev_logsv_mc_chain_greeks_fixed": [_lp, c_int, _dp, _dp, _dp, _dp, _ip, _dp, _i8p, POINTER(c_void_p), POINTER(c_void_p), _ip, _dp,
+                                               c_longlong, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     "b200sv_dev_spot_moments": [c_void_p, c_longlong, c_double, c_void_p, c_void_p],
     "b200sv_dev_hawkesjd_slice": [c_void_p, c_void_p, c_void_p, c_longlong, c_longlong, c_int, _kp, c_int, c_double, c_int, c_double, c_uint64,
                                   c_int, c_void_p, c_void_p, c_void_p],

@@ -1176,6 +1176,47 @@ __global__ void __launch_bounds__(kSliceThreads, B200SV_SLICE_MINBLOCKS) mc_tang
   }
 }
 
+// logsv_step_fixed_fast_kernel with the LogSV tangents (DESIGN.md §4.7): the same unit normals W0, W1 [S][n] read from HBM and the same
+// clamped primal step (LogsvTangentPath::step<true> calls LogsvPath<double>::step<true> unchanged), so the state it writes back is the fast
+// kernel's bit for bit; a.init starts every path at (0, v_init, 0) with the initial tangents.  Per-CTA partials [gridDim.x][2 + P] of
+// SpotMoments over the new x: the chain driver keeps the P tangent terms (sum F e^x dx_p) and takes the two re-centring moments from
+// spot_moments_impl, as the pricing route does.
+__global__ void __launch_bounds__(kThreads, B200SV_SLICE_MINBLOCKS) logsv_tangent_step_fixed_kernel(SliceArgs<double> a, TangentState t,
+                                                                                                  const double* __restrict__ W0,
+                                                                                                  const double* __restrict__ W1,
+                                                                                                  const __grid_constant__ LogsvTangentConsts consts) {
+  constexpr int NP = LogsvTangentPath::NP;
+  exp_table_init();
+  SpotMoments<2 + NP, kThreads> mom;
+  LogsvTangentPath p(consts);
+  const long long stride = (long long)gridDim.x * kThreads;
+  for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < a.n; i += stride) {
+    double xi = 0.0, vi = a.v_init, qi = 0.0;
+    if (!a.init) {
+      xi = a.x[i];
+      vi = a.v[i];
+      qi = a.q[i];
+    }
+    p.load(xi, vi, qi, t, i, a.n, a.init != 0);
+    for (int s = 0; s < a.nsteps; ++s) p.step<true>(__ldg(W0 + (size_t)s * a.n + i), __ldg(W1 + (size_t)s * a.n + i));
+    const double xT = p.x();
+    a.x[i] = xT;
+    a.v[i] = p.sigma();
+    a.q[i] = p.q();
+    const double spot = a.forward * exp(xT);
+#pragma unroll
+    for (int k = 0; k < NP; ++k) {
+      const double d = p.tx(k);
+      t.dx[k * a.n + i] = d;
+      t.dv[k * a.n + i] = p.tv(k);
+      t.dq[k * a.n + i] = p.tq(k);
+      mom.add_term(spot, k, d);
+    }
+    mom.add(spot);
+  }
+  mom.store(a.partials);
+}
+
 // Per-strike sums of the payoff and of its pathwise derivatives.  U = re-centred spot S (LOG_RETURN) or q/ttm (Q_VAR);
 // dS_p = F e^x dx_p - mean(F e^x dx_p) over the nanmean's set, dS/dF = S/F; dU_p = dq_p/ttm, dU/dF = 0 under Q_VAR.
 // pay = h(U) (C/P) or h(U)/S (IC/IP) with h = (U-K)^+ or (K-U)^+; g = h'(U) dU or (h'(U) dU - pay dS)/S.  A path whose payoff is NaN
@@ -1866,6 +1907,19 @@ struct GreeksChainIO : ChainIO {
     }
     return 0;
   }
+
+  // the device-level twin of copy_back: the result block's rows copied on the stream into the caller's device arrays prices_out, stderr_out
+  // [Jtot] and greeks_out, greeks_se_out [1 + NP][Jtot]; no synchronisation
+  int copy_to_device(double* prices_out, double* stderr_out, double* greeks_out, double* greeks_se_out) const {
+    const size_t J = (size_t)Jtot, G = (size_t)(1 + NP) * J;
+    if (J == 0) return 0;
+    const double* o = d_out.as<double>();
+    B200SV_CUDA(cudaMemcpyAsync(prices_out, o, sizeof(double) * J, cudaMemcpyDeviceToDevice, st));
+    B200SV_CUDA(cudaMemcpyAsync(stderr_out, o + J, sizeof(double) * J, cudaMemcpyDeviceToDevice, st));
+    B200SV_CUDA(cudaMemcpyAsync(greeks_out, o + 2 * J, sizeof(double) * G, cudaMemcpyDeviceToDevice, st));
+    B200SV_CUDA(cudaMemcpyAsync(greeks_se_out, o + 2 * J + G, sizeof(double) * G, cudaMemcpyDeviceToDevice, st));
+    return 0;
+  }
 };
 
 // The [3][n] fp64 path state (x, vol, qvar) of a host-level call on the device, or its tangents ([3][NP * n]), and the caller's three arrays
@@ -2121,6 +2175,49 @@ static int mc_chain_greeks_host(const Params& p, int M, const double* ttms, cons
                                     cudaMemcpyDeviceToHost, st));
   }
   return io.copy_back(sync, prices_out, stderr_out, greeks_out, greeks_se_out, gamma_out, gamma_se_out);
+}
+
+// chain driver on fixed unit normals resident on the device (DESIGN.md §4.7), per maturity: logsv_tangent_step_fixed_kernel -> its P tangent
+// means, the two re-centring moments from spot_moments_impl over x -> per-strike sensitivity sums -> the price and std-error rows from the
+// pricing route's own launches (ChainIO::payoff), written over the ones greeks_finalize_kernel left.  So prices and std errors are those of
+// b200sv_dev_logsv_step_fixed(fast) + b200sv_dev_spot_moments + b200sv_dev_payoff_sums + b200sv_dev_payoff_finalize on the same normals bit
+// for bit, whatever the launch shapes; a maturity without strikes is stepped and not priced, as there.  Asynchronous on `st`.
+static int logsv_chain_greeks_fixed(const b200sv_logsv_params& p, int M, const double* ttms, const double* forwards, const double* discfactors,
+                                    const double* etas, const int* offsets, const double* strikes, const int8_t* types,
+                                    const double* const* W0s, const double* const* W1s, const int* nsteps, const double* dts, long long N,
+                                    int is_spot, int variable_type, double* prices_out, double* stderr_out, double* greeks_out,
+                                    double* greeks_se_out, cudaStream_t st) {
+  constexpr int NP = LogsvTangentPath::NP;
+  B200SV_REQUIRE(W0s && W1s && nsteps && dts, "null pointer");
+  B200SV_REQUIRE(N >= 1, "N must be >= 1");
+  if (int rc = validate_chain(M, ttms, offsets, strikes, types, variable_type)) return rc;
+  for (int m = 0; m < M; ++m) {
+    B200SV_REQUIRE(W0s[m] && W1s[m], "null pointer");
+    B200SV_REQUIRE(nsteps[m] >= 1 && dts[m] > 0.0, "nsteps and dts must be positive");
+  }
+  B200SV_REQUIRE(offsets[M] == offsets[0] || (prices_out && stderr_out && greeks_out && greeks_se_out), "null pointer");
+  ensure_pool_threshold();
+  const size_t n = (size_t)N;
+  DevBuf d_state(st);
+  GreeksChainIO<NP> io(M, ttms, forwards, discfactors, offsets, types, variable_type, N, st);
+  B200SV_CUDA(d_state.alloc(sizeof(double) * (3 * n + 3 * (size_t)NP * n)));
+  if (int rc = io.upload(strikes)) return rc;
+  double *x = d_state.as<double>(), *v = x + n, *q = v + n;
+  const TangentState t{q + n, q + n + NP * n, q + n + 2 * NP * n};
+  const Grid g = persistent_grid(logsv_tangent_step_fixed_kernel, kThreads, N);
+  for (int m = 0; m < M; ++m) {
+    const LogsvTangentConsts c = make_logsv_tangent_consts(p, etas ? etas[m] : 1.0, is_spot != 0, dts[m]);
+    if (int rc = slice_moments("logsv_tangent_step_fixed_kernel", 2 + NP, g.blocks, io.moments(), st, nullptr, [&](double* partials) {
+          const SliceArgs<double> a{x, v, q, N, 0ull, m == 0, p.sigma0, nsteps[m], (unsigned int)m, 0ull, forwards[m], partials};
+          logsv_tangent_step_fixed_kernel<<<g.blocks, g.threads, 0, st>>>(a, t, W0s[m], W1s[m], c);
+        }))
+      return rc;
+    if (offsets[m + 1] == offsets[m]) continue;
+    if (int rc = spot_moments_impl(x, N, forwards[m], io.moments(), st, nullptr)) return rc;
+    if (int rc = io.payoff(m, x, q, t.dx, t.dq, (double)N)) return rc;
+    if (int rc = io.ChainIO::payoff(0, m, x, q, false, N, (double)N, false)) return rc;
+  }
+  return io.copy_to_device(prices_out, stderr_out, greeks_out, greeks_se_out);
 }
 
 // one slice from the initial state (0, v_init, 0) with initial tangents, for paths [path_offset, path_offset + n) of Philox slice
@@ -2406,6 +2503,16 @@ int b200sv_dev_heston_step_fixed(double* x, double* var, double* qvar, const dou
   Grid g = persistent_grid(heston_step_fixed_kernel, kThreads, N);
   heston_step_fixed_kernel<<<g.blocks, g.threads, 0, (cudaStream_t)stream>>>(x, var, qvar, W0, W1, S, N, *params, dt);
   return check_launch("heston_step_fixed_kernel");
+}
+
+int b200sv_dev_logsv_mc_chain_greeks_fixed(const b200sv_logsv_params* params, int M, const double* ttms, const double* forwards,
+                                           const double* discfactors, const double* etas, const int* offsets, const double* strikes,
+                                           const int8_t* types, const double* const* W0s, const double* const* W1s, const int* nsteps,
+                                           const double* dts, long long N, int is_spot_measure, int variable_type, double* prices_out,
+                                           double* stderr_out, double* greeks_out, double* greeks_se_out, void* stream) {
+  B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets, "null pointer");
+  return logsv_chain_greeks_fixed(*params, M, ttms, forwards, discfactors, etas, offsets, strikes, types, W0s, W1s, nsteps, dts, N,
+                                  is_spot_measure, variable_type, prices_out, stderr_out, greeks_out, greeks_se_out, (cudaStream_t)stream);
 }
 
 int b200sv_dev_spot_moments(const double* x, long long n, double forward, double* moments_out, void* stream) {

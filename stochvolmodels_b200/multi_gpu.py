@@ -463,3 +463,27 @@ def _fixed_randoms_chain_device(rnd, ttms, forwards, discfactors, strikes_ttms, 
             C.call("b200sv_dev_payoff_finalize", ptr(sums[3 * jo:]), J, float(discfactors[m]), n, ptr(out[0, jo:]), ptr(out[1, jo:]), None, stream)
         host = out.cpu().numpy()
     return C.split_chain(host[0], offsets), C.split_chain(host[1], offsets)
+
+
+def _fixed_randoms_chain_greeks_device(rnd, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, params_c, etas, is_spot_measure,
+                                       variable_type):
+    """_fixed_randoms_chain_device(rnd, ..., fast=True) plus the pathwise sensitivities in one call on the same stream
+    (b200sv_dev_logsv_mc_chain_greeks_fixed): (prices, std errors, greeks [1+6, J], greeks_se [1+6, J], offsets), prices and std errors
+    bit-identical to _fixed_randoms_chain_device's, greeks row 0 the forward delta, then engine.LOGSV_GREEK_PARAMS."""
+    import torch
+    dev = rnd.device
+    ch = engine._chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
+    if len(rnd.W0s) != ch.M:
+        raise ValueError("the DeviceRandoms must hold one block of normals per maturity")
+    etas = C.f64(etas)
+    J, P = ch.strikes.shape[0], len(engine.LOGSV_GREEK_PARAMS)
+    ptrs = lambda ws: (c_void_p * ch.M)(*(w.data_ptr() for w in ws))
+    nsteps = np.array([w.shape[0] for w in rnd.W0s], dtype=np.int32)
+    with torch.cuda.device(dev):
+        out = torch.empty((2 * (2 + P), max(J, 1)), dtype=torch.float64, device=dev)     # [prices | std errors | greeks | greeks_se]
+        ptr = lambda r: c_void_p(out[r].data_ptr())
+        C.call("b200sv_dev_logsv_mc_chain_greeks_fixed", byref(params_c), *C.chain_ptrs(ch, etas), ptrs(rnd.W0s), ptrs(rnd.W1s), C.iptr(nsteps),
+               C.dptr(C.f64(rnd.dts)), rnd.nb_path, int(bool(is_spot_measure)), engine.variable_code(variable_type), ptr(0), ptr(1), ptr(2),
+               ptr(3 + P), c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+        host = out[:, :J].cpu().numpy()
+    return C.split_chain(host[0], ch.offsets), C.split_chain(host[1], ch.offsets), host[2: 3 + P].copy(), host[3 + P:].copy(), ch.offsets

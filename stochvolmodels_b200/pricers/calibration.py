@@ -18,6 +18,11 @@ fixed-random stepper -- the same objective values as the reference for the same 
 ``b200sv_logsv_mc_chain_batch`` call in which the counter-based generator re-draws identical normals for every set (nothing stored or
 streamed; statistically equivalent objective, different sample).
 
+``gradient='exact'`` (ANALYTIC engine) and ``gradient='pathwise'`` (MC and ROUGH_MC engines) replace the difference by one sensitivity call
+per point through ``ExactGradientObjective``: the Fourier implied-vol sensitivities (DESIGN.md §4.6), resp. the pathwise Monte Carlo
+sensitivities on the fit's fixed normals mapped to implied-vol rows (§4.7) -- the exact derivative of the sample objective the difference
+route approximates, with no step size.
+
 Quotes whose model price falls outside the no-arbitrage bounds have no implied vol: the GPU inversion returns NaN for them and the
 objective's ``nansum`` (the reference's own reduction, :292-294) leaves them out of that evaluation, exactly as the reference does with the NaNs
 of its third-party inverter.  Which quotes that inverter would flag is not pinned (the package is absent, DESIGN.md 2); ``BatchedObjective``
@@ -228,14 +233,18 @@ class ScipyDifferenceObjective:
         return self._g.copy()
 
 
-GRADIENTS = ("difference", "exact")
+GRADIENTS = ("difference", "exact", "pathwise")
 
 
-def check_gradient(gradient: str) -> str:
-    """the ``gradient`` argument of the calibration drivers: 'difference' (default: SLSQP's forward difference, priced as one batch) or
-    'exact' (ExactGradientObjective)"""
+def check_gradient(gradient: str, pathwise: bool = False) -> str:
+    """the ``gradient`` argument of the calibration drivers: 'difference' (default: SLSQP's forward difference, priced as one batch),
+    'exact' (ExactGradientObjective on the Fourier sensitivities) or 'pathwise' (ExactGradientObjective on the Monte Carlo sensitivities of
+    the fixed normals; only drivers with a Monte Carlo engine pass ``pathwise=True``, the others reject it before any library call)"""
     if gradient not in GRADIENTS:
-        raise ValueError("gradient must be 'difference' or 'exact'")
+        raise ValueError("gradient must be 'difference', 'exact' or 'pathwise'")
+    if gradient == "pathwise" and not pathwise:
+        raise NotImplementedError("gradient='pathwise' covers LogSVPricer.calibrate_model_params_to_chain with CalibrationEngine.MC or ROUGH_MC "
+                                  "(PARAMS4 / PARAMS5) only")
     return gradient
 
 
@@ -389,14 +398,24 @@ def calibrate_logsv(pricer, option_chain, params0, params_min, params_max, is_ve
                     calibration_engine: CalibrationEngine, nb_path: int, nb_steps: int, seed: int, is_spot_measure: bool = True,
                     disp: bool = False, return_info: bool = False, fd_step: Optional[float] = None, mc_randoms: str = "numpy",
                     gradient: str = "difference"):
-    if check_gradient(gradient) == "exact":
+    if check_gradient(gradient, pathwise=True) == "exact":
         if calibration_engine != CalibrationEngine.ANALYTIC:
-            raise NotImplementedError(f"gradient='exact' covers CalibrationEngine.ANALYTIC only, not {calibration_engine}")
+            raise NotImplementedError(f"gradient='exact' covers CalibrationEngine.ANALYTIC only, not {calibration_engine} "
+                                      "(the Monte Carlo engines have gradient='pathwise')")
         if model_calibration_type not in (LogsvModelCalibrationType.PARAMS4, LogsvModelCalibrationType.PARAMS5):
             raise NotImplementedError(f"gradient='exact' covers PARAMS4 and PARAMS5 only, not {model_calibration_type} (the eta backbone "
                                       "of PARAMS_WITH_VARSWAP_FIT is refitted at every point and is not differentiated)")
+    if gradient == "pathwise":
+        if calibration_engine not in (CalibrationEngine.MC, CalibrationEngine.ROUGH_MC):
+            raise NotImplementedError(f"gradient='pathwise' covers CalibrationEngine.MC and ROUGH_MC only, not {calibration_engine} "
+                                      "(the ANALYTIC engine has gradient='exact')")
+        if model_calibration_type not in (LogsvModelCalibrationType.PARAMS4, LogsvModelCalibrationType.PARAMS5):
+            raise NotImplementedError(f"gradient='pathwise' covers PARAMS4 and PARAMS5 only, not {model_calibration_type} (the eta backbone "
+                                      "of PARAMS_WITH_VARSWAP_FIT is refitted at every point and is not differentiated)")
     from ..multi_gpu import _fixed_randoms_chain_device
-    from .logsv_pricer import DeviceRandoms, _params_c, get_randoms_for_chain_valuation
+    from .fourier_greeks import to_chain_ivol_sensitivities
+    from .logsv_pricer import DeviceRandoms, _params_c, get_randoms_for_chain_valuation, logsv_mc_chain_greeks_fixed_randoms
+    from .mc_greeks import to_mc_chain_greeks
     vol_scaler = pricer.set_vol_scaler(option_chain=option_chain)
     _, market_vols_ttms = option_chain.get_chain_data_as_xy()
     market_vols = to_flat_np_array(market_vols_ttms)
@@ -406,6 +425,12 @@ def calibrate_logsv(pricer, option_chain, params0, params_min, params_max, is_ve
     codec = LogSvParameterCodec(params0, params_min, params_max, model_calibration_type, varswap_strikes)
     p0, bounds = codec.initial_and_bounds()
     ttms = option_chain.ttms
+    resets = np.zeros(len(ttms), dtype=np.int64)       # ROUGH_MC pathwise: per maturity, the most paths any evaluation saw reset
+
+    def mc_ivol_rows(res):
+        """engine.*_mc_chain_greeks output -> (vols [J], d vols / d LOGSV_GREEK_PARAMS [6, J])"""
+        sens = to_chain_ivol_sensitivities(option_chain, to_mc_chain_greeks(res, engine.LOGSV_GREEK_PARAMS))
+        return flat_ivol_rows(sens, engine.LOGSV_GREEK_PARAMS)
 
     if gradient == "exact":
         # one compute_chain_ivol_greeks call per point, on the grid the difference route pins too (set_vol_scaler above)
@@ -433,6 +458,15 @@ def calibrate_logsv(pricer, option_chain, params0, params_min, params_max, is_ve
                                                       option_chain.strikes_ttms, option_chain.optiontypes_ttms, nb_path, nb_steps,
                                                       is_spot_measure, seed, flags)
             return ivols
+
+        def ivol_greeks(x: np.ndarray):
+            # the vols are the batch pricer's, so that the objective is the difference route's bit for bit; the sensitivity pass prices
+            # the same paths with another reduction order (~1e-13 apart) and supplies only the derivatives
+            s = codec.parse(x)
+            res = engine.logsv_mc_chain_greeks(_params_c(s), ttms, option_chain.forwards, option_chain.discfactors,
+                                               s.get_vol_backbone_etas(ttms=ttms), option_chain.strikes_ttms, option_chain.optiontypes_ttms,
+                                               nb_path, nb_steps, is_spot_measure, 1, seed, flags)
+            return batch_vols(x[None, :])[0], mc_ivol_rows(res)[1]
     elif calibration_engine == CalibrationEngine.MC:
         if mc_randoms != "numpy":
             raise ValueError("mc_randoms must be 'numpy' or 'philox'")
@@ -448,6 +482,14 @@ def calibrate_logsv(pricer, option_chain, params0, params_min, params_max, is_ve
                                                         is_spot_measure, 1, True)
                 rows.append(to_flat_np_array(option_chain.compute_model_ivols_from_chain_data(model_prices=prices)))
             return np.vstack(rows)
+
+        def ivol_greeks(x: np.ndarray):
+            s = codec.parse(x)
+            res = logsv_mc_chain_greeks_fixed_randoms(ttms, option_chain.forwards, option_chain.discfactors, option_chain.strikes_ttms,
+                                                      option_chain.optiontypes_ttms, rnd, v0=s.sigma0, theta=s.theta, kappa1=s.kappa1,
+                                                      kappa2=s.kappa2, beta=s.beta, volvol=s.volvol,
+                                                      vol_backbone_etas=s.get_vol_backbone_etas(ttms=ttms), is_spot_measure=is_spot_measure)
+            return flat_ivol_rows(to_chain_ivol_sensitivities(option_chain, res), engine.LOGSV_GREEK_PARAMS)
     elif calibration_engine == CalibrationEngine.ROUGH_MC:
         # reference :528-533 + :266-289: fixed normals of get_randoms_for_rough_vol_chain_valuation; here the n + 1 finite-difference
         # parameter sets of an optimizer step share ONE upload of them (or none: mc_randoms="philox" draws in-kernel on a fixed seed)
@@ -469,16 +511,30 @@ def calibrate_logsv(pricer, option_chain, params0, params_min, params_max, is_ve
                                                             option_chain.discfactors, option_chain.strikes_ttms, option_chain.optiontypes_ttms,
                                                             nb_path, nsteps, hs, Z0, Z1, 1, seed, flags, with_ivols=True)
             return ivols
+
+        def ivol_greeks(x: np.ndarray):
+            res = engine.rough_logsv_mc_chain_greeks(_params_c(codec.parse(x)), params0.weights, params0.nodes, ttms, option_chain.forwards,
+                                                     option_chain.discfactors, option_chain.strikes_ttms, option_chain.optiontypes_ttms,
+                                                     nb_path, nsteps, hs, Z0, Z1, 1, seed, flags)
+            np.maximum(resets, res[7], out=resets)
+            return mc_ivol_rows(res[:5])
     else:
         raise NotImplementedError(f"{calibration_engine}")
 
     if gradient == "difference":
         objective = BatchedObjective(batch_vols=batch_vols, market_vols=market_vols, weights=weights, bounds=bounds, eps=fd_step or SLSQP_EPS)
+    elif gradient == "pathwise":
+        objective = ExactGradientObjective(ivol_greeks=ivol_greeks, field_jacobian=codec.field_jacobian, market_vols=market_vols,
+                                           weights=weights)
+        if calibration_engine == CalibrationEngine.MC and mc_randoms == "philox":
+            objective.CALLS_PER_EVALUATION = 3       # the batch pricer's vols as well (ivol_greeks above)
     x, result = run_slsqp(objective, p0, bounds, build_logsv_constraints(codec, constraints_type), disp=disp)
     fit = codec.parse(x)
     if return_info:
-        return fit, {"fun": float(result.fun), "nit": int(result.nit), "nb_batches": objective.nb_batches, "x": x,
-                     "nan_quotes": objective.nan_quotes}
+        info = {"fun": float(result.fun), "nit": int(result.nit), "nb_batches": objective.nb_batches, "x": x, "nan_quotes": objective.nan_quotes}
+        if gradient == "pathwise" and calibration_engine == CalibrationEngine.ROUGH_MC:
+            info["reset_paths"] = resets
+        return fit, info
     return fit
 
 

@@ -9,7 +9,7 @@ transform grid is held fixed.  No step size to choose.
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import Dict, List, Sequence
+from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 
@@ -40,10 +40,10 @@ class ChainIvolGreeks:
     """implied-vol sensitivities of a chain (DESIGN.md §4.6), one array per maturity: ``ivols`` (bit-identical to
     ``compute_chain_prices_with_vols`` with the same arguments), ``delta`` / ``gamma`` (d ivol / d forward, d^2 ivol / d forward^2, sticky
     strike) and ``params``: parameter name -> d ivol / d parameter.  NaN where the ivol is NaN, 0 where it is an end of the inversion
-    bracket (1e-8 or 10)."""
+    bracket (1e-8 or 10).  ``gamma`` is None for Monte Carlo sensitivities without a gamma row."""
     ivols: List[np.ndarray]
     delta: List[np.ndarray]
-    gamma: List[np.ndarray]
+    gamma: Optional[List[np.ndarray]]
     params: Dict[str, List[np.ndarray]]
 
 
@@ -61,10 +61,14 @@ def _flat(rows_ttms) -> np.ndarray:
 
 def to_chain_ivol_sensitivities(option_chain, greeks: FourierChainGreeks):
     """``FourierChainGreeks`` -> ``ChainIvolGreeks``, ``FourierChainHessian`` -> ``ChainIvolHessian``: the price rows mapped to implied-vol
-    rows on the chain's forwards and discount factors by one engine.bsm_implied_vol_sensitivities call"""
+    rows on the chain's forwards and discount factors by one engine.bsm_implied_vol_sensitivities call.  A Monte Carlo ``McChainGreeks``
+    maps the same way (its standard errors are not carried over); without a gamma row (``gamma`` None) the transform gets zeros in its place
+    and the result has ``gamma=None``, the other rows being independent of it."""
     from .. import engine
     names = list(greeks.params)
-    rows = np.vstack([_flat(greeks.delta), _flat(greeks.gamma), *(_flat(greeks.params[n]) for n in names)])
+    delta = _flat(greeks.delta)
+    gamma = np.zeros_like(delta) if greeks.gamma is None else _flat(greeks.gamma)
+    rows = np.vstack([delta, gamma, *(_flat(greeks.params[n]) for n in names)])
     second = isinstance(greeks, FourierChainHessian)
     vanna = np.vstack([_flat(greeks.vanna[n]) for n in names]) if second else None
     hessian = np.vstack([_flat(greeks.hessian[p][q]) for i, p in enumerate(names) for q in names[i:]]) if second else None
@@ -74,7 +78,8 @@ def to_chain_ivol_sensitivities(option_chain, greeks: FourierChainGreeks):
     offsets = np.zeros(len(ivols) + 1, dtype=np.int64)
     offsets[1:] = np.cumsum([a.size for a in ivols])
     split = lambda row: C.split_chain(row, offsets)
-    first = ChainIvolGreeks(ivols=ivols, delta=split(g[0]), gamma=split(g[1]), params={n: split(g[2 + k]) for k, n in enumerate(names)})
+    first = ChainIvolGreeks(ivols=ivols, delta=split(g[0]), gamma=None if greeks.gamma is None else split(g[1]),
+                            params={n: split(g[2 + k]) for k, n in enumerate(names)})
     if not second:
         return first
     hess: Dict[str, Dict[str, List[np.ndarray]]] = {n: {} for n in names}

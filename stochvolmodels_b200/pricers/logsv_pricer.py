@@ -27,6 +27,7 @@ from .. import _capi as C
 from .. import engine
 from ..data.option_chain import OptionChain
 from ..multi_gpu import CudaMcEngine, _fixed_randoms_chain_device, _shared_seed, _use_distributed, mc_chain_distributed, shard_paths
+from ..multi_gpu import _fixed_randoms_chain_greeks_device
 from ..multi_gpu import SHARD_MIN_PATHS  # noqa: F401  (the MC routing policy lives in multi_gpu; this name stays importable from here)
 from ..utils.config import VariableType
 from ..utils.funcs import set_time_grid, timer
@@ -215,7 +216,12 @@ class LogSVPricer(ModelPricer):
         ``constraints_type`` (reference :441-558; same arguments, bounds and return type).  The objective and its finite-difference
         gradient are ONE batched GPU call per optimizer evaluation (pricers/calibration.py).  ``return_info=True`` also returns
         {fun, nit, nb_batches, x}.  ``gradient='exact'`` (ANALYTIC engine, PARAMS4 / PARAMS5) hands SLSQP the exact gradient of the
-        objective from one ``compute_chain_ivol_greeks`` call per point instead of the forward difference (DESIGN.md §4.6)."""
+        objective from one ``compute_chain_ivol_greeks`` call per point instead of the forward difference (DESIGN.md §4.6).
+        ``gradient='pathwise'`` (MC engine with either ``mc_randoms``, ROUGH_MC; PARAMS4 / PARAMS5) hands SLSQP the pathwise derivative of the
+        sample objective on the fit's fixed normals from one Monte Carlo sensitivity pass per point (DESIGN.md §4.7); it is the derivative
+        of the sample objective, not of the model.  A ROUGH_MC pathwise fit's ``return_info`` adds ``reset_paths``: per maturity, the most
+        paths any evaluation saw take the reset-to-1e-6 branch; where it is non-zero the gradient misses the mass those paths move across
+        that switch."""
         params_min = params_min or LogSvParams(sigma0=0.1, theta=0.1, kappa1=0.25, kappa2=0.25, beta=-3.0, volvol=0.2)
         params_max = params_max or LogSvParams(sigma0=1.5, theta=1.5, kappa1=10.0, kappa2=10.0, beta=3.0, volvol=3.0)
         return calibrate_logsv(self, option_chain, params0, params_min, params_max, is_vega_weighted, is_unit_ttm_vega,
@@ -628,6 +634,28 @@ def logsv_mc_chain_pricer_fixed_randoms(ttms, forwards, discfactors, strikes_ttm
         if return_states:
             states.append((x.copy(), s.copy(), q.copy()))
     return (prices, stds, states) if return_states else (prices, stds)
+
+
+def logsv_mc_chain_greeks_fixed_randoms(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, W0s, W1s=None, dts=None,
+                                        v0: float = None, theta: float = None, kappa1: float = None, kappa2: float = None,
+                                        beta: float = None, volvol: float = None, vol_backbone_etas: np.ndarray = None,
+                                        is_spot_measure: bool = True, variable_type: VariableType = VariableType.LOG_RETURN):
+    """``logsv_mc_chain_pricer_fixed_randoms`` plus pathwise sensitivities in the same pass (DESIGN.md §4.7) -> ``McChainGreeks``: the forward
+    delta and d price / d (sigma0, theta, kappa1, kappa2, beta, volvol) with standard errors.  ``kappa2`` is held fixed when kappa1 or
+    theta moves; the vol backbone and the discount factors are not differentiated.  On fixed normals the sensitivities are the exact
+    derivatives of the sample prices, the limit a common-random-number difference approximates.
+
+    ``W0s`` may be a :class:`DeviceRandoms`, used in place; host arrays ``W0s``, ``W1s``, ``dts`` are uploaded once into one.  Prices and std
+    errors are bit-identical to ``logsv_mc_chain_pricer_fixed_randoms(DeviceRandoms, fast=True)`` on the same normals; they agree with the
+    strict host-array stepper only to ~1e-14."""
+    from .mc_greeks import to_mc_chain_greeks
+    params_c = engine.logsv_params_c(v0, theta, kappa1, kappa2, beta, volvol)
+    if vol_backbone_etas is None:
+        vol_backbone_etas = np.ones(len(ttms))
+    rnd = W0s if isinstance(W0s, DeviceRandoms) else DeviceRandoms(W0s, W1s, dts)
+    res = _fixed_randoms_chain_greeks_device(rnd, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, params_c, vol_backbone_etas,
+                                             is_spot_measure, variable_type)
+    return to_mc_chain_greeks(res, engine.LOGSV_GREEK_PARAMS)
 
 
 def v0_implied(atm: float, beta: float, volvol: float, theta: float, kappa1: float, ttm: float) -> float:
