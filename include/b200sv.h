@@ -456,6 +456,27 @@ int b200sv_heston_price_chain_hessian(const b200sv_heston_params* params, int M,
                                       int variable_type, double vol_scaler, int P, double* prices_out, double* greeks_out,
                                       double* dlog_mgf_out, double* vanna_out, double* hessian_out, double* d2log_mgf_out);
 
+/* theta of the Fourier chain pricers (DESIGN.md §4.8), LOG_RETURN only (else -4).  The arguments and outputs of the _greeks twin
+ * (bit-identical to it), then theta_out [J]: -d price / d ttms[m] per year, with the slice forward and discount factor, the earlier
+ * maturities, etas and the transform grid held (vol_scaler <= 0 resolved on the unmoved chain); the adaptive routes hold the accepted mesh
+ * of slice m and move its last step only.  Optional (may be NULL): dlog_mgf_theta_out [M][P] complex128 interleaved, d log_mgf / d ttms[m]
+ * of slice m; theta_nfev_out [P] (LogSV, Hawkes), the right-hand-side evaluations of the theta kernel's own primal solve per grid point,
+ * equal to nfev_out when it ran the pricing mesh. */
+int b200sv_logsv_price_chain_greeks_theta(const b200sv_logsv_params* params, int M, const double* ttms, const double* forwards,
+                                          const double* discfactors, const double* etas, const int* offsets, const double* strikes,
+                                          const int8_t* types, int is_spot_measure, int variable_type, int expansion_order,
+                                          double vol_scaler, int P, double* prices_out, double* greeks_out, double* dlog_mgf_out,
+                                          int* nfev_out, double* theta_out, double* dlog_mgf_theta_out, int* theta_nfev_out);
+int b200sv_heston_price_chain_greeks_theta(const b200sv_heston_params* params, int M, const double* ttms, const double* forwards,
+                                           const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
+                                           int variable_type, double vol_scaler, int P, double* prices_out, double* greeks_out,
+                                           double* dlog_mgf_out, double* theta_out, double* dlog_mgf_theta_out);
+int b200sv_hawkesjd_price_chain_greeks_theta(const b200sv_hawkes_params* params, int M, const double* ttms, const double* forwards,
+                                             const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
+                                             int is_spot_measure, double vol_scaler, int P, double* prices_out, double* greeks_out,
+                                             double* dlog_mgf_out, int* nfev_out, double* theta_out, double* dlog_mgf_theta_out,
+                                             int* theta_nfev_out);
+
 /* B parameter sets on ONE chain in one pass -- the objective of the calibration drivers and its finite-difference gradient:
  * _LogSvCalibrationObjective.__call__ (pricers/logsv_pricer.py:234-294: compute_model_ivols_for_chain = logsv_chain_pricer +
  * option_chain.compute_model_ivols_from_chain_data), which scipy SLSQP evaluates n+1 times per iteration, one parameter set at a time.
@@ -554,6 +575,13 @@ int b200sv_bsm_implied_vol_sensitivities(int M, const double* ttms, const double
                                          const double* strikes, const int8_t* types, const double* prices, int NP, const double* greeks,
                                          const double* vanna, const double* hessian, double* ivols_out, double* ivol_greeks_out,
                                          double* ivol_vanna_out, double* ivol_hessian_out);
+/* implied-vol theta (DESIGN.md §4.8).  The chain and prices[] as b200sv_bsm_implied_vols, theta [J] = -d price / d ttms[m] as the
+ * b200sv_*_price_chain_greeks_theta entry points return it.  Outputs: ivols_out [J], bit-identical to b200sv_bsm_implied_vols, and
+ * ivol_theta_out [J] = -d ivol / d ttms[m] = (theta + d B / d ttm) / vega, B the discounted Black-76 price at the same discount factor.  NaN
+ * where the ivol is NaN, 0 where it is an end of the inversion bracket (1e-8 or 10).  Unknown type codes: -3. */
+int b200sv_bsm_implied_vol_theta(int M, const double* ttms, const double* forwards, const double* discfactors, const int* offsets,
+                                 const double* strikes, const int8_t* types, const double* prices, const double* theta, double* ivols_out,
+                                 double* ivol_theta_out);
 
 #ifdef __cplusplus
 }

@@ -128,6 +128,11 @@ SIGNATURES = {
     "b200sv_logsv_price_chain_greeks": [_lp, c_int, _dp, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_int, c_int, c_double, c_int, _dp, _dp, _dp, _ip],
     "b200sv_heston_price_chain_greeks": [_hp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_double, c_int, _dp, _dp, _dp],
     "b200sv_hawkesjd_price_chain_greeks": [_kp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_double, c_int, _dp, _dp, _dp, _ip],
+    "b200sv_logsv_price_chain_greeks_theta": [_lp, c_int, _dp, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_int, c_int, c_double, c_int, _dp, _dp, _dp,
+                                              _ip, _dp, _dp, _ip],
+    "b200sv_heston_price_chain_greeks_theta": [_hp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_double, c_int, _dp, _dp, _dp, _dp, _dp],
+    "b200sv_hawkesjd_price_chain_greeks_theta": [_kp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_double, c_int, _dp, _dp, _dp, _ip, _dp, _dp,
+                                                 _ip],
     "b200sv_logsv_price_chain_hessian": [_lp, c_int, _dp, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_int, c_int, c_double, c_int, _dp, _dp, _dp, _ip,
                                          _dp, _dp, _dp],
     "b200sv_heston_price_chain_hessian": [_hp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_double, c_int, _dp, _dp, _dp, _dp, _dp, _dp],
@@ -142,6 +147,7 @@ SIGNATURES = {
     "b200sv_bsm_implied_vols": [c_int, _dp, _dp, _dp, _ip, _dp, _i8p, _dp, _dp],
     "b200sv_debug_bsm_implied_vols": [c_int, _dp, _dp, _dp, _ip, _dp, _i8p, _dp, _dp, _ip],
     "b200sv_bsm_implied_vol_sensitivities": [c_int, _dp, _dp, _dp, _ip, _dp, _i8p, _dp, c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp],
+    "b200sv_bsm_implied_vol_theta": [c_int, _dp, _dp, _dp, _ip, _dp, _i8p, _dp, _dp, _dp, _dp],
     "b200sv_logsv_mgf_grid": [_dp, _dp, c_int, c_double, _dp, _lp, c_double, c_int, c_int, _dp],
     "b200sv_logsv_mgf_grid_analytic": [_dp, _dp, c_int, c_double, _dp, _lp, c_int, c_int, c_int, _dp],
     "b200sv_logsv_mgf_grid_bdf": [_dp, _dp, c_int, c_double, _dp, _lp, c_double, c_int, c_int, _dp],

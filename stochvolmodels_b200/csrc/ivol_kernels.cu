@@ -96,6 +96,24 @@ __global__ void __launch_bounds__(64) black_ivol_sensitivities_kernel(const Quot
   }
 }
 
+// Implied-vol theta (DESIGN.md §4.8): B(sigma, T) = P(T) at fixed F and D gives -d sigma / dT = (theta + B_T) / B_sigma with theta = -P_T
+// and B_T = B_sigma sigma / (2 T) (Black-76 depends on T through sigma sqrt T only).  One thread per quote, the same inversion as
+// black_ivol_kernel (bit-identical ivols) and the same NaN / bracket-end rules as the sensitivity rows.
+__global__ void __launch_bounds__(64) black_ivol_theta_kernel(const QuoteSpec* __restrict__ q, int n, const double* __restrict__ theta,
+                                                              double* __restrict__ ivols, double* __restrict__ ivol_theta) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const QuoteSpec s = q[i];
+  const double vol = black_implied_vol(s.forward, s.strike, s.ttm, s.discfactor, s.price, s.type);
+  ivols[i] = vol;
+  if (vol != vol || black_vol_at_bracket_end(vol)) {
+    ivol_theta[i] = vol != vol ? vol : 0.0;
+    return;
+  }
+  const double vega = black_partials(s.forward, s.strike, s.ttm, s.discfactor, vol, s.type).vega;
+  ivol_theta[i] = (theta[i] + vega * vol / (2.0 * s.ttm)) / vega;
+}
+
 constexpr int IVOL_SENS_MAX_NP = 15;     // the Hawkes parameter count, the largest of the Fourier chain pricers
 
 template <int NP>
@@ -115,18 +133,26 @@ static int launch_ivol_sensitivities(int np, bool second, int n, const QuoteSpec
 
 using namespace b200sv;
 
+// one QuoteSpec per quote of the chain, flat in chain order; -3 on an unknown type code
+static int quote_specs(int M, const double* ttms, const double* forwards, const double* discfactors, const int* offsets, const double* strikes,
+                       const int8_t* types, const double* prices, std::vector<QuoteSpec>& q) {
+  q.resize(offsets[M] - offsets[0]);
+  for (int m = 0; m < M; ++m)
+    for (int j = offsets[m]; j < offsets[m + 1]; ++j) {
+      if (types[j] < 0 || types[j] > 3) return fail(-3, "unknown option payoff code");
+      q[j - offsets[0]] = QuoteSpec{forwards[m], strikes[j], ttms[m], discfactors[m], prices[j - offsets[0]], (int)types[j]};
+    }
+  return 0;
+}
+
 static int bsm_implied_vols(int M, const double* ttms, const double* forwards, const double* discfactors, const int* offsets,
                             const double* strikes, const int8_t* types, const double* prices, double* ivols_out, int* iterations_out) {
   B200SV_REQUIRE(ttms && forwards && discfactors && offsets && strikes && types && prices && ivols_out, "null pointer");
   B200SV_REQUIRE(M >= 1, "M >= 1");
   const int n = offsets[M] - offsets[0];
   if (n <= 0) return 0;
-  std::vector<QuoteSpec> q(n);
-  for (int m = 0; m < M; ++m)
-    for (int j = offsets[m]; j < offsets[m + 1]; ++j) {
-      if (types[j] < 0 || types[j] > 3) return fail(-3, "unknown option payoff code");
-      q[j - offsets[0]] = QuoteSpec{forwards[m], strikes[j], ttms[m], discfactors[m], prices[j - offsets[0]], (int)types[j]};
-    }
+  std::vector<QuoteSpec> q;
+  if (int rc = quote_specs(M, ttms, forwards, discfactors, offsets, strikes, types, prices, q)) return rc;
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
   StreamSync sync(st);
@@ -173,12 +199,8 @@ extern "C" int b200sv_bsm_implied_vol_sensitivities(int M, const double* ttms, c
   const bool second = vanna != nullptr;
   const int n = offsets[M] - offsets[0];
   if (n <= 0) return 0;
-  std::vector<QuoteSpec> q(n);
-  for (int m = 0; m < M; ++m)
-    for (int j = offsets[m]; j < offsets[m + 1]; ++j) {
-      if (types[j] < 0 || types[j] > 3) return fail(-3, "unknown option payoff code");
-      q[j - offsets[0]] = QuoteSpec{forwards[m], strikes[j], ttms[m], discfactors[m], prices[j - offsets[0]], (int)types[j]};
-    }
+  std::vector<QuoteSpec> q;
+  if (int rc = quote_specs(M, ttms, forwards, discfactors, offsets, strikes, types, prices, q)) return rc;
   const size_t nh = (size_t)NP * (NP + 1) / 2, n1 = 2 + NP, nrows = n1 + (second ? NP + nh : 0);
   std::vector<double> rows(nrows * n);                      // the input rows packed as the kernel reads them: one upload
   std::memcpy(rows.data(), greeks, sizeof(double) * n1 * n);
@@ -205,4 +227,29 @@ extern "C" int b200sv_bsm_implied_vol_sensitivities(int M, const double* ttms, c
     std::memcpy(ivol_hessian_out, o + (1 + n1 + NP) * n, sizeof(double) * nh * n);
   }
   return 0;
+}
+
+extern "C" int b200sv_bsm_implied_vol_theta(int M, const double* ttms, const double* forwards, const double* discfactors, const int* offsets,
+                                            const double* strikes, const int8_t* types, const double* prices, const double* theta,
+                                            double* ivols_out, double* ivol_theta_out) {
+  B200SV_REQUIRE(ttms && forwards && discfactors && offsets && strikes && types && prices && theta && ivols_out && ivol_theta_out,
+                 "null pointer");
+  B200SV_REQUIRE(M >= 1, "M >= 1");
+  const int n = offsets[M] - offsets[0];
+  if (n <= 0) return 0;
+  std::vector<QuoteSpec> q;
+  if (int rc = quote_specs(M, ttms, forwards, discfactors, offsets, strikes, types, prices, q)) return rc;
+  cudaStream_t st = current_stream();
+  ensure_pool_threshold();
+  StreamSync sync(st);
+  DevBuf dq(st), dth(st), dv(st), dt(st);
+  B200SV_CUDA(dq.upload(q.data(), n));
+  B200SV_CUDA(dth.upload(theta, n));
+  B200SV_CUDA(dv.alloc(sizeof(double) * n));
+  B200SV_CUDA(dt.alloc(sizeof(double) * n));
+  black_ivol_theta_kernel<<<(n + 63) / 64, 64, 0, st>>>(dq.as<QuoteSpec>(), n, dth.as<double>(), dv.as<double>(), dt.as<double>());
+  if (int rc = check_launch("black_ivol_theta_kernel")) return rc;
+  B200SV_CUDA(dv.download(ivols_out, n));
+  B200SV_CUDA(dt.download(ivol_theta_out, n));
+  return sync.done();
 }

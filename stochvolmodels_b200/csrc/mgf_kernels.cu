@@ -657,7 +657,9 @@ struct HestonClosedForm {
     psi_m = b1 + zeta;
     two_zeta = 2.0 * zeta;
   }
-  __device__ __forceinline__ void step(double tau, T& a, T& b) const {
+  // Tau: double, or dcd for the theta kernel, which seeds d tau = 1
+  template <class Tau>
+  __device__ __forceinline__ void step(Tau tau, T& a, T& b) const {
     const T ez = exp_(-(tau * zeta));
     const T c_p = (psi_p + vv2 * b) / two_zeta, c_m = (psi_m - vv2 * b) / two_zeta;
     const T den = c_p * ez + c_m;
@@ -1849,6 +1851,165 @@ __global__ void __launch_bounds__(kHawkesHessianTPB) hawkes_mgf_hessian_kernel(c
 }
 
 // --------------------------------------------------------------------------------------------------------------------
+// Theta of the Fourier chain pricers (DESIGN.md §4.8): d log_mgf / d T_m with the accepted mesh t_0 < ... < t_{K-1} of slice m held and
+// only its last step h_K = T_m - t_{K-1} moving (dh_K / dT_m = 1); earlier maturities, the backbone and the grid are held.
+// --------------------------------------------------------------------------------------------------------------------
+// The derivative of one Dormand-Prince step in its length h at a fixed start y:  G_s = k_s + h dk_s,  dY_s = sum_{j<s} a_sj G_j,
+// dk_s = J(Y_s) dY_s (dk_0 = 0),  dy = sum_j b_j G_j.  It is formed on every attempt of rk45_generic and an accepted attempt commits it, so
+// after the solve dy is the last accepted step's.  Jvp: ``void operator()(const cd (&Y)[N], const cd (&dY)[N], cd (&out)[N]) const`` =
+// J(Y) dY (LogsvJvpFn, or HawkesTanRhsFn with zero constant derivatives).  G in shared memory: stage s holds dk_s until stage s + 1 turns
+// it into G_s; stage 6 parks the candidate dy until the acceptance.
+template <int N, int TPB, typename Jvp>
+struct ThetaHook {
+  Jvp f;
+  StageStore<N, TPB> K, G;     // K: rk45_generic's own stage store (read only)
+  cd dy[N];
+
+  __device__ __forceinline__ void finish_stage(int s, double h) {      // dk_s -> G_s = k_s + h dk_s
+#pragma unroll
+    for (int k = 0; k < N; ++k) G.at(s, k) = K.at(s, k) + h * G.at(s, k);
+  }
+  __device__ __forceinline__ void start(const cd (&)[N]) {}
+  __device__ __forceinline__ void stage(int s, const cd (&yt)[N], double h) {
+    if (s == 1) {
+#pragma unroll
+      for (int k = 0; k < N; ++k) G.at(0, k) = K.at(0, k);           // G_0 = k_0
+    } else {
+      finish_stage(s - 1, h);
+    }
+    cd dyt[N], o[N];
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+      cd acc = G.at(0, k) * c_A[s][0];
+#pragma unroll
+      for (int jj = 1; jj < 5; ++jj) acc = acc + G.at(jj, k) * c_A[s][jj];
+      dyt[k] = acc;
+    }
+    f(yt, dyt, o);
+#pragma unroll
+    for (int k = 0; k < N; ++k) G.at(s, k) = o[k];
+  }
+  __device__ __forceinline__ void last(const cd (&)[N], double h) {
+    constexpr double B[6] = {35.0 / 384, 0, 500.0 / 1113, 125.0 / 192, -2187.0 / 6784, 11.0 / 84};
+    finish_stage(5, h);
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+      cd acc = G.at(0, k) * B[0];
+#pragma unroll
+      for (int jj = 2; jj < 6; ++jj) acc = acc + G.at(jj, k) * B[jj];
+      G.at(6, k) = acc;
+    }
+  }
+  __device__ __forceinline__ void accept() {
+#pragma unroll
+    for (int k = 0; k < N; ++k) dy[k] = G.at(6, k);
+  }
+};
+
+// J(A) dA of the LogSV coefficient ODEs: the Jacobian half of rhs_tangent
+template <int N, int TPB>
+struct LogsvJvpFn {
+  const LogsvModel* m;
+  const CoefView<TPB>* c;
+  __device__ __forceinline__ void operator()(const cd (&Y)[N], const cd (&dY)[N], cd (&out)[N]) const {
+    cd dq[8];
+    sym_products<N>(Y, dY, dq);
+    rhs_rows<N, TPB, false>(dq, dY, m->v2, m->qv, m->qv2, *c, out);
+  }
+};
+
+constexpr int kThetaTPB = 8;        // one thread per grid point: 1000 points spread over 125 SMs
+
+// One thread = one grid point: the primal integration of logsv_mgf_kernel (same rk45_generic, same mesh: nfev [P] shows it) plus the theta
+// tangent, reset at every slice.  Output dlog_mgf_theta [M][P] = sum_k dA_k y^k.
+template <int N>
+__global__ void __launch_bounds__(kThetaTPB) logsv_mgf_theta_kernel(const cd* __restrict__ phi, int P, int M, const ChainSpec* __restrict__ spec,
+                                                                     double y, cd* __restrict__ dlog_mgf_theta, int* __restrict__ nfev) {
+  constexpr int TPB = kThetaTPB;
+  __shared__ cd stage_smem[6 * N * TPB];
+  __shared__ cd g_smem[7 * N * TPB];
+  __shared__ cd coef_smem[14 * TPB];
+  const int p = blockIdx.x * TPB + threadIdx.x;
+  if (p >= P) return;
+#pragma unroll
+  for (int i = 0; i < 6 * N; ++i) stage_smem[threadIdx.x + i * TPB] = mk(0.0);
+#pragma unroll
+  for (int i = 0; i < 7 * N; ++i) g_smem[threadIdx.x + i * TPB] = mk(0.0);
+  StageStore<N, TPB> K{stage_smem + threadIdx.x};
+  const CoefView<TPB> c{coef_smem + threadIdx.x};
+  ThetaHook<N, TPB, LogsvJvpFn<N, TPB>> tan{LogsvJvpFn<N, TPB>{nullptr, &c}, K, StageStore<N, TPB>{g_smem + threadIdx.x}, {}};
+  cd A[N];
+#pragma unroll
+  for (int k = 0; k < N; ++k) A[k] = mk(0.0);
+  const cd ph = phi[p], ps = mk(0.0);
+  const double y2 = y * y;
+  const double ys[5] = {1.0, y, y2, y2 * y, y2 * y2};
+  int nf = 0;
+  for (int mm = 0; mm < M; ++mm) {
+    const LogsvModel model = spec[mm].model;
+    store_coef<TPB>(coef_smem + threadIdx.x, make_coef(model, ph, ps));
+    tan.f.m = &model;
+#pragma unroll
+    for (int k = 0; k < N; ++k) tan.dy[k] = mk(0.0);
+    int nfe = 0;
+    rk45_generic<N, TPB>(A, spec[mm].dtau, LogsvRhsFn<N, TPB>{model, c}, K, &nfe, &tan);
+    nf += nfe;
+    cd dlm = mk(0.0);
+#pragma unroll
+    for (int k = 0; k < N; ++k) dlm = dlm + tan.dy[k] * ys[k];
+    dlog_mgf_theta[(size_t)mm * P + p] = dlm;
+  }
+  if (nfev) nfev[p] = nf;
+}
+
+// The Hawkes twin: the primal of hawkes_mgf_kernel plus the theta tangent; dlog_mgf_theta [M][P] = da0 + da_p lambda_p + da_m lambda_m.
+__global__ void __launch_bounds__(kThetaTPB) hawkes_mgf_theta_kernel(const cd* __restrict__ phi, int P, int M, const double* __restrict__ dtaus,
+                                                                    HawkesMgfConsts c, cd* __restrict__ dlog_mgf_theta, int* __restrict__ nfev) {
+  constexpr int TPB = kThetaTPB;
+  __shared__ cd stage_smem[6 * 3 * TPB];
+  __shared__ cd g_smem[7 * 3 * TPB];
+  const int p = blockIdx.x * TPB + threadIdx.x;
+  if (p >= P) return;
+#pragma unroll
+  for (int i = 0; i < 18; ++i) stage_smem[threadIdx.x + i * TPB] = mk(0.0);
+#pragma unroll
+  for (int i = 0; i < 21; ++i) g_smem[threadIdx.x + i * TPB] = mk(0.0);
+  StageStore<3, TPB> K{stage_smem + threadIdx.x};
+  const cd ph = phi[p];
+  const cd h0 = 0.5 * ((ph + mk(1.0)) * ph);
+  const HawkesRhsFn f{c, ph, c.sigma2 * h0};
+  const HawkesMgfConsts zero{0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};      // no explicit d/dT of the right-hand side
+  ThetaHook<3, TPB, HawkesTanRhsFn> tan{HawkesTanRhsFn{c, zero, ph, h0}, K, StageStore<3, TPB>{g_smem + threadIdx.x}, {}};
+  cd A[3] = {mk(0.0), mk(0.0), mk(0.0)};
+  int nf = 0;
+  for (int m = 0; m < M; ++m) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) tan.dy[k] = mk(0.0);
+    int nfe = 0;
+    rk45_generic<3, TPB>(A, dtaus[m], f, K, &nfe, &tan);
+    nf += nfe;
+    dlog_mgf_theta[(size_t)m * P + p] = (tan.dy[0] + tan.dy[1] * c.lambda_p) + tan.dy[2] * c.lambda_m;
+  }
+  if (nfev) nfev[p] = nf;
+}
+
+// The Heston closed form on dual numbers in tau: (a, b) carried over the earlier slices with their derivatives zeroed at every slice
+// start, then the slice's step with d tau = 1.  dlog_mgf_theta [M][P] = da + db v0.
+__global__ void heston_mgf_theta_kernel(const cd* __restrict__ phi, int P, int M, const double* __restrict__ dtaus, b200sv_heston_params hp,
+                                        cd* __restrict__ dlog_mgf_theta) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= P) return;
+  const HestonClosedForm<dcd, dcd> cf(dmk(mk(hp.theta)), dmk(mk(hp.kappa)), dmk(mk(hp.rho)), dmk(mk(hp.volvol)), phi[p], mk(0.0));
+  dcd a = dmk(mk(0.0)), b = dmk(mk(0.0));
+  for (int mm = 0; mm < M; ++mm) {
+    a.d = mk(0.0);
+    b.d = mk(0.0);
+    cf.step(dmk(mk(dtaus[mm]), mk(1.0)), a, b);
+    dlog_mgf_theta[(size_t)mm * P + p] = a.d + b.d * hp.v0;
+  }
+}
+
+// --------------------------------------------------------------------------------------------------------------------
 // host side
 // --------------------------------------------------------------------------------------------------------------------
 // Latency regime (few grid points in total): lane-parallel kernel; throughput regime (batches, the 40000-point psi grid): one thread per
@@ -2934,6 +3095,39 @@ static int queue_hessian_sums(ChainDev& d, const FourierChain& c, const cd* log_
   return 0;
 }
 
+// The theta launches of b200sv_*_price_chain_greeks_theta after the greeks launches of the twin (whose outputs they do not touch): the
+// theta kernel writes dlm [M][P] (and nfev [P] for the adaptive routes), then fourier_vanilla_greeks_kernel<1> sums it on the log-MGF the
+// parameter rows were summed on: its row 2 is scale * S_T = d price / d T, so theta = -row 2 (DESIGN.md §4.8).
+struct ThetaDev {
+  DevBuf dlm, nfev, g;
+  explicit ThetaDev(cudaStream_t s) : dlm(s), nfev(s), g(s) {}
+
+  int alloc(const FourierChain& c, bool adaptive) {
+    B200SV_CUDA(dlm.alloc(sizeof(cd) * (size_t)c.M * c.P));
+    if (adaptive) B200SV_CUDA(nfev.alloc(sizeof(int) * c.P));
+    B200SV_CUDA(g.alloc(sizeof(double) * 3 * c.ss.size()));
+    return 0;
+  }
+  int sums(const ChainDev& d, const FourierChain& c, const cd* log_mgf) {
+    if (int rc = check_launch("theta kernel")) return rc;
+    if (c.Jtot == 0) return 0;
+    fourier_vanilla_greeks_kernel<1><<<c.Jtot, kFourierThreads, 0, d.st>>>(log_mgf, dlm.as<cd>(), d.phi.as<cd>(), c.P, c.M,
+                                                                           d.rows.as<StrikeSpec>(), c.spot ? 1 : 0, g.as<double>());
+    return check_launch("fourier_vanilla_greeks_kernel");
+  }
+  // queues the copies of d price / d T into theta_out and of dlm / nfev (when asked); finish() negates after the closing synchronisation
+  int download(const FourierChain& c, double* theta_out, double* dlog_mgf_theta_out, int* nfev_out) {
+    if (c.Jtot > 0)
+      B200SV_CUDA(cudaMemcpyAsync(theta_out, g.as<double>() + 2 * (size_t)c.Jtot, sizeof(double) * c.Jtot, cudaMemcpyDeviceToHost, g.st));
+    B200SV_CUDA(dlm.download(cplx(dlog_mgf_theta_out), (size_t)c.M * c.P));
+    B200SV_CUDA(nfev.download(nfev_out, c.P));
+    return 0;
+  }
+  static void finish(const FourierChain& c, double* theta_out) {
+    for (int j = 0; j < c.Jtot; ++j) theta_out[j] = -theta_out[j];
+  }
+};
+
 static int check_expansion_order(int expansion_order) {
   if (expansion_order != B200SV_ORDER_FIRST && expansion_order != B200SV_ORDER_SECOND) return fail(-4, "expansion_order not implemented");
   return 0;
@@ -3179,6 +3373,80 @@ int b200sv_hawkesjd_price_chain_hessian(const b200sv_hawkes_params* params, int 
   // the tangent kernel's primal log-MGF and tangents, as for the first-order rows
   if (int rc = queue_hessian_sums<NP>(d, c, g.lm.as<cd>(), g.dlm.as<cd>(), d_d2lm, vanna_out, hessian_out, d2log_mgf_out)) return rc;
   return g.download(d, c, greeks_out, dlog_mgf_out, nfev_out);
+}
+
+/* ---- theta of the three Fourier chain pricers (DESIGN.md §4.8) ----
+ * The launches of b200sv_*_price_chain_greeks unchanged (bit-identical outputs), then the theta kernel and fourier_vanilla_greeks_kernel<1>
+ * on the log-MGF the parameter rows were summed on; one synchronisation at the end. */
+int b200sv_logsv_price_chain_greeks_theta(const b200sv_logsv_params* params, int M, const double* ttms, const double* forwards,
+                                          const double* discfactors, const double* etas, const int* offsets, const double* strikes,
+                                          const int8_t* types, int is_spot_measure, int variable_type, int expansion_order,
+                                          double vol_scaler, int P, double* prices_out, double* greeks_out, double* dlog_mgf_out,
+                                          int* nfev_out, double* theta_out, double* dlog_mgf_theta_out, int* theta_nfev_out) {
+  B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && greeks_out && theta_out, "null pointer");
+  if (variable_type != B200SV_LOG_RETURN) return fail(-4, "variable_type not implemented: sensitivities cover LOG_RETURN only");
+  FourierChain c;
+  if (int rc = prepare_logsv_chain(c, params, M, ttms, forwards, discfactors, offsets, strikes, types, is_spot_measure, variable_type,
+                                   expansion_order, vol_scaler, P))
+    return rc;
+  ChainDev d;
+  GreeksDev<1 + kLogsvOdeDirs> g(d.st);
+  if (int rc = queue_logsv_greeks(d, g, c, params, etas, expansion_order, prices_out)) return rc;
+  ThetaDev t(d.st);
+  if (int rc = t.alloc(c, true)) return rc;
+  const auto theta = expansion_order == B200SV_ORDER_FIRST ? logsv_mgf_theta_kernel<3> : logsv_mgf_theta_kernel<5>;
+  theta<<<(c.P + kThetaTPB - 1) / kThetaTPB, kThetaTPB, 0, d.st>>>(d.phi.as<cd>(), c.P, M, d.spec.as<ChainSpec>(), params->sigma0 - params->theta,
+                                                                   t.dlm.as<cd>(), t.nfev.as<int>());
+  if (int rc = t.sums(d, c, g.lm.as<cd>())) return rc;
+  if (int rc = t.download(c, theta_out, dlog_mgf_theta_out, theta_nfev_out)) return rc;
+  if (int rc = g.download(d, c, greeks_out, dlog_mgf_out, nfev_out)) return rc;
+  ThetaDev::finish(c, theta_out);
+  return 0;
+}
+
+int b200sv_heston_price_chain_greeks_theta(const b200sv_heston_params* params, int M, const double* ttms, const double* forwards,
+                                           const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
+                                           int variable_type, double vol_scaler, int P, double* prices_out, double* greeks_out,
+                                           double* dlog_mgf_out, double* theta_out, double* dlog_mgf_theta_out) {
+  B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && greeks_out && theta_out, "null pointer");
+  if (variable_type != B200SV_LOG_RETURN) return fail(-4, "variable_type not implemented: sensitivities cover LOG_RETURN only");
+  FourierChain c;
+  if (int rc = prepare_heston_chain(c, params, M, ttms, forwards, discfactors, offsets, strikes, types, variable_type, vol_scaler, P)) return rc;
+  ChainDev d;
+  GreeksDev<1 + kHestonOdeDirs> g(d.st);
+  if (int rc = queue_heston_greeks(d, g, c, params, prices_out)) return rc;
+  ThetaDev t(d.st);
+  if (int rc = t.alloc(c, false)) return rc;
+  heston_mgf_theta_kernel<<<(c.P + 63) / 64, 64, 0, d.st>>>(d.phi.as<cd>(), c.P, M, d.dt.as<double>(), *params, t.dlm.as<cd>());
+  if (int rc = t.sums(d, c, d.lm.as<cd>())) return rc;
+  if (int rc = t.download(c, theta_out, dlog_mgf_theta_out, nullptr)) return rc;
+  if (int rc = g.download(d, c, greeks_out, dlog_mgf_out, nullptr)) return rc;
+  ThetaDev::finish(c, theta_out);
+  return 0;
+}
+
+int b200sv_hawkesjd_price_chain_greeks_theta(const b200sv_hawkes_params* params, int M, const double* ttms, const double* forwards,
+                                             const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
+                                             int is_spot_measure, double vol_scaler, int P, double* prices_out, double* greeks_out,
+                                             double* dlog_mgf_out, int* nfev_out, double* theta_out, double* dlog_mgf_theta_out,
+                                             int* theta_nfev_out) {
+  B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && greeks_out && theta_out, "null pointer");
+  FourierChain c;
+  if (int rc = prepare_hawkes_chain(c, params, M, ttms, forwards, discfactors, offsets, strikes, types, is_spot_measure, vol_scaler, P, NAN))
+    return rc;
+  const HawkesMgfConsts k = make_hawkes_mgf_consts(*params);
+  ChainDev d;
+  GreeksDev<kHawkesGreekParams> g(d.st);
+  if (int rc = queue_hawkes_greeks(d, g, c, *params, k, prices_out)) return rc;
+  ThetaDev t(d.st);
+  if (int rc = t.alloc(c, true)) return rc;
+  hawkes_mgf_theta_kernel<<<(c.P + kThetaTPB - 1) / kThetaTPB, kThetaTPB, 0, d.st>>>(d.phi.as<cd>(), c.P, M, d.dt.as<double>(), k,
+                                                                                     t.dlm.as<cd>(), t.nfev.as<int>());
+  if (int rc = t.sums(d, c, g.lm.as<cd>())) return rc;
+  if (int rc = t.download(c, theta_out, dlog_mgf_theta_out, theta_nfev_out)) return rc;
+  if (int rc = g.download(d, c, greeks_out, dlog_mgf_out, nfev_out)) return rc;
+  ThetaDev::finish(c, theta_out);
+  return 0;
 }
 
 /* B Hawkes parameter sets on one chain in one pass (the calibration drivers' objective and its finite-difference neighbours).  The Riccati

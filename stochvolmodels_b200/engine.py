@@ -551,9 +551,11 @@ def hawkesjd_price_chain(params: C.HawkesParamsC, ttms, forwards, discfactors, s
 
 
 def _price_chain_greeks(symbol: str, params, chain, etas, is_spot_measure: bool, head, vol_scaler, max_phi: int, return_grids: bool, names,
-                        with_nfev: bool):
+                        with_nfev: bool, with_theta: bool = False):
     """the Fourier greeks entry points: C arguments (params, chain block, *head, vol_scaler, max_phi, prices, greeks [2 + P, J],
-    dlog_mgf [P, M, max_phi][, nfev [max_phi]]) -> (prices per maturity, greeks, offsets[, dlog_mgf[, nfev]])"""
+    dlog_mgf [P, M, max_phi][, nfev [max_phi]]) -> (prices per maturity, greeks, offsets[, dlog_mgf[, nfev]]).  ``with_theta``: the
+    symbol's _theta twin, which also takes theta [J], dlog_mgf_theta [M, max_phi][, theta_nfev [max_phi]], returned after the rest as
+    (theta[, dlog_mgf_theta[, theta_nfev]])"""
     _check_fourier_types(chain[4], is_spot_measure)
     ch = _chain_arrays(*chain)
     etas = _backbone(etas, ch.M)
@@ -562,29 +564,38 @@ def _price_chain_greeks(symbol: str, params, chain, etas, is_spot_measure: bool,
     grids = (np.empty((n, ch.M, max_phi), dtype=np.complex128) if return_grids else None,)
     if with_nfev:
         grids += (np.empty(max_phi, dtype=np.int32) if return_grids else None,)
+    theta_args, theta_out = (), ()
+    if with_theta:
+        symbol += "_theta"
+        theta_out = (np.empty(J), np.empty((ch.M, max_phi), dtype=np.complex128) if return_grids else None)
+        if with_nfev:
+            theta_out += (np.empty(max_phi, dtype=np.int32) if return_grids else None,)
+        theta_args = (C.dptr(theta_out[0]), C.dptr(theta_out[1]), *map(C.iptr, theta_out[2:]))
     C.call(symbol, byref(params), *C.chain_ptrs(ch, *etas), *head, C.vol_scaler_arg(vol_scaler), max_phi, C.dptr(prices), C.dptr(greeks),
-           C.dptr(grids[0]), *map(C.iptr, grids[1:]))
-    out = (C.split_chain(prices, ch.offsets), greeks, ch.offsets)
-    return out + grids if return_grids else out
+           C.dptr(grids[0]), *map(C.iptr, grids[1:]), *theta_args)
+    out = (C.split_chain(prices, ch.offsets), greeks, ch.offsets) + (grids if return_grids else ())
+    return out + (theta_out if return_grids else theta_out[:1])
 
 
 def logsv_price_chain_greeks(params: C.LogsvParamsC, ttms, forwards, discfactors, etas, strikes_ttms, optiontypes_ttms,
                              is_spot_measure: bool = True, expansion_order: int = C.ORDER_SECOND, vol_scaler: Optional[float] = None,
-                             max_phi: Optional[int] = None, return_grids: bool = False):
+                             max_phi: Optional[int] = None, return_grids: bool = False, with_theta: bool = False):
     """Fourier prices and forward-mode sensitivities of the chain (b200sv_logsv_price_chain_greeks).  Returns (prices per maturity,
     greeks [2 + 6, J], offsets) -- greeks rows: delta, gamma, then LOGSV_GREEK_PARAMS -- and with ``return_grids`` also
-    (dlog_mgf [6, M, P], nfev [P])."""
+    (dlog_mgf [6, M, P], nfev [P]).  ``with_theta`` (b200sv_logsv_price_chain_greeks_theta, the rest bit for bit) appends theta [J] and,
+    with ``return_grids``, (dlog_mgf_theta [M, P], theta_nfev [P])."""
     return _price_chain_greeks("b200sv_logsv_price_chain_greeks", params, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms), (etas,),
                                is_spot_measure, (int(bool(is_spot_measure)), C.LOG_RETURN, int(expansion_order)), vol_scaler,
-                               int(max_phi or 1000), return_grids, LOGSV_GREEK_PARAMS, True)
+                               int(max_phi or 1000), return_grids, LOGSV_GREEK_PARAMS, True, with_theta)
 
 
 def heston_price_chain_greeks(params: C.HestonParamsC, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms,
-                              vol_scaler: Optional[float] = None, max_phi: Optional[int] = None, return_grids: bool = False):
+                              vol_scaler: Optional[float] = None, max_phi: Optional[int] = None, return_grids: bool = False,
+                              with_theta: bool = False):
     """Heston twin of logsv_price_chain_greeks (b200sv_heston_price_chain_greeks): greeks rows = delta, gamma, then HESTON_GREEK_PARAMS;
-    ``return_grids`` adds dlog_mgf [5, M, P]."""
+    ``return_grids`` adds dlog_mgf [5, M, P]; ``with_theta`` appends theta [J] (and dlog_mgf_theta [M, P] with ``return_grids``)."""
     return _price_chain_greeks("b200sv_heston_price_chain_greeks", params, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms), (),
-                               True, (C.LOG_RETURN,), vol_scaler, int(max_phi or 1000), return_grids, HESTON_GREEK_PARAMS, False)
+                               True, (C.LOG_RETURN,), vol_scaler, int(max_phi or 1000), return_grids, HESTON_GREEK_PARAMS, False, with_theta)
 
 
 def _price_chain_hessian(symbol: str, params, chain, etas, is_spot_measure: bool, head, vol_scaler, max_phi: int, return_grids: bool, names,
@@ -627,12 +638,13 @@ def heston_price_chain_hessian(params: C.HestonParamsC, ttms, forwards, discfact
 
 def hawkesjd_price_chain_greeks(params: C.HawkesParamsC, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms,
                                 is_spot_measure: bool = True, vol_scaler: Optional[float] = None, max_phi: Optional[int] = None,
-                                return_grids: bool = False):
+                                return_grids: bool = False, with_theta: bool = False):
     """Hawkes twin of logsv_price_chain_greeks without a risk kernel (b200sv_hawkesjd_price_chain_greeks): greeks rows = delta, gamma, then
-    HAWKES_GREEK_PARAMS; ``return_grids`` adds (dlog_mgf [15, M, P], nfev [P]).  P defaults to the route's 500 points."""
+    HAWKES_GREEK_PARAMS; ``return_grids`` adds (dlog_mgf [15, M, P], nfev [P]).  P defaults to the route's 500 points.  ``with_theta`` as
+    for logsv_price_chain_greeks."""
     return _price_chain_greeks("b200sv_hawkesjd_price_chain_greeks", params, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms), (),
                                is_spot_measure, (int(bool(is_spot_measure)),), vol_scaler, int(max_phi or 500), return_grids,
-                               HAWKES_GREEK_PARAMS, True)
+                               HAWKES_GREEK_PARAMS, True, with_theta)
 
 
 def hawkesjd_price_chain_hessian(params: C.HawkesParamsC, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms,
@@ -833,6 +845,21 @@ def bsm_implied_vol_sensitivities(ttms, forwards, discfactors, strikes_ttms, opt
     C.call("b200sv_bsm_implied_vol_sensitivities", *C.chain_ptrs(ch), C.dptr(prices), P, C.dptr(greeks), C.dptr(vanna), C.dptr(hessian),
            C.dptr(ivols), C.dptr(ivol_greeks), C.dptr(ivol_vanna), C.dptr(ivol_hessian))
     return C.split_chain(ivols, ch.offsets), ivol_greeks, ivol_vanna, ivol_hessian
+
+
+def bsm_implied_vol_theta(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, prices_ttms, theta):
+    """implied vols of the model prices and their theta in one kernel launch (b200sv_bsm_implied_vol_theta; DESIGN.md §4.8).  ``theta`` [J]:
+    -d price / d ttm as the *_price_chain_greeks entry points return it with ``with_theta``.  Returns (ivols per maturity, ivol_theta [J]) --
+    -d ivol / d ttm at fixed forward and discount factor; the ivols bit-identical to bsm_implied_vols."""
+    ch = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
+    prices = C.f64(np.concatenate([np.asarray(p, dtype=np.float64).ravel() for p in prices_ttms]))
+    J = ch.strikes.shape[0]
+    theta = C.f64(theta)
+    if prices.shape[0] != J or theta.shape != (J,):
+        raise ValueError(f"model prices and theta must have {J} entries, one per strike")
+    ivols, ivol_theta = np.empty(J), np.empty(J)
+    C.call("b200sv_bsm_implied_vol_theta", *C.chain_ptrs(ch), C.dptr(prices), C.dptr(theta), C.dptr(ivols), C.dptr(ivol_theta))
+    return C.split_chain(ivols, ch.offsets), ivol_theta
 
 
 def infer_bsm_ivols_from_model_chain_prices(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, model_prices_ttms):

@@ -8,7 +8,7 @@ transform grid is held fixed.  No step size to choose.
 """
 from __future__ import annotations
 
-from dataclasses import dataclass
+from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence
 
 import numpy as np
@@ -19,11 +19,13 @@ from .. import _capi as C
 @dataclass
 class FourierChainGreeks:
     """prices / delta (d price / d forward) / gamma (d^2 price / d forward^2): one array per maturity.  ``params``: parameter name
-    (dataclass field, after ``__post_init__``) -> one array per maturity of d price / d parameter."""
+    (dataclass field, after ``__post_init__``) -> one array per maturity of d price / d parameter.  ``theta`` (with ``with_theta=True``,
+    else None): one array per maturity of -d price / d ttm per year, DESIGN.md §4.8."""
     prices: List[np.ndarray]
     delta: List[np.ndarray]
     gamma: List[np.ndarray]
     params: Dict[str, List[np.ndarray]]
+    theta: Optional[List[np.ndarray]] = field(default=None, kw_only=True)
 
 
 @dataclass
@@ -40,11 +42,13 @@ class ChainIvolGreeks:
     """implied-vol sensitivities of a chain (DESIGN.md §4.6), one array per maturity: ``ivols`` (bit-identical to
     ``compute_chain_prices_with_vols`` with the same arguments), ``delta`` / ``gamma`` (d ivol / d forward, d^2 ivol / d forward^2, sticky
     strike) and ``params``: parameter name -> d ivol / d parameter.  NaN where the ivol is NaN, 0 where it is an end of the inversion
-    bracket (1e-8 or 10).  ``gamma`` is None for Monte Carlo sensitivities without a gamma row."""
+    bracket (1e-8 or 10).  ``gamma`` is None for Monte Carlo sensitivities without a gamma row.  ``theta`` (with ``with_theta=True``, else
+    None): -d ivol / d ttm per year at fixed forward and discount factor, under the same NaN / bracket-end rules (DESIGN.md §4.8)."""
     ivols: List[np.ndarray]
     delta: List[np.ndarray]
     gamma: Optional[List[np.ndarray]]
     params: Dict[str, List[np.ndarray]]
+    theta: Optional[List[np.ndarray]] = field(default=None, kw_only=True)
 
 
 @dataclass
@@ -63,7 +67,8 @@ def to_chain_ivol_sensitivities(option_chain, greeks: FourierChainGreeks):
     """``FourierChainGreeks`` -> ``ChainIvolGreeks``, ``FourierChainHessian`` -> ``ChainIvolHessian``: the price rows mapped to implied-vol
     rows on the chain's forwards and discount factors by one engine.bsm_implied_vol_sensitivities call.  A Monte Carlo ``McChainGreeks``
     maps the same way (its standard errors are not carried over); without a gamma row (``gamma`` None) the transform gets zeros in its place
-    and the result has ``gamma=None``, the other rows being independent of it."""
+    and the result has ``gamma=None``, the other rows being independent of it.  A ``theta`` row is mapped by a second call,
+    engine.bsm_implied_vol_theta, on the same prices (the same ivols, bit for bit)."""
     from .. import engine
     names = list(greeks.params)
     delta = _flat(greeks.delta)
@@ -78,8 +83,13 @@ def to_chain_ivol_sensitivities(option_chain, greeks: FourierChainGreeks):
     offsets = np.zeros(len(ivols) + 1, dtype=np.int64)
     offsets[1:] = np.cumsum([a.size for a in ivols])
     split = lambda row: C.split_chain(row, offsets)
+    theta = None
+    if getattr(greeks, "theta", None) is not None:
+        theta = split(engine.bsm_implied_vol_theta(option_chain.ttms, option_chain.forwards, option_chain.discfactors,
+                                                   option_chain.strikes_ttms, option_chain.optiontypes_ttms, greeks.prices,
+                                                   _flat(greeks.theta))[1])
     first = ChainIvolGreeks(ivols=ivols, delta=split(g[0]), gamma=None if greeks.gamma is None else split(g[1]),
-                            params={n: split(g[2 + k]) for k, n in enumerate(names)})
+                            params={n: split(g[2 + k]) for k, n in enumerate(names)}, theta=theta)
     if not second:
         return first
     hess: Dict[str, Dict[str, List[np.ndarray]]] = {n: {} for n in names}
@@ -110,15 +120,17 @@ def check_fourier_greeks_kwargs(kwargs) -> None:
 
 
 def check_fourier_hessian_kwargs(kwargs) -> None:
-    """the same rejections for ``price_chain_hessian``"""
+    """the same rejections for ``price_chain_hessian``, which has no theta (second-order time terms are not covered)"""
+    if kwargs.get("with_theta"):
+        raise NotImplementedError("price_chain_hessian does not cover theta (with_theta): use price_chain_greeks(with_theta=True)")
     _check_fourier_kwargs(kwargs, "price_chain_hessian")
 
 
-def to_fourier_chain_greeks(prices, greeks, offsets, names: Sequence[str]) -> FourierChainGreeks:
-    """engine.*_price_chain_greeks output -> FourierChainGreeks"""
+def to_fourier_chain_greeks(prices, greeks, offsets, names: Sequence[str], theta=None) -> FourierChainGreeks:
+    """engine.*_price_chain_greeks output -> FourierChainGreeks; ``theta`` [J] (with_theta) or None"""
     split = lambda row: C.split_chain(row, offsets)
     return FourierChainGreeks(prices=prices, delta=split(greeks[0]), gamma=split(greeks[1]),
-                              params={n: split(greeks[2 + k]) for k, n in enumerate(names)})
+                              params={n: split(greeks[2 + k]) for k, n in enumerate(names)}, theta=None if theta is None else split(theta))
 
 
 def to_fourier_chain_hessian(prices, greeks, vanna, hessian, offsets, names: Sequence[str]) -> FourierChainHessian:

@@ -94,23 +94,26 @@ class HawkesJDPricer(ModelPricer):
         return pricer(model_params=params, ttms=option_chain.ttms, forwards=option_chain.forwards, discfactors=option_chain.discfactors,
                       strikes_ttms=option_chain.strikes_ttms, optiontypes_ttms=option_chain.optiontypes_ttms, is_spot_measure=is_spot_measure, **kwargs)
 
-    def price_chain_greeks(self, option_chain: OptionChain, params: HawkesJDParams, is_spot_measure: bool = True, **kwargs):
+    def price_chain_greeks(self, option_chain: OptionChain, params: HawkesJDParams, is_spot_measure: bool = True, with_theta: bool = False,
+                           **kwargs):
         """Fourier prices (bit-identical to ``price_chain`` with the same arguments) plus forward-mode sensitivities in one call ->
         ``FourierChainGreeks``: delta and gamma in the slice forward and d price / d HAWKES_GREEK_PARAMS (every field but ``mu``, which the
         Fourier route does not read, and ``risk_premia_gamma``).  The compensators are differentiated through ``shift`` and ``mean``.  Takes
         ``vol_scaler`` like ``price_chain``; the transform grid is held fixed, so the dependence of the default ``vol_scaler`` on ``sigma``
         (through clip(sigma, 0.2, 0.5)) is not differentiated, nor are the discount factors.  A risk kernel (``risk_premia_gamma``), the BDF
-        branch and Q_VAR raise NotImplementedError."""
+        branch and Q_VAR raise NotImplementedError.  ``with_theta``: also ``theta`` = -d price / d ttm per maturity (DESIGN.md §4.8), exact on
+        the solver's accepted mesh with the earlier maturities and the grid held; every other output bit for bit."""
         from .fourier_greeks import check_fourier_greeks_kwargs, to_fourier_chain_greeks
         if params.risk_premia_gamma is not None:
             raise NotImplementedError("price_chain_greeks does not cover the risk-kernel pricer (risk_premia_gamma)")
         check_fourier_greeks_kwargs(kwargs)
         d = params.to_dict()
         d.pop("risk_premia_gamma", None)
-        prices, greeks, offsets = engine.hawkesjd_price_chain_greeks(
+        out = engine.hawkesjd_price_chain_greeks(
             _params_c(**d), option_chain.ttms, option_chain.forwards, option_chain.discfactors, option_chain.strikes_ttms,
-            option_chain.optiontypes_ttms, is_spot_measure=is_spot_measure, vol_scaler=kwargs.get("vol_scaler"), max_phi=MAX_PHI)
-        return to_fourier_chain_greeks(prices, greeks, offsets, engine.HAWKES_GREEK_PARAMS)
+            option_chain.optiontypes_ttms, is_spot_measure=is_spot_measure, vol_scaler=kwargs.get("vol_scaler"), max_phi=MAX_PHI,
+            **({"with_theta": True} if with_theta else {}))
+        return to_fourier_chain_greeks(*out[:3], engine.HAWKES_GREEK_PARAMS, *out[3:])
 
     def price_chain_hessian(self, option_chain: OptionChain, params: HawkesJDParams, is_spot_measure: bool = True, **kwargs):
         """``price_chain_greeks`` (bit for bit) plus the second order in one call -> ``FourierChainHessian``: vanna (d^2 price / d forward

@@ -58,16 +58,18 @@ class HestonPricer(ModelPricer):
                                    strikes_ttms=option_chain.strikes_ttms, optiontypes_ttms=option_chain.optiontypes_ttms,
                                    vol_scaler=kwargs.get("vol_scaler"))
 
-    def price_chain_greeks(self, option_chain: OptionChain, params: HestonParams, **kwargs):
+    def price_chain_greeks(self, option_chain: OptionChain, params: HestonParams, with_theta: bool = False, **kwargs):
         """Fourier prices (bit-identical to ``price_chain`` with the same ``vol_scaler``) plus forward-mode sensitivities in one call ->
         ``FourierChainGreeks``: delta and gamma in the slice forward and d price / d (v0, theta, kappa, rho, volvol), exact derivatives of
-        the closed form on a fixed transform grid.  Q_VAR raises NotImplementedError."""
+        the closed form on a fixed transform grid.  Q_VAR raises NotImplementedError.  ``with_theta``: also ``theta`` = -d price / d ttm per
+        maturity (DESIGN.md §4.8), exact in the slice length with the earlier maturities and the grid held; every other output bit for bit."""
         from .fourier_greeks import check_fourier_greeks_kwargs, to_fourier_chain_greeks
         check_fourier_greeks_kwargs(kwargs)
-        prices, greeks, offsets = engine.heston_price_chain_greeks(
+        out = engine.heston_price_chain_greeks(
             _params_c(params.v0, params.theta, params.kappa, params.rho, params.volvol), option_chain.ttms, option_chain.forwards,
-            option_chain.discfactors, option_chain.strikes_ttms, option_chain.optiontypes_ttms, vol_scaler=kwargs.get("vol_scaler"))
-        return to_fourier_chain_greeks(prices, greeks, offsets, engine.HESTON_GREEK_PARAMS)
+            option_chain.discfactors, option_chain.strikes_ttms, option_chain.optiontypes_ttms, vol_scaler=kwargs.get("vol_scaler"),
+            **({"with_theta": True} if with_theta else {}))
+        return to_fourier_chain_greeks(*out[:3], engine.HESTON_GREEK_PARAMS, *out[3:])
 
     def price_chain_hessian(self, option_chain: OptionChain, params: HestonParams, **kwargs):
         """``price_chain_greeks`` (bit for bit) plus vanna and the symmetric Hessian over (v0, theta, kappa, rho, volvol) in one call ->

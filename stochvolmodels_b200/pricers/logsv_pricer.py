@@ -171,20 +171,23 @@ class LogSVPricer(ModelPricer):
                                   discfactors=option_chain.discfactors, strikes_ttms=option_chain.strikes_ttms,
                                   optiontypes_ttms=option_chain.optiontypes_ttms, is_spot_measure=is_spot_measure, **kwargs)
 
-    def price_chain_greeks(self, option_chain: OptionChain, params: LogSvParams, is_spot_measure: bool = True, **kwargs):
+    def price_chain_greeks(self, option_chain: OptionChain, params: LogSvParams, is_spot_measure: bool = True, with_theta: bool = False,
+                           **kwargs):
         """Fourier prices (bit-identical to ``price_chain`` with the same arguments) plus forward-mode sensitivities in one call ->
         ``FourierChainGreeks``: delta and gamma in the slice forward and d price / d (sigma0, theta, kappa1, kappa2, beta, volvol).  Takes
         ``expansion_order``, ``vol_scaler`` and ``max_phi`` like ``price_chain``; ``kappa2`` is the value after ``__post_init__`` and is held
         fixed when kappa1 or theta moves; the vol backbone, the discount factors and the transform grid are not differentiated.  The
-        semi-analytic and BDF branches, Q_VAR and the rough-vol route raise NotImplementedError."""
+        semi-analytic and BDF branches, Q_VAR and the rough-vol route raise NotImplementedError.  ``with_theta``: also ``theta`` = -d price /
+        d ttm per maturity (DESIGN.md §4.8), exact on the solver's accepted mesh with the earlier maturities, the backbone and the grid held;
+        every other output bit for bit as without it."""
         from .fourier_greeks import check_fourier_greeks_kwargs, to_fourier_chain_greeks
         check_fourier_greeks_kwargs(kwargs)
-        prices, greeks, offsets = engine.logsv_price_chain_greeks(
+        out = engine.logsv_price_chain_greeks(
             _params_c(params), option_chain.ttms, option_chain.forwards, option_chain.discfactors,
             params.get_vol_backbone_etas(ttms=option_chain.ttms), option_chain.strikes_ttms, option_chain.optiontypes_ttms,
             is_spot_measure=is_spot_measure, expansion_order=_order_code(kwargs.get("expansion_order", ExpansionOrder.SECOND)),
-            vol_scaler=kwargs.get("vol_scaler"), max_phi=kwargs.get("max_phi"))
-        return to_fourier_chain_greeks(prices, greeks, offsets, engine.LOGSV_GREEK_PARAMS)
+            vol_scaler=kwargs.get("vol_scaler"), max_phi=kwargs.get("max_phi"), **({"with_theta": True} if with_theta else {}))
+        return to_fourier_chain_greeks(*out[:3], engine.LOGSV_GREEK_PARAMS, *out[3:])
 
     def price_chain_hessian(self, option_chain: OptionChain, params: LogSvParams, is_spot_measure: bool = True, **kwargs):
         """``price_chain_greeks`` (bit for bit) plus the second-order sensitivities in one call -> ``FourierChainHessian``: vanna

@@ -40,17 +40,20 @@ class ModelPricer(ABC):
         model_ivols = option_chain.compute_model_ivols_from_chain_data(model_prices=model_prices)
         return model_prices, model_ivols
 
-    def compute_chain_ivol_greeks(self, option_chain: OptionChain, params: ModelParams, **kwargs):
+    def compute_chain_ivol_greeks(self, option_chain: OptionChain, params: ModelParams, with_theta: bool = False, **kwargs):
         """implied vols and their first-order sensitivities -> ``ChainIvolGreeks`` (DESIGN.md §4.6): ``self.price_chain_greeks`` with the
         same kwargs (and so its rejections, before any GPU work), then one GPU call that inverts the prices and maps the price rows to
         implied-vol rows.  The ivols are bit-identical to ``compute_chain_prices_with_vols`` with the same arguments; the rows are exact
-        derivatives of them on the transform grid the pricer holds fixed."""
+        derivatives of them on the transform grid the pricer holds fixed.  ``with_theta``: also the ivol theta -d ivol / d ttm (§4.8), from
+        ``price_chain_greeks(with_theta=True)`` and one more GPU call."""
         from .fourier_greeks import to_chain_ivol_sensitivities
+        if with_theta:
+            kwargs["with_theta"] = True
         return to_chain_ivol_sensitivities(option_chain, self.price_chain_greeks(option_chain, params, **kwargs))
 
     def compute_chain_ivol_hessian(self, option_chain: OptionChain, params: ModelParams, **kwargs):
         """``compute_chain_ivol_greeks`` plus the second order -> ``ChainIvolHessian``: from ``self.price_chain_hessian`` with the same
-        kwargs (same ivols, bit for bit)."""
+        kwargs (same ivols, bit for bit).  ``with_theta=True`` raises NotImplementedError, as ``price_chain_hessian`` does."""
         from .fourier_greeks import to_chain_ivol_sensitivities
         return to_chain_ivol_sensitivities(option_chain, self.price_chain_hessian(option_chain, params, **kwargs))
 
