@@ -402,6 +402,11 @@ int b200sv_debug_box_muller(const uint32_t* words, long long n, int flags, doubl
  * fast_div(a, b), fast_sqrt(a), fast_sqrt_pos(a), neg2_log(a) = -2 ln(a), exp_table(a) */
 enum { B200SV_DEBUG_FAST_DIV = 0, B200SV_DEBUG_FAST_SQRT = 1, B200SV_DEBUG_FAST_SQRT_POS = 2, B200SV_DEBUG_NEG2_LOG = 3, B200SV_DEBUG_EXP_TABLE = 4 };
 int b200sv_debug_fastmath(int op, const double* a, const double* b, long long n, double* out);
+/* test hook: the Hawkes stepper's jump-clock functions on caller-chosen 32-bit words r[i] against intensities lambda[i] at step dt (host
+ * arrays; params supplies shift / mean of the sizes).  out[n][6] = u = (r + 1/2) 2^-32, the clock -ln(u)/dt, the jump sizes
+ * shift_p + mean_p (-ln u) and shift_m - (-mean_m)(-ln u) as b200sv_hawkesjd_device_draws exports them, then 1.0 / 0.0 for the candidate
+ * filter on the raw word and for the fused firing decision of the in-kernel stepper, which must equal lambda > clock. */
+int b200sv_debug_hawkes_clocks(const uint32_t* r, const double* lambda, long long n, double dt, const b200sv_hawkes_params* params, double* out);
 
 /* ------------------------------------------------------------------------------------------------------------------
  * Fourier / MGF, host-level

@@ -123,6 +123,7 @@ SIGNATURES = {
     "b200sv_debug_exp_pair_scaled": [_dp, c_longlong, _dp],
     "b200sv_debug_box_muller": [POINTER(ctypes.c_uint32), c_longlong, c_int, _dp],
     "b200sv_debug_fastmath": [c_int, _dp, _dp, c_longlong, _dp],
+    "b200sv_debug_hawkes_clocks": [POINTER(ctypes.c_uint32), _dp, c_longlong, c_double, _kp, _dp],
     "b200sv_logsv_price_chain": [_lp, c_int, _dp, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_int, c_int, c_double, c_int, _dp, _dp, _dp],
     "b200sv_heston_price_chain": [_hp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_double, c_int, _dp, _dp],
     "b200sv_logsv_price_chain_greeks": [_lp, c_int, _dp, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_int, c_int, c_double, c_int, _dp, _dp, _dp, _ip],

@@ -113,8 +113,9 @@ struct HawkesSliceArgs {
 // Throughput stepper.  Per step the common case (no jump, ~99.5 % of the steps at the reference's parameters) is 8 contracted fp64
 // operations; whether a clock CAN fire is decided on the raw 32-bit word: -ln(u) >= 1 - u, so a jump needs 1 - u < lambda dt, i.e.
 // r >= floor(2^32 (1 - lambda dt (1 + 1e-9))) - 1 (one DFMA + F2I + integer compare; the margins cover the rounding of the product and of
-// the floor).  Only then are the logarithm, the exact comparison lambda > -ln(u)/dt of the reference (:767-768) and -- if it fires -- the
-// size stream evaluated.  Same draws as b200sv_hawkesjd_device_draws exports; agreement with the strict kernel ~1e-15 (FMA contraction).
+// the floor, tests/test_gpu_hawkes_edges.py checks the filter at its edge words).  Only then are the logarithm, the exact comparison
+// lambda > -ln(u)/dt of the reference (:767-768) and -- if it fires -- the size stream evaluated.  Same draws as b200sv_hawkesjd_device_draws
+// exports; agreement with the strict kernel ~1e-15 (FMA contraction).
 struct HawkesFast {
   double ssd;                // sigma sqrt(dt)
   double kdt_p, kdt_m;       // kappa dt
@@ -124,13 +125,22 @@ struct HawkesFast {
 
 // Does the clock with word r fire against intensity lam, i.e. is lam > -ln(u)/dt as the reference evaluates it (:767-768)?  With e = 1 - u
 // (exact in fp64): -ln(u) <= e + e^2 for e <= 1/2, so e + e^2 < lam dt (1 - 1e-9) settles it without a logarithm; the band in between
-// (relative width ~e, i.e. ~0.5 % of the candidates) takes the exact comparison, out of line.
+// (relative width ~e, i.e. ~0.5 % of the candidates) takes the exact comparison, out of line.  tests/test_gpu_hawkes_edges.py checks the
+// bound on both sides of its edge and at lam dt up to 50, where e + e^2 alone would accept wrongly beyond e ~ 0.68.
 __device__ __noinline__ bool hawkes_fires_exact(double lam, double u, double dt) { return lam > __ddiv_rn(-log(u), dt); }
 __device__ __forceinline__ bool hawkes_fires(double lam, uint32_t r, double dt, double dt_lo) {
   const double u = hawkes_uniform(r), e = 1.0 - u;
   if (e <= 0.5 && fma(e, e, e) < lam * dt_lo) return true;
   return hawkes_fires_exact(lam, u, dt);
 }
+// Can the clock with word r fire against lam at all (the filter above)?  fma(-lam, thr, 2^32) converts with saturation: lam <= 0 and
+// lam thr < 1 give UINT_MAX (only the two top words pass), lam dt >= 1 gives 0, which max(., 1) - 1 keeps at 0 (every word passes).
+__device__ __forceinline__ bool hawkes_candidate(double lam, uint32_t r, const HawkesFast& f) {
+  const uint32_t t = __double2uint_rd(fma(-lam, f.thr, 4294967296.0));
+  return r >= max(t, 1u) - 1u;
+}
+// The stepper's firing decision is hawkes_candidate(lam, r, f) && hawkes_fires(lam, r, dt, dt_lo), == (lam > hawkes_clock(hawkes_uniform(r))).
+// It is written out at its call sites rather than wrapped: any function layer around the && changes the slice kernels' machine code.
 // both clocks firing in one step (~1e-5 of the steps): out of line
 __device__ __noinline__ double2 hawkes_two_sizes(uint32_t wx, uint32_t wy, double shift_p, double mean_p, double shift_m, double mean_m) {
   return make_double2(__dadd_rn(shift_p, __dmul_rn(mean_p, -log(hawkes_uniform(wx)))), __dadd_rn(shift_m, -__dmul_rn(-mean_m, -log(hawkes_uniform(wy)))));
@@ -153,8 +163,7 @@ __device__ __forceinline__ void hawkes_path_steps(double& xi, double& lp, double
                                                   Hook& hk) {
   auto one_step = [&](double z, uint32_t rp, uint32_t rm, uint32_t step) {
     const double lp0 = lp, lm0 = lm;
-    const uint32_t tp = __double2uint_rd(fma(-lp, f.thr, 4294967296.0)), tm = __double2uint_rd(fma(-lm, f.thr, 4294967296.0));
-    const bool cand_p = rp >= max(tp, 1u) - 1u, cand_m = rm >= max(tm, 1u) - 1u;
+    const bool cand_p = hawkes_candidate(lp, rp, f), cand_m = hawkes_candidate(lm, rm, f);
     double jp = 0.0, jm = 0.0;
     bool fp_ = false, fm_ = false;
     if (cand_p || cand_m) {                                                     // ~1 % of the lane-steps: a clock may fire
@@ -434,6 +443,24 @@ __global__ void hawkes_device_draws_kernel(unsigned long long seed, unsigned lon
     J_P[o] = hawkes_size_p(hawkes_uniform(sz.x), c);
     J_M[o] = hawkes_size_m(hawkes_uniform(sz.y), c);
   }
+}
+
+// jump-clock self-test kernel (tests): per (word, intensity) pair out[6i..6i+5] = u, hawkes_clock(u), hawkes_size_p(u), hawkes_size_m(u),
+// the candidate flag and the stepper's firing decision, through the device functions hawkes_path_steps runs
+__global__ void hawkes_clocks_kernel(const uint32_t* __restrict__ r, const double* __restrict__ lam, long long n, HawkesConsts c,
+                                     double* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const HawkesFast f = hawkes_fast(c);
+  const uint32_t w = r[i];
+  const double l = lam[i], u = hawkes_uniform(w);
+  const bool cand = hawkes_candidate(l, w, f);
+  out[6 * i] = u;
+  out[6 * i + 1] = hawkes_clock(u, c);
+  out[6 * i + 2] = hawkes_size_p(u, c);
+  out[6 * i + 3] = hawkes_size_m(u, c);
+  out[6 * i + 4] = cand ? 1.0 : 0.0;
+  out[6 * i + 5] = cand && hawkes_fires(l, w, c.dt, f.dt_lo) ? 1.0 : 0.0;            // the decision of hawkes_path_steps' one_step
 }
 
 // one slice of the pricing kernel, or with `tan` of the tangent kernel on the same grid (moments_out then holds 2 + 15 values)

@@ -2677,6 +2677,24 @@ int b200sv_debug_fastmath(int op, const double* a, const double* b, long long n,
   return sync.done();
 }
 
+int b200sv_debug_hawkes_clocks(const uint32_t* r, const double* lambda, long long n, double dt, const b200sv_hawkes_params* params,
+                               double* out) {
+  B200SV_REQUIRE(r && lambda && params && out && n >= 1 && dt > 0.0, "null pointer / n / dt");
+  cudaStream_t st = current_stream();
+  StreamSync sync(st);
+  DevBuf dr(st), dl(st), dout(st);
+  B200SV_CUDA(dr.alloc(sizeof(uint32_t) * n));
+  B200SV_CUDA(dl.alloc(sizeof(double) * n));
+  B200SV_CUDA(dout.alloc(sizeof(double) * 6 * n));
+  B200SV_CUDA(cudaMemcpyAsync(dr.p, r, sizeof(uint32_t) * n, cudaMemcpyHostToDevice, st));
+  B200SV_CUDA(cudaMemcpyAsync(dl.p, lambda, sizeof(double) * n, cudaMemcpyHostToDevice, st));
+  hawkes_clocks_kernel<<<(int)((n + 127) / 128), 128, 0, st>>>(dr.as<uint32_t>(), dl.as<double>(), n, make_hawkes_consts(*params, dt),
+                                                               dout.as<double>());
+  if (int rc = check_launch("hawkes_clocks_kernel")) return rc;
+  B200SV_CUDA(cudaMemcpyAsync(out, dout.p, sizeof(double) * 6 * n, cudaMemcpyDeviceToHost, st));
+  return sync.done();
+}
+
 int b200sv_debug_exp_pair(const double* L, long long n, double* out /* 2n */) {
   B200SV_REQUIRE(L && out && n >= 1, "null pointer / n");
   cudaStream_t st = current_stream();

@@ -485,6 +485,17 @@ def debug_fastmath(op: int, a, b=None):
     return out
 
 
+def debug_hawkes_clocks(words, lam, dt: float, params: C.HawkesParamsC):
+    """the Hawkes stepper's jump-clock functions on 32-bit words against intensities (b200sv_debug_hawkes_clocks) -> [n, 6] float64:
+    u, clock -ln(u)/dt, size_p, size_m, candidate flag, fused firing decision."""
+    w = np.ascontiguousarray(np.asarray(words, dtype=np.uint32).ravel())
+    lam = C.f64(np.broadcast_to(np.asarray(lam, dtype=np.float64), w.shape))
+    out = np.empty((w.shape[0], 6))
+    C.call("b200sv_debug_hawkes_clocks", w.ctypes.data_as(ctypes.POINTER(ctypes.c_uint32)), C.dptr(lam), w.shape[0], float(dt), byref(params),
+           C.dptr(out))
+    return out
+
+
 # ---- Fourier / MGF --------------------------------------------------------------------------------------------------------
 def _check_fourier_types(optiontypes_ttms, is_spot_measure: bool):
     for types in optiontypes_ttms:
