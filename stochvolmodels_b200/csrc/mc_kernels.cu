@@ -779,7 +779,7 @@ __global__ void payoff_finalize_kernel(const double* __restrict__ sums, int J, d
   const double cnt = gat.world ? p2p_gather(gat, 3 * j + 2) : sums[3 * j + 2];
   const double mean = s1 / cnt;
   double var = s2 / cnt - mean * mean;
-  var = var > 0.0 ? var : 0.0;
+  var = var < 0.0 ? 0.0 : var;                                 // a NaN variance (infinite payoff sums) stays NaN, as in np.nanstd
   prices[j] = discfactor * mean;                               // discfactor*np.nanmean(payoff)
   stderrs[j] = discfactor * sqrt(var) / sqrt(total_paths);     // discfactor*np.nanstd(payoff) / sqrt(x0.shape[0])
   if (iv.ivols) iv.ivols[j] = black_implied_vol(iv.forward, iv.strikes[j], iv.ttm, discfactor, discfactor * mean, iv.types[j]);
