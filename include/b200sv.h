@@ -145,6 +145,25 @@ int b200sv_heston_mc_chain_greeks_gamma(const b200sv_heston_params* params, int 
                                         long long nb_path, int nb_steps_per_year, int variable_type, uint64_t seed, int flags, int scheme,
                                         double* prices_out, double* stderr_out, double* greeks_out, double* greeks_se_out, double* gamma_out,
                                         double* gamma_se_out, long long n_paths_out, double* laststep_out);
+/* The _greeks_gamma calls above (gamma_out == NULL: no gamma, and none of its launches) plus the Monte Carlo theta -d price / d ttms[m] of
+ * every strike (DESIGN.md §3.12): theta_out and theta_se_out [J], per year, the standard error with the greeks' convention.  Pathwise in
+ * the step length of maturity m's slice with its step count int((ttms[m] - ttms[m-1]) * nb_steps_per_year) + 1 held, and with the slice's
+ * forward, discount factor and vol backbone eta and the earlier maturities held: unbiased for the discretised scheme.  Every other output is
+ * bit-identical to the _greeks / _greeks_gamma call with the same arguments; the same flags and schemes are rejected.  Optional test hook
+ * (dtheta_out may be NULL): dtheta_out [M][2][n_paths_out] = (dx, dq) / d dt of paths [0, n_paths_out) after maturity m, dt the slice's
+ * step length. */
+int b200sv_logsv_mc_chain_greeks_theta(const b200sv_logsv_params* params, int M, const double* ttms, const double* forwards,
+                                       const double* discfactors, const double* etas, const int* offsets, const double* strikes,
+                                       const int8_t* types, long long nb_path, int nb_steps_per_year, int is_spot_measure, int variable_type,
+                                       uint64_t seed, int flags, double* prices_out, double* stderr_out, double* greeks_out,
+                                       double* greeks_se_out, double* gamma_out, double* gamma_se_out, long long n_paths_out,
+                                       double* laststep_out, double* theta_out, double* theta_se_out, double* dtheta_out);
+int b200sv_heston_mc_chain_greeks_theta(const b200sv_heston_params* params, int M, const double* ttms, const double* forwards,
+                                        const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
+                                        long long nb_path, int nb_steps_per_year, int variable_type, uint64_t seed, int flags, int scheme,
+                                        double* prices_out, double* stderr_out, double* greeks_out, double* greeks_se_out, double* gamma_out,
+                                        double* gamma_se_out, long long n_paths_out, double* laststep_out, double* theta_out,
+                                        double* theta_se_out, double* dtheta_out);
 
 /* test entry points of the tangent stepper: one slice of ttm from (0, sigma0 | v0, 0) for the global paths [path_offset, path_offset + nb_path)
  * of Philox slice `slice_index`.  x, sigma | var, qvar: nb_path doubles; dx, dsigma | dvar, dqvar: [P][nb_path] tangents in the parameter
@@ -302,6 +321,19 @@ int b200sv_rough_logsv_mc_chain_greeks(const b200sv_logsv_params* params, int n_
                                        const double* Z0, const double* Z1, long long z_rows, int variable_type, uint64_t seed, int flags,
                                        double* prices_out, double* stderr_out, double* greeks_out, double* greeks_se_out, double* states_out,
                                        double* tangents_out, double* resets_out);
+/* The call above plus the Monte Carlo theta -d price / d ttms[m] of every strike (DESIGN.md §3.12): theta_out and theta_se_out [J], per year,
+ * the standard error df std / sqrt(nb_path).  Every maturity restarts at t = 0 on its grid of nsteps[m] steps of hs[m]; theta is pathwise in
+ * that step length with nsteps[m] held (d / d ttms[m] = (1 / nsteps[m]) d / d h), with the forward and discount factor held; the theta row
+ * omits the same reset-branch mass as the parameter rows (resets_out).  Every other output is bit-identical to the _greeks call with the same
+ * arguments.  Optional test hook (dtheta_out may be NULL): dtheta_out [M][2][n_paths_out] = (d log_spot, d qv) / d h of paths
+ * [0, n_paths_out) at maturity m. */
+int b200sv_rough_logsv_mc_chain_greeks_theta(const b200sv_logsv_params* params, int n_factors, const double* weights, const double* nodes, int M,
+                                             const double* ttms, const double* forwards, const double* discfactors, const int* offsets,
+                                             const double* strikes, const int8_t* types, long long nb_path, const int* nsteps, const double* hs,
+                                             const double* Z0, const double* Z1, long long z_rows, int variable_type, uint64_t seed, int flags,
+                                             double* prices_out, double* stderr_out, double* greeks_out, double* greeks_se_out, double* states_out,
+                                             double* tangents_out, double* resets_out, double* theta_out, double* theta_se_out,
+                                             long long n_paths_out, double* dtheta_out);
 
 /* Hawkes jump-diffusion Monte Carlo (pricers/hawkes_jd_pricer.py): 1800 steps per year (:752), state (x, lambda_p, lambda_m).
  * b200sv_hawkesjd_mc_chain   = hawkesjd_mc_chain_pricer (:644-715): chained slices, forward-recentred payoffs on x; in-kernel draws (Philox;

@@ -69,6 +69,10 @@ SIGNATURES = {
                                            _dp, _dp, _dp, _dp, _dp, c_longlong, _dp],
     "b200sv_heston_mc_chain_greeks_gamma": [_hp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_longlong, c_int, c_int, c_uint64, c_int, c_int, _dp, _dp,
                                             _dp, _dp, _dp, _dp, c_longlong, _dp],
+    "b200sv_logsv_mc_chain_greeks_theta": [_lp, c_int, _dp, _dp, _dp, _dp, _ip, _dp, _i8p, c_longlong, c_int, c_int, c_int, c_uint64, c_int, _dp,
+                                           _dp, _dp, _dp, _dp, _dp, c_longlong, _dp, _dp, _dp, _dp],
+    "b200sv_heston_mc_chain_greeks_theta": [_hp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_longlong, c_int, c_int, c_uint64, c_int, c_int, _dp, _dp,
+                                            _dp, _dp, _dp, _dp, c_longlong, _dp, _dp, _dp, _dp],
     "b200sv_logsv_tangent_terminal": [_lp, c_double, c_longlong, c_int, c_int, c_double, c_uint64, c_int, c_int, c_longlong, _dp, _dp, _dp,
                                       _dp, _dp, _dp],
     "b200sv_heston_tangent_terminal": [_hp, c_double, c_longlong, c_int, c_uint64, c_int, c_int, c_longlong, _dp, _dp, _dp, _dp, _dp, _dp],
@@ -84,6 +88,8 @@ SIGNATURES = {
                                     c_int, c_uint64, c_int, _dp, _dp, _dp, _dp],
     "b200sv_rough_logsv_mc_chain_greeks": [_lp, c_int, _dp, _dp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_longlong, _ip, _dp, _dp, _dp, c_longlong,
                                            c_int, c_uint64, c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp],
+    "b200sv_rough_logsv_mc_chain_greeks_theta": [_lp, c_int, _dp, _dp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_longlong, _ip, _dp, _dp, _dp,
+                                                 c_longlong, c_int, c_uint64, c_int, _dp, _dp, _dp, _dp, _dp, _dp, _dp, _dp, _dp, c_longlong, _dp],
     "b200sv_hawkesjd_mc_chain": [_kp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_longlong, c_int, c_uint64, c_int, _dp, _dp],
     "b200sv_hawkesjd_mc_chain_greeks": [_kp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_longlong, c_int, c_uint64, c_int, _dp, _dp, _dp, _dp,
                                         c_longlong, _dp, _dp],

@@ -1122,6 +1122,133 @@ struct LastStepPath : TPath {
   }
 };
 
+// Monte Carlo theta (DESIGN.md §3.12): the one tangent direction d/d dt of a slice's step length, its step count S held, starting at 0 at
+// the slice's first step (the state at ttms[m - 1] does not depend on ttms[m]).  Every step constant is proportional to dt or sqrt(dt), so
+// its explicit derivative is c / dt or c / (2 dt); the *d members below hold those.  tq() hands the payoff kernel dq - qshift q with
+// qshift = S / ttm: the Q_VAR underlying is q / ttm and ttm moves by S per unit dt, so its derivative is tq() / ttm with no payoff branch.
+struct LogsvThetaConsts {
+  LogsvConsts c;
+  double a1, a2;                     // natural-unit a1, a2 (the recursion's Jacobian 1 - a1/sigma + a2*sigma)
+  double cx2, cq2;                   // 2 cx, 2 cq
+  double a0d, a1d, a2d, b0h, b1h;    // a0/dt, a1/dt, a2/dt, b0/(2dt), b1/(2dt)
+  double cxd, ceh, cqd;              // cx/dt, ce/(2dt), cq/dt
+  double qshift;
+};
+
+struct HestonThetaConsts {
+  HestonConsts c;
+  double kappa, hdt, hsdt;           // kappa, 1/(2dt), 1/(2 sqrt(dt))
+  double qshift;
+};
+
+static LogsvThetaConsts make_logsv_theta_consts(const b200sv_logsv_params& p, double eta, bool spot, double dt, double qshift) {
+  LogsvThetaConsts k;
+  k.c = make_logsv_consts(p, eta, spot, dt);
+  k.a1 = k.c.a1;
+  k.a2 = k.c.a2;
+  k.cx2 = 2.0 * k.c.cx;
+  k.cq2 = 2.0 * k.c.cq;
+  k.a0d = k.c.a0 / dt;
+  k.a1d = k.c.a1 / dt;
+  k.a2d = k.c.a2 / dt;
+  k.b0h = 0.5 * k.c.b0 / dt;
+  k.b1h = 0.5 * k.c.b1 / dt;
+  k.cxd = k.c.cx / dt;
+  k.ceh = 0.5 * k.c.ce / dt;
+  k.cqd = k.c.cq / dt;
+  k.qshift = qshift;
+  return k;
+}
+
+static HestonThetaConsts make_heston_theta_consts(const b200sv_heston_params& p, double dt, double qshift) {
+  HestonThetaConsts k;
+  k.c = make_heston_consts(p, dt, B200SV_HESTON_EULER_FLOOR);
+  k.kappa = p.kappa;
+  k.hdt = 0.5 / dt;
+  k.hsdt = 0.5 / std::sqrt(dt);
+  k.qshift = qshift;
+  return k;
+}
+
+// LogSV, on the old sigma:  dL' = dL (1 - a1/sigma + a2 sigma) + (a0 + a1/sigma + a2 sigma)/dt + (b0 z0 + b1 z1)/(2dt), 0 through a clamp;
+// dx += (2 cx sigma^2 + ce sigma z0) dL + (cx sigma^2 + ce sigma z0 / 2)/dt;  dq += 2 cq (sigma^2 dL + sigma'^2 dL') + cq (sigma^2 + sigma'^2)/dt
+struct LogsvThetaPath {
+  static constexpr int NP = 1;
+  static constexpr bool kPrefetch = B200SV_SLICE_PREFETCH != 0;
+  static constexpr bool kRecordsLastStep = false;
+  using Consts = LogsvThetaConsts;
+  LogsvPath<double> b;
+  double dx, dL, dq;
+  double s_first;
+  const Consts& k;     // the kernel's __grid_constant__ parameter
+  __device__ __forceinline__ LogsvThetaPath(const Consts& k_) : b(k_.c), k(k_) {}
+  __device__ __forceinline__ void load(double x, double v, double q, const TangentState&, long long, long long, bool) {
+    b.load(x, v, q);
+    s_first = v;
+    dx = dL = dq = 0.0;
+  }
+  template <bool SAFE>
+  __device__ __forceinline__ void step(double z0, double z1) {
+    const double so = b.s, io = b.inv;
+    b.template step<SAFE>(z0, z1);
+    const double sn = b.s, so2 = so * so, sn2 = sn * sn;
+    const double jac = fma(k.a2, so, fma(-k.a1, io, 1.0));
+    const double drive = fma(k.b0h, z0, fma(k.b1h, z1, fma(k.a2d, so, fma(k.a1d, io, k.a0d))));
+    const double sz = so * z0;
+    dx = fma(so * fma(k.cx2, so, k.c.ce * z0), dL, dx) + fma(k.cxd, so2, k.ceh * sz);
+    const bool clamped = SAFE && fabs(b.Ls) == kLogScaledMax;
+    const double dLn = clamped ? 0.0 : fma(jac, dL, drive);
+    dq += fma(k.cq2, fma(so2, dL, sn2 * dLn), k.cqd * (so2 + sn2));
+    dL = dLn;
+  }
+  __device__ __forceinline__ bool overflowed() const { return b.overflowed(); }
+  __device__ __forceinline__ double sigma() const { return b.sigma(); }
+  // LogsvTangentPath::x() / q(): the production kernels' contraction spelled out
+  __device__ __forceinline__ double s2_diff() const { return fma(s_first, s_first, -__dmul_rn(b.s, b.s)); }
+  __device__ __forceinline__ double x() const { return fma(b.ce, b.XM, fma(b.cx, s2_diff() + b.A, b.x0)); }
+  __device__ __forceinline__ double q() const { return fma(b.cq, s2_diff() + 2.0 * b.A, b.q0); }
+  __device__ __forceinline__ double tx(int) const { return dx; }
+  __device__ __forceinline__ double tq(int) const { return fma(-k.qshift, q(), dq); }
+  __device__ __forceinline__ double tv(int) const { return dL; }
+};
+
+// Heston floor-Euler, on the old v:  dv' = dv (1 - kappa dt) + kappa (theta - v) + dv (c0 z0 + c1 z1)/(2 sqrt v) + sqrt(v) (c0 z0 + c1 z1)/(2dt),
+// 0 where the floor binds;  dx += (-dt/2 + sqrt(dt) z0 / (2 sqrt v)) dv - v/2 + sqrt(v) z0 / (2 sqrt dt);  dq += dt dv + v
+struct HestonThetaPath {
+  static constexpr int NP = 1;
+  static constexpr bool kPrefetch = B200SV_SLICE_PREFETCH != 0;
+  static constexpr bool kRecordsLastStep = false;
+  using Consts = HestonThetaConsts;
+  HestonPath<double, false> b;
+  double dx, dv, dq;
+  const Consts& k;     // the kernel's __grid_constant__ parameter
+  __device__ __forceinline__ HestonThetaPath(const Consts& k_) : b(k_.c), k(k_) {}
+  __device__ __forceinline__ void load(double x, double v, double q, const TangentState&, long long, long long, bool) {
+    b.load(x, v, q);
+    dx = dv = dq = 0.0;
+  }
+  template <bool SAFE>
+  __device__ __forceinline__ void step(double z0, double z1) {
+    const double v = b.v, sig = sqrt(v), hs = 0.5 / sig;
+    b.template step<SAFE>(z0, z1);
+    const bool live = b.v > 1e-4;
+    const double noise = fma(b.c0, z0, b.c1 * z1);
+    const double fx = fma(b.sdt * z0, hs, b.hx);
+    const double jac = fma(noise, hs, 1.0 - b.kdt);
+    const double drive = fma(sig * noise, k.hdt, k.kappa * (b.theta - v));
+    dx = fma(fx, dv, dx) + fma(-0.5, v, sig * z0 * k.hsdt);
+    dq = fma(b.dt, dv, dq) + v;
+    dv = live ? fma(jac, dv, drive) : 0.0;
+  }
+  __device__ __forceinline__ bool overflowed() const { return false; }
+  __device__ __forceinline__ double sigma() const { return b.sigma(); }
+  __device__ __forceinline__ double x() const { return b.x(); }
+  __device__ __forceinline__ double q() const { return b.q(); }
+  __device__ __forceinline__ double tx(int) const { return dx; }
+  __device__ __forceinline__ double tq(int) const { return fma(-k.qshift, q(), dq); }
+  __device__ __forceinline__ double tv(int) const { return dv; }
+};
+
 // mc_slice_kernel with tangents: same persistent grid-stride loop, same Philox stream (counter = global path id, slice), same
 // overflow re-run.  Per-CTA partials [gridDim.x][2 + P]: sum F e^x, count, sum F e^x dx_p over the non-NaN spots.
 template <typename TPath, int GAUSS>
@@ -1418,6 +1545,22 @@ __global__ void gamma_finalize_kernel(const double* __restrict__ gsums, const do
   gamma_se[j] = discfactor * sqrt(var) / sqrt(total_paths);
 }
 
+// theta[Jtot] = -df mean(g) / S, theta_se = df std(g) / (S sqrt(total_paths)), g = the d/d dt row of payoff_greeks_kernel<1> over the theta
+// pass (column 5, 6 of its KV = 7 sums; the count is column 2, the price row's)
+__global__ void theta_finalize_kernel(const double* __restrict__ sums, int J, double discfactor, double nsteps, double total_paths,
+                                      double* __restrict__ theta, double* __restrict__ theta_se) {
+  constexpr int KV = 3 + 2 * 2;
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= J) return;
+  const double* s = sums + (size_t)KV * j;
+  const double cnt = s[2];
+  const double mean = s[5] / cnt;
+  double var = s[6] / cnt - mean * mean;
+  var = var > 0.0 ? var : 0.0;
+  theta[j] = -discfactor * mean / nsteps;
+  theta_se[j] = discfactor * sqrt(var) / (nsteps * sqrt(total_paths));
+}
+
 // --------------------------------------------------------------------------------------------------------------------
 // debug / parity export of the normals the fused kernel draws
 // --------------------------------------------------------------------------------------------------------------------
@@ -1592,8 +1735,16 @@ static LogsvTangentConsts tangent_consts(const b200sv_logsv_params& p, double et
 static HestonTangentConsts tangent_consts(const b200sv_heston_params& p, double, bool, double dt) { return make_heston_tangent_consts(p, dt); }
 static double v_init(const b200sv_logsv_params& p) { return p.sigma0; }
 static double v_init(const b200sv_heston_params& p) { return p.v0; }
+static LogsvThetaConsts theta_consts(const b200sv_logsv_params& p, double eta, bool spot, double dt, double qshift) {
+  return make_logsv_theta_consts(p, eta, spot, dt, qshift);
+}
+static HestonThetaConsts theta_consts(const b200sv_heston_params& p, double, bool, double dt, double qshift) {
+  return make_heston_theta_consts(p, dt, qshift);
+}
 template <typename TConsts>
 using TangentPathOf = std::conditional_t<std::is_same<TConsts, LogsvTangentConsts>::value, LogsvTangentPath, HestonTangentPath>;
+template <typename TConsts>
+using ThetaPathOf = std::conditional_t<std::is_same<TConsts, LogsvThetaConsts>::value, LogsvThetaPath, HestonThetaPath>;
 
 // (model, Heston scheme, state precision Real, Gaussian mode g) -> mc_slice_kernel; nullptr: the paired check mode on fp32 state
 template <typename Real, typename Consts>
@@ -1808,20 +1959,25 @@ struct ChainIO {
 // [prices | std errors | greeks [1 + NP] | greeks_se [1 + NP]][Jalloc].
 // SCORE: the payoff launches add the likelihood-ratio term of a score array (payoff_score_greeks_kernel, LOG_RETURN only)
 // with_gamma: two more result rows [gamma | gamma_se][Jalloc] after those, filled by payoff_gamma().
+// with_theta: two more rows [theta | theta_se][Jalloc] after all of those, filled by payoff_theta() from the theta pass's own moments
+// theta_moments() [3] and payoff sums (DESIGN.md §3.12).
 template <int NP, bool SCORE = false>
 struct GreeksChainIO : ChainIO {
   static constexpr int KV = 3 + 2 * (1 + NP);
+  static constexpr int KVT = 3 + 2 * 2;     // payoff_greeks_kernel<1>: price, delta, d/d dt
   long long n;
-  bool with_gamma;
+  bool with_gamma, with_theta;
   Grid gp;      // payoff_greeks_kernel's persistent grid, its blocks split across the strike chunks of a slice
   Grid gg;      // payoff_gamma_kernel's, likewise
-  DevBuf d_part, d_gpart, d_gsums;
+  Grid gt;      // payoff_greeks_kernel<1>'s, likewise
+  DevBuf d_part, d_gpart, d_gsums, d_tpart, d_tsums, d_tmom;
 
   GreeksChainIO(int M_, const double* ttms_, const double* forwards_, const double* discfactors_, const int* offsets_, const int8_t* types_,
-                int variable_type_, long long nb_path, cudaStream_t s, bool with_gamma_ = false)
+                int variable_type_, long long nb_path, cudaStream_t s, bool with_gamma_ = false, bool with_theta_ = false)
       : ChainIO(1, M_, ttms_, forwards_, discfactors_, offsets_, types_, variable_type_, s), n(nb_path), with_gamma(with_gamma_),
-        gp(payoff_grid(nb_path)), gg(with_gamma_ ? persistent_grid(payoff_gamma_kernel, kThreads, nb_path) : Grid{}), d_part(s), d_gpart(s),
-        d_gsums(s) {}
+        with_theta(with_theta_), gp(payoff_grid(nb_path)), gg(with_gamma_ ? persistent_grid(payoff_gamma_kernel, kThreads, nb_path) : Grid{}),
+        gt(with_theta_ ? persistent_grid(payoff_greeks_kernel<1>, kThreads, nb_path) : Grid{}), d_part(s), d_gpart(s), d_gsums(s), d_tpart(s),
+        d_tsums(s), d_tmom(s) {}
 
   static Grid payoff_grid(long long nb_path) {
     if constexpr (SCORE) return persistent_grid(payoff_score_greeks_kernel<NP>, kThreads, nb_path);
@@ -1838,7 +1994,32 @@ struct GreeksChainIO : ChainIO {
       B200SV_CUDA(d_gpart.alloc(sizeof(double) * (size_t)2 * kGammaStrikeChunk * gamma_chunks * gg.blocks));
       B200SV_CUDA(d_gsums.alloc(sizeof(double) * 2 * (size_t)Jalloc));
     }
-    return ChainIO::upload(strikes, 2 + NP, KV, 2 * (2 + NP) + (with_gamma ? 2 : 0));
+    if (with_theta) {
+      B200SV_CUDA(d_tpart.alloc(sizeof(double) * (size_t)KVT * kGreeksStrikeChunk * max_chunks * gt.blocks));
+      B200SV_CUDA(d_tsums.alloc(sizeof(double) * KVT * (size_t)Jalloc));
+      B200SV_CUDA(d_tmom.alloc(sizeof(double) * 3));
+    }
+    return ChainIO::upload(strikes, 2 + NP, KV, 2 * (2 + NP) + (with_gamma ? 2 : 0) + (with_theta ? 2 : 0));
+  }
+  double* theta_moments() const { return d_tmom.as<double>(); }
+
+  // maturity m of S steps: per-strike sums over the state (x, q) and the theta pass's tangents (dx, dq - qshift q) [n] under its moments
+  // theta_moments() -> the theta rows of the result block
+  int payoff_theta(int m, const double* x, const double* q, const double* dx, const double* dq, int S) {
+    const int J = offsets[m + 1] - offsets[m], jo = offsets[m] - offsets[0];
+    if (J == 0) return 0;
+    const int chunks = (J + kGreeksStrikeChunk - 1) / kGreeksStrikeChunk;
+    const int Kpad = KVT * kGreeksStrikeChunk * chunks;
+    const int blocks = std::max(1, gt.blocks / chunks);
+    payoff_greeks_kernel<1><<<dim3(blocks, chunks), gt.threads, 0, st>>>(x, q, dx, dq, n, ttms[m], forwards[m], d_strikes.as<double>() + jo,
+                                                                         d_types.as<int8_t>() + jo, J, variable_type, theta_moments(),
+                                                                         d_tpart.as<double>(), Kpad);
+    if (int rc = check_launch("payoff_greeks_kernel")) return rc;
+    reduce_partials_kernel<<<1, 256, 0, st>>>(d_tpart.as<double>(), blocks, Kpad, KVT * J, d_tsums.as<double>(), P2pPublish{});
+    if (int rc = check_launch("reduce_partials_kernel")) return rc;
+    double* o = d_out.as<double>() + (size_t)(2 * (2 + NP) + (with_gamma ? 2 : 0)) * Jalloc + jo;
+    theta_finalize_kernel<<<(J + 127) / 128, 128, 0, st>>>(d_tsums.as<double>(), J, discfactors[m], (double)S, (double)n, o, o + Jalloc);
+    return check_launch("theta_finalize_kernel");
   }
 
   // maturity m, after payoff(): per-strike sums of the smoothed gamma over the state (x, q) and the last step's laststep [2][n] = (s, mu)
@@ -1891,9 +2072,9 @@ struct GreeksChainIO : ChainIO {
   // and greeks_out, greeks_se_out [1 + NP][Jtot] (a non-empty chain has Jalloc == Jtot, so the block's rows are already the caller's);
   // with_gamma also gamma_out, gamma_se_out [Jtot]
   int copy_back(StreamSync& sync, double* prices_out, double* stderr_out, double* greeks_out, double* greeks_se_out, double* gamma_out = nullptr,
-                double* gamma_se_out = nullptr) const {
-    const size_t J = (size_t)Jtot, G = (size_t)(1 + NP) * J;
-    std::vector<double> h(2 * J + 2 * G + (with_gamma ? 2 * J : 0));
+                double* gamma_se_out = nullptr, double* theta_out = nullptr, double* theta_se_out = nullptr) const {
+    const size_t J = (size_t)Jtot, G = (size_t)(1 + NP) * J, T = 2 * J + 2 * G + (with_gamma ? 2 * J : 0);
+    std::vector<double> h(T + (with_theta ? 2 * J : 0));
     if (J > 0) B200SV_CUDA(d_out.download(h.data(), h.size()));
     if (int rc = sync.done()) return rc;
     if (J == 0) return 0;
@@ -1904,6 +2085,10 @@ struct GreeksChainIO : ChainIO {
     if (with_gamma) {
       memcpy(gamma_out, h.data() + 2 * J + 2 * G, sizeof(double) * J);
       memcpy(gamma_se_out, h.data() + 3 * J + 2 * G, sizeof(double) * J);
+    }
+    if (with_theta) {
+      memcpy(theta_out, h.data() + T, sizeof(double) * J);
+      memcpy(theta_se_out, h.data() + T + J, sizeof(double) * J);
     }
     return 0;
   }
@@ -2132,19 +2317,37 @@ static int launch_tangent_slice(int gauss, double* x, double* v, double* q, cons
   });
 }
 
+// the theta pass of one maturity slice (DESIGN.md §3.12): mc_tangent_slice_kernel<ThetaPathOf<.>> on the same Philox stream and grid shape
+// as the tangent pass, its primal the same LogsvPath / HestonPath step; moments_out[3] = (sum F e^x, count, sum F e^x dx_theta)
+template <typename HConsts>
+static int launch_theta_slice(int gauss, double* x, double* v, double* q, const TangentState& t, long long n, int init, double v_init, int nsteps,
+                              int slice_index, double forward, uint64_t seed, const HConsts& c, double* moments_out, cudaStream_t st) {
+  using HPath = ThetaPathOf<HConsts>;
+  const auto kernel = gauss == kGaussF64 ? mc_tangent_slice_kernel<HPath, kGaussF64> : mc_tangent_slice_kernel<HPath, kGaussF32>;
+  const Grid g = persistent_grid(kernel, kSliceThreads, n);
+  return slice_moments("mc_tangent_slice_kernel", 2 + HPath::NP, g.blocks, moments_out, st, nullptr, [&](double* partials) {
+    const SliceArgs<double> a{x, v, q, n, 0ull, init, v_init, nsteps, (unsigned int)slice_index, seed, forward, partials};
+    kernel<<<g.blocks, g.threads, 0, st>>>(a, t, c);
+  });
+}
+
 // chain driver: per maturity tangent slice -> moments -> per-strike payoff / sensitivity sums -> finalize (stand-alone launches, fixed-order
 // reductions).  greeks_out / greeks_se_out: [1 + P][Jtot], row 0 = forward delta.  gamma_out != nullptr: the slices record their last
 // step and the smoothed gamma rows gamma_out / gamma_se_out [Jtot] are added (DESIGN.md §3.9), the other outputs unchanged; laststep_out
 // [M][2][n_paths_out] (test hook, may be NULL) receives (s, mu) of paths [0, n_paths_out) after every maturity.
+// theta_out != nullptr: before each tangent slice a theta pass steps a copy of the state at ttms[m - 1] through the same slice with the
+// d/d dt tangent, and theta_out / theta_se_out [Jtot] = -d price / d ttms[m] are added (DESIGN.md §3.12), the other outputs and launches
+// unchanged; dtheta_out [M][2][n_paths_out] (test hook, may be NULL) receives (dx, dq) / d dt of paths [0, n_paths_out) after every maturity.
 template <typename Params>
 static int mc_chain_greeks_host(const Params& p, int M, const double* ttms, const double* forwards, const double* discfactors, const double* etas,
                                 const int* offsets, const double* strikes, const int8_t* types, long long nb_path, int nb_steps_per_year,
                                 int is_spot, int variable_type, uint64_t seed, int flags, double* prices_out, double* stderr_out,
                                 double* greeks_out, double* greeks_se_out, double* gamma_out = nullptr, double* gamma_se_out = nullptr,
-                                long long n_paths_out = 0, double* laststep_out = nullptr) {
+                                long long n_paths_out = 0, double* laststep_out = nullptr, double* theta_out = nullptr,
+                                double* theta_se_out = nullptr, double* dtheta_out = nullptr) {
   using TConsts = decltype(tangent_consts(p, 1.0, false, 1.0));
   constexpr int NP = TangentPathOf<TConsts>::NP;
-  const bool with_gamma = gamma_out != nullptr;
+  const bool with_gamma = gamma_out != nullptr, with_theta = theta_out != nullptr;
   B200SV_REQUIRE(nb_path >= 1, "nb_path must be >= 1");
   B200SV_REQUIRE(nb_steps_per_year >= 1, "nb_steps_per_year must be >= 1");
   B200SV_REQUIRE(n_paths_out >= 0 && n_paths_out <= nb_path, "n_paths_out must be in [0, nb_path]");
@@ -2154,27 +2357,53 @@ static int mc_chain_greeks_host(const Params& p, int M, const double* ttms, cons
   cudaStream_t st = current_stream();
   ensure_pool_threshold();
   StreamSync sync(st);
-  const size_t n = (size_t)nb_path, no = laststep_out ? (size_t)n_paths_out : 0;
+  const size_t n = (size_t)nb_path, no = laststep_out ? (size_t)n_paths_out : 0, nt = dtheta_out ? (size_t)n_paths_out : 0;
   DevBuf d_state(st);
-  GreeksChainIO<NP> io(M, ttms, forwards, discfactors, offsets, types, variable_type, nb_path, st, with_gamma);
-  B200SV_CUDA(d_state.alloc(sizeof(double) * (3 * n + 3 * (size_t)NP * n + (with_gamma ? 2 * n : 0))));
+  GreeksChainIO<NP> io(M, ttms, forwards, discfactors, offsets, types, variable_type, nb_path, st, with_gamma, with_theta);
+  B200SV_CUDA(d_state.alloc(sizeof(double) * (3 * n + 3 * (size_t)NP * n + (with_gamma ? 2 * n : 0) + (with_theta ? 6 * n : 0))));
   if (int rc = io.upload(strikes)) return rc;
   double *x = d_state.as<double>(), *v = x + n, *q = v + n;
   const TangentState t{q + n, q + n + NP * n, q + n + 2 * NP * n};
   double* laststep = with_gamma ? q + n + 3 * NP * n : nullptr;     // [2][n], reused across maturities
+  double* hstate = q + n + 3 * NP * n + (with_gamma ? 2 * n : 0);     // theta pass: (x, v, q) [3][n], then (dx, dv, dq) [3][n]
+  const TangentState ht{hstate + 3 * n, hstate + 4 * n, hstate + 5 * n};
+  std::vector<double> h_q(nt * M), qshift(M);                        // the hook's q and S / ttm, to undo tq()'s shift on the host
   for (int m = 0; m < M; ++m) {
     const auto [S, dt] = maturity_grid(ttms, m, nb_steps_per_year);
-    const TConsts c = tangent_consts(p, etas ? etas[m] : 1.0, is_spot != 0, dt);
+    const double eta = etas ? etas[m] : 1.0;
+    qshift[m] = (double)S / ttms[m];
+    if (with_theta) {
+      if (m > 0) B200SV_CUDA(cudaMemcpyAsync(hstate, x, sizeof(double) * 3 * n, cudaMemcpyDeviceToDevice, st));   // x, v, q are contiguous
+      const auto hc = theta_consts(p, eta, is_spot != 0, dt, qshift[m]);
+      if (int rc = launch_theta_slice(gauss, hstate, hstate + n, hstate + 2 * n, ht, nb_path, m == 0, v_init(p), S, m, forwards[m], seed, hc,
+                                      io.theta_moments(), st))
+        return rc;
+    }
+    const TConsts c = tangent_consts(p, eta, is_spot != 0, dt);
     if (int rc = launch_tangent_slice(gauss, x, v, q, t, nb_path, 0, m == 0, v_init(p), S, m, forwards[m], seed, c, io.moments(), st, laststep))
       return rc;
     if (int rc = io.payoff(m, x, q, t.dx, t.dq, (double)nb_path)) return rc;
-    if (!with_gamma) continue;
-    if (int rc = io.payoff_gamma(m, x, q, laststep)) return rc;
-    if (no)
-      B200SV_CUDA(cudaMemcpy2DAsync(laststep_out + 2 * no * m, sizeof(double) * no, laststep, sizeof(double) * n, sizeof(double) * no, 2,
+    if (with_gamma) {
+      if (int rc = io.payoff_gamma(m, x, q, laststep)) return rc;
+      if (no)
+        B200SV_CUDA(cudaMemcpy2DAsync(laststep_out + 2 * no * m, sizeof(double) * no, laststep, sizeof(double) * n, sizeof(double) * no, 2,
+                                      cudaMemcpyDeviceToHost, st));
+    }
+    if (!with_theta) continue;
+    // the theta rows re-centre with the pricing route's own (sum F e^x, count): the theta pass's primal is the same code on the same
+    // normals, and this makes the rows' state and re-centring those of the prices by construction
+    B200SV_CUDA(cudaMemcpyAsync(io.theta_moments(), io.moments(), sizeof(double) * 2, cudaMemcpyDeviceToDevice, st));
+    if (int rc = io.payoff_theta(m, x, q, ht.dx, ht.dq, S)) return rc;
+    if (nt) {
+      B200SV_CUDA(cudaMemcpy2DAsync(dtheta_out + 2 * nt * m, sizeof(double) * nt, ht.dx, sizeof(double) * 2 * n, sizeof(double) * nt, 2,
                                     cudaMemcpyDeviceToHost, st));
+      B200SV_CUDA(cudaMemcpyAsync(h_q.data() + nt * m, hstate + 2 * n, sizeof(double) * nt, cudaMemcpyDeviceToHost, st));
+    }
   }
-  return io.copy_back(sync, prices_out, stderr_out, greeks_out, greeks_se_out, gamma_out, gamma_se_out);
+  if (int rc = io.copy_back(sync, prices_out, stderr_out, greeks_out, greeks_se_out, gamma_out, gamma_se_out, theta_out, theta_se_out)) return rc;
+  for (int m = 0; m < M; ++m)
+    for (size_t i = 0; i < nt; ++i) dtheta_out[(2 * m + 1) * nt + i] += qshift[m] * h_q[nt * m + i];
+  return 0;
 }
 
 // chain driver on fixed unit normals resident on the device (DESIGN.md §4.7), per maturity: logsv_tangent_step_fixed_kernel -> its P tangent
@@ -2381,6 +2610,35 @@ int b200sv_heston_mc_chain_greeks_gamma(const b200sv_heston_params* params, int 
   return mc_chain_greeks_host(*params, M, ttms, forwards, discfactors, nullptr, offsets, strikes, types, nb_path, nb_steps_per_year, 1,
                               variable_type, seed, flags, prices_out, stderr_out, greeks_out, greeks_se_out, gamma_out, gamma_se_out, n_paths_out,
                               laststep_out);
+}
+
+int b200sv_logsv_mc_chain_greeks_theta(const b200sv_logsv_params* params, int M, const double* ttms, const double* forwards,
+                                       const double* discfactors, const double* etas, const int* offsets, const double* strikes,
+                                       const int8_t* types, long long nb_path, int nb_steps_per_year, int is_spot_measure, int variable_type,
+                                       uint64_t seed, int flags, double* prices_out, double* stderr_out, double* greeks_out,
+                                       double* greeks_se_out, double* gamma_out, double* gamma_se_out, long long n_paths_out,
+                                       double* laststep_out, double* theta_out, double* theta_se_out, double* dtheta_out) {
+  B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && stderr_out && greeks_out && greeks_se_out && theta_out &&
+                     theta_se_out && (!gamma_out || gamma_se_out),
+                 "null pointer");
+  return mc_chain_greeks_host(*params, M, ttms, forwards, discfactors, etas, offsets, strikes, types, nb_path, nb_steps_per_year, is_spot_measure,
+                              variable_type, seed, flags, prices_out, stderr_out, greeks_out, greeks_se_out, gamma_out, gamma_se_out, n_paths_out,
+                              gamma_out ? laststep_out : nullptr, theta_out, theta_se_out, dtheta_out);
+}
+
+int b200sv_heston_mc_chain_greeks_theta(const b200sv_heston_params* params, int M, const double* ttms, const double* forwards,
+                                        const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
+                                        long long nb_path, int nb_steps_per_year, int variable_type, uint64_t seed, int flags, int scheme,
+                                        double* prices_out, double* stderr_out, double* greeks_out, double* greeks_se_out, double* gamma_out,
+                                        double* gamma_se_out, long long n_paths_out, double* laststep_out, double* theta_out,
+                                        double* theta_se_out, double* dtheta_out) {
+  B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && stderr_out && greeks_out && greeks_se_out && theta_out &&
+                     theta_se_out && (!gamma_out || gamma_se_out),
+                 "null pointer");
+  B200SV_REQUIRE(scheme == B200SV_HESTON_EULER_FLOOR, "pathwise sensitivities need scheme = B200SV_HESTON_EULER_FLOOR");
+  return mc_chain_greeks_host(*params, M, ttms, forwards, discfactors, nullptr, offsets, strikes, types, nb_path, nb_steps_per_year, 1,
+                              variable_type, seed, flags, prices_out, stderr_out, greeks_out, greeks_se_out, gamma_out, gamma_se_out, n_paths_out,
+                              gamma_out ? laststep_out : nullptr, theta_out, theta_se_out, dtheta_out);
 }
 
 int b200sv_logsv_tangent_terminal(const b200sv_logsv_params* params, double ttm, long long nb_path, int nb_steps_per_year, int is_spot_measure,
@@ -2757,6 +3015,21 @@ int b200sv_rough_logsv_mc_chain_greeks(const b200sv_logsv_params* params, int n_
   return rough_chain_greeks_host(*params, n_factors, weights, nodes, M, ttms, forwards, discfactors, offsets, strikes, types, nb_path, nsteps, hs, Z0,
                                  Z1, z_rows, variable_type, seed, flags, prices_out, stderr_out, greeks_out, greeks_se_out, states_out, tangents_out,
                                  resets_out);
+}
+
+int b200sv_rough_logsv_mc_chain_greeks_theta(const b200sv_logsv_params* params, int n_factors, const double* weights, const double* nodes, int M,
+                                             const double* ttms, const double* forwards, const double* discfactors, const int* offsets,
+                                             const double* strikes, const int8_t* types, long long nb_path, const int* nsteps, const double* hs,
+                                             const double* Z0, const double* Z1, long long z_rows, int variable_type, uint64_t seed, int flags,
+                                             double* prices_out, double* stderr_out, double* greeks_out, double* greeks_se_out, double* states_out,
+                                             double* tangents_out, double* resets_out, double* theta_out, double* theta_se_out,
+                                             long long n_paths_out, double* dtheta_out) {
+  B200SV_REQUIRE(params && weights && nodes && ttms && forwards && discfactors && offsets && nsteps && hs && prices_out && stderr_out && greeks_out &&
+                     greeks_se_out && theta_out && theta_se_out,
+                 "null pointer");
+  return rough_chain_greeks_host(*params, n_factors, weights, nodes, M, ttms, forwards, discfactors, offsets, strikes, types, nb_path, nsteps, hs, Z0,
+                                 Z1, z_rows, variable_type, seed, flags, prices_out, stderr_out, greeks_out, greeks_se_out, states_out, tangents_out,
+                                 resets_out, theta_out, theta_se_out, n_paths_out, dtheta_out);
 }
 
 // ---- Hawkes jump-diffusion MC (hawkes_kernels.cuh) ---------------------------------------------------------------------------

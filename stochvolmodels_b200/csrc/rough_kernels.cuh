@@ -457,6 +457,191 @@ static int launch_rough_tangent(int n, double* ls, double* vol, double* qv, doub
   });
 }
 
+// --------------------------------------------------------------------------------------------------------------------
+// Monte Carlo theta of the rough chain, DESIGN.md §3.12
+// --------------------------------------------------------------------------------------------------------------------
+// Every maturity restarts at t = 0 on its own grid h = ttm / S, so d/d ttm = (1/S) d/d h over the whole path, from a zero tangent.  The
+// production RoughPath steps the primal; this object is its hook (the diffusion exponent, the reset branch, vw / volw_h / term1 / term2)
+// and then advances dv[N], dls, dy in h.  The two RK4 half-steps (hh = h/2) are differentiated with their explicit hh-dependence: the
+// stage slopes are replayed through RoughPath::slope from the step's start value, and their tangents chained as the parameter rows chain
+// them.  The exponent contributes vv z0 / (2 sqrt h) - vv^2 / 2 (0 where clamp_log clamps), term1 is differentiated in its exact-arithmetic
+// form (1/vartheta) ((volw_h - vw) / W + h rest), term2 and y are proportional to h, and the reset branch has zero factor tangents.
+struct RoughThetaConsts {
+  double dex_a, dex_b;       // d ex_raw / d h = dex_a z0 + dex_b:  vv / (2 sqrt h), -vv^2 / 2
+  double qshift;             // S / ttm: tq = dy - qshift y, the Q_VAR payoff's dU = tq / ttm
+};
+
+template <int N>
+struct RoughThetaPath {
+  static constexpr bool kRedrawPair = true;
+  RoughPath<N> p;
+  double dv[N], dls, dy;
+  double ex_raw, ex, e, vw, vhw, term1, term2;
+  bool was_reset;
+  __device__ __forceinline__ void stage(int, double) {}
+  __device__ __forceinline__ void diffusion(double, double ex_raw_, double ex_, double e_) {
+    ex_raw = ex_raw_;
+    ex = ex_;
+    e = e_;
+  }
+  __device__ __forceinline__ void reset() { was_reset = true; }
+  __device__ __forceinline__ void spot(double vw_, double vhw_, double t1, double t2) {
+    vw = vw_;
+    vhw = vhw_;
+    term1 = t1;
+    term2 = t2;
+  }
+  __device__ __forceinline__ void init(const RoughConsts& c) {
+    p.init(c);
+#pragma unroll
+    for (int i = 0; i < N; ++i) dv[i] = 0.0;
+    dls = 0.0;
+    dy = 0.0;
+  }
+  // tangent of the drift slope at z with the parameters held: ds_i = -x_i dz_i + dg
+  __device__ __forceinline__ static void slope_h(const RoughConsts& c, const double (&z)[N], const double (&dz)[N], double (&ds)[N]) {
+    const double zw = RoughPath<N>::wsum_of(c, z), dzw = RoughPath<N>::wsum_of(c, dz);
+    const double dg = dzw * (c.kappa2 * (c.theta - zw) - fma(c.kappa2, zw, c.kappa1));
+#pragma unroll
+    for (int i = 0; i < N; ++i) ds[i] = fma(-c.nodes[i], dz[i], dg);
+  }
+  // RoughPath::drift over hh = h/2 and its h-tangent (d hh / d h = 1/2): z, dz in, both advanced
+  __device__ __forceinline__ static void drift_h(const RoughConsts& c, double (&z)[N], double (&dz)[N], double hh) {
+    RoughNoHook none;
+    double s[N], ds[N], acc[N], dacc[N], t[N], dt[N];
+    RoughPath<N>::slope(c, z, s, none, 0);
+    slope_h(c, z, dz, ds);
+#pragma unroll
+    for (int i = 0; i < N; ++i) {
+      acc[i] = s[i];
+      dacc[i] = ds[i];
+      t[i] = fma(0.5 * hh, s[i], z[i]);
+      dt[i] = fma(0.5 * hh, ds[i], fma(0.25, s[i], dz[i]));
+    }
+    RoughPath<N>::slope(c, t, s, none, 0);
+    slope_h(c, t, dt, ds);
+#pragma unroll
+    for (int i = 0; i < N; ++i) {
+      acc[i] = fma(2.0, s[i], acc[i]);
+      dacc[i] = fma(2.0, ds[i], dacc[i]);
+      t[i] = fma(0.5 * hh, s[i], z[i]);
+      dt[i] = fma(0.5 * hh, ds[i], fma(0.25, s[i], dz[i]));
+    }
+    RoughPath<N>::slope(c, t, s, none, 0);
+    slope_h(c, t, dt, ds);
+#pragma unroll
+    for (int i = 0; i < N; ++i) {
+      acc[i] = fma(2.0, s[i], acc[i]);
+      dacc[i] = fma(2.0, ds[i], dacc[i]);
+      t[i] = fma(hh, s[i], z[i]);
+      dt[i] = fma(hh, ds[i], fma(0.5, s[i], dz[i]));
+    }
+    RoughPath<N>::slope(c, t, s, none, 0);
+    slope_h(c, t, dt, ds);
+#pragma unroll
+    for (int i = 0; i < N; ++i) {
+      acc[i] += s[i];
+      dacc[i] += ds[i];
+      z[i] = fma(hh / 6.0, acc[i], z[i]);
+      dz[i] = fma(hh / 6.0, dacc[i], fma(1.0 / 12.0, acc[i], dz[i]));
+    }
+  }
+  __device__ __forceinline__ void step(const RoughConsts& c, const RoughThetaConsts& k, double z0, double z1) {
+    double z[N], dz[N];
+    double dvw = 0.0, dwlv = 0.0, wlv = 0.0;
+#pragma unroll
+    for (int i = 0; i < N; ++i) {
+      z[i] = p.v[i];
+      dz[i] = dv[i];
+      dvw = fma(c.weight[i], dz[i], dvw);
+      dwlv = fma(c.wlam[i], dz[i], dwlv);
+      wlv = fma(c.wlam[i], z[i], wlv);
+    }
+    was_reset = false;
+    p.step(c, z0, z1, *this);
+    drift_h(c, z, dz, c.half_h);
+    const double yw = RoughPath<N>::wsum_of(c, z), dyw = RoughPath<N>::wsum_of(c, dz);
+    const double dex = ex != ex_raw ? 0.0 : fma(k.dex_a, z0, k.dex_b);
+    const double Q = c.w_inv * (yw * e - yw), dQ = c.w_inv * (e * fma(yw, dex, dyw) - dyw);
+#pragma unroll
+    for (int i = 0; i < N; ++i) {
+      z[i] += Q;
+      dz[i] += dQ;
+    }
+    drift_h(c, z, dz, c.half_h);
+    double dvhw = 0.0, dwlvh = 0.0, wlvh = 0.0;
+#pragma unroll
+    for (int i = 0; i < N; ++i) {
+      if (was_reset) {
+        z[i] = 1e-6;
+        dz[i] = 0.0;
+      }
+      dvhw = fma(c.weight[i], dz[i], dvhw);
+      dwlvh = fma(c.wlam[i], dz[i], dwlvh);
+      wlvh = fma(c.wlam[i], z[i], wlvh);
+      dv[i] = dz[i];
+    }
+    const double a_mean = 0.5 * vw + 0.5 * vhw, a_sq = 0.5 * vw * vw + 0.5 * vhw * vhw, dsum = fma(vw, dvw, vhw * dvhw);
+    const double rest = (0.5 * wlv + 0.5 * wlvh - c.w_lam_v0) * c.w_inv - c.kappa1 * c.theta + (c.kappa1 - c.kappa2 * c.theta) * a_mean +
+                        c.kappa2 * a_sq;
+    const double drest = (0.5 * dwlv + 0.5 * dwlvh) * c.w_inv + (c.kappa1 - c.kappa2 * c.theta) * (0.5 * dvw + 0.5 * dvhw) + c.kappa2 * dsum;
+    const double dterm1 = c.inv_volvol * ((dvhw - dvw) * c.w_inv + fma(c.h, drest, rest));
+    const double dterm2 = fma(c.h, dsum, a_sq);
+    const double dsq = term2 > 0.0 ? 0.5 * dterm2 / sqrt(term2) : 0.0;
+    dls += fma(c.rho_comp * dsq, z1, fma(-0.5, dterm2, c.rho * dterm1));
+    dy += dterm2;
+  }
+};
+
+// the theta pass of one maturity: the pricing route's grid-stride loop and normals (rough_run_path) with RoughThetaPath; writes dls_out [P]
+// = d ls / d h and dq_out [P] = d y / d h - qshift y, and per-CTA partials [gridDim.x][3]: sum F e^ls, count, sum F e^ls dls
+template <int N>
+struct RoughThetaRunner {
+  static constexpr bool kRedrawPair = RoughThetaPath<N>::kRedrawPair;
+  RoughThetaPath<N> t;
+  const RoughThetaConsts& k;
+  __device__ __forceinline__ explicit RoughThetaRunner(const RoughThetaConsts& k_) : k(k_) {}
+  __device__ __forceinline__ void step(const RoughConsts& c, double z0, double z1) { t.step(c, k, z0, z1); }
+};
+
+template <int N, int GAUSS>
+__global__ void __launch_bounds__(kThreads) rough_logsv_theta_kernel(double* __restrict__ dls_out, double* __restrict__ dq_out,
+                                                                    const double* __restrict__ Z0, const double* __restrict__ Z1, int S, long long P,
+                                                                    RoughConsts c, RoughThetaConsts k, unsigned long long seed, double forward,
+                                                                    double* __restrict__ partials) {
+  exp_table_init();
+  if constexpr (GAUSS != kGaussF32) gauss64_table_init();
+  SpotMoments<3, kThreads> mom;
+  const long long stride = (long long)gridDim.x * kThreads;
+  for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < P; i += stride) {
+    RoughThetaRunner<N> r(k);
+    r.t.init(c);
+    rough_run_path<GAUSS>(r, c, Z0, Z1, S, P, i, seed, 0ull);
+    const double spot = forward * exp(r.t.p.ls);
+    dls_out[i] = r.t.dls;
+    dq_out[i] = fma(-k.qshift, r.t.p.y, r.t.dy);
+    mom.add_term(spot, 0, r.t.dls);
+    mom.add(spot);
+  }
+  mom.store(partials);
+}
+
+static int launch_rough_theta(int n, double* dls, double* dq, const double* Z0, const double* Z1, int S, long long P, const RoughConsts& c,
+                              double ttm, uint64_t seed, int gauss, double forward, double* moments_out, cudaStream_t st) {
+  RoughThetaConsts k;
+  k.dex_a = 0.5 * c.vv / c.sqrt_h;
+  k.dex_b = -0.5 * c.vv * c.vv;
+  k.qshift = (double)S / ttm;
+  return with_factors(n, [&](auto nf) {
+    constexpr int N = decltype(nf)::value;
+    const int blocks = persistent_grid(rough_logsv_theta_kernel<N, kGaussF32>, kThreads, P).blocks;
+    const auto kernel = gauss == kGaussF64 ? rough_logsv_theta_kernel<N, kGaussF64> : rough_logsv_theta_kernel<N, kGaussF32>;
+    return slice_moments("rough_logsv_theta_kernel", 3, blocks, moments_out, st, nullptr, [&](double* partials) {
+      kernel<<<blocks, kThreads, 0, st>>>(dls, dq, Z0, Z1, S, P, c, k, seed, forward, partials);
+    });
+  });
+}
+
 // The argument checks both rough chain drivers make after their own factor-count check, and the caller's normals: the Gauss mode, the longest
 // grid Smax, and Z0 / Z1 [Smax][P] on the device (left null with in-kernel Philox draws).
 struct RoughChainArgs {
@@ -529,8 +714,11 @@ static int rough_chain_greeks_host(const b200sv_logsv_params& p, int n, const do
                                    const double* forwards, const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
                                    long long nb_path, const int* nsteps, const double* hs, const double* Z0, const double* Z1, long long z_rows,
                                    int variable_type, uint64_t seed, int flags, double* prices_out, double* stderr_out, double* greeks_out,
-                                   double* greeks_se_out, double* states_out, double* tangents_out, double* resets_out) {
+                                   double* greeks_se_out, double* states_out, double* tangents_out, double* resets_out, double* theta_out = nullptr,
+                                   double* theta_se_out = nullptr, long long n_paths_out = 0, double* dtheta_out = nullptr) {
   constexpr int NP = kRoughParams;
+  const bool with_theta = theta_out != nullptr;
+  B200SV_REQUIRE(n_paths_out >= 0 && n_paths_out <= nb_path, "n_paths_out must be in [0, nb_path]");
   B200SV_REQUIRE(n >= 1 && n <= kMaxRoughFactors, "1 <= n_factors <= 8");
   cudaStream_t st = current_stream();
   RoughChainArgs a(st);
@@ -538,8 +726,10 @@ static int rough_chain_greeks_host(const b200sv_logsv_params& p, int n, const do
   ensure_pool_threshold();
   StreamSync sync(st);
   const size_t P = (size_t)nb_path;
-  DevBuf d_state(st), d_tan(st), d_dvol(st), d_resets(st);
-  GreeksChainIO<NP> io(M, ttms, forwards, discfactors, offsets, types, variable_type, nb_path, st);
+  const size_t nt = dtheta_out ? (size_t)n_paths_out : 0;
+  DevBuf d_state(st), d_tan(st), d_dvol(st), d_resets(st), d_theta(st);
+  GreeksChainIO<NP> io(M, ttms, forwards, discfactors, offsets, types, variable_type, nb_path, st, false, with_theta);
+  if (with_theta) B200SV_CUDA(d_theta.alloc(sizeof(double) * 2 * P));     // theta pass: dls, dy - S y / ttm
   B200SV_CUDA(d_state.alloc(sizeof(double) * (size_t)(n + 2) * P));
   B200SV_CUDA(d_tan.alloc(sizeof(double) * 2 * NP * P));
   if (tangents_out) B200SV_CUDA(d_dvol.alloc(sizeof(double) * (size_t)NP * n * P));
@@ -549,6 +739,7 @@ static int rough_chain_greeks_host(const b200sv_logsv_params& p, int n, const do
   if (int rc = io.upload(strikes)) return rc;
   double *d_ls = d_state.as<double>(), *d_vol = d_ls + P, *d_qv = d_ls + (size_t)(n + 1) * P;
   double *d_dls = d_tan.as<double>(), *d_dqv = d_dls + NP * P, *d_dv = d_dvol.as<double>();      // d_dv: null without tangents_out
+  std::vector<double> h_q(nt * M);
   for (int m = 0; m < M; ++m) {
     const RoughConsts c = make_rough_consts(p, n, weights, nodes, hs[m]);
     RoughTangentConsts k = make_rough_tangent_consts(p, c);
@@ -568,11 +759,27 @@ static int rough_chain_greeks_host(const b200sv_logsv_params& p, int n, const do
     }
     // the price row keeps the route's un-normalised std (total_paths = 1), the sensitivity rows are standard errors
     if (int rc = io.payoff(m, d_ls, d_qv, d_dls, d_dqv, 1.0)) return rc;
+    if (!with_theta) continue;
+    // the theta pass replays the maturity's path on the same normals; its rows re-centre with the tangent pass's (sum F e^ls, count)
+    double *d_th = d_theta.as<double>(), *d_thq = d_th + P;
+    if (int rc = launch_rough_theta(n, d_th, d_thq, a.z0.as<double>(), a.z1.as<double>(), nsteps[m], nb_path, c, ttms[m], seed, a.gauss, forwards[m],
+                                    io.theta_moments(), st))
+      return rc;
+    B200SV_CUDA(cudaMemcpyAsync(io.theta_moments(), io.moments(), sizeof(double) * 2, cudaMemcpyDeviceToDevice, st));
+    if (int rc = io.payoff_theta(m, d_ls, d_qv, d_th, d_thq, nsteps[m])) return rc;
+    if (nt) {
+      B200SV_CUDA(cudaMemcpy2DAsync(dtheta_out + 2 * nt * m, sizeof(double) * nt, d_th, sizeof(double) * P, sizeof(double) * nt, 2,
+                                    cudaMemcpyDeviceToHost, st));
+      B200SV_CUDA(cudaMemcpyAsync(h_q.data() + nt * m, d_qv, sizeof(double) * nt, cudaMemcpyDeviceToHost, st));
+    }
   }
   std::vector<unsigned long long> h_resets(M);
   B200SV_CUDA(d_resets.download(h_resets.data(), M));
-  if (int rc = io.copy_back(sync, prices_out, stderr_out, greeks_out, greeks_se_out)) return rc;
+  if (int rc = io.copy_back(sync, prices_out, stderr_out, greeks_out, greeks_se_out, nullptr, nullptr, theta_out, theta_se_out)) return rc;
   for (int m = 0; m < M && resets_out; ++m) resets_out[m] = (double)h_resets[m];
+  // the hook reports d y / d h: undo the payoff's shift with the maturity's y
+  for (int m = 0; m < M; ++m)
+    for (size_t i = 0; i < nt; ++i) dtheta_out[(2 * m + 1) * nt + i] += (double)nsteps[m] / ttms[m] * h_q[nt * m + i];
   return 0;
 }
 

@@ -175,6 +175,39 @@ def heston_mc_chain_greeks_gamma(params: C.HestonParamsC, ttms, forwards, discfa
                                   len(HESTON_GREEK_PARAMS), n_paths_out)
 
 
+def _mc_chain_greeks_theta(symbol: str, params, chain, etas, head, variable_type, seed: int, flags: int, tail, n_greeks: int,
+                           with_gamma: bool, n_paths_out: int):
+    M, J, n_out = len(chain[3]), sum(len(s) for s in chain[3]), int(n_paths_out)
+    gamma, gamma_se = (np.empty(J), np.empty(J)) if with_gamma else (None, None)
+    theta, theta_se = np.empty(J), np.empty(J)
+    dtheta = np.empty((M, 2, n_out)) if n_out else None
+    res = _mc_chain(symbol, params, chain, etas, head, variable_type, seed, flags, tail, n_greeks=n_greeks,
+                    post=(C.dptr(gamma), C.dptr(gamma_se), n_out, None, C.dptr(theta), C.dptr(theta_se), C.dptr(dtheta)))
+    return (*res, gamma, gamma_se, theta, theta_se, dtheta)
+
+
+def logsv_mc_chain_greeks_theta(params: C.LogsvParamsC, ttms, forwards, discfactors, etas, strikes_ttms, optiontypes_ttms, nb_path: int,
+                                nb_steps_per_year: int, is_spot_measure: bool, variable_type, seed: int, flags: int, with_gamma: bool = False,
+                                n_paths_out: int = 0):
+    """logsv_mc_chain_greeks (with_gamma: logsv_mc_chain_greeks_gamma) plus the Monte Carlo theta -d price / d ttm per year, pathwise in
+    each slice's step length with its step count held (b200sv_logsv_mc_chain_greeks_theta; DESIGN.md §3.12).  Returns (prices, std errors,
+    greeks [1+6, J], greeks_se [1+6, J], offsets, gamma [J] | None, gamma_se [J] | None, theta [J], theta_se [J], dtheta): the rest
+    bit-identical to the call without theta; with ``n_paths_out`` > 0, dtheta [M, 2, n_paths_out] = (dx, dq) / d dt of the first paths after
+    each maturity, else None."""
+    return _mc_chain_greeks_theta("b200sv_logsv_mc_chain_greeks_theta", params, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms),
+                                  (etas,), (int(nb_path), int(nb_steps_per_year), int(bool(is_spot_measure))), variable_type, seed, flags, (),
+                                  len(LOGSV_GREEK_PARAMS), with_gamma, n_paths_out)
+
+
+def heston_mc_chain_greeks_theta(params: C.HestonParamsC, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, nb_path: int,
+                                 nb_steps_per_year: int, variable_type, seed: int, flags: int, scheme: int = C.HESTON_EULER_FLOOR,
+                                 with_gamma: bool = False, n_paths_out: int = 0):
+    """Heston twin of logsv_mc_chain_greeks_theta (b200sv_heston_mc_chain_greeks_theta)."""
+    return _mc_chain_greeks_theta("b200sv_heston_mc_chain_greeks_theta", params, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms),
+                                  (), (int(nb_path), int(nb_steps_per_year)), variable_type, seed, flags, (int(scheme),),
+                                  len(HESTON_GREEK_PARAMS), with_gamma, n_paths_out)
+
+
 def hawkesjd_mc_chain_greeks(params: C.HawkesParamsC, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, nb_path: int, variable_type,
                              seed: int, flags: int, n_paths_out: int = 0):
     """chain MC of the Hawkes jump-diffusion with Monte Carlo sensitivities (b200sv_hawkesjd_mc_chain_greeks; DESIGN.md §3.11).  Returns
@@ -262,11 +295,14 @@ def _rough_grid_normals(M: int, nb_path: int, nsteps, hs, Z0, Z1):
 
 def rough_logsv_mc_chain_greeks(params: C.LogsvParamsC, weights, nodes, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms,
                                 nb_path: int, nsteps, hs, Z0=None, Z1=None, variable_type=1, seed: int = 0, flags: int = 0,
-                                return_states: bool = False, return_tangents: bool = False):
+                                return_states: bool = False, return_tangents: bool = False, with_theta: bool = False, n_paths_out: int = 0):
     """one parameter set through the rough-LogSV chain MC with pathwise sensitivities (b200sv_rough_logsv_mc_chain_greeks).  Arguments as
     rough_logsv_mc_chain with ``weights`` / ``nodes`` [n].  Returns (prices, std errors, greeks [1+6, J], greeks_se [1+6, J], offsets,
     states [M, n + 2, nb_path] | None, tangents [M, 6, n + 2, nb_path] | None, resets [M]): greeks row 0 the forward delta, then
-    LOGSV_GREEK_PARAMS; resets[m] = the number of paths that took the reset-to-1e-6 branch at any step of maturity m's grid."""
+    LOGSV_GREEK_PARAMS; resets[m] = the number of paths that took the reset-to-1e-6 branch at any step of maturity m's grid.
+    ``with_theta`` (b200sv_rough_logsv_mc_chain_greeks_theta; DESIGN.md §3.12) appends (theta [J], theta_se [J], dtheta): -d price / d ttm
+    per year, pathwise in each maturity's step length with its step count held, the rest bit-identical; with ``n_paths_out`` > 0, dtheta
+    [M, 2, n_paths_out] = (d log_spot, d qv) / d h of the first paths at each maturity, else None."""
     vt = variable_code(variable_type)
     ch = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
     weights, nodes = C.f64(weights), C.f64(nodes)
@@ -279,11 +315,19 @@ def rough_logsv_mc_chain_greeks(params: C.LogsvParamsC, weights, nodes, ttms, fo
     states = np.empty((ch.M, n + 2, int(nb_path))) if return_states else None
     tangents = np.empty((ch.M, P, n + 2, int(nb_path))) if return_tangents else None
     resets = np.empty(ch.M)
-    C.call("b200sv_rough_logsv_mc_chain_greeks", byref(params), n, C.dptr(weights), C.dptr(nodes), *C.chain_ptrs(ch), int(nb_path), C.iptr(nsteps),
-           C.dptr(hs), C.dptr(Z0), C.dptr(Z1), int(z_rows), vt, C.seed64(seed), int(flags), C.dptr(prices), C.dptr(stds), C.dptr(greeks),
-           C.dptr(greeks_se), C.dptr(states), C.dptr(tangents), C.dptr(resets))
-    return (C.split_chain(prices, ch.offsets), C.split_chain(stds, ch.offsets), greeks, greeks_se, ch.offsets, states, tangents,
-            resets.astype(np.int64))
+    args = (byref(params), n, C.dptr(weights), C.dptr(nodes), *C.chain_ptrs(ch), int(nb_path), C.iptr(nsteps), C.dptr(hs), C.dptr(Z0), C.dptr(Z1),
+            int(z_rows), vt, C.seed64(seed), int(flags), C.dptr(prices), C.dptr(stds), C.dptr(greeks), C.dptr(greeks_se), C.dptr(states),
+            C.dptr(tangents), C.dptr(resets))
+    if with_theta:
+        n_out = int(n_paths_out)
+        theta, theta_se = np.empty(J), np.empty(J)
+        dtheta = np.empty((ch.M, 2, n_out)) if n_out else None
+        C.call("b200sv_rough_logsv_mc_chain_greeks_theta", *args, C.dptr(theta), C.dptr(theta_se), n_out, C.dptr(dtheta))
+    else:
+        C.call("b200sv_rough_logsv_mc_chain_greeks", *args)
+    res = (C.split_chain(prices, ch.offsets), C.split_chain(stds, ch.offsets), greeks, greeks_se, ch.offsets, states, tangents,
+           resets.astype(np.int64))
+    return (*res, theta, theta_se, dtheta) if with_theta else res
 
 
 def rough_logsv_mc_chain(params_list, weights, nodes, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, nb_path: int, nsteps, hs,

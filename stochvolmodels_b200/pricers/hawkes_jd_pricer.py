@@ -150,8 +150,11 @@ class HawkesJDPricer(ModelPricer):
         likelihood-ratio score of the decisions (DESIGN.md §3.11): unbiased for the discretised scheme the pricer simulates.  LOG_RETURN,
         fp64 state, ``gauss`` 'fp32' / 'fp64'; Q_VAR, ``exchange``, another ``precision`` or a set ``risk_premia_gamma`` raise
         NotImplementedError, ``mean_p == 0`` or ``mean_m == 0`` (degenerate jump sizes) ValueError.  Under torch.distributed every rank prices all paths (replicated, bit-identical results)."""
-        from .mc_greeks import check_hawkes_mc_greeks_kwargs, check_no_gamma, to_mc_chain_greeks
+        from .mc_greeks import check_hawkes_mc_greeks_kwargs, check_no_gamma, check_no_theta, to_mc_chain_greeks
         check_no_gamma(kwargs, "HawkesJDPricer.model_mc_chain_greeks")
+        check_no_theta(kwargs, "HawkesJDPricer.model_mc_chain_greeks",
+                       "the firing clock's dt enters through the likelihood-ratio score and the dt*(1 +- 1e-9) comparison constants; "
+                       "price_chain_greeks(with_theta=True) has the Fourier theta")
         check_hawkes_mc_greeks_kwargs(kwargs, gauss, params)
         d = params.to_dict()
         d.pop("risk_premia_gamma", None)

@@ -105,10 +105,13 @@ class HestonPricer(ModelPricer):
                                       exchange=kwargs.get("exchange"))
 
     def model_mc_chain_greeks(self, option_chain: OptionChain, params: HestonParams, nb_path: int = 100000,
-                              variable_type: VariableType = VariableType.LOG_RETURN, with_gamma: bool = False, **kwargs):
+                              variable_type: VariableType = VariableType.LOG_RETURN, with_gamma: bool = False, with_theta: bool = False,
+                              **kwargs):
         """MC prices and standard errors as ``model_mc_price_chain`` (same defaults and kwargs, same numbers on the same seed) plus pathwise
         sensitivities in the same pass: the forward delta and d price / d (v0, theta, kappa, rho, volvol), each with its standard error ->
         ``McChainGreeks``.  ``with_gamma=True`` also fills ``gamma`` / ``gamma_se`` (DESIGN.md §3.9) and leaves every other number unchanged.
+        ``with_theta=True`` also fills ``theta`` / ``theta_se`` (-d price / d ttm per year, pathwise in each slice's step length with its
+        step count held, DESIGN.md §3.12), alone or with ``with_gamma``, and leaves every other number unchanged.
         Floor-Euler scheme and fp64 state only; no ``exchange``.  Under torch.distributed every rank prices all paths (replicated,
         bit-identical results)."""
         from .mc_greeks import check_greeks_kwargs, to_mc_chain_greeks
@@ -117,10 +120,13 @@ class HestonPricer(ModelPricer):
             raise NotImplementedError("model_mc_chain_greeks needs scheme='euler_floor'")
         vt = engine.variable_code(variable_type)
         flags = engine.mc_flags("fp64", kwargs.get("gauss", "fp32"))
-        route = engine.heston_mc_chain_greeks_gamma if with_gamma else engine.heston_mc_chain_greeks
-        res = route(_params_c(params.v0, params.theta, params.kappa, params.rho, params.volvol), option_chain.ttms, option_chain.forwards,
-                    option_chain.discfactors, option_chain.strikes_ttms, option_chain.optiontypes_ttms, nb_path,
-                    kwargs.get("nb_steps_per_year", 360), vt, _shared_seed(kwargs.get("seed")), flags)
+        args = (_params_c(params.v0, params.theta, params.kappa, params.rho, params.volvol), option_chain.ttms, option_chain.forwards,
+                option_chain.discfactors, option_chain.strikes_ttms, option_chain.optiontypes_ttms, nb_path,
+                kwargs.get("nb_steps_per_year", 360), vt, _shared_seed(kwargs.get("seed")), flags)
+        if with_theta:
+            res = engine.heston_mc_chain_greeks_theta(*args, with_gamma=with_gamma)
+        else:
+            res = (engine.heston_mc_chain_greeks_gamma if with_gamma else engine.heston_mc_chain_greeks)(*args)
         return to_mc_chain_greeks(res, engine.HESTON_GREEK_PARAMS)
 
     @timer

@@ -270,34 +270,42 @@ class LogSVPricer(ModelPricer):
     @timer
     def model_mc_chain_greeks(self, option_chain: OptionChain, params: LogSvParams, is_spot_measure: bool = True,
                               variable_type: VariableType = VariableType.LOG_RETURN, nb_path: int = 100000,
-                              nb_steps: Optional[int] = None, with_gamma: bool = False, **kwargs):
+                              nb_steps: Optional[int] = None, with_gamma: bool = False, with_theta: bool = False, **kwargs):
         """MC prices and standard errors as ``model_mc_price_chain`` (same defaults, ``seed`` / ``gauss`` kwargs, same numbers on the same
         seed) plus pathwise sensitivities in the same pass: the forward delta and d price / d (sigma0, theta, kappa1, kappa2, beta, volvol),
         each with its standard error -> ``McChainGreeks``.  ``kappa2`` is the value after ``__post_init__`` and is held fixed when kappa1 or
         theta moves; the vol backbone and discount factors are not differentiated.  fp64 state only; no ``exchange``; the rough-vol route has its own ``rough_mc_chain_greeks``.
         ``with_gamma=True`` also fills ``gamma`` / ``gamma_se`` (d^2 price / d forward^2 by conditional smoothing of the last step,
         DESIGN.md §3.9) and leaves every other number unchanged.
+        ``with_theta=True`` also fills ``theta`` / ``theta_se`` (-d price / d ttm per year, pathwise in each slice's step length with the
+        step count, forward, discount factor and vol backbone held, DESIGN.md §3.12), alone or with ``with_gamma``, and leaves every other
+        number unchanged.
         Under torch.distributed every rank prices all paths (replicated, bit-identical results)."""
         from .mc_greeks import check_greeks_kwargs, to_mc_chain_greeks
         check_greeks_kwargs(kwargs)
         vt = engine.variable_code(variable_type)
         flags = engine.mc_flags("fp64", kwargs.get("gauss", "fp32"))
-        route = engine.logsv_mc_chain_greeks_gamma if with_gamma else engine.logsv_mc_chain_greeks
-        res = route(_params_c(params), option_chain.ttms, option_chain.forwards, option_chain.discfactors,
-                    params.get_vol_backbone_etas(ttms=option_chain.ttms), option_chain.strikes_ttms, option_chain.optiontypes_ttms, nb_path,
-                    nb_steps or int(360 * np.max(option_chain.ttms)) + 1, is_spot_measure, vt, _shared_seed(kwargs.get("seed")), flags)
+        args = (_params_c(params), option_chain.ttms, option_chain.forwards, option_chain.discfactors,
+                params.get_vol_backbone_etas(ttms=option_chain.ttms), option_chain.strikes_ttms, option_chain.optiontypes_ttms, nb_path,
+                nb_steps or int(360 * np.max(option_chain.ttms)) + 1, is_spot_measure, vt, _shared_seed(kwargs.get("seed")), flags)
+        if with_theta:
+            res = engine.logsv_mc_chain_greeks_theta(*args, with_gamma=with_gamma)
+        else:
+            res = (engine.logsv_mc_chain_greeks_gamma if with_gamma else engine.logsv_mc_chain_greeks)(*args)
         return to_mc_chain_greeks(res, engine.LOGSV_GREEK_PARAMS)
 
     @timer
     def rough_mc_chain_greeks(self, option_chain: OptionChain, params: LogSvParams, nb_path: int = 100000, nb_steps: Optional[int] = None,
-                              variable_type: VariableType = VariableType.LOG_RETURN, **kwargs):
+                              variable_type: VariableType = VariableType.LOG_RETURN, with_theta: bool = False, **kwargs):
         """pathwise sensitivities of the rough-vol route (DESIGN.md §3.10): prices and "std errors" equal to
         ``model_mc_price_chain(use_rough_mc=True)`` with the same arguments (``seed`` required; ``gauss=None`` the RandomState normals of
         get_randoms_for_rough_vol_chain_valuation, 'fp32' / 'fp64' in-kernel Philox; ``nb_steps`` passed through as given), plus the forward
         delta and d price / d (sigma0, theta, kappa1, kappa2, beta, volvol) with standard errors -> ``McChainGreeks``.  ``volvol`` is the
         orthogonal vol-of-vol, as on the price route; ``params.weights`` / ``params.nodes`` are inputs, not differentiated.  ``reset_paths``
         counts, per maturity, the paths that hit the reset-to-1e-6 branch (their mass across it is not in the rows).  fp64 only, no
-        ``exchange``; under torch.distributed every rank prices all paths (replicated, bit-identical results)."""
+        ``exchange``; under torch.distributed every rank prices all paths (replicated, bit-identical results).
+        ``with_theta=True`` also fills ``theta`` / ``theta_se``: -d price / d ttm per year, pathwise in each maturity's step length with its
+        step count held (every maturity restarts at t = 0 on its own grid, DESIGN.md §3.12); ``reset_paths`` describes the theta row too."""
         from .mc_greeks import check_no_gamma, check_rough_greeks_kwargs, to_mc_chain_greeks
         check_no_gamma(kwargs, "rough_mc_chain_greeks")
         check_rough_greeks_kwargs(kwargs)
@@ -313,9 +321,11 @@ class LogSVPricer(ModelPricer):
                                                                        params.volvol), weights, nodes, option_chain.ttms, option_chain.forwards,
                                                  option_chain.discfactors, option_chain.strikes_ttms, option_chain.optiontypes_ttms, nb_path,
                                                  [g.size - 1 for g in grids], [float(g[1] - g[0]) for g in grids], Z0, Z1, vt, seed,
-                                                 engine.mc_flags("fp64", gauss or "fp32"))
+                                                 engine.mc_flags("fp64", gauss or "fp32"), with_theta=with_theta)
         out = to_mc_chain_greeks(res[:5], engine.LOGSV_GREEK_PARAMS)
         out.reset_paths = res[7]
+        if with_theta:
+            out.theta, out.theta_se = C.split_chain(res[8], res[4]), C.split_chain(res[9], res[4])
         return out
 
     @timer

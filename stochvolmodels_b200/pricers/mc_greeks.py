@@ -26,7 +26,9 @@ class McChainGreeks:
     only, else None): per maturity, the number of paths that took the reset-to-1e-6 branch at any step; the pathwise rows omit the price
     mass such paths move across that switch, so they are unbiased for the scheme only where it is 0.  ``gamma`` / ``gamma_se`` (LogSV and
     Heston with ``with_gamma=True``, else None): one array per maturity of d^2 price / d forward^2 by conditional smoothing of the
-    last step (DESIGN.md §3.9) and its standard error."""
+    last step (DESIGN.md §3.9) and its standard error.  ``theta`` / ``theta_se`` (LogSV and Heston with ``with_theta=True``, else None):
+    one array per maturity of -d price / d ttm per year, pathwise in the slice's step length with its step count held (DESIGN.md §3.12),
+    and its standard error; named as ``FourierChainGreeks.theta``.  ``params["theta"]`` stays d price / d theta."""
     prices: List[np.ndarray]
     std_errors: List[np.ndarray]
     delta: List[np.ndarray]
@@ -36,6 +38,8 @@ class McChainGreeks:
     reset_paths: Optional[np.ndarray] = None
     gamma: Optional[List[np.ndarray]] = None
     gamma_se: Optional[List[np.ndarray]] = None
+    theta: Optional[List[np.ndarray]] = None
+    theta_se: Optional[List[np.ndarray]] = None
 
 
 def check_greeks_kwargs(kwargs, precision_default: str = "fp64") -> None:
@@ -86,14 +90,23 @@ def check_no_gamma(kwargs, method: str) -> None:
         raise NotImplementedError(f"{method} has no Monte Carlo gamma: with_gamma=True covers LogSVPricer and HestonPricer.model_mc_chain_greeks")
 
 
+def check_no_theta(kwargs, method: str, reason: str) -> None:
+    """the routes without a Monte Carlo theta reject ``with_theta=True`` before any GPU work"""
+    if kwargs.get("with_theta"):
+        raise NotImplementedError(f"{method} has no Monte Carlo theta: {reason}")
+
+
 def to_mc_chain_greeks(result, names: Sequence[str]) -> McChainGreeks:
     """engine.*_mc_chain_greeks output -> McChainGreeks; engine.*_mc_chain_greeks_gamma output (gamma and gamma_se after the offsets) fills
-    ``gamma`` / ``gamma_se`` as well"""
+    ``gamma`` / ``gamma_se`` as well; engine.*_mc_chain_greeks_theta output (gamma, gamma_se -- None without gamma --, theta, theta_se, dtheta
+    after the offsets) fills ``theta`` / ``theta_se`` and, where given, ``gamma`` / ``gamma_se``"""
     prices, stds, greeks, greeks_se, offsets = result[:5]
-    split = lambda row: C.split_chain(row, offsets)
+    split = lambda row: None if row is None else C.split_chain(row, offsets)
     out = McChainGreeks(prices=prices, std_errors=stds, delta=split(greeks[0]), delta_se=split(greeks_se[0]),
                         params={n: split(greeks[1 + k]) for k, n in enumerate(names)},
                         params_se={n: split(greeks_se[1 + k]) for k, n in enumerate(names)})
     if len(result) > 5:
         out.gamma, out.gamma_se = split(result[5]), split(result[6])
+    if len(result) > 9:
+        out.theta, out.theta_se = split(result[7]), split(result[8])
     return out
