@@ -530,6 +530,24 @@ int b200sv_heston_price_chain_batch(const b200sv_heston_params* params, int B, i
                                     const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
                                     double vol_scaler, int P, double* prices_out, double* ivols_out);
 
+/* B parameter sets over K chains in one call -- the objectives of K calibrations run in lock-step, one call per optimizer round.  Set b
+ * is priced on chain chain_of_set[b] (0 <= . < K).  The chains are concatenated: chain k has Ms[k] maturities at ttms / forwards /
+ * discfactors [Ms[0] + .. + Ms[k-1]] and its Ms[k] + 1 offsets into strikes / types at offsets [(Ms[0] + 1) + .. + (Ms[k-1] + 1)].  Every
+ * Ms[k] must be >= 1, since it places the chains after k; of a chain that no set points at nothing else is read.  LogSV etas (NULL = 1):
+ * each set's own Ms[chain_of_set[b]] backbone values, set after set.
+ * vol_scalers[K]: the grid of each chain's sets, <= 0 for each set's own default grid.  prices_out / ivols_out (NULL = skip the fused
+ * Black-76 inversion): the rows of the sets one after the other, set b's row holding the J of its own chain.  LOG_RETURN only.
+ * Row b equals, bit for bit, row i of b200sv_*_price_chain_batch called on chain chain_of_set[b] with the sets of this call on that chain,
+ * in call order, b being the i-th of them: whatever else shares the call. */
+int b200sv_logsv_price_chains_batch(const b200sv_logsv_params* params, int B, const int* chain_of_set, int K, const int* Ms,
+                                    const double* ttms, const double* forwards, const double* discfactors, const double* etas,
+                                    const int* offsets, const double* strikes, const int8_t* types, int is_spot_measure, int expansion_order,
+                                    const double* vol_scalers, int P, double* prices_out, double* ivols_out);
+int b200sv_heston_price_chains_batch(const b200sv_heston_params* params, int B, const int* chain_of_set, int K, const int* Ms,
+                                     const double* ttms, const double* forwards, const double* discfactors, const int* offsets,
+                                     const double* strikes, const int8_t* types, const double* vol_scalers, int P, double* prices_out,
+                                     double* ivols_out);
+
 /* same for the Hawkes jump-diffusion: the objectives of HawkesJDPricer.calibrate_model_params_to_chain and
  * calibrate_risk_premia_gamma_to_chain (pricers/hawkes_jd_pricer.py:230-357).  B Hawkes parameter sets on one chain in one pass.
  * gammas: NULL = no risk kernel, else [B] finite risk_premia_gamma per set (all sets on the risk-kernel route: 'C' / 'P' under the spot

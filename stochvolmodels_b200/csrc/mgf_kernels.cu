@@ -18,6 +18,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
+#include <mutex>
 #include <type_traits>
 #include <vector>
 
@@ -3133,6 +3134,197 @@ static int check_expansion_order(int expansion_order) {
   return 0;
 }
 
+// ---- several chains in one call (b200sv_*_price_chains_batch) ----
+// The sets of one chain form a group.  A group is validated by the same FourierChain code as b200sv_*_price_chain_batch on those sets
+// alone and runs on exactly the launch that call would queue for its log-MGF (same kernel, block size and set mapping, all chosen from
+// the group's |S_k| P), so every row equals that call's bit for bit and no warp ever mixes chains.  The groups' log-MGF launches go to
+// streams forked from the call's stream, so that they run side by side; then ONE Fourier-sum launch prices every (set, strike) of the
+// call, each CTA reading its own set's log-MGF rows and grid.
+template <class Params>
+struct ChainsCall {
+  struct Group {
+    int chain = 0, mat0 = 0;          // the chain, and its first entry in ttms / forwards / discfactors
+    std::vector<int> sets;            // the call's sets on this chain, in call order
+    std::vector<Params> params;
+    std::vector<double> etas;         // [sets][M] (LogSV with etas only)
+    FourierChain c;
+    size_t slice0 = 0, grid0 = 0;     // the group's first log-MGF row [.][P] and first grid [.][P] in the call's buffers
+  };
+  std::vector<Group> groups;          // the chains that have sets, in chain order
+  std::vector<StrikeSpec> rows;       // [sum_b J_k(b)]: set b's strikes in call order (slice / grid index the call's buffers)
+  size_t slices = 0, grids = 0;
+
+  // Ms[K]; chain k's maturities at ttms / forwards / discfactors [sum Ms[:k]], its Ms[k] + 1 offsets into strikes / types at
+  // offsets [sum (Ms[:k] + 1)]; etas (may be NULL) [sum_b Ms[chain_of_set[b]]].  Every Ms[k] must be >= 1 (it places the chains
+  // after k); of a chain that no set points at nothing else is read.
+  int prepare(const Params* params, int B, const int* chain_of_set, int K, const int* Ms, const double* ttms, const double* forwards,
+              const double* discfactors, const double* etas, const int* offsets, const double* strikes, const int8_t* types, bool spot,
+              const double* vol_scalers, int P) {
+    B200SV_REQUIRE(params && chain_of_set && Ms && ttms && forwards && discfactors && offsets && strikes && types && vol_scalers,
+                   "null pointer");
+    B200SV_REQUIRE(B >= 1 && K >= 1, "B >= 1, K >= 1");
+    std::vector<int> mat0(K), off0(K), group_of(K, -1);
+    for (int k = 0, m = 0; k < K; m += Ms[k], ++k) {
+      B200SV_REQUIRE(Ms[k] >= 1, "every chain needs M >= 1");
+      mat0[k] = m;
+      off0[k] = m + k;
+    }
+    for (int b = 0; b < B; ++b) B200SV_REQUIRE(chain_of_set[b] >= 0 && chain_of_set[b] < K, "chain_of_set out of range");
+    std::vector<size_t> eta0(B);
+    for (int b = 0, e = 0; b < B; e += Ms[chain_of_set[b]], ++b) eta0[b] = e;
+    for (int k = 0; k < K; ++k)
+      for (int b = 0; b < B; ++b) {
+        if (chain_of_set[b] != k) continue;
+        if (group_of[k] < 0) {
+          group_of[k] = (int)groups.size();
+          groups.emplace_back();
+          groups.back().chain = k;
+          groups.back().mat0 = mat0[k];
+        }
+        Group& g = groups[group_of[k]];
+        g.sets.push_back(b);
+        g.params.push_back(params[b]);
+        if (etas) g.etas.insert(g.etas.end(), etas + eta0[b], etas + eta0[b] + Ms[k]);
+      }
+    for (Group& g : groups) {
+      const int k = g.chain, m0 = g.mat0, *off = offsets + off0[k];
+      if (int rc = g.c.init(true, (int)g.sets.size(), Ms[k], P > 0 ? P : 1000, off)) return rc;
+      if (int rc = g.c.build(g.params.data(), ttms + m0, forwards + m0, discfactors + m0, off, strikes, types, spot, ChainTypes::kFourier,
+                             vol_scalers[k]))
+        return rc;
+      g.slice0 = slices;
+      g.grid0 = grids;
+      slices += (size_t)g.c.B * g.c.M;
+      grids += g.c.phi.size() / (2 * (size_t)g.c.P);
+    }
+    std::vector<int> index(B);                // position of each set within its group
+    for (const Group& g : groups)
+      for (size_t i = 0; i < g.sets.size(); ++i) index[g.sets[i]] = (int)i;
+    for (int b = 0; b < B; ++b) {
+      const Group& g = groups[group_of[chain_of_set[b]]];
+      for (int j = 0; j < g.c.Jtot; ++j) {
+        StrikeSpec s = g.c.ss[(size_t)index[b] * g.c.Jtot + j];
+        s.slice += (int)g.slice0;
+        s.grid += (int)g.grid0;
+        rows.push_back(s);
+      }
+    }
+    return 0;
+  }
+
+  int P() const { return groups[0].c.P; }
+  std::vector<double> phi() const {
+    std::vector<double> all;
+    for (const Group& g : groups) all.insert(all.end(), g.c.phi.begin(), g.c.phi.end());
+    return all;
+  }
+};
+
+// Streams forked from `st` and joined back into it: n = 1 is `st` itself, more are taken from a process-wide pool per device, created on
+// first use and kept (creating them cost more than a small call's launches).  The destructor joins (if join() did not), so that the call's
+// stream-ordered frees and its closing synchronisation come after every forked launch.  Two calls that share a pooled stream only wait
+// for each other.
+class ForkedStreams {
+ public:
+  ForkedStreams(cudaStream_t st, int n) : st_(st) {
+    if (n <= 1) {
+      s_.push_back(st);
+      return;
+    }
+    if ((err_ = pooled(n, s_)) != cudaSuccess) return;
+    cudaEvent_t e;
+    if ((err_ = cudaEventCreateWithFlags(&e, cudaEventDisableTiming)) != cudaSuccess) return;
+    ev_.push_back(e);
+    if ((err_ = cudaEventRecord(e, st)) != cudaSuccess) return;
+    for (cudaStream_t s : s_)
+      if ((err_ = cudaStreamWaitEvent(s, e, 0)) != cudaSuccess) return;
+    forked_ = true;
+  }
+  ForkedStreams(const ForkedStreams&) = delete;
+  ForkedStreams& operator=(const ForkedStreams&) = delete;
+  cudaError_t error() const { return err_; }
+  cudaStream_t operator[](size_t i) const { return s_[i % s_.size()]; }
+  cudaError_t join() {
+    if (!forked_) return err_;
+    forked_ = false;
+    for (cudaStream_t s : s_) {
+      cudaEvent_t e;
+      cudaError_t rc = cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
+      if (rc == cudaSuccess) {
+        ev_.push_back(e);
+        rc = cudaEventRecord(e, s);
+      }
+      if (rc == cudaSuccess) rc = cudaStreamWaitEvent(st_, e, 0);
+      if (rc != cudaSuccess) {
+        cudaStreamSynchronize(s);          // st_ could not be ordered after s: wait for it here
+        if (err_ == cudaSuccess) err_ = rc;
+      }
+    }
+    return err_;
+  }
+  ~ForkedStreams() {
+    join();
+    for (cudaEvent_t e : ev_) cudaEventDestroy(e);      // released once the waits on them are done
+  }
+
+ private:
+  static cudaError_t pooled(int n, std::vector<cudaStream_t>& out) {
+    static std::mutex mu;
+    static std::vector<std::vector<cudaStream_t>> pool;   // [device]
+    int dev = 0;
+    if (cudaError_t e = cudaGetDevice(&dev)) return e;
+    std::lock_guard<std::mutex> lock(mu);
+    if ((int)pool.size() <= dev) pool.resize(dev + 1);
+    std::vector<cudaStream_t>& p = pool[dev];
+    while ((int)p.size() < n) {
+      cudaStream_t s;
+      if (cudaError_t e = cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking)) return e;
+      p.push_back(s);
+    }
+    out.assign(p.begin(), p.begin() + n);
+    return cudaSuccess;
+  }
+
+  cudaStream_t st_;
+  std::vector<cudaStream_t> s_;
+  std::vector<cudaEvent_t> ev_;
+  cudaError_t err_ = cudaSuccess;
+  bool forked_ = false;
+};
+
+constexpr int kChainsStreams = 16;   // concurrent log-MGF launches of a multi-chain call (H100 runs up to 128 kernels at once)
+
+// The device side of a prepared multi-chain call on host.st: grids and strike rows up, `per_group(g, stream, phi, lm)` queues group g's
+// log-MGF launch on a forked stream (reading its grids at phi, writing its [B_k][M_k][P] rows at lm), then the one Fourier-sum launch and
+// the copies back.
+template <class Params, class PerGroup>
+static int run_chains(HostCall& host, const ChainsCall<Params>& call, int is_spot, double* prices_out, double* ivols_out, PerGroup per_group) {
+  const cudaStream_t st = host.st;
+  const int P = call.P();
+  const size_t nq = call.rows.size();
+  const std::vector<double> phi = call.phi();
+  DevBuf d_phi(st), d_rows(st), d_lm(st), d_pr(st), d_iv(st);
+  B200SV_CUDA(d_phi.upload(cplx(phi.data()), phi.size() / 2));
+  B200SV_CUDA(d_rows.upload(call.rows.data(), nq));
+  B200SV_CUDA(d_lm.alloc(sizeof(cd) * call.slices * P));
+  B200SV_CUDA(d_pr.alloc(sizeof(double) * nq));
+  if (ivols_out) B200SV_CUDA(d_iv.alloc(sizeof(double) * nq));
+  {
+    ForkedStreams fork(st, (int)std::min<size_t>(call.groups.size(), kChainsStreams));
+    B200SV_CUDA(fork.error());
+    for (size_t g = 0; g < call.groups.size(); ++g)
+      if (int rc = per_group(call.groups[g], fork[g], d_phi.as<cd>() + call.groups[g].grid0 * P, d_lm.as<cd>() + call.groups[g].slice0 * P))
+        return rc;
+    B200SV_CUDA(fork.join());
+  }
+  fourier_vanilla_kernel<<<(unsigned)nq, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_phi.as<cd>(), P, d_rows.as<StrikeSpec>(), is_spot, 1,
+                                                                    d_pr.as<double>(), d_iv.as<double>());
+  if (int rc = check_launch("fourier sum kernel")) return rc;
+  B200SV_CUDA(d_pr.download(prices_out, nq));
+  B200SV_CUDA(d_iv.download(ivols_out, nq));
+  return host.sync.done();
+}
+
 }  // namespace b200sv
 
 using namespace b200sv;
@@ -3289,6 +3481,80 @@ int b200sv_heston_price_chain_batch(const b200sv_heston_params* params, int B, i
   ChainDev d;
   if (int rc = queue_heston_prices(d, c, params, prices_out, ivols_out)) return rc;
   return d.sync.done();
+}
+
+/* ---- batched chain pricers over several chains: B parameter sets, set b on chain chain_of_set[b], in one call ---- */
+int b200sv_logsv_price_chains_batch(const b200sv_logsv_params* params, int B, const int* chain_of_set, int K, const int* Ms,
+                                    const double* ttms, const double* forwards, const double* discfactors, const double* etas,
+                                    const int* offsets, const double* strikes, const int8_t* types, int is_spot_measure, int expansion_order,
+                                    const double* vol_scalers, int P, double* prices_out, double* ivols_out) {
+  B200SV_REQUIRE(prices_out, "null pointer");
+  if (expansion_order != B200SV_ORDER_FIRST && expansion_order != B200SV_ORDER_SECOND) return fail(-4, "expansion_order not implemented");
+  const int N = expansion_order == B200SV_ORDER_FIRST ? 3 : 5;
+  ChainsCall<b200sv_logsv_params> call;
+  if (int rc = call.prepare(params, B, chain_of_set, K, Ms, ttms, forwards, discfactors, etas, offsets, strikes, types, is_spot_measure != 0,
+                            vol_scalers, P))
+    return rc;
+  // per-group model inputs as queue_logsv_prices builds them: spec [B_k][M_k], yb [B_k]
+  std::vector<ChainSpec> spec;
+  std::vector<double> yb;
+  std::vector<size_t> spec0, a0;
+  size_t na = 0;
+  for (const auto& g : call.groups) {
+    spec0.push_back(spec.size());
+    a0.push_back(na);
+    na += (size_t)g.c.B * g.c.M * g.c.P * N;
+    for (int b = 0; b < g.c.B; ++b) {
+      yb.push_back(g.params[b].sigma0 - g.params[b].theta);
+      for (int m = 0; m < g.c.M; ++m)
+        spec.push_back(ChainSpec{g.c.dtaus[m], make_model(g.params[b], g.etas.empty() ? 1.0 : g.etas[(size_t)b * g.c.M + m], g.c.spot)});
+    }
+  }
+  HostCall host;
+  DevBuf d_spec(host.st), d_y(host.st), d_a(host.st);
+  B200SV_CUDA(d_spec.upload(spec.data(), spec.size()));
+  B200SV_CUDA(d_y.upload(yb.data(), yb.size()));
+  B200SV_CUDA(d_a.alloc(sizeof(cd) * na));
+  size_t gi = 0, y0 = 0;
+  return run_chains(host, call, is_spot_measure != 0 ? 1 : 0, prices_out, ivols_out, [&](const auto& g, cudaStream_t s, const cd* phi, cd* lm) {
+    launch_logsv_mgf(N, s, phi, nullptr, g.c.P, g.c.M, d_spec.as<ChainSpec>() + spec0[gi], nullptr, d_a.as<cd>() + a0[gi], lm, 0.0, g.c.B,
+                     d_y.as<double>() + y0, g.c.per_set_grid ? g.c.P : 0);
+    ++gi;
+    y0 += g.c.B;
+    return check_launch("logsv_mgf_kernel");
+  });
+}
+
+int b200sv_heston_price_chains_batch(const b200sv_heston_params* params, int B, const int* chain_of_set, int K, const int* Ms,
+                                     const double* ttms, const double* forwards, const double* discfactors, const int* offsets,
+                                     const double* strikes, const int8_t* types, const double* vol_scalers, int P, double* prices_out,
+                                     double* ivols_out) {
+  B200SV_REQUIRE(prices_out, "null pointer");
+  ChainsCall<b200sv_heston_params> call;
+  if (int rc = call.prepare(params, B, chain_of_set, K, Ms, ttms, forwards, discfactors, nullptr, offsets, strikes, types, true, vol_scalers, P))
+    return rc;
+  std::vector<double> dt;
+  std::vector<b200sv_heston_params> hp;
+  std::vector<size_t> dt0, hp0;
+  for (const auto& g : call.groups) {
+    dt0.push_back(dt.size());
+    hp0.push_back(hp.size());
+    dt.insert(dt.end(), g.c.dtaus.begin(), g.c.dtaus.end());
+    hp.insert(hp.end(), g.params.begin(), g.params.end());
+  }
+  HostCall host;
+  DevBuf d_dt(host.st), d_hp(host.st);
+  B200SV_CUDA(d_dt.upload(dt.data(), dt.size()));
+  B200SV_CUDA(d_hp.upload(hp.data(), hp.size()));
+  size_t gi = 0;
+  return run_chains(host, call, 1, prices_out, ivols_out, [&](const auto& g, cudaStream_t s, const cd* phi, cd* lm) {
+    // queue_heston_prices' batch launch: 64 threads, blockIdx.y = set
+    heston_mgf_kernel<<<dim3((g.c.P + 63) / 64, g.c.B), 64, 0, s>>>(phi, nullptr, g.c.P, g.c.M, d_dt.as<double>() + dt0[gi], g.params[0], nullptr,
+                                                                    nullptr, nullptr, nullptr, lm, d_hp.as<b200sv_heston_params>() + hp0[gi],
+                                                                    g.c.per_set_grid ? g.c.P : 0);
+    ++gi;
+    return check_launch("heston_mgf_kernel");
+  });
 }
 
 /* Hawkes jump-diffusion Fourier chain (hawkesjd_chain_pricer / hawkesjd_chain_pricer_with_risk_premia, hawkes_jd_pricer.py:365-515).

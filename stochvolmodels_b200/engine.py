@@ -731,6 +731,70 @@ def heston_price_chain_batch(params_list: Sequence[C.HestonParamsC], ttms, forwa
                         optiontypes_ttms), (), (C.vol_scaler_arg(vol_scaler), int(max_phi)), 1, with_ivols)
 
 
+def _chains_batch(symbol: str, struct, params_list, chain_of_set, chains, etas, vol_scalers, is_spot_measure: bool, head, tail,
+                  with_ivols: bool):
+    """the multi-chain batched entry points: C arguments (params [B], B, chain_of_set [B], K, Ms [K], concatenated ttms / forwards /
+    discfactors, [etas,] per-chain offsets, strikes, types, *head, vol_scalers [K], *tail, prices, ivols | NULL) -> (prices, ivols | None),
+    each a list of B rows, row b of length J of chain chain_of_set[b].  ``etas`` = (LogSV per-set backbones or None,) or ()."""
+    B, K = len(params_list), len(chains)
+    if B < 1 or K < 1:
+        raise ValueError("need at least one parameter set and one chain")
+    cos = np.asarray(chain_of_set)
+    if cos.shape != (B,) or (B and cos.dtype.kind not in "iu"):
+        raise ValueError(f"chain_of_set must hold {B} chain indices")
+    if cos.min() < 0 or cos.max() >= K:
+        raise ValueError(f"chain_of_set must lie in [0, {K})")
+    cos = np.ascontiguousarray(cos, dtype=np.int32)
+    if vol_scalers is None:
+        vol_scalers = [None] * K
+    if len(vol_scalers) != K:
+        raise ValueError(f"vol_scalers must hold one value per chain ({K})")
+    scalers = C.f64([C.vol_scaler_arg(v) for v in vol_scalers])
+    chs = [_chain_arrays(*c) for c in chains]
+    types = np.ascontiguousarray(np.concatenate([c.types for c in chs]), dtype=np.int8)
+    if is_spot_measure and (types >= C.INV_CALL).any():
+        raise ValueError("not implemented")       # _check_fourier_types on the encoded types (unknown codes raised in _chain_arrays)
+    flat_etas = []
+    for e in etas:
+        if e is not None:
+            if len(e) != B:
+                raise ValueError(f"etas must hold one backbone per set ({B})")
+            e = [C.f64(x) for x in e]
+            if any(x.shape != (chs[k].M,) for x, k in zip(e, cos)):
+                raise ValueError("etas[b] must hold one value per maturity of set b's chain")
+            e = C.f64(np.concatenate(e))
+        flat_etas.append(e)
+    Ms = np.array([c.M for c in chs], dtype=np.int32)
+    starts = np.cumsum([0] + [c.strikes.shape[0] for c in chs])
+    offsets = np.ascontiguousarray(np.concatenate([c.offsets + s for c, s in zip(chs, starts)]), dtype=np.int32)
+    cat = [C.f64(np.concatenate([getattr(c, f) for c in chs])) for f in ("ttms", "forwards", "discfactors", "strikes")]
+    J = np.array([chs[k].strikes.shape[0] for k in cos])
+    prices = np.empty(int(J.sum()))
+    ivols = np.empty_like(prices) if with_ivols else None
+    C.call(symbol, (struct * B)(*params_list), B, C.iptr(cos), K, C.iptr(Ms), *map(C.dptr, cat[:3]), *map(C.dptr, flat_etas),
+           C.iptr(offsets), C.dptr(cat[3]), C.i8ptr(types), *head, C.dptr(scalers), *tail, C.dptr(prices), C.dptr(ivols))
+    ends = np.cumsum(J).tolist()
+    spans = list(zip([0] + ends[:-1], ends))
+    return [prices[a:b] for a, b in spans], ([ivols[a:b] for a, b in spans] if with_ivols else None)
+
+
+def logsv_price_chains_batch(params_list: Sequence[C.LogsvParamsC], chain_of_set, chains, etas=None, vol_scalers=None,
+                             is_spot_measure: bool = True, expansion_order: int = C.ORDER_SECOND, max_phi: int = 1000, with_ivols: bool = True):
+    """B parameter sets over K chains in one pass -> (prices, ivols | None), each a list of B rows in chain order.  ``chains[k]`` =
+    (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms); set b is priced on chains[chain_of_set[b]].  ``etas``: None or one vol
+    backbone per set over its own chain's maturities; ``vol_scalers``: None or one per chain (None / <= 0: each set's default grid).  Row b
+    is bit for bit row b of logsv_price_chain_batch on its chain with the sets of this call on that chain, in order."""
+    return _chains_batch("b200sv_logsv_price_chains_batch", C.LogsvParamsC, params_list, chain_of_set, chains, (etas,), vol_scalers,
+                         is_spot_measure, (int(bool(is_spot_measure)), int(expansion_order)), (int(max_phi),), with_ivols)
+
+
+def heston_price_chains_batch(params_list: Sequence[C.HestonParamsC], chain_of_set, chains, vol_scalers=None, max_phi: int = 1000,
+                              with_ivols: bool = True):
+    """B Heston parameter sets over K chains in one pass -> (prices, ivols | None); arguments as logsv_price_chains_batch."""
+    return _chains_batch("b200sv_heston_price_chains_batch", C.HestonParamsC, params_list, chain_of_set, chains, (), vol_scalers, True, (),
+                         (int(max_phi),), with_ivols)
+
+
 def hawkesjd_price_chain_batch(params_list: Sequence[C.HawkesParamsC], ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms,
                                is_spot_measure: bool = True, vol_scaler: Optional[float] = None, max_phi: int = 500, gammas=None,
                                with_ivols: bool = True):

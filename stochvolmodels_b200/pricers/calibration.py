@@ -30,6 +30,7 @@ counts the skipped quotes per evaluation in ``nan_quotes`` so that a caller can 
 """
 from __future__ import annotations
 
+import threading
 from dataclasses import dataclass
 from enum import Enum
 from typing import Callable, List, Optional, Sequence, Tuple
@@ -397,7 +398,9 @@ def calibrate_logsv(pricer, option_chain, params0, params_min, params_max, is_ve
                     model_calibration_type: LogsvModelCalibrationType, constraints_type: ConstraintsType,
                     calibration_engine: CalibrationEngine, nb_path: int, nb_steps: int, seed: int, is_spot_measure: bool = True,
                     disp: bool = False, return_info: bool = False, fd_step: Optional[float] = None, mc_randoms: str = "numpy",
-                    gradient: str = "difference"):
+                    gradient: str = "difference", price_batch: Optional[Callable] = None):
+    """``price_batch``: what the ANALYTIC difference objective prices its points with, engine.logsv_price_chain_batch (None) or a
+    callable with its arguments and return value (the lock-step drivers of calibrate_chains_lockstep)"""
     if check_gradient(gradient, pathwise=True) == "exact":
         if calibration_engine != CalibrationEngine.ANALYTIC:
             raise NotImplementedError(f"gradient='exact' covers CalibrationEngine.ANALYTIC only, not {calibration_engine} "
@@ -444,9 +447,10 @@ def calibrate_logsv(pricer, option_chain, params0, params_min, params_max, is_ve
         def batch_vols(points: np.ndarray) -> np.ndarray:
             sets = [codec.parse(p) for p in points]
             etas = np.array([s.get_vol_backbone_etas(ttms=ttms) for s in sets], dtype=float)
-            _, ivols = engine.logsv_price_chain_batch([_params_c(s) for s in sets], ttms, option_chain.forwards, option_chain.discfactors,
-                                                      etas, option_chain.strikes_ttms, option_chain.optiontypes_ttms,
-                                                      is_spot_measure=is_spot_measure, vol_scaler=vol_scaler)
+            _, ivols = (price_batch or engine.logsv_price_chain_batch)([_params_c(s) for s in sets], ttms, option_chain.forwards,
+                                                                       option_chain.discfactors, etas, option_chain.strikes_ttms,
+                                                                       option_chain.optiontypes_ttms, is_spot_measure=is_spot_measure,
+                                                                       vol_scaler=vol_scaler)
             return ivols
     elif calibration_engine == CalibrationEngine.MC and mc_randoms == "philox":
         flags = engine.mc_flags("fp64", "fp32")
@@ -549,7 +553,9 @@ def heston_default_vol_scaler(v0: float, ttm0: float) -> float:
 
 
 def calibrate_heston(pricer, option_chain, params0, is_vega_weighted: bool, is_unit_ttm_vega: bool, disp: bool = False,
-                     return_info: bool = False, fd_step: Optional[float] = None, gradient: str = "difference"):
+                     return_info: bool = False, fd_step: Optional[float] = None, gradient: str = "difference",
+                     price_batch: Optional[Callable] = None):
+    """``price_batch``: engine.heston_price_chain_batch (None) or a callable with its arguments and return value, as for calibrate_logsv"""
     from .heston_pricer import HestonParams, _params_c
     check_gradient(gradient)
     p0 = (np.array([params0.v0, params0.theta, params0.kappa, params0.rho, params0.volvol], dtype=float) if params0 is not None
@@ -571,8 +577,8 @@ def calibrate_heston(pricer, option_chain, params0, is_vega_weighted: bool, is_u
 
     def batch_vols(points: np.ndarray) -> np.ndarray:
         sets = [_params_c(*p) for p in points]
-        _, ivols = engine.heston_price_chain_batch(sets, option_chain.ttms, option_chain.forwards, option_chain.discfactors,
-                                                   option_chain.strikes_ttms, option_chain.optiontypes_ttms)
+        _, ivols = (price_batch or engine.heston_price_chain_batch)(sets, option_chain.ttms, option_chain.forwards, option_chain.discfactors,
+                                                                    option_chain.strikes_ttms, option_chain.optiontypes_ttms)
         return ivols
 
     def feller(pars):                     # 2 kappa theta - volvol^2 >= 0 (heston_pricer.py:152-160)
@@ -586,3 +592,230 @@ def calibrate_heston(pricer, option_chain, params0, is_vega_weighted: bool, is_u
     if return_info:
         return fit, {"fun": float(result.fun), "nit": int(result.nit), "nb_batches": objective.nb_batches, "x": x}
     return fit
+
+
+# ---- several chains in lock-step ------------------------------------------------------------------------------------------------
+class _LockStep:
+    """rendezvous of K fits run in threads and the caller's thread, which prices their points: a fit's ``post(k, request)`` blocks until
+    the round it belongs to has been priced.  A round closes once every live fit has posted or left, so each round holds one request per
+    live fit and the rounds of a run are max_k nb_batches_k.  Only the caller's thread waits on the condition and each fit on an event
+    of its own, so a round wakes each thread once."""
+
+    def __init__(self, n: int):
+        self._cv = threading.Condition()
+        self._live = n
+        self._posted = {}
+        self._answers = {}
+        self._ready = [threading.Event() for _ in range(n)]
+        self._closed: Optional[BaseException] = None
+
+    def post(self, k: int, request):
+        with self._cv:
+            if self._closed is not None:
+                raise self._closed
+            self._posted[k] = request
+            if len(self._posted) == self._live:
+                self._cv.notify()
+        self._ready[k].wait()
+        self._ready[k].clear()
+        answer = self._answers.pop(k)
+        if isinstance(answer, BaseException):
+            raise answer
+        return answer
+
+    def leave(self) -> None:
+        with self._cv:
+            self._live -= 1
+            if len(self._posted) == self._live:
+                self._cv.notify()
+
+    def _answer(self, pending: dict, answers: dict) -> None:
+        """hand answers[k] to every fit k of ``pending``; a fit leaves ``pending`` once woken, so after an interrupt part-way through,
+        ``pending`` holds exactly the fits still waiting"""
+        for k in list(pending):
+            self._answers[k] = answers[k]
+            self._ready[k].set()
+            del pending[k]
+
+    def serve(self, price_round: Callable[[dict], Tuple[dict, int]]) -> int:
+        """price rounds until every fit has left -> the number of library calls.  ``price_round({k: request}) -> ({k: rows}, calls)``;
+        an exception it raises is the answer of every fit of that round.  A BaseException that is not an Exception (KeyboardInterrupt,
+        SystemExit) raised anywhere in here -- inside ``price_round`` too -- is handed to every fit still waiting, the round in flight
+        included, closes the rendezvous to later posts and is re-raised, so that every fit thread ends."""
+        calls = 0
+        in_flight: dict = {}
+        try:
+            while True:
+                with self._cv:
+                    self._cv.wait_for(lambda: len(self._posted) == self._live)
+                    if self._live == 0:
+                        return calls
+                    in_flight, self._posted = self._posted, {}
+                try:
+                    answers, n = price_round(in_flight)
+                    calls += n
+                except Exception as exc:              # noqa: BLE001 (handed to the fits of the round)
+                    answers = {k: exc for k in in_flight}
+                self._answer(in_flight, answers)
+        except BaseException as exc:                  # no fit may wait for a round that never comes
+            with self._cv:
+                self._closed = exc
+                pending = {**in_flight, **self._posted}
+                self._posted = {}
+            self._answer(pending, {k: exc for k in pending})
+            raise
+
+
+def _pack(posted: dict, max_sets_per_call: Optional[int]) -> List[List[int]]:
+    """the fits of a round split into library calls of at most ``max_sets_per_call`` sets, in chain order; a fit's sets are never split (its
+    rows must come from one group of one call to equal the single-chain call's)"""
+    calls, sets = [], 0
+    for k in sorted(posted):
+        n = len(posted[k][0])
+        if not calls or (max_sets_per_call is not None and sets + n > max_sets_per_call):
+            calls.append([])
+            sets = 0
+        calls[-1].append(k)
+        sets += n
+    return calls
+
+
+def calibrate_chains_lockstep(fit: Callable[[int, Callable], object], n: int, price_call: Callable, max_sets_per_call: Optional[int],
+                              return_exceptions: bool):
+    """K = n single-chain fits in lock-step.  ``fit(k, price_batch)`` runs fit k (calibrate_logsv / calibrate_heston with ``price_batch``
+    injected and ``return_info=True``) and returns its (fit, info); ``price_call(requests) -> [ivols [B_i, J_i]]`` prices the requests
+    (price_batch's positional arguments, keyword arguments) of several fits in one library call.  Each fit runs in a thread of its own; the caller's thread, whose
+    CUDA stream the library calls keep (b200sv_set_stream is per thread), prices every round and waits for all threads before it returns.
+    -> (fits, infos), ``rounds`` (library calls of the whole run) added to every info dict; a failed fit's slot holds its exception (info
+    None) with ``return_exceptions``, else the lowest-index exception is raised."""
+    lock = _LockStep(n)
+    results = [None] * n
+
+    def run(k: int) -> None:
+        try:
+            results[k] = fit(k, lambda *args, **kw: (None, lock.post(k, (args[0], args, kw))))
+        except BaseException as exc:                  # noqa: BLE001 (reported per chain below)
+            results[k] = exc
+        finally:
+            lock.leave()
+
+    def price_round(posted: dict):
+        answers = {}
+        calls = _pack(posted, max_sets_per_call)
+        for ks in calls:
+            for k, rows in zip(ks, price_call([posted[k][1:] for k in ks])):
+                answers[k] = rows
+        return answers, len(calls)
+
+    threads = [threading.Thread(target=run, args=(k,), name=f"calibrate-chain-{k}") for k in range(n)]
+    for t in threads:
+        t.start()
+    try:
+        rounds = lock.serve(price_round)
+    finally:
+        for t in threads:
+            t.join()
+    if not return_exceptions:
+        for r in results:
+            if isinstance(r, BaseException):
+                raise r
+    fits, infos = [], []
+    for r in results:
+        if isinstance(r, BaseException):
+            fits.append(r)
+            infos.append(None)
+        else:
+            fits.append(r[0])
+            infos.append(dict(r[1], rounds=rounds))
+    return fits, infos
+
+
+def per_chain(value, n: int, name: str) -> list:
+    """one value for every chain, or a list / tuple of exactly one per chain"""
+    if isinstance(value, (list, tuple)):
+        if len(value) != n:
+            raise ValueError(f"{name} must be one value or one per chain ({n}), not {len(value)}")
+        return list(value)
+    return [value] * n
+
+
+def check_lockstep_args(option_chains, max_sets_per_call, gradient: str) -> int:
+    """the checks every lock-step driver makes before any library call -> the number of chains"""
+    if gradient != "difference":
+        if gradient in GRADIENTS:
+            raise NotImplementedError(f"calibrate_model_params_to_chains has gradient='difference' only, not {gradient!r}")
+        check_gradient(gradient)
+    n = len(option_chains)
+    if n == 0:
+        raise ValueError("option_chains is empty")
+    if max_sets_per_call is not None and int(max_sets_per_call) < 1:
+        raise ValueError("max_sets_per_call must be at least 1")
+    return n
+
+
+def calibrate_logsv_chains(pricer, option_chains, params0, params_min, params_max, is_vega_weighted: bool, is_unit_ttm_vega: bool,
+                           model_calibration_type: LogsvModelCalibrationType, constraints_type: ConstraintsType,
+                           calibration_engine: CalibrationEngine, is_spot_measure: bool = True, disp: bool = False, return_info: bool = False,
+                           fd_step: Optional[float] = None, gradient: str = "difference", return_exceptions: bool = False,
+                           max_sets_per_call: Optional[int] = None):
+    """calibrate_logsv on every chain, ANALYTIC engine, in lock-step: one engine.logsv_price_chains_batch call per optimizer round"""
+    n = check_lockstep_args(option_chains, max_sets_per_call, gradient)
+    if calibration_engine != CalibrationEngine.ANALYTIC:
+        raise NotImplementedError(f"calibrate_model_params_to_chains covers CalibrationEngine.ANALYTIC only, not {calibration_engine}")
+    if model_calibration_type not in (LogsvModelCalibrationType.PARAMS4, LogsvModelCalibrationType.PARAMS5,
+                                      LogsvModelCalibrationType.PARAMS_WITH_VARSWAP_FIT):
+        raise NotImplementedError(f"{model_calibration_type}")
+    p0s, los, his = (per_chain(v, n, name) for v, name in ((params0, "params0"), (params_min, "params_min"), (params_max, "params_max")))
+
+    def fit(k: int, price_batch):
+        return calibrate_logsv(pricer, option_chains[k], p0s[k], los[k], his[k], is_vega_weighted, is_unit_ttm_vega, model_calibration_type,
+                               constraints_type, calibration_engine, 0, 0, 0,          # nb_path, nb_steps, seed: Monte Carlo engines only
+                               is_spot_measure=is_spot_measure, disp=disp, return_info=True,
+                               fd_step=fd_step, price_batch=price_batch)
+
+    def price_call(requests):
+        # request = (args, kwargs) of engine.logsv_price_chain_batch(params_list, ttms, forwards, discfactors, etas, strikes, types, ...)
+        params, chain_of_set, chains, etas, scalers = [], [], [], [], []
+        for i, (args, kw) in enumerate(requests):
+            sets, ttms, forwards, discfactors, e, strikes_ttms, optiontypes_ttms = args
+            params += list(sets)
+            chain_of_set += [i] * len(sets)
+            chains.append((ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms))
+            etas += list(e)
+            scalers.append(kw["vol_scaler"])
+        _, ivols = engine.logsv_price_chains_batch(params, chain_of_set, chains, etas, scalers, is_spot_measure=is_spot_measure)
+        return _rows_by_request(ivols, chain_of_set, len(requests))
+
+    out = calibrate_chains_lockstep(fit, n, price_call, max_sets_per_call, return_exceptions)
+    return out if return_info else out[0]
+
+
+def calibrate_heston_chains(pricer, option_chains, params0, is_vega_weighted: bool, is_unit_ttm_vega: bool, disp: bool = False,
+                            return_info: bool = False, fd_step: Optional[float] = None, gradient: str = "difference",
+                            return_exceptions: bool = False, max_sets_per_call: Optional[int] = None):
+    """calibrate_heston on every chain in lock-step: one engine.heston_price_chains_batch call per optimizer round"""
+    n = check_lockstep_args(option_chains, max_sets_per_call, gradient)
+    p0s = per_chain(params0, n, "params0")
+
+    def fit(k: int, price_batch):
+        return calibrate_heston(pricer, option_chains[k], p0s[k], is_vega_weighted, is_unit_ttm_vega, disp=disp, return_info=True,
+                                fd_step=fd_step, price_batch=price_batch)
+
+    def price_call(requests):
+        # request = (args, kwargs) of engine.heston_price_chain_batch(params_list, ttms, forwards, discfactors, strikes, types)
+        params, chain_of_set, chains = [], [], []
+        for i, (args, _) in enumerate(requests):
+            params += list(args[0])
+            chain_of_set += [i] * len(args[0])
+            chains.append(tuple(args[1:6]))
+        _, ivols = engine.heston_price_chains_batch(params, chain_of_set, chains)
+        return _rows_by_request(ivols, chain_of_set, len(requests))
+
+    out = calibrate_chains_lockstep(fit, n, price_call, max_sets_per_call, return_exceptions)
+    return out if return_info else out[0]
+
+
+def _rows_by_request(ivols, chain_of_set, n: int) -> List[np.ndarray]:
+    """the B rows of a multi-chain call -> one [B_i, J_i] array per request (request i's sets are the i-th run of chain_of_set)"""
+    ends = np.cumsum(np.bincount(chain_of_set, minlength=n)).tolist()
+    return [np.vstack(ivols[a:b]) for a, b in zip([0] + ends[:-1], ends)]

@@ -93,6 +93,20 @@ class HestonPricer(ModelPricer):
                                 return_info=bool(kwargs.get("return_info", False)), fd_step=kwargs.get("fd_step"),
                                 gradient=kwargs.get("gradient", "difference"))
 
+    def calibrate_model_params_to_chains(self, option_chains: List[OptionChain], params0=None, is_vega_weighted: bool = True,
+                                         is_unit_ttm_vega: bool = False, return_exceptions: bool = False,
+                                         max_sets_per_call: Optional[int] = None, **kwargs):
+        """``calibrate_model_params_to_chain`` on every chain of ``option_chains``, in lock-step: one ``engine.heston_price_chains_batch``
+        call per optimizer round, every fit bit for bit the single-chain driver's (DESIGN.md §4.9).  ``params0``: None, one HestonParams
+        or a list of one per chain; ``gradient='difference'`` only.  Return value, ``return_info``, ``return_exceptions`` and
+        ``max_sets_per_call`` as LogSVPricer.calibrate_model_params_to_chains.  Slower than fitting the chains one after the other on the H100
+        measured so far (DESIGN.md §4.9)."""
+        from .calibration import calibrate_heston_chains
+        return calibrate_heston_chains(self, option_chains, params0, is_vega_weighted, is_unit_ttm_vega, disp=bool(kwargs.get("disp", False)),
+                                       return_info=bool(kwargs.get("return_info", False)), fd_step=kwargs.get("fd_step"),
+                                       gradient=kwargs.get("gradient", "difference"), return_exceptions=return_exceptions,
+                                       max_sets_per_call=max_sets_per_call)
+
     def model_mc_price_chain(self, option_chain: OptionChain, params: HestonParams, nb_path: int = 100000,
                              variable_type: VariableType = VariableType.LOG_RETURN, **kwargs) -> Tuple[List[np.ndarray], List[np.ndarray]]:
         return heston_mc_chain_pricer(v0=params.v0, theta=params.theta, kappa=params.kappa, rho=params.rho, volvol=params.volvol,

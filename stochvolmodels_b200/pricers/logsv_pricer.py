@@ -233,6 +233,35 @@ class LogSVPricer(ModelPricer):
                                return_info=bool(kwargs.get("return_info", False)), fd_step=kwargs.get("fd_step"),
                                mc_randoms=kwargs.get("mc_randoms", "numpy"), gradient=kwargs.get("gradient", "difference"))
 
+    def calibrate_model_params_to_chains(self, option_chains: List[OptionChain], params0, params_min=None, params_max=None,
+                                         is_vega_weighted: bool = True, is_unit_ttm_vega: bool = False,
+                                         model_calibration_type: LogsvModelCalibrationType = LogsvModelCalibrationType.PARAMS5,
+                                         constraints_type: ConstraintsType = ConstraintsType.UNCONSTRAINT,
+                                         calibration_engine: CalibrationEngine = CalibrationEngine.ANALYTIC, return_exceptions: bool = False,
+                                         max_sets_per_call: Optional[int] = None, **kwargs):
+        """``calibrate_model_params_to_chain`` on every chain of ``option_chains`` (a series of daily chains, say), the fits run in
+        lock-step: each optimizer round prices the pending points of every fit in one ``engine.logsv_price_chains_batch`` call, and every
+        fit equals, bit for bit, the single-chain driver's on its chain (DESIGN.md §4.9).  ``params0`` / ``params_min`` / ``params_max``:
+        one LogSvParams for all chains or a list of one per chain.  ANALYTIC engine, ``gradient='difference'``; PARAMS4, PARAMS5 and
+        PARAMS_WITH_VARSWAP_FIT.  ``max_sets_per_call`` caps the parameter sets of one library call (a round then takes several; a fit's
+        n + 1 sets always share one); without it a round is one call of about (n + 1) K sets, ~320 kB of ODE state per set on a
+        four-maturity chain, so pass it for long series.  Every chain gets a thread.  Not faster than fitting the chains one after the
+        other on the H100 measured so far: the Python optimizer work dominates (DESIGN.md §4.9).  Returns the list of fits, with ``return_info=True`` also the list of info dicts, each with
+        ``rounds``, the library calls of the whole run.  A fit that fails raises its error after all fits have ended (the lowest chain
+        index first), or with ``return_exceptions=True`` takes the exception's place in the list (its info is None)."""
+        from .calibration import calibrate_logsv_chains, per_chain
+        n = len(option_chains)
+        params_min = [p or LogSvParams(sigma0=0.1, theta=0.1, kappa1=0.25, kappa2=0.25, beta=-3.0, volvol=0.2)
+                      for p in per_chain(params_min, n, "params_min")]
+        params_max = [p or LogSvParams(sigma0=1.5, theta=1.5, kappa1=10.0, kappa2=10.0, beta=3.0, volvol=3.0)
+                      for p in per_chain(params_max, n, "params_max")]
+        return calibrate_logsv_chains(self, option_chains, params0, params_min, params_max, is_vega_weighted, is_unit_ttm_vega,
+                                      model_calibration_type, constraints_type, calibration_engine,
+                                      is_spot_measure=kwargs.get("is_spot_measure", True), disp=bool(kwargs.get("disp", False)),
+                                      return_info=bool(kwargs.get("return_info", False)), fd_step=kwargs.get("fd_step"),
+                                      gradient=kwargs.get("gradient", "difference"), return_exceptions=return_exceptions,
+                                      max_sets_per_call=max_sets_per_call)
+
     @timer
     def model_mc_price_chain(self, option_chain: OptionChain, params: LogSvParams, is_spot_measure: bool = True,
                              variable_type: VariableType = VariableType.LOG_RETURN, nb_path: int = 100000,
