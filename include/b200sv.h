@@ -547,6 +547,12 @@ int b200sv_heston_price_chains_batch(const b200sv_heston_params* params, int B, 
                                      const double* ttms, const double* forwards, const double* discfactors, const int* offsets,
                                      const double* strikes, const int8_t* types, const double* vol_scalers, int P, double* prices_out,
                                      double* ivols_out);
+/* the Hawkes twin, without a risk kernel: layout, vol_scalers and row equality as above, against b200sv_hawkesjd_price_chain_batch with
+ * gammas = NULL (P <= 0: 500).  Each chain's sets are integrated by one Riccati launch. */
+int b200sv_hawkesjd_price_chains_batch(const b200sv_hawkes_params* params, int B, const int* chain_of_set, int K, const int* Ms,
+                                       const double* ttms, const double* forwards, const double* discfactors, const int* offsets,
+                                       const double* strikes, const int8_t* types, int is_spot_measure, const double* vol_scalers, int P,
+                                       double* prices_out, double* ivols_out);
 
 /* same for the Hawkes jump-diffusion: the objectives of HawkesJDPricer.calibrate_model_params_to_chain and
  * calibrate_risk_premia_gamma_to_chain (pricers/hawkes_jd_pricer.py:230-357).  B Hawkes parameter sets on one chain in one pass.

@@ -884,6 +884,76 @@ __global__ void __launch_bounds__(TPB) hawkes_mgf_kernel(const cd* __restrict__ 
   if (status) status[p] = st;
 }
 
+// ---- several Hawkes parameter sets in one Riccati launch (b200sv_hawkesjd_price_chains_batch, DESIGN.md §4.10) ----
+// hawkes_mgf_kernel reads its constants as kernel parameters, and ptxas contracts HawkesRhsFn's plain fp64 products and sums around
+// them: it sinks the loop-invariant sigma^2 drift and comp * phi products into fused multiply-adds inside the step loop, fuses the
+// A-products of z and of the outputs, and leaves Smith's division unfused.  With the constants in registers it hoists those products
+// instead, and rows move by an ulp.  So the set-major kernel's right-hand side spells out, with rounding intrinsics that ptxas may
+// neither fuse nor split, the operations hawkes_mgf_kernel's SASS performs, and the two kernels carry the same fp64 instructions
+// (DESIGN.md §4.10).  exp_ (sincos, exp) is shared.
+
+// Smith's division as operator/ compiles in HawkesRhsFn: every product and sum rounded on its own
+__device__ __forceinline__ cd cdiv_rn(cd a, cd b) {
+  if (fabs(b.re) >= fabs(b.im)) {
+    const double r = __ddiv_rn(b.im, b.re), d = __dadd_rn(b.re, __dmul_rn(b.im, r));
+    return cd{__ddiv_rn(__dadd_rn(a.re, __dmul_rn(a.im, r)), d), __ddiv_rn(__dsub_rn(a.im, __dmul_rn(a.re, r)), d)};
+  }
+  const double r = __ddiv_rn(b.re, b.im), d = __dadd_rn(__dmul_rn(b.re, r), b.im);
+  return cd{__ddiv_rn(__dadd_rn(__dmul_rn(a.re, r), a.im), d), __ddiv_rn(__dsub_rn(__dmul_rn(a.im, r), a.re), d)};
+}
+
+// E(z) - 1 of HawkesRhsFn: exp(-shift z) / (1 + mean z) - 1
+__device__ __forceinline__ cd hawkes_jump_rn(cd z, double shift, double mean) {
+  const cd q = cdiv_rn(exp_(cd{__dmul_rn(-shift, z.re), __dmul_rn(-shift, z.im)}), cd{__fma_rn(z.re, mean, 1.0), __fma_rn(z.im, mean, 0.0)});
+  return cd{__dadd_rn(q.re, -1.0), q.im};
+}
+
+// HawkesRhsFn for constants in registers.  d = (phi + 1) phi / 2 - psi with psi = 0: the sigma^2 product of drift0 is fused into out[0].
+struct HawkesSetsRhsFn {
+  const HawkesMgfConsts& c;
+  cd phi, d;
+  __device__ __forceinline__ void operator()(const cd (&A)[3], cd (&out)[3]) const {
+    const cd zp{__fma_rn(-c.beta1_m, A[2].re, __fma_rn(-c.beta1_p, A[1].re, phi.re)),
+                __fma_rn(-c.beta1_m, A[2].im, __fma_rn(-c.beta1_p, A[1].im, phi.im))};
+    const cd zm{__fma_rn(-c.beta2_m, A[2].re, __fma_rn(-c.beta2_p, A[1].re, phi.re)),
+                __fma_rn(-c.beta2_m, A[2].im, __fma_rn(-c.beta2_p, A[1].im, phi.im))};
+    const cd jp = hawkes_jump_rn(zp, c.shift_p, c.mean_p), jm = hawkes_jump_rn(zm, c.shift_m, c.mean_m);
+    out[0] = cd{__fma_rn(d.re, c.sigma2, __fma_rn(A[1].re, c.kt_p, __dmul_rn(A[2].re, c.kt_m))),
+                __fma_rn(d.im, c.sigma2, __fma_rn(A[1].im, c.kt_p, __dmul_rn(A[2].im, c.kt_m)))};
+    out[1] = cd{__fma_rn(phi.re, c.comp_p, __fma_rn(-A[1].re, c.kappa_p, jp.re)), __fma_rn(phi.im, c.comp_p, __fma_rn(-A[1].im, c.kappa_p, jp.im))};
+    out[2] = cd{__fma_rn(phi.re, c.comp_m, __fma_rn(-A[2].re, c.kappa_m, jm.re)), __fma_rn(phi.im, c.comp_m, __fma_rn(-A[2].im, c.kappa_m, jm.im))};
+  }
+};
+
+// One thread = one (set, transform point) of B sets sharing the maturity increments dtaus [M]: the set is the FASTEST thread index (the
+// logsv_mgf_kernel batch mapping: the lanes of a warp integrate one point for neighbouring sets, which take nearly the same steps).
+// consts [B], phi [B][P] (phi_stride = P) or one grid (0); log_mgf [B][M][P].  A starts at 0 and is carried over the maturities.
+// Every value equals hawkes_mgf_kernel's for that set alone, bit for bit, whatever block size either runs at.
+template <int TPB>
+__global__ void __launch_bounds__(TPB) hawkes_mgf_sets_kernel(const cd* __restrict__ phi, int P, int M, const double* __restrict__ dtaus,
+                                                              const HawkesMgfConsts* __restrict__ consts, int B, int phi_stride,
+                                                              cd* __restrict__ log_mgf) {
+  __shared__ cd stage_smem[6 * 3 * TPB];
+  const long long t = (long long)blockIdx.x * TPB + threadIdx.x;
+  if (t >= (long long)B * P) return;
+  const int b = (int)(t % B), p = (int)(t / B);
+  const HawkesMgfConsts c = consts[b];
+  StageStore<3, TPB> K{stage_smem + threadIdx.x};
+#pragma unroll
+  for (int i = 0; i < 18; ++i) stage_smem[threadIdx.x + i * TPB] = mk(0.0);
+  cd A[3] = {mk(0.0), mk(0.0), mk(0.0)};
+  const cd ph = phi[(size_t)b * phi_stride + p];
+  const cd p1{__dadd_rn(ph.re, 1.0), __dadd_rn(ph.im, 0.0)};                                    // phi + 1
+  const cd pp{__fma_rn(p1.re, ph.re, -__dmul_rn(p1.im, ph.im)), __fma_rn(p1.re, ph.im, __dmul_rn(p1.im, ph.re))};   // (phi + 1) phi
+  const HawkesSetsRhsFn f{c, ph, cd{__fma_rn(pp.re, 0.5, -0.0), __fma_rn(pp.im, 0.5, -0.0)}};
+  cd* lm = log_mgf + (size_t)b * M * P + p;
+  for (int m = 0; m < M; ++m) {
+    rk45_generic<3, TPB>(A, dtaus[m], f, K, nullptr);
+    lm[(size_t)m * P] = cd{__fma_rn(A[2].re, c.lambda_m, __fma_rn(A[1].re, c.lambda_p, A[0].re)),
+                           __fma_rn(A[2].im, c.lambda_m, __fma_rn(A[1].im, c.lambda_p, A[0].im))};
+  }
+}
+
 // slice_pricer_with_mgf_grid_with_gamma (utils/mgf_pricer.py:273-320): general weights -(dp/pi) / ((phi + g + 1)(phi + g)) (its fast branch
 // compares Re(phi) with +(1/2 + g) while the grid sits on -(1/2 + g), so it never runs), calls gamma_forward - n K^(1+g) S, puts K - n K^(1+g) S;
 // no discount factor (both as in the reference).  Row grid sp.grid sits on Re phi = -1/2 - gammas[sp.grid]; norm_gfwd[2 sp.slice + {0, 1}] =
@@ -2654,6 +2724,23 @@ static void launch_hawkes_mgf(cudaStream_t st, const cd* phi, const cd* psi, int
   k<<<(P + tpb - 1) / tpb, tpb, 0, st>>>(phi, psi, P, M, dtaus, c, a_in, a_out, lm, restart, nullptr);
 }
 
+// hawkes_mgf_sets_kernel over the B * P (set, point) threads of B sets; block size as for hawkes_mgf_kernel, from the threads in flight
+using HawkesMgfSetsKernel = decltype(&hawkes_mgf_sets_kernel<64>);
+static void launch_hawkes_mgf_sets(cudaStream_t st, const cd* phi, int P, int M, const double* dtaus, const HawkesMgfConsts* consts, int B,
+                                   int phi_stride, cd* lm) {
+  const long long n = (long long)B * P;
+  const int tpb = mgf_block_threads((int)std::min<long long>(n, 1 << 30));
+  HawkesMgfSetsKernel k;
+  switch (tpb) {
+    case 4: k = hawkes_mgf_sets_kernel<4>; break;
+    case 8: k = hawkes_mgf_sets_kernel<8>; break;
+    case 16: k = hawkes_mgf_sets_kernel<16>; break;
+    case 32: k = hawkes_mgf_sets_kernel<32>; break;
+    default: k = hawkes_mgf_sets_kernel<64>;
+  }
+  k<<<(unsigned)((n + tpb - 1) / tpb), tpb, 0, st>>>(phi, P, M, dtaus, consts, B, phi_stride, lm);
+}
+
 // hawkes_mgf_tangent_kernel over the P * 13 (point, direction) threads; block size as for hawkes_mgf_kernel, from the threads in flight
 using HawkesTangentKernel = decltype(&hawkes_mgf_tangent_kernel<64>);
 static void launch_hawkes_mgf_tangent(cudaStream_t st, const cd* phi, int P, int M, const double* dtaus, const HawkesMgfConsts& c,
@@ -3554,6 +3641,41 @@ int b200sv_heston_price_chains_batch(const b200sv_heston_params* params, int B, 
                                                                     g.c.per_set_grid ? g.c.P : 0);
     ++gi;
     return check_launch("heston_mgf_kernel");
+  });
+}
+
+// The Hawkes twin without a risk kernel: each group is validated as b200sv_hawkesjd_price_chain_batch validates its sets (default P =
+// 500, Re phi = -1/2 under both measures) and integrated by ONE hawkes_mgf_sets_kernel launch, whose rows equal the single-set
+// hawkes_mgf_kernel launches of that call bit for bit.
+int b200sv_hawkesjd_price_chains_batch(const b200sv_hawkes_params* params, int B, const int* chain_of_set, int K, const int* Ms,
+                                       const double* ttms, const double* forwards, const double* discfactors, const int* offsets,
+                                       const double* strikes, const int8_t* types, int is_spot_measure, const double* vol_scalers, int P,
+                                       double* prices_out, double* ivols_out) {
+  B200SV_REQUIRE(prices_out, "null pointer");
+  ChainsCall<b200sv_hawkes_params> call;
+  if (int rc = call.prepare(params, B, chain_of_set, K, Ms, ttms, forwards, discfactors, nullptr, offsets, strikes, types, is_spot_measure != 0,
+                            vol_scalers, P > 0 ? P : 500))                // MAX_PHI, hawkes_jd_pricer.py:37
+    return rc;
+  std::vector<double> dt;
+  std::vector<HawkesMgfConsts> k;
+  std::vector<size_t> dt0, k0;
+  for (auto& g : call.groups) {
+    for (size_t i = 0; i < g.c.phi.size(); i += 2) g.c.phi[i] = -0.5;     // prepare_hawkes_batch without gammas
+    dt0.push_back(dt.size());
+    k0.push_back(k.size());
+    dt.insert(dt.end(), g.c.dtaus.begin(), g.c.dtaus.end());
+    for (const auto& p : g.params) k.push_back(make_hawkes_mgf_consts(p));
+  }
+  HostCall host;
+  DevBuf d_dt(host.st), d_k(host.st);
+  B200SV_CUDA(d_dt.upload(dt.data(), dt.size()));
+  B200SV_CUDA(d_k.upload(k.data(), k.size()));
+  size_t gi = 0;
+  return run_chains(host, call, is_spot_measure != 0 ? 1 : 0, prices_out, ivols_out, [&](const auto& g, cudaStream_t s, const cd* phi, cd* lm) {
+    launch_hawkes_mgf_sets(s, phi, g.c.P, g.c.M, d_dt.as<double>() + dt0[gi], d_k.as<HawkesMgfConsts>() + k0[gi], g.c.B,
+                           g.c.per_set_grid ? g.c.P : 0, lm);
+    ++gi;
+    return check_launch("hawkes_mgf_sets_kernel");
   });
 }
 

@@ -813,6 +813,14 @@ def hawkesjd_price_chain_batch(params_list: Sequence[C.HawkesParamsC], ttms, for
                         with_ivols)
 
 
+def hawkesjd_price_chains_batch(params_list: Sequence[C.HawkesParamsC], chain_of_set, chains, vol_scalers=None, is_spot_measure: bool = True,
+                                max_phi: int = 500, with_ivols: bool = True):
+    """B Hawkes parameter sets over K chains in one pass, no risk kernel -> (prices, ivols | None); arguments as logsv_price_chains_batch.
+    Row b is bit for bit row b of hawkesjd_price_chain_batch on its chain with the sets of this call on that chain, in order."""
+    return _chains_batch("b200sv_hawkesjd_price_chains_batch", C.HawkesParamsC, params_list, chain_of_set, chains, (), vol_scalers,
+                         is_spot_measure, (int(bool(is_spot_measure)),), (int(max_phi),), with_ivols)
+
+
 def _logsv_mgf_grid(symbol: str, phi, psi, dtau: float, a_t0, params: C.LogsvParamsC, expansion_order: int, args):
     """the three LogSV grid solvers: C arguments (phi, psi, P, dtau, a, params, *args, log_mgf) -> (a_t1 [P, n], log_mgf [P])"""
     phi = C.c128(phi)

@@ -28,7 +28,8 @@ from ..data.option_chain import OptionChain
 from ..multi_gpu import _shared_seed, _use_distributed, mc_chain_distributed
 from ..utils.config import VariableType
 from ..utils.funcs import set_time_grid, timer
-from .calibration import SLSQP_EPS, ExactGradientObjective, ScipyDifferenceObjective, check_gradient, flat_ivol_rows
+from .calibration import (SLSQP_EPS, ExactGradientObjective, ScipyDifferenceObjective, _rows_by_request, calibrate_chains_lockstep,
+                          check_gradient, check_lockstep_args, flat_ivol_rows, per_chain)
 from .model_pricer import ModelParams, ModelPricer
 
 _KEYS = tuple(k for k, _ in C.HawkesParamsC._fields_)
@@ -174,32 +175,20 @@ class HawkesJDPricer(ModelPricer):
         in one ``hawkesjd_price_chain_batch`` call; objective and gradient are bit for bit what SLSQP differences from the one-set objective,
         so the fit is too.  ``return_info``: (fit, {"fun", "nit", "nb_batches", "x", "nan_quotes"}).  ``gradient='exact'`` hands SLSQP the
         exact gradient from one ``compute_chain_ivol_greeks`` call per point, on ``params0``'s default grid (DESIGN.md §4.6)."""
-        from scipy.optimize import minimize
-        gradient = check_gradient(kwargs.get("gradient", "difference"))
-        p0 = np.array([params0.sigma, params0.mean_p, params0.mean_m, params0.theta_p, params0.theta_m, 0.5 * (params0.kappa_p + params0.kappa_m),
-                       0.5 * (params0.beta1_p - params0.beta2_p), 0.5 * (params0.beta2_p - params0.beta2_m)])
-        bounds = ((0.10, 2.0), (0.01, 0.99), (-0.99, -0.01), (0.01, 100.0), (0.01, 100.0), (1.0, 100.0), (1.0, 100.0), (1.0, 100.0))
+        return calibrate_hawkes(self, option_chain, params0, is_vega_weighted, is_unit_ttm_vega, return_info, **kwargs)
 
-        def unpack(x: np.ndarray) -> HawkesJDParams:
-            return HawkesJDParams(mu=0.0, sigma=x[0], shift_p=params0.shift_p, mean_p=x[1], shift_m=params0.shift_m, mean_m=x[2],
-                                  lambda_p=params0.lambda_p, theta_p=x[3], kappa_p=x[5], beta1_p=x[6], beta2_p=-x[6], lambda_m=params0.lambda_m,
-                                  theta_m=x[4], kappa_m=x[5], beta1_m=x[7], beta2_m=-x[7])
-
-        stationary = {"type": "ineq", "fun": lambda x: unpack(x).jump1_cond + unpack(x).jump2_cond}
-        options = {"disp": bool(kwargs.get("disp", False)), "ftol": 1e-8}
-        if "maxiter" in kwargs:
-            options["maxiter"] = int(kwargs["maxiter"])
-        if gradient == "exact":
-            objective = _exact_vol_objective(self, option_chain, unpack, is_vega_weighted, is_unit_ttm_vega,
-                                             set_vol_scaler(params0.sigma, float(option_chain.ttms[0])))
-        else:
-            objective = _batched_vol_objective(option_chain, unpack, is_vega_weighted, is_unit_ttm_vega, bounds, SLSQP_EPS)
-        res = minimize(objective.fun, p0, args=None, method="SLSQP", jac=objective.jac, constraints=stationary, bounds=bounds, options=options)
-        fit = unpack(res.x)
-        if return_info:
-            return fit, {"fun": float(res.fun), "nit": int(res.nit), "nb_batches": objective.nb_batches, "x": res.x,
-                         "nan_quotes": objective.nan_quotes}
-        return fit
+    def calibrate_model_params_to_chains(self, option_chains: List[OptionChain], params0, is_vega_weighted: bool = True,
+                                         is_unit_ttm_vega: bool = False, return_info: bool = False, gradient: str = "difference",
+                                         return_exceptions: bool = False, max_sets_per_call: Optional[int] = None, **kwargs):
+        """``calibrate_model_params_to_chain`` on every chain of ``option_chains``, in lock-step: one ``engine.hawkesjd_price_chains_batch``
+        call per optimizer round, each chain's parameter sets in one Riccati launch, every fit bit for bit the single-chain driver's
+        (DESIGN.md §4.10).  ``params0``: one HawkesJDParams or a list of one per chain (``risk_premia_gamma`` ignored, as by the single-chain
+        fit); ``gradient='difference'`` only; ``disp`` / ``maxiter`` (extras) as there.  -> list of fits, with ``return_info`` (fits, infos)
+        whose info dicts add ``rounds`` (library calls of the run).  ``return_exceptions``: a failed fit's slot holds its exception instead
+        of raising the first one after all fits have ended.  ``max_sets_per_call`` splits a round into calls of at most that many sets
+        (never one fit's sets).  Every chain runs in a thread of its own while the caller's thread prices."""
+        return calibrate_hawkes_chains(self, option_chains, params0, is_vega_weighted, is_unit_ttm_vega, return_info=return_info,
+                                       gradient=gradient, return_exceptions=return_exceptions, max_sets_per_call=max_sets_per_call, **kwargs)
 
     @timer
     def calibrate_risk_premia_gamma_to_chain(self, option_chain: OptionChain, params0: HawkesJDParams, is_vega_weighted: bool = True,
@@ -306,6 +295,64 @@ def set_vol_scaler(sigma0: float, ttm: float) -> float:
     return float(np.clip(sigma0, 0.2, 0.5) * np.sqrt(np.minimum(ttm, 1.0 / 12.0)))
 
 
+def calibrate_hawkes(pricer, option_chain: OptionChain, params0: HawkesJDParams, is_vega_weighted: bool, is_unit_ttm_vega: bool,
+                     return_info: bool = False, price_batch=None, **kwargs):
+    """HawkesJDPricer.calibrate_model_params_to_chain.  ``price_batch``: what the difference objective prices its points with,
+    engine.hawkesjd_price_chain_batch (None) or a callable with its arguments and return value (calibrate_hawkes_chains)"""
+    from scipy.optimize import minimize
+    gradient = check_gradient(kwargs.get("gradient", "difference"))
+    p0 = np.array([params0.sigma, params0.mean_p, params0.mean_m, params0.theta_p, params0.theta_m, 0.5 * (params0.kappa_p + params0.kappa_m),
+                   0.5 * (params0.beta1_p - params0.beta2_p), 0.5 * (params0.beta2_p - params0.beta2_m)])
+    bounds = ((0.10, 2.0), (0.01, 0.99), (-0.99, -0.01), (0.01, 100.0), (0.01, 100.0), (1.0, 100.0), (1.0, 100.0), (1.0, 100.0))
+
+    def unpack(x: np.ndarray) -> HawkesJDParams:
+        return HawkesJDParams(mu=0.0, sigma=x[0], shift_p=params0.shift_p, mean_p=x[1], shift_m=params0.shift_m, mean_m=x[2],
+                              lambda_p=params0.lambda_p, theta_p=x[3], kappa_p=x[5], beta1_p=x[6], beta2_p=-x[6], lambda_m=params0.lambda_m,
+                              theta_m=x[4], kappa_m=x[5], beta1_m=x[7], beta2_m=-x[7])
+
+    stationary = {"type": "ineq", "fun": lambda x: unpack(x).jump1_cond + unpack(x).jump2_cond}
+    options = {"disp": bool(kwargs.get("disp", False)), "ftol": 1e-8}
+    if "maxiter" in kwargs:
+        options["maxiter"] = int(kwargs["maxiter"])
+    if gradient == "exact":
+        objective = _exact_vol_objective(pricer, option_chain, unpack, is_vega_weighted, is_unit_ttm_vega,
+                                         set_vol_scaler(params0.sigma, float(option_chain.ttms[0])))
+    else:
+        objective = _batched_vol_objective(option_chain, unpack, is_vega_weighted, is_unit_ttm_vega, bounds, SLSQP_EPS,
+                                           price_batch=price_batch)
+    res = minimize(objective.fun, p0, args=None, method="SLSQP", jac=objective.jac, constraints=stationary, bounds=bounds, options=options)
+    fit = unpack(res.x)
+    if return_info:
+        return fit, {"fun": float(res.fun), "nit": int(res.nit), "nb_batches": objective.nb_batches, "x": res.x,
+                     "nan_quotes": objective.nan_quotes}
+    return fit
+
+
+def calibrate_hawkes_chains(pricer, option_chains, params0, is_vega_weighted: bool, is_unit_ttm_vega: bool, return_info: bool = False,
+                            gradient: str = "difference", return_exceptions: bool = False, max_sets_per_call: Optional[int] = None, **kwargs):
+    """calibrate_hawkes on every chain in lock-step: one engine.hawkesjd_price_chains_batch call per optimizer round"""
+    n = check_lockstep_args(option_chains, max_sets_per_call, gradient)
+    p0s = per_chain(params0, n, "params0")
+
+    def fit(k: int, price_batch):
+        return calibrate_hawkes(pricer, option_chains[k], p0s[k], is_vega_weighted, is_unit_ttm_vega, return_info=True, price_batch=price_batch,
+                                **kwargs)
+
+    def price_call(requests):
+        # request = (args, kwargs) of engine.hawkesjd_price_chain_batch(params_list, ttms, forwards, discfactors, strikes, types,
+        # max_phi=MAX_PHI, gammas=None)
+        params, chain_of_set, chains = [], [], []
+        for i, (args, _) in enumerate(requests):
+            params += list(args[0])
+            chain_of_set += [i] * len(args[0])
+            chains.append(tuple(args[1:6]))
+        _, ivols = engine.hawkesjd_price_chains_batch(params, chain_of_set, chains, max_phi=MAX_PHI)
+        return _rows_by_request(ivols, chain_of_set, len(requests))
+
+    out = calibrate_chains_lockstep(fit, n, price_call, max_sets_per_call, return_exceptions)
+    return out if return_info else out[0]
+
+
 def _fourier_chain(model_params: HawkesJDParams, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, is_stiff_solver, is_spot_measure,
                    variable_type, vol_scaler, gamma, return_grids=False):
     if getattr(variable_type, "value", variable_type) != VariableType.LOG_RETURN.value:
@@ -359,19 +406,20 @@ def _exact_vol_objective(pricer, option_chain: OptionChain, to_params, is_vega_w
 
 
 def _batched_vol_objective(option_chain: OptionChain, to_params, is_vega_weighted: bool, is_unit_ttm_vega: bool, bounds, eps: float,
-                           scale: float = 1.0, on_point=None) -> ScipyDifferenceObjective:
+                           scale: float = 1.0, on_point=None, price_batch=None) -> ScipyDifferenceObjective:
     """the drivers' objective: weighted squared difference of model and mid implied vols, nansum over the chain (quotes whose model price
     leaves the no-arbitrage bounds drop out), with the weights of the reference (per-slice normalised vegas, times ``scale``).  The model vols
     of a point, and of its difference neighbours together, come from hawkesjd_price_chain_batch, on the risk-kernel route when the
-    parameter sets carry a risk_premia_gamma -- the same prices and vols as compute_model_ivols_for_chain per set."""
+    parameter sets carry a risk_premia_gamma -- the same prices and vols as compute_model_ivols_for_chain per set.  ``price_batch``: a callable
+    with hawkesjd_price_chain_batch's arguments and return value in its place (the lock-step driver)."""
     market, weights = _market_and_weights(option_chain, is_vega_weighted, is_unit_ttm_vega)
 
     def batch_vols(points: np.ndarray) -> np.ndarray:
         sets = [to_params(p) for p in points]
         gammas = None if sets[0].risk_premia_gamma is None else [s.risk_premia_gamma for s in sets]
-        _, ivols = engine.hawkesjd_price_chain_batch([_params_c(**s.to_dict()) for s in sets], option_chain.ttms, option_chain.forwards,
-                                                     option_chain.discfactors, option_chain.strikes_ttms, option_chain.optiontypes_ttms,
-                                                     max_phi=MAX_PHI, gammas=gammas)
+        _, ivols = (price_batch or engine.hawkesjd_price_chain_batch)([_params_c(**s.to_dict()) for s in sets], option_chain.ttms,
+                                                                      option_chain.forwards, option_chain.discfactors, option_chain.strikes_ttms,
+                                                                      option_chain.optiontypes_ttms, max_phi=MAX_PHI, gammas=gammas)
         return ivols
     return ScipyDifferenceObjective(batch_vols=batch_vols, market_vols=market, weights=scale * weights, bounds=bounds, eps=eps,
                                     on_point=on_point)
