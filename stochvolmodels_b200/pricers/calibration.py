@@ -104,12 +104,23 @@ def validate_optimization_result(result, bounds) -> np.ndarray:
     return x
 
 
-def calibration_weights(option_chain, market_vols: np.ndarray, is_vega_weighted: bool, is_unit_ttm_vega: bool) -> np.ndarray:
-    """flattened objective weights: per-slice normalised Black vegas or ones (reference logsv_pricer.py:196-207)."""
+def calibration_weights(option_chain, market_vols: np.ndarray, is_vega_weighted: bool, is_unit_ttm_vega: bool,
+                        slice_sum: Callable = sum) -> np.ndarray:
+    """flattened objective weights: the Black vegas of each slice divided by their ``slice_sum``, or ones (reference
+    logsv_pricer.py:196-207).  The LogSV and Heston drivers normalise with the builtin ``sum`` (left to right), the Hawkes drivers with
+    ``np.sum`` (pairwise from 8 quotes a slice) -- the two differ in the last bit, so each driver names its own."""
     if not is_vega_weighted:
         return np.ones_like(market_vols)
     vegas_ttms = option_chain.get_chain_vegas(is_unit_ttm_vega=is_unit_ttm_vega)
-    return to_flat_np_array([v / sum(v) for v in vegas_ttms])
+    return to_flat_np_array([v / slice_sum(v) for v in vegas_ttms])
+
+
+def market_and_weights(option_chain, is_vega_weighted: bool, is_unit_ttm_vega: bool, slice_sum: Callable = sum
+                       ) -> Tuple[np.ndarray, np.ndarray]:
+    """(mid vols, calibration_weights) flat in chain order: what every driver's objective compares the model vols with"""
+    _, mid_vols = option_chain.get_chain_data_as_xy()
+    market = to_flat_np_array(mid_vols)
+    return market, calibration_weights(option_chain, market, is_vega_weighted, is_unit_ttm_vega, slice_sum)
 
 
 @dataclass
@@ -296,14 +307,21 @@ def flat_ivol_rows(sens, names: Sequence[str]) -> Tuple[np.ndarray, np.ndarray]:
     return (to_flat_np_array(sens.ivols), np.vstack([to_flat_np_array(sens.params[n]) for n in names]))
 
 
-def run_slsqp(objective: BatchedObjective, p0: np.ndarray, bounds, constraints=None, disp: bool = False):
-    """``scipy.optimize.minimize(method='SLSQP', options={'ftol': 1e-8})`` as in the reference (:543-555), with the batched gradient."""
+def run_slsqp(objective, p0: np.ndarray, bounds, constraints=None, disp: bool = False, tol: Optional[float] = None, validate: bool = True,
+              **options):
+    """``scipy.optimize.minimize(method='SLSQP', options={'ftol': 1e-8})`` as in the reference (:543-555), with the objective's own
+    gradient -> (x, result).  ``options`` (``maxiter``, ``eps``, another ``ftol``) and ``tol`` go to SLSQP as given.  ``validate``: x is
+    the vector validate_optimization_result accepts (the LogSV and Heston drivers, as the reference's), else ``result.x`` unchecked (the
+    Hawkes drivers, as the reference's hawkes_jd_pricer.py:296-298)."""
     from scipy.optimize import minimize      # host-side optimizer; scipy is already a dependency of the reference
-    kwargs = dict(method="SLSQP", jac=objective.jac, bounds=bounds, options={"disp": disp, "ftol": 1e-8})
-    if constraints is not None:
-        kwargs["constraints"] = constraints
-    result = minimize(objective.fun, np.asarray(p0, dtype=float), **kwargs)
-    return validate_optimization_result(result, bounds), result
+    result = minimize(objective.fun, np.asarray(p0, dtype=float), method="SLSQP", jac=objective.jac, bounds=bounds,
+                      constraints=() if constraints is None else constraints, tol=tol, options={"disp": disp, "ftol": 1e-8, **options})
+    return (validate_optimization_result(result, bounds) if validate else result.x), result
+
+
+def fit_info(result, x: np.ndarray, objective, **extra) -> dict:
+    """the ``return_info`` dict of a fit: SLSQP's last value and iterations, the library calls of the objective, the fitted vector"""
+    return {"fun": float(result.fun), "nit": int(result.nit), "nb_batches": objective.nb_batches, "x": x, **extra}
 
 
 # ---- LogSV ------------------------------------------------------------------------------------------------------------------
@@ -399,30 +417,27 @@ def calibrate_logsv(pricer, option_chain, params0, params_min, params_max, is_ve
                     calibration_engine: CalibrationEngine, nb_path: int, nb_steps: int, seed: int, is_spot_measure: bool = True,
                     disp: bool = False, return_info: bool = False, fd_step: Optional[float] = None, mc_randoms: str = "numpy",
                     gradient: str = "difference", price_batch: Optional[Callable] = None):
-    """``price_batch``: what the ANALYTIC difference objective prices its points with, engine.logsv_price_chain_batch (None) or a
-    callable with its arguments and return value (the lock-step drivers of calibrate_chains_lockstep)"""
-    if check_gradient(gradient, pathwise=True) == "exact":
-        if calibration_engine != CalibrationEngine.ANALYTIC:
-            raise NotImplementedError(f"gradient='exact' covers CalibrationEngine.ANALYTIC only, not {calibration_engine} "
-                                      "(the Monte Carlo engines have gradient='pathwise')")
+    """``params_min`` / ``params_max``: None for the default bounds.  ``price_batch``: what the ANALYTIC difference objective prices its
+    points with, engine.logsv_price_chain_batch (None) or a callable with its arguments and return value (calibrate_chains_lockstep)"""
+    routes = {"exact": ((CalibrationEngine.ANALYTIC,), "CalibrationEngine.ANALYTIC only", "the Monte Carlo engines have gradient='pathwise'"),
+              "pathwise": ((CalibrationEngine.MC, CalibrationEngine.ROUGH_MC), "CalibrationEngine.MC and ROUGH_MC only",
+                           "the ANALYTIC engine has gradient='exact'")}
+    if check_gradient(gradient, pathwise=True) in routes:
+        engines, covered, other = routes[gradient]
+        if calibration_engine not in engines:
+            raise NotImplementedError(f"gradient={gradient!r} covers {covered}, not {calibration_engine} ({other})")
         if model_calibration_type not in (LogsvModelCalibrationType.PARAMS4, LogsvModelCalibrationType.PARAMS5):
-            raise NotImplementedError(f"gradient='exact' covers PARAMS4 and PARAMS5 only, not {model_calibration_type} (the eta backbone "
-                                      "of PARAMS_WITH_VARSWAP_FIT is refitted at every point and is not differentiated)")
-    if gradient == "pathwise":
-        if calibration_engine not in (CalibrationEngine.MC, CalibrationEngine.ROUGH_MC):
-            raise NotImplementedError(f"gradient='pathwise' covers CalibrationEngine.MC and ROUGH_MC only, not {calibration_engine} "
-                                      "(the ANALYTIC engine has gradient='exact')")
-        if model_calibration_type not in (LogsvModelCalibrationType.PARAMS4, LogsvModelCalibrationType.PARAMS5):
-            raise NotImplementedError(f"gradient='pathwise' covers PARAMS4 and PARAMS5 only, not {model_calibration_type} (the eta backbone "
-                                      "of PARAMS_WITH_VARSWAP_FIT is refitted at every point and is not differentiated)")
+            raise NotImplementedError(f"gradient={gradient!r} covers PARAMS4 and PARAMS5 only, not {model_calibration_type} (the eta "
+                                      "backbone of PARAMS_WITH_VARSWAP_FIT is refitted at every point and is not differentiated)")
     from ..multi_gpu import _fixed_randoms_chain_device
     from .fourier_greeks import to_chain_ivol_sensitivities
-    from .logsv_pricer import DeviceRandoms, _params_c, get_randoms_for_chain_valuation, logsv_mc_chain_greeks_fixed_randoms
+    from .logsv_pricer import (DeviceRandoms, LogSvParams, _params_c, get_randoms_for_chain_valuation,
+                               logsv_mc_chain_greeks_fixed_randoms)
     from .mc_greeks import to_mc_chain_greeks
+    params_min = params_min or LogSvParams(sigma0=0.1, theta=0.1, kappa1=0.25, kappa2=0.25, beta=-3.0, volvol=0.2)
+    params_max = params_max or LogSvParams(sigma0=1.5, theta=1.5, kappa1=10.0, kappa2=10.0, beta=3.0, volvol=3.0)
     vol_scaler = pricer.set_vol_scaler(option_chain=option_chain)
-    _, market_vols_ttms = option_chain.get_chain_data_as_xy()
-    market_vols = to_flat_np_array(market_vols_ttms)
-    weights = calibration_weights(option_chain, market_vols, is_vega_weighted, is_unit_ttm_vega)
+    market_vols, weights = market_and_weights(option_chain, is_vega_weighted, is_unit_ttm_vega)
     varswap_strikes = (option_chain.get_slice_varswap_strikes(floor_with_atm_vols=True)
                        if model_calibration_type == LogsvModelCalibrationType.PARAMS_WITH_VARSWAP_FIT else None)
     codec = LogSvParameterCodec(params0, params_min, params_max, model_calibration_type, varswap_strikes)
@@ -535,7 +550,7 @@ def calibrate_logsv(pricer, option_chain, params0, params_min, params_max, is_ve
     x, result = run_slsqp(objective, p0, bounds, build_logsv_constraints(codec, constraints_type), disp=disp)
     fit = codec.parse(x)
     if return_info:
-        info = {"fun": float(result.fun), "nit": int(result.nit), "nb_batches": objective.nb_batches, "x": x, "nan_quotes": objective.nan_quotes}
+        info = fit_info(result, x, objective, nan_quotes=objective.nan_quotes)
         if gradient == "pathwise" and calibration_engine == CalibrationEngine.ROUGH_MC:
             info["reset_paths"] = resets
         return fit, info
@@ -560,9 +575,7 @@ def calibrate_heston(pricer, option_chain, params0, is_vega_weighted: bool, is_u
     check_gradient(gradient)
     p0 = (np.array([params0.v0, params0.theta, params0.kappa, params0.rho, params0.volvol], dtype=float) if params0 is not None
           else np.array([0.1, 0.1, 2.0, -0.2, 1.0]))
-    _, market_vols_ttms = option_chain.get_chain_data_as_xy()
-    market_vols = to_flat_np_array(market_vols_ttms)
-    weights = calibration_weights(option_chain, market_vols, is_vega_weighted, is_unit_ttm_vega)
+    market_vols, weights = market_and_weights(option_chain, is_vega_weighted, is_unit_ttm_vega)
 
     if gradient == "exact":
         # the grid is pinned at the start point's default scaler; the difference route re-grids every set (the default depends on v0)
@@ -589,9 +602,113 @@ def calibrate_heston(pricer, option_chain, params0, is_vega_weighted: bool, is_u
                                      eps=fd_step or SLSQP_EPS)
     x, result = run_slsqp(objective, p0, HESTON_BOUNDS, {"type": "ineq", "fun": feller}, disp=disp)
     fit = HestonParams(v0=x[0], theta=x[1], kappa=x[2], rho=x[3], volvol=x[4])
-    if return_info:
-        return fit, {"fun": float(result.fun), "nit": int(result.nit), "nb_batches": objective.nb_batches, "x": x}
-    return fit
+    return (fit, fit_info(result, x, objective)) if return_info else fit
+
+
+# ---- Hawkes jump-diffusion --------------------------------------------------------------------------------------------------
+def calibrate_hawkes(pricer, option_chain, params0, is_vega_weighted: bool, is_unit_ttm_vega: bool, return_info: bool = False,
+                     price_batch: Optional[Callable] = None, **kwargs):
+    """HawkesJDPricer.calibrate_model_params_to_chain (reference hawkes_jd_pricer.py:230-300).  ``price_batch``: what the difference
+    objective prices its points with, engine.hawkesjd_price_chain_batch (None) or a callable with its arguments and return value, as for
+    calibrate_logsv"""
+    from .hawkes_jd_pricer import HawkesJDParams, set_vol_scaler
+    gradient = check_gradient(kwargs.get("gradient", "difference"))
+    p0 = np.array([params0.sigma, params0.mean_p, params0.mean_m, params0.theta_p, params0.theta_m, 0.5 * (params0.kappa_p + params0.kappa_m),
+                   0.5 * (params0.beta1_p - params0.beta2_p), 0.5 * (params0.beta2_p - params0.beta2_m)])
+    bounds = ((0.10, 2.0), (0.01, 0.99), (-0.99, -0.01), (0.01, 100.0), (0.01, 100.0), (1.0, 100.0), (1.0, 100.0), (1.0, 100.0))
+
+    def unpack(x: np.ndarray):
+        return HawkesJDParams(mu=0.0, sigma=x[0], shift_p=params0.shift_p, mean_p=x[1], shift_m=params0.shift_m, mean_m=x[2],
+                              lambda_p=params0.lambda_p, theta_p=x[3], kappa_p=x[5], beta1_p=x[6], beta2_p=-x[6], lambda_m=params0.lambda_m,
+                              theta_m=x[4], kappa_m=x[5], beta1_m=x[7], beta2_m=-x[7])
+
+    stationary = {"type": "ineq", "fun": lambda x: unpack(x).jump1_cond + unpack(x).jump2_cond}
+    if gradient == "exact":
+        objective = _exact_vol_objective(pricer, option_chain, unpack, is_vega_weighted, is_unit_ttm_vega,
+                                         set_vol_scaler(params0.sigma, float(option_chain.ttms[0])))
+    else:
+        objective = _batched_vol_objective(option_chain, unpack, is_vega_weighted, is_unit_ttm_vega, bounds, SLSQP_EPS,
+                                           price_batch=price_batch)
+    x, result = run_slsqp(objective, p0, bounds, stationary, disp=bool(kwargs.get("disp", False)), validate=False,
+                          **({"maxiter": int(kwargs["maxiter"])} if "maxiter" in kwargs else {}))
+    fit = unpack(x)
+    return (fit, fit_info(result, x, objective, nan_quotes=objective.nan_quotes)) if return_info else fit
+
+
+def calibrate_hawkes_risk_premia(option_chain, params0, is_vega_weighted: bool, is_unit_ttm_vega: bool, maxiter: int = 100,
+                                 print_iter: bool = True, return_info: bool = False, **kwargs):
+    """HawkesJDPricer.calibrate_risk_premia_gamma_to_chain (reference hawkes_jd_pricer.py:303-357): (sigma, gamma / 8) with the rest of
+    ``params0`` fixed, weights x 1e4, SLSQP with difference step 0.025 and ftol = tol = 1e-16"""
+    from .hawkes_jd_pricer import _KEYS, HawkesJDParams
+    if check_gradient(kwargs.get("gradient", "difference")) == "exact":
+        raise NotImplementedError("gradient='exact' does not cover calibrate_risk_premia_gamma_to_chain: the risk-kernel pricer has no "
+                                  "sensitivities")
+    gamma_scaler = 8.0
+    fixed = {k: v for k, v in params0.to_dict().items() if k in _KEYS}
+    bounds = ((0.01, 1.5), (-1.0, 1.0))
+
+    def announce(x: np.ndarray) -> None:
+        print(f"unpack_pars: sigma={x[0]}, gamma={gamma_scaler * x[1]}")
+
+    def to_params(x: np.ndarray):
+        return HawkesJDParams(**{**fixed, "sigma": float(x[0])}, risk_premia_gamma=float(gamma_scaler * x[1]))
+
+    p0 = np.array([params0.sigma, (params0.risk_premia_gamma or 0.0) / gamma_scaler])
+    objective = _batched_vol_objective(option_chain, to_params, is_vega_weighted, is_unit_ttm_vega, bounds, 0.025, scale=10000.0,
+                                       on_point=announce if print_iter else None)
+    x, result = run_slsqp(objective, p0, bounds, disp=bool(kwargs.get("disp", False)), tol=1e-16, validate=False, ftol=1e-16,
+                          maxiter=maxiter, eps=0.025)
+    if print_iter:
+        announce(x)
+    fit = to_params(x)
+    return (fit, fit_info(result, x, objective, nan_quotes=objective.nan_quotes)) if return_info else fit
+
+
+# d HAWKES_GREEK_PARAMS / d x of calibrate_hawkes's x = (sigma, mean_p, mean_m, theta_p, theta_m, kappa, beta_p, beta_m): kappa feeds
+# kappa_p and kappa_m, beta_p feeds beta1_p = +x and beta2_p = -x, beta_m feeds beta1_m = +x and beta2_m = -x
+_HAWKES_FIT_FIELDS = ((("sigma", 1.0),), (("mean_p", 1.0),), (("mean_m", 1.0),), (("theta_p", 1.0),), (("theta_m", 1.0),),
+                      (("kappa_p", 1.0), ("kappa_m", 1.0)), (("beta1_p", 1.0), ("beta2_p", -1.0)), (("beta1_m", 1.0), ("beta2_m", -1.0)))
+
+
+def hawkes_fit_jacobian() -> np.ndarray:
+    D = np.zeros((len(engine.HAWKES_GREEK_PARAMS), len(_HAWKES_FIT_FIELDS)))
+    for col, fields in enumerate(_HAWKES_FIT_FIELDS):
+        for name, sign in fields:
+            D[engine.HAWKES_GREEK_PARAMS.index(name), col] = sign
+    return D
+
+
+def _exact_vol_objective(pricer, option_chain, to_params, is_vega_weighted: bool, is_unit_ttm_vega: bool,
+                         vol_scaler: float) -> ExactGradientObjective:
+    """the Hawkes objective with its exact gradient: one compute_chain_ivol_greeks call per point on the grid of ``vol_scaler``"""
+    market, weights = market_and_weights(option_chain, is_vega_weighted, is_unit_ttm_vega, slice_sum=np.sum)
+    D = hawkes_fit_jacobian()
+
+    def ivol_greeks(x: np.ndarray):
+        sens = pricer.compute_chain_ivol_greeks(option_chain, to_params(x), vol_scaler=vol_scaler)
+        return flat_ivol_rows(sens, engine.HAWKES_GREEK_PARAMS)
+    return ExactGradientObjective(ivol_greeks=ivol_greeks, field_jacobian=lambda x: D, market_vols=market, weights=weights)
+
+
+def _batched_vol_objective(option_chain, to_params, is_vega_weighted: bool, is_unit_ttm_vega: bool, bounds, eps: float,
+                           scale: float = 1.0, on_point=None, price_batch=None) -> ScipyDifferenceObjective:
+    """the Hawkes drivers' objective: weighted squared difference of model and mid implied vols, nansum over the chain (quotes whose model
+    price leaves the no-arbitrage bounds drop out), with the weights of the reference (per-slice normalised vegas, times ``scale``).  The
+    model vols of a point, and of its difference neighbours together, come from hawkesjd_price_chain_batch, on the risk-kernel route when
+    the parameter sets carry a risk_premia_gamma -- the same prices and vols as compute_model_ivols_for_chain per set.  ``price_batch``: a
+    callable with hawkesjd_price_chain_batch's arguments and return value in its place (the lock-step driver)."""
+    from .hawkes_jd_pricer import MAX_PHI, _params_c
+    market, weights = market_and_weights(option_chain, is_vega_weighted, is_unit_ttm_vega, slice_sum=np.sum)
+
+    def batch_vols(points: np.ndarray) -> np.ndarray:
+        sets = [to_params(p) for p in points]
+        gammas = None if sets[0].risk_premia_gamma is None else [s.risk_premia_gamma for s in sets]
+        _, ivols = (price_batch or engine.hawkesjd_price_chain_batch)([_params_c(**s.to_dict()) for s in sets], option_chain.ttms,
+                                                                      option_chain.forwards, option_chain.discfactors, option_chain.strikes_ttms,
+                                                                      option_chain.optiontypes_ttms, max_phi=MAX_PHI, gammas=gammas)
+        return ivols
+    return ScipyDifferenceObjective(batch_vols=batch_vols, market_vols=market, weights=scale * weights, bounds=bounds, eps=eps,
+                                    on_point=on_point)
 
 
 # ---- several chains in lock-step ------------------------------------------------------------------------------------------------
@@ -680,31 +797,52 @@ def _pack(posted: dict, max_sets_per_call: Optional[int]) -> List[List[int]]:
     return calls
 
 
-def calibrate_chains_lockstep(fit: Callable[[int, Callable], object], n: int, price_call: Callable, max_sets_per_call: Optional[int],
-                              return_exceptions: bool):
-    """K = n single-chain fits in lock-step.  ``fit(k, price_batch)`` runs fit k (calibrate_logsv / calibrate_heston with ``price_batch``
-    injected and ``return_info=True``) and returns its (fit, info); ``price_call(requests) -> [ivols [B_i, J_i]]`` prices the requests
-    (price_batch's positional arguments, keyword arguments) of several fits in one library call.  Each fit runs in a thread of its own; the caller's thread, whose
-    CUDA stream the library calls keep (b200sv_set_stream is per thread), prices every round and waits for all threads before it returns.
-    -> (fits, infos), ``rounds`` (library calls of the whole run) added to every info dict; a failed fit's slot holds its exception (info
-    None) with ``return_exceptions``, else the lowest-index exception is raised."""
+def calibrate_chains_lockstep(fit: Callable, option_chains, price_chains: Callable, gradient: str, max_sets_per_call: Optional[int],
+                              return_exceptions: bool, return_info: bool, extras: Optional[Callable] = None, **per_chain_args):
+    """one single-chain fit per chain of ``option_chains``, in lock-step.  Before any library call: ``gradient`` ('difference' only),
+    ``option_chains`` (not empty), ``max_sets_per_call`` (None or at least 1), then per_chain on each of ``per_chain_args`` in turn.
+    ``fit(option_chain, price_batch, **args)`` runs the fit of one chain on its values of ``per_chain_args`` (calibrate_logsv /
+    calibrate_heston / calibrate_hawkes with ``price_batch`` injected and ``return_info=True``) and returns its (fit, info).  The requests
+    of the fits priced together -- price_batch's (positional arguments, keyword arguments) -- go to ``price_chains(params, chain_of_set,
+    chains, *args, **kwargs)``, the model's engine.*_price_chains_batch, with each fit's sets, its chain's arrays and ``(args, kwargs) =
+    extras(requests)``, the model's other arguments (none without ``extras``).  Each fit runs in a thread of its own; the caller's thread,
+    whose CUDA stream the library calls keep (b200sv_set_stream is per thread), prices every round and waits for all threads before it
+    returns.  -> the fits, with ``return_info`` (fits, infos) whose info dicts add ``rounds`` (library calls of the whole run); a failed
+    fit's slot holds its exception (info None) with ``return_exceptions``, else the lowest-index exception is raised."""
+    if gradient != "difference":
+        if gradient in GRADIENTS:
+            raise NotImplementedError(f"calibrate_model_params_to_chains has gradient='difference' only, not {gradient!r}")
+        check_gradient(gradient)
+    n = len(option_chains)
+    if n == 0:
+        raise ValueError("option_chains is empty")
+    if max_sets_per_call is not None and int(max_sets_per_call) < 1:
+        raise ValueError("max_sets_per_call must be at least 1")
+    columns = {name: per_chain(value, n, name) for name, value in per_chain_args.items()}
     lock = _LockStep(n)
     results = [None] * n
 
     def run(k: int) -> None:
         try:
-            results[k] = fit(k, lambda *args, **kw: (None, lock.post(k, (args[0], args, kw))))
+            results[k] = fit(option_chains[k], lambda *args, **kw: (None, lock.post(k, (args[0], args, kw))),
+                             **{name: values[k] for name, values in columns.items()})
         except BaseException as exc:                  # noqa: BLE001 (reported per chain below)
             results[k] = exc
         finally:
             lock.leave()
 
     def price_round(posted: dict):
-        answers = {}
-        calls = _pack(posted, max_sets_per_call)
+        answers, calls = {}, _pack(posted, max_sets_per_call)
         for ks in calls:
-            for k, rows in zip(ks, price_call([posted[k][1:] for k in ks])):
-                answers[k] = rows
+            params, chain_of_set, chains = [], [], []
+            for i, k in enumerate(ks):
+                c = option_chains[k]                  # the arrays fit k hands price_batch
+                params += list(posted[k][0])
+                chain_of_set += [i] * len(posted[k][0])
+                chains.append((c.ttms, c.forwards, c.discfactors, c.strikes_ttms, c.optiontypes_ttms))
+            args, kw = extras([posted[k][1:] for k in ks]) if extras is not None else ((), {})
+            _, ivols = price_chains(params, chain_of_set, chains, *args, **kw)
+            answers.update(zip(ks, _rows_by_request(ivols, chain_of_set, len(ks))))
         return answers, len(calls)
 
     threads = [threading.Thread(target=run, args=(k,), name=f"calibrate-chain-{k}") for k in range(n)]
@@ -719,15 +857,10 @@ def calibrate_chains_lockstep(fit: Callable[[int, Callable], object], n: int, pr
         for r in results:
             if isinstance(r, BaseException):
                 raise r
-    fits, infos = [], []
-    for r in results:
-        if isinstance(r, BaseException):
-            fits.append(r)
-            infos.append(None)
-        else:
-            fits.append(r[0])
-            infos.append(dict(r[1], rounds=rounds))
-    return fits, infos
+    fits = [r if isinstance(r, BaseException) else r[0] for r in results]
+    if not return_info:
+        return fits
+    return fits, [None if isinstance(r, BaseException) else dict(r[1], rounds=rounds) for r in results]
 
 
 def per_chain(value, n: int, name: str) -> list:
@@ -739,80 +872,55 @@ def per_chain(value, n: int, name: str) -> list:
     return [value] * n
 
 
-def check_lockstep_args(option_chains, max_sets_per_call, gradient: str) -> int:
-    """the checks every lock-step driver makes before any library call -> the number of chains"""
-    if gradient != "difference":
-        if gradient in GRADIENTS:
-            raise NotImplementedError(f"calibrate_model_params_to_chains has gradient='difference' only, not {gradient!r}")
-        check_gradient(gradient)
-    n = len(option_chains)
-    if n == 0:
-        raise ValueError("option_chains is empty")
-    if max_sets_per_call is not None and int(max_sets_per_call) < 1:
-        raise ValueError("max_sets_per_call must be at least 1")
-    return n
-
-
 def calibrate_logsv_chains(pricer, option_chains, params0, params_min, params_max, is_vega_weighted: bool, is_unit_ttm_vega: bool,
                            model_calibration_type: LogsvModelCalibrationType, constraints_type: ConstraintsType,
                            calibration_engine: CalibrationEngine, is_spot_measure: bool = True, disp: bool = False, return_info: bool = False,
                            fd_step: Optional[float] = None, gradient: str = "difference", return_exceptions: bool = False,
                            max_sets_per_call: Optional[int] = None):
     """calibrate_logsv on every chain, ANALYTIC engine, in lock-step: one engine.logsv_price_chains_batch call per optimizer round"""
-    n = check_lockstep_args(option_chains, max_sets_per_call, gradient)
     if calibration_engine != CalibrationEngine.ANALYTIC:
         raise NotImplementedError(f"calibrate_model_params_to_chains covers CalibrationEngine.ANALYTIC only, not {calibration_engine}")
     if model_calibration_type not in (LogsvModelCalibrationType.PARAMS4, LogsvModelCalibrationType.PARAMS5,
                                       LogsvModelCalibrationType.PARAMS_WITH_VARSWAP_FIT):
         raise NotImplementedError(f"{model_calibration_type}")
-    p0s, los, his = (per_chain(v, n, name) for v, name in ((params0, "params0"), (params_min, "params_min"), (params_max, "params_max")))
 
-    def fit(k: int, price_batch):
-        return calibrate_logsv(pricer, option_chains[k], p0s[k], los[k], his[k], is_vega_weighted, is_unit_ttm_vega, model_calibration_type,
+    def fit(option_chain, price_batch, params0, params_min, params_max):
+        return calibrate_logsv(pricer, option_chain, params0, params_min, params_max, is_vega_weighted, is_unit_ttm_vega, model_calibration_type,
                                constraints_type, calibration_engine, 0, 0, 0,          # nb_path, nb_steps, seed: Monte Carlo engines only
-                               is_spot_measure=is_spot_measure, disp=disp, return_info=True,
-                               fd_step=fd_step, price_batch=price_batch)
+                               is_spot_measure=is_spot_measure, disp=disp, return_info=True, fd_step=fd_step, price_batch=price_batch)
 
-    def price_call(requests):
-        # request = (args, kwargs) of engine.logsv_price_chain_batch(params_list, ttms, forwards, discfactors, etas, strikes, types, ...)
-        params, chain_of_set, chains, etas, scalers = [], [], [], [], []
-        for i, (args, kw) in enumerate(requests):
-            sets, ttms, forwards, discfactors, e, strikes_ttms, optiontypes_ttms = args
-            params += list(sets)
-            chain_of_set += [i] * len(sets)
-            chains.append((ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms))
-            etas += list(e)
-            scalers.append(kw["vol_scaler"])
-        _, ivols = engine.logsv_price_chains_batch(params, chain_of_set, chains, etas, scalers, is_spot_measure=is_spot_measure)
-        return _rows_by_request(ivols, chain_of_set, len(requests))
+    def extras(requests):
+        # request = (args, kwargs) of engine.logsv_price_chain_batch(params_list, ttms, forwards, discfactors, etas, strikes, types, ...,
+        # vol_scaler=): the eta row of every set, the grid scaler of every chain
+        return ([row for args, _ in requests for row in args[4]], [kw["vol_scaler"] for _, kw in requests]), {"is_spot_measure": is_spot_measure}
 
-    out = calibrate_chains_lockstep(fit, n, price_call, max_sets_per_call, return_exceptions)
-    return out if return_info else out[0]
+    return calibrate_chains_lockstep(fit, option_chains, engine.logsv_price_chains_batch, gradient, max_sets_per_call, return_exceptions,
+                                     return_info, extras, params0=params0, params_min=params_min, params_max=params_max)
 
 
 def calibrate_heston_chains(pricer, option_chains, params0, is_vega_weighted: bool, is_unit_ttm_vega: bool, disp: bool = False,
                             return_info: bool = False, fd_step: Optional[float] = None, gradient: str = "difference",
                             return_exceptions: bool = False, max_sets_per_call: Optional[int] = None):
     """calibrate_heston on every chain in lock-step: one engine.heston_price_chains_batch call per optimizer round"""
-    n = check_lockstep_args(option_chains, max_sets_per_call, gradient)
-    p0s = per_chain(params0, n, "params0")
-
-    def fit(k: int, price_batch):
-        return calibrate_heston(pricer, option_chains[k], p0s[k], is_vega_weighted, is_unit_ttm_vega, disp=disp, return_info=True,
+    def fit(option_chain, price_batch, params0):
+        return calibrate_heston(pricer, option_chain, params0, is_vega_weighted, is_unit_ttm_vega, disp=disp, return_info=True,
                                 fd_step=fd_step, price_batch=price_batch)
 
-    def price_call(requests):
-        # request = (args, kwargs) of engine.heston_price_chain_batch(params_list, ttms, forwards, discfactors, strikes, types)
-        params, chain_of_set, chains = [], [], []
-        for i, (args, _) in enumerate(requests):
-            params += list(args[0])
-            chain_of_set += [i] * len(args[0])
-            chains.append(tuple(args[1:6]))
-        _, ivols = engine.heston_price_chains_batch(params, chain_of_set, chains)
-        return _rows_by_request(ivols, chain_of_set, len(requests))
+    return calibrate_chains_lockstep(fit, option_chains, engine.heston_price_chains_batch, gradient, max_sets_per_call, return_exceptions,
+                                     return_info, params0=params0)
 
-    out = calibrate_chains_lockstep(fit, n, price_call, max_sets_per_call, return_exceptions)
-    return out if return_info else out[0]
+
+def calibrate_hawkes_chains(pricer, option_chains, params0, is_vega_weighted: bool, is_unit_ttm_vega: bool, return_info: bool = False,
+                            gradient: str = "difference", return_exceptions: bool = False, max_sets_per_call: Optional[int] = None, **kwargs):
+    """calibrate_hawkes on every chain in lock-step: one engine.hawkesjd_price_chains_batch call per optimizer round"""
+    from .hawkes_jd_pricer import MAX_PHI
+
+    def fit(option_chain, price_batch, params0):
+        return calibrate_hawkes(pricer, option_chain, params0, is_vega_weighted, is_unit_ttm_vega, return_info=True, price_batch=price_batch,
+                                **kwargs)
+
+    return calibrate_chains_lockstep(fit, option_chains, engine.hawkesjd_price_chains_batch, gradient, max_sets_per_call, return_exceptions,
+                                     return_info, lambda requests: ((), {"max_phi": MAX_PHI}), params0=params0)
 
 
 def _rows_by_request(ivols, chain_of_set, n: int) -> List[np.ndarray]:

@@ -7,7 +7,7 @@
 * ``HawkesJDPricer.price_chain``              (:125-155) -> ``hawkesjd_chain_pricer`` (:365-417) / ``hawkesjd_chain_pricer_with_risk_premia`` (:420-484),
   ``hawkesjd_forwards_under_risk_kernel`` (:487-515), ``compute_hawkes_a_mgf_grid`` / ``solve_a_ode_grid`` (:518-579)
 * ``HawkesJDPricer.calibrate_model_params_to_chain`` (:230-300), ``calibrate_risk_premia_gamma_to_chain`` (:303-357): host SLSQP loops around the
-  batched GPU chain pricer (``b200sv_hawkesjd_price_chain_batch``), fits bit-identical to SLSQP differencing the one-set objective
+  batched GPU chain pricer (``b200sv_hawkesjd_price_chain_batch``), fits bit-identical to SLSQP differencing the one-set objective (pricers/calibration.py)
 
 Monte Carlo: the reference draws every random input from numpy's process-global generator; here they are drawn in-kernel from the Philox
 stream keyed by an explicit ``seed`` (default: the ``set_seed`` stream or OS entropy).  ``simulate_hawkesjd_terminal`` additionally accepts the five
@@ -28,8 +28,8 @@ from ..data.option_chain import OptionChain
 from ..multi_gpu import _shared_seed, _use_distributed, mc_chain_distributed
 from ..utils.config import VariableType
 from ..utils.funcs import set_time_grid, timer
-from .calibration import (SLSQP_EPS, ExactGradientObjective, ScipyDifferenceObjective, _rows_by_request, calibrate_chains_lockstep,
-                          check_gradient, check_lockstep_args, flat_ivol_rows, per_chain)
+from .calibration import calibrate_hawkes, calibrate_hawkes_chains, calibrate_hawkes_risk_premia
+from .calibration import _batched_vol_objective, hawkes_fit_jacobian  # noqa: F401  (imported from this module by callers)
 from .model_pricer import ModelParams, ModelPricer
 
 _KEYS = tuple(k for k, _ in C.HawkesParamsC._fields_)
@@ -200,32 +200,8 @@ class HawkesJDPricer(ModelPricer):
         call, with the fit of the one-set objective bit for bit; ``print_iter`` prints a line per point in the order that objective would (the neighbours
         only when SLSQP asks for the gradient).  ``return_info``: (fit, {"fun", "nit", "nb_batches", "x", "nan_quotes"}).  The risk kernel
         has no sensitivities, so ``gradient='exact'`` raises NotImplementedError."""
-        from scipy.optimize import minimize
-        if check_gradient(kwargs.get("gradient", "difference")) == "exact":
-            raise NotImplementedError("gradient='exact' does not cover calibrate_risk_premia_gamma_to_chain: the risk-kernel pricer has no "
-                                      "sensitivities")
-        gamma_scaler = 8.0
-        fixed = {k: v for k, v in params0.to_dict().items() if k in _KEYS}
-        bounds = ((0.01, 1.5), (-1.0, 1.0))
-
-        def announce(x: np.ndarray) -> None:
-            print(f"unpack_pars: sigma={x[0]}, gamma={gamma_scaler * x[1]}")
-
-        def to_params(x: np.ndarray) -> HawkesJDParams:
-            return HawkesJDParams(**{**fixed, "sigma": float(x[0])}, risk_premia_gamma=float(gamma_scaler * x[1]))
-
-        p0 = np.array([params0.sigma, (params0.risk_premia_gamma or 0.0) / gamma_scaler])
-        objective = _batched_vol_objective(option_chain, to_params, is_vega_weighted, is_unit_ttm_vega, bounds, 0.025, scale=10000.0,
-                                           on_point=announce if print_iter else None)
-        res = minimize(objective.fun, p0, args=None, method="SLSQP", jac=objective.jac, bounds=bounds,
-                       options={"disp": bool(kwargs.get("disp", False)), "ftol": 1e-16, "maxiter": maxiter, "eps": 0.025}, tol=1e-16)
-        if print_iter:
-            announce(res.x)
-        fit = to_params(res.x)
-        if return_info:
-            return fit, {"fun": float(res.fun), "nit": int(res.nit), "nb_batches": objective.nb_batches, "x": res.x,
-                         "nan_quotes": objective.nan_quotes}
-        return fit
+        return calibrate_hawkes_risk_premia(option_chain, params0, is_vega_weighted, is_unit_ttm_vega, maxiter=maxiter, print_iter=print_iter,
+                                            return_info=return_info, **kwargs)
 
     @timer
     def simulate_terminal_values(self, params: HawkesJDParams, ttm: float = 1.0, nb_path: int = 100000, is_spot_measure: bool = True, **kwargs
@@ -295,64 +271,6 @@ def set_vol_scaler(sigma0: float, ttm: float) -> float:
     return float(np.clip(sigma0, 0.2, 0.5) * np.sqrt(np.minimum(ttm, 1.0 / 12.0)))
 
 
-def calibrate_hawkes(pricer, option_chain: OptionChain, params0: HawkesJDParams, is_vega_weighted: bool, is_unit_ttm_vega: bool,
-                     return_info: bool = False, price_batch=None, **kwargs):
-    """HawkesJDPricer.calibrate_model_params_to_chain.  ``price_batch``: what the difference objective prices its points with,
-    engine.hawkesjd_price_chain_batch (None) or a callable with its arguments and return value (calibrate_hawkes_chains)"""
-    from scipy.optimize import minimize
-    gradient = check_gradient(kwargs.get("gradient", "difference"))
-    p0 = np.array([params0.sigma, params0.mean_p, params0.mean_m, params0.theta_p, params0.theta_m, 0.5 * (params0.kappa_p + params0.kappa_m),
-                   0.5 * (params0.beta1_p - params0.beta2_p), 0.5 * (params0.beta2_p - params0.beta2_m)])
-    bounds = ((0.10, 2.0), (0.01, 0.99), (-0.99, -0.01), (0.01, 100.0), (0.01, 100.0), (1.0, 100.0), (1.0, 100.0), (1.0, 100.0))
-
-    def unpack(x: np.ndarray) -> HawkesJDParams:
-        return HawkesJDParams(mu=0.0, sigma=x[0], shift_p=params0.shift_p, mean_p=x[1], shift_m=params0.shift_m, mean_m=x[2],
-                              lambda_p=params0.lambda_p, theta_p=x[3], kappa_p=x[5], beta1_p=x[6], beta2_p=-x[6], lambda_m=params0.lambda_m,
-                              theta_m=x[4], kappa_m=x[5], beta1_m=x[7], beta2_m=-x[7])
-
-    stationary = {"type": "ineq", "fun": lambda x: unpack(x).jump1_cond + unpack(x).jump2_cond}
-    options = {"disp": bool(kwargs.get("disp", False)), "ftol": 1e-8}
-    if "maxiter" in kwargs:
-        options["maxiter"] = int(kwargs["maxiter"])
-    if gradient == "exact":
-        objective = _exact_vol_objective(pricer, option_chain, unpack, is_vega_weighted, is_unit_ttm_vega,
-                                         set_vol_scaler(params0.sigma, float(option_chain.ttms[0])))
-    else:
-        objective = _batched_vol_objective(option_chain, unpack, is_vega_weighted, is_unit_ttm_vega, bounds, SLSQP_EPS,
-                                           price_batch=price_batch)
-    res = minimize(objective.fun, p0, args=None, method="SLSQP", jac=objective.jac, constraints=stationary, bounds=bounds, options=options)
-    fit = unpack(res.x)
-    if return_info:
-        return fit, {"fun": float(res.fun), "nit": int(res.nit), "nb_batches": objective.nb_batches, "x": res.x,
-                     "nan_quotes": objective.nan_quotes}
-    return fit
-
-
-def calibrate_hawkes_chains(pricer, option_chains, params0, is_vega_weighted: bool, is_unit_ttm_vega: bool, return_info: bool = False,
-                            gradient: str = "difference", return_exceptions: bool = False, max_sets_per_call: Optional[int] = None, **kwargs):
-    """calibrate_hawkes on every chain in lock-step: one engine.hawkesjd_price_chains_batch call per optimizer round"""
-    n = check_lockstep_args(option_chains, max_sets_per_call, gradient)
-    p0s = per_chain(params0, n, "params0")
-
-    def fit(k: int, price_batch):
-        return calibrate_hawkes(pricer, option_chains[k], p0s[k], is_vega_weighted, is_unit_ttm_vega, return_info=True, price_batch=price_batch,
-                                **kwargs)
-
-    def price_call(requests):
-        # request = (args, kwargs) of engine.hawkesjd_price_chain_batch(params_list, ttms, forwards, discfactors, strikes, types,
-        # max_phi=MAX_PHI, gammas=None)
-        params, chain_of_set, chains = [], [], []
-        for i, (args, _) in enumerate(requests):
-            params += list(args[0])
-            chain_of_set += [i] * len(args[0])
-            chains.append(tuple(args[1:6]))
-        _, ivols = engine.hawkesjd_price_chains_batch(params, chain_of_set, chains, max_phi=MAX_PHI)
-        return _rows_by_request(ivols, chain_of_set, len(requests))
-
-    out = calibrate_chains_lockstep(fit, n, price_call, max_sets_per_call, return_exceptions)
-    return out if return_info else out[0]
-
-
 def _fourier_chain(model_params: HawkesJDParams, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, is_stiff_solver, is_spot_measure,
                    variable_type, vol_scaler, gamma, return_grids=False):
     if getattr(variable_type, "value", variable_type) != VariableType.LOG_RETURN.value:
@@ -367,62 +285,6 @@ def _fourier_chain(model_params: HawkesJDParams, ttms, forwards, discfactors, st
     d.pop("risk_premia_gamma", None)
     return engine.hawkesjd_price_chain(_params_c(**d), ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, is_spot_measure, vol_scaler,
                                        MAX_PHI, gamma, return_grids)
-
-
-def _market_and_weights(option_chain: OptionChain, is_vega_weighted: bool, is_unit_ttm_vega: bool):
-    """(mid vols, objective weights) flat in chain order: per-slice normalised vegas, or ones"""
-    market = np.concatenate([np.asarray(v, dtype=float) for v in option_chain.get_mid_vols()])
-    if is_vega_weighted:
-        weights = np.concatenate([v / np.sum(v) for v in option_chain.get_chain_vegas(is_unit_ttm_vega=is_unit_ttm_vega)])
-    else:
-        weights = np.ones_like(market)
-    return market, weights
-
-
-# d HAWKES_GREEK_PARAMS / d x of calibrate_model_params_to_chain's x = (sigma, mean_p, mean_m, theta_p, theta_m, kappa, beta_p, beta_m):
-# kappa feeds kappa_p and kappa_m, beta_p feeds beta1_p = +x and beta2_p = -x, beta_m feeds beta1_m = +x and beta2_m = -x
-_HAWKES_FIT_FIELDS = ((("sigma", 1.0),), (("mean_p", 1.0),), (("mean_m", 1.0),), (("theta_p", 1.0),), (("theta_m", 1.0),),
-                      (("kappa_p", 1.0), ("kappa_m", 1.0)), (("beta1_p", 1.0), ("beta2_p", -1.0)), (("beta1_m", 1.0), ("beta2_m", -1.0)))
-
-
-def hawkes_fit_jacobian() -> np.ndarray:
-    D = np.zeros((len(engine.HAWKES_GREEK_PARAMS), len(_HAWKES_FIT_FIELDS)))
-    for col, fields in enumerate(_HAWKES_FIT_FIELDS):
-        for name, sign in fields:
-            D[engine.HAWKES_GREEK_PARAMS.index(name), col] = sign
-    return D
-
-
-def _exact_vol_objective(pricer, option_chain: OptionChain, to_params, is_vega_weighted: bool, is_unit_ttm_vega: bool,
-                         vol_scaler: float) -> ExactGradientObjective:
-    """the same objective with its exact gradient: one compute_chain_ivol_greeks call per point on the grid of ``vol_scaler``"""
-    market, weights = _market_and_weights(option_chain, is_vega_weighted, is_unit_ttm_vega)
-    D = hawkes_fit_jacobian()
-
-    def ivol_greeks(x: np.ndarray):
-        sens = pricer.compute_chain_ivol_greeks(option_chain, to_params(x), vol_scaler=vol_scaler)
-        return flat_ivol_rows(sens, engine.HAWKES_GREEK_PARAMS)
-    return ExactGradientObjective(ivol_greeks=ivol_greeks, field_jacobian=lambda x: D, market_vols=market, weights=weights)
-
-
-def _batched_vol_objective(option_chain: OptionChain, to_params, is_vega_weighted: bool, is_unit_ttm_vega: bool, bounds, eps: float,
-                           scale: float = 1.0, on_point=None, price_batch=None) -> ScipyDifferenceObjective:
-    """the drivers' objective: weighted squared difference of model and mid implied vols, nansum over the chain (quotes whose model price
-    leaves the no-arbitrage bounds drop out), with the weights of the reference (per-slice normalised vegas, times ``scale``).  The model vols
-    of a point, and of its difference neighbours together, come from hawkesjd_price_chain_batch, on the risk-kernel route when the
-    parameter sets carry a risk_premia_gamma -- the same prices and vols as compute_model_ivols_for_chain per set.  ``price_batch``: a callable
-    with hawkesjd_price_chain_batch's arguments and return value in its place (the lock-step driver)."""
-    market, weights = _market_and_weights(option_chain, is_vega_weighted, is_unit_ttm_vega)
-
-    def batch_vols(points: np.ndarray) -> np.ndarray:
-        sets = [to_params(p) for p in points]
-        gammas = None if sets[0].risk_premia_gamma is None else [s.risk_premia_gamma for s in sets]
-        _, ivols = (price_batch or engine.hawkesjd_price_chain_batch)([_params_c(**s.to_dict()) for s in sets], option_chain.ttms,
-                                                                      option_chain.forwards, option_chain.discfactors, option_chain.strikes_ttms,
-                                                                      option_chain.optiontypes_ttms, max_phi=MAX_PHI, gammas=gammas)
-        return ivols
-    return ScipyDifferenceObjective(batch_vols=batch_vols, market_vols=market, weights=scale * weights, bounds=bounds, eps=eps,
-                                    on_point=on_point)
 
 
 def hawkesjd_chain_pricer(model_params: HawkesJDParams, ttms: np.ndarray, forwards: np.ndarray, discfactors: np.ndarray, strikes_ttms, optiontypes_ttms,

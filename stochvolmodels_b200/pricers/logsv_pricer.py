@@ -225,8 +225,6 @@ class LogSVPricer(ModelPricer):
         of the sample objective, not of the model.  A ROUGH_MC pathwise fit's ``return_info`` adds ``reset_paths``: per maturity, the most
         paths any evaluation saw take the reset-to-1e-6 branch; where it is non-zero the gradient misses the mass those paths move across
         that switch."""
-        params_min = params_min or LogSvParams(sigma0=0.1, theta=0.1, kappa1=0.25, kappa2=0.25, beta=-3.0, volvol=0.2)
-        params_max = params_max or LogSvParams(sigma0=1.5, theta=1.5, kappa1=10.0, kappa2=10.0, beta=3.0, volvol=3.0)
         return calibrate_logsv(self, option_chain, params0, params_min, params_max, is_vega_weighted, is_unit_ttm_vega,
                                model_calibration_type, constraints_type, calibration_engine, nb_path, nb_steps, seed,
                                is_spot_measure=kwargs.get("is_spot_measure", True), disp=bool(kwargs.get("disp", False)),
@@ -249,12 +247,7 @@ class LogSVPricer(ModelPricer):
         other on the H100 measured so far: the Python optimizer work dominates (DESIGN.md §4.9).  Returns the list of fits, with ``return_info=True`` also the list of info dicts, each with
         ``rounds``, the library calls of the whole run.  A fit that fails raises its error after all fits have ended (the lowest chain
         index first), or with ``return_exceptions=True`` takes the exception's place in the list (its info is None)."""
-        from .calibration import calibrate_logsv_chains, per_chain
-        n = len(option_chains)
-        params_min = [p or LogSvParams(sigma0=0.1, theta=0.1, kappa1=0.25, kappa2=0.25, beta=-3.0, volvol=0.2)
-                      for p in per_chain(params_min, n, "params_min")]
-        params_max = [p or LogSvParams(sigma0=1.5, theta=1.5, kappa1=10.0, kappa2=10.0, beta=3.0, volvol=3.0)
-                      for p in per_chain(params_max, n, "params_max")]
+        from .calibration import calibrate_logsv_chains
         return calibrate_logsv_chains(self, option_chains, params0, params_min, params_max, is_vega_weighted, is_unit_ttm_vega,
                                       model_calibration_type, constraints_type, calibration_engine,
                                       is_spot_measure=kwargs.get("is_spot_measure", True), disp=bool(kwargs.get("disp", False)),
