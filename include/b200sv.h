@@ -553,6 +553,13 @@ int b200sv_hawkesjd_price_chains_batch(const b200sv_hawkes_params* params, int B
                                        const double* ttms, const double* forwards, const double* discfactors, const int* offsets,
                                        const double* strikes, const int8_t* types, int is_spot_measure, const double* vol_scalers, int P,
                                        double* prices_out, double* ivols_out);
+/* ... and under the risk kernel: gammas [B] (all finite) the risk_premia_gamma of each set, spot measure and 'C' / 'P' only (else -5), row
+ * equality against b200sv_hawkesjd_price_chain_batch with gammas.  One Riccati launch per chain plus two: every (set, maturity)
+ * normaliser solve of the call in one launch, and one Fourier-sum launch. */
+int b200sv_hawkesjd_price_chains_batch_gamma(const b200sv_hawkes_params* params, const double* gammas, int B, const int* chain_of_set, int K,
+                                             const int* Ms, const double* ttms, const double* forwards, const double* discfactors,
+                                             const int* offsets, const double* strikes, const int8_t* types, int is_spot_measure,
+                                             const double* vol_scalers, int P, double* prices_out, double* ivols_out);
 
 /* same for the Hawkes jump-diffusion: the objectives of HawkesJDPricer.calibrate_model_params_to_chain and
  * calibrate_risk_premia_gamma_to_chain (pricers/hawkes_jd_pricer.py:230-357).  B Hawkes parameter sets on one chain in one pass.

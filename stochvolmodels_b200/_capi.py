@@ -151,6 +151,7 @@ SIGNATURES = {
     "b200sv_heston_price_chains_batch": [_hp, c_int, _ip, c_int, _ip, _dp, _dp, _dp, _ip, _dp, _i8p, _dp, c_int, _dp, _dp],
     "b200sv_hawkesjd_price_chain_batch": [_kp, c_int, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_double, c_int, _dp, _dp, _dp],
     "b200sv_hawkesjd_price_chains_batch": [_kp, c_int, _ip, c_int, _ip, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, _dp, c_int, _dp, _dp],
+    "b200sv_hawkesjd_price_chains_batch_gamma": [_kp, _dp, c_int, _ip, c_int, _ip, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, _dp, c_int, _dp, _dp],
     "b200sv_fourier_qvar": [_dp, _dp, c_int, c_double, _dp, _i8p, c_int, c_double, _dp],
     "b200sv_fourier_pdf": [_dp, _dp, c_int, _dp, c_int, _dp],
     "b200sv_fourier_digital": [_dp, _dp, c_int, c_double, _dp, _i8p, c_int, c_double, _dp],

@@ -929,10 +929,13 @@ struct HawkesSetsRhsFn {
 // logsv_mgf_kernel batch mapping: the lanes of a warp integrate one point for neighbouring sets, which take nearly the same steps).
 // consts [B], phi [B][P] (phi_stride = P) or one grid (0); log_mgf [B][M][P].  A starts at 0 and is carried over the maturities.
 // Every value equals hawkes_mgf_kernel's for that set alone, bit for bit, whatever block size either runs at.
-template <int TPB>
+// RESTART: hawkes_mgf_kernel's restart mode for sets of different maturity counts (the risk-kernel normalisers of several chains, DESIGN.md
+// §4.11).  Set b owns the rows set_m0[b] .. set_m0[b + 1] - 1: every row restarts from A = 0 and integrates over its full maturity
+// dtaus[row] (the set's chain's ttms, one copy per set), and log_mgf is [rows][P]; M is not read.
+template <int TPB, bool RESTART = false>
 __global__ void __launch_bounds__(TPB) hawkes_mgf_sets_kernel(const cd* __restrict__ phi, int P, int M, const double* __restrict__ dtaus,
                                                               const HawkesMgfConsts* __restrict__ consts, int B, int phi_stride,
-                                                              cd* __restrict__ log_mgf) {
+                                                              cd* __restrict__ log_mgf, const int* __restrict__ set_m0 = nullptr) {
   __shared__ cd stage_smem[6 * 3 * TPB];
   const long long t = (long long)blockIdx.x * TPB + threadIdx.x;
   if (t >= (long long)B * P) return;
@@ -946,8 +949,20 @@ __global__ void __launch_bounds__(TPB) hawkes_mgf_sets_kernel(const cd* __restri
   const cd p1{__dadd_rn(ph.re, 1.0), __dadd_rn(ph.im, 0.0)};                                    // phi + 1
   const cd pp{__fma_rn(p1.re, ph.re, -__dmul_rn(p1.im, ph.im)), __fma_rn(p1.re, ph.im, __dmul_rn(p1.im, ph.re))};   // (phi + 1) phi
   const HawkesSetsRhsFn f{c, ph, cd{__fma_rn(pp.re, 0.5, -0.0), __fma_rn(pp.im, 0.5, -0.0)}};
-  cd* lm = log_mgf + (size_t)b * M * P + p;
+  if (RESTART) {
+    const int m0 = set_m0[b];
+    M = set_m0[b + 1] - m0;
+    dtaus += m0;
+    log_mgf += (size_t)m0 * P;
+  } else {
+    log_mgf += (size_t)b * M * P;
+  }
+  cd* lm = log_mgf + p;
   for (int m = 0; m < M; ++m) {
+    if (RESTART) {
+#pragma unroll
+      for (int k = 0; k < 3; ++k) A[k] = mk(0.0);
+    }
     rk45_generic<3, TPB>(A, dtaus[m], f, K, nullptr);
     lm[(size_t)m * P] = cd{__fma_rn(A[2].re, c.lambda_m, __fma_rn(A[1].re, c.lambda_p, A[0].re)),
                            __fma_rn(A[2].im, c.lambda_m, __fma_rn(A[1].im, c.lambda_p, A[0].im))};
@@ -2724,21 +2739,22 @@ static void launch_hawkes_mgf(cudaStream_t st, const cd* phi, const cd* psi, int
   k<<<(P + tpb - 1) / tpb, tpb, 0, st>>>(phi, psi, P, M, dtaus, c, a_in, a_out, lm, restart, nullptr);
 }
 
-// hawkes_mgf_sets_kernel over the B * P (set, point) threads of B sets; block size as for hawkes_mgf_kernel, from the threads in flight
-using HawkesMgfSetsKernel = decltype(&hawkes_mgf_sets_kernel<64>);
+// hawkes_mgf_sets_kernel over the B * P (set, point) threads of B sets; block size as for hawkes_mgf_kernel, from the threads in flight.
+// RESTART: set_m0 [B + 1] (device) places each set's rows, see the kernel.
+template <bool RESTART = false>
 static void launch_hawkes_mgf_sets(cudaStream_t st, const cd* phi, int P, int M, const double* dtaus, const HawkesMgfConsts* consts, int B,
-                                   int phi_stride, cd* lm) {
+                                   int phi_stride, cd* lm, const int* set_m0 = nullptr) {
   const long long n = (long long)B * P;
   const int tpb = mgf_block_threads((int)std::min<long long>(n, 1 << 30));
-  HawkesMgfSetsKernel k;
+  decltype(&hawkes_mgf_sets_kernel<64, RESTART>) k;
   switch (tpb) {
-    case 4: k = hawkes_mgf_sets_kernel<4>; break;
-    case 8: k = hawkes_mgf_sets_kernel<8>; break;
-    case 16: k = hawkes_mgf_sets_kernel<16>; break;
-    case 32: k = hawkes_mgf_sets_kernel<32>; break;
-    default: k = hawkes_mgf_sets_kernel<64>;
+    case 4: k = hawkes_mgf_sets_kernel<4, RESTART>; break;
+    case 8: k = hawkes_mgf_sets_kernel<8, RESTART>; break;
+    case 16: k = hawkes_mgf_sets_kernel<16, RESTART>; break;
+    case 32: k = hawkes_mgf_sets_kernel<32, RESTART>; break;
+    default: k = hawkes_mgf_sets_kernel<64, RESTART>;
   }
-  k<<<(unsigned)((n + tpb - 1) / tpb), tpb, 0, st>>>(phi, P, M, dtaus, consts, B, phi_stride, lm);
+  k<<<(unsigned)((n + tpb - 1) / tpb), tpb, 0, st>>>(phi, P, M, dtaus, consts, B, phi_stride, lm, set_m0);
 }
 
 // hawkes_mgf_tangent_kernel over the P * 13 (point, direction) threads; block size as for hawkes_mgf_kernel, from the threads in flight
@@ -2977,9 +2993,17 @@ static int queue_hawkes_prices(ChainDev& d, const FourierChain& c, const HawkesM
   return d.sums(c, prices_out, ivols_out, gammas, norm_gfwd);
 }
 
+// The (normaliser, gamma forward) of one slice from its two restarted log-MGFs lm2 [2] (complex: lm2[0] at -gamma, lm2[2] at -gamma - 1):
+// ng = (1 / e^{lm(-gamma)}, forward e^{lm(-gamma - 1)} / e^{lm(-gamma)}).  On the host, where every route that prices under the risk kernel
+// forms it, so that they all get the same bits.
+static void risk_kernel_slice(const double* lm2, double forward, double* ng) {
+  ng[0] = 1.0 / std::exp(lm2[0]);
+  ng[1] = forward * std::exp(lm2[2]) * ng[0];
+}
+
 // hawkesjd_forwards_under_risk_kernel (:487-515) for B parameter sets k[B] under gammas[B]: two single-point solves per (set, maturity) at
 // phi = -gamma and -gamma - 1, each restarted from A = 0 and integrated over the full maturity ttms[m]; one copy back, then on the host
-// ng [B][M][2] = (normaliser, gamma forward) = (1 / e^{lm(-gamma)}, forwards[m] e^{lm(-gamma - 1)} / e^{lm(-gamma)}).
+// ng [B][M][2] = risk_kernel_slice of each (set, maturity).
 static int risk_kernel_normalizers(cudaStream_t st, const HawkesMgfConsts* k, const double* gammas, int B, int M, const double* ttms,
                                    const double* forwards, std::vector<double>& ng) {
   std::vector<double> two(4 * (size_t)B, 0.0), lm2(4 * (size_t)B * M);
@@ -3001,10 +3025,22 @@ static int risk_kernel_normalizers(cudaStream_t st, const HawkesMgfConsts* k, co
   for (int b = 0; b < B; ++b)
     for (int m = 0; m < M; ++m) {                                            // log_mgf layout [b][m][point]
       const size_t s = (size_t)b * M + m;
-      ng[2 * s] = 1.0 / std::exp(lm2[2 * (2 * s + 0)]);
-      ng[2 * s + 1] = forwards[m] * std::exp(lm2[2 * (2 * s + 1)]) * ng[2 * s];
+      risk_kernel_slice(lm2.data() + 4 * s, forwards[m], ng.data() + 2 * s);
     }
   return 0;
+}
+
+// The Re phi of the grids of a built batch chain (prepare_hawkes_batch, and each group of b200sv_hawkesjd_price_chains_batch_gamma).
+static void hawkes_batch_grids(FourierChain& c, const double* gammas) {
+  const int B = c.B;
+  if (gammas && !c.per_set_grid) {
+    const std::vector<double> one(c.phi);
+    for (int b = 1; b < B; ++b) c.phi.insert(c.phi.end(), one.begin(), one.end());
+    for (size_t i = 0; i < c.ss.size(); ++i) c.ss[i].grid = (int)(i / c.Jtot);
+    c.per_set_grid = true;
+  }
+  for (int g = 0; g < (c.per_set_grid ? B : 1); ++g)
+    for (int i = 0; i < c.P; ++i) c.phi[2 * ((size_t)g * c.P + i)] = gammas ? -0.5 - gammas[g] : -0.5;
 }
 
 // Validation of b200sv_hawkesjd_price_chain_batch: sizes, the risk-premia gammas (all finite), then the chain.  The grids follow
@@ -3019,14 +3055,7 @@ static int prepare_hawkes_batch(FourierChain& c, const b200sv_hawkes_params* par
   if (int rc = c.build(params, ttms, forwards, discfactors, offsets, strikes, types, is_spot_measure != 0,
                        gammas ? ChainTypes::kGamma : ChainTypes::kFourier, vol_scaler))
     return rc;
-  if (gammas && !c.per_set_grid) {
-    const std::vector<double> one(c.phi);
-    for (int b = 1; b < B; ++b) c.phi.insert(c.phi.end(), one.begin(), one.end());
-    for (size_t i = 0; i < c.ss.size(); ++i) c.ss[i].grid = (int)(i / c.Jtot);
-    c.per_set_grid = true;
-  }
-  for (int g = 0; g < (c.per_set_grid ? B : 1); ++g)
-    for (int i = 0; i < c.P; ++i) c.phi[2 * ((size_t)g * c.P + i)] = gammas ? -0.5 - gammas[g] : -0.5;
+  hawkes_batch_grids(c, gammas);
   return 0;
 }
 
@@ -3234,6 +3263,7 @@ struct ChainsCall {
     std::vector<int> sets;            // the call's sets on this chain, in call order
     std::vector<Params> params;
     std::vector<double> etas;         // [sets][M] (LogSV with etas only)
+    std::vector<double> gammas;       // [sets] (Hawkes under the risk kernel only)
     FourierChain c;
     size_t slice0 = 0, grid0 = 0;     // the group's first log-MGF row [.][P] and first grid [.][P] in the call's buffers
   };
@@ -3243,10 +3273,11 @@ struct ChainsCall {
 
   // Ms[K]; chain k's maturities at ttms / forwards / discfactors [sum Ms[:k]], its Ms[k] + 1 offsets into strikes / types at
   // offsets [sum (Ms[:k] + 1)]; etas (may be NULL) [sum_b Ms[chain_of_set[b]]].  Every Ms[k] must be >= 1 (it places the chains
-  // after k); of a chain that no set points at nothing else is read.
+  // after k); of a chain that no set points at nothing else is read.  gammas (may be NULL) [B]: the Hawkes risk-premia gammas, each group
+  // then validated and gridded as prepare_hawkes_batch does its sets, and every set on a grid of its own.
   int prepare(const Params* params, int B, const int* chain_of_set, int K, const int* Ms, const double* ttms, const double* forwards,
               const double* discfactors, const double* etas, const int* offsets, const double* strikes, const int8_t* types, bool spot,
-              const double* vol_scalers, int P) {
+              const double* vol_scalers, int P, const double* gammas = nullptr) {
     B200SV_REQUIRE(params && chain_of_set && Ms && ttms && forwards && discfactors && offsets && strikes && types && vol_scalers,
                    "null pointer");
     B200SV_REQUIRE(B >= 1 && K >= 1, "B >= 1, K >= 1");
@@ -3272,13 +3303,16 @@ struct ChainsCall {
         g.sets.push_back(b);
         g.params.push_back(params[b]);
         if (etas) g.etas.insert(g.etas.end(), etas + eta0[b], etas + eta0[b] + Ms[k]);
+        if (gammas) g.gammas.push_back(gammas[b]);
       }
     for (Group& g : groups) {
       const int k = g.chain, m0 = g.mat0, *off = offsets + off0[k];
       if (int rc = g.c.init(true, (int)g.sets.size(), Ms[k], P > 0 ? P : 1000, off)) return rc;
-      if (int rc = g.c.build(g.params.data(), ttms + m0, forwards + m0, discfactors + m0, off, strikes, types, spot, ChainTypes::kFourier,
-                             vol_scalers[k]))
+      for (double y : g.gammas) B200SV_REQUIRE(std::isfinite(y), "gammas must be finite (NULL: no risk kernel)");
+      if (int rc = g.c.build(g.params.data(), ttms + m0, forwards + m0, discfactors + m0, off, strikes, types, spot,
+                             gammas ? ChainTypes::kGamma : ChainTypes::kFourier, vol_scalers[k]))
         return rc;
+      if (gammas) hawkes_batch_grids(g.c, g.gammas.data());
       g.slice0 = slices;
       g.grid0 = grids;
       slices += (size_t)g.c.B * g.c.M;
@@ -3383,9 +3417,11 @@ constexpr int kChainsStreams = 16;   // concurrent log-MGF launches of a multi-c
 
 // The device side of a prepared multi-chain call on host.st: grids and strike rows up, `per_group(g, stream, phi, lm)` queues group g's
 // log-MGF launch on a forked stream (reading its grids at phi, writing its [B_k][M_k][P] rows at lm), then the one Fourier-sum launch and
-// the copies back.
+// the copies back.  gammas [grids] and norm_gfwd [slices][2] (device, both or neither): the risk kernel's gamma of each grid and
+// (normaliser, gamma forward) of each slice, priced by the gamma slice pricer (ChainDev::sums).
 template <class Params, class PerGroup>
-static int run_chains(HostCall& host, const ChainsCall<Params>& call, int is_spot, double* prices_out, double* ivols_out, PerGroup per_group) {
+static int run_chains(HostCall& host, const ChainsCall<Params>& call, int is_spot, double* prices_out, double* ivols_out, PerGroup per_group,
+                      const double* gammas = nullptr, const double* norm_gfwd = nullptr) {
   const cudaStream_t st = host.st;
   const int P = call.P();
   const size_t nq = call.rows.size();
@@ -3404,8 +3440,12 @@ static int run_chains(HostCall& host, const ChainsCall<Params>& call, int is_spo
         return rc;
     B200SV_CUDA(fork.join());
   }
-  fourier_vanilla_kernel<<<(unsigned)nq, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_phi.as<cd>(), P, d_rows.as<StrikeSpec>(), is_spot, 1,
-                                                                    d_pr.as<double>(), d_iv.as<double>());
+  if (gammas)
+    fourier_gamma_batch_kernel<<<(unsigned)nq, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_phi.as<cd>(), P, d_rows.as<StrikeSpec>(), gammas,
+                                                                          norm_gfwd, d_pr.as<double>(), d_iv.as<double>());
+  else
+    fourier_vanilla_kernel<<<(unsigned)nq, kFourierThreads, 0, st>>>(d_lm.as<cd>(), d_phi.as<cd>(), P, d_rows.as<StrikeSpec>(), is_spot, 1,
+                                                                      d_pr.as<double>(), d_iv.as<double>());
   if (int rc = check_launch("fourier sum kernel")) return rc;
   B200SV_CUDA(d_pr.download(prices_out, nq));
   B200SV_CUDA(d_iv.download(ivols_out, nq));
@@ -3677,6 +3717,67 @@ int b200sv_hawkesjd_price_chains_batch(const b200sv_hawkes_params* params, int B
     ++gi;
     return check_launch("hawkes_mgf_sets_kernel");
   });
+}
+
+// The risk-kernel twin (DESIGN.md §4.11): gammas [B] as in b200sv_hawkesjd_price_chain_batch, each group validated and gridded as
+// prepare_hawkes_batch does its sets.  ONE restarted hawkes_mgf_sets_kernel launch solves the two normaliser points of every (set,
+// maturity) of the call over that maturity's full ttm; one copy back and synchronise, and risk_kernel_slice forms the (normaliser, gamma
+// forward) of each slice on the host as the single-chain routes do.  Then one Riccati launch per chain and ONE gamma Fourier-sum launch.
+int b200sv_hawkesjd_price_chains_batch_gamma(const b200sv_hawkes_params* params, const double* gammas, int B, const int* chain_of_set, int K,
+                                             const int* Ms, const double* ttms, const double* forwards, const double* discfactors,
+                                             const int* offsets, const double* strikes, const int8_t* types, int is_spot_measure,
+                                             const double* vol_scalers, int P, double* prices_out, double* ivols_out) {
+  B200SV_REQUIRE(gammas && prices_out, "null pointer");
+  ChainsCall<b200sv_hawkes_params> call;
+  if (int rc = call.prepare(params, B, chain_of_set, K, Ms, ttms, forwards, discfactors, nullptr, offsets, strikes, types, is_spot_measure != 0,
+                            vol_scalers, P > 0 ? P : 500, gammas))                // MAX_PHI, hawkes_jd_pricer.py:37
+    return rc;
+  // Per set in grid order (the groups in chain order, a group's sets in call order): its constants, gamma, normaliser points and first
+  // slice m0; per slice its ttm and forward; per group its maturity increments from dt0.
+  std::vector<HawkesMgfConsts> k;
+  std::vector<double> gam, two, tt, fw, dt;
+  std::vector<int> m0;
+  std::vector<size_t> dt0;
+  for (const auto& g : call.groups) {
+    dt0.push_back(dt.size());
+    dt.insert(dt.end(), g.c.dtaus.begin(), g.c.dtaus.end());
+    for (size_t i = 0; i < g.sets.size(); ++i) {
+      k.push_back(make_hawkes_mgf_consts(g.params[i]));
+      gam.push_back(g.gammas[i]);
+      two.insert(two.end(), {-g.gammas[i], 0.0, -g.gammas[i] - 1.0, 0.0});
+      m0.push_back((int)tt.size());
+      tt.insert(tt.end(), ttms + g.mat0, ttms + g.mat0 + g.c.M);
+      fw.insert(fw.end(), forwards + g.mat0, forwards + g.mat0 + g.c.M);
+    }
+  }
+  m0.push_back((int)tt.size());
+  const size_t slices = tt.size();
+  HostCall host;
+  DevBuf d_k(host.st), d_two(host.st), d_tt(host.st), d_m0(host.st), d_lm2(host.st), d_dt(host.st), d_gam(host.st), d_ng(host.st);
+  B200SV_CUDA(d_k.upload(k.data(), k.size()));
+  B200SV_CUDA(d_two.upload(cplx(two.data()), two.size() / 2));
+  B200SV_CUDA(d_tt.upload(tt.data(), slices));
+  B200SV_CUDA(d_m0.upload(m0.data(), m0.size()));
+  B200SV_CUDA(d_lm2.alloc(sizeof(cd) * 2 * slices));
+  launch_hawkes_mgf_sets<true>(host.st, d_two.as<cd>(), 2, 0, d_tt.as<double>(), d_k.as<HawkesMgfConsts>(), (int)k.size(), 2, d_lm2.as<cd>(),
+                               d_m0.as<int>());
+  if (int rc = check_launch("hawkes_mgf_sets_kernel")) return rc;
+  std::vector<double> lm2(4 * slices), ng(2 * slices);
+  B200SV_CUDA(d_lm2.download(cplx(lm2.data()), 2 * slices));
+  B200SV_CUDA(cudaStreamSynchronize(host.st));
+  for (size_t s = 0; s < slices; ++s) risk_kernel_slice(lm2.data() + 4 * s, fw[s], ng.data() + 2 * s);
+  B200SV_CUDA(d_dt.upload(dt.data(), dt.size()));
+  B200SV_CUDA(d_gam.upload(gam.data(), gam.size()));
+  B200SV_CUDA(d_ng.upload(ng.data(), ng.size()));
+  size_t gi = 0;
+  return run_chains(
+      host, call, 1, prices_out, ivols_out,
+      [&](const auto& g, cudaStream_t s, const cd* phi, cd* lm) {
+        launch_hawkes_mgf_sets(s, phi, g.c.P, g.c.M, d_dt.as<double>() + dt0[gi], d_k.as<HawkesMgfConsts>() + g.grid0, g.c.B, g.c.P, lm);
+        ++gi;
+        return check_launch("hawkes_mgf_sets_kernel");
+      },
+      d_gam.as<double>(), d_ng.as<double>());
 }
 
 /* Hawkes jump-diffusion Fourier chain (hawkesjd_chain_pricer / hawkesjd_chain_pricer_with_risk_premia, hawkes_jd_pricer.py:365-515).

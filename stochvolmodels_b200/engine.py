@@ -732,8 +732,8 @@ def heston_price_chain_batch(params_list: Sequence[C.HestonParamsC], ttms, forwa
 
 
 def _chains_batch(symbol: str, struct, params_list, chain_of_set, chains, etas, vol_scalers, is_spot_measure: bool, head, tail,
-                  with_ivols: bool):
-    """the multi-chain batched entry points: C arguments (params [B], B, chain_of_set [B], K, Ms [K], concatenated ttms / forwards /
+                  with_ivols: bool, lead=()):
+    """the multi-chain batched entry points: C arguments (params [B], *lead, B, chain_of_set [B], K, Ms [K], concatenated ttms / forwards /
     discfactors, [etas,] per-chain offsets, strikes, types, *head, vol_scalers [K], *tail, prices, ivols | NULL) -> (prices, ivols | None),
     each a list of B rows, row b of length J of chain chain_of_set[b].  ``etas`` = (LogSV per-set backbones or None,) or ()."""
     B, K = len(params_list), len(chains)
@@ -771,7 +771,7 @@ def _chains_batch(symbol: str, struct, params_list, chain_of_set, chains, etas, 
     J = np.array([chs[k].strikes.shape[0] for k in cos])
     prices = np.empty(int(J.sum()))
     ivols = np.empty_like(prices) if with_ivols else None
-    C.call(symbol, (struct * B)(*params_list), B, C.iptr(cos), K, C.iptr(Ms), *map(C.dptr, cat[:3]), *map(C.dptr, flat_etas),
+    C.call(symbol, (struct * B)(*params_list), *lead, B, C.iptr(cos), K, C.iptr(Ms), *map(C.dptr, cat[:3]), *map(C.dptr, flat_etas),
            C.iptr(offsets), C.dptr(cat[3]), C.i8ptr(types), *head, C.dptr(scalers), *tail, C.dptr(prices), C.dptr(ivols))
     ends = np.cumsum(J).tolist()
     spans = list(zip([0] + ends[:-1], ends))
@@ -814,9 +814,19 @@ def hawkesjd_price_chain_batch(params_list: Sequence[C.HawkesParamsC], ttms, for
 
 
 def hawkesjd_price_chains_batch(params_list: Sequence[C.HawkesParamsC], chain_of_set, chains, vol_scalers=None, is_spot_measure: bool = True,
-                                max_phi: int = 500, with_ivols: bool = True):
-    """B Hawkes parameter sets over K chains in one pass, no risk kernel -> (prices, ivols | None); arguments as logsv_price_chains_batch.
-    Row b is bit for bit row b of hawkesjd_price_chain_batch on its chain with the sets of this call on that chain, in order."""
+                                max_phi: int = 500, with_ivols: bool = True, gammas=None):
+    """B Hawkes parameter sets over K chains in one pass -> (prices, ivols | None); arguments as logsv_price_chains_batch.  ``gammas``: None
+    (no risk kernel) or [B] risk_premia_gamma per set, every set then priced under its risk kernel (b200sv_hawkesjd_price_chains_batch_gamma).
+    Row b is bit for bit row b of hawkesjd_price_chain_batch (with the same gammas) on its chain with the sets of this call on that chain,
+    in order."""
+    if gammas is not None:
+        if not is_spot_measure or any(str(t) not in ("C", "P") for chain in chains for types in chain[4] for t in types):
+            raise ValueError("not implemented")           # utils/mgf_pricer.py:310-318
+        gammas = C.f64(gammas)
+        if gammas.shape != (len(params_list),):
+            raise ValueError(f"gammas must have shape ({len(params_list)},)")
+        return _chains_batch("b200sv_hawkesjd_price_chains_batch_gamma", C.HawkesParamsC, params_list, chain_of_set, chains, (), vol_scalers,
+                             is_spot_measure, (int(bool(is_spot_measure)),), (int(max_phi),), with_ivols, lead=(C.dptr(gammas),))
     return _chains_batch("b200sv_hawkesjd_price_chains_batch", C.HawkesParamsC, params_list, chain_of_set, chains, (), vol_scalers,
                          is_spot_measure, (int(bool(is_spot_measure)),), (int(max_phi),), with_ivols)
 

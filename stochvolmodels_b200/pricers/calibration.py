@@ -636,9 +636,11 @@ def calibrate_hawkes(pricer, option_chain, params0, is_vega_weighted: bool, is_u
 
 
 def calibrate_hawkes_risk_premia(option_chain, params0, is_vega_weighted: bool, is_unit_ttm_vega: bool, maxiter: int = 100,
-                                 print_iter: bool = True, return_info: bool = False, **kwargs):
+                                 print_iter: bool = True, return_info: bool = False, price_batch: Optional[Callable] = None,
+                                 line_sink: Callable[[str], None] = print, **kwargs):
     """HawkesJDPricer.calibrate_risk_premia_gamma_to_chain (reference hawkes_jd_pricer.py:303-357): (sigma, gamma / 8) with the rest of
-    ``params0`` fixed, weights x 1e4, SLSQP with difference step 0.025 and ftol = tol = 1e-16"""
+    ``params0`` fixed, weights x 1e4, SLSQP with difference step 0.025 and ftol = tol = 1e-16.  ``price_batch`` as for calibrate_hawkes;
+    ``line_sink`` receives the ``print_iter`` lines (the lock-step driver collects each chain's)"""
     from .hawkes_jd_pricer import _KEYS, HawkesJDParams
     if check_gradient(kwargs.get("gradient", "difference")) == "exact":
         raise NotImplementedError("gradient='exact' does not cover calibrate_risk_premia_gamma_to_chain: the risk-kernel pricer has no "
@@ -648,14 +650,14 @@ def calibrate_hawkes_risk_premia(option_chain, params0, is_vega_weighted: bool, 
     bounds = ((0.01, 1.5), (-1.0, 1.0))
 
     def announce(x: np.ndarray) -> None:
-        print(f"unpack_pars: sigma={x[0]}, gamma={gamma_scaler * x[1]}")
+        line_sink(f"unpack_pars: sigma={x[0]}, gamma={gamma_scaler * x[1]}")
 
     def to_params(x: np.ndarray):
         return HawkesJDParams(**{**fixed, "sigma": float(x[0])}, risk_premia_gamma=float(gamma_scaler * x[1]))
 
     p0 = np.array([params0.sigma, (params0.risk_premia_gamma or 0.0) / gamma_scaler])
     objective = _batched_vol_objective(option_chain, to_params, is_vega_weighted, is_unit_ttm_vega, bounds, 0.025, scale=10000.0,
-                                       on_point=announce if print_iter else None)
+                                       on_point=announce if print_iter else None, price_batch=price_batch)
     x, result = run_slsqp(objective, p0, bounds, disp=bool(kwargs.get("disp", False)), tol=1e-16, validate=False, ftol=1e-16,
                           maxiter=maxiter, eps=0.025)
     if print_iter:
@@ -798,7 +800,8 @@ def _pack(posted: dict, max_sets_per_call: Optional[int]) -> List[List[int]]:
 
 
 def calibrate_chains_lockstep(fit: Callable, option_chains, price_chains: Callable, gradient: str, max_sets_per_call: Optional[int],
-                              return_exceptions: bool, return_info: bool, extras: Optional[Callable] = None, **per_chain_args):
+                              return_exceptions: bool, return_info: bool, extras: Optional[Callable] = None,
+                              method: str = "calibrate_model_params_to_chains", **per_chain_args):
     """one single-chain fit per chain of ``option_chains``, in lock-step.  Before any library call: ``gradient`` ('difference' only),
     ``option_chains`` (not empty), ``max_sets_per_call`` (None or at least 1), then per_chain on each of ``per_chain_args`` in turn.
     ``fit(option_chain, price_batch, **args)`` runs the fit of one chain on its values of ``per_chain_args`` (calibrate_logsv /
@@ -808,10 +811,11 @@ def calibrate_chains_lockstep(fit: Callable, option_chains, price_chains: Callab
     extras(requests)``, the model's other arguments (none without ``extras``).  Each fit runs in a thread of its own; the caller's thread,
     whose CUDA stream the library calls keep (b200sv_set_stream is per thread), prices every round and waits for all threads before it
     returns.  -> the fits, with ``return_info`` (fits, infos) whose info dicts add ``rounds`` (library calls of the whole run); a failed
-    fit's slot holds its exception (info None) with ``return_exceptions``, else the lowest-index exception is raised."""
+    fit's slot holds its exception (info None) with ``return_exceptions``, else the lowest-index exception is raised.  ``method`` names the
+    caller in the ``gradient`` rejection."""
     if gradient != "difference":
         if gradient in GRADIENTS:
-            raise NotImplementedError(f"calibrate_model_params_to_chains has gradient='difference' only, not {gradient!r}")
+            raise NotImplementedError(f"{method} has gradient='difference' only, not {gradient!r}")
         check_gradient(gradient)
     n = len(option_chains)
     if n == 0:
@@ -921,6 +925,32 @@ def calibrate_hawkes_chains(pricer, option_chains, params0, is_vega_weighted: bo
 
     return calibrate_chains_lockstep(fit, option_chains, engine.hawkesjd_price_chains_batch, gradient, max_sets_per_call, return_exceptions,
                                      return_info, lambda requests: ((), {"max_phi": MAX_PHI}), params0=params0)
+
+
+def calibrate_hawkes_risk_premia_chains(option_chains, params0, is_vega_weighted: bool, is_unit_ttm_vega: bool, maxiter: int = 100,
+                                        print_iter: bool = False, return_info: bool = False, gradient: str = "difference",
+                                        return_exceptions: bool = False, max_sets_per_call: Optional[int] = None, **kwargs):
+    """calibrate_hawkes_risk_premia on every chain in lock-step: one risk-kernel engine.hawkesjd_price_chains_batch call per optimizer
+    round.  ``print_iter``: each chain's lines are collected and printed as one block per chain, in chain order, once every fit has ended"""
+    from .hawkes_jd_pricer import MAX_PHI
+    lines: List[List[str]] = [[] for _ in option_chains]
+
+    def fit(option_chain, price_batch, params0, line_sink):
+        return calibrate_hawkes_risk_premia(option_chain, params0, is_vega_weighted, is_unit_ttm_vega, maxiter=maxiter, print_iter=print_iter,
+                                            return_info=True, price_batch=price_batch, line_sink=line_sink, **kwargs)
+
+    def extras(requests):
+        # request = (args, kwargs) of engine.hawkesjd_price_chain_batch(params_list, ..., max_phi=, gammas=): every set's gamma, in call order
+        return (), {"max_phi": MAX_PHI, "gammas": [g for _, kw in requests for g in kw["gammas"]]}
+
+    try:
+        return calibrate_chains_lockstep(fit, option_chains, engine.hawkesjd_price_chains_batch, gradient, max_sets_per_call, return_exceptions,
+                                         return_info, extras, method="calibrate_risk_premia_gamma_to_chains", params0=params0,
+                                         line_sink=[chain_lines.append for chain_lines in lines])
+    finally:
+        for chain_lines in lines:
+            for line in chain_lines:
+                print(line)
 
 
 def _rows_by_request(ivols, chain_of_set, n: int) -> List[np.ndarray]:

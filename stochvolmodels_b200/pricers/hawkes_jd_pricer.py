@@ -7,7 +7,8 @@
 * ``HawkesJDPricer.price_chain``              (:125-155) -> ``hawkesjd_chain_pricer`` (:365-417) / ``hawkesjd_chain_pricer_with_risk_premia`` (:420-484),
   ``hawkesjd_forwards_under_risk_kernel`` (:487-515), ``compute_hawkes_a_mgf_grid`` / ``solve_a_ode_grid`` (:518-579)
 * ``HawkesJDPricer.calibrate_model_params_to_chain`` (:230-300), ``calibrate_risk_premia_gamma_to_chain`` (:303-357): host SLSQP loops around the
-  batched GPU chain pricer (``b200sv_hawkesjd_price_chain_batch``), fits bit-identical to SLSQP differencing the one-set objective (pricers/calibration.py)
+  batched GPU chain pricer (``b200sv_hawkesjd_price_chain_batch``), fits bit-identical to SLSQP differencing the one-set objective (pricers/calibration.py);
+  their ``*_to_chains`` twins fit a series of chains in lock-step on ``b200sv_hawkesjd_price_chains_batch{,_gamma}``
 
 Monte Carlo: the reference draws every random input from numpy's process-global generator; here they are drawn in-kernel from the Philox
 stream keyed by an explicit ``seed`` (default: the ``set_seed`` stream or OS entropy).  ``simulate_hawkesjd_terminal`` additionally accepts the five
@@ -28,7 +29,7 @@ from ..data.option_chain import OptionChain
 from ..multi_gpu import _shared_seed, _use_distributed, mc_chain_distributed
 from ..utils.config import VariableType
 from ..utils.funcs import set_time_grid, timer
-from .calibration import calibrate_hawkes, calibrate_hawkes_chains, calibrate_hawkes_risk_premia
+from .calibration import calibrate_hawkes, calibrate_hawkes_chains, calibrate_hawkes_risk_premia, calibrate_hawkes_risk_premia_chains
 from .calibration import _batched_vol_objective, hawkes_fit_jacobian  # noqa: F401  (imported from this module by callers)
 from .model_pricer import ModelParams, ModelPricer
 
@@ -202,6 +203,20 @@ class HawkesJDPricer(ModelPricer):
         has no sensitivities, so ``gradient='exact'`` raises NotImplementedError."""
         return calibrate_hawkes_risk_premia(option_chain, params0, is_vega_weighted, is_unit_ttm_vega, maxiter=maxiter, print_iter=print_iter,
                                             return_info=return_info, **kwargs)
+
+    def calibrate_risk_premia_gamma_to_chains(self, option_chains: List[OptionChain], params0, is_vega_weighted: bool = True,
+                                              is_unit_ttm_vega: bool = False, maxiter: int = 100, print_iter: bool = False,
+                                              return_info: bool = False, gradient: str = "difference", return_exceptions: bool = False,
+                                              max_sets_per_call: Optional[int] = None, **kwargs):
+        """``calibrate_risk_premia_gamma_to_chain`` on every chain of ``option_chains``, in lock-step: one risk-kernel
+        ``engine.hawkesjd_price_chains_batch`` call per optimizer round, every fit bit for bit the single-chain driver's (DESIGN.md §4.11).
+        ``params0``: one HawkesJDParams or a list of one per chain, each with its own start (sigma, gamma; a ``None`` gamma starts at 0) and
+        fixed fields.  ``print_iter``: each chain's lines, exactly what the single-chain driver prints, as one block per chain in chain order
+        once every fit has ended.  ``gradient='difference'`` only.  ``return_info``, ``return_exceptions`` and ``max_sets_per_call`` as for
+        ``calibrate_model_params_to_chains``, and the info dicts add ``rounds``."""
+        return calibrate_hawkes_risk_premia_chains(option_chains, params0, is_vega_weighted, is_unit_ttm_vega, maxiter=maxiter,
+                                                   print_iter=print_iter, return_info=return_info, gradient=gradient,
+                                                   return_exceptions=return_exceptions, max_sets_per_call=max_sets_per_call, **kwargs)
 
     @timer
     def simulate_terminal_values(self, params: HawkesJDParams, ttm: float = 1.0, nb_path: int = 100000, is_spot_measure: bool = True, **kwargs
