@@ -380,6 +380,18 @@ int b200sv_hawkesjd_price_chain_greeks(const b200sv_hawkes_params* params, int M
                                        const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
                                        int is_spot_measure, double vol_scaler, int P, double* prices_out, double* greeks_out,
                                        double* dlog_mgf_out, int* nfev_out);
+/* forward-mode sensitivities of the Hawkes Fourier chain under the risk kernel exp(-gamma x) (DESIGN.md §4.12): prices_out bit-identical
+ * to b200sv_hawkesjd_price_chain with the same risk_premia_gamma (spot measure, calls and puts, no discount factor, as there);
+ * greeks_out [2 + 16][J]: d price / d forwards[m], d^2 price / d forwards[m]^2, then d price / d (sigma, shift_p, mean_p, shift_m, mean_m,
+ * lambda_p, theta_p, kappa_p, beta1_p, beta2_p, lambda_m, theta_m, kappa_m, beta1_m, beta2_m, risk_premia_gamma), exact on the solver's
+ * own meshes with the grid's imaginary parts held fixed.  Optional outputs (may be NULL): dlog_mgf_out [16][M][P] complex128 interleaved;
+ * dlog_norm_out [16][M][2]: the derivatives of Re log-MGF at the normaliser points -gamma and -gamma - 1 (each solved from A = 0 over
+ * the full ttms[m]); nfev_out [P].  -1: a null required pointer or a non-finite risk_premia_gamma; -5: not the spot measure, or a type
+ * other than call / put; sizes, maturities and strikes as b200sv_hawkesjd_price_chain.  Every check runs before any device work. */
+int b200sv_hawkesjd_price_chain_risk_premia_greeks(const b200sv_hawkes_params* params, int M, const double* ttms, const double* forwards,
+                                                   const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
+                                                   int is_spot_measure, double vol_scaler, int P, double risk_premia_gamma, double* prices_out,
+                                                   double* greeks_out, double* dlog_mgf_out, double* dlog_norm_out, int* nfev_out);
 /* second-order sensitivities of the Hawkes Fourier chain without a risk kernel (DESIGN.md §4.5).  The arguments and outputs of
  * b200sv_hawkesjd_price_chain_greeks (bit-identical to it), then vanna_out [15][J]: d^2 price / d forwards[m] d parameter, and
  * hessian_out [120][J]: d^2 price / d p d q for p <= q, the upper triangle row-major in that parameter order ((0,0), (0,1), .., (0,14),

@@ -2,7 +2,7 @@
 behind the reference's Pricer API.  See DESIGN.md / INTEGRATION.md.  There is no CPU fallback: computing needs
 ``lib/libb200sv.so`` (built by ``python -m stochvolmodels_b200._build``) and a CUDA device."""
 from .data.option_chain import OptionChain, OptionSlice, get_btc_test_chain_data
-from .engine import HAWKES_GREEK_PARAMS, infer_bsm_ivols_from_model_chain_prices, infer_bsm_ivols_from_slice_prices
+from .engine import HAWKES_GREEK_PARAMS, HAWKES_RISK_PREMIA_GREEK_PARAMS, infer_bsm_ivols_from_model_chain_prices, infer_bsm_ivols_from_slice_prices
 from .pricers.calibration import CalibrationEngine, CalibrationError, ConstraintsType, LogsvModelCalibrationType
 from .pricers.hawkes_jd_pricer import HawkesJDParams, HawkesJDPricer
 from .pricers.fourier_greeks import ChainIvolGreeks, ChainIvolHessian, FourierChainGreeks, FourierChainHessian
@@ -21,4 +21,4 @@ __all__ = ["HawkesJDParams", "HawkesJDPricer", "OptionChain", "get_btc_test_chai
            "LogSvParams", "LogSVPricer", "CalibrationEngine", "CalibrationError", "ConstraintsType", "LogsvModelCalibrationType", "LOGSV_BTC_PARAMS", "ModelParams", "ModelPricer", "OptionType", "VariableType", "set_seed", "set_time_grid",
            "compute_integration_weights", "OptionSlice", "compute_analytic_qvar", "infer_bsm_ivols_from_slice_prices",
            "infer_bsm_ivols_from_model_chain_prices", "McChainGreeks", "FourierChainGreeks", "FourierChainHessian",
-           "ChainIvolGreeks", "ChainIvolHessian", "HAWKES_GREEK_PARAMS"]
+           "ChainIvolGreeks", "ChainIvolHessian", "HAWKES_GREEK_PARAMS", "HAWKES_RISK_PREMIA_GREEK_PARAMS"]

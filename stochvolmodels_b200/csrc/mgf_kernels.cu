@@ -1451,6 +1451,126 @@ __global__ void __launch_bounds__(kFourierThreads) fourier_vanilla_greeks_kernel
   }
 }
 
+// ---- Hawkes jump-diffusion under the risk kernel (DESIGN.md §4.12) ----
+// risk_premia_gamma moves every transform point, on the grid (Re phi = -1/2 - gamma) and at the two normaliser points (-gamma,
+// -gamma - 1), by d phi / d gamma = -1: a 14th tangent direction, in the transform variable, next to the 13 ODE directions.
+constexpr int kHawkesRpDirs = kHawkesOdeDirs + 1;
+constexpr int kHawkesRpParams = kHawkesGreekParams + 1;      // HAWKES_RISK_PREMIA_GREEK_PARAMS: HAWKES_GREEK_PARAMS, then risk_premia_gamma
+
+// HawkesTanRhsFn plus a move dphi of the transform variable (psi = 0, so drift0 = sigma^2 (phi + 1) phi / 2):
+// d rhs0 += sigma^2 (phi + 1/2) dphi,  dz_p = dz_m += dphi,  d rhs1 += comp_p dphi,  d rhs2 += comp_m dphi.
+struct HawkesRpTanRhsFn {
+  const HawkesMgfConsts& c;
+  HawkesMgfConsts d;
+  cd phi, h0;              // h0 = (phi + 1) phi / 2
+  double dphi;             // 0 on the ODE directions, -1 on the gamma direction (whose d is zero)
+  __device__ __forceinline__ void operator()(const cd (&A)[3], const cd (&dA)[3], cd (&out)[3]) const {
+    const cd zp = (phi - c.beta1_p * A[1]) - c.beta1_m * A[2], zm = (phi - c.beta2_p * A[1]) - c.beta2_m * A[2];
+    const cd dzp = mk(dphi) - (((c.beta1_p * dA[1] + c.beta1_m * dA[2]) + d.beta1_p * A[1]) + d.beta1_m * A[2]);
+    const cd dzm = mk(dphi) - (((c.beta2_p * dA[1] + c.beta2_m * dA[2]) + d.beta2_p * A[1]) + d.beta2_m * A[2]);
+    out[0] = ((((c.kt_p * dA[1] + c.kt_m * dA[2]) + d.kt_p * A[1]) + d.kt_m * A[2]) + d.sigma2 * h0) + (c.sigma2 * dphi) * (phi + mk(0.5));
+    out[1] = ((hawkes_djump(zp, dzp, c.shift_p, c.mean_p, d.shift_p, d.mean_p) - (c.kappa_p * dA[1] + d.kappa_p * A[1])) + d.comp_p * phi) +
+             mk(c.comp_p * dphi);
+    out[2] = ((hawkes_djump(zm, dzm, c.shift_m, c.mean_m, d.shift_m, d.mean_m) - (c.kappa_m * dA[2] + d.kappa_m * A[2])) + d.comp_m * phi) +
+             mk(c.comp_m * dphi);
+  }
+};
+
+// hawkes_mgf_tangent_kernel with the gamma direction: one thread = one (point, direction), 14 directions, the primal integration of
+// hawkes_mgf_kernel (same rk45_generic, same mesh) plus one tangent.  restart = 0: A and dA carried over the maturity increments dtaus
+// (the grid); restart != 0: every maturity restarts from A = dA = 0 and integrates over its full ttm dtaus[m] (the normaliser points, as
+// hawkes_mgf_kernel's restart mode).  Outputs: dlog_mgf [16][M][P] (HAWKES_RISK_PREMIA_GREEK_PARAMS order: rows 5 / 10 = a_p / a_m,
+// row 15 = d/d gamma), log_mgf [M][P] and nfev [P] (both optional).
+template <int TPB>
+__global__ void __launch_bounds__(TPB) hawkes_mgf_rp_tangent_kernel(const cd* __restrict__ phi, int P, int M, const double* __restrict__ dtaus,
+                                                                    HawkesMgfConsts c, HawkesTangentDirs dirs, int restart,
+                                                                    cd* __restrict__ dlog_mgf, cd* __restrict__ log_mgf, int* __restrict__ nfev) {
+  constexpr int D = kHawkesRpDirs;
+  __shared__ cd stage_smem[6 * 3 * TPB];
+  __shared__ cd tan_smem[8 * 3 * TPB];
+  const int t = blockIdx.x * TPB + threadIdx.x;
+  if (t >= P * D) return;
+  const int p = t / D, dir = t % D;
+  const bool gdir = dir == kHawkesOdeDirs;
+#pragma unroll
+  for (int i = 0; i < 18; ++i) stage_smem[threadIdx.x + i * TPB] = mk(0.0);
+#pragma unroll
+  for (int i = 0; i < 24; ++i) tan_smem[threadIdx.x + i * TPB] = mk(0.0);
+  StageStore<3, TPB> K{stage_smem + threadIdx.x};
+  const cd ph = phi[p];
+  const cd h0 = 0.5 * ((ph + mk(1.0)) * ph);
+  const HawkesRhsFn f{c, ph, c.sigma2 * h0};
+  const HawkesMgfConsts zero{0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+  TangentHook<3, TPB, HawkesRpTanRhsFn> tan{HawkesRpTanRhsFn{c, gdir ? zero : dirs.d[dir], ph, h0, gdir ? -1.0 : 0.0},
+                                           {StageStore<3, TPB>{tan_smem + threadIdx.x}, {}}};   // dy = 0
+  cd A[3] = {mk(0.0), mk(0.0), mk(0.0)};
+  const int row = gdir ? kHawkesGreekParams : hawkes_dir_row(dir);
+  int nf = 0;
+  for (int m = 0; m < M; ++m) {
+    if (restart) {
+#pragma unroll
+      for (int k = 0; k < 3; ++k) A[k] = tan.t.dy[k] = mk(0.0);
+    }
+    int nfe = 0;
+    rk45_generic<3, TPB>(A, dtaus[m], f, K, &nfe, &tan);
+    nf += nfe;
+    dlog_mgf[((size_t)row * M + m) * P + p] = (tan.t.dy[0] + tan.t.dy[1] * c.lambda_p) + tan.t.dy[2] * c.lambda_m;
+    if (dir == 0) {
+      dlog_mgf[((size_t)5 * M + m) * P + p] = A[1];
+      dlog_mgf[((size_t)10 * M + m) * P + p] = A[2];
+      if (log_mgf) log_mgf[(size_t)m * P + p] = (A[0] + A[1] * c.lambda_p) + A[2] * c.lambda_m;
+    }
+  }
+  if (dir == 0 && nfev) nfev[p] = nf;
+}
+
+// Sums of fourier_gamma_batch_kernel (same weight branch, same NaN skip) and their derivatives, one CTA per strike, fixed-order block_sum:
+// with e = exp(lm - x phi), x = ln(F/K):  S = sum Re(w e),  S_x = sum Re(-w phi e),  S_xx = sum Re(w phi^2 e),  S_p = sum Re(w e dlm_p),
+// and for gamma S_g = sum Re(w e (x + dlm_g)) (the grid moves, phi + gamma does not, so w is fixed).  The prices C = G - n K^(1+g) S,
+// P = K - n K^(1+g) S with n = e^{-l0}, G = F e^{l1} n (norm_gfwd [M][2], the pricing route's own) give
+//   delta = [C] G / F - n K^(1+g) S_x / F,   gamma = -n K^(1+g) (S_xx - S_x) / F^2,
+//   d/dp  = [C] G (l1_p - l0_p) - n K^(1+g) (S_p - l0_p S [+ ln K S for gamma]),
+// where l0_p, l1_p = Re dnorm [16][M][2] (the restarted tangents at -gamma, -gamma - 1).  greeks [2 + 16][J].
+__global__ void __launch_bounds__(kFourierThreads) fourier_gamma_greeks_kernel(const cd* __restrict__ log_mgf, const cd* __restrict__ dlog_mgf,
+                                                                              const cd* __restrict__ dnorm, const cd* __restrict__ phi, int P,
+                                                                              int M, const StrikeSpec* __restrict__ specs, double gamma,
+                                                                              const double* __restrict__ norm_gfwd, double* __restrict__ greeks) {
+  constexpr int NP = kHawkesRpParams;
+  const StrikeSpec sp = specs[blockIdx.x];
+  const cd* lm = log_mgf + (size_t)sp.slice * P;
+  const double x = log(sp.forward / sp.strike);
+  const bool fast = fabs(phi[0].re - (0.5 + gamma)) < 1e-10;
+  double acc[3 + NP] = {};
+  strike_sum(phi, P, acc, [&](int j, double dp, cd ph) {
+    const cd pg = ph + mk(gamma);
+    const cd w = fast ? mk((dp / M_PI) / (ph.im * ph.im + 0.25)) : -(mk(dp / M_PI) / ((pg + mk(1.0)) * pg));
+    const cd e = cexp_(lm[j] - x * ph);
+    const cd term = w * e;
+    if (term.re == term.re) {
+      acc[0] += term.re;
+      acc[1] += (w * -(ph * e)).re;
+      acc[2] += (w * ((ph * ph) * e)).re;
+#pragma unroll
+      for (int k = 0; k < NP - 1; ++k) acc[3 + k] += (term * dlog_mgf[((size_t)k * M + sp.slice) * P + j]).re;
+      acc[2 + NP] += (term * (mk(x) + dlog_mgf[((size_t)(NP - 1) * M + sp.slice) * P + j])).re;
+    }
+  });
+  if (threadIdx.x == 0) {
+    const double S = acc[0], Sx = acc[1], Sxx = acc[2], F = sp.forward, K = sp.strike;
+    const double n = norm_gfwd[2 * (size_t)sp.slice], G = norm_gfwd[2 * (size_t)sp.slice + 1], ngk = n * pow(K, 1.0 + gamma);
+    const int J = gridDim.x;
+    const bool call = sp.type == B200SV_CALL;
+    greeks[blockIdx.x] = (call ? G / F : 0.0) - ngk * Sx / F;
+    greeks[J + blockIdx.x] = -ngk * (Sxx - Sx) / (F * F);
+#pragma unroll
+    for (int k = 0; k < NP; ++k) {
+      const double l0 = dnorm[((size_t)k * M + sp.slice) * 2].re, l1 = dnorm[((size_t)k * M + sp.slice) * 2 + 1].re;
+      const double s = (acc[3 + k] - l0 * S) + (k == NP - 1 ? log(K) * S : 0.0);
+      greeks[(size_t)(2 + k) * J + blockIdx.x] = (call ? G * (l1 - l0) : 0.0) - ngk * s;
+    }
+  }
+}
+
 // --------------------------------------------------------------------------------------------------------------------
 // Second-order forward-mode sensitivities of the Fourier chain pricers (DESIGN.md §4.4)
 // --------------------------------------------------------------------------------------------------------------------
@@ -2773,6 +2893,21 @@ static void launch_hawkes_mgf_tangent(cudaStream_t st, const cd* phi, int P, int
   k<<<(n + tpb - 1) / tpb, tpb, 0, st>>>(phi, P, M, dtaus, c, dirs, dlm, lm, nullptr, nfev);
 }
 
+// hawkes_mgf_rp_tangent_kernel over the P * 14 (point, direction) threads, block size chosen the same way
+static void launch_hawkes_mgf_rp_tangent(cudaStream_t st, const cd* phi, int P, int M, const double* dtaus, const HawkesMgfConsts& c,
+                                         const HawkesTangentDirs& dirs, int restart, cd* dlm, cd* lm, int* nfev) {
+  const int n = P * kHawkesRpDirs, tpb = mgf_block_threads(n);
+  decltype(&hawkes_mgf_rp_tangent_kernel<64>) k;
+  switch (tpb) {
+    case 4: k = hawkes_mgf_rp_tangent_kernel<4>; break;
+    case 8: k = hawkes_mgf_rp_tangent_kernel<8>; break;
+    case 16: k = hawkes_mgf_rp_tangent_kernel<16>; break;
+    case 32: k = hawkes_mgf_rp_tangent_kernel<32>; break;
+    default: k = hawkes_mgf_rp_tangent_kernel<64>;
+  }
+  k<<<(n + tpb - 1) / tpb, tpb, 0, st>>>(phi, P, M, dtaus, c, dirs, restart, dlm, lm, nfev);
+}
+
 // ---- chain preparation ----
 // Default transform-grid scale when the caller passes vol_scaler <= 0; t0 is the first (shortest) maturity.
 static double default_vol_scaler(const b200sv_logsv_params& p, double t0) {      // logsv_pricer.py:664-666
@@ -3831,6 +3966,56 @@ int b200sv_hawkesjd_price_chain_greeks(const b200sv_hawkes_params* params, int M
   GreeksDev<kHawkesGreekParams> g(d.st);
   if (int rc = queue_hawkes_greeks(d, g, c, *params, k, prices_out)) return rc;
   return g.download(d, c, greeks_out, dlog_mgf_out, nfev_out);
+}
+
+/* Forward-mode sensitivities of the Hawkes Fourier chain under the risk kernel (DESIGN.md §4.12): the pricing launches of
+ * b200sv_hawkesjd_price_chain with risk_premia_gamma unchanged (the restarted normaliser launch, its one synchronisation, the Riccati
+ * launch and the gamma sums: bit-identical prices), then hawkes_mgf_rp_tangent_kernel at the two normaliser points (restarted) and on the
+ * grid (carried), and fourier_gamma_greeks_kernel on the grid tangent kernel's own primal log-MGF; one synchronisation at the end.
+ * greeks_out [2 + 16][J]: delta, gamma, HAWKES_GREEK_PARAMS, risk_premia_gamma.  Optional: dlog_mgf_out [16][M][P] (complex),
+ * dlog_norm_out [16][M][2] (the derivatives of Re log-MGF at -gamma and -gamma - 1), nfev_out [P]. */
+int b200sv_hawkesjd_price_chain_risk_premia_greeks(const b200sv_hawkes_params* params, int M, const double* ttms, const double* forwards,
+                                                   const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
+                                                   int is_spot_measure, double vol_scaler, int P, double risk_premia_gamma, double* prices_out,
+                                                   double* greeks_out, double* dlog_mgf_out, double* dlog_norm_out, int* nfev_out) {
+  B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && greeks_out, "null pointer");
+  B200SV_REQUIRE(std::isfinite(risk_premia_gamma), "risk_premia_gamma must be finite");
+  FourierChain c;
+  if (int rc = prepare_hawkes_chain(c, params, M, ttms, forwards, discfactors, offsets, strikes, types, is_spot_measure, vol_scaler, P,
+                                    risk_premia_gamma))
+    return rc;
+  P = c.P;
+  constexpr int NP = kHawkesRpParams;
+  const HawkesMgfConsts k = make_hawkes_mgf_consts(*params);
+  ChainDev d;
+  DevBuf d_gam(d.st), d_ng(d.st), d_two(d.st), d_ttm(d.st), d_dn(d.st);
+  std::vector<double> ng;
+  if (int rc = risk_kernel_normalizers(d.st, &k, &risk_premia_gamma, 1, M, ttms, forwards, ng)) return rc;
+  B200SV_CUDA(d_gam.upload(&risk_premia_gamma, 1));
+  B200SV_CUDA(d_ng.upload(ng.data(), ng.size()));
+  if (int rc = queue_hawkes_prices(d, c, &k, prices_out, nullptr, d_gam.as<double>(), d_ng.as<double>())) return rc;
+  const HawkesTangentDirs dirs = make_hawkes_tangents(*params);
+  const double two[4] = {-risk_premia_gamma, 0.0, -risk_premia_gamma - 1.0, 0.0};
+  B200SV_CUDA(d_two.upload(cplx(two), 2));
+  B200SV_CUDA(d_ttm.upload(ttms, M));
+  B200SV_CUDA(d_dn.alloc(sizeof(cd) * (size_t)NP * M * 2));
+  launch_hawkes_mgf_rp_tangent(d.st, d_two.as<cd>(), 2, M, d_ttm.as<double>(), k, dirs, 1, d_dn.as<cd>(), nullptr, nullptr);
+  if (int rc = check_launch("hawkes_mgf_rp_tangent_kernel")) return rc;
+  GreeksDev<NP> g(d.st);
+  if (int rc = g.alloc(c, true)) return rc;
+  launch_hawkes_mgf_rp_tangent(d.st, d.phi.as<cd>(), P, M, d.dt.as<double>(), k, dirs, 0, g.dlm.as<cd>(), g.lm.as<cd>(), g.nfev.as<int>());
+  if (int rc = check_launch("hawkes_mgf_rp_tangent_kernel")) return rc;
+  if (c.Jtot > 0) {
+    fourier_gamma_greeks_kernel<<<c.Jtot, kFourierThreads, 0, d.st>>>(g.lm.as<cd>(), g.dlm.as<cd>(), d_dn.as<cd>(), d.phi.as<cd>(), P, M,
+                                                                      d.rows.as<StrikeSpec>(), risk_premia_gamma, d_ng.as<double>(),
+                                                                      g.g.as<double>());
+    if (int rc = check_launch("fourier_gamma_greeks_kernel")) return rc;
+  }
+  std::vector<cd> dn(dlog_norm_out ? (size_t)NP * M * 2 : 0);
+  B200SV_CUDA(d_dn.download(dlog_norm_out ? dn.data() : nullptr, dn.size()));
+  if (int rc = g.download(d, c, greeks_out, dlog_mgf_out, nfev_out)) return rc;
+  for (size_t i = 0; i < dn.size(); ++i) dlog_norm_out[i] = dn[i].re;
+  return 0;
 }
 
 /* Second-order sensitivities of the Hawkes Fourier chain without a risk kernel (DESIGN.md §4.5): the launches of

@@ -127,6 +127,8 @@ HESTON_GREEK_PARAMS = ("v0", "theta", "kappa", "rho", "volvol")
 # HawkesJDParams fields in dataclass order without mu (the Fourier route never reads it) and risk_premia_gamma (not covered)
 HAWKES_GREEK_PARAMS = ("sigma", "shift_p", "mean_p", "shift_m", "mean_m", "lambda_p", "theta_p", "kappa_p", "beta1_p", "beta2_p",
                        "lambda_m", "theta_m", "kappa_m", "beta1_m", "beta2_m")
+# the rows of the risk-kernel pricer's sensitivities (DESIGN.md §4.12)
+HAWKES_RISK_PREMIA_GREEK_PARAMS = HAWKES_GREEK_PARAMS + ("risk_premia_gamma",)
 
 
 def logsv_mc_chain_greeks(params: C.LogsvParamsC, ttms, forwards, discfactors, etas, strikes_ttms, optiontypes_ttms, nb_path: int,
@@ -711,6 +713,26 @@ def hawkesjd_price_chain_hessian(params: C.HawkesParamsC, ttms, forwards, discfa
     return _price_chain_hessian("b200sv_hawkesjd_price_chain_hessian", params, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms),
                                 (), is_spot_measure, (int(bool(is_spot_measure)),), vol_scaler, int(max_phi or 500), return_grids,
                                 HAWKES_GREEK_PARAMS, True)
+
+
+def hawkesjd_price_chain_risk_premia_greeks(params: C.HawkesParamsC, gamma: float, ttms, forwards, discfactors, strikes_ttms,
+                                            optiontypes_ttms, vol_scaler: Optional[float] = None, max_phi: Optional[int] = None,
+                                            return_grids: bool = False):
+    """Fourier prices and forward-mode sensitivities of the Hawkes chain under the risk kernel exp(-gamma x)
+    (b200sv_hawkesjd_price_chain_risk_premia_greeks; spot measure, calls and puts, DESIGN.md §4.12).  Returns (prices per maturity,
+    greeks [18, J], offsets) -- greeks rows: delta, gamma, then HAWKES_RISK_PREMIA_GREEK_PARAMS -- and with ``return_grids`` also
+    (dlog_mgf [16, M, P], dlog_norm [16, M, 2], nfev [P]); dlog_norm holds the derivatives of Re log-MGF at -gamma and -gamma - 1.  The
+    prices are bit-identical to hawkesjd_price_chain with the same gamma.  P defaults to the route's 500 points."""
+    ch = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
+    max_phi, n, J = int(max_phi or 500), len(HAWKES_RISK_PREMIA_GREEK_PARAMS), ch.strikes.shape[0]
+    prices, greeks = np.empty(J), np.empty((2 + n, J))
+    dlm = np.empty((n, ch.M, max_phi), dtype=np.complex128) if return_grids else None
+    dnorm = np.empty((n, ch.M, 2)) if return_grids else None
+    nfev = np.empty(max_phi, dtype=np.int32) if return_grids else None
+    C.call("b200sv_hawkesjd_price_chain_risk_premia_greeks", byref(params), *C.chain_ptrs(ch), 1, C.vol_scaler_arg(vol_scaler), max_phi,
+           float(gamma), C.dptr(prices), C.dptr(greeks), C.dptr(dlm), C.dptr(dnorm), C.iptr(nfev))
+    out = (C.split_chain(prices, ch.offsets), greeks, ch.offsets)
+    return out + (dlm, dnorm, nfev) if return_grids else out
 
 
 def logsv_price_chain_batch(params_list: Sequence[C.LogsvParamsC], ttms, forwards, discfactors, etas, strikes_ttms, optiontypes_ttms,

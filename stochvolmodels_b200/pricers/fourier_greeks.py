@@ -59,6 +59,9 @@ class ChainIvolHessian(ChainIvolGreeks):
     hessian: Dict[str, Dict[str, List[np.ndarray]]]
 
 
+_MAX_IVOL_ROWS = 15     # parameter rows per b200sv_bsm_implied_vol_sensitivities call
+
+
 def _flat(rows_ttms) -> np.ndarray:
     return np.concatenate([np.asarray(r, dtype=np.float64).ravel() for r in rows_ttms])
 
@@ -77,9 +80,14 @@ def to_chain_ivol_sensitivities(option_chain, greeks: FourierChainGreeks):
     second = isinstance(greeks, FourierChainHessian)
     vanna = np.vstack([_flat(greeks.vanna[n]) for n in names]) if second else None
     hessian = np.vstack([_flat(greeks.hessian[p][q]) for i, p in enumerate(names) for q in names[i:]]) if second else None
-    ivols, g, v, h = engine.bsm_implied_vol_sensitivities(option_chain.ttms, option_chain.forwards, option_chain.discfactors,
-                                                          option_chain.strikes_ttms, option_chain.optiontypes_ttms, greeks.prices, rows,
-                                                          vanna, hessian)
+    chain = (option_chain.ttms, option_chain.forwards, option_chain.discfactors, option_chain.strikes_ttms, option_chain.optiontypes_ttms)
+    ivols, g, v, h = engine.bsm_implied_vol_sensitivities(*chain, greeks.prices, rows[:2 + _MAX_IVOL_ROWS], vanna, hessian)
+    if rows.shape[0] > 2 + _MAX_IVOL_ROWS:
+        # a first-order parameter row maps on its own (d ivol / d p = d price / d p / vega): the rows past the transform's limit go through
+        # a further call on the same prices, with delta and gamma again in front
+        for r0 in range(2 + _MAX_IVOL_ROWS, rows.shape[0], _MAX_IVOL_ROWS):
+            more = engine.bsm_implied_vol_sensitivities(*chain, greeks.prices, np.vstack([rows[:2], rows[r0:r0 + _MAX_IVOL_ROWS]]))[1]
+            g = np.vstack([g, more[2:]])
     offsets = np.zeros(len(ivols) + 1, dtype=np.int64)
     offsets[1:] = np.cumsum([a.size for a in ivols])
     split = lambda row: C.split_chain(row, offsets)

@@ -87,6 +87,22 @@ def _params_c(**kw) -> C.HawkesParamsC:
     return C.HawkesParamsC(*[float(kw[k]) for k in _KEYS])
 
 
+def _check_risk_premia_greeks(option_chain: OptionChain, params: HawkesJDParams, is_spot_measure: bool, kwargs, method: str) -> float:
+    """what the risk-kernel sensitivities reject, before any library call; returns gamma"""
+    from .fourier_greeks import _check_fourier_kwargs
+    gamma = params.risk_premia_gamma
+    if gamma is None:
+        raise ValueError(f"{method} needs params.risk_premia_gamma; price_chain_greeks covers the pricer without a risk kernel")
+    if not np.isfinite(gamma):
+        raise ValueError(f"{method}: risk_premia_gamma must be finite, got {gamma}")
+    if kwargs.get("with_theta"):
+        raise NotImplementedError(f"{method} does not cover theta (with_theta) under the risk kernel")
+    _check_fourier_kwargs(kwargs, method)
+    if not is_spot_measure or any(str(t) not in ("C", "P") for types in option_chain.optiontypes_ttms for t in types):
+        raise ValueError("not implemented")           # utils/mgf_pricer.py:310-318, as price_chain
+    return float(gamma)
+
+
 class HawkesJDPricer(ModelPricer):
     """ModelPricer for the Hawkes jump-diffusion model: Fourier and Monte Carlo routes on the GPU."""
 
@@ -131,6 +147,34 @@ class HawkesJDPricer(ModelPricer):
             _params_c(**d), option_chain.ttms, option_chain.forwards, option_chain.discfactors, option_chain.strikes_ttms,
             option_chain.optiontypes_ttms, is_spot_measure=is_spot_measure, vol_scaler=kwargs.get("vol_scaler"), max_phi=MAX_PHI)
         return to_fourier_chain_hessian(prices, greeks, vanna, hessian, offsets, engine.HAWKES_GREEK_PARAMS)
+
+    def price_chain_risk_premia_greeks(self, option_chain: OptionChain, params: HawkesJDParams, is_spot_measure: bool = True, **kwargs):
+        """Fourier prices under the risk kernel exp(-gamma x), gamma = ``params.risk_premia_gamma`` (bit-identical to ``price_chain``
+        with the same arguments), plus forward-mode sensitivities in one call -> ``FourierChainGreeks`` keyed by
+        HAWKES_RISK_PREMIA_GREEK_PARAMS: delta and gamma in the slice forward, d price / d HAWKES_GREEK_PARAMS and d price /
+        d risk_premia_gamma, through the grid (which sits on Re phi = -1/2 - gamma), the two normaliser solves and K^(1 + gamma)
+        (DESIGN.md §4.12).  Exact on the solver's own meshes with the grid's imaginary parts held fixed: pin ``vol_scaler`` to compare
+        against re-pricings, since the default's dependence on ``sigma`` is not differentiated.  Rejects, before any GPU work: no
+        ``risk_premia_gamma`` (ValueError: ``price_chain_greeks`` covers the plain pricer), a non-finite one (ValueError), the BDF
+        branch, Q_VAR and ``with_theta`` (NotImplementedError), another measure or types other than 'C' / 'P' (ValueError, as
+        ``price_chain``)."""
+        from .fourier_greeks import to_fourier_chain_greeks
+        gamma = _check_risk_premia_greeks(option_chain, params, is_spot_measure, kwargs, "price_chain_risk_premia_greeks")
+        d = params.to_dict()
+        d.pop("risk_premia_gamma", None)
+        out = engine.hawkesjd_price_chain_risk_premia_greeks(
+            _params_c(**d), gamma, option_chain.ttms, option_chain.forwards, option_chain.discfactors, option_chain.strikes_ttms,
+            option_chain.optiontypes_ttms, vol_scaler=kwargs.get("vol_scaler"), max_phi=MAX_PHI)
+        return to_fourier_chain_greeks(*out, engine.HAWKES_RISK_PREMIA_GREEK_PARAMS)
+
+    def compute_chain_risk_premia_ivol_greeks(self, option_chain: OptionChain, params: HawkesJDParams, is_spot_measure: bool = True,
+                                              **kwargs):
+        """implied-vol sensitivities under the risk kernel -> ``ChainIvolGreeks`` keyed by HAWKES_RISK_PREMIA_GREEK_PARAMS, among them
+        d ivol / d risk_premia_gamma: ``price_chain_risk_premia_greeks`` mapped by the Black-76 transform (DESIGN.md §4.6).  The ivols are
+        bit-identical to ``compute_chain_prices_with_vols`` with the same arguments; same rejections as ``price_chain_risk_premia_greeks``."""
+        from .fourier_greeks import to_chain_ivol_sensitivities
+        _check_risk_premia_greeks(option_chain, params, is_spot_measure, kwargs, "compute_chain_risk_premia_ivol_greeks")
+        return to_chain_ivol_sensitivities(option_chain, self.price_chain_risk_premia_greeks(option_chain, params, is_spot_measure, **kwargs))
 
     @timer
     def model_mc_price_chain(self, option_chain: OptionChain, params: HawkesJDParams, nb_path: int = 100000, **kwargs
