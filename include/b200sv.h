@@ -392,6 +392,18 @@ int b200sv_hawkesjd_price_chain_risk_premia_greeks(const b200sv_hawkes_params* p
                                                    const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
                                                    int is_spot_measure, double vol_scaler, int P, double risk_premia_gamma, double* prices_out,
                                                    double* greeks_out, double* dlog_mgf_out, double* dlog_norm_out, int* nfev_out);
+/* second-order sensitivities of the Hawkes Fourier chain under the risk kernel (DESIGN.md §4.13).  The arguments and outputs of
+ * b200sv_hawkesjd_price_chain_risk_premia_greeks (bit-identical to it), then vanna_out [16][J]: d^2 price / d forwards[m] d parameter, and
+ * hessian_out [136][J]: d^2 price / d p d q for p <= q, the upper triangle row-major in the order of greeks_out's 16 parameter rows
+ * ((0,0), (0,1), .., (0,15), (1,1), ..), exact on the solver's own meshes with the grid's imaginary parts held fixed.  Optional (may be
+ * NULL): d2log_mgf_out [136][M][P] complex128 interleaved; d2log_norm_out [136][M][2]: the second derivatives of Re log-MGF at the
+ * normaliser points -gamma and -gamma - 1.  Return codes as b200sv_hawkesjd_price_chain_risk_premia_greeks (vanna_out and hessian_out are
+ * required); every check runs before any device work. */
+int b200sv_hawkesjd_price_chain_risk_premia_hessian(const b200sv_hawkes_params* params, int M, const double* ttms, const double* forwards,
+                                                    const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
+                                                    int is_spot_measure, double vol_scaler, int P, double risk_premia_gamma, double* prices_out,
+                                                    double* greeks_out, double* dlog_mgf_out, double* dlog_norm_out, int* nfev_out,
+                                                    double* vanna_out, double* hessian_out, double* d2log_mgf_out, double* d2log_norm_out);
 /* second-order sensitivities of the Hawkes Fourier chain without a risk kernel (DESIGN.md §4.5).  The arguments and outputs of
  * b200sv_hawkesjd_price_chain_greeks (bit-identical to it), then vanna_out [15][J]: d^2 price / d forwards[m] d parameter, and
  * hessian_out [120][J]: d^2 price / d p d q for p <= q, the upper triangle row-major in that parameter order ((0,0), (0,1), .., (0,14),

@@ -137,6 +137,8 @@ SIGNATURES = {
     "b200sv_hawkesjd_price_chain_greeks": [_kp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_double, c_int, _dp, _dp, _dp, _ip],
     "b200sv_hawkesjd_price_chain_risk_premia_greeks": [_kp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_double, c_int, c_double, _dp, _dp,
                                                        _dp, _dp, _ip],
+    "b200sv_hawkesjd_price_chain_risk_premia_hessian": [_kp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_double, c_int, c_double, _dp, _dp,
+                                                        _dp, _dp, _ip, _dp, _dp, _dp, _dp],
     "b200sv_logsv_price_chain_greeks_theta": [_lp, c_int, _dp, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_int, c_int, c_double, c_int, _dp, _dp, _dp,
                                               _ip, _dp, _dp, _ip],
     "b200sv_heston_price_chain_greeks_theta": [_hp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_double, c_int, _dp, _dp, _dp, _dp, _dp],

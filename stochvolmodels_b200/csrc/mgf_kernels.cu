@@ -2056,6 +2056,180 @@ __global__ void __launch_bounds__(kHawkesHessianTPB) hawkes_mgf_hessian_kernel(c
   }
 }
 
+// ---- Hawkes jump-diffusion under the risk kernel, second order (DESIGN.md §4.13) ----
+constexpr int kHawkesRpPairs = kHawkesRpDirs * (kHawkesRpDirs + 1) / 2;   // 105 pairs over the 13 ODE directions and phi
+
+// HawkesTan2RhsFn with the transform variable among the seeded variables: phi = (phi, dphi_p, dphi_q, 0), dphi = -1 on the gamma direction
+// and 0 on the ODE directions, so the hyper-dual algebra also forms every phi cross term (h0 = (phi + 1) phi / 2, comp phi and z = phi -
+// beta a inside the jump MGFs).  phi is linear in gamma: its own second part is zero.
+struct HawkesRpTan2RhsFn {
+  const HawkesMgfConsts& c;
+  HawkesMgfConsts dp, dq, d2;
+  hcd phi;
+  __device__ __forceinline__ hcd k(double HawkesMgfConsts::*f) const { return hcd{mk(c.*f), mk(dp.*f), mk(dq.*f), mk(d2.*f)}; }
+  __device__ __forceinline__ void operator()(const cd (&Y)[3], const cd (&dYp)[3], const cd (&dYq)[3], const cd (&d2Y)[3], cd (&op)[3],
+                                             cd (&oq)[3], cd (&opq)[3]) const {
+    using H = HawkesMgfConsts;
+    const hcd a1{Y[1], dYp[1], dYq[1], d2Y[1]}, a2{Y[2], dYp[2], dYq[2], d2Y[2]}, one = hmk(mk(1.0));
+    const hcd zp = (phi - k(&H::beta1_p) * a1) - k(&H::beta1_m) * a2, zm = (phi - k(&H::beta2_p) * a1) - k(&H::beta2_m) * a2;
+    const hcd jp = exp_(-(k(&H::shift_p) * zp)) / (one + k(&H::mean_p) * zp);
+    const hcd jm = exp_(-(k(&H::shift_m) * zm)) / (one + k(&H::mean_m) * zm);
+    const hcd h0 = 0.5 * ((phi + one) * phi);
+    const hcd o[3] = {(k(&H::kt_p) * a1 + k(&H::kt_m) * a2) + k(&H::sigma2) * h0, (jp - k(&H::kappa_p) * a1) + k(&H::comp_p) * phi,
+                      (jm - k(&H::kappa_m) * a2) + k(&H::comp_m) * phi};
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+      op[i] = o[i].d1;
+      oq[i] = o[i].d2;
+      opq[i] = o[i].d12;
+    }
+  }
+};
+
+// hawkes_mgf_hessian_kernel with the gamma direction of hawkes_mgf_rp_tangent_kernel: one thread = one (point, pair p <= q of the 14
+// directions), the primal integration of hawkes_mgf_kernel (same rk45_generic, same mesh) plus the tangents of p and q and their mixed
+// second-order tangent.  restart = 0: carried over the maturity increments dtaus (the grid); restart != 0: every maturity restarts from
+// A = 0 and integrates over its full ttm dtaus[m] (the normaliser points).  As there, the lambdas have no ODE tangent: the diagonal thread of
+// direction d writes (lambda_p, d) = da_p / dd and (lambda_m, d) = da_m / dd (for the phi direction da / dgamma = -da / dphi), pair 0 the
+// three lambda-lambda zeros.  d2c [105]: the second field derivatives per pair (zero on the pairs with phi).  Output d2log_mgf [136][M][P]
+// (tri_index over HAWKES_RISK_PREMIA_GREEK_PARAMS).
+__global__ void __launch_bounds__(kHawkesHessianTPB) hawkes_mgf_rp_hessian_kernel(const cd* __restrict__ phi, int P, int M,
+                                                                                  const double* __restrict__ dtaus, HawkesMgfConsts c,
+                                                                                  HawkesTangentDirs dirs, const HawkesMgfConsts* __restrict__ d2c,
+                                                                                  int restart, cd* __restrict__ d2log_mgf) {
+  constexpr int TPB = kHawkesHessianTPB, D = kHawkesRpDirs, NP = kHawkesRpParams;
+  __shared__ cd stage_smem[6 * 3 * TPB];
+  __shared__ cd tan_smem[3 * 8 * 3 * TPB];
+  const int t = blockIdx.x * TPB + threadIdx.x;
+  if (t >= P * kHawkesRpPairs) return;
+  const int p = t / kHawkesRpPairs, pair = t % kHawkesRpPairs;
+  int dp, dq;
+  tri_pair(pair, D, dp, dq);
+#pragma unroll
+  for (int i = 0; i < 18; ++i) stage_smem[threadIdx.x + i * TPB] = mk(0.0);
+#pragma unroll
+  for (int i = 0; i < 72; ++i) tan_smem[threadIdx.x + i * TPB] = mk(0.0);
+  StageStore<3, TPB> K{stage_smem + threadIdx.x};
+  const cd ph = phi[p];
+  const cd h0 = 0.5 * ((ph + mk(1.0)) * ph);
+  const HawkesRhsFn f{c, ph, c.sigma2 * h0};
+  const HawkesMgfConsts zero{0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+  const bool gp = dp == kHawkesOdeDirs, gq = dq == kHawkesOdeDirs;
+  const hcd hph{ph, mk(gp ? -1.0 : 0.0), mk(gq ? -1.0 : 0.0), mk(0.0)};
+  Tangent2Hook<3, TPB, HawkesRpTan2RhsFn> tan{HawkesRpTan2RhsFn{c, gp ? zero : dirs.d[dp], gq ? zero : dirs.d[dq], d2c[pair], hph},
+                                              {StageStore<3, TPB>{tan_smem + threadIdx.x}, {}},
+                                              {StageStore<3, TPB>{tan_smem + 24 * TPB + threadIdx.x}, {}},
+                                              {StageStore<3, TPB>{tan_smem + 48 * TPB + threadIdx.x}, {}}};   // dy = 0
+  cd A[3] = {mk(0.0), mk(0.0), mk(0.0)};
+  const int rp = gp ? kHawkesGreekParams : hawkes_dir_row(dp), rq = gq ? kHawkesGreekParams : hawkes_dir_row(dq);
+  for (int m = 0; m < M; ++m) {
+    if (restart) {
+#pragma unroll
+      for (int k = 0; k < 3; ++k) A[k] = tan.p.dy[k] = tan.q.dy[k] = tan.pq.dy[k] = mk(0.0);
+    }
+    rk45_generic<3, TPB>(A, dtaus[m], f, K, nullptr, &tan);
+    d2log_mgf[((size_t)tri_index(rp, rq, NP) * M + m) * P + p] = (tan.pq.dy[0] + tan.pq.dy[1] * c.lambda_p) + tan.pq.dy[2] * c.lambda_m;
+    if (dp == dq) {
+      d2log_mgf[((size_t)tri_index(min(5, rp), max(5, rp), NP) * M + m) * P + p] = tan.p.dy[1];
+      d2log_mgf[((size_t)tri_index(min(10, rp), max(10, rp), NP) * M + m) * P + p] = tan.p.dy[2];
+    }
+    if (pair == 0) {
+      d2log_mgf[((size_t)tri_index(5, 5, NP) * M + m) * P + p] = mk(0.0);
+      d2log_mgf[((size_t)tri_index(5, 10, NP) * M + m) * P + p] = mk(0.0);
+      d2log_mgf[((size_t)tri_index(10, 10, NP) * M + m) * P + p] = mk(0.0);
+    }
+  }
+}
+
+// The second-order risk-kernel sums next to fourier_gamma_greeks_kernel's (same weight branch, same NaN skip, fixed-order block_sum), a
+// strike split over the CTAs blockIdx.y as in fourier_vanilla_hessian_split_kernel.  With e = exp(lm - x phi), x = ln(F/K), the per-strike
+// tangents T_p = dlm_p (T_gamma = dlm_gamma + x) and T_pq = d2lm_pq:
+//   S = sum Re(w e),  S_x = sum Re(-w phi e),  S_p = sum Re(w e T_p),  S_xp = sum Re(w e (-phi T_p + [p = gamma])),
+//   S_pq = sum Re(w e (T_p T_q + T_pq)).
+// blockIdx.y = 0: S, S_x, S_p, S_xp and vanna_p = ([C] G g_p - c (S_xp + c_p S_x)) / F;  blockIdx.y = b > 0: S, S_p and the Hessian rows
+// [(b - 1) NP, b NP):  hessian_pq = [C] G (g_p g_q + g_pq) - c (S_pq + c_p S_q + c_q S_p + (c_p c_q + c_pq) S),  with c = n K^(1+gamma),
+// g = l1 - l0, c_p = -l0_p [+ ln K for gamma], c_pq = -l0_pq; l0 / l1 the normaliser log-MGFs (Re dnorm [16][M][2], Re d2norm [136][M][2])
+// and (n, G) = norm_gfwd [M][2], the pricing route's own.  vanna [16][J], hessian [136][J] (tri_index rows).
+__global__ void __launch_bounds__(kFourierThreads) fourier_gamma_hessian_kernel(const cd* __restrict__ log_mgf, const cd* __restrict__ dlog_mgf,
+                                                                               const cd* __restrict__ d2log_mgf, const cd* __restrict__ dnorm,
+                                                                               const cd* __restrict__ d2norm, const cd* __restrict__ phi,
+                                                                               int P, int M, const StrikeSpec* __restrict__ specs,
+                                                                               double gamma, const double* __restrict__ norm_gfwd,
+                                                                               double* __restrict__ vanna, double* __restrict__ hessian) {
+  constexpr int NP = kHawkesRpParams, NH = NP * (NP + 1) / 2, R = NP;     // Hessian rows per CTA
+  const StrikeSpec sp = specs[blockIdx.x];
+  const cd* lm = log_mgf + (size_t)sp.slice * P;
+  const double x = log(sp.forward / sp.strike);
+  const size_t rs = (size_t)M * P;                                         // the row stride of dlog_mgf / d2log_mgf
+  const cd* dl = dlog_mgf + (size_t)sp.slice * P;
+  const cd* d2l = d2log_mgf + (size_t)sp.slice * P;
+  const bool fast = fabs(phi[0].re - (0.5 + gamma)) < 1e-10;
+  const bool vanna_rows = blockIdx.y == 0;
+  const int r0 = vanna_rows ? 0 : ((int)blockIdx.y - 1) * R;
+  int p0 = 0, q0 = 0;
+  if (!vanna_rows) tri_pair(r0, NP, p0, q0);
+  // acc: S, S_x | S_p [NP] | the vanna CTA's S_xp [NP] or a Hessian CTA's S_pq [R]
+  double acc[2 + 2 * NP] = {};
+  strike_sum(phi, P, acc, [&](int j, double dp, cd ph) {
+    const cd pg = ph + mk(gamma);
+    const cd w = fast ? mk((dp / M_PI) / (ph.im * ph.im + 0.25)) : -(mk(dp / M_PI) / ((pg + mk(1.0)) * pg));
+    const cd e = cexp_(lm[j] - x * ph);
+    const cd term = w * e;
+    if (term.re == term.re) {
+      const auto T = [&](int k) {
+        const cd v = dl[k * rs + j];
+        return k == NP - 1 ? v + mk(x) : v;
+      };
+      acc[0] += term.re;
+#pragma unroll
+      for (int k = 0; k < NP; ++k) acc[2 + k] += (term * T(k)).re;
+      if (vanna_rows) {
+        acc[1] += (w * -(ph * e)).re;
+#pragma unroll
+        for (int k = 0; k < NP; ++k) acc[2 + NP + k] += (term * (k == NP - 1 ? mk(1.0) - ph * T(k) : -(ph * T(k)))).re;
+      } else {
+        int p = p0, q = q0;
+#pragma unroll
+        for (int i = 0; i < R; ++i) {
+          const int r = r0 + i;
+          if (r < NH) acc[2 + NP + i] += (term * (T(p) * T(q) + d2l[r * rs + j])).re;
+          if (++q == NP) q = ++p;
+        }
+      }
+    }
+  });
+  if (threadIdx.x == 0) {
+    const double S = acc[0], F = sp.forward, K = sp.strike;
+    const double n = norm_gfwd[2 * (size_t)sp.slice], G = norm_gfwd[2 * (size_t)sp.slice + 1], ngk = n * pow(K, 1.0 + gamma);
+    const int J = gridDim.x;
+    const bool call = sp.type == B200SV_CALL;
+    const auto l0 = [&](const cd* v, int r) { return v[((size_t)r * M + sp.slice) * 2].re; };
+    const auto l1 = [&](const cd* v, int r) { return v[((size_t)r * M + sp.slice) * 2 + 1].re; };
+    const auto cp = [&](int k) { return -l0(dnorm, k) + (k == NP - 1 ? log(K) : 0.0); };
+    if (vanna_rows) {
+#pragma unroll
+      for (int k = 0; k < NP; ++k)
+        vanna[(size_t)k * J + blockIdx.x] = ((call ? G * (l1(dnorm, k) - l0(dnorm, k)) : 0.0) - ngk * (acc[2 + NP + k] + cp(k) * acc[1])) / F;
+    } else {
+      __shared__ double Sp[NP];             // S_p by a run-time index, without moving acc to local memory
+#pragma unroll
+      for (int k = 0; k < NP; ++k) Sp[k] = acc[2 + k];
+      int p = p0, q = q0;
+#pragma unroll
+      for (int i = 0; i < R; ++i) {
+        const int r = r0 + i;
+        if (r < NH) {
+          const double gp = l1(dnorm, p) - l0(dnorm, p), gq = l1(dnorm, q) - l0(dnorm, q), gpq = l1(d2norm, r) - l0(d2norm, r);
+          const double cpp = cp(p), cqq = cp(q), cpq = -l0(d2norm, r);
+          hessian[(size_t)r * J + blockIdx.x] = (call ? G * (gp * gq + gpq) : 0.0) -
+                                                ngk * (((acc[2 + NP + i] + cpp * Sp[q]) + cqq * Sp[p]) + (cpp * cqq + cpq) * S);
+        }
+        if (++q == NP) q = ++p;
+      }
+    }
+  }
+}
+
 // --------------------------------------------------------------------------------------------------------------------
 // Theta of the Fourier chain pricers (DESIGN.md §4.8): d log_mgf / d T_m with the accepted mesh t_0 < ... < t_{K-1} of slice m held and
 // only its last step h_K = T_m - t_{K-1} moving (dh_K / dT_m = 1); earlier maturities, the backbone and the grid are held.
@@ -3317,6 +3491,44 @@ static int queue_hawkes_greeks(ChainDev& d, GreeksDev<kHawkesGreekParams>& t, co
   return t.sums(d, c, t.lm.as<cd>());
 }
 
+// The device side of the risk kernel's normaliser points, kept for the launches that follow the first-order ones: gamma, (normaliser, gamma
+// forward) ng [M][2], the two points (-gamma, -gamma - 1), ttms [M] and the restarted tangents dn [16][M][2] (complex).
+struct HawkesRpDev {
+  DevBuf gam, ng, two, ttm, dn;
+  explicit HawkesRpDev(cudaStream_t s) : gam(s), ng(s), two(s), ttm(s), dn(s) {}
+};
+
+// The first-order launches of b200sv_hawkesjd_price_chain_risk_premia_greeks on a prepared chain (DESIGN.md §4.12): the pricing launches of
+// b200sv_hawkesjd_price_chain with the gamma (the restarted normaliser launch, its one synchronisation, the Riccati launch and the gamma
+// sums: bit-identical prices), then hawkes_mgf_rp_tangent_kernel at the two normaliser points (restarted) and on the grid (carried), and
+// fourier_gamma_greeks_kernel on the grid tangent kernel's own primal log-MGF (no launch on an empty chain).
+static int queue_hawkes_rp_greeks(ChainDev& d, GreeksDev<kHawkesRpParams>& g, HawkesRpDev& r, const FourierChain& c,
+                                  const b200sv_hawkes_params& params, const HawkesMgfConsts& k, const double* ttms, const double* forwards,
+                                  double gamma, double* prices_out) {
+  const int M = c.M, P = c.P;
+  std::vector<double> ng;
+  if (int rc = risk_kernel_normalizers(d.st, &k, &gamma, 1, M, ttms, forwards, ng)) return rc;
+  B200SV_CUDA(r.gam.upload(&gamma, 1));
+  B200SV_CUDA(r.ng.upload(ng.data(), ng.size()));
+  if (int rc = queue_hawkes_prices(d, c, &k, prices_out, nullptr, r.gam.as<double>(), r.ng.as<double>())) return rc;
+  const HawkesTangentDirs dirs = make_hawkes_tangents(params);
+  const double two[4] = {-gamma, 0.0, -gamma - 1.0, 0.0};
+  B200SV_CUDA(r.two.upload(cplx(two), 2));
+  B200SV_CUDA(r.ttm.upload(ttms, M));
+  B200SV_CUDA(r.dn.alloc(sizeof(cd) * (size_t)kHawkesRpParams * M * 2));
+  launch_hawkes_mgf_rp_tangent(d.st, r.two.as<cd>(), 2, M, r.ttm.as<double>(), k, dirs, 1, r.dn.as<cd>(), nullptr, nullptr);
+  if (int rc = check_launch("hawkes_mgf_rp_tangent_kernel")) return rc;
+  if (int rc = g.alloc(c, true)) return rc;
+  launch_hawkes_mgf_rp_tangent(d.st, d.phi.as<cd>(), P, M, d.dt.as<double>(), k, dirs, 0, g.dlm.as<cd>(), g.lm.as<cd>(), g.nfev.as<int>());
+  if (int rc = check_launch("hawkes_mgf_rp_tangent_kernel")) return rc;
+  if (c.Jtot > 0) {
+    fourier_gamma_greeks_kernel<<<c.Jtot, kFourierThreads, 0, d.st>>>(g.lm.as<cd>(), g.dlm.as<cd>(), r.dn.as<cd>(), d.phi.as<cd>(), P, M,
+                                                                      d.rows.as<StrikeSpec>(), gamma, r.ng.as<double>(), g.g.as<double>());
+    if (int rc = check_launch("fourier_gamma_greeks_kernel")) return rc;
+  }
+  return 0;
+}
+
 // The second-order sums of b200sv_*_price_chain_hessian after its Hessian kernel wrote d2lm [NH][M][P]: fourier_vanilla_hessian_kernel
 // (fourier_vanilla_hessian_split_kernel for Hawkes' 15 parameters) on log_mgf and the first-order tangents dlm [NP][M][P] (no launch on an
 // empty chain), then vanna, the Hessian rows and d2lm come back; the first-order outputs follow with GreeksDev::download().
@@ -3968,10 +4180,8 @@ int b200sv_hawkesjd_price_chain_greeks(const b200sv_hawkes_params* params, int M
   return g.download(d, c, greeks_out, dlog_mgf_out, nfev_out);
 }
 
-/* Forward-mode sensitivities of the Hawkes Fourier chain under the risk kernel (DESIGN.md §4.12): the pricing launches of
- * b200sv_hawkesjd_price_chain with risk_premia_gamma unchanged (the restarted normaliser launch, its one synchronisation, the Riccati
- * launch and the gamma sums: bit-identical prices), then hawkes_mgf_rp_tangent_kernel at the two normaliser points (restarted) and on the
- * grid (carried), and fourier_gamma_greeks_kernel on the grid tangent kernel's own primal log-MGF; one synchronisation at the end.
+/* Forward-mode sensitivities of the Hawkes Fourier chain under the risk kernel (DESIGN.md §4.12): the launches of
+ * queue_hawkes_rp_greeks (bit-identical prices to b200sv_hawkesjd_price_chain with the same gamma); one synchronisation at the end.
  * greeks_out [2 + 16][J]: delta, gamma, HAWKES_GREEK_PARAMS, risk_premia_gamma.  Optional: dlog_mgf_out [16][M][P] (complex),
  * dlog_norm_out [16][M][2] (the derivatives of Re log-MGF at -gamma and -gamma - 1), nfev_out [P]. */
 int b200sv_hawkesjd_price_chain_risk_premia_greeks(const b200sv_hawkes_params* params, int M, const double* ttms, const double* forwards,
@@ -3984,37 +4194,76 @@ int b200sv_hawkesjd_price_chain_risk_premia_greeks(const b200sv_hawkes_params* p
   if (int rc = prepare_hawkes_chain(c, params, M, ttms, forwards, discfactors, offsets, strikes, types, is_spot_measure, vol_scaler, P,
                                     risk_premia_gamma))
     return rc;
-  P = c.P;
   constexpr int NP = kHawkesRpParams;
   const HawkesMgfConsts k = make_hawkes_mgf_consts(*params);
   ChainDev d;
-  DevBuf d_gam(d.st), d_ng(d.st), d_two(d.st), d_ttm(d.st), d_dn(d.st);
-  std::vector<double> ng;
-  if (int rc = risk_kernel_normalizers(d.st, &k, &risk_premia_gamma, 1, M, ttms, forwards, ng)) return rc;
-  B200SV_CUDA(d_gam.upload(&risk_premia_gamma, 1));
-  B200SV_CUDA(d_ng.upload(ng.data(), ng.size()));
-  if (int rc = queue_hawkes_prices(d, c, &k, prices_out, nullptr, d_gam.as<double>(), d_ng.as<double>())) return rc;
-  const HawkesTangentDirs dirs = make_hawkes_tangents(*params);
-  const double two[4] = {-risk_premia_gamma, 0.0, -risk_premia_gamma - 1.0, 0.0};
-  B200SV_CUDA(d_two.upload(cplx(two), 2));
-  B200SV_CUDA(d_ttm.upload(ttms, M));
-  B200SV_CUDA(d_dn.alloc(sizeof(cd) * (size_t)NP * M * 2));
-  launch_hawkes_mgf_rp_tangent(d.st, d_two.as<cd>(), 2, M, d_ttm.as<double>(), k, dirs, 1, d_dn.as<cd>(), nullptr, nullptr);
-  if (int rc = check_launch("hawkes_mgf_rp_tangent_kernel")) return rc;
+  HawkesRpDev r(d.st);
   GreeksDev<NP> g(d.st);
-  if (int rc = g.alloc(c, true)) return rc;
-  launch_hawkes_mgf_rp_tangent(d.st, d.phi.as<cd>(), P, M, d.dt.as<double>(), k, dirs, 0, g.dlm.as<cd>(), g.lm.as<cd>(), g.nfev.as<int>());
-  if (int rc = check_launch("hawkes_mgf_rp_tangent_kernel")) return rc;
-  if (c.Jtot > 0) {
-    fourier_gamma_greeks_kernel<<<c.Jtot, kFourierThreads, 0, d.st>>>(g.lm.as<cd>(), g.dlm.as<cd>(), d_dn.as<cd>(), d.phi.as<cd>(), P, M,
-                                                                      d.rows.as<StrikeSpec>(), risk_premia_gamma, d_ng.as<double>(),
-                                                                      g.g.as<double>());
-    if (int rc = check_launch("fourier_gamma_greeks_kernel")) return rc;
-  }
+  if (int rc = queue_hawkes_rp_greeks(d, g, r, c, *params, k, ttms, forwards, risk_premia_gamma, prices_out)) return rc;
   std::vector<cd> dn(dlog_norm_out ? (size_t)NP * M * 2 : 0);
-  B200SV_CUDA(d_dn.download(dlog_norm_out ? dn.data() : nullptr, dn.size()));
+  B200SV_CUDA(r.dn.download(dlog_norm_out ? dn.data() : nullptr, dn.size()));
   if (int rc = g.download(d, c, greeks_out, dlog_mgf_out, nfev_out)) return rc;
   for (size_t i = 0; i < dn.size(); ++i) dlog_norm_out[i] = dn[i].re;
+  return 0;
+}
+
+/* Second-order sensitivities of the Hawkes Fourier chain under the risk kernel (DESIGN.md §4.13): the launches of
+ * b200sv_hawkesjd_price_chain_risk_premia_greeks unchanged (bit-identical first-order outputs), then hawkes_mgf_rp_hessian_kernel at the
+ * two normaliser points (restarted) and on the grid (carried), and fourier_gamma_hessian_kernel; one synchronisation at the end. */
+int b200sv_hawkesjd_price_chain_risk_premia_hessian(const b200sv_hawkes_params* params, int M, const double* ttms, const double* forwards,
+                                                    const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
+                                                    int is_spot_measure, double vol_scaler, int P, double risk_premia_gamma, double* prices_out,
+                                                    double* greeks_out, double* dlog_mgf_out, double* dlog_norm_out, int* nfev_out,
+                                                    double* vanna_out, double* hessian_out, double* d2log_mgf_out, double* d2log_norm_out) {
+  B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && greeks_out && vanna_out && hessian_out, "null pointer");
+  B200SV_REQUIRE(std::isfinite(risk_premia_gamma), "risk_premia_gamma must be finite");
+  FourierChain c;
+  if (int rc = prepare_hawkes_chain(c, params, M, ttms, forwards, discfactors, offsets, strikes, types, is_spot_measure, vol_scaler, P,
+                                    risk_premia_gamma))
+    return rc;
+  P = c.P;
+  constexpr int NP = kHawkesRpParams, NH = NP * (NP + 1) / 2, TPB = kHawkesHessianTPB;
+  const HawkesMgfConsts k = make_hawkes_mgf_consts(*params);
+  ChainDev d;
+  HawkesRpDev r(d.st);
+  GreeksDev<NP> g(d.st);
+  if (int rc = queue_hawkes_rp_greeks(d, g, r, c, *params, k, ttms, forwards, risk_premia_gamma, prices_out)) return rc;
+  // the second field derivatives per pair of the 14 directions: make_hawkes_hessian's on the ODE pairs, none with phi
+  HawkesMgfConsts h[kHawkesOdePairs], h2[kHawkesRpPairs];
+  make_hawkes_hessian(*params, h);
+  for (int a = 0; a < kHawkesRpDirs; ++a)
+    for (int b = a; b < kHawkesRpDirs; ++b)
+      h2[tri_index(a, b, kHawkesRpDirs)] = b < kHawkesOdeDirs ? h[tri_index(a, b, kHawkesOdeDirs)]
+                                                              : HawkesMgfConsts{0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+  const HawkesTangentDirs dirs = make_hawkes_tangents(*params);
+  DevBuf d_d2c(d.st), d_d2n(d.st), d_d2lm(d.st), d_v(d.st), d_h(d.st);
+  B200SV_CUDA(d_d2c.upload(h2, kHawkesRpPairs));
+  B200SV_CUDA(d_d2n.alloc(sizeof(cd) * (size_t)NH * M * 2));
+  B200SV_CUDA(d_d2lm.alloc(sizeof(cd) * (size_t)NH * M * P));
+  hawkes_mgf_rp_hessian_kernel<<<(2 * kHawkesRpPairs + TPB - 1) / TPB, TPB, 0, d.st>>>(r.two.as<cd>(), 2, M, r.ttm.as<double>(), k, dirs,
+                                                                                       d_d2c.as<HawkesMgfConsts>(), 1, d_d2n.as<cd>());
+  if (int rc = check_launch("hawkes_mgf_rp_hessian_kernel")) return rc;
+  hawkes_mgf_rp_hessian_kernel<<<(P * kHawkesRpPairs + TPB - 1) / TPB, TPB, 0, d.st>>>(d.phi.as<cd>(), P, M, d.dt.as<double>(), k, dirs,
+                                                                                       d_d2c.as<HawkesMgfConsts>(), 0, d_d2lm.as<cd>());
+  if (int rc = check_launch("hawkes_mgf_rp_hessian_kernel")) return rc;
+  if (c.Jtot > 0) {       // the vanna CTA and NH / NP Hessian CTAs per strike
+    B200SV_CUDA(d_v.alloc(sizeof(double) * (size_t)NP * c.Jtot));
+    B200SV_CUDA(d_h.alloc(sizeof(double) * (size_t)NH * c.Jtot));
+    const dim3 grid(c.Jtot, 1 + (NH + NP - 1) / NP);
+    fourier_gamma_hessian_kernel<<<grid, kFourierThreads, 0, d.st>>>(g.lm.as<cd>(), g.dlm.as<cd>(), d_d2lm.as<cd>(), r.dn.as<cd>(),
+                                                                     d_d2n.as<cd>(), d.phi.as<cd>(), P, M, d.rows.as<StrikeSpec>(),
+                                                                     risk_premia_gamma, r.ng.as<double>(), d_v.as<double>(), d_h.as<double>());
+    if (int rc = check_launch("fourier_gamma_hessian_kernel")) return rc;
+    B200SV_CUDA(d_v.download(vanna_out, (size_t)NP * c.Jtot));
+    B200SV_CUDA(d_h.download(hessian_out, (size_t)NH * c.Jtot));
+  }
+  B200SV_CUDA(d_d2lm.download(cplx(d2log_mgf_out), (size_t)NH * M * P));
+  std::vector<cd> dn(dlog_norm_out ? (size_t)NP * M * 2 : 0), d2n(d2log_norm_out ? (size_t)NH * M * 2 : 0);
+  B200SV_CUDA(r.dn.download(dlog_norm_out ? dn.data() : nullptr, dn.size()));
+  B200SV_CUDA(d_d2n.download(d2log_norm_out ? d2n.data() : nullptr, d2n.size()));
+  if (int rc = g.download(d, c, greeks_out, dlog_mgf_out, nfev_out)) return rc;
+  for (size_t i = 0; i < dn.size(); ++i) dlog_norm_out[i] = dn[i].re;
+  for (size_t i = 0; i < d2n.size(); ++i) d2log_norm_out[i] = d2n[i].re;
   return 0;
 }
 

@@ -735,6 +735,30 @@ def hawkesjd_price_chain_risk_premia_greeks(params: C.HawkesParamsC, gamma: floa
     return out + (dlm, dnorm, nfev) if return_grids else out
 
 
+def hawkesjd_price_chain_risk_premia_hessian(params: C.HawkesParamsC, gamma: float, ttms, forwards, discfactors, strikes_ttms,
+                                             optiontypes_ttms, vol_scaler: Optional[float] = None, max_phi: Optional[int] = None,
+                                             return_grids: bool = False):
+    """hawkesjd_price_chain_risk_premia_greeks plus the second-order sensitivities (b200sv_hawkesjd_price_chain_risk_premia_hessian,
+    DESIGN.md §4.13): vanna [16, J] and hessian [136, J] over HAWKES_RISK_PREMIA_GREEK_PARAMS (upper triangle, row-major).  Returns
+    (prices per maturity, greeks [18, J], vanna, hessian, offsets) and with ``return_grids`` also (dlog_mgf [16, M, P], dlog_norm [16, M, 2],
+    nfev [P], d2log_mgf [136, M, P], d2log_norm [136, M, 2]); d2log_norm holds the second derivatives of Re log-MGF at -gamma and
+    -gamma - 1.  The first-order outputs are bit-identical to hawkesjd_price_chain_risk_premia_greeks."""
+    ch = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
+    max_phi, n, J = int(max_phi or 500), len(HAWKES_RISK_PREMIA_GREEK_PARAMS), ch.strikes.shape[0]
+    nh = n * (n + 1) // 2
+    prices, greeks, vanna, hessian = np.empty(J), np.empty((2 + n, J)), np.empty((n, J)), np.empty((nh, J))
+    dlm = np.empty((n, ch.M, max_phi), dtype=np.complex128) if return_grids else None
+    dnorm = np.empty((n, ch.M, 2)) if return_grids else None
+    nfev = np.empty(max_phi, dtype=np.int32) if return_grids else None
+    d2lm = np.empty((nh, ch.M, max_phi), dtype=np.complex128) if return_grids else None
+    d2norm = np.empty((nh, ch.M, 2)) if return_grids else None
+    C.call("b200sv_hawkesjd_price_chain_risk_premia_hessian", byref(params), *C.chain_ptrs(ch), 1, C.vol_scaler_arg(vol_scaler), max_phi,
+           float(gamma), C.dptr(prices), C.dptr(greeks), C.dptr(dlm), C.dptr(dnorm), C.iptr(nfev), C.dptr(vanna), C.dptr(hessian),
+           C.dptr(d2lm), C.dptr(d2norm))
+    out = (C.split_chain(prices, ch.offsets), greeks, vanna, hessian, ch.offsets)
+    return out + (dlm, dnorm, nfev, d2lm, d2norm) if return_grids else out
+
+
 def logsv_price_chain_batch(params_list: Sequence[C.LogsvParamsC], ttms, forwards, discfactors, etas, strikes_ttms, optiontypes_ttms,
                             is_spot_measure: bool = True, expansion_order: int = C.ORDER_SECOND, vol_scaler: Optional[float] = None,
                             max_phi: int = 1000, with_ivols: bool = True):

@@ -71,23 +71,44 @@ def to_chain_ivol_sensitivities(option_chain, greeks: FourierChainGreeks):
     rows on the chain's forwards and discount factors by one engine.bsm_implied_vol_sensitivities call.  A Monte Carlo ``McChainGreeks``
     maps the same way (its standard errors are not carried over); without a gamma row (``gamma`` None) the transform gets zeros in its place
     and the result has ``gamma=None``, the other rows being independent of it.  A ``theta`` row is mapped by a second call,
-    engine.bsm_implied_vol_theta, on the same prices (the same ivols, bit for bit)."""
+    engine.bsm_implied_vol_theta, on the same prices (the same ivols, bit for bit).  Past the transform's 15 parameter rows, further calls
+    on the same prices map the remaining rows, first or second order (DESIGN.md §4.12, §4.13)."""
     from .. import engine
     names = list(greeks.params)
     delta = _flat(greeks.delta)
     gamma = np.zeros_like(delta) if greeks.gamma is None else _flat(greeks.gamma)
     rows = np.vstack([delta, gamma, *(_flat(greeks.params[n]) for n in names)])
     second = isinstance(greeks, FourierChainHessian)
-    vanna = np.vstack([_flat(greeks.vanna[n]) for n in names]) if second else None
-    hessian = np.vstack([_flat(greeks.hessian[p][q]) for i, p in enumerate(names) for q in names[i:]]) if second else None
+    head = names[:_MAX_IVOL_ROWS]
+    tri = lambda group: np.vstack([_flat(greeks.hessian[p][q]) for i, p in enumerate(group) for q in group[i:]])
+    vanna = np.vstack([_flat(greeks.vanna[n]) for n in head]) if second else None
+    hessian = tri(head) if second else None
     chain = (option_chain.ttms, option_chain.forwards, option_chain.discfactors, option_chain.strikes_ttms, option_chain.optiontypes_ttms)
     ivols, g, v, h = engine.bsm_implied_vol_sensitivities(*chain, greeks.prices, rows[:2 + _MAX_IVOL_ROWS], vanna, hessian)
-    if rows.shape[0] > 2 + _MAX_IVOL_ROWS:
+    pair_rows = {(p, q): h[r] for r, (p, q) in enumerate((p, q) for i, p in enumerate(head) for q in head[i:])} if second else None
+    if rows.shape[0] > 2 + _MAX_IVOL_ROWS and not second:
         # a first-order parameter row maps on its own (d ivol / d p = d price / d p / vega): the rows past the transform's limit go through
         # a further call on the same prices, with delta and gamma again in front
         for r0 in range(2 + _MAX_IVOL_ROWS, rows.shape[0], _MAX_IVOL_ROWS):
             more = engine.bsm_implied_vol_sensitivities(*chain, greeks.prices, np.vstack([rows[:2], rows[r0:r0 + _MAX_IVOL_ROWS]]))[1]
             g = np.vstack([g, more[2:]])
+    elif rows.shape[0] > 2 + _MAX_IVOL_ROWS:
+        # second order past the limit: sigma_pq = (P_pq - B_ss sigma_p sigma_q) / B_s and vanna_p need only the rows of p and q, so each
+        # further name e goes through calls on the same prices with e first and at most 14 of the names before it, [e, p1..p14], [e, p15],
+        # ...; e's first-order row, vanna and (e, e) come from its first call, each (e, q) from the call that holds q
+        v = list(v)
+        for i in range(_MAX_IVOL_ROWS, len(names)):
+            e = names[i]
+            for c0 in range(0, i, _MAX_IVOL_ROWS - 1):
+                group = [e] + names[c0:min(i, c0 + _MAX_IVOL_ROWS - 1)]
+                sel = [names.index(n) for n in group]
+                _, mg, mv, mh = engine.bsm_implied_vol_sensitivities(*chain, greeks.prices, np.vstack([rows[:2], rows[[2 + k for k in sel]]]),
+                                                                     np.vstack([_flat(greeks.vanna[n]) for n in group]), tri(group))
+                if c0 == 0:
+                    g, v = np.vstack([g, mg[2:3]]), v + [mv[0]]
+                    pair_rows[(e, e)] = mh[0]
+                for k, q in enumerate(group[1:], 1):
+                    pair_rows[(q, e)] = mh[k]
     offsets = np.zeros(len(ivols) + 1, dtype=np.int64)
     offsets[1:] = np.cumsum([a.size for a in ivols])
     split = lambda row: C.split_chain(row, offsets)
@@ -101,11 +122,9 @@ def to_chain_ivol_sensitivities(option_chain, greeks: FourierChainGreeks):
     if not second:
         return first
     hess: Dict[str, Dict[str, List[np.ndarray]]] = {n: {} for n in names}
-    r = 0
     for i, p in enumerate(names):
         for q in names[i:]:
-            hess[p][q] = hess[q][p] = split(h[r])
-            r += 1
+            hess[p][q] = hess[q][p] = split(pair_rows[(p, q)])
     return ChainIvolHessian(ivols=first.ivols, delta=first.delta, gamma=first.gamma, params=first.params,
                             vanna={n: split(v[k]) for k, n in enumerate(names)}, hessian=hess)
 

@@ -176,6 +176,30 @@ class HawkesJDPricer(ModelPricer):
         _check_risk_premia_greeks(option_chain, params, is_spot_measure, kwargs, "compute_chain_risk_premia_ivol_greeks")
         return to_chain_ivol_sensitivities(option_chain, self.price_chain_risk_premia_greeks(option_chain, params, is_spot_measure, **kwargs))
 
+    def price_chain_risk_premia_hessian(self, option_chain: OptionChain, params: HawkesJDParams, is_spot_measure: bool = True, **kwargs):
+        """``price_chain_risk_premia_greeks`` (bit for bit) plus the second order in one call -> ``FourierChainHessian`` keyed by
+        HAWKES_RISK_PREMIA_GREEK_PARAMS: vanna (d^2 price / d forward d parameter) and the symmetric Hessian d^2 price / d p d q, the
+        curvature in ``risk_premia_gamma`` included, through the grid, the two normaliser solves and K^(1 + gamma) (DESIGN.md §4.13).  The
+        exact second derivatives of the scheme on the solver's own meshes with the grid's imaginary parts held fixed; same conventions and
+        the same rejections as ``price_chain_risk_premia_greeks``."""
+        from .fourier_greeks import to_fourier_chain_hessian
+        gamma = _check_risk_premia_greeks(option_chain, params, is_spot_measure, kwargs, "price_chain_risk_premia_hessian")
+        d = params.to_dict()
+        d.pop("risk_premia_gamma", None)
+        prices, greeks, vanna, hessian, offsets = engine.hawkesjd_price_chain_risk_premia_hessian(
+            _params_c(**d), gamma, option_chain.ttms, option_chain.forwards, option_chain.discfactors, option_chain.strikes_ttms,
+            option_chain.optiontypes_ttms, vol_scaler=kwargs.get("vol_scaler"), max_phi=MAX_PHI)
+        return to_fourier_chain_hessian(prices, greeks, vanna, hessian, offsets, engine.HAWKES_RISK_PREMIA_GREEK_PARAMS)
+
+    def compute_chain_risk_premia_ivol_hessian(self, option_chain: OptionChain, params: HawkesJDParams, is_spot_measure: bool = True,
+                                               **kwargs):
+        """implied-vol second order under the risk kernel -> ``ChainIvolHessian`` keyed by HAWKES_RISK_PREMIA_GREEK_PARAMS:
+        ``price_chain_risk_premia_hessian`` mapped by the Black-76 transform (DESIGN.md §4.6, §4.13).  The ivols are bit-identical to
+        ``compute_chain_prices_with_vols`` with the same arguments; same rejections as ``price_chain_risk_premia_greeks``."""
+        from .fourier_greeks import to_chain_ivol_sensitivities
+        _check_risk_premia_greeks(option_chain, params, is_spot_measure, kwargs, "compute_chain_risk_premia_ivol_hessian")
+        return to_chain_ivol_sensitivities(option_chain, self.price_chain_risk_premia_hessian(option_chain, params, is_spot_measure, **kwargs))
+
     @timer
     def model_mc_price_chain(self, option_chain: OptionChain, params: HawkesJDParams, nb_path: int = 100000, **kwargs
                              ) -> Tuple[List[np.ndarray], List[np.ndarray]]:
