@@ -424,6 +424,28 @@ int b200sv_hawkesjd_terminal(const b200sv_hawkes_params* params, double ttm, lon
                              int use_initial_arrays, double* x_inout, double* lambda_p_inout, double* lambda_m_inout);
 int b200sv_hawkesjd_step_fixed(double* x, double* lambda_p, double* lambda_m, const double* W0, const double* U_P, const double* U_M,
                                const double* J_P, const double* J_M, int S, long long N, double dt, const b200sv_hawkes_params* params);
+/* Exact event-driven Monte Carlo of the Hawkes jump-diffusion (DESIGN.md §3.13): no time grid.  Per path and maturity interval the jumps
+ * are simulated event by event by thinning against the sum over both intensities of the largest value of their deterministic path until
+ * the interval end (max(lambda, theta, 0) for kappa >= 0, max(lambda, lambda(T), 0) for kappa < 0, any sign of kappa is exact), the
+ * intensities move in closed form between events, the compensator c lambda (c = e^shift / (1 - mean) - 1) is integrated exactly and the diffusion is one
+ * fp64 normal per interval.  The continuous-time limit of b200sv_hawkesjd_mc_chain's Euler step; where the intensities cannot become
+ * negative (lambda0, theta >= 0, beta1_p, beta1_m >= 0, beta2_p, beta2_m <= 0) the model the Fourier route prices.  Draws: Philox keyed
+ * by seed, counter (global path id, candidate index | 0xFFFFFFFF for the normal, maturity index | 0xC0000000), so results do not depend
+ * on the launch shape or on sharding.  flags: fp64 state only (B200SV_STATE_F32 returns -1); the B200SV_GAUSS_* bits are not consulted.
+ * max_candidates: candidates per path and maturity interval before the call fails; <= 0 selects the default 2^20.  A path that reaches
+ * it stops and the call returns -6 without writing prices_out / stderr_out or the state arrays.
+ * b200sv_hawkesjd_mc_chain_exact = b200sv_hawkesjd_mc_chain on the exact route (arguments as there, then the budget).  Optional test hooks
+ *                              for paths [0, n_paths_out) (each may be NULL): states_out [M][3][n_paths_out] = (x, lambda_p, lambda_m) after
+ *                              maturity m, events_out [M][3][n_paths_out] = (accepted '+', accepted '-', candidates) in interval m, as doubles.
+ * b200sv_hawkesjd_terminal_exact = b200sv_hawkesjd_terminal on the exact route over one interval of length ttm, with the same
+ *                              use_initial_arrays convention. */
+int b200sv_hawkesjd_mc_chain_exact(const b200sv_hawkes_params* params, int M, const double* ttms, const double* forwards, const double* discfactors,
+                                   const int* offsets, const double* strikes, const int8_t* types, long long nb_path, int variable_type,
+                                   uint64_t seed, int flags, double* prices_out, double* stderr_out, long long max_candidates,
+                                   long long n_paths_out, double* states_out, double* events_out);
+int b200sv_hawkesjd_terminal_exact(const b200sv_hawkes_params* params, double ttm, long long nb_path, uint64_t seed, int flags, int slice_index,
+                                   int use_initial_arrays, long long max_candidates, double* x_inout, double* lambda_p_inout,
+                                   double* lambda_m_inout);
 int b200sv_hawkesjd_device_draws(uint64_t seed, long long path0, long long n, int slice, int S, double dt, const b200sv_hawkes_params* params,
                                  int flags, double* W0, double* U_P, double* U_M, double* J_P, double* J_M);
 
@@ -442,6 +464,12 @@ int b200sv_dev_spot_moments(const double* x, long long n, double forward, double
 int b200sv_dev_hawkesjd_slice(double* x, double* lambda_p, double* lambda_m, long long n_local, long long path_offset, int init,
                               const b200sv_hawkes_params* params, int nsteps, double dt, int slice_index, double forward, uint64_t seed,
                               int flags, double* moments_out, void* p2p_ctx, void* stream);
+/* the device-level twin of b200sv_dev_hawkesjd_slice on the exact route (b200sv_hawkesjd_mc_chain_exact): one maturity interval of length
+ * tau, max_candidates as there; overflow is a device int the kernel sets to nonzero when a path ran out of candidates (the caller zeroes
+ * it before the chain and checks it after synchronising: a nonzero flag means the prices must not be used). */
+int b200sv_dev_hawkesjd_exact_slice(double* x, double* lambda_p, double* lambda_m, long long n_local, long long path_offset, int init,
+                                    const b200sv_hawkes_params* params, double tau, int slice_index, double forward, uint64_t seed,
+                                    long long max_candidates, int* overflow, double* moments_out, void* p2p_ctx, void* stream);
 int b200sv_dev_rough_logsv_slice(double* log_spot, double* vol_factors, double* qvar, long long n_local, long long path_offset,
                                  const b200sv_logsv_params* params, int n_factors, const double* weights, const double* nodes, int nsteps,
                                  double h, double forward, uint64_t seed, int flags, double* moments_out, void* p2p_ctx, void* stream);

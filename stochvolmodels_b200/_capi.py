@@ -93,6 +93,9 @@ SIGNATURES = {
     "b200sv_hawkesjd_mc_chain": [_kp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_longlong, c_int, c_uint64, c_int, _dp, _dp],
     "b200sv_hawkesjd_mc_chain_greeks": [_kp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_longlong, c_int, c_uint64, c_int, _dp, _dp, _dp, _dp,
                                         c_longlong, _dp, _dp],
+    "b200sv_hawkesjd_mc_chain_exact": [_kp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_longlong, c_int, c_uint64, c_int, _dp, _dp, c_longlong,
+                                       c_longlong, _dp, _dp],
+    "b200sv_hawkesjd_terminal_exact": [_kp, c_double, c_longlong, c_uint64, c_int, c_int, c_int, c_longlong, _dp, _dp, _dp],
     "b200sv_hawkesjd_price_chain": [_kp, c_int, _dp, _dp, _dp, _ip, _dp, _i8p, c_int, c_double, c_int, c_double, _dp, _dp, _dp, _dp, _dp],
     "b200sv_hawkesjd_mgf_grid": [_dp, _dp, c_int, c_double, _dp, _kp, _dp],
     "b200sv_fourier_gamma": [_dp, _dp, c_int, c_double, c_double, c_double, c_double, _dp, _i8p, c_int, c_int, _dp],
@@ -123,6 +126,8 @@ SIGNATURES = {
     "b200sv_dev_spot_moments": [c_void_p, c_longlong, c_double, c_void_p, c_void_p],
     "b200sv_dev_hawkesjd_slice": [c_void_p, c_void_p, c_void_p, c_longlong, c_longlong, c_int, _kp, c_int, c_double, c_int, c_double, c_uint64,
                                   c_int, c_void_p, c_void_p, c_void_p],
+    "b200sv_dev_hawkesjd_exact_slice": [c_void_p, c_void_p, c_void_p, c_longlong, c_longlong, c_int, _kp, c_double, c_int, c_double, c_uint64,
+                                        c_longlong, c_void_p, c_void_p, c_void_p, c_void_p],
     "b200sv_dev_rough_logsv_slice": [c_void_p, c_void_p, c_void_p, c_longlong, c_longlong, _lp, c_int, _dp, _dp, c_int, c_double, c_double,
                                      c_uint64, c_int, c_void_p, c_void_p, c_void_p],
     "b200sv_debug_exp_pair": [_dp, c_longlong, _dp],

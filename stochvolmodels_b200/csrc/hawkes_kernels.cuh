@@ -581,4 +581,243 @@ static int hawkes_chain_greeks_host(const b200sv_hawkes_params* p, int M, const 
   return 0;
 }
 
+// ---- exact event-driven route (DESIGN.md §3.13) --------------------------------------------------------------------------------
+// The continuous-time limit of the Euler step above, simulated without a grid by thinning (Ogata).  Per path and maturity interval of
+// length T the state (x, lambda_p, lambda_m) is carried in as the Euler chain carries it; between events both intensities move
+// deterministically, lambda(s) = theta + (lambda - theta) e^{-kappa s} (toward theta for kappa > 0, away from it for kappa < 0), a clock
+// fires at rate max(lambda, 0), the compensator is c lambda (c = e^shift / (1 - mean) - 1, linear in lambda as in the Euler step) and the
+// Brownian part of x over the interval is one Gaussian draw.
+//   bound      at each candidate's start s, per intensity the largest value of its monotone deterministic path on [s, T]: max(lambda, theta,
+//              0) for kappa >= 0 (theta is its limit), max(lambda, lambda(T), 0) for kappa < 0 (it grows away from theta, largest at T);
+//              Lbar = the sum of the two; Lbar = 0: no event, advance to T
+//   candidate  d = E / Lbar, E = -ln(u53); s + d >= T: advance to T; else advance by d, accept '+' if v Lbar < max(lambda_p, 0), '-' if
+//              v Lbar < max(lambda_p, 0) + max(lambda_m, 0), else reject
+//   segment    lambda <- theta + (lambda - theta) e^{-kappa d}, int lambda += theta d + (lambda - theta) (1 - e^{-kappa d}) / kappa (d at kappa = 0)
+//   end        x += (mu - sigma^2/2) T - c_p int lambda_p - c_m int lambda_m + sigma sqrt(T) z
+// Draws (counter word 3 = slice | 0xC0000000, a stream none of the Euler kernel's three -- slice, | 0x80000000, | 0x40000000 -- can reach):
+//   candidate k (word 2 = k): (x, y) the 53-bit uniform u53 = (((x:y) >> 11) + 1) 2^-53 in (0, 1] of the waiting time, z the thinning
+//              uniform v = (z + 1/2) 2^-32, w the jump size's unit exponential -ln((w + 1/2) 2^-32), read only when the candidate is accepted
+//   normal     word 2 = 0xFFFFFFFF: z = Z0 of box_muller_f64_fast (gauss64.cuh) on that block
+// oracle/hawkes_exact.py restates this path by path.
+constexpr unsigned int kHawkesExactStream = 0xC0000000u;
+constexpr unsigned int kHawkesExactNormalCall = 0xFFFFFFFFu;
+constexpr long long kHawkesExactDefaultBudget = 1ll << 20;      // candidates per path and maturity (include/b200sv.h)
+constexpr long long kHawkesExactMaxBudget = 0xFFFFFFFEll;        // the candidate index is counter word 2, below the normal's word
+
+struct HawkesExactConsts {
+  double drift;                 // mu - sigma^2 / 2
+  double c_p, c_m;              // e^shift / (1 - mean) - 1 = comp / dt of make_hawkes_consts
+  double sigma;
+  double shift_p, mean_p, shift_m, mean_m;
+  double theta_p, kappa_p, beta1_p, beta2_p, theta_m, kappa_m, beta1_m, beta2_m;
+};
+
+static HawkesExactConsts make_hawkes_exact_consts(const b200sv_hawkes_params& p) {
+  return HawkesExactConsts{p.mu - 0.5 * p.sigma * p.sigma,
+                           std::exp(p.shift_p) / (1.0 - p.mean_p) - 1.0,
+                           std::exp(p.shift_m) / (1.0 - p.mean_m) - 1.0,
+                           p.sigma, p.shift_p, p.mean_p, p.shift_m, p.mean_m,
+                           p.theta_p, p.kappa_p, p.beta1_p, p.beta2_p, p.theta_m, p.kappa_m, p.beta1_m, p.beta2_m};
+}
+
+struct HawkesExactArgs {
+  double *x, *lam_p, *lam_m;
+  long long n;
+  unsigned long long path_offset;
+  int init;                     // 1: start every path from (0, lambda_p0, lambda_m0)
+  double lam_p0, lam_m0;
+  double T, sqrt_T;             // the interval's length
+  unsigned int slice;
+  unsigned long long seed;
+  long long budget;             // candidates per path in this interval; a path that would draw one more stops and raises *overflow
+  double forward;
+  double* partials;             // [gridDim.x][2]: (sum F e^x over non-NaN, count) for the forward re-centring
+  int* overflow;
+  double* events;               // optional [3][n_out]: accepted '+', accepted '-', candidates of local paths [0, n_out)
+  long long n_out;
+};
+
+// one deterministic segment of length d of one intensity: its value at the end and its integral over the segment
+__device__ __forceinline__ void hawkes_exact_decay(double& lam, double& integral, double theta, double kappa, double d) {
+  const double em = expm1(-kappa * d);                       // e^{-kappa d} - 1
+  const double g = kappa != 0.0 ? -em / kappa : d;           // (1 - e^{-kappa d}) / kappa
+  const double dev = lam - theta;
+  integral += theta * d + dev * g;
+  lam = theta + dev * (1.0 + em);
+}
+
+// the bound of one intensity's firing rate max(lambda, 0) from the candidate's start to the interval end, `rest` ahead, until the next
+// event: the deterministic path is monotone, so its largest value is at one end (theta, its limit, bounds it for kappa >= 0)
+__device__ __forceinline__ double hawkes_exact_rate_bound(double lam, double theta, double kappa, double rest) {
+  const double far = kappa >= 0.0 ? theta : theta + (lam - theta) * exp(-kappa * rest);
+  return fmax(fmax(lam, far), 0.0);
+}
+
+__device__ __forceinline__ double hawkes_u53(uint32_t hi, uint32_t lo) {
+  const unsigned long long b = (((unsigned long long)hi << 32) | lo) >> 11;
+  return (double)(b + 1ull) * 1.1102230246251565e-16;         // 2^-53
+}
+
+__global__ void __launch_bounds__(kThreads) hawkes_exact_slice_kernel(HawkesExactArgs a, HawkesExactConsts c) {
+  gauss64_table_init();
+  SpotMoments<2, kThreads> mom;
+  const uint2 key = make_uint2((uint32_t)a.seed, (uint32_t)(a.seed >> 32));
+  const uint32_t tag = a.slice | kHawkesExactStream;
+  const long long stride = (long long)gridDim.x * kThreads;
+  for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < a.n; i += stride) {
+    double xi = 0.0, lp = a.lam_p0, lm = a.lam_m0;
+    if (!a.init) {
+      xi = a.x[i];
+      lp = a.lam_p[i];
+      lm = a.lam_m[i];
+    }
+    const unsigned long long path = a.path_offset + (unsigned long long)i;
+    const uint32_t plo = (uint32_t)path, phi = (uint32_t)(path >> 32);
+    double s = 0.0, ip = 0.0, im = 0.0;
+    long long k = 0, np_ = 0, nm_ = 0;
+    for (;;) {
+      const double bound = hawkes_exact_rate_bound(lp, c.theta_p, c.kappa_p, a.T - s) + hawkes_exact_rate_bound(lm, c.theta_m, c.kappa_m, a.T - s);
+      double d = a.T - s;
+      bool cand = false;
+      uint4 w = make_uint4(0u, 0u, 0u, 0u);
+      if (bound > 0.0) {
+        w = philox4x32_10(make_uint4(plo, phi, (uint32_t)k, tag), key);
+        const double dc = -log(hawkes_u53(w.x, w.y)) / bound;
+        if (s + dc < a.T) {
+          d = dc;
+          cand = true;
+        }
+      }
+      if (cand && k >= a.budget) {
+        atomicOr(a.overflow, 1);
+        break;
+      }
+      hawkes_exact_decay(lp, ip, c.theta_p, c.kappa_p, d);
+      hawkes_exact_decay(lm, im, c.theta_m, c.kappa_m, d);
+      if (!cand) break;
+      s += d;
+      ++k;
+      const double v = fma((double)w.z, 2.3283064365386963e-10, 1.1641532182693481e-10) * bound;
+      const double pp = fmax(lp, 0.0);
+      const bool fire_p = v < pp, fire_m = !fire_p && v < pp + fmax(lm, 0.0);
+      if (fire_p || fire_m) {
+        const double e = -log(fma((double)w.w, 2.3283064365386963e-10, 1.1641532182693481e-10));
+        if (fire_p) {
+          const double jump = c.shift_p + c.mean_p * e;
+          xi += jump;
+          lp += c.beta1_p * jump;
+          lm += c.beta1_m * jump;
+          ++np_;
+        } else {
+          const double jump = c.shift_m + c.mean_m * e;
+          xi += jump;
+          lp += c.beta2_p * jump;
+          lm += c.beta2_m * jump;
+          ++nm_;
+        }
+      }
+    }
+    double z, z1;
+    box_muller_f64_fast(philox4x32_10(make_uint4(plo, phi, kHawkesExactNormalCall, tag), key), z, z1);
+    xi += ((c.drift * a.T - c.c_p * ip) - c.c_m * im) + c.sigma * a.sqrt_T * z;
+    a.x[i] = xi;
+    a.lam_p[i] = lp;
+    a.lam_m[i] = lm;
+    if (i < a.n_out) {
+      a.events[i] = (double)np_;
+      a.events[a.n_out + i] = (double)nm_;
+      a.events[2 * a.n_out + i] = (double)k;
+    }
+    mom.add(a.forward * exp(xi));
+  }
+  mom.store(a.partials);
+}
+
+// one interval of the exact route on paths [path_offset, path_offset + n), then their re-centring moments into moments_out.  events:
+// [3][n_out] device rows for the first n_out local paths (n_out = 0: none).
+static int launch_hawkes_exact_slice(double* x, double* lp, double* lm, long long n, long long path_offset, int init, const b200sv_hawkes_params& p,
+                                     double T, int slice_index, double forward, uint64_t seed, long long budget, int* overflow, double* events,
+                                     long long n_out, double* moments_out, cudaStream_t st, P2pCtx* p2p = nullptr) {
+  HawkesExactArgs a;
+  a.x = x;
+  a.lam_p = lp;
+  a.lam_m = lm;
+  a.n = n;
+  a.path_offset = (unsigned long long)path_offset;
+  a.init = init;
+  a.lam_p0 = p.lambda_p;
+  a.lam_m0 = p.lambda_m;
+  a.T = T;
+  a.sqrt_T = std::sqrt(T);
+  a.slice = (unsigned int)slice_index;
+  a.seed = seed;
+  a.budget = budget;
+  a.forward = forward;
+  a.overflow = overflow;
+  a.events = events;
+  a.n_out = events ? n_out : 0;
+  const HawkesExactConsts c = make_hawkes_exact_consts(p);
+  const Grid grid = persistent_grid(hawkes_exact_slice_kernel, kThreads, n);
+  return slice_moments("hawkes_exact_slice_kernel", 2, grid.blocks, moments_out, st, p2p, [&](double* partials) {
+    a.partials = partials;
+    hawkes_exact_slice_kernel<<<grid.blocks, grid.threads, 0, st>>>(a, c);
+  });
+}
+
+// the candidate budget of the exact entry points: <= 0 selects the default
+static long long hawkes_exact_budget(long long max_candidates) {
+  return max_candidates <= 0 ? kHawkesExactDefaultBudget : std::min(max_candidates, kHawkesExactMaxBudget);
+}
+
+// Chain of the exact route: hawkes_chain_host's structure (one slice launch and one payoff per maturity, one copy back) on the intervals
+// ttms[m] - ttms[m - 1].  The overflow flag is read before any result is copied out: a path that ran out of candidates fails the call
+// with -6 and prices_out / stderr_out stay unwritten.  states_out [M][3][n_out] and events_out [M][3][n_out] (test hooks, may be NULL):
+// the state and the event counts of paths [0, n_out) after each maturity.
+static int hawkes_exact_chain_host(const b200sv_hawkes_params* p, int M, const double* ttms, const double* forwards, const double* discfactors,
+                                   const int* offsets, const double* strikes, const int8_t* types, long long nb_path, int variable_type,
+                                   uint64_t seed, int flags, double* prices_out, double* stderr_out, long long max_candidates,
+                                   long long n_paths_out, double* states_out, double* events_out) {
+  B200SV_REQUIRE(nb_path >= 1, "nb_path must be >= 1");
+  B200SV_REQUIRE(n_paths_out >= 0 && n_paths_out <= nb_path, "n_paths_out must be in [0, nb_path]");
+  B200SV_REQUIRE(!(flags & B200SV_STATE_F32), "the Hawkes route is float64 only");
+  if (int rc = validate_chain(M, ttms, offsets, strikes, types, variable_type)) return rc;
+  const long long budget = hawkes_exact_budget(max_candidates);
+  cudaStream_t st = current_stream();
+  ensure_pool_threshold();
+  StreamSync sync(st);
+  DevBuf d(st), d_flag(st), d_events(st);
+  ChainIO io(1, M, ttms, forwards, discfactors, offsets, types, variable_type, st);
+  const size_t N = (size_t)nb_path, no = (states_out || events_out) ? (size_t)n_paths_out : 0;
+  B200SV_CUDA(d.alloc(sizeof(double) * 3 * N));
+  B200SV_CUDA(d_flag.alloc(sizeof(int)));
+  B200SV_CUDA(d_events.alloc(sizeof(double) * 3 * std::max(no, (size_t)1)));
+  B200SV_CUDA(cudaMemsetAsync(d_flag.p, 0, sizeof(int), st));
+  if (int rc = io.upload(strikes)) return rc;
+  double* x = d.as<double>();
+  std::vector<double> h_paths(no * 6 * M);
+  for (int m = 0; m < M; ++m) {
+    const double T = ttms[m] - (m > 0 ? ttms[m - 1] : 0.0);
+    if (int rc = launch_hawkes_exact_slice(x, x + N, x + 2 * N, nb_path, 0, m == 0, *p, T, m, forwards[m], seed, budget, d_flag.as<int>(),
+                                           no ? d_events.as<double>() : nullptr, (long long)no, io.moments(), st))
+      return rc;
+    if (int rc = io.payoff(0, m, x, x, false, nb_path, (double)nb_path, false)) return rc;
+    if (no) {
+      B200SV_CUDA(cudaMemcpy2DAsync(h_paths.data() + no * 6 * m, sizeof(double) * no, x, sizeof(double) * N, sizeof(double) * no, 3,
+                                    cudaMemcpyDeviceToHost, st));
+      B200SV_CUDA(cudaMemcpyAsync(h_paths.data() + no * (6 * m + 3), d_events.p, sizeof(double) * 3 * no, cudaMemcpyDeviceToHost, st));
+    }
+  }
+  int overflow = 0;
+  B200SV_CUDA(cudaMemcpyAsync(&overflow, d_flag.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+  B200SV_CUDA(cudaStreamSynchronize(st));
+  if (overflow) return fail(-6, "candidate budget exhausted: a path of the exact Hawkes route drew more than " + std::to_string(budget) +
+                                    " candidates in one maturity interval");
+  if (int rc = io.copy_back(sync, prices_out, stderr_out, nullptr)) return rc;
+  for (size_t m = 0; m < (size_t)M && no; ++m) {
+    if (states_out) memcpy(states_out + 3 * no * m, h_paths.data() + no * 6 * m, sizeof(double) * 3 * no);
+    if (events_out) memcpy(events_out + 3 * no * m, h_paths.data() + no * (6 * m + 3), sizeof(double) * 3 * no);
+  }
+  return 0;
+}
+
 }  // namespace b200sv

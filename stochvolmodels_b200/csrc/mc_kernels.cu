@@ -2791,6 +2791,15 @@ int b200sv_dev_hawkesjd_slice(double* x, double* lambda_p, double* lambda_m, lon
                              moments_out, (cudaStream_t)stream, (P2pCtx*)p2p);
 }
 
+int b200sv_dev_hawkesjd_exact_slice(double* x, double* lambda_p, double* lambda_m, long long n_local, long long path_offset, int init,
+                                    const b200sv_hawkes_params* params, double tau, int slice_index, double forward, uint64_t seed,
+                                    long long max_candidates, int* overflow, double* moments_out, void* p2p, void* stream) {
+  B200SV_REQUIRE(x && lambda_p && lambda_m && params && overflow && moments_out, "null pointer");
+  B200SV_REQUIRE(n_local >= 1 && tau > 0.0 && slice_index >= 0, "n_local and tau must be positive");
+  return launch_hawkes_exact_slice(x, lambda_p, lambda_m, n_local, path_offset, init, *params, tau, slice_index, forward, seed,
+                                   hawkes_exact_budget(max_candidates), overflow, nullptr, 0, moments_out, (cudaStream_t)stream, (P2pCtx*)p2p);
+}
+
 int b200sv_dev_rough_logsv_slice(double* log_spot, double* vol_factors, double* qvar, long long n_local, long long path_offset,
                                  const b200sv_logsv_params* params, int n_factors, const double* weights, const double* nodes, int nsteps,
                                  double h, double forward, uint64_t seed, int flags, double* moments_out, void* p2p, void* stream) {
@@ -3065,6 +3074,44 @@ int b200sv_hawkesjd_terminal(const b200sv_hawkes_params* params, double ttm, lon
   if (int rc = launch_hawkes_slice(s.dev(0), s.dev(1), s.dev(2), nb_path, 0, use_initial_arrays ? 0 : 1, *params, S, dt, slice_index, 1.0, seed,
                                    flags, d_mom.as<double>(), st))
     return rc;
+  if (int rc = s.download()) return rc;
+  return sync.done();
+}
+
+// exact event-driven route (hawkes_kernels.cuh, DESIGN.md §3.13)
+int b200sv_hawkesjd_mc_chain_exact(const b200sv_hawkes_params* params, int M, const double* ttms, const double* forwards, const double* discfactors,
+                                   const int* offsets, const double* strikes, const int8_t* types, long long nb_path, int variable_type,
+                                   uint64_t seed, int flags, double* prices_out, double* stderr_out, long long max_candidates,
+                                   long long n_paths_out, double* states_out, double* events_out) {
+  B200SV_REQUIRE(params && ttms && forwards && discfactors && offsets && prices_out && stderr_out, "null pointer");
+  return hawkes_exact_chain_host(params, M, ttms, forwards, discfactors, offsets, strikes, types, nb_path, variable_type, seed, flags, prices_out,
+                                 stderr_out, max_candidates, n_paths_out, states_out, events_out);
+}
+
+int b200sv_hawkesjd_terminal_exact(const b200sv_hawkes_params* params, double ttm, long long nb_path, uint64_t seed, int flags, int slice_index,
+                                   int use_initial_arrays, long long max_candidates, double* x_inout, double* lambda_p_inout,
+                                   double* lambda_m_inout) {
+  B200SV_REQUIRE(params && x_inout && lambda_p_inout && lambda_m_inout, "null pointer");
+  B200SV_REQUIRE(nb_path >= 1 && ttm > 0.0 && slice_index >= 0, "nb_path, ttm must be positive");
+  B200SV_REQUIRE(!(flags & B200SV_STATE_F32), "the Hawkes route is float64 only");
+  const long long budget = hawkes_exact_budget(max_candidates);
+  cudaStream_t st = current_stream();
+  ensure_pool_threshold();
+  StreamSync sync(st);
+  HostState s(x_inout, lambda_p_inout, lambda_m_inout, nb_path, st);
+  DevBuf d_mom(st), d_flag(st);
+  if (int rc = s.alloc(use_initial_arrays != 0)) return rc;
+  B200SV_CUDA(d_mom.alloc(sizeof(double) * 2));
+  B200SV_CUDA(d_flag.alloc(sizeof(int)));
+  B200SV_CUDA(cudaMemsetAsync(d_flag.p, 0, sizeof(int), st));
+  if (int rc = launch_hawkes_exact_slice(s.dev(0), s.dev(1), s.dev(2), nb_path, 0, use_initial_arrays ? 0 : 1, *params, ttm, slice_index, 1.0,
+                                         seed, budget, d_flag.as<int>(), nullptr, 0, d_mom.as<double>(), st))
+    return rc;
+  int overflow = 0;
+  B200SV_CUDA(cudaMemcpyAsync(&overflow, d_flag.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+  B200SV_CUDA(cudaStreamSynchronize(st));
+  if (overflow) return fail(-6, "candidate budget exhausted: a path of the exact Hawkes route drew more than " + std::to_string(budget) +
+                                    " candidates");
   if (int rc = s.download()) return rc;
   return sync.done();
 }

@@ -122,6 +122,23 @@ def hawkesjd_mc_chain(params: C.HawkesParamsC, ttms, forwards, discfactors, stri
                      variable_type, seed, flags)
 
 
+HAWKES_EXACT_DEFAULT_BUDGET = 1 << 20      # candidates per path and maturity interval of the exact route (include/b200sv.h)
+
+
+def hawkesjd_mc_chain_exact(params: C.HawkesParamsC, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, nb_path: int, variable_type,
+                            seed: int, flags: int = 0, max_candidates: int = HAWKES_EXACT_DEFAULT_BUDGET, n_paths_out: int = 0):
+    """chain MC of the Hawkes jump-diffusion on the exact event-driven route (b200sv_hawkesjd_mc_chain_exact; DESIGN.md §3.13).  Returns
+    (prices, std errors, states, events): with ``n_paths_out`` > 0 states [M, 3, n_paths_out] = (x, lambda_p, lambda_m) and events
+    [M, 3, n_paths_out] = (accepted '+', accepted '-', candidates) of the first paths per maturity, else None.  A path that draws more than
+    ``max_candidates`` candidates in one interval fails the call (B200svError -6)."""
+    M, n_out = C.f64(ttms).shape[0], int(n_paths_out)
+    states = np.empty((M, 3, n_out)) if n_out else None
+    events = np.empty((M, 3, n_out)) if n_out else None
+    prices, stds = _mc_chain("b200sv_hawkesjd_mc_chain_exact", params, (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms), (),
+                             (int(nb_path),), variable_type, seed, flags, post=(int(max_candidates), n_out, C.dptr(states), C.dptr(events)))
+    return prices, stds, states, events
+
+
 LOGSV_GREEK_PARAMS = ("sigma0", "theta", "kappa1", "kappa2", "beta", "volvol")
 HESTON_GREEK_PARAMS = ("v0", "theta", "kappa", "rho", "volvol")
 # HawkesJDParams fields in dataclass order without mu (the Fourier route never reads it) and risk_premia_gamma (not covered)
@@ -399,6 +416,14 @@ def hawkesjd_terminal(params: C.HawkesParamsC, ttm: float, x, lambda_p, lambda_m
     without ``per_path`` every path starts from (0, params.lambda_p, params.lambda_m)"""
     C.call("b200sv_hawkesjd_terminal", byref(params), float(ttm), int(x.shape[0]), C.seed64(seed), flags, int(slice_index), 1 if per_path else 0,
            C.dptr(x), C.dptr(lambda_p), C.dptr(lambda_m))
+    return x, lambda_p, lambda_m
+
+
+def hawkesjd_terminal_exact(params: C.HawkesParamsC, ttm: float, x, lambda_p, lambda_m, seed: int, slice_index: int, per_path: bool,
+                            max_candidates: int = HAWKES_EXACT_DEFAULT_BUDGET, flags: int = 0):
+    """the exact event-driven twin of hawkesjd_terminal over one interval of length ``ttm`` (b200sv_hawkesjd_terminal_exact), in place"""
+    C.call("b200sv_hawkesjd_terminal_exact", byref(params), float(ttm), int(x.shape[0]), C.seed64(seed), int(flags), int(slice_index),
+           1 if per_path else 0, int(max_candidates), C.dptr(x), C.dptr(lambda_p), C.dptr(lambda_m))
     return x, lambda_p, lambda_m
 
 

@@ -187,12 +187,14 @@ def release_p2p():
 class CudaMcEngine:
     """Device-resident MC state + kernel launches on the current CUDA device (used for N>=1 ranks and by bench.py)."""
 
-    MODELS = ("logsv", "heston", "hawkes", "rough")
+    MODELS = ("logsv", "heston", "hawkes", "hawkes_exact", "rough")
 
     def __init__(self, model: str, params_c, n_local: int, path_offset: int, flags: int, max_strikes: int, device=None, scheme: int = 0,
                  factors=None):
         """``model``: 'logsv' / 'heston' (state x, vol or var, qvar), 'hawkes' (state x, lambda_p, lambda_m; x stands in for qvar in the
-        payoff, hawkes_jd_pricer.py:703) or 'rough' (state log_spot, n vol factors, qvar; ``factors`` = (weights, nodes) of the kernel)."""
+        payoff, hawkes_jd_pricer.py:703), 'hawkes_exact' (the same state on the exact event-driven route, DESIGN.md §3.13: ``simulate_slice``
+        reads ``dt`` as the interval's length and ``nsteps`` not at all) or 'rough' (state log_spot, n vol factors, qvar; ``factors`` =
+        (weights, nodes) of the kernel)."""
         import torch
         if not torch.cuda.is_available():
             raise RuntimeError("CudaMcEngine needs a CUDA device; stochvolmodels_b200 has no CPU fallback")
@@ -205,13 +207,13 @@ class CudaMcEngine:
         self.params_c = params_c
         self.n_local, self.path_offset, self.flags = int(n_local), int(path_offset), int(flags)
         self.device = torch.device(device if device is not None else f"cuda:{torch.cuda.current_device()}")
-        if model in ("hawkes", "rough") and (flags & C.STATE_F32):
+        if model in ("hawkes", "hawkes_exact", "rough") and (flags & C.STATE_F32):
             raise ValueError("the Hawkes and rough-vol routes are float64 only")
         sdtype = torch.float32 if (flags & C.STATE_F32) else torch.float64
         self.factors = None
         self.set_factors(factors)
         rows = 3 if model != "rough" else len(self.factors[0]) + 2
-        self.qrow = {"hawkes": 0, "rough": rows - 1}.get(model, 2)          # the state row the Q_VAR payoff reads
+        self.qrow = {"hawkes": 0, "hawkes_exact": 0, "rough": rows - 1}.get(model, 2)          # the state row the Q_VAR payoff reads
         self.state = torch.empty((rows, max(self.n_local, 1)), dtype=sdtype, device=self.device)
         self.moments = torch.zeros(2, dtype=torch.float64, device=self.device)
         self.sums = torch.zeros(3 * max(max_strikes, 1), dtype=torch.float64, device=self.device)
@@ -220,6 +222,9 @@ class CudaMcEngine:
         self.p2p = None          # libb200sv P2P mailbox context (void*), see enable_p2p
         self._chain_dev = None   # per-chain buffers reused across calls (see chain_buffers)
         self._chain_host = None
+        # exact Hawkes route: candidates per path and interval, and the device flag its kernel raises when a path runs out of them
+        self.max_candidates = engine.HAWKES_EXACT_DEFAULT_BUDGET
+        self.overflow = torch.zeros(1, dtype=torch.int32, device=self.device) if model == "hawkes_exact" else None
 
     def set_factors(self, factors):
         """(weights, nodes) of the rough kernel's Markovian lift (host float64 arrays of equal length <= 8); None for the other models."""
@@ -279,6 +284,10 @@ class CudaMcEngine:
         elif self.model == "hawkes":
             C.call("b200sv_dev_hawkesjd_slice", x, v, q, self.n_local, self.path_offset, int(init), byref(self.params_c), int(nsteps), float(dt),
                    int(m), float(forward), seed, self.flags, c_void_p(self.moments.data_ptr()), self.p2p, self._stream())
+        elif self.model == "hawkes_exact":
+            C.call("b200sv_dev_hawkesjd_exact_slice", x, v, q, self.n_local, self.path_offset, int(init), byref(self.params_c), float(dt), int(m),
+                   float(forward), seed, int(self.max_candidates), c_void_p(self.overflow.data_ptr()), c_void_p(self.moments.data_ptr()),
+                   self.p2p, self._stream())
         elif self.model == "rough":       # every maturity restarts at t = 0 on its own grid: `init` and `m` do not enter
             w, nodes = self.factors
             C.call("b200sv_dev_rough_logsv_slice", x, c_void_p(self.state[1].data_ptr()), c_void_p(self.state[self.qrow].data_ptr()), self.n_local,
@@ -289,6 +298,18 @@ class CudaMcEngine:
                    float(dt), int(m), float(forward), seed, self.flags, self.scheme,
                    c_void_p(self.moments.data_ptr()), self.p2p, self._stream())
         return self.moments
+
+    def check_overflow(self, group=None, world: int = 1):
+        """raise B200svError(-6) if a path of the exact Hawkes route ran out of candidates since the flag was last cleared, on this rank or
+        (``world`` > 1: one all-reduce over ``group``) on any rank, then clear the flag.  Synchronises the stream."""
+        if world > 1:
+            import torch.distributed as dist
+            dist.all_reduce(self.overflow, op=dist.ReduceOp.MAX, group=group)
+        hit = int(self.overflow.item())
+        self.overflow.zero_()
+        if hit:
+            raise C.B200svError(-6, f"candidate budget exhausted: a path of the exact Hawkes route drew more than {self.max_candidates} "
+                                    "candidates in one maturity interval")
 
     def payoff_sums(self, ttm: float, forward: float, strikes_dev, types_dev, J: int, variable_type: int, kinds: int = 0):
         """LOCAL per-strike (sum, sum^2, count) given the GLOBAL moments in ``self.moments``; returns a view of 3*J doubles."""
@@ -316,14 +337,16 @@ def mc_chain_distributed(model: str, params_c, ttms, forwards, discfactors, etas
                          nb_steps_per_year: int, is_spot_measure: bool, variable_type: int, seed: int, flags: int,
                          group=None, engine_factory: Optional[Callable] = None, return_engine: bool = False, scheme: int = 0,
                          exchange: Optional[str] = None, grid: Optional[Sequence[Tuple[int, float]]] = None, factors=None,
-                         se_paths: Optional[int] = None):
+                         se_paths: Optional[int] = None, max_candidates: Optional[int] = None):
     """Chain MC with ``nb_path`` TOTAL paths split over the ranks of ``group`` (default: the world; works unsharded when
     torch.distributed is not initialised).  Every rank returns the same (prices, std errors) lists.
 
     Mirrors the slice loop of logsv_mc_chain_pricer / heston_mc_chain_pricer (pricers/logsv_pricer.py:840-865,
     pricers/heston_pricer.py:304-329): the terminal state of slice m seeds slice m+1.  ``model`` 'hawkes' (hawkes_jd_pricer.py:687-715,
     ``nb_steps_per_year`` = 1800 there) and 'rough' (logsv_pricer.py:1199-1216: ``grid`` = the (nb_steps, h) of every maturity's OWN grid
-    from t = 0, ``factors`` = (weights, nodes), ``se_paths`` = 1 for that route's un-normalised standard errors) shard the same way.
+    from t = 0, ``factors`` = (weights, nodes), ``se_paths`` = 1 for that route's un-normalised standard errors) shard the same way, and so
+    does 'hawkes_exact' (DESIGN.md §3.13: ``grid`` = (1, interval length) per maturity, ``max_candidates`` its candidate budget; a path
+    that runs out of candidates on any rank raises B200svError(-6) on every rank).
     """
     import torch
     import torch.distributed as dist
@@ -358,6 +381,10 @@ def mc_chain_distributed(model: str, params_c, ttms, forwards, discfactors, etas
             use_p2p = False
     if not use_p2p and getattr(eng, "p2p", None) is not None:
         eng.p2p = None            # a cached engine may carry the mailbox of an earlier p2p call
+    exact = getattr(eng, "overflow", None) is not None
+    if exact:
+        eng.overflow.zero_()
+        eng.max_candidates = engine.HAWKES_EXACT_DEFAULT_BUDGET if max_candidates is None else int(max_candidates)
     etas = np.ones(M) if etas is None else np.asarray(etas, dtype=np.float64)
     Jtot = int(offsets[-1])
     chain_out = hasattr(eng, "chain_buffers")   # CUDA engine: results stay on the device until ONE copy at the end of the chain
@@ -403,6 +430,8 @@ def mc_chain_distributed(model: str, params_c, ttms, forwards, discfactors, etas
         else:
             prices, stds = eng.finalize(sums, J, float(discfactors[m]), int(nb_path if se_paths is None else se_paths))
             results.append((prices.clone(), stds.clone()))
+    if exact:
+        eng.check_overflow(group, world)          # before any price leaves the device: a stopped path biases every shard's moments
     prices_out: List[np.ndarray] = []
     stds_out: List[np.ndarray] = []
     if chain_out:

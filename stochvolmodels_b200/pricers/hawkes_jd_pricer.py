@@ -2,7 +2,7 @@
 
 * ``HawkesJDParams``                          (hawkes_jd_pricer.py:41-119)
 * ``HawkesJDPricer.model_mc_price_chain``     (:156-171) -> ``hawkesjd_mc_chain_pricer`` (:644-715); ``model_mc_chain_greeks`` adds Monte Carlo
-  sensitivities (DESIGN.md §3.11)
+  sensitivities (DESIGN.md §3.11); ``scheme="exact"`` opts into the exact event-driven route (DESIGN.md §3.13, not in the reference)
 * ``HawkesJDPricer.simulate_terminal_values`` (:193-224) -> ``simulate_hawkesjd_terminal`` (:718-779)
 * ``HawkesJDPricer.price_chain``              (:125-155) -> ``hawkesjd_chain_pricer`` (:365-417) / ``hawkesjd_chain_pricer_with_risk_premia`` (:420-484),
   ``hawkesjd_forwards_under_risk_kernel`` (:487-515), ``compute_hawkes_a_mgf_grid`` / ``solve_a_ode_grid`` (:518-579)
@@ -85,6 +85,47 @@ class HawkesJDParams(ModelParams):
 
 def _params_c(**kw) -> C.HawkesParamsC:
     return C.HawkesParamsC(*[float(kw[k]) for k in _KEYS])
+
+
+SCHEMES = ("euler", "exact")
+# the exact route refuses a parameter set whose bound on the expected events per path over the simulated horizon exceeds this
+HAWKES_EXACT_MAX_EXPECTED_EVENTS = 5000.0
+
+
+def _is_exact(scheme) -> bool:
+    """'euler' (default: the reference's 1800-steps-per-year scheme, the numbers the goldens pin) | 'exact' (opt-in event-driven simulation
+    of the continuous-time model without a grid, DESIGN.md §3.13; not in the reference)"""
+    if scheme not in SCHEMES:
+        raise ValueError("scheme must be 'euler' or 'exact'")
+    return scheme == "exact"
+
+
+def hawkes_expected_events_bound(horizon: float, lambda_p: float, lambda_m: float, shift_p: float, mean_p: float, shift_m: float, mean_m: float,
+                                 theta_p: float, kappa_p: float, beta1_p: float, beta2_p: float, theta_m: float, kappa_m: float, beta1_m: float,
+                                 beta2_m: float, **_) -> float:
+    """an upper bound on the expected number of events per path over [0, horizon], for any sign of the parameters: the integral of
+    m_p + m_m from the comparison system d m / dt = |K theta| - K m + B m, m(0) = |lambda(0)|, B_ij = |beta_ij| (|shift_j| + |mean_j|).
+    Between events d|lambda|/dt <= |kappa theta| - kappa |lambda|, a jump adds at most |beta| |J| at the rate max(lambda_j, 0) <= |lambda_j|,
+    and the system is cooperative, so m >= E|lambda| >= E[max(lambda, 0)], the firing rate (DESIGN.md §3.13).  inf where the bound does not
+    exist in floating point."""
+    from scipy.linalg import expm
+    ej_p, ej_m = abs(shift_p) + abs(mean_p), abs(shift_m) + abs(mean_m)
+    a = np.zeros((4, 4))
+    a[0, :2] = (abs(beta1_p) * ej_p - kappa_p, abs(beta2_p) * ej_m)
+    a[1, :2] = (abs(beta1_m) * ej_p, abs(beta2_m) * ej_m - kappa_m)
+    a[:2, 2] = (abs(kappa_p * theta_p), abs(kappa_m * theta_m))
+    a[3, :2] = 1.0
+    with np.errstate(all="ignore"):
+        y = expm(a * float(horizon)) @ np.array([abs(lambda_p), abs(lambda_m), 1.0, 0.0])
+    return float(y[3]) if np.isfinite(y[3]) else float("inf")
+
+
+def _check_exact_events(horizon: float, kw) -> None:
+    """refuse, before any GPU work, a parameter set the exact route would spend a runaway number of events on"""
+    bound = hawkes_expected_events_bound(horizon, **kw)
+    if not bound <= HAWKES_EXACT_MAX_EXPECTED_EVENTS:
+        raise ValueError(f"scheme='exact': up to {bound:.4g} expected events per path over {horizon} years exceeds the limit "
+                         f"{HAWKES_EXACT_MAX_EXPECTED_EVENTS:g} (HAWKES_EXACT_MAX_EXPECTED_EVENTS)")
 
 
 def _check_risk_premia_greeks(option_chain: OptionChain, params: HawkesJDParams, is_spot_measure: bool, kwargs, method: str) -> float:
@@ -201,26 +242,33 @@ class HawkesJDPricer(ModelPricer):
         return to_chain_ivol_sensitivities(option_chain, self.price_chain_risk_premia_hessian(option_chain, params, is_spot_measure, **kwargs))
 
     @timer
-    def model_mc_price_chain(self, option_chain: OptionChain, params: HawkesJDParams, nb_path: int = 100000, **kwargs
+    def model_mc_price_chain(self, option_chain: OptionChain, params: HawkesJDParams, nb_path: int = 100000, scheme: str = "euler", **kwargs
                              ) -> Tuple[List[np.ndarray], List[np.ndarray]]:
+        """MC prices and standard errors of the chain (reference :156-171).  ``scheme``: 'euler' (default, the reference's scheme) or
+        'exact', the event-driven simulation of the continuous-time model the Fourier route prices (DESIGN.md §3.13); see
+        ``hawkesjd_mc_chain_pricer``."""
         d = params.to_dict()
         d.pop("risk_premia_gamma", None)
         return hawkesjd_mc_chain_pricer(ttms=option_chain.ttms, forwards=option_chain.forwards, discfactors=option_chain.discfactors,
                                         strikes_ttms=option_chain.strikes_ttms, optiontypes_ttms=option_chain.optiontypes_ttms, nb_path=nb_path,
                                         seed=kwargs.get("seed"), gauss=kwargs.get("gauss", "fp32"),
                                         variable_type=kwargs.get("variable_type", VariableType.LOG_RETURN),
-                                        distributed=kwargs.get("distributed", True), exchange=kwargs.get("exchange"), **d)
+                                        distributed=kwargs.get("distributed", True), exchange=kwargs.get("exchange"), scheme=scheme,
+                                        max_candidates=kwargs.get("max_candidates"), **d)
 
     @timer
     def model_mc_chain_greeks(self, option_chain: OptionChain, params: HawkesJDParams, nb_path: int = 100000, seed: Optional[int] = None,
-                              gauss: str = "fp32", **kwargs):
+                              gauss: str = "fp32", scheme: str = "euler", **kwargs):
         """MC prices and standard errors bit-identical to ``model_mc_price_chain`` with the same ``nb_path`` / ``seed`` / ``gauss`` (one GPU),
         plus the forward delta and d price / d HAWKES_GREEK_PARAMS (the Fourier route's 15 names and order; ``mu`` is excluded there too),
         each with its standard error df std(g) / sqrt(N) -> ``McChainGreeks``.  Pathwise with the firing decisions frozen plus the
         likelihood-ratio score of the decisions (DESIGN.md §3.11): unbiased for the discretised scheme the pricer simulates.  LOG_RETURN,
         fp64 state, ``gauss`` 'fp32' / 'fp64'; Q_VAR, ``exchange``, another ``precision`` or a set ``risk_premia_gamma`` raise
-        NotImplementedError, ``mean_p == 0`` or ``mean_m == 0`` (degenerate jump sizes) ValueError.  Under torch.distributed every rank prices all paths (replicated, bit-identical results)."""
+        NotImplementedError, ``mean_p == 0`` or ``mean_m == 0`` (degenerate jump sizes) ValueError.  Under torch.distributed every rank prices all paths (replicated, bit-identical results).
+        ``scheme``: 'euler' only; 'exact' (no sensitivities on that route) raises NotImplementedError, another value ValueError."""
         from .mc_greeks import check_hawkes_mc_greeks_kwargs, check_no_gamma, check_no_theta, to_mc_chain_greeks
+        if _is_exact(scheme):
+            raise NotImplementedError("model_mc_chain_greeks covers scheme='euler' only: the exact route has no sensitivities")
         check_no_gamma(kwargs, "HawkesJDPricer.model_mc_chain_greeks")
         check_no_theta(kwargs, "HawkesJDPricer.model_mc_chain_greeks",
                        "the firing clock's dt enters through the likelihood-ratio score and the dt*(1 +- 1e-9) comparison constants; "
@@ -287,24 +335,46 @@ class HawkesJDPricer(ModelPricer):
                                                    return_exceptions=return_exceptions, max_sets_per_call=max_sets_per_call, **kwargs)
 
     @timer
-    def simulate_terminal_values(self, params: HawkesJDParams, ttm: float = 1.0, nb_path: int = 100000, is_spot_measure: bool = True, **kwargs
-                                 ) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    def simulate_terminal_values(self, params: HawkesJDParams, ttm: float = 1.0, nb_path: int = 100000, is_spot_measure: bool = True,
+                                 scheme: str = "euler", **kwargs) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """terminal (x, lambda_p, lambda_m) from (0, lambda_p, lambda_m) (reference :193-224); ``scheme`` as in ``model_mc_price_chain``"""
         d = {k: v for k, v in params.to_dict().items() if k in _KEYS and k not in ("lambda_p", "lambda_m")}
         return simulate_hawkesjd_terminal(ttm=ttm, x0=np.zeros(1), lambda_p0=params.lambda_p * np.ones(1), lambda_m0=params.lambda_m * np.ones(1),
-                                          nb_path=nb_path, seed=kwargs.get("seed"), gauss=kwargs.get("gauss", "fp32"), **d)
+                                          nb_path=nb_path, seed=kwargs.get("seed"), gauss=kwargs.get("gauss", "fp32"), scheme=scheme,
+                                          max_candidates=kwargs.get("max_candidates"), **d)
 
 
 def hawkesjd_mc_chain_pricer(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, lambda_p: float, lambda_m: float, mu: float, sigma: float,
                              shift_p: float, mean_p: float, shift_m: float, mean_m: float, theta_p: float, kappa_p: float, beta1_p: float,
                              beta2_p: float, theta_m: float, kappa_m: float, beta1_m: float, beta2_m: float, risk_premia_gamma: float = 0.0,
                              nb_path: int = 100000, variable_type: VariableType = VariableType.LOG_RETURN, seed: Optional[int] = None,
-                             gauss: str = "fp32", distributed: bool = True, exchange: Optional[str] = None
-                             ) -> Tuple[List[np.ndarray], List[np.ndarray]]:
+                             gauss: str = "fp32", distributed: bool = True, exchange: Optional[str] = None, scheme: str = "euler",
+                             max_candidates: Optional[int] = None) -> Tuple[List[np.ndarray], List[np.ndarray]]:
     """chain prices and standard errors by simulating the jump-diffusion (reference :644-715): the terminal (x, lambda_p, lambda_m) of slice m
     seeds slice m+1; payoffs are forward-recentred on x (utils/mc_payoffs.py).  Under an initialised torch.distributed world ``nb_path`` is
-    the TOTAL path count, sharded over the ranks by global path id (the LogSV chain's two exchanges per maturity, multi_gpu.py)."""
+    the TOTAL path count, sharded over the ranks by global path id (the LogSV chain's two exchanges per maturity, multi_gpu.py).
+
+    ``scheme``: 'euler' (default) steps the reference's scheme at 1800 steps per year, the route whose numbers the reference pins.
+    'exact' simulates the continuous-time model event by event by thinning, with no time grid and no discretisation bias (DESIGN.md
+    §3.13): where the intensities cannot become negative it is the model the Fourier route prices.  The two are different discretisations,
+    not two implementations of one result.  On the exact route ``gauss`` is not consulted (its draws are fp64), a parameter set whose bound
+    on the expected events per path over the chain exceeds HAWKES_EXACT_MAX_EXPECTED_EVENTS raises ValueError before any GPU work, and
+    ``max_candidates`` (default engine.HAWKES_EXACT_DEFAULT_BUDGET) caps the candidates per path and maturity: a path that reaches it fails
+    the call with B200svError(-6), never with biased prices."""
+    exact = _is_exact(scheme)
     vt = engine.variable_code(variable_type)
     pc = _params_c(**locals())
+    if exact:
+        _check_exact_events(float(np.max(ttms)), {k: getattr(pc, k) for k in _KEYS})
+        budget = engine.HAWKES_EXACT_DEFAULT_BUDGET if max_candidates is None else int(max_candidates)
+        flags = engine.mc_flags("fp64")
+        seed = _shared_seed(seed)
+        if _use_distributed({"distributed": distributed, "nb_path": nb_path, "exchange": exchange}):
+            t = np.asarray(ttms, dtype=np.float64)
+            grid = [(1, float(t[m] - (t[m - 1] if m > 0 else 0.0))) for m in range(t.shape[0])]
+            return mc_chain_distributed("hawkes_exact", pc, ttms, forwards, discfactors, None, strikes_ttms, optiontypes_ttms, nb_path,
+                                        STEPS_PER_YEAR, True, vt, seed, flags, exchange=exchange, grid=grid, max_candidates=budget)
+        return engine.hawkesjd_mc_chain_exact(pc, ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms, nb_path, vt, seed, flags, budget)[:2]
     seed = _shared_seed(seed)
     if _use_distributed({"distributed": distributed, "nb_path": nb_path, "exchange": exchange}):
         return mc_chain_distributed("hawkes", pc, ttms, forwards, discfactors, None, strikes_ttms, optiontypes_ttms, nb_path, STEPS_PER_YEAR,
@@ -315,10 +385,16 @@ def hawkesjd_mc_chain_pricer(ttms, forwards, discfactors, strikes_ttms, optionty
 def simulate_hawkesjd_terminal(ttm: float, x0: np.ndarray, lambda_p0: np.ndarray, lambda_m0: np.ndarray, mu: float, sigma: float, shift_p: float,
                                mean_p: float, shift_m: float, mean_m: float, theta_p: float, kappa_p: float, beta1_p: float, beta2_p: float,
                                theta_m: float, kappa_m: float, beta1_m: float, beta2_m: float, nb_path: int = 100000, seed: Optional[int] = None,
-                               gauss: str = "fp32", slice_index: int = 0, inputs=None) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+                               gauss: str = "fp32", slice_index: int = 0, inputs=None, scheme: str = "euler", max_candidates: Optional[int] = None
+                               ) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
     """terminal (log-return, lambda_p, lambda_m) with both Hawkes intensities evolving jointly (reference :718-779).  Length-1 initial
     arrays broadcast as in the reference (:742-750: x0 -> zeros, intensities -> constants).  ``inputs = (W0, U_P, U_M, J_P, J_M)`` (extra;
-    [nb_steps, nb_path] each, in the form :753-757 builds them) runs the strict kernel on caller-supplied draws."""
+    [nb_steps, nb_path] each, in the form :753-757 builds them) runs the strict kernel on caller-supplied draws.  ``scheme``, ``gauss``
+    and ``max_candidates`` as in ``hawkesjd_mc_chain_pricer``; ``inputs`` are Euler draws, so ``scheme='exact'`` with ``inputs`` raises
+    ValueError."""
+    exact = _is_exact(scheme)
+    if exact and inputs is not None:
+        raise ValueError("inputs= feeds the Euler scheme's strict kernel: it cannot be combined with scheme='exact'")
     x0, lambda_p0, lambda_m0 = np.atleast_1d(x0), np.atleast_1d(lambda_p0), np.atleast_1d(lambda_m0)
     for a in (x0, lambda_p0, lambda_m0):
         assert a.shape[0] in (1, nb_path)
@@ -334,6 +410,11 @@ def simulate_hawkesjd_terminal(ttm: float, x0: np.ndarray, lambda_p0: np.ndarray
             raise ValueError(f"inputs must be five arrays of shape ({nb_steps}, {nb_path})")
         return engine.hawkesjd_step_fixed(x, lp, lm, blocks, nb_steps, nb_path, dt, pc)
     const_start = x0.shape[0] == 1 and lambda_p0.shape[0] == 1 and lambda_m0.shape[0] == 1
+    if exact:
+        kw = {k: getattr(pc, k) for k in _KEYS}
+        _check_exact_events(float(ttm), {**kw, "lambda_p": float(np.max(np.abs(lp))), "lambda_m": float(np.max(np.abs(lm)))})
+        return engine.hawkesjd_terminal_exact(pc, ttm, x, lp, lm, engine.fresh_seed() if seed is None else int(seed), slice_index, not const_start,
+                                              engine.HAWKES_EXACT_DEFAULT_BUDGET if max_candidates is None else int(max_candidates))
     return engine.hawkesjd_terminal(pc, ttm, x, lp, lm, engine.fresh_seed() if seed is None else int(seed), engine.mc_flags("fp64", gauss),
                                     slice_index, not const_start)
 
