@@ -1348,35 +1348,48 @@ __device__ __forceinline__ cd hawkes_djump(cd z, cd dz, double s, double m, doub
   return e * (-((mk(s) + m * r) * dz) - z * (mk(ds) + dm * r));
 }
 
-// d f(A) = J(A) dA + d_p f(A) of HawkesRhsFn for one direction, d = d(consts)/d(direction)
+// d f(A) = J(A) dA + d_p f(A) of HawkesRhsFn for one direction, d = d(consts)/d(direction).  Phi adds a move dphi of the transform
+// variable (the risk kernel, DESIGN.md §4.12; psi = 0 there, so drift0 = sigma^2 (phi + 1) phi / 2):
+// d rhs0 += sigma^2 (phi + 1/2) dphi,  dz_p = dz_m += dphi,  d rhs1 += comp_p dphi,  d rhs2 += comp_m dphi.
+template <bool Phi>
 struct HawkesTanRhsFn {
   const HawkesMgfConsts& c;
   HawkesMgfConsts d;
   cd phi, h0;              // h0 = (phi + 1) phi / 2 - psi: drift0 = sigma^2 h0
+  double dphi;             // Phi: 0 on the ODE directions, -1 on the gamma direction (whose d is zero)
   __device__ __forceinline__ void operator()(const cd (&A)[3], const cd (&dA)[3], cd (&out)[3]) const {
     const cd zp = (phi - c.beta1_p * A[1]) - c.beta1_m * A[2], zm = (phi - c.beta2_p * A[1]) - c.beta2_m * A[2];
-    const cd dzp = -(((c.beta1_p * dA[1] + c.beta1_m * dA[2]) + d.beta1_p * A[1]) + d.beta1_m * A[2]);
-    const cd dzm = -(((c.beta2_p * dA[1] + c.beta2_m * dA[2]) + d.beta2_p * A[1]) + d.beta2_m * A[2]);
+    const cd bp = ((c.beta1_p * dA[1] + c.beta1_m * dA[2]) + d.beta1_p * A[1]) + d.beta1_m * A[2];
+    const cd bm = ((c.beta2_p * dA[1] + c.beta2_m * dA[2]) + d.beta2_p * A[1]) + d.beta2_m * A[2];
+    const cd dzp = Phi ? mk(dphi) - bp : -bp, dzm = Phi ? mk(dphi) - bm : -bm;
     out[0] = (((c.kt_p * dA[1] + c.kt_m * dA[2]) + d.kt_p * A[1]) + d.kt_m * A[2]) + d.sigma2 * h0;
+    if (Phi) out[0] = out[0] + (c.sigma2 * dphi) * (phi + mk(0.5));
     out[1] = (hawkes_djump(zp, dzp, c.shift_p, c.mean_p, d.shift_p, d.mean_p) - (c.kappa_p * dA[1] + d.kappa_p * A[1])) + d.comp_p * phi;
+    if (Phi) out[1] = out[1] + mk(c.comp_p * dphi);
     out[2] = (hawkes_djump(zm, dzm, c.shift_m, c.mean_m, d.shift_m, d.mean_m) - (c.kappa_m * dA[2] + d.kappa_m * A[2])) + d.comp_m * phi;
+    if (Phi) out[2] = out[2] + mk(c.comp_m * dphi);
   }
 };
 
-// hawkes_mgf_kernel in forward mode: one thread = one (grid point, ODE direction), the primal integration of hawkes_mgf_kernel (same
-// rk45_generic, same mesh) plus one tangent, A and dA carried over the maturities.  The 13 directions of a point are neighbouring threads,
-// so a warp runs few meshes.  Outputs: dlog_mgf [15][M][P] (HAWKES_GREEK_PARAMS order; rows 5 / 10 = a_p / a_m), log_mgf [M][P],
-// status [P], nfev [P] (each optional but dlog_mgf).
-template <int TPB>
+// hawkes_mgf_kernel in forward mode: one thread = one (grid point, direction), the primal integration of hawkes_mgf_kernel (same
+// rk45_generic, same mesh) plus one tangent.  The D = 13 ODE directions of a point, and with Phi the gamma direction of the risk kernel
+// (DESIGN.md §4.12) as the 14th, are neighbouring threads, so a warp runs few meshes.  restart = 0: A and dA carried over the maturity
+// increments dtaus (the grid); restart != 0 (Phi only): every maturity restarts from A = dA = 0 and integrates over its full ttm dtaus[m]
+// (the normaliser points, as hawkes_mgf_kernel's restart mode).  Outputs: dlog_mgf [15 + Phi][M][P] (HAWKES_GREEK_PARAMS order, then
+// HAWKES_RISK_PREMIA_GREEK_PARAMS' row 15 = d/d gamma; rows 5 / 10 = a_p / a_m), log_mgf [M][P], status [P] (!Phi only), nfev [P] (each
+// optional but dlog_mgf).
+template <int TPB, bool Phi>
 __global__ void __launch_bounds__(TPB) hawkes_mgf_tangent_kernel(const cd* __restrict__ phi, int P, int M, const double* __restrict__ dtaus,
-                                                                 HawkesMgfConsts c, HawkesTangentDirs dirs, cd* __restrict__ dlog_mgf,
-                                                                 cd* __restrict__ log_mgf, int* __restrict__ status, int* __restrict__ nfev) {
-  constexpr int D = kHawkesOdeDirs;
+                                                                 HawkesMgfConsts c, HawkesTangentDirs dirs, int restart,
+                                                                 cd* __restrict__ dlog_mgf, cd* __restrict__ log_mgf, int* __restrict__ status,
+                                                                 int* __restrict__ nfev) {
+  constexpr int D = kHawkesOdeDirs + Phi;
   __shared__ cd stage_smem[6 * 3 * TPB];
   __shared__ cd tan_smem[8 * 3 * TPB];
   const int t = blockIdx.x * TPB + threadIdx.x;
   if (t >= P * D) return;
   const int p = t / D, dir = t % D;
+  const bool gdir = Phi && dir == kHawkesOdeDirs;
 #pragma unroll
   for (int i = 0; i < 18; ++i) stage_smem[threadIdx.x + i * TPB] = mk(0.0);
 #pragma unroll
@@ -1385,11 +1398,17 @@ __global__ void __launch_bounds__(TPB) hawkes_mgf_tangent_kernel(const cd* __res
   const cd ph = phi[p];
   const cd h0 = 0.5 * ((ph + mk(1.0)) * ph);
   const HawkesRhsFn f{c, ph, c.sigma2 * h0};
-  TangentHook<3, TPB, HawkesTanRhsFn> tan{HawkesTanRhsFn{c, dirs.d[dir], ph, h0}, {StageStore<3, TPB>{tan_smem + threadIdx.x}, {}}};   // dy = 0
+  const HawkesMgfConsts zero{0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+  TangentHook<3, TPB, HawkesTanRhsFn<Phi>> tan{HawkesTanRhsFn<Phi>{c, gdir ? zero : dirs.d[dir], ph, h0, gdir ? -1.0 : 0.0},
+                                               {StageStore<3, TPB>{tan_smem + threadIdx.x}, {}}};   // dy = 0
   cd A[3] = {mk(0.0), mk(0.0), mk(0.0)};
-  const int row = hawkes_dir_row(dir);
+  const int row = gdir ? kHawkesGreekParams : hawkes_dir_row(dir);
   int st = 0, nf = 0;
   for (int m = 0; m < M; ++m) {
+    if (Phi && restart) {
+#pragma unroll
+      for (int k = 0; k < 3; ++k) A[k] = tan.t.dy[k] = mk(0.0);
+    }
     int nfe = 0;
     st |= rk45_generic<3, TPB>(A, dtaus[m], f, K, &nfe, &tan);
     nf += nfe;
@@ -1401,7 +1420,7 @@ __global__ void __launch_bounds__(TPB) hawkes_mgf_tangent_kernel(const cd* __res
     }
   }
   if (dir == 0) {
-    if (status) status[p] = st;
+    if (!Phi && status) status[p] = st;
     if (nfev) nfev[p] = nf;
   }
 }
@@ -1453,76 +1472,9 @@ __global__ void __launch_bounds__(kFourierThreads) fourier_vanilla_greeks_kernel
 
 // ---- Hawkes jump-diffusion under the risk kernel (DESIGN.md §4.12) ----
 // risk_premia_gamma moves every transform point, on the grid (Re phi = -1/2 - gamma) and at the two normaliser points (-gamma,
-// -gamma - 1), by d phi / d gamma = -1: a 14th tangent direction, in the transform variable, next to the 13 ODE directions.
-constexpr int kHawkesRpDirs = kHawkesOdeDirs + 1;
+// -gamma - 1), by d phi / d gamma = -1: a 14th tangent direction, in the transform variable, next to the 13 ODE directions (the Phi
+// instantiations of HawkesTanRhsFn, hawkes_mgf_tangent_kernel, HawkesTan2RhsFn and hawkes_mgf_hessian_kernel).
 constexpr int kHawkesRpParams = kHawkesGreekParams + 1;      // HAWKES_RISK_PREMIA_GREEK_PARAMS: HAWKES_GREEK_PARAMS, then risk_premia_gamma
-
-// HawkesTanRhsFn plus a move dphi of the transform variable (psi = 0, so drift0 = sigma^2 (phi + 1) phi / 2):
-// d rhs0 += sigma^2 (phi + 1/2) dphi,  dz_p = dz_m += dphi,  d rhs1 += comp_p dphi,  d rhs2 += comp_m dphi.
-struct HawkesRpTanRhsFn {
-  const HawkesMgfConsts& c;
-  HawkesMgfConsts d;
-  cd phi, h0;              // h0 = (phi + 1) phi / 2
-  double dphi;             // 0 on the ODE directions, -1 on the gamma direction (whose d is zero)
-  __device__ __forceinline__ void operator()(const cd (&A)[3], const cd (&dA)[3], cd (&out)[3]) const {
-    const cd zp = (phi - c.beta1_p * A[1]) - c.beta1_m * A[2], zm = (phi - c.beta2_p * A[1]) - c.beta2_m * A[2];
-    const cd dzp = mk(dphi) - (((c.beta1_p * dA[1] + c.beta1_m * dA[2]) + d.beta1_p * A[1]) + d.beta1_m * A[2]);
-    const cd dzm = mk(dphi) - (((c.beta2_p * dA[1] + c.beta2_m * dA[2]) + d.beta2_p * A[1]) + d.beta2_m * A[2]);
-    out[0] = ((((c.kt_p * dA[1] + c.kt_m * dA[2]) + d.kt_p * A[1]) + d.kt_m * A[2]) + d.sigma2 * h0) + (c.sigma2 * dphi) * (phi + mk(0.5));
-    out[1] = ((hawkes_djump(zp, dzp, c.shift_p, c.mean_p, d.shift_p, d.mean_p) - (c.kappa_p * dA[1] + d.kappa_p * A[1])) + d.comp_p * phi) +
-             mk(c.comp_p * dphi);
-    out[2] = ((hawkes_djump(zm, dzm, c.shift_m, c.mean_m, d.shift_m, d.mean_m) - (c.kappa_m * dA[2] + d.kappa_m * A[2])) + d.comp_m * phi) +
-             mk(c.comp_m * dphi);
-  }
-};
-
-// hawkes_mgf_tangent_kernel with the gamma direction: one thread = one (point, direction), 14 directions, the primal integration of
-// hawkes_mgf_kernel (same rk45_generic, same mesh) plus one tangent.  restart = 0: A and dA carried over the maturity increments dtaus
-// (the grid); restart != 0: every maturity restarts from A = dA = 0 and integrates over its full ttm dtaus[m] (the normaliser points, as
-// hawkes_mgf_kernel's restart mode).  Outputs: dlog_mgf [16][M][P] (HAWKES_RISK_PREMIA_GREEK_PARAMS order: rows 5 / 10 = a_p / a_m,
-// row 15 = d/d gamma), log_mgf [M][P] and nfev [P] (both optional).
-template <int TPB>
-__global__ void __launch_bounds__(TPB) hawkes_mgf_rp_tangent_kernel(const cd* __restrict__ phi, int P, int M, const double* __restrict__ dtaus,
-                                                                    HawkesMgfConsts c, HawkesTangentDirs dirs, int restart,
-                                                                    cd* __restrict__ dlog_mgf, cd* __restrict__ log_mgf, int* __restrict__ nfev) {
-  constexpr int D = kHawkesRpDirs;
-  __shared__ cd stage_smem[6 * 3 * TPB];
-  __shared__ cd tan_smem[8 * 3 * TPB];
-  const int t = blockIdx.x * TPB + threadIdx.x;
-  if (t >= P * D) return;
-  const int p = t / D, dir = t % D;
-  const bool gdir = dir == kHawkesOdeDirs;
-#pragma unroll
-  for (int i = 0; i < 18; ++i) stage_smem[threadIdx.x + i * TPB] = mk(0.0);
-#pragma unroll
-  for (int i = 0; i < 24; ++i) tan_smem[threadIdx.x + i * TPB] = mk(0.0);
-  StageStore<3, TPB> K{stage_smem + threadIdx.x};
-  const cd ph = phi[p];
-  const cd h0 = 0.5 * ((ph + mk(1.0)) * ph);
-  const HawkesRhsFn f{c, ph, c.sigma2 * h0};
-  const HawkesMgfConsts zero{0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-  TangentHook<3, TPB, HawkesRpTanRhsFn> tan{HawkesRpTanRhsFn{c, gdir ? zero : dirs.d[dir], ph, h0, gdir ? -1.0 : 0.0},
-                                           {StageStore<3, TPB>{tan_smem + threadIdx.x}, {}}};   // dy = 0
-  cd A[3] = {mk(0.0), mk(0.0), mk(0.0)};
-  const int row = gdir ? kHawkesGreekParams : hawkes_dir_row(dir);
-  int nf = 0;
-  for (int m = 0; m < M; ++m) {
-    if (restart) {
-#pragma unroll
-      for (int k = 0; k < 3; ++k) A[k] = tan.t.dy[k] = mk(0.0);
-    }
-    int nfe = 0;
-    rk45_generic<3, TPB>(A, dtaus[m], f, K, &nfe, &tan);
-    nf += nfe;
-    dlog_mgf[((size_t)row * M + m) * P + p] = (tan.t.dy[0] + tan.t.dy[1] * c.lambda_p) + tan.t.dy[2] * c.lambda_m;
-    if (dir == 0) {
-      dlog_mgf[((size_t)5 * M + m) * P + p] = A[1];
-      dlog_mgf[((size_t)10 * M + m) * P + p] = A[2];
-      if (log_mgf) log_mgf[(size_t)m * P + p] = (A[0] + A[1] * c.lambda_p) + A[2] * c.lambda_m;
-    }
-  }
-  if (dir == 0 && nfev) nfev[p] = nf;
-}
 
 // Sums of fourier_gamma_batch_kernel (same weight branch, same NaN skip) and their derivatives, one CTA per strike, fixed-order block_sum:
 // with e = exp(lm - x phi), x = ln(F/K):  S = sum Re(w e),  S_x = sum Re(-w phi e),  S_xx = sum Re(w phi^2 e),  S_p = sum Re(w e dlm_p),
@@ -1958,13 +1910,11 @@ __global__ void __launch_bounds__(kFourierThreads) fourier_vanilla_hessian_split
 }
 
 // ---- Hawkes jump-diffusion, second order (DESIGN.md §4.5) ----
-constexpr int kHawkesOdePairs = kHawkesOdeDirs * (kHawkesOdeDirs + 1) / 2;  // 91 pairs over the 13 ODE directions
-
-// d2(HawkesMgfConsts field) / d(direction p) d(direction q) for the kHawkesOdePairs pairs (tri_index order over the ODE directions of
-// make_hawkes_tangents).  Nonzero: sigma2 = sigma^2, kt = kappa theta and comp = e^shift / (1 - mean) - 1.
-static void make_hawkes_hessian(const b200sv_hawkes_params& p, HawkesMgfConsts (&h)[kHawkesOdePairs]) {
-  for (auto& t : h) t = HawkesMgfConsts{0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-  constexpr int D = kHawkesOdeDirs;
+// d2(HawkesMgfConsts field) / d(direction p) d(direction q) for the D (D + 1) / 2 pairs of the D directions of hawkes_mgf_hessian_kernel
+// (tri_index order over the ODE directions of make_hawkes_tangents, then with D = 14 the transform variable, which no field depends on).
+// Nonzero: sigma2 = sigma^2, kt = kappa theta and comp = e^shift / (1 - mean) - 1.
+static std::vector<HawkesMgfConsts> make_hawkes_hessian(const b200sv_hawkes_params& p, int D) {
+  std::vector<HawkesMgfConsts> h((size_t)D * (D + 1) / 2, HawkesMgfConsts{0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0});
   const double ep = std::exp(p.shift_p) / (1.0 - p.mean_p), em = std::exp(p.shift_m) / (1.0 - p.mean_m);
   h[tri_index(0, 0, D)].sigma2 = 2.0;                                                  // sigma sigma
   h[tri_index(5, 6, D)].kt_p = 1.0;                                                    // theta_p kappa_p
@@ -1975,28 +1925,35 @@ static void make_hawkes_hessian(const b200sv_hawkes_params& p, HawkesMgfConsts (
   h[tri_index(3, 3, D)].comp_m = em;                                                   // shift_m shift_m
   h[tri_index(3, 4, D)].comp_m = em / (1.0 - p.mean_m);                                // shift_m mean_m
   h[tri_index(4, 4, D)].comp_m = 2.0 * em / ((1.0 - p.mean_m) * (1.0 - p.mean_m));     // mean_m mean_m
+  return h;
 }
 
-// The three right-hand sides of one ODE pair (p, q) in one hyper-dual evaluation of HawkesRhsFn's arithmetic: with A_k = (A, dA_p, dA_q,
+// The three right-hand sides of one pair (p, q) in one hyper-dual evaluation of HawkesRhsFn's arithmetic: with A_k = (A, dA_p, dA_q,
 // d2A_pq) and every HawkesMgfConsts field f = (f, df/dp, df/dq, d2f/dp dq), the parts .d1 / .d2 are the tangent right-hand sides
 // J(A) dA_p + d_p f(A) (HawkesTanRhsFn) and J(A) dA_q + d_q f(A), and .d12 is
 //   J(A) d2A + f_AA(dA_p, dA_q) + d_p J(A) dA_q + d_q J(A) dA_p + d_pq f(A).
 // The jump-size MGF E(z; s, m) = e^{-s z} / (1 + m z) goes through hcd's exp_ and Smith division jointly in (z, s, m); the constant -1 of
-// E - 1 has no derivative and is left out.
+// E - 1 has no derivative and is left out.  phi = (phi, dphi_p, dphi_q, 0): without Phi, hmk(phi), and h0 comes precomputed.  Phi puts the
+// transform variable among the seeded variables (the risk kernel, DESIGN.md §4.13): dphi = -1 on the gamma direction and 0 on the ODE
+// directions, so the hyper-dual algebra also forms every phi cross term (h0 = (phi + 1) phi / 2, comp phi and z = phi - beta a inside the
+// jump MGFs).  phi is linear in gamma: its own second part is zero.
+template <bool Phi>
 struct HawkesTan2RhsFn {
   const HawkesMgfConsts& c;
   HawkesMgfConsts dp, dq, d2;
-  cd phi, h0;              // h0 = (phi + 1) phi / 2 - psi: drift0 = sigma^2 h0
+  hcd phi;
+  cd h0;                   // !Phi: h0 = (phi + 1) phi / 2 - psi: drift0 = sigma^2 h0
   __device__ __forceinline__ hcd k(double HawkesMgfConsts::*f) const { return hcd{mk(c.*f), mk(dp.*f), mk(dq.*f), mk(d2.*f)}; }
   __device__ __forceinline__ void operator()(const cd (&Y)[3], const cd (&dYp)[3], const cd (&dYq)[3], const cd (&d2Y)[3], cd (&op)[3],
                                              cd (&oq)[3], cd (&opq)[3]) const {
     using H = HawkesMgfConsts;
-    const hcd a1{Y[1], dYp[1], dYq[1], d2Y[1]}, a2{Y[2], dYp[2], dYq[2], d2Y[2]}, ph = hmk(phi), one = hmk(mk(1.0));
-    const hcd zp = (ph - k(&H::beta1_p) * a1) - k(&H::beta1_m) * a2, zm = (ph - k(&H::beta2_p) * a1) - k(&H::beta2_m) * a2;
+    const hcd a1{Y[1], dYp[1], dYq[1], d2Y[1]}, a2{Y[2], dYp[2], dYq[2], d2Y[2]}, one = hmk(mk(1.0));
+    const hcd zp = (phi - k(&H::beta1_p) * a1) - k(&H::beta1_m) * a2, zm = (phi - k(&H::beta2_p) * a1) - k(&H::beta2_m) * a2;
     const hcd jp = exp_(-(k(&H::shift_p) * zp)) / (one + k(&H::mean_p) * zp);
     const hcd jm = exp_(-(k(&H::shift_m) * zm)) / (one + k(&H::mean_m) * zm);
-    const hcd o[3] = {(k(&H::kt_p) * a1 + k(&H::kt_m) * a2) + k(&H::sigma2) * hmk(h0), (jp - k(&H::kappa_p) * a1) + k(&H::comp_p) * ph,
-                      (jm - k(&H::kappa_m) * a2) + k(&H::comp_m) * ph};
+    const hcd h = Phi ? 0.5 * ((phi + one) * phi) : hmk(h0);
+    const hcd o[3] = {(k(&H::kt_p) * a1 + k(&H::kt_m) * a2) + k(&H::sigma2) * h, (jp - k(&H::kappa_p) * a1) + k(&H::comp_p) * phi,
+                      (jm - k(&H::kappa_m) * a2) + k(&H::comp_m) * phi};
 #pragma unroll
     for (int i = 0; i < 3; ++i) {
       op[i] = o[i].d1;
@@ -2008,101 +1965,27 @@ struct HawkesTan2RhsFn {
 
 constexpr int kHawkesHessianTPB = 32;   // static shared memory per thread: 6 x 3 primal + 3 x 8 x 3 tangent stages = 1 440 B, 45 KB per CTA
 
-// One thread = one (grid point, ODE pair p <= q): the primal integration of hawkes_mgf_kernel (same rk45_generic, same mesh) plus the
-// tangents of p and q and their mixed second-order tangent (Tangent2Hook), carried over the maturities like A.  The 91 pairs of a point are
-// neighbouring threads.  lm = a0 + a_p lambda_p + a_m lambda_m is linear in the lambdas and they have no ODE tangent, so
+// One thread = one (grid point, pair p <= q of the D = 13 ODE directions, with Phi also the gamma direction of hawkes_mgf_tangent_kernel):
+// the primal integration of hawkes_mgf_kernel (same rk45_generic, same mesh) plus the tangents of p and q and their mixed second-order
+// tangent (Tangent2Hook).  The D (D + 1) / 2 pairs of a point are neighbouring threads.  restart = 0: carried over the maturity increments
+// dtaus like A (the grid); restart != 0 (Phi only): every maturity restarts from A = 0 and integrates over its full ttm dtaus[m] (the
+// normaliser points).  lm = a0 + a_p lambda_p + a_m lambda_m is linear in the lambdas and they have no ODE tangent, so
 //   d2lm_pq = d2a0 + d2a_p lambda_p + d2a_m lambda_m,  d2lm / dlambda_p dq = da_p / dq,  d2lm / dlambda_m dq = da_m / dq,  d2lm / dlambda dlambda = 0:
-// the diagonal thread of direction d also writes (lambda_p, d) and (lambda_m, d), pair 0 the three lambda-lambda rows.  dirs: the first
-// field derivatives (make_hawkes_tangents), d2c [91]: the second (make_hawkes_hessian).  Output d2log_mgf [120][M][P] (tri_index over
-// HAWKES_GREEK_PARAMS).
+// the diagonal thread of direction d also writes (lambda_p, d) and (lambda_m, d) (for the phi direction da / dgamma = -da / dphi), pair 0
+// the three lambda-lambda rows.  dirs: the first field derivatives (make_hawkes_tangents), d2c [D (D + 1) / 2]: the second
+// (make_hawkes_hessian).  Output d2log_mgf [NP (NP + 1) / 2][M][P] (tri_index over HAWKES_GREEK_PARAMS, NP = 15, or with Phi over
+// HAWKES_RISK_PREMIA_GREEK_PARAMS, NP = 16).
+template <bool Phi>
 __global__ void __launch_bounds__(kHawkesHessianTPB) hawkes_mgf_hessian_kernel(const cd* __restrict__ phi, int P, int M,
                                                                                const double* __restrict__ dtaus, HawkesMgfConsts c,
                                                                                HawkesTangentDirs dirs, const HawkesMgfConsts* __restrict__ d2c,
-                                                                               cd* __restrict__ d2log_mgf) {
-  constexpr int TPB = kHawkesHessianTPB, D = kHawkesOdeDirs, NP = kHawkesGreekParams;
+                                                                               int restart, cd* __restrict__ d2log_mgf) {
+  constexpr int TPB = kHawkesHessianTPB, D = kHawkesOdeDirs + Phi, NP = kHawkesGreekParams + Phi, NPAIRS = D * (D + 1) / 2;
   __shared__ cd stage_smem[6 * 3 * TPB];
   __shared__ cd tan_smem[3 * 8 * 3 * TPB];
   const int t = blockIdx.x * TPB + threadIdx.x;
-  if (t >= P * kHawkesOdePairs) return;
-  const int p = t / kHawkesOdePairs, pair = t % kHawkesOdePairs;
-  int dp, dq;
-  tri_pair(pair, D, dp, dq);
-#pragma unroll
-  for (int i = 0; i < 18; ++i) stage_smem[threadIdx.x + i * TPB] = mk(0.0);
-#pragma unroll
-  for (int i = 0; i < 72; ++i) tan_smem[threadIdx.x + i * TPB] = mk(0.0);
-  StageStore<3, TPB> K{stage_smem + threadIdx.x};
-  const cd ph = phi[p];
-  const cd h0 = 0.5 * ((ph + mk(1.0)) * ph);
-  const HawkesRhsFn f{c, ph, c.sigma2 * h0};
-  Tangent2Hook<3, TPB, HawkesTan2RhsFn> tan{HawkesTan2RhsFn{c, dirs.d[dp], dirs.d[dq], d2c[pair], ph, h0},
-                                            {StageStore<3, TPB>{tan_smem + threadIdx.x}, {}},
-                                            {StageStore<3, TPB>{tan_smem + 24 * TPB + threadIdx.x}, {}},
-                                            {StageStore<3, TPB>{tan_smem + 48 * TPB + threadIdx.x}, {}}};   // dy = 0
-  cd A[3] = {mk(0.0), mk(0.0), mk(0.0)};
-  const int rp = hawkes_dir_row(dp), rq = hawkes_dir_row(dq);
-  for (int m = 0; m < M; ++m) {
-    rk45_generic<3, TPB>(A, dtaus[m], f, K, nullptr, &tan);
-    d2log_mgf[((size_t)tri_index(rp, rq, NP) * M + m) * P + p] = (tan.pq.dy[0] + tan.pq.dy[1] * c.lambda_p) + tan.pq.dy[2] * c.lambda_m;
-    if (dp == dq) {
-      d2log_mgf[((size_t)tri_index(min(5, rp), max(5, rp), NP) * M + m) * P + p] = tan.p.dy[1];
-      d2log_mgf[((size_t)tri_index(min(10, rp), max(10, rp), NP) * M + m) * P + p] = tan.p.dy[2];
-    }
-    if (pair == 0) {
-      d2log_mgf[((size_t)tri_index(5, 5, NP) * M + m) * P + p] = mk(0.0);
-      d2log_mgf[((size_t)tri_index(5, 10, NP) * M + m) * P + p] = mk(0.0);
-      d2log_mgf[((size_t)tri_index(10, 10, NP) * M + m) * P + p] = mk(0.0);
-    }
-  }
-}
-
-// ---- Hawkes jump-diffusion under the risk kernel, second order (DESIGN.md §4.13) ----
-constexpr int kHawkesRpPairs = kHawkesRpDirs * (kHawkesRpDirs + 1) / 2;   // 105 pairs over the 13 ODE directions and phi
-
-// HawkesTan2RhsFn with the transform variable among the seeded variables: phi = (phi, dphi_p, dphi_q, 0), dphi = -1 on the gamma direction
-// and 0 on the ODE directions, so the hyper-dual algebra also forms every phi cross term (h0 = (phi + 1) phi / 2, comp phi and z = phi -
-// beta a inside the jump MGFs).  phi is linear in gamma: its own second part is zero.
-struct HawkesRpTan2RhsFn {
-  const HawkesMgfConsts& c;
-  HawkesMgfConsts dp, dq, d2;
-  hcd phi;
-  __device__ __forceinline__ hcd k(double HawkesMgfConsts::*f) const { return hcd{mk(c.*f), mk(dp.*f), mk(dq.*f), mk(d2.*f)}; }
-  __device__ __forceinline__ void operator()(const cd (&Y)[3], const cd (&dYp)[3], const cd (&dYq)[3], const cd (&d2Y)[3], cd (&op)[3],
-                                             cd (&oq)[3], cd (&opq)[3]) const {
-    using H = HawkesMgfConsts;
-    const hcd a1{Y[1], dYp[1], dYq[1], d2Y[1]}, a2{Y[2], dYp[2], dYq[2], d2Y[2]}, one = hmk(mk(1.0));
-    const hcd zp = (phi - k(&H::beta1_p) * a1) - k(&H::beta1_m) * a2, zm = (phi - k(&H::beta2_p) * a1) - k(&H::beta2_m) * a2;
-    const hcd jp = exp_(-(k(&H::shift_p) * zp)) / (one + k(&H::mean_p) * zp);
-    const hcd jm = exp_(-(k(&H::shift_m) * zm)) / (one + k(&H::mean_m) * zm);
-    const hcd h0 = 0.5 * ((phi + one) * phi);
-    const hcd o[3] = {(k(&H::kt_p) * a1 + k(&H::kt_m) * a2) + k(&H::sigma2) * h0, (jp - k(&H::kappa_p) * a1) + k(&H::comp_p) * phi,
-                      (jm - k(&H::kappa_m) * a2) + k(&H::comp_m) * phi};
-#pragma unroll
-    for (int i = 0; i < 3; ++i) {
-      op[i] = o[i].d1;
-      oq[i] = o[i].d2;
-      opq[i] = o[i].d12;
-    }
-  }
-};
-
-// hawkes_mgf_hessian_kernel with the gamma direction of hawkes_mgf_rp_tangent_kernel: one thread = one (point, pair p <= q of the 14
-// directions), the primal integration of hawkes_mgf_kernel (same rk45_generic, same mesh) plus the tangents of p and q and their mixed
-// second-order tangent.  restart = 0: carried over the maturity increments dtaus (the grid); restart != 0: every maturity restarts from
-// A = 0 and integrates over its full ttm dtaus[m] (the normaliser points).  As there, the lambdas have no ODE tangent: the diagonal thread of
-// direction d writes (lambda_p, d) = da_p / dd and (lambda_m, d) = da_m / dd (for the phi direction da / dgamma = -da / dphi), pair 0 the
-// three lambda-lambda zeros.  d2c [105]: the second field derivatives per pair (zero on the pairs with phi).  Output d2log_mgf [136][M][P]
-// (tri_index over HAWKES_RISK_PREMIA_GREEK_PARAMS).
-__global__ void __launch_bounds__(kHawkesHessianTPB) hawkes_mgf_rp_hessian_kernel(const cd* __restrict__ phi, int P, int M,
-                                                                                  const double* __restrict__ dtaus, HawkesMgfConsts c,
-                                                                                  HawkesTangentDirs dirs, const HawkesMgfConsts* __restrict__ d2c,
-                                                                                  int restart, cd* __restrict__ d2log_mgf) {
-  constexpr int TPB = kHawkesHessianTPB, D = kHawkesRpDirs, NP = kHawkesRpParams;
-  __shared__ cd stage_smem[6 * 3 * TPB];
-  __shared__ cd tan_smem[3 * 8 * 3 * TPB];
-  const int t = blockIdx.x * TPB + threadIdx.x;
-  if (t >= P * kHawkesRpPairs) return;
-  const int p = t / kHawkesRpPairs, pair = t % kHawkesRpPairs;
+  if (t >= P * NPAIRS) return;
+  const int p = t / NPAIRS, pair = t % NPAIRS;
   int dp, dq;
   tri_pair(pair, D, dp, dq);
 #pragma unroll
@@ -2114,16 +1997,16 @@ __global__ void __launch_bounds__(kHawkesHessianTPB) hawkes_mgf_rp_hessian_kerne
   const cd h0 = 0.5 * ((ph + mk(1.0)) * ph);
   const HawkesRhsFn f{c, ph, c.sigma2 * h0};
   const HawkesMgfConsts zero{0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-  const bool gp = dp == kHawkesOdeDirs, gq = dq == kHawkesOdeDirs;
+  const bool gp = Phi && dp == kHawkesOdeDirs, gq = Phi && dq == kHawkesOdeDirs;
   const hcd hph{ph, mk(gp ? -1.0 : 0.0), mk(gq ? -1.0 : 0.0), mk(0.0)};
-  Tangent2Hook<3, TPB, HawkesRpTan2RhsFn> tan{HawkesRpTan2RhsFn{c, gp ? zero : dirs.d[dp], gq ? zero : dirs.d[dq], d2c[pair], hph},
-                                              {StageStore<3, TPB>{tan_smem + threadIdx.x}, {}},
-                                              {StageStore<3, TPB>{tan_smem + 24 * TPB + threadIdx.x}, {}},
-                                              {StageStore<3, TPB>{tan_smem + 48 * TPB + threadIdx.x}, {}}};   // dy = 0
+  Tangent2Hook<3, TPB, HawkesTan2RhsFn<Phi>> tan{HawkesTan2RhsFn<Phi>{c, gp ? zero : dirs.d[dp], gq ? zero : dirs.d[dq], d2c[pair], hph, h0},
+                                                 {StageStore<3, TPB>{tan_smem + threadIdx.x}, {}},
+                                                 {StageStore<3, TPB>{tan_smem + 24 * TPB + threadIdx.x}, {}},
+                                                 {StageStore<3, TPB>{tan_smem + 48 * TPB + threadIdx.x}, {}}};   // dy = 0
   cd A[3] = {mk(0.0), mk(0.0), mk(0.0)};
   const int rp = gp ? kHawkesGreekParams : hawkes_dir_row(dp), rq = gq ? kHawkesGreekParams : hawkes_dir_row(dq);
   for (int m = 0; m < M; ++m) {
-    if (restart) {
+    if (Phi && restart) {
 #pragma unroll
       for (int k = 0; k < 3; ++k) A[k] = tan.p.dy[k] = tan.q.dy[k] = tan.pq.dy[k] = mk(0.0);
     }
@@ -2141,6 +2024,7 @@ __global__ void __launch_bounds__(kHawkesHessianTPB) hawkes_mgf_rp_hessian_kerne
   }
 }
 
+// ---- Hawkes jump-diffusion under the risk kernel, second order (DESIGN.md §4.13) ----
 // The second-order risk-kernel sums next to fourier_gamma_greeks_kernel's (same weight branch, same NaN skip, fixed-order block_sum), a
 // strike split over the CTAs blockIdx.y as in fourier_vanilla_hessian_split_kernel.  With e = exp(lm - x phi), x = ln(F/K), the per-strike
 // tangents T_p = dlm_p (T_gamma = dlm_gamma + x) and T_pq = d2lm_pq:
@@ -2359,7 +2243,7 @@ __global__ void __launch_bounds__(kThetaTPB) hawkes_mgf_theta_kernel(const cd* _
   const cd h0 = 0.5 * ((ph + mk(1.0)) * ph);
   const HawkesRhsFn f{c, ph, c.sigma2 * h0};
   const HawkesMgfConsts zero{0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};      // no explicit d/dT of the right-hand side
-  ThetaHook<3, TPB, HawkesTanRhsFn> tan{HawkesTanRhsFn{c, zero, ph, h0}, K, StageStore<3, TPB>{g_smem + threadIdx.x}, {}};
+  ThetaHook<3, TPB, HawkesTanRhsFn<false>> tan{HawkesTanRhsFn<false>{c, zero, ph, h0}, K, StageStore<3, TPB>{g_smem + threadIdx.x}, {}};
   cd A[3] = {mk(0.0), mk(0.0), mk(0.0)};
   int nf = 0;
   for (int m = 0; m < M; ++m) {
@@ -3051,35 +2935,21 @@ static void launch_hawkes_mgf_sets(cudaStream_t st, const cd* phi, int P, int M,
   k<<<(unsigned)((n + tpb - 1) / tpb), tpb, 0, st>>>(phi, P, M, dtaus, consts, B, phi_stride, lm, set_m0);
 }
 
-// hawkes_mgf_tangent_kernel over the P * 13 (point, direction) threads; block size as for hawkes_mgf_kernel, from the threads in flight
-using HawkesTangentKernel = decltype(&hawkes_mgf_tangent_kernel<64>);
+// hawkes_mgf_tangent_kernel<TPB, Phi> over the P * (13 + Phi) (point, direction) threads; block size as for hawkes_mgf_kernel, from the
+// threads in flight
+template <bool Phi>
 static void launch_hawkes_mgf_tangent(cudaStream_t st, const cd* phi, int P, int M, const double* dtaus, const HawkesMgfConsts& c,
-                                      const HawkesTangentDirs& dirs, cd* dlm, cd* lm, int* nfev) {
-  const int n = P * kHawkesOdeDirs, tpb = mgf_block_threads(n);
-  HawkesTangentKernel k;
+                                      const HawkesTangentDirs& dirs, int restart, cd* dlm, cd* lm, int* nfev) {
+  const int n = P * (kHawkesOdeDirs + Phi), tpb = mgf_block_threads(n);
+  decltype(&hawkes_mgf_tangent_kernel<64, Phi>) k;
   switch (tpb) {
-    case 4: k = hawkes_mgf_tangent_kernel<4>; break;
-    case 8: k = hawkes_mgf_tangent_kernel<8>; break;
-    case 16: k = hawkes_mgf_tangent_kernel<16>; break;
-    case 32: k = hawkes_mgf_tangent_kernel<32>; break;
-    default: k = hawkes_mgf_tangent_kernel<64>;
+    case 4: k = hawkes_mgf_tangent_kernel<4, Phi>; break;
+    case 8: k = hawkes_mgf_tangent_kernel<8, Phi>; break;
+    case 16: k = hawkes_mgf_tangent_kernel<16, Phi>; break;
+    case 32: k = hawkes_mgf_tangent_kernel<32, Phi>; break;
+    default: k = hawkes_mgf_tangent_kernel<64, Phi>;
   }
-  k<<<(n + tpb - 1) / tpb, tpb, 0, st>>>(phi, P, M, dtaus, c, dirs, dlm, lm, nullptr, nfev);
-}
-
-// hawkes_mgf_rp_tangent_kernel over the P * 14 (point, direction) threads, block size chosen the same way
-static void launch_hawkes_mgf_rp_tangent(cudaStream_t st, const cd* phi, int P, int M, const double* dtaus, const HawkesMgfConsts& c,
-                                         const HawkesTangentDirs& dirs, int restart, cd* dlm, cd* lm, int* nfev) {
-  const int n = P * kHawkesRpDirs, tpb = mgf_block_threads(n);
-  decltype(&hawkes_mgf_rp_tangent_kernel<64>) k;
-  switch (tpb) {
-    case 4: k = hawkes_mgf_rp_tangent_kernel<4>; break;
-    case 8: k = hawkes_mgf_rp_tangent_kernel<8>; break;
-    case 16: k = hawkes_mgf_rp_tangent_kernel<16>; break;
-    case 32: k = hawkes_mgf_rp_tangent_kernel<32>; break;
-    default: k = hawkes_mgf_rp_tangent_kernel<64>;
-  }
-  k<<<(n + tpb - 1) / tpb, tpb, 0, st>>>(phi, P, M, dtaus, c, dirs, restart, dlm, lm, nfev);
+  k<<<(n + tpb - 1) / tpb, tpb, 0, st>>>(phi, P, M, dtaus, c, dirs, restart, dlm, lm, nullptr, nfev);
 }
 
 // ---- chain preparation ----
@@ -3485,8 +3355,8 @@ static int queue_hawkes_greeks(ChainDev& d, GreeksDev<kHawkesGreekParams>& t, co
                                const HawkesMgfConsts& k, double* prices_out) {
   if (int rc = queue_hawkes_prices(d, c, &k, prices_out)) return rc;
   if (int rc = t.alloc(c, true)) return rc;
-  launch_hawkes_mgf_tangent(d.st, d.phi.as<cd>(), c.P, c.M, d.dt.as<double>(), k, make_hawkes_tangents(params), t.dlm.as<cd>(), t.lm.as<cd>(),
-                            t.nfev.as<int>());
+  launch_hawkes_mgf_tangent<false>(d.st, d.phi.as<cd>(), c.P, c.M, d.dt.as<double>(), k, make_hawkes_tangents(params), 0, t.dlm.as<cd>(),
+                                   t.lm.as<cd>(), t.nfev.as<int>());
   if (int rc = check_launch("hawkes_mgf_tangent_kernel")) return rc;
   return t.sums(d, c, t.lm.as<cd>());
 }
@@ -3500,7 +3370,7 @@ struct HawkesRpDev {
 
 // The first-order launches of b200sv_hawkesjd_price_chain_risk_premia_greeks on a prepared chain (DESIGN.md §4.12): the pricing launches of
 // b200sv_hawkesjd_price_chain with the gamma (the restarted normaliser launch, its one synchronisation, the Riccati launch and the gamma
-// sums: bit-identical prices), then hawkes_mgf_rp_tangent_kernel at the two normaliser points (restarted) and on the grid (carried), and
+// sums: bit-identical prices), then hawkes_mgf_tangent_kernel<TPB, true> at the two normaliser points (restarted) and on the grid (carried), and
 // fourier_gamma_greeks_kernel on the grid tangent kernel's own primal log-MGF (no launch on an empty chain).
 static int queue_hawkes_rp_greeks(ChainDev& d, GreeksDev<kHawkesRpParams>& g, HawkesRpDev& r, const FourierChain& c,
                                   const b200sv_hawkes_params& params, const HawkesMgfConsts& k, const double* ttms, const double* forwards,
@@ -3516,17 +3386,39 @@ static int queue_hawkes_rp_greeks(ChainDev& d, GreeksDev<kHawkesRpParams>& g, Ha
   B200SV_CUDA(r.two.upload(cplx(two), 2));
   B200SV_CUDA(r.ttm.upload(ttms, M));
   B200SV_CUDA(r.dn.alloc(sizeof(cd) * (size_t)kHawkesRpParams * M * 2));
-  launch_hawkes_mgf_rp_tangent(d.st, r.two.as<cd>(), 2, M, r.ttm.as<double>(), k, dirs, 1, r.dn.as<cd>(), nullptr, nullptr);
-  if (int rc = check_launch("hawkes_mgf_rp_tangent_kernel")) return rc;
+  launch_hawkes_mgf_tangent<true>(d.st, r.two.as<cd>(), 2, M, r.ttm.as<double>(), k, dirs, 1, r.dn.as<cd>(), nullptr, nullptr);
+  if (int rc = check_launch("hawkes_mgf_tangent_kernel")) return rc;
   if (int rc = g.alloc(c, true)) return rc;
-  launch_hawkes_mgf_rp_tangent(d.st, d.phi.as<cd>(), P, M, d.dt.as<double>(), k, dirs, 0, g.dlm.as<cd>(), g.lm.as<cd>(), g.nfev.as<int>());
-  if (int rc = check_launch("hawkes_mgf_rp_tangent_kernel")) return rc;
+  launch_hawkes_mgf_tangent<true>(d.st, d.phi.as<cd>(), P, M, d.dt.as<double>(), k, dirs, 0, g.dlm.as<cd>(), g.lm.as<cd>(), g.nfev.as<int>());
+  if (int rc = check_launch("hawkes_mgf_tangent_kernel")) return rc;
   if (c.Jtot > 0) {
     fourier_gamma_greeks_kernel<<<c.Jtot, kFourierThreads, 0, d.st>>>(g.lm.as<cd>(), g.dlm.as<cd>(), r.dn.as<cd>(), d.phi.as<cd>(), P, M,
                                                                       d.rows.as<StrikeSpec>(), gamma, r.ng.as<double>(), g.g.as<double>());
     if (int rc = check_launch("fourier_gamma_greeks_kernel")) return rc;
   }
   return 0;
+}
+
+// hawkes_mgf_hessian_kernel<Phi> at the n points phi, one thread per (point, pair), on the second field derivatives d2c (make_hawkes_hessian)
+template <bool Phi>
+static int launch_hawkes_mgf_hessian(cudaStream_t st, const cd* phi, int n, int M, const double* dtaus, const HawkesMgfConsts& k,
+                                     const HawkesTangentDirs& dirs, const DevBuf& d2c, int restart, cd* d2lm) {
+  constexpr int D = kHawkesOdeDirs + Phi, TPB = kHawkesHessianTPB;
+  hawkes_mgf_hessian_kernel<Phi><<<(n * (D * (D + 1) / 2) + TPB - 1) / TPB, TPB, 0, st>>>(phi, n, M, dtaus, k, dirs, d2c.as<HawkesMgfConsts>(),
+                                                                                          restart, d2lm);
+  return check_launch("hawkes_mgf_hessian_kernel");
+}
+
+// The grid launch of both Hawkes Hessian entry points, after their first-order launches: make_hawkes_hessian's table for the 13 + Phi
+// directions into d2c, then hawkes_mgf_hessian_kernel<Phi> carried over the grid into d2lm [NH][M][P] (NH = 120, or 136 with Phi)
+template <bool Phi>
+static int queue_hawkes_hessian(ChainDev& d, const FourierChain& c, const b200sv_hawkes_params& params, const HawkesMgfConsts& k,
+                                const HawkesTangentDirs& dirs, DevBuf& d2c, DevBuf& d2lm) {
+  constexpr int NP = kHawkesGreekParams + Phi, NH = NP * (NP + 1) / 2;
+  const std::vector<HawkesMgfConsts> h = make_hawkes_hessian(params, kHawkesOdeDirs + Phi);
+  B200SV_CUDA(d2c.upload(h.data(), h.size()));
+  B200SV_CUDA(d2lm.alloc(sizeof(cd) * (size_t)NH * c.M * c.P));
+  return launch_hawkes_mgf_hessian<Phi>(d.st, d.phi.as<cd>(), c.P, c.M, d.dt.as<double>(), k, dirs, d2c, 0, d2lm.as<cd>());
 }
 
 // The second-order sums of b200sv_*_price_chain_hessian after its Hessian kernel wrote d2lm [NH][M][P]: fourier_vanilla_hessian_kernel
@@ -4208,8 +4100,8 @@ int b200sv_hawkesjd_price_chain_risk_premia_greeks(const b200sv_hawkes_params* p
 }
 
 /* Second-order sensitivities of the Hawkes Fourier chain under the risk kernel (DESIGN.md §4.13): the launches of
- * b200sv_hawkesjd_price_chain_risk_premia_greeks unchanged (bit-identical first-order outputs), then hawkes_mgf_rp_hessian_kernel at the
- * two normaliser points (restarted) and on the grid (carried), and fourier_gamma_hessian_kernel; one synchronisation at the end. */
+ * b200sv_hawkesjd_price_chain_risk_premia_greeks unchanged (bit-identical first-order outputs), then hawkes_mgf_hessian_kernel<true> on the
+ * grid (carried) and at the two normaliser points (restarted), and fourier_gamma_hessian_kernel; one synchronisation at the end. */
 int b200sv_hawkesjd_price_chain_risk_premia_hessian(const b200sv_hawkes_params* params, int M, const double* ttms, const double* forwards,
                                                     const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
                                                     int is_spot_measure, double vol_scaler, int P, double risk_premia_gamma, double* prices_out,
@@ -4222,30 +4114,17 @@ int b200sv_hawkesjd_price_chain_risk_premia_hessian(const b200sv_hawkes_params* 
                                     risk_premia_gamma))
     return rc;
   P = c.P;
-  constexpr int NP = kHawkesRpParams, NH = NP * (NP + 1) / 2, TPB = kHawkesHessianTPB;
+  constexpr int NP = kHawkesRpParams, NH = NP * (NP + 1) / 2;
   const HawkesMgfConsts k = make_hawkes_mgf_consts(*params);
   ChainDev d;
   HawkesRpDev r(d.st);
   GreeksDev<NP> g(d.st);
   if (int rc = queue_hawkes_rp_greeks(d, g, r, c, *params, k, ttms, forwards, risk_premia_gamma, prices_out)) return rc;
-  // the second field derivatives per pair of the 14 directions: make_hawkes_hessian's on the ODE pairs, none with phi
-  HawkesMgfConsts h[kHawkesOdePairs], h2[kHawkesRpPairs];
-  make_hawkes_hessian(*params, h);
-  for (int a = 0; a < kHawkesRpDirs; ++a)
-    for (int b = a; b < kHawkesRpDirs; ++b)
-      h2[tri_index(a, b, kHawkesRpDirs)] = b < kHawkesOdeDirs ? h[tri_index(a, b, kHawkesOdeDirs)]
-                                                              : HawkesMgfConsts{0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
   const HawkesTangentDirs dirs = make_hawkes_tangents(*params);
   DevBuf d_d2c(d.st), d_d2n(d.st), d_d2lm(d.st), d_v(d.st), d_h(d.st);
-  B200SV_CUDA(d_d2c.upload(h2, kHawkesRpPairs));
+  if (int rc = queue_hawkes_hessian<true>(d, c, *params, k, dirs, d_d2c, d_d2lm)) return rc;
   B200SV_CUDA(d_d2n.alloc(sizeof(cd) * (size_t)NH * M * 2));
-  B200SV_CUDA(d_d2lm.alloc(sizeof(cd) * (size_t)NH * M * P));
-  hawkes_mgf_rp_hessian_kernel<<<(2 * kHawkesRpPairs + TPB - 1) / TPB, TPB, 0, d.st>>>(r.two.as<cd>(), 2, M, r.ttm.as<double>(), k, dirs,
-                                                                                       d_d2c.as<HawkesMgfConsts>(), 1, d_d2n.as<cd>());
-  if (int rc = check_launch("hawkes_mgf_rp_hessian_kernel")) return rc;
-  hawkes_mgf_rp_hessian_kernel<<<(P * kHawkesRpPairs + TPB - 1) / TPB, TPB, 0, d.st>>>(d.phi.as<cd>(), P, M, d.dt.as<double>(), k, dirs,
-                                                                                       d_d2c.as<HawkesMgfConsts>(), 0, d_d2lm.as<cd>());
-  if (int rc = check_launch("hawkes_mgf_rp_hessian_kernel")) return rc;
+  if (int rc = launch_hawkes_mgf_hessian<true>(d.st, r.two.as<cd>(), 2, M, r.ttm.as<double>(), k, dirs, d_d2c, 1, d_d2n.as<cd>())) return rc;
   if (c.Jtot > 0) {       // the vanna CTA and NH / NP Hessian CTAs per strike
     B200SV_CUDA(d_v.alloc(sizeof(double) * (size_t)NP * c.Jtot));
     B200SV_CUDA(d_h.alloc(sizeof(double) * (size_t)NH * c.Jtot));
@@ -4268,7 +4147,7 @@ int b200sv_hawkesjd_price_chain_risk_premia_hessian(const b200sv_hawkes_params* 
 }
 
 /* Second-order sensitivities of the Hawkes Fourier chain without a risk kernel (DESIGN.md §4.5): the launches of
- * b200sv_hawkesjd_price_chain_greeks unchanged (bit-identical first-order outputs), then hawkes_mgf_hessian_kernel and the split
+ * b200sv_hawkesjd_price_chain_greeks unchanged (bit-identical first-order outputs), then hawkes_mgf_hessian_kernel<false> and the split
  * second-order sums; one synchronisation at the end. */
 int b200sv_hawkesjd_price_chain_hessian(const b200sv_hawkes_params* params, int M, const double* ttms, const double* forwards,
                                         const double* discfactors, const int* offsets, const double* strikes, const int8_t* types,
@@ -4282,19 +4161,11 @@ int b200sv_hawkesjd_price_chain_hessian(const b200sv_hawkes_params* params, int 
   ChainDev d;
   GreeksDev<kHawkesGreekParams> g(d.st);
   if (int rc = queue_hawkes_greeks(d, g, c, *params, k, prices_out)) return rc;
-  constexpr int NP = kHawkesGreekParams, NH = NP * (NP + 1) / 2, TPB = kHawkesHessianTPB;
-  P = c.P;
-  HawkesMgfConsts h[kHawkesOdePairs];
-  make_hawkes_hessian(*params, h);
   DevBuf d_d2c(d.st), d_d2lm(d.st);
-  B200SV_CUDA(d_d2c.upload(h, kHawkesOdePairs));
-  B200SV_CUDA(d_d2lm.alloc(sizeof(cd) * (size_t)NH * M * P));
-  hawkes_mgf_hessian_kernel<<<(P * kHawkesOdePairs + TPB - 1) / TPB, TPB, 0, d.st>>>(d.phi.as<cd>(), P, M, d.dt.as<double>(), k,
-                                                                                     make_hawkes_tangents(*params),
-                                                                                     d_d2c.as<HawkesMgfConsts>(), d_d2lm.as<cd>());
-  if (int rc = check_launch("hawkes_mgf_hessian_kernel")) return rc;
+  if (int rc = queue_hawkes_hessian<false>(d, c, *params, k, make_hawkes_tangents(*params), d_d2c, d_d2lm)) return rc;
   // the tangent kernel's primal log-MGF and tangents, as for the first-order rows
-  if (int rc = queue_hessian_sums<NP>(d, c, g.lm.as<cd>(), g.dlm.as<cd>(), d_d2lm, vanna_out, hessian_out, d2log_mgf_out)) return rc;
+  if (int rc = queue_hessian_sums<kHawkesGreekParams>(d, c, g.lm.as<cd>(), g.dlm.as<cd>(), d_d2lm, vanna_out, hessian_out, d2log_mgf_out))
+    return rc;
   return g.download(d, c, greeks_out, dlog_mgf_out, nfev_out);
 }
 

@@ -740,6 +740,26 @@ def hawkesjd_price_chain_hessian(params: C.HawkesParamsC, ttms, forwards, discfa
                                 HAWKES_GREEK_PARAMS, True)
 
 
+def _hawkesjd_risk_premia(symbol: str, params, gamma: float, chain, vol_scaler, max_phi: Optional[int], return_grids: bool, second: bool):
+    """the risk-kernel sensitivity entry points: C arguments (params, chain block, spot measure, vol_scaler, max_phi, gamma, prices,
+    greeks [2 + n, J], dlog_mgf [n, M, P], dlog_norm [n, M, 2], nfev [P][, vanna [n, J], hessian [nh, J], d2log_mgf [nh, M, P],
+    d2log_norm [nh, M, 2]]) -> (prices per maturity, greeks[, vanna, hessian], offsets) and with ``return_grids`` the grids in that order"""
+    ch = _chain_arrays(*chain)
+    max_phi, n, J = int(max_phi or 500), len(HAWKES_RISK_PREMIA_GREEK_PARAMS), ch.strikes.shape[0]
+    nh = n * (n + 1) // 2
+    prices, greeks = np.empty(J), np.empty((2 + n, J))
+    rows = (np.empty((n, J)), np.empty((nh, J))) if second else ()
+    grids = (np.empty((n, ch.M, max_phi), dtype=np.complex128), np.empty((n, ch.M, 2)), np.empty(max_phi, dtype=np.int32))
+    if second:
+        grids += (np.empty((nh, ch.M, max_phi), dtype=np.complex128), np.empty((nh, ch.M, 2)))
+    if not return_grids:
+        grids = (None,) * len(grids)
+    C.call(symbol, byref(params), *C.chain_ptrs(ch), 1, C.vol_scaler_arg(vol_scaler), max_phi, float(gamma), C.dptr(prices),
+           C.dptr(greeks), C.dptr(grids[0]), C.dptr(grids[1]), C.iptr(grids[2]), *map(C.dptr, rows), *map(C.dptr, grids[3:]))
+    out = (C.split_chain(prices, ch.offsets), greeks, *rows, ch.offsets)
+    return out + grids if return_grids else out
+
+
 def hawkesjd_price_chain_risk_premia_greeks(params: C.HawkesParamsC, gamma: float, ttms, forwards, discfactors, strikes_ttms,
                                             optiontypes_ttms, vol_scaler: Optional[float] = None, max_phi: Optional[int] = None,
                                             return_grids: bool = False):
@@ -748,16 +768,8 @@ def hawkesjd_price_chain_risk_premia_greeks(params: C.HawkesParamsC, gamma: floa
     greeks [18, J], offsets) -- greeks rows: delta, gamma, then HAWKES_RISK_PREMIA_GREEK_PARAMS -- and with ``return_grids`` also
     (dlog_mgf [16, M, P], dlog_norm [16, M, 2], nfev [P]); dlog_norm holds the derivatives of Re log-MGF at -gamma and -gamma - 1.  The
     prices are bit-identical to hawkesjd_price_chain with the same gamma.  P defaults to the route's 500 points."""
-    ch = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
-    max_phi, n, J = int(max_phi or 500), len(HAWKES_RISK_PREMIA_GREEK_PARAMS), ch.strikes.shape[0]
-    prices, greeks = np.empty(J), np.empty((2 + n, J))
-    dlm = np.empty((n, ch.M, max_phi), dtype=np.complex128) if return_grids else None
-    dnorm = np.empty((n, ch.M, 2)) if return_grids else None
-    nfev = np.empty(max_phi, dtype=np.int32) if return_grids else None
-    C.call("b200sv_hawkesjd_price_chain_risk_premia_greeks", byref(params), *C.chain_ptrs(ch), 1, C.vol_scaler_arg(vol_scaler), max_phi,
-           float(gamma), C.dptr(prices), C.dptr(greeks), C.dptr(dlm), C.dptr(dnorm), C.iptr(nfev))
-    out = (C.split_chain(prices, ch.offsets), greeks, ch.offsets)
-    return out + (dlm, dnorm, nfev) if return_grids else out
+    return _hawkesjd_risk_premia("b200sv_hawkesjd_price_chain_risk_premia_greeks", params, gamma,
+                                 (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms), vol_scaler, max_phi, return_grids, False)
 
 
 def hawkesjd_price_chain_risk_premia_hessian(params: C.HawkesParamsC, gamma: float, ttms, forwards, discfactors, strikes_ttms,
@@ -768,20 +780,8 @@ def hawkesjd_price_chain_risk_premia_hessian(params: C.HawkesParamsC, gamma: flo
     (prices per maturity, greeks [18, J], vanna, hessian, offsets) and with ``return_grids`` also (dlog_mgf [16, M, P], dlog_norm [16, M, 2],
     nfev [P], d2log_mgf [136, M, P], d2log_norm [136, M, 2]); d2log_norm holds the second derivatives of Re log-MGF at -gamma and
     -gamma - 1.  The first-order outputs are bit-identical to hawkesjd_price_chain_risk_premia_greeks."""
-    ch = _chain_arrays(ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms)
-    max_phi, n, J = int(max_phi or 500), len(HAWKES_RISK_PREMIA_GREEK_PARAMS), ch.strikes.shape[0]
-    nh = n * (n + 1) // 2
-    prices, greeks, vanna, hessian = np.empty(J), np.empty((2 + n, J)), np.empty((n, J)), np.empty((nh, J))
-    dlm = np.empty((n, ch.M, max_phi), dtype=np.complex128) if return_grids else None
-    dnorm = np.empty((n, ch.M, 2)) if return_grids else None
-    nfev = np.empty(max_phi, dtype=np.int32) if return_grids else None
-    d2lm = np.empty((nh, ch.M, max_phi), dtype=np.complex128) if return_grids else None
-    d2norm = np.empty((nh, ch.M, 2)) if return_grids else None
-    C.call("b200sv_hawkesjd_price_chain_risk_premia_hessian", byref(params), *C.chain_ptrs(ch), 1, C.vol_scaler_arg(vol_scaler), max_phi,
-           float(gamma), C.dptr(prices), C.dptr(greeks), C.dptr(dlm), C.dptr(dnorm), C.iptr(nfev), C.dptr(vanna), C.dptr(hessian),
-           C.dptr(d2lm), C.dptr(d2norm))
-    out = (C.split_chain(prices, ch.offsets), greeks, vanna, hessian, ch.offsets)
-    return out + (dlm, dnorm, nfev, d2lm, d2norm) if return_grids else out
+    return _hawkesjd_risk_premia("b200sv_hawkesjd_price_chain_risk_premia_hessian", params, gamma,
+                                 (ttms, forwards, discfactors, strikes_ttms, optiontypes_ttms), vol_scaler, max_phi, return_grids, True)
 
 
 def logsv_price_chain_batch(params_list: Sequence[C.LogsvParamsC], ttms, forwards, discfactors, etas, strikes_ttms, optiontypes_ttms,
